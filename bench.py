@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- detection hot path benchmark (contract: the task statement / DESIGN.md section 6).
+"""bench.py -- detection hot path benchmark (DESIGN.md section 6).
 
-    python bench.py --gpus N --steps K --warmup W                      # this build (sm_100a kernels), default config v8n_b32
+    python bench.py --gpus N --steps K --warmup W                      # this build (sm_90a kernels), default config v8n_b32
     python bench.py --impl reference --gpus N --steps K --warmup W     # the reference's CPU path on the host cores
     python bench.py --config {v8n_b32,v5s_b1,retina_b16,rcnn_b8} ...   # the other BASELINE.json configs (N = 1)
 
@@ -15,9 +15,11 @@ value = whole-job frames/s with inputs resident in HBM; e2e = the same step thro
 in pinned HOST memory (H2D inside the timed region) and the compact detections copied back (D2H inside the timed region).
 Both arms print the same `config` dict (same workload, same stages: pre-process + decode + NMS).
 
-Timing: W warm-up steps, then blocks of EXACTLY K steps each bracketed by CUDA events (barrier + synchronize on both sides);
-as many blocks as it takes to cover >= 0.35 s, so that the 100 ms clock sampler has samples INSIDE the timed windows;
-ms_per_step = mean block time / K (max over ranks per block).  Prints ONE JSON line on rank 0.
+Timing: W warm-up steps, then ONE block of exactly K steps bracketed by CUDA events (barrier + synchronize on both sides);
+ms_per_step = block time / K (max over ranks).  The 100 ms clock sampler reports samples only from inside the timed windows,
+so take K large enough for the block to last a few tenths of a second.  Prints ONE JSON line on rank 0.
+--dump-outputs DIR writes what the last timed step computed to DIR/<name>.npy (see dump_outputs); the inputs are seeded,
+so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -25,7 +27,6 @@ import argparse
 import ctypes as C
 import hashlib
 import json
-import math
 import os
 import statistics
 import subprocess
@@ -56,7 +57,8 @@ CONFIGS = {
 }
 ALGO_BYTES_PER_IMAGE = (4 + NC) * sum((NET // s) ** 2 for s in STRIDES) * 4  # 2 822 400 B, SURVEY 8d
 LETTERBOX_BYTES_PER_IMAGE = NET * NET * 3 + 3 * NET * NET * 4                  # 6 144 000 B, SURVEY 8d
-MIN_TIMED_S = 0.35
+L2_MB = 50           # H100: inputs rotate over enough distinct sets that a step never finds its inputs in L2
+DUMP_SAMPLE = 1 << 21   # --dump-outputs: seeded sample of an output larger than this many elements
 
 
 def _env_int(name, default):
@@ -82,7 +84,7 @@ def host_cores() -> int:
 
 
 # --------------------------------------------------------------------------------------------------
-# clocks: nvidia-smi sampled DURING the timed regions (B200_PROFILING.md "clocks line")
+# clocks: nvidia-smi sampled DURING the timed regions
 # --------------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
@@ -128,8 +130,11 @@ class ClockSampler:
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), f[5:9]):
                 if v.lower().startswith("active"):
                     reasons.add(name)
-        return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(smax) if smax else None,
-                "reasons": sorted(reasons), "samples": inside, "sampled": "inside the timed windows only (100 ms period)"}
+        out = {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(smax) if smax else None,
+               "reasons": sorted(reasons), "samples": inside, "sampled": "inside the timed windows only (100 ms period)"}
+        if inside == 0:
+            out["note"] = "no sample fell inside the timed windows: raise --steps until a timed block lasts a few tenths of a second"
+        return out
 
 
 class AllGpuSampler:
@@ -407,7 +412,7 @@ def cpu_rows(run: CpuRunner, cores: int) -> dict:
             continue
         rows[f"B1_nms_only_{label}_1thread_us"] = 1e6 / run.run(f"nms_{label}", n1, 1)[0]
         rows[f"B1_nms_only_{label}_8workers_us"] = 1e6 / run.run(f"nms_{label}", n8, w8)[0]
-    rows["B1_kind"] = cp.nms_kind + (" (compiled from /root/reference into oracle/_ref)" if cp.ref is not None else " (oracle restatement)")
+    rows["B1_kind"] = cp.nms_kind + (" (the reference's host code, compiled into oracle/_ref)" if cp.ref is not None else " (oracle restatement)")
     rows["B2_decode_nms_1thread_us"] = 1e6 / run.run("dec_nms", max(B, 32), 1)[0]
     rows["B2_decode_nms_8workers_us"] = 1e6 / run.run("dec_nms", n8, w8)[0]
     rows["B2_decode_nms_all_cores_us"] = 1e6 / run.run("dec_nms", max(n8, 16 * cores), cores)[0]
@@ -537,7 +542,7 @@ PER_RANK_MS = []   # N > 1: one list per timed block with every rank's own block
 
 
 def timed_blocks(step, K, W, stream, dev, world, dist, flush=None, pre=None, run_many=None):
-    """W warm-up steps, then blocks of exactly K steps; returns (mean ms per block, [(t0, t1) wall windows], n_blocks)."""
+    """W warm-up steps, then one block of exactly K steps; returns (ms of the block, [(t0, t1) wall window], 1)."""
     import torch
 
     def block(first):
@@ -579,15 +584,8 @@ def timed_blocks(step, K, W, stream, dev, world, dist, flush=None, pre=None, run
             step(i)
     if flush is not None:
         flush(W - 1)
-    ms0, w0 = block(W)
-    n = max(1, math.ceil(MIN_TIMED_S * 1e3 / max(ms0, 1e-3)))   # same on every rank: ms0 is the max over ranks
-    n = min(n, 4000)
-    res, wins = [ms0], [w0]
-    for b in range(1, n):
-        ms, w = block(W + b * K)
-        res.append(ms)
-        wins.append(w)
-    return sum(res) / len(res), wins, len(res)
+    ms, w = block(W)
+    return ms, [w], 1
 
 
 def time_kernel_loop(fn, n, stream, dev):
@@ -610,7 +608,38 @@ def peak_hbm():
         peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())
         return float(peaks["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s)"
+
+
+def _sample(t, name: str) -> dict:
+    """`name` whole, or DUMP_SAMPLE elements of it at seeded positions (`name`_sample + their flat indices)."""
+    import numpy as np
+    import torch
+    if t.numel() <= DUMP_SAMPLE:
+        return {name: t.float().cpu().numpy()}
+    idx = np.sort(np.random.default_rng(0).choice(t.numel(), DUMP_SAMPLE, replace=False))
+    vals = t.reshape(-1)[torch.from_numpy(idx).to(t.device)].float().cpu().numpy()
+    return {name + "_sample": vals, name + "_sample_index": idx.astype(np.float64)}
+
+
+def _live_rows(out, row_floats: int):
+    """Compact detections [B, 1 + max_det*row_floats] with the slots past each image's count zeroed: a caller reads the
+    count and that many rows; the slots behind them keep whatever an earlier step left there."""
+    o = out.float().cpu().numpy().copy()
+    for b in range(o.shape[0]):
+        o[b, 1 + int(o[b, 0]) * row_floats:] = 0
+    return o
+
+
+def dump_outputs(d: str, arrays: dict) -> None:
+    """--dump-outputs: the arrays the last timed step computed, as <d>/<name>.npy in float32, <= 64 MB in all."""
+    import numpy as np
+    out = Path(d)
+    out.mkdir(parents=True, exist_ok=True)
+    total = sum(np.asarray(a).nbytes for a in arrays.values())
+    assert total <= 64 << 20, f"--dump-outputs: {total} bytes > 64 MB"
+    for name, a in arrays.items():
+        np.save(out / f"{name}.npy", np.ascontiguousarray(a))
 
 
 def run_v8(args, rank, world, local_rank):
@@ -835,6 +864,10 @@ def run_v8(args, rank, world, local_rank):
         if peer is not None:   # whole groups only
             K, W = max(G, K // G * G), max(G, (W + G - 1) // G * G)
         ms_dev, win_dev, nb_dev = timed_blocks(step_dev, K, W, stream, dev, world, dist, flush_dev, run_many=run_dev)
+        if args.dump_outputs and rank == 0:
+            j = (W + K - 1) % R   # the input set of the last timed step
+            last = pipes_dev[j].fused.out if peer is None or peer.fused else outs2[j][replays[0] % 2]  # flush_dev ran one replay later
+            dump_outputs(args.dump_outputs, {"detections": _live_rows(last, 7), **_sample(pipes_dev[j].net_input, "letterbox")})
         per_rank_ms = None   # N > 1: every rank's own mean ms per step over the timed blocks (ms_per_step is built from the per-block maxima)
         try:
             if PER_RANK_MS:
@@ -933,11 +966,11 @@ def run_v8(args, rank, world, local_rank):
         "config": config_dict("v8n_b32", world),
         "run": {"parallelism": f"dp{world}: batch-sharded, gather = {gather_mode}" if world > 1 else "single GPU",
                 "l2": f"inputs rotate over {R} distinct sets ({R * head_bytes / 1e6:.0f} MB of head tensors + "
-                      f"{R * BATCH * NET * NET * 3 / 1e6:.0f} MB of frames > 126 MB L2)",
+                      f"{R * BATCH * NET * NET * 3 / 1e6:.0f} MB of frames > {L2_MB} MB L2)",
                 "cuda_graphs": not args.no_graph,
                 "overlap": (f"{G} steps per graph as two concurrent chains: letterbox launches || (scan -> NMS) launches" if G > 1 else
                             ("letterbox || (scan -> NMS) as parallel graph branches" if not args.no_overlap else "serial")),
-                "timed_blocks": {"device": nb_dev, "e2e": nb_e2e, "steps_per_block": K, "min_timed_s": MIN_TIMED_S},
+                "timed_blocks": {"device": nb_dev, "e2e": nb_e2e, "steps_per_block": K},
                 "per_rank_ms_per_step": per_rank_ms,
                 "gpus_during_device_blocks": all_gpus.summary(win_dev) if all_gpus is not None else None,
                 "gather_timeouts": gather_err, "gather_verified": gather_verified,
@@ -1069,6 +1102,14 @@ def run_other(args, local_rank):
         sampler.start()
         time.sleep(0.25)
         ms_dev, win_dev, nb = timed_blocks(step_dev, K, W, stream, dev, 1, None)
+        if args.dump_outputs:
+            j = (W + K - 1) % R   # the input set of the last timed step
+            if name == "rcnn_b8":
+                outs = {"scores": chain.fs.cpu().numpy(), "boxes": chain.fb.cpu().numpy(), "classes": chain.fc.cpu().numpy()}
+            else:
+                det = _live_rows(pipes[j].fused.out, 7) if name == "v5s_b1" else _live_rows(pipes[j].out, 17)
+                outs = {"detections": det, **_sample(pipes[j].net_input, "letterbox")}
+            dump_outputs(args.dump_outputs, outs)
         ms_e2e, win_e2e, nb2 = timed_blocks(step_e2e, K, W, stream, dev, 1, None)
         sampler.stop()
     fps, fps_e2e = B * K / (ms_dev * 1e-3), B * K / (ms_e2e * 1e-3)
@@ -1092,7 +1133,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", default="graft", choices=["graft", "reference"])
     ap.add_argument("--config", default="v8n_b32", choices=sorted(CONFIGS))
-    ap.add_argument("--sets", type=int, default=4, help="distinct input sets rotated to defeat the 126 MB L2")
+    ap.add_argument("--sets", type=int, default=4, help=f"distinct input sets rotated to defeat the {L2_MB} MB L2")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed to DIR/<name>.npy")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--rows", action="store_true", help="--impl reference: also time the CPU rows B1 / B2 / B3 of BASELINE.md section 2")
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel from Python instead of CUDA graphs")

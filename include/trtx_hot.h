@@ -1,5 +1,5 @@
 /*
- * trtx_hot.h -- C ABI of the B200-native detection hot path (libtrtx_hot.so).
+ * trtx_hot.h -- C ABI of the H100-native detection hot path (libtrtx_hot.so).
  *
  * This is the drop-in boundary: every entry point below is what a TensorRT plugin's
  * enqueue()/getWorkspaceSize() (or the driver's cuda_* helper) in wang-xinyu/tensorrtx
@@ -10,7 +10,7 @@
  * enqueue() convention, yolov8/plugin/yololayer.cu:171), non-zero = TRTX_ERR_*; the library
  * never throws and never asserts.
  *
- * Reference citations are relative to /root/reference (wang-xinyu/tensorrtx @ 3ff22bb4).
+ * Reference citations are relative to the root of wang-xinyu/tensorrtx @ 3ff22bb4.
  * The header-only TensorRT adapters that forward the IPluginV2DynamicExt / IPluginV2IOExt /
  * IPluginV2Ext virtuals to these functions live in include/trtx_plugins.h; the binding a
  * maintainer adds on the reference side is shown in INTEGRATION.md.
@@ -99,8 +99,8 @@ typedef struct trtx_yolo_params {
     int32_t in_dtype;    /* TRTX_F32 (parity mode, what the reference accepts, yololayer.h:32-35) | TRTX_F16 */
     /* Launch tuning of the scan kernel.  Plain per-call data: the library keeps NO mutable state, so concurrent enqueues
      * (TensorRT calls enqueue() on clones from several threads, SURVEY 8b "Threading") with different tunings are
-     * independent.  0 everywhere -- what memset / trtx_yolo_params_init_v8 leave -- selects the defaults taken from the
-     * B200 sweep in profiles/.  A combination that is not built returns TRTX_ERR_UNSUPPORTED. */
+     * independent.  0 everywhere -- what memset / trtx_yolo_params_init_v8 leave -- selects the defaults chosen on an H100 for
+     * the overlapped benchmark step (DESIGN.md section 4.1).  A combination that is not built returns TRTX_ERR_UNSUPPORTED. */
     int32_t tune_class_slices;   /* warps of a CTA splitting the class range: 1, 2, 4, 8; 0 = 2 */
     int32_t tune_rows_in_flight; /* channel rows loaded per group; 0 = 5 (fp16 inputs, 8 anchors per lane: 10).  Built (slices, rows): (1,8) (1,16) (2,4) (2,5)
                                     (2,8) (2,10) (2,20) (4,4) (4,5) (4,10) (4,20) (8,5) (8,10) */

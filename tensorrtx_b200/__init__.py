@@ -1,4 +1,4 @@
-"""tensorrtx_b200 -- B200-native (sm_100a) detection decode / NMS / pre-process hot path.
+"""tensorrtx_b200 -- H100-native (sm_90a) detection decode / NMS / pre-process hot path.
 
 Product = libtrtx_hot.so (C ABI, include/trtx_hot.h) + this thin host-side mirror of the
 reference's plugin interface.  Importing `tensorrtx_b200.plugins` requires the built library

@@ -1,7 +1,7 @@
 """ctypes binding of libtrtx_hot.so (the C ABI declared in include/trtx_hot.h).
 
 There is NO fallback: if the shared library is missing or fails to load, importing the product
-path raises.  The library is built in-tree by tensorrtx_b200/build.py (nvcc, sm_100a).
+path raises.  The library is built in-tree by tensorrtx_b200/build.py (nvcc, sm_90a).
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""In-tree build of libtrtx_hot.so (sm_100a) with nvcc.
+"""In-tree build of libtrtx_hot.so (sm_90a) with nvcc.
 
 The shared library is the product: a C-ABI (include/trtx_hot.h) with no torch / Python types in
 its signatures.  It is built IN-TREE (tensorrtx_b200/lib/) so that it travels to the GPU box with
@@ -21,7 +21,7 @@ LIB = LIBDIR / "libtrtx_hot.so"
 SOURCES = ["yolo_decode.cu", "yolo_scan_pipe.cu", "nms.cu", "retina_decode.cu", "rcnn.cu", "preprocess.cu", "mask.cu", "roi_align.cu", "calib_host.cu"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-fvisibility=hidden",
     "--expt-relaxed-constexpr",
@@ -45,7 +45,7 @@ def _stamp(sources: list[Path]) -> str:
 
 
 def build(force: bool = False, verbose: bool = False, probe: bool = False, defines: tuple = (), suffix: str = "") -> Path:
-    """Compile every CUDA source for sm_100a into tensorrtx_b200/lib/libtrtx_hot.so.
+    """Compile every CUDA source for sm_90a into tensorrtx_b200/lib/libtrtx_hot.so.
     probe=True builds libtrtx_hot_probe.so instead: the same sources with -DTRTX_NMS_PROBE (clock64 phase stamps in
     nms_kernel + trtx_probe_set_nms_stamps), used by tools/nms_probe.py only.  `defines` + `suffix`: further experiment
     builds (tools/scan_probe.py), never loaded by the product path."""

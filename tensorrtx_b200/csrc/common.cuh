@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for libtrtx_hot (sm_100a only).
+// common.cuh -- shared device helpers for libtrtx_hot (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>

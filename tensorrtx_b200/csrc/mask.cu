@@ -1,4 +1,4 @@
-// mask.cu -- instance masks of the segmentation models for sm_100a (SURVEY 8f rank 1).
+// mask.cu -- instance masks of the segmentation models for sm_90a (SURVEY 8f rank 1).
 // Replaces the HOST function process_mask(): yolov8/yolov8_seg.cpp:17-60 (the same body in yolov5/src/postprocess.cpp:
 // 94-125, yolo11/12 seg drivers), which runs on one CPU core after a D2H copy of the 32 x 160 x 160 prototype tensor:
 //     rect   = get_downscale_rect(bbox, 4)

@@ -897,9 +897,9 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
 // Completes a gather of `nslots` slots on this rank: spins until every rank's publish counter of each slot has reached this
 // rank's own (its own publish precedes this kernel in stream order).  One warp; gives up after ~2 s of SM clocks (ctrl[2] = 1)
 // instead of hanging the GPU.  The polls are RELAXED system-scope loads and there is no fence: whatever reads the gathered rows
-// is a later kernel (or copy) of the stream, and the kernel boundary orders it after these loads.  (Measured, tools/
-// gather_probe.py and profiles/r02e_gather.log: every system-scope fence or release / acquire executed while the step's
-// kernels stream at ~6 TB/s stalls the whole step by several microseconds.)
+// is a later kernel (or copy) of the stream, and the kernel boundary orders it after these loads.  (tools/gather_probe.py
+// measures it: a system-scope fence or release / acquire executed while the step's kernels stream from HBM stalls the whole
+// step.)
 __global__ void __launch_bounds__(64) gather_wait_kernel(NmsArgs::Gather g, int nslots) {
     const int lane = threadIdx.x;  // one thread per (rank, slot): world * nslots <= 64
     const unsigned* fl = g.flags[g.rank];
@@ -932,8 +932,8 @@ struct PushSrc {
 };
 __global__ void __launch_bounds__(256) gather_copy_kernel(NmsArgs::Gather g, PushSrc ps, int batch, int cols, int max_det, int R) {
     // one CTA per (step, image): the kernel is a chain of dependent latencies (count -> rows -> stores), so its duration is one
-    // such chain, not their sum (8 CTAs walking 16 blocks each took ~40 us under the step's traffic and, because the NMS that
-    // overwrites a block has to wait for this copy, stalled the scan -> NMS chain by that much: profiles/r02e_gather.log)
+    // such chain, not their sum (a few CTAs walking many blocks each take far longer under the step's traffic and, because the
+    // NMS that overwrites a block has to wait for this copy, stall the scan -> NMS chain by that much)
     const int tid = threadIdx.x;
     const int w = blockIdx.x;
     const int k = w / batch, b = w - k * batch;

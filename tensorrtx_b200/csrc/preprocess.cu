@@ -1,10 +1,10 @@
-// preprocess.cu -- batched letterbox warp-affine + BGR->RGB + /255 + HWC->CHW (+fp16) for sm_100a.
+// preprocess.cu -- batched letterbox warp-affine + BGR->RGB + /255 + HWC->CHW (+fp16) for sm_90a.
 // Replaces warpaffine_kernel / cuda_preprocess / cuda_batch_preprocess, yolov8/src/preprocess.cu:7-127
 // (identical bodies in yolov5/7/9/10/11/12/13/26), which launch once per image and synchronise the
 // stream after every image (:119-127).  Here: ONE launch for the whole batch, per-image descriptors
 // and affine matrices in the kernel parameter block (no H2D copy of metadata); a warp covers 32
 // adjacent destination columns and every thread produces a strip of rows of its column.  Measured and
-// rejected (profiles/): 4 adjacent pixels per lane (L1 sector-bound), staging the source band in shared
+// rejected: 4 adjacent pixels per lane (L1 sector-bound), staging the source band in shared
 // memory (2x slower).
 //
 // Roofline: HBM-bound; algorithmic bytes per image = src_w*src_h*3 (u8 read once) +
@@ -45,8 +45,8 @@ __device__ __forceinline__ float div255(float x) {
 
 // One thread = ONE destination column x kRowsPerThread destination rows; the 32 lanes of a warp are 32 adjacent
 // columns, so a warp-level byte load spans 32 px * 3 B = 96 B = 3-4 sectors and the planar stores are 128 contiguous
-// bytes per warp.  ncu (profiles/r01k_letterbox_ncu.txt) shows the kernel bound by INSTRUCTION ISSUE (81 % issue
-// active, 136 SASS instructions per pixel before the fast path below), not by HBM, and a rolled, row-serial variant
+// bytes per warp.  The kernel is bound by INSTRUCTION ISSUE (over a hundred SASS
+// instructions per pixel before the fast path below), not by HBM, and a rolled, row-serial variant
 // with fewer instructions was slower still (too few loads in flight): so everything is straight-line code that
 // issues all of a strip's loads before the first use.
 //   * the letterbox matrix has no rotation (m[1] = m[3] = -0.0f, preprocess.cu:99-104), so everything that depends on
@@ -60,10 +60,10 @@ __device__ __forceinline__ float div255(float x) {
 // The fast path converts every other sample this way so that neither the XU pipe nor the issue slots saturate.
 __device__ __forceinline__ float u8_to_float_alu(uint32_t i) { return __uint_as_float(0x4B000000u | i) - 8388608.0f; }
 
-constexpr int kRowsPerThread = 4;  // 8-row strips measured slower (profiles/r01k_lb_probe.log)
+constexpr int kRowsPerThread = 4;  // 8-row strips measured slower on an earlier GPU, not re-measured on H100 (tools/lb_probe.py)
 
 // __launch_bounds__(256, 8): 32 registers -> 64 resident warps per SM.  The kernel is latency-bound once the instruction
-// count is down (no pipe above 60 %), and occupancy is what hides it: 59.4 us at 60 registers, 53.7 at 40, 51.9 at 32.
+// count is down, and occupancy is what hides it: fewer registers per thread measured faster (on an earlier GPU; not re-measured on H100).
 template <typename OutT>
 __global__ void __launch_bounds__(256, 8) letterbox_kernel(const __grid_constant__ PreArgs a, OutT* __restrict__ dst) {
     constexpr int R = kRowsPerThread;
@@ -323,7 +323,7 @@ static bool unit_scale_image(const trtx_image_desc& d, const float m[6], UnitIma
     u->ox = (int)floorf(tx);
     u->oy = (int)floorf(ty);
     // TMA fetches the box from byte column 3 * (64 * tile + ox): the start of a box must be 16-byte aligned in global memory
-    // (an unaligned start is an illegal instruction on sm_100a), so horizontal offsets that are not a multiple of 16 pixels
+    // (an unaligned start is an illegal instruction on sm_90a), so horizontal offsets that are not a multiple of 16 pixels
     // (e.g. a 624-wide source centred in 640) take the general kernel
     if (u->ox % 16 != 0) return false;
     u->lx = tx - floorf(tx);

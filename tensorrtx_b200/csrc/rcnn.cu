@@ -1,4 +1,4 @@
-// rcnn.cu -- Faster R-CNN plugins for sm_100a: RpnDecode, RpnNms, PredictorDecode, BatchedNms.
+// rcnn.cu -- Faster R-CNN plugins for sm_90a: RpnDecode, RpnNms, PredictorDecode, BatchedNms.
 // Replaces rcnn/RpnDecode.cu, RpnNms.cu, PredictorDecode.cu, BatchedNms.cu, which per IMAGE (host loop)
 // run 1-2 cub::DeviceRadixSort passes + thrust transforms/gathers + an NMS kernel that iterates
 // `for m in 0..N` with a __syncthreads() per m (and, launched over ceil(N/1024) blocks, races across

@@ -1,4 +1,4 @@
-// retina_decode.cu -- Decode_TRT (RetinaFace) for sm_100a.
+// retina_decode.cu -- Decode_TRT (RetinaFace) for sm_90a.
 // Replaces CalDetection/forwardGpu of retinaface/decode.cu:110-191 (3 launches + B memsets, float
 // atomics on one counter per image) with one scan launch over all strides/images + one pack launch.
 //

@@ -1,4 +1,4 @@
-// roi_align.cu -- RoIAlign + MaskRcnnInference for sm_100a (SURVEY 8f rank 2).
+// roi_align.cu -- RoIAlign + MaskRcnnInference for sm_90a (SURVEY 8f rank 2).
 // Replaces roiAlign / RoIAlignForward (rcnn/RoiAlign.cu:29-183) and maskRcnnInference / MaskRcnnInferenceKernel
 // (rcnn/MaskRcnnInference.cu:8-63), which launch once per image and call cudaDeviceSynchronize() after every launch
 // (RoiAlign.cu:178, MaskRcnnInference.cu:59) -- a full-device stall inside enqueue().  Here: one launch for the whole
@@ -11,8 +11,9 @@
 // outputs of a (proposal, channel) pair are stored contiguously (coalesced).
 // Roofline: HBM-write-bound: N*C*P*P*4 bytes per image (803 MB at N=1000, C=1024, P=14).
 //
-// Arithmetic mirrors the reference kernel statement by statement and is left to nvcc's default FMA contraction,
-// exactly like the reference's own build (tests/test_vs_reference_gpu.py compares against the reference kernel).
+// Arithmetic mirrors the reference kernel statement by statement; where the compiler could contract it more than one way
+// (the bilinear sum, bilinear_sum below) the contraction of the reference's own build is written out
+// (tests/test_vs_reference_gpu.py compares against the reference kernel).
 #include "common.cuh"
 
 namespace trtx {
@@ -53,6 +54,13 @@ __device__ __forceinline__ AxisTap axis_tap(float y, int size) {
     t.l = y - y_low;
     t.h = 1. - t.l;
     return t;
+}
+
+// :76 `w1 * v1 + w2 * v2 + w3 * v3 + w4 * v4` as the reference's build for sm_90a contracts it: one multiply, then three
+// fused multiply-adds in source order.  Left to nvcc, `w1 * v1 + w2 * v2` may fuse either product (for sm_90a it fuses the
+// other one here), which moves sums of many samples by a few ulps.
+__device__ __forceinline__ float bilinear_sum(float w1, float v1, float w2, float v2, float w3, float v3, float w4, float v4) {
+    return __fmaf_rn(w4, v4, __fmaf_rn(w3, v3, __fmaf_rn(w2, v2, __fmul_rn(w1, v1))));
 }
 
 // Geometry of one proposal (RoiAlign.cu:104-127 -- "Do not using rounding; this implementation detail is critical")
@@ -122,7 +130,7 @@ __device__ __forceinline__ void roi_align_direct(const RoiArgs& a, const RoiGeom
                     if (k < nch) {
                         const float* f = fm + (size_t)k * plane;
                         const float v1 = __ldg(f + o1), v2 = __ldg(f + o2), v3 = __ldg(f + o3), v4 = __ldg(f + o4);
-                        const float val = w1 * v1 + w2 * v2 + w3 * v3 + w4 * v4;  // :76
+                        const float val = bilinear_sum(w1, v1, w2, v2, w3, v3, w4, v4);  // :76
                         output_val[k] += val;
                     }
                 }
@@ -215,22 +223,22 @@ __device__ __forceinline__ void roi_window_taps(const char* win, const WinTap* t
                     const float4 a3 = *reinterpret_cast<const float4*>(p3 + 16 * g), a4 = *reinterpret_cast<const float4*>(p4 + 16 * g);
                     {
                         const float v1 = a1.x, v2 = a2.x, v3 = a3.x, v4 = a4.x;
-                        const float val = w1 * v1 + w2 * v2 + w3 * v3 + w4 * v4;  // :76
+                        const float val = bilinear_sum(w1, v1, w2, v2, w3, v3, w4, v4);  // :76
                         output_val[4 * g + 0] += val;
                     }
                     {
                         const float v1 = a1.y, v2 = a2.y, v3 = a3.y, v4 = a4.y;
-                        const float val = w1 * v1 + w2 * v2 + w3 * v3 + w4 * v4;
+                        const float val = bilinear_sum(w1, v1, w2, v2, w3, v3, w4, v4);
                         output_val[4 * g + 1] += val;
                     }
                     {
                         const float v1 = a1.z, v2 = a2.z, v3 = a3.z, v4 = a4.z;
-                        const float val = w1 * v1 + w2 * v2 + w3 * v3 + w4 * v4;
+                        const float val = bilinear_sum(w1, v1, w2, v2, w3, v3, w4, v4);
                         output_val[4 * g + 2] += val;
                     }
                     {
                         const float v1 = a1.w, v2 = a2.w, v3 = a3.w, v4 = a4.w;
-                        const float val = w1 * v1 + w2 * v2 + w3 * v3 + w4 * v4;
+                        const float val = bilinear_sum(w1, v1, w2, v2, w3, v3, w4, v4);
                         output_val[4 * g + 3] += val;
                     }
                 }

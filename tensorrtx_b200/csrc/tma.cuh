@@ -1,4 +1,4 @@
-// tma.cuh -- mbarrier / TMA (cp.async.bulk.tensor) PTX wrappers and the host-side tensor-map encoder (sm_100a).
+// tma.cuh -- mbarrier / TMA (cp.async.bulk.tensor) PTX wrappers and the host-side tensor-map encoder (sm_90a).
 // Shared by the YoloLayer TMA pipeline (yolo_scan_pipe.cu) and the TMA-staged letterbox (preprocess.cu).
 #pragma once
 #include <cuda.h>  // CUtensorMap (types only; the encoder is fetched through cudaGetDriverEntryPoint -- no -lcuda)

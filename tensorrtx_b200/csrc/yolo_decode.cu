@@ -1,4 +1,4 @@
-// yolo_decode.cu -- YoloLayer_TRT hot path for sm_100a.
+// yolo_decode.cu -- YoloLayer_TRT hot path for sm_90a.
 //
 // Replaces CalDetection/forwardGpu of yolov8/plugin/yololayer.cu:178-316 (anchor-free) and
 // yolov5/plugin/yololayer.cu:161-227 (anchor-based) with
@@ -750,8 +750,9 @@ int yolo_fill_args(const trtx_yolo_params* p, int batch, const void* const* inpu
     const bool pipe = p->tune_tma_pipeline && p->variant == TRTX_YOLO_V8 && vec >= 4 && yolo_pipe_supported(p, inputs_dev);
     YoloLayout L = yolo_layout(p, batch, pipe ? 1 : vec);
     L.pipe = pipe ? 1 : 0;
+    // defaults chosen on an H100 for the overlapped step, not for the scan alone (DESIGN.md section 4.1, "Defaults")
     L.slices = p->tune_class_slices ? p->tune_class_slices : 2;
-    L.unroll = p->tune_rows_in_flight ? p->tune_rows_in_flight : (vec == 8 ? 10 : 5);  // B200 sweep, profiles/r02c_sweep_graph.log
+    L.unroll = p->tune_rows_in_flight ? p->tune_rows_in_flight : (vec == 8 ? 10 : 5);
     L.pipe_stages = p->tune_tma_stages;
     if (workspace_bytes < L.total_bytes) return TRTX_ERR_WORKSPACE;
     if (reinterpret_cast<uintptr_t>(workspace_dev) % 16 != 0) return TRTX_ERR_INVALID;
@@ -882,7 +883,7 @@ using namespace trtx;
 
 extern "C" {
 
-TRTX_API const char* trtx_version(void) { return "trtx_hot 0.1 (sm_100a)"; }
+TRTX_API const char* trtx_version(void) { return "trtx_hot 0.1 (sm_90a)"; }
 TRTX_API int trtx_last_cuda_error(void) { return g_last_cuda_error; }
 TRTX_API size_t trtx_abi_sizeof(int which) {
     switch (which) {

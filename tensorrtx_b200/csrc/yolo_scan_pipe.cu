@@ -1,4 +1,4 @@
-// yolo_scan_pipe.cu -- the YoloLayer scan as a persistent, TMA-fed pipeline (sm_100a).
+// yolo_scan_pipe.cu -- the YoloLayer scan as a persistent, TMA-fed pipeline (sm_90a).
 //
 // One CTA per SM, resident for the whole launch.  A producer thread streams 64-anchor tiles of the level
 // tensors (all C channel rows, 21.5 KB for YOLOv8 fp32) into a ring of shared-memory stages with ONE TMA
@@ -11,11 +11,11 @@
 // Warps never synchronise with each other; with 10 stages that is 20 consumer warps per SM, enough
 // thread-level parallelism to hide the LDS/ALU latency of the scan while TMA refills the other stages.
 //
-// Layouts tried before this one, kept for the record (profiles/r01b..r01d sweep logs): one 512-byte
-// cp.async.bulk per channel row (84 descriptors per tile throttle the copy engine: 1.7 TB/s); one tensor
-// copy per tile with all consumer warps cooperating on each tile (tiles strictly one after another:
-// 2.2 TB/s); one consumer warp per stage (5 warps per SM are latency-bound: 2.7 TB/s).
-// tools/tma_bench.cu measures the copy-engine ceiling of this access pattern: 5.3 TB/s.
+// Layouts tried before this one, kept for the record (tools/sweep_scan.py): one 512-byte
+// cp.async.bulk per channel row (84 descriptors per tile throttle the copy engine); one tensor
+// copy per tile with all consumer warps cooperating on each tile (tiles strictly one after another);
+// one consumer warp per stage (5 warps per SM are latency-bound).
+// tools/tma_bench.cu measures the copy-engine ceiling of this access pattern.
 //
 // The arithmetic is the same bit-exact running-max scheme as yolo_decode.cu::scan_classes.
 // HBM traffic = algorithmic bytes (every row is read exactly once); candidates add <= 4%.

@@ -60,7 +60,7 @@ class DetectionPipeline:
         of batch i are decoded while the frames of batch i+1 are pre-processed), so the two halves are issued as
         parallel branches: scan -> NMS on a high-priority side stream forked from the current stream, the letterbox on
         the current stream, joined at the end.  Captured into a CUDA graph this becomes two concurrent branches; the
-        latency-bound NMS (one CTA per image, 32 of 148 SMs) then runs underneath the HBM-bound letterbox instead of
+        latency-bound NMS (one CTA per image, 32 of 132 SMs) then runs underneath the HBM-bound letterbox instead of
         after it."""
         if not overlap or self._side is None or stream is not None:
             self.pre.enqueue(stream)

@@ -9,7 +9,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: run with -m gpu)")
 
 
 @pytest.fixture(scope="session")

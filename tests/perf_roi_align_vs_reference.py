@@ -1,6 +1,6 @@
 """Timing of the REFERENCE's own roiAlign (oracle/_ref/libref_rcnn.so, built from /root/reference/rcnn/RoiAlign.cu) next to
 trtx_roi_align on the same inputs -- test infrastructure (it executes oracle/_ref), not collected by pytest.
-Run on the GPU box: python tests/perf_roi_align_vs_reference.py   (profiles/r01k_roi_probe.log)"""
+Run on a GPU: python tests/perf_roi_align_vs_reference.py"""
 import runpy
 import sys
 from pathlib import Path

@@ -25,7 +25,7 @@ def test_library_exports_every_declared_symbol():
     assert declared == set(L.SYMBOLS), declared ^ set(L.SYMBOLS)
     for name in declared:
         assert hasattr(lib, name), name
-    assert b"sm_100a" in lib.trtx_version()
+    assert b"sm_90a" in lib.trtx_version()
     out = subprocess.run(["nm", "-D", "--defined-only", str(L.LIB_PATH)], capture_output=True, text=True).stdout
     exported = {l.split()[-1] for l in out.splitlines() if " T " in l}
     # exactly the declared C ABI is exported: no C++ symbols, no undeclared tuning / profiling hooks

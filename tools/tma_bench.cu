@@ -1,7 +1,7 @@
 // tma_bench.cu -- microbenchmark: how fast can a persistent CTA-per-SM kernel stream a [B, C, g] fp32 tensor
 // through shared memory with TMA tensor copies, as a function of box shape / stages / boxes per tile.
 // Consumers only wait + release (no compute), so this is the copy-engine ceiling for the scan kernel.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/tma_bench tools/tma_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/tma_bench tools/tma_bench.cu
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
