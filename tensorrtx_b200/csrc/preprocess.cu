@@ -5,7 +5,8 @@
 // and affine matrices in the kernel parameter block (no H2D copy of metadata); a warp covers 32
 // adjacent destination columns and every thread produces a strip of rows of its column.  Measured and
 // rejected: 4 adjacent pixels per lane (L1 sector-bound), staging the source band in shared
-// memory (2x slower).
+// memory (2x slower).  Sources that are only translated / padded into the network input (scale 1, e.g. 640x640 -> 640x640)
+// take letterbox_unit_kernel instead: full-width destination row bands whose source rows arrive by TMA (see below).
 //
 // Roofline: HBM-bound; algorithmic bytes per image = src_w*src_h*3 (u8 read once) +
 // 3*dst_w*dst_h*sizeof(out) (SURVEY 8d: 6 144 000 B for 640x640 -> 640x640 fp32).
@@ -182,8 +183,8 @@ __global__ void __launch_bounds__(256, 8) letterbox_kernel(const __grid_constant
 
 
 // =====================================================================================================================
-// Unit-scale letterbox, TMA-staged (the 640x640 -> 640x640 benchmark and every source that fits the network input in
-// one dimension: scale == 1, the image is only translated / padded).
+// Unit-scale letterbox, streamed in full-width row bands (the 640x640 -> 640x640 benchmark and every source that fits the
+// network input in one dimension: scale == 1, the image is only translated / padded).
 //
 // With scale == 1 the d2s matrix is {1, -0, tx, -0, 1, ty} with 2*tx, 2*ty integers (preprocess.cu:98-110), so for every
 // destination pixel  x_low = dx + ox,  y_low = dy + oy  and the bilinear fractions lx, ly are image-wide constants in
@@ -193,17 +194,22 @@ __global__ void __launch_bounds__(256, 8) letterbox_kernel(const __grid_constant
 // (:25-30: the weights sum to exactly 1).  The kernel is therefore bit-identical to the reference by construction;
 // tests assert array_equal against the reference's compiled kernel.
 //
-// A CTA owns a TW x TH destination tile.  Its (TH+1) x (TW+1)-pixel source window is fetched by ONE TMA tensor copy
-// (u8 tensor map over the image, box [kBoxBytes, TH+1]; rows/columns outside the image arrive as zeros and are patched
-// to 128 by the few border tiles) -- no per-lane byte loads, no address arithmetic per tap.  Each thread then produces
-// 4 ADJACENT pixels x 4 rows: per source row 4 conflict-free LDS.32 (15 bytes = 5 BGR pixels), every byte converted
-// once with one PRMT (byte -> mantissa of 2^23) + one FADD and shared by the 2x2 destination pixels that use it, and
-// one 16-byte store per plane and row (8 bytes for fp16 output).  Half-warps take row groups 4 rows apart, which puts
-// their LDS on disjoint banks (4 * 52 words = 16 mod 32).
-// Instructions per destination pixel: ~33 (the per-lane-byte-load kernel above: 79).
-constexpr int kUnitTW = 64;                   // destination columns per CTA = 16 lanes x 4 pixels
-constexpr int kUnitBoxBytes = 208;            // >= (kUnitTW + 1) * 3 = 195, multiple of 16 (TMA inner box extent)
+// The kernel is HBM-bound (4 output bytes per input byte for fp32) and streams at about the rate of a plain contiguous
+// u8 -> fp32 expand of the same bytes (tools/lb_ceiling, DESIGN 8).  A CTA owns kUnitBand destination rows x ALL dw columns
+// of one image: every plane of a CTA is one contiguous run of kUnitBand * dw outputs, every warp store instruction writes
+// 512 contiguous bytes (32 lanes x 4 pixels x fp32), and the band's source window -- kUnitBand + 1 whole source rows --
+// arrives by TMA tensor copies: a u8 tensor map over the image(s), boxes of [kUnitBoxBytes, kUnitBand + 1] laid side by side
+// in shared memory (box k holds byte columns [256k, 256k + 256) of every window row).  Rows / columns outside the image
+// arrive as zeros (hardware bounds check: no byte outside the image is read) and the taps there are replaced by 128 with
+// selects.  Each thread produces 4 ADJACENT pixels x kUnitBand rows: per source row 4 conflict-free LDS.32 (15 bytes = 5 BGR
+// pixels; lanes 12 bytes apart hit 32 distinct banks, and a box boundary moves the address by a multiple of 128 bytes),
+// every byte converted once with one PRMT (byte -> mantissa of 2^23) + one FADD, a horizontal pass shared by the two
+// destination rows that use the source row, and one 16-byte store per plane and row (8 bytes for fp16).  CTAs are
+// short-lived (one band each, 10 KB of shared memory at 640 columns), so SMs free up for concurrent work as the grid drains.
+constexpr int kUnitBand = 4;             // destination rows per CTA (8 measured slower)
+constexpr int kUnitBoxBytes = 256;       // TMA inner box extent: the most one box may span
 constexpr int kMaxUnitImages = 64;
+constexpr int kUnitMaxThreads = 160;     // 640 columns = 160 threads x 4 pixels; wider inputs loop
 
 struct UnitImage {
     int ox, oy;    // x_low(dx = 0), y_low(dy = 0)
@@ -216,100 +222,97 @@ struct alignas(64) UnitArgs {
     CUtensorMap map[kMaxUnitImages];
     UnitImage img[kMaxUnitImages];
     int dw, dh;
+    int nbox;  // boxes per window row: nbox * kUnitBoxBytes >= 3 * dw + 4 (the last thread's 16 bytes)
 };
 
-template <typename OutT, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32) letterbox_unit_kernel(const __grid_constant__ UnitArgs a, OutT* __restrict__ dst) {
-    constexpr int TW = kUnitTW, TH = WARPS * 8, BOXW = kUnitBoxBytes, ROWS = TH + 1;
-    __shared__ __align__(128) uint8_t box[ROWS * BOXW];
+template <typename OutT, int BAND>
+__global__ void __launch_bounds__(kUnitMaxThreads) letterbox_unit_kernel(const __grid_constant__ UnitArgs a, OutT* __restrict__ dst) {
+    constexpr int ROWS = BAND + 1, BOXW = kUnitBoxBytes, BOXB = ROWS * BOXW;
+    extern __shared__ __align__(128) uint8_t win[];  // a.nbox boxes of [ROWS][BOXW]
     __shared__ uint64_t bar;
-    const int tid = threadIdx.x;
-    const UnitImage& im = a.img[blockIdx.z];
-    const int dx0 = blockIdx.x * TW, dy0 = blockIdx.y * TH;
-    const int sx0 = dx0 + im.ox, sy0 = dy0 + im.oy;  // source pixel under the tile's first tap
+    const int tid = threadIdx.x, nt = blockDim.x;
+    const UnitImage& im = a.img[blockIdx.y];
+    const int dw = a.dw, dy0 = blockIdx.x * BAND;
+    const int sx0 = im.ox, sy0 = dy0 + im.oy;  // source pixel under the band's first tap
     const int sw = im.sw, sh = im.sh;
-    const bool all_out = sx0 + TW < 0 || sx0 >= sw || sy0 + TH < 0 || sy0 >= sh;
-    const bool interior = sx0 >= 0 && sx0 + TW < sw && sy0 >= 0 && sy0 + TH < sh;
+    const int nbox = a.nbox;
+    // window byte column c of window row r
+    auto at = [&](int c, int r) { return (c >> 8) * BOXB + r * BOXW + (c & (BOXW - 1)); };
 
-    if (tid == 0) {
-        mbar_init(&bar, 1);
-        mbar_fence_init();
-    }
-    __syncthreads();
-    if (!all_out) {
+    if (sy0 + BAND >= 0 && sy0 < sh) {  // a pure padding band fetches nothing: every tap is the border value
         if (tid == 0) {
-            mbar_arrive_expect_tx(&bar, ROWS * BOXW);
-            tma_load_3d(box, &a.map[im.map], sx0 * 3, sy0, im.z, &bar);
+            mbar_init(&bar, 1);
+            mbar_fence_init();
+        }
+        __syncthreads();
+        if (tid < 32) {
+            if (tid == 0) mbar_arrive_expect_tx(&bar, nbox * BOXB);
+            __syncwarp();
+            for (int k = tid; k < nbox; k += 32) tma_load_3d(win + k * BOXB, &a.map[im.map], sx0 * 3 + k * BOXW, sy0, im.z, &bar);
         }
         mbar_wait(&bar, 0);
-        if (!interior) {
-            // border tile: pixels of the window outside the image -> const_value_st = 128 (preprocess.cu:115)
-            for (int i = tid; i < ROWS * (TW + 1); i += WARPS * 32) {
-                const int r = i / (TW + 1), c = i - r * (TW + 1);
-                const int y = sy0 + r, x = sx0 + c;
-                if (y < 0 || y >= sh || x < 0 || x >= sw) {
-                    uint8_t* q = box + r * BOXW + c * 3;
-                    q[0] = 128;
-                    q[1] = 128;
-                    q[2] = 128;
-                }
-            }
-            __syncthreads();
-        }
-    } else {  // pure padding tile: every tap is the border value
-        for (int i = tid; i < ROWS * BOXW / 4; i += WARPS * 32) reinterpret_cast<uint32_t*>(box)[i] = 0x80808080u;
-        __syncthreads();
     }
+    const bool rows_in = sy0 >= 0 && sy0 + BAND < sh;  // every window row inside the image
 
-    const int lane = tid & 31, warp = tid >> 5;
-    const int k = lane & 15;
-    const int r0 = warp * 8 + (lane >> 4) * 4;  // half-warps 4 rows apart: disjoint banks
-    const int dx = dx0 + 4 * k;
-    if (dx >= a.dw) return;
     const float lx = im.lx, ly = im.ly, hx = 1 - lx, hy = 1 - ly;
-    const float w1 = hy * hx, w2 = hy * lx, w3 = ly * hx, w4 = ly * lx;  // preprocess.cu:34-35
-    const size_t area = (size_t)a.dw * a.dh;
-    OutT* o = dst + (size_t)im.dst_idx * 3 * area + (size_t)(dy0 + r0) * a.dw + dx;
-    const uint8_t* p = box + r0 * BOXW + 12 * k;
-
-    auto load_row = [&](const uint8_t* q, float (&t)[15]) {
-        uint32_t w[4];
+    const size_t area = (size_t)dw * a.dh;
+    const int rows = a.dh - dy0;  // destination rows of this band
+    for (int x4 = tid; x4 < dw / 4; x4 += nt) {
+        const int dx = 4 * x4;
+        OutT* o = dst + (size_t)im.dst_idx * 3 * area + (size_t)dy0 * dw + dx;
+        int off[4];  // the thread's 16 window bytes 12 * x4 .. 12 * x4 + 15, as 4 words (a word never straddles two boxes)
 #pragma unroll
-        for (int j = 0; j < 4; ++j) w[j] = reinterpret_cast<const uint32_t*>(q)[j];
+        for (int j = 0; j < 4; ++j) off[j] = at(12 * x4 + 4 * j, 0);
+        unsigned xin = 0;  // bit p: the thread's window pixel p (source column sx0 + dx + p) lies inside the image
 #pragma unroll
-        for (int i = 0; i < 15; ++i)  // byte i -> float: 2^23 + v is exact with v in the mantissa
-            t[i] = __uint_as_float(__byte_perm(w[i >> 2], 0x4B000000u, 0x7650u + (i & 3))) - 8388608.0f;
-    };
-    float top[15], bot[15];
-    load_row(p, top);
-    const int rows = a.dh - (dy0 + r0);  // rows of this strip inside the destination
+        for (int p = 0; p < 5; ++p) xin |= (unsigned)(sx0 + dx + p >= 0 && sx0 + dx + p < sw) << p;
+        // horizontal pass of window row r: h[3j + c] = hx * px[j][c] + lx * px[j + 1][c] for the thread's 4 pixels (exact)
+        auto hrow = [&](int r, float (&h)[12]) {
+            uint32_t w[4];
 #pragma unroll
-    for (int r = 0; r < 4; ++r) {
-        load_row(p + (r + 1) * BOXW, bot);
-        if (r < rows) {
-            float v[3][4];
+            for (int j = 0; j < 4; ++j) w[j] = *reinterpret_cast<const uint32_t*>(win + off[j] + r * BOXW);
+            float t[15];
 #pragma unroll
-            for (int j = 0; j < 4; ++j)
+            for (int i = 0; i < 15; ++i)  // byte i -> float: 2^23 + v is exact with v in the mantissa
+                t[i] = __uint_as_float(__byte_perm(w[i >> 2], 0x4B000000u, 0x7650u + (i & 3))) - 8388608.0f;
+            if (!(rows_in && xin == 0x1fu)) {  // taps outside the image -> const_value_st = 128 (preprocess.cu:115)
+                const bool yin = sy0 + r >= 0 && sy0 + r < sh;
 #pragma unroll
-                for (int c = 0; c < 3; ++c)  // :59-61, bgr -> rgb and /255 :64-74
-                    v[c][j] = div255(w1 * top[3 * j + c] + w2 * top[3 * j + 3 + c] + w3 * bot[3 * j + c] + w4 * bot[3 * j + 3 + c]);
-            OutT* orow = o + (size_t)r * a.dw;
+                for (int i = 0; i < 15; ++i) t[i] = yin && (xin >> (i / 3) & 1u) ? t[i] : 128.0f;
+            }
 #pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                OutT* q = orow + (size_t)(2 - c) * area;
-                if constexpr (sizeof(OutT) == 4) {
-                    *reinterpret_cast<float4*>(q) = make_float4(v[c][0], v[c][1], v[c][2], v[c][3]);
-                } else {
-                    const __half2 h0 = __floats2half2_rn(v[c][0], v[c][1]), h1 = __floats2half2_rn(v[c][2], v[c][3]);
-                    uint2 u;
-                    u.x = *reinterpret_cast<const uint32_t*>(&h0);
-                    u.y = *reinterpret_cast<const uint32_t*>(&h1);
-                    *reinterpret_cast<uint2*>(q) = u;
+            for (int i = 0; i < 12; ++i) h[i] = hx * t[i] + lx * t[i + 3];
+        };
+        float top[12], bot[12];
+        hrow(0, top);
+#pragma unroll
+        for (int r = 0; r < BAND; ++r) {
+            hrow(r + 1, bot);
+            if (r < rows) {
+                float v[3][4];
+#pragma unroll
+                for (int j = 0; j < 4; ++j)
+#pragma unroll
+                    for (int c = 0; c < 3; ++c)  // :59-61 regrouped (exact), bgr -> rgb and /255 :64-74
+                        v[c][j] = div255(hy * top[3 * j + c] + ly * bot[3 * j + c]);
+                OutT* orow = o + (size_t)r * dw;
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {
+                    OutT* q = orow + (size_t)(2 - c) * area;
+                    if constexpr (sizeof(OutT) == 4) {
+                        *reinterpret_cast<float4*>(q) = make_float4(v[c][0], v[c][1], v[c][2], v[c][3]);
+                    } else {
+                        const __half2 h0 = __floats2half2_rn(v[c][0], v[c][1]), h1 = __floats2half2_rn(v[c][2], v[c][3]);
+                        uint2 u;
+                        u.x = *reinterpret_cast<const uint32_t*>(&h0);
+                        u.y = *reinterpret_cast<const uint32_t*>(&h1);
+                        *reinterpret_cast<uint2*>(q) = u;
+                    }
                 }
             }
-        }
 #pragma unroll
-        for (int i = 0; i < 15; ++i) top[i] = bot[i];
+            for (int i = 0; i < 12; ++i) top[i] = bot[i];
+        }
     }
 }
 
@@ -322,9 +325,9 @@ static bool unit_scale_image(const trtx_image_desc& d, const float m[6], UnitIma
     if (reinterpret_cast<uintptr_t>(d.data_dev) % 16 != 0 || d.pitch % 16 != 0) return false;  // TMA base / stride
     u->ox = (int)floorf(tx);
     u->oy = (int)floorf(ty);
-    // TMA fetches the box from byte column 3 * (64 * tile + ox): the start of a box must be 16-byte aligned in global memory
-    // (an unaligned start is an illegal instruction on sm_90a), so horizontal offsets that are not a multiple of 16 pixels
-    // (e.g. a 624-wide source centred in 640) take the general kernel
+    // TMA fetches box k of a window from byte column 3 * ox + 256 * k: the start of a box must be 16-byte aligned in global
+    // memory (an unaligned start is an illegal instruction on sm_90a), so horizontal offsets that are not a multiple of 16
+    // pixels (e.g. a 624-wide source centred in 640) take the general kernel
     if (u->ox % 16 != 0) return false;
     u->lx = tx - floorf(tx);
     u->ly = ty - floorf(ty);
@@ -333,29 +336,41 @@ static bool unit_scale_image(const trtx_image_desc& d, const float m[6], UnitIma
     return true;
 }
 
-static bool encode_image_map(CUtensorMap* map, const uint8_t* base, int sw, int sh, int pitch, int n, size_t image_stride,
-                             int box_rows) {
+static bool encode_image_map(CUtensorMap* map, const uint8_t* base, int sw, int sh, int pitch, int n, size_t image_stride) {
     EncodeTiledFn enc = tma_encoder();
     if (!enc) return false;
     const cuuint64_t gdim[3] = {(cuuint64_t)sw * 3u, (cuuint64_t)sh, (cuuint64_t)n};
     const cuuint64_t gstr[2] = {(cuuint64_t)pitch, (cuuint64_t)image_stride};
-    const cuuint32_t bdim[3] = {(cuuint32_t)kUnitBoxBytes, (cuuint32_t)box_rows, 1u};
+    const cuuint32_t bdim[3] = {(cuuint32_t)kUnitBoxBytes, (cuuint32_t)(kUnitBand + 1), 1u};
     const cuuint32_t estr[3] = {1u, 1u, 1u};
     return enc(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<uint8_t*>(base), gdim, gstr, bdim, estr,
                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-constexpr int kUnitWarps = 4;
-
 // Launch the unit-scale kernel for `n` images (descriptors d[i], unit info u[i] already filled but for map/z).
-// Returns TRTX_ERR_UNSUPPORTED when no tensor map can be made (caller falls back to the general kernel).
+// Returns TRTX_ERR_UNSUPPORTED when no tensor map can be made or the window does not fit in shared memory (the caller
+// falls back to the general kernel).
+template <typename OutT>
+static int launch_unit_t(const UnitArgs& a, int n, size_t smem, OutT* dst, cudaStream_t st) {
+    auto* k = letterbox_unit_kernel<OutT, kUnitBand>;
+    if (smem > 48 * 1024 && cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+        cudaGetLastError();
+        return TRTX_ERR_UNSUPPORTED;
+    }
+    const int threads = min((a.dw / 4 + kWarp - 1) / kWarp * kWarp, kUnitMaxThreads);
+    k<<<dim3((a.dh + kUnitBand - 1) / kUnitBand, n), threads, smem, st>>>(a, dst);
+    return check_launch();
+}
+
 static int launch_unit(const trtx_image_desc* const* d, UnitImage* u, int n, void* dst, int dw, int dh, int out_dtype,
                        cudaStream_t st) {
     UnitArgs a;
     a.dw = dw;
     a.dh = dh;
-    constexpr int box_rows = kUnitWarps * 8 + 1;
+    a.nbox = (3 * dw + 4 + kUnitBoxBytes - 1) / kUnitBoxBytes;
+    const size_t smem = (size_t)a.nbox * kUnitBoxBytes * (kUnitBand + 1);
+    if (smem > 227 * 1024) return TRTX_ERR_UNSUPPORTED;
     // one 3-D map for the whole group when the images are equally sized and equally spaced (a frame ring / one batch
     // tensor): one encode instead of n
     bool uniform = n > 1;
@@ -365,7 +380,7 @@ static int launch_unit(const trtx_image_desc* const* d, UnitImage* u, int n, voi
                   d[i]->data_dev - d[i - 1]->data_dev == step;
     uniform = uniform && step > 0 && step % 16 == 0 && (size_t)step >= (size_t)d[0]->pitch * (size_t)d[0]->height;
     if (uniform) {
-        if (!encode_image_map(&a.map[0], d[0]->data_dev, d[0]->width, d[0]->height, d[0]->pitch, n, (size_t)step, box_rows))
+        if (!encode_image_map(&a.map[0], d[0]->data_dev, d[0]->width, d[0]->height, d[0]->pitch, n, (size_t)step))
             return TRTX_ERR_UNSUPPORTED;
     }
     for (int i = 0; i < n; ++i) {
@@ -374,19 +389,15 @@ static int launch_unit(const trtx_image_desc* const* d, UnitImage* u, int n, voi
             u[i].z = i;
         } else {
             if (!encode_image_map(&a.map[i], d[i]->data_dev, d[i]->width, d[i]->height, d[i]->pitch, 1,
-                                  (size_t)d[i]->pitch * (size_t)d[i]->height, box_rows))
+                                  (size_t)d[i]->pitch * (size_t)d[i]->height))
                 return TRTX_ERR_UNSUPPORTED;
             u[i].map = i;
             u[i].z = 0;
         }
         a.img[i] = u[i];
     }
-    dim3 grid((dw + kUnitTW - 1) / kUnitTW, (dh + kUnitWarps * 8 - 1) / (kUnitWarps * 8), n);
-    if (out_dtype == TRTX_F32)
-        letterbox_unit_kernel<float, kUnitWarps><<<grid, kUnitWarps * 32, 0, st>>>(a, static_cast<float*>(dst));
-    else
-        letterbox_unit_kernel<__half, kUnitWarps><<<grid, kUnitWarps * 32, 0, st>>>(a, static_cast<__half*>(dst));
-    return check_launch();
+    if (out_dtype == TRTX_F32) return launch_unit_t(a, n, smem, static_cast<float*>(dst), st);
+    return launch_unit_t(a, n, smem, static_cast<__half*>(dst), st);
 }
 
 }  // namespace trtx
