@@ -49,7 +49,7 @@ TRTX_API const char* trtx_version(void);
 TRTX_API int trtx_last_cuda_error(void);
 /* sizeof() of the parameter structs as THIS library was compiled, so that an FFI binding (ctypes, cgo, ...) can check its
  * mirror of the layout: which = 0 trtx_yolo_params, 1 trtx_nms_params, 2 trtx_retina_params, 3 trtx_image_desc,
- * 4 trtx_mask_params; anything else 0. */
+ * 4 trtx_mask_params, 5 trtx_rcnn_post_params; anything else 0. */
 TRTX_API size_t trtx_abi_sizeof(int which);
 
 /* =====================================================================================
@@ -406,6 +406,38 @@ typedef struct trtx_mask_params {
  * masks_dev: [batch, max_masks, net_h, net_w] fp32; slots >= count are left untouched.  One launch. */
 TRTX_API int trtx_process_mask_enqueue(const trtx_mask_params* p, int batch, const float* proto_dev, const float* dets_dev,
                                        int max_rows, float* masks_dev, trtx_stream_t stream);
+
+/* =====================================================================================
+ * 7. Mask R-CNN post-process
+ *    replaces the HOST loop of rcnn/rcnn.cpp:516-550, which runs after a D2H copy of BatchedNms's and
+ *    MaskRcnnInference's outputs: rescale every box with score > SCORE_THRESH from the padded network
+ *    input to the original image, and (MASK_ON) paste its mask into a w_ori x h_ori 8-bit canvas.
+ * ===================================================================================== */
+/* The four pads preprocessImg writes (rcnn/common.hpp:79-102), pads = {left, right, top, bottom}.  net_w / net_h are the
+ * model input (INPUT_W / INPUT_H of calculateSize, rcnn/rcnn.cpp:349-366).  Host function. */
+TRTX_API int trtx_rcnn_letterbox_pads(int img_w, int img_h, int net_w, int net_h, int pads[4]);
+
+typedef struct trtx_rcnn_post_params {
+    int32_t net_w, net_h;      /* INPUT_W, INPUT_H */
+    int32_t img_w, img_h;      /* w_ori, h_ori: one original size per call (mixed sizes: one call each, offset pointers) */
+    int32_t detections_per_im; /* DETECTIONS_PER_IMAGE (100): rows of BatchedNms's outputs */
+    int32_t mask_size;         /* POOLER_RESOLUTION (14): masks are [S, S]; at most 32 */
+    int32_t max_masks;         /* canvases written per image: the first min(count, max_masks) kept rows */
+    float score_thresh;        /* SCORE_THRESH (0.6f); kept when score > score_thresh (a NaN score is not kept) */
+} trtx_rcnn_post_params;
+
+/* scores_dev [B, D], boxes_dev [B, D, 4] (x1, y1, x2, y2 in network-input pixels), classes_dev [B, D]: BatchedNms outputs;
+ * masks_dev [B, D, S, S]: MaskRcnnInference output, or NULL for boxes only (Faster R-CNN, MASK_ON off).
+ * rows_dev [B, 1 + D*7]: per image a count, then one row (x1, y1, x2, y2, score, class, slot) per slot i with
+ *   score > score_thresh, in ascending i (the reference's loop order); slot = i indexes the inputs.  The box is
+ *   (box - pad) * ratio with ratio = (float)img / (net - (pad_a + pad_b)) (rcnn.cpp:516-526).  Rows past the count are zeroed.
+ * masks_out_dev [B, max_masks, img_h, img_w] u8, or NULL (both mask pointers NULL or both non-NULL): canvas k of image b is
+ *   255 where cv::resize(mask, r.size()) (bilinear) > 0.5 inside the paste rectangle r of the k-th kept row (:543-550) and 0
+ *   elsewhere; all zeros where the reference throws (empty r, r leaving the image, non-finite box).  Canvases at or past
+ *   min(count, max_masks) are left untouched.  Two launches, no workspace. */
+TRTX_API int trtx_rcnn_postprocess_enqueue(const trtx_rcnn_post_params* p, int batch, const float* scores_dev,
+                                           const float* boxes_dev, const float* classes_dev, const float* masks_dev,
+                                           float* rows_dev, uint8_t* masks_out_dev, trtx_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -93,6 +93,11 @@ class MaskParams(C.Structure):
                                          "coeff_offset", "max_masks")]
 
 
+class RcnnPostParams(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("net_w", "net_h", "img_w", "img_h", "detections_per_im", "mask_size", "max_masks")] + \
+               [("score_thresh", C.c_float)]
+
+
 # TRTX_LIB: another build of the same ABI (the probe build of tools/nms_probe.py); default = the in-tree release library
 LIB_PATH = Path(os.environ.get("TRTX_LIB") or Path(__file__).resolve().parent / "lib" / "libtrtx_hot.so")
 
@@ -133,6 +138,8 @@ SYMBOLS = {
     "trtx_process_decode_ptr_host_obb": (_i, [C.POINTER(C.c_float), _i, _i, C.POINTER(C.c_float)]),
     "trtx_scale_mask_rect": (_i, [_i, _i, _i, _i, C.POINTER(C.c_int)]),
     "trtx_scale_mask_enqueue": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    "trtx_rcnn_letterbox_pads": (_i, [_i, _i, _i, _i, C.POINTER(C.c_int)]),
+    "trtx_rcnn_postprocess_enqueue": (_i, [C.POINTER(RcnnPostParams), _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "trtx_yolo_decode_nms_gather_enqueue": (_i, [C.POINTER(YoloParams), C.POINTER(NmsParams), _i, _pp, _vp, _vp, _vp, _sz,
                                                  C.POINTER(Gather), _vp]),
     "trtx_gather_wait_enqueue": (_i, [C.POINTER(Gather), _vp]),
@@ -163,7 +170,7 @@ def load() -> C.CDLL:
         fn = getattr(lib, name)  # AttributeError if the library does not export a declared symbol
         fn.restype = res
         fn.argtypes = args
-    for which, st in enumerate((YoloParams, NmsParams, RetinaParams, ImageDesc, MaskParams)):
+    for which, st in enumerate((YoloParams, NmsParams, RetinaParams, ImageDesc, MaskParams, RcnnPostParams)):
         if lib.trtx_abi_sizeof(which) != C.sizeof(st):
             raise TrtxError(f"{LIB_PATH} was built from a different trtx_hot.h: sizeof({st.__name__}) = "
                             f"{lib.trtx_abi_sizeof(which)} in the library, {C.sizeof(st)} in the binding (rebuild)")

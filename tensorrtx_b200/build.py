@@ -89,10 +89,11 @@ def build(force: bool = False, verbose: bool = False, probe: bool = False, defin
 
 
 def build_oracle() -> Path:
-    """Compile the CPU oracle (test infrastructure) and, when /root/reference exists, oracle/_ref."""
-    r = subprocess.run(["make", "-C", str(ROOT / "oracle")], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    if r.returncode != 0:
-        raise RuntimeError(f"oracle build failed:\n{r.stdout}")
+    """Compile the CPU oracles (test infrastructure) and, when /root/reference exists, oracle/_ref."""
+    for extra in ([], ["-f", "rcnn_post.mk"]):   # rcnn_post.mk: the Mask R-CNN post-process oracle and its reference build
+        r = subprocess.run(["make", "-C", str(ROOT / "oracle"), *extra], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+        if r.returncode != 0:
+            raise RuntimeError(f"oracle build failed:\n{r.stdout}")
     return ROOT / "oracle" / "libtrtx_oracle.so"
 
 

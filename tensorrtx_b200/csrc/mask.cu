@@ -16,6 +16,9 @@
 // without FMA contraction), sigmoid is 1/(1+expf(-e)) (CUDA expf vs glibc expf: <= 2 ulp); the resize follows OpenCV's
 // float bilinear kernel: fx = (dx + 0.5) * (src/dst) - 0.5, sx = floor(fx) clamped to [0, src-1] (fraction 0 when
 // clamped), horizontal pass then vertical pass, every product and sum rounded to float.
+//
+// Also here: scale_mask of the yolov8 seg driver, and the Mask R-CNN post-process of rcnn/rcnn.cpp:516-550 (box rescale to
+// the original image, mask paste into u8 canvases), which reuses the same resize taps.
 #include "common.cuh"
 
 namespace trtx {
@@ -201,6 +204,148 @@ __global__ void __launch_bounds__(256) scale_mask_kernel(const __grid_constant__
     }
 }
 
+// Mask R-CNN post-process, rcnn/rcnn.cpp:516-550 (host code in the reference).  Two launches, stream-ordered, no workspace:
+//   rcnn_rows_kernel  one warp per image: keeps slot i when score > thresh (ascending i), rescales its box to the original
+//                     image, (box - pad) * ratio unfused (:523-526), and zeroes the rows past the count;
+//   rcnn_paste_kernel one CTA per (image, mask slot, band of full-width rows): the canvas of the k-th kept row is 255 where
+//                     cv::resize(mask, r.size()) > 0.5 inside the paste rectangle r (:543-550), 0 elsewhere.
+// The paste is bound by HBM writes (one byte per canvas pixel).  Each thread owns 16 adjacent columns (one 16-byte store per
+// row) and computes their horizontal taps once for all the rows of its band; a band that misses r's rows stores zeros only.
+constexpr int kRcnnRowFloats = 7;      // x1, y1, x2, y2, score, class, slot
+constexpr int kRcnnMaxMask = 32;       // largest mask_size the shared-memory stage holds
+constexpr int kPasteThreads = 256;
+constexpr int kPastePasses = 8;        // row passes per CTA: band = kPastePasses * blockDim.y rows (~30 KB)
+
+struct RcnnRowsArgs {
+    const float* scores;   // [B, D]
+    const float* boxes;    // [B, D, 4]
+    const float* classes;  // [B, D]
+    float* rows;           // [B, 1 + D * 7]
+    int batch, dets;
+    float thresh;
+    int pad_l, pad_t;
+    float w_ratio, h_ratio;
+};
+
+__global__ void __launch_bounds__(128) rcnn_rows_kernel(const __grid_constant__ RcnnRowsArgs a) {
+    const int b = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (b >= a.batch) return;
+    const size_t base = (size_t)b * a.dets;
+    float* out = a.rows + (size_t)b * (1 + (size_t)a.dets * kRcnnRowFloats);
+    int n = 0;
+    for (int i0 = 0; i0 < a.dets; i0 += 32) {
+        const int i = i0 + lane;
+        const float s = i < a.dets ? a.scores[base + i] : 0.0f;
+        const bool keep = i < a.dets && s > a.thresh;  // :522; a NaN score is not kept
+        const unsigned m = __ballot_sync(0xffffffffu, keep);
+        if (keep) {
+            float* r = out + 1 + (size_t)(n + __popc(m & ((1u << lane) - 1u))) * kRcnnRowFloats;
+            const float* bx = a.boxes + (base + i) * 4;
+            r[0] = __fmul_rn(__fsub_rn(bx[0], (float)a.pad_l), a.w_ratio);
+            r[1] = __fmul_rn(__fsub_rn(bx[1], (float)a.pad_t), a.h_ratio);
+            r[2] = __fmul_rn(__fsub_rn(bx[2], (float)a.pad_l), a.w_ratio);
+            r[3] = __fmul_rn(__fsub_rn(bx[3], (float)a.pad_t), a.h_ratio);
+            r[4] = s;
+            r[5] = a.classes[base + i];
+            r[6] = (float)i;
+        }
+        n += __popc(m);
+    }
+    for (int e = n * kRcnnRowFloats + lane; e < a.dets * kRcnnRowFloats; e += 32) out[1 + e] = 0.0f;
+    if (lane == 0) out[0] = (float)n;
+}
+
+// One axis of the paste rectangle (:543-546): floor(lo) - 1 clamped at 0, ceil(hi) + 1 clamped at `size`, then cv::Rect's
+// normalisation (min corner, |delta|).  False where the reference throws: a corner outside the image makes
+// Mat::operator()(Rect) throw, an empty size makes cv::resize throw.  In float, floor(c) - 1 is exact wherever it can
+// land inside the image, so the comparisons match the reference's double ones.
+__device__ __forceinline__ bool rcnn_rect_axis(float c0, float c1, int size, int& o, int& len) {
+    float lo = floorf(c0) - 1.0f;
+    lo = lo < 0.0f ? 0.0f : lo;
+    float hi = ceilf(c1) + 1.0f;
+    hi = hi > (float)size ? (float)size : hi;
+    if (lo > (float)size || hi < 0.0f) return false;
+    const int p = (int)lo, q = (int)hi;
+    o = min(p, q);
+    len = abs(q - p);
+    return len > 0;
+}
+
+__device__ __forceinline__ bool rcnn_mask_rect(const float* r, int img_w, int img_h, int& rx, int& ry, int& rw, int& rh) {
+    if (!(isfinite(r[0]) && isfinite(r[1]) && isfinite(r[2]) && isfinite(r[3]))) return false;
+    return rcnn_rect_axis(r[0], r[2], img_w, rx, rw) && rcnn_rect_axis(r[1], r[3], img_h, ry, rh);
+}
+
+struct RcnnPasteArgs {
+    const float* rows;   // [B, 1 + D * 7], written by rcnn_rows_kernel
+    const float* masks;  // [B, D, S, S]
+    uint8_t* out;        // [B, max_masks, img_h, img_w]
+    int dets, S, img_w, img_h, max_masks;
+    int chunks, bands, band_rows;  // 16-column chunks per row; bands per canvas; rows per band
+};
+
+__global__ void __launch_bounds__(kPasteThreads) rcnn_paste_kernel(const __grid_constant__ RcnnPasteArgs a) {
+    __shared__ float s_m[kRcnnMaxMask * kRcnnMaxMask];
+    const int item = blockIdx.x / a.bands, band = blockIdx.x - item * a.bands;
+    const int b = item / a.max_masks, k = item - b * a.max_masks;
+    const float* img = a.rows + (size_t)b * (1 + (size_t)a.dets * kRcnnRowFloats);
+    const int count = min((int)img[0], min(a.dets, a.max_masks));
+    if (k >= count) return;  // slots past the image's kept rows are left untouched
+    const float* row = img + 1 + (size_t)k * kRcnnRowFloats;
+    int rx = 0, ry = 0, rw = 1, rh = 1;
+    const bool pasted = rcnn_mask_rect(row, a.img_w, a.img_h, rx, ry, rw, rh);
+    const int y0 = band * a.band_rows, y1 = min(y0 + a.band_rows, a.img_h);
+    const bool touches = pasted && ry < y1 && ry + rh > y0;  // uniform over the CTA
+    const int S = a.S;
+    if (touches) {
+        const float* m = a.masks + ((size_t)b * a.dets + (int)row[6]) * S * S;
+        for (int e = threadIdx.y * blockDim.x + threadIdx.x; e < S * S; e += blockDim.x * blockDim.y) s_m[e] = m[e];
+        __syncthreads();
+    }
+    const double scale_x = (double)S / (double)rw, scale_y = (double)S / (double)rh;
+    uint8_t* plane = a.out + ((size_t)b * a.max_masks + k) * (size_t)a.img_h * a.img_w;
+    for (int c = threadIdx.x; c < a.chunks; c += blockDim.x) {
+        const int x0 = c * 16;
+        int sx[16];
+        float fx[16];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            sx[j] = -1;  // outside r: 0
+            fx[j] = 0.0f;
+            if (touches && x0 + j >= rx && x0 + j < rx + rw) resize_tap(x0 + j - rx, scale_x, S, sx[j], fx[j]);
+        }
+        for (int y = y0 + threadIdx.y; y < y1; y += blockDim.y) {
+            uint32_t w[4] = {0u, 0u, 0u, 0u};
+            if (touches && y >= ry && y < ry + rh) {
+                int sy;
+                float fy;
+                resize_tap(y - ry, scale_y, S, sy, fy);
+                const float* r0 = s_m + sy * S;
+                const float* r1 = s_m + min(sy + 1, S - 1) * S;
+                const float b0 = 1.0f - fy, b1 = fy;
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    if (sx[j] < 0) continue;
+                    const int sx1 = min(sx[j] + 1, S - 1);
+                    const float a0 = 1.0f - fx[j], a1 = fx[j];
+                    const float h0 = __fadd_rn(__fmul_rn(r0[sx[j]], a0), __fmul_rn(r0[sx1], a1));  // HResizeLinear
+                    const float h1 = __fadd_rn(__fmul_rn(r1[sx[j]], a0), __fmul_rn(r1[sx1], a1));
+                    const float v = __fadd_rn(__fmul_rn(h0, b0), __fmul_rn(h1, b1));                // VResizeLinear
+                    if (v > 0.5f) w[j >> 2] |= 0xffu << (8 * (j & 3));                               // :549 threshold
+                }
+            }
+            uint8_t* dst = plane + (size_t)y * a.img_w + x0;
+            if (x0 + 16 <= a.img_w && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+                *reinterpret_cast<uint4*>(dst) = make_uint4(w[0], w[1], w[2], w[3]);
+            } else {  // unaligned rows (width not a multiple of 16) and the last chunk of a row
+#pragma unroll
+                for (int j = 0; j < 16; ++j)
+                    if (x0 + j < a.img_w) dst[j] = (uint8_t)(w[j >> 2] >> (8 * (j & 3)));
+            }
+        }
+    }
+}
+
 }  // namespace trtx
 
 using namespace trtx;
@@ -271,6 +416,83 @@ TRTX_API int trtx_scale_mask_enqueue(const float* masks_dev, int n, int net_w, i
     ScaleMaskArgs a{masks_dev, out_dev, net_w, net_h, img_w, img_h, r[0], r[1], r[2], r[3]};
     dim3 grid((img_w + 255) / 256, (img_h + 3) / 4, n);
     scale_mask_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
+    return check_launch();
+}
+
+// preprocessImg's pads, rcnn/common.hpp:79-102: `input_w / (img.cols*1.0)` is a double division stored to float, `r_w *
+// img.rows` a float product truncated to int, `(input_h - h) / 2.f` float; each pad is round() of that float -/+ 0.1 (double)
+TRTX_API int trtx_rcnn_letterbox_pads(int img_w, int img_h, int net_w, int net_h, int pads[4]) {
+    if (!pads || img_w <= 0 || img_h <= 0 || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
+    int w, h;
+    float x, y;
+    const float r_w = (float)(net_w / (img_w * 1.0));
+    const float r_h = (float)(net_h / (img_h * 1.0));
+    if (r_h > r_w) {
+        w = net_w;
+        h = (int)(r_w * (float)img_h);
+        x = 0.0f;
+        y = (float)(net_h - h) / 2.f;
+    } else {
+        w = (int)(r_h * (float)img_w);
+        h = net_h;
+        x = (float)(net_w - w) / 2.f;
+        y = 0.0f;
+    }
+    (void)w;
+    (void)h;
+    pads[0] = (int)round(x - 0.1);
+    pads[1] = (int)round(x + 0.1);
+    pads[2] = (int)round(y - 0.1);
+    pads[3] = (int)round(y + 0.1);
+    return TRTX_OK;
+}
+
+TRTX_API int trtx_rcnn_postprocess_enqueue(const trtx_rcnn_post_params* p, int batch, const float* scores_dev,
+                                           const float* boxes_dev, const float* classes_dev, const float* masks_dev,
+                                           float* rows_dev, uint8_t* masks_out_dev, trtx_stream_t stream) {
+    if (!p || batch <= 0 || !scores_dev || !boxes_dev || !classes_dev || !rows_dev) return TRTX_ERR_INVALID;
+    if ((masks_dev == nullptr) != (masks_out_dev == nullptr)) return TRTX_ERR_INVALID;
+    if (p->net_w <= 0 || p->net_h <= 0 || p->img_w <= 0 || p->img_h <= 0 || p->detections_per_im <= 0 || p->mask_size <= 0 ||
+        p->max_masks <= 0)
+        return TRTX_ERR_INVALID;
+    if (p->mask_size > kRcnnMaxMask) return TRTX_ERR_INVALID;
+    int pads[4];
+    trtx_rcnn_letterbox_pads(p->img_w, p->img_h, p->net_w, p->net_h, pads);
+    RcnnRowsArgs ra;
+    ra.scores = scores_dev;
+    ra.boxes = boxes_dev;
+    ra.classes = classes_dev;
+    ra.rows = rows_dev;
+    ra.batch = batch;
+    ra.dets = p->detections_per_im;
+    ra.thresh = p->score_thresh;
+    ra.pad_l = pads[0];
+    ra.pad_t = pads[2];
+    ra.h_ratio = (float)p->img_h / (float)(p->net_h - (pads[2] + pads[3]));  // rcnn.cpp:516-517
+    ra.w_ratio = (float)p->img_w / (float)(p->net_w - (pads[0] + pads[1]));
+    // bands of full-width rows: blockDim.x threads over the 16-column chunks, blockDim.y rows per pass
+    const int chunks = (p->img_w + 15) / 16;
+    const int tx = min(chunks, kPasteThreads), ty = kPasteThreads / tx;
+    const int band_rows = ty * kPastePasses, bands = (p->img_h + band_rows - 1) / band_rows;
+    const long long ctas = (long long)batch * p->max_masks * bands;
+    if (masks_dev && ctas > 0x7fffffffLL) return TRTX_ERR_UNSUPPORTED;
+    const cudaStream_t s = static_cast<cudaStream_t>(stream);
+    rcnn_rows_kernel<<<(batch + 3) / 4, 128, 0, s>>>(ra);
+    const int rc = check_launch();
+    if (rc || !masks_dev) return rc;
+    RcnnPasteArgs pa;
+    pa.rows = rows_dev;
+    pa.masks = masks_dev;
+    pa.out = masks_out_dev;
+    pa.dets = p->detections_per_im;
+    pa.S = p->mask_size;
+    pa.img_w = p->img_w;
+    pa.img_h = p->img_h;
+    pa.max_masks = p->max_masks;
+    pa.chunks = chunks;
+    pa.bands = bands;
+    pa.band_rows = band_rows;
+    rcnn_paste_kernel<<<(unsigned)ctas, dim3(tx, ty), 0, s>>>(pa);
     return check_launch();
 }
 

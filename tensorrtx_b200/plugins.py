@@ -988,6 +988,43 @@ def scale_mask(masks: torch.Tensor, img_w: int, img_h: int, out=None, stream=Non
     return out
 
 
+def rcnn_letterbox_pads(img_w: int, img_h: int, net_w: int, net_h: int):
+    """The pads preprocessImg (rcnn/common.hpp:79-102) puts around an img_w x img_h image in the net_w x net_h model input:
+    (left, right, top, bottom)."""
+    p = (C.c_int * 4)()
+    L.check(L.load().trtx_rcnn_letterbox_pads(img_w, img_h, net_w, net_h, p), "trtx_rcnn_letterbox_pads")
+    return tuple(p)
+
+
+def rcnn_postprocess(scores: torch.Tensor, boxes: torch.Tensor, classes: torch.Tensor, masks: torch.Tensor | None = None, *,
+                     img_w: int, img_h: int, net_w: int, net_h: int, score_thresh: float = 0.6, max_masks: int | None = None,
+                     out=None, stream=None):
+    """GPU drop-in for the post-process loop of rcnn/rcnn.cpp:516-550 for a batch of images of one original size.
+    scores [B, D], boxes [B, D, 4], classes [B, D] (BatchedNms outputs), masks [B, D, S, S] (MaskRcnnInference output) or
+    None -> (rows [B, 1 + D*7] fp32: count, then (x1, y1, x2, y2, score, class, slot) per kept detection in original-image
+    pixels; canvases [B, max_masks, img_h, img_w] uint8 with 255 inside each kept detection's pasted mask, or None).
+    `out` = (rows, canvases) to reuse buffers; canvases at or past an image's count are not written (new ones start zeroed)."""
+    lib = L.load()
+    B, D = scores.shape
+    S = 1 if masks is None else masks.shape[-1]
+    if tuple(boxes.shape) != (B, D, 4) or tuple(classes.shape) != (B, D) or (masks is not None and tuple(masks.shape) != (B, D, S, S)):
+        raise ValueError("expected scores [B, D], boxes [B, D, 4], classes [B, D], masks [B, D, S, S]")
+    max_masks = D if max_masks is None else int(max_masks)
+    q = L.RcnnPostParams(net_w, net_h, img_w, img_h, D, S, max_masks, score_thresh)
+    rows, canvases = out if out is not None else (None, None)
+    if rows is None:
+        rows = torch.empty((B, 1 + D * 7), dtype=torch.float32, device=scores.device)
+    if masks is not None and canvases is None:
+        canvases = torch.zeros((B, max_masks, img_h, img_w), dtype=torch.uint8, device=scores.device)
+    if masks is None:
+        canvases = None
+    L.check(lib.trtx_rcnn_postprocess_enqueue(C.byref(q), B, _ptr(scores), _ptr(boxes), _ptr(classes),
+                                              None if masks is None else _ptr(masks), _ptr(rows),
+                                              None if canvases is None else _ptr(canvases), _stream(stream)),
+            "trtx_rcnn_postprocess_enqueue")
+    return rows, canvases
+
+
 def letterbox_matrix(src_w: int, src_h: int, dst_w: int, dst_h: int):
     m = (C.c_float * 6)()
     L.load().trtx_letterbox_matrix(src_w, src_h, dst_w, dst_h, m)
