@@ -408,14 +408,26 @@ TRTX_API int trtx_process_mask_enqueue(const trtx_mask_params* p, int batch, con
                                        int max_rows, float* masks_dev, trtx_stream_t stream);
 
 /* =====================================================================================
- * 7. Mask R-CNN post-process
- *    replaces the HOST loop of rcnn/rcnn.cpp:516-550, which runs after a D2H copy of BatchedNms's and
- *    MaskRcnnInference's outputs: rescale every box with score > SCORE_THRESH from the padded network
- *    input to the original image, and (MASK_ON) paste its mask into a w_ori x h_ori 8-bit canvas.
+ * 7. Mask R-CNN pre- and post-process
+ *    replaces the HOST pre-process of rcnn/rcnn.cpp:497-506 (preprocessImg, a float widening loop, then an
+ *    H2D copy of the fp32 batch) and the HOST loop of rcnn/rcnn.cpp:516-550, which runs after a D2H copy of
+ *    BatchedNms's and MaskRcnnInference's outputs: rescale every box with score > SCORE_THRESH from the padded
+ *    network input to the original image, and (MASK_ON) paste its mask into a w_ori x h_ori 8-bit canvas.
  * ===================================================================================== */
 /* The four pads preprocessImg writes (rcnn/common.hpp:79-102), pads = {left, right, top, bottom}.  net_w / net_h are the
  * model input (INPUT_W / INPUT_H of calculateSize, rcnn/rcnn.cpp:349-366).  Host function. */
 TRTX_API int trtx_rcnn_letterbox_pads(int img_w, int img_h, int net_w, int net_h, int pads[4]);
+
+/* preprocessImg (rcnn/common.hpp:79-110) + the float widening of rcnn.cpp:504-505 for a whole batch, one launch per
+ * <= 64 images: images_host = `batch` u8 HWC BGR descriptors (trtx_image_desc, any pitch, mixed sizes allowed);
+ * dst_dev = [batch, net_h, net_w, 3] fp32 BGR, 0..255, 128 outside the resized rectangle: the engine input of
+ * rcnn.cpp:259, ready for enqueue.  Image b is resized (OpenCV 4.x's 8-bit INTER_LINEAR, bit for bit) into the rectangle
+ * between the pads of trtx_rcnn_letterbox_pads, of size (net_w - left - right) x (net_h - top - bottom).  Every descriptor is
+ * checked before the first launch: TRTX_ERR_INVALID for a null pointer, batch / net sizes <= 0, pitch < 3 * width or a
+ * dst_dev that is not 4-byte aligned; TRTX_ERR_UNSUPPORTED for an image whose rectangle is empty (cv::resize throws there)
+ * or wider than 4 842 pixels (the kernel's shared-memory rows).  No workspace. */
+TRTX_API int trtx_rcnn_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h,
+                                          float* dst_dev, trtx_stream_t stream);
 
 typedef struct trtx_rcnn_post_params {
     int32_t net_w, net_h;      /* INPUT_W, INPUT_H */

@@ -140,6 +140,7 @@ SYMBOLS = {
     "trtx_scale_mask_enqueue": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "trtx_rcnn_letterbox_pads": (_i, [_i, _i, _i, _i, C.POINTER(C.c_int)]),
     "trtx_rcnn_postprocess_enqueue": (_i, [C.POINTER(RcnnPostParams), _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "trtx_rcnn_preprocess_enqueue": (_i, [C.POINTER(ImageDesc), _i, _i, _i, _vp, _vp]),
     "trtx_yolo_decode_nms_gather_enqueue": (_i, [C.POINTER(YoloParams), C.POINTER(NmsParams), _i, _pp, _vp, _vp, _vp, _sz,
                                                  C.POINTER(Gather), _vp]),
     "trtx_gather_wait_enqueue": (_i, [C.POINTER(Gather), _vp]),

@@ -22,20 +22,13 @@ struct ResizeAxis {
     short* coef;  // 2 fixed-point weights per destination index, sum = 2048
 };
 
-// OpenCV resize(): fx = (float)((dx + 0.5) * scale - 0.5); sx = cvFloor(fx); fx -= sx; [x only: borders zero the fraction]
 static void resize_axis(ResizeAxis a, int dn, int sn, bool clamp) {
     const double scale = (double)sn / dn;
     for (int d = 0; d < dn; ++d) {
-        float f = (float)((d + 0.5) * scale - 0.5);
-        int s = (int)floorf(f);
-        f -= s;
-        if (clamp) {
-            if (s < 0) f = 0, s = 0;
-            if (s >= sn - 1) f = 0, s = sn - 1;
-        }
-        a.idx[d] = s;
-        a.coef[2 * d] = (short)lrintf((1.f - f) * 2048.f);  // saturate_cast<short>(float): cvRound, round-half-even
-        a.coef[2 * d + 1] = (short)lrintf(f * 2048.f);
+        const LinearTap t = cv_linear_tap(d, scale, sn, clamp);
+        a.idx[d] = t.s;
+        a.coef[2 * d] = t.c0;
+        a.coef[2 * d + 1] = t.c1;
     }
 }
 

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 
 #include "trtx_hot.h"
@@ -81,6 +82,41 @@ __device__ __forceinline__ float logist(float x) { return 1.0f / (1.0f + expf(-x
 __device__ __forceinline__ uint32_t float_key(float f) {
     uint32_t b = __float_as_uint(f);
     return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+
+// One destination index d of OpenCV 4.x's 8-bit INTER_LINEAR resize (imgproc/src/resize.cpp) along an axis of `sn` source
+// samples: fx = (float)((d + 0.5) * scale - 0.5), s = cvFloor(fx), fx -= s; with `clamp` (the x axis) a tap outside [0, sn - 1)
+// moves to the border with a zero fraction, without it (the y axis) s and fx are kept and the rows are clipped where they are
+// read; the weights are saturate_cast<short>((1 - fx) * 2048) and (fx * 2048), cvRound = round half to even.  The library's
+// only floating-point step of that resize, shared by the host calibrator (calib_host.cu) and the R-CNN pre-process kernel
+// (preprocess.cu).  The device spells the double expression with _rn intrinsics: left to itself nvcc may contract it into
+// a DFMA, which rounds once where the host rounds twice.
+struct LinearTap {
+    int s;           // low tap (x: clamped; y: not clamped)
+    short c0, c1;    // fixed-point weights, c0 + c1 = 2048
+};
+__host__ __device__ inline LinearTap cv_linear_tap(int d, double scale, int sn, bool clamp) {
+#ifdef __CUDA_ARCH__
+    float f = __double2float_rn(__dadd_rn(__dmul_rn(__dadd_rn((double)d, 0.5), scale), -0.5));
+#else
+    float f = (float)((d + 0.5) * scale - 0.5);
+#endif
+    int s = (int)floorf(f);
+    f -= (float)s;
+    if (clamp) {
+        if (s < 0) f = 0, s = 0;
+        if (s >= sn - 1) f = 0, s = sn - 1;
+    }
+    LinearTap t;
+    t.s = s;
+#ifdef __CUDA_ARCH__
+    t.c0 = (short)__float2int_rn(__fmul_rn(__fsub_rn(1.f, f), 2048.f));
+    t.c1 = (short)__float2int_rn(__fmul_rn(f, 2048.f));
+#else
+    t.c0 = (short)lrintf((1.f - f) * 2048.f);
+    t.c1 = (short)lrintf(f * 2048.f);
+#endif
+    return t;
 }
 
 __device__ __forceinline__ int warp_excl_scan(int v, int lane, int* total) {

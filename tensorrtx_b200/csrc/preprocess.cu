@@ -400,6 +400,135 @@ static int launch_unit(const trtx_image_desc* const* d, UnitImage* u, int n, voi
     return launch_unit_t(a, n, smem, static_cast<__half*>(dst), st);
 }
 
+// =====================================================================================================================
+// Mask R-CNN pre-process: preprocessImg (rcnn/common.hpp:79-110) + the float widening of rcnn.cpp:504-505, i.e.
+// cv::resize(INTER_LINEAR) of the 8-bit BGR image into the rectangle between the pads, pasted on a 128-grey canvas, every byte
+// widened to float: [net_h, net_w, 3] fp32 BGR, 0..255 per image.  The resize is OpenCV 4.x's fixed-point one, as
+// calib_host.cu restates it: taps and weights from cv_linear_tap, horizontal pass h = S[sx] * c0 + S[sx1] * c1 in int, vertical
+// pass ((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2 saturated to 0..255 (VResizeLinearVec_32s8u).
+//
+// Bound by HBM writes: 4 output bytes per canvas byte (b8 at 1067 x 800: 81.9 MB written, 7.4 MB of u8 read).  A CTA owns a band
+// of kRcnnPreBand full-width destination rows of one image (flat grid over images x bands), which in HWC is ONE contiguous run of
+// band * net_w * 3 floats:
+//   1. y taps: one per destination row of the band inside the rectangle; the distinct clipped source rows they read (at most
+//      2 * band) become the band's slots;
+//   2. horizontal pass: each thread computes the x taps of its columns once and runs them over every slot row; the results,
+//      already >> 4 (all the vertical pass reads of them, <= 32640), are staged as int16 rows in shared memory and shared by
+//      the destination rows that use the same source row;
+//   3. stores: the run is written with 16-byte stores (a head of 0..3 floats up to the first 16-byte boundary and a tail
+//      of 0..3 floats are scalar: rows are 12 * net_w bytes and dst may be only 4-byte aligned); an element outside the
+//      rectangle is 128.0f.  A band wholly in the top / bottom padding skips 1 and 2 and reads nothing.
+constexpr int kRcnnPreBand = 4;            // destination rows per CTA
+constexpr int kRcnnPreSlots = 2 * kRcnnPreBand;  // staged source rows: two taps per destination row at most
+constexpr int kRcnnPreThreads = 256;
+constexpr int kMaxRcnnPreImages = 64;      // descriptors per launch (kernel parameter block)
+
+struct RcnnPreImage {
+    const uint8_t* src;
+    double scale_x, scale_y;  // cv::resize: 1. / ((double)dsize / ssize)
+    int sw, sh, pitch;
+    int x0, y0, rw, rh;       // the resized rectangle on the canvas: (pad_left, pad_top, net - pads)
+    int dst_idx;
+};
+struct RcnnPreArgs {
+    RcnnPreImage img[kMaxRcnnPreImages];
+    int net_w, net_h, bands;
+    int stride;               // int16 per staged row: 3 * the widest rectangle of the launch
+};
+
+__global__ void __launch_bounds__(kRcnnPreThreads) rcnn_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
+                                                                          float* __restrict__ dst) {
+    constexpr int R = kRcnnPreBand;
+    extern __shared__ __align__(16) int16_t hrows[];  // [slots][a.stride]
+    __shared__ int s_row[kRcnnPreSlots];              // source row of each slot
+    __shared__ int s_slot[R][2];                      // slots of the two taps of destination row k
+    __shared__ int s_coef[R][2];                      // their weights b0, b1
+    __shared__ int s_nslots;
+    const int item = blockIdx.x / a.bands, band = blockIdx.x - item * a.bands;
+    const RcnnPreImage& im = a.img[item];
+    const int y0 = band * R, rows = min(R, a.net_h - y0);
+    const int k_lo = max(im.y0 - y0, 0), k_hi = min(im.y0 + im.rh - y0, rows);  // band rows inside the rectangle
+    const int stride = a.stride;
+    if (k_lo < k_hi) {  // uniform over the CTA
+        if (threadIdx.x == 0) {
+            int n = 0;
+            for (int k = k_lo; k < k_hi; ++k) {
+                const LinearTap t = cv_linear_tap(y0 + k - im.y0, im.scale_y, im.sh, false);
+#pragma unroll
+                for (int j = 0; j < 2; ++j) {
+                    const int sy = min(max(t.s + j, 0), im.sh - 1);  // y taps are clipped where they are read
+                    int slot = -1;
+                    for (int i = 0; i < n; ++i) slot = s_row[i] == sy ? i : slot;
+                    if (slot < 0) {
+                        s_row[n] = sy;
+                        slot = n++;
+                    }
+                    s_slot[k][j] = slot;
+                }
+                s_coef[k][0] = t.c0;
+                s_coef[k][1] = t.c1;
+            }
+            s_nslots = n;
+        }
+        __syncthreads();
+        const int n = s_nslots;
+        for (int x = threadIdx.x; x < im.rw; x += blockDim.x) {
+            const LinearTap t = cv_linear_tap(x, im.scale_x, im.sw, true);
+            const int o0 = 3 * t.s, o1 = 3 * min(t.s + 1, im.sw - 1);
+            for (int j0 = 0; j0 < n; j0 += 4) {
+                uint32_t px[4][6];  // the loads of 4 slot rows are in flight before the first use
+#pragma unroll
+                for (int j = 0; j < 4; ++j)
+                    if (j0 + j < n) {
+                        const uint8_t* S = im.src + (size_t)s_row[j0 + j] * (size_t)im.pitch;
+#pragma unroll
+                        for (int c = 0; c < 3; ++c) px[j][c] = __ldg(S + o0 + c), px[j][3 + c] = __ldg(S + o1 + c);
+                    }
+#pragma unroll
+                for (int j = 0; j < 4; ++j)
+                    if (j0 + j < n) {
+                        int16_t* h = hrows + (j0 + j) * stride + 3 * x;
+#pragma unroll
+                        for (int c = 0; c < 3; ++c) h[c] = (int16_t)(((int)px[j][c] * t.c0 + (int)px[j][3 + c] * t.c1) >> 4);
+                    }
+            }
+        }
+        __syncthreads();
+    }
+    const int L = 3 * a.net_w;  // floats per canvas row
+    const int total = rows * L;
+    float* base = dst + ((size_t)im.dst_idx * a.net_h + y0) * (size_t)L;
+    const int e_lo = 3 * im.x0, e_n = 3 * im.rw;  // row elements [e_lo, e_lo + e_n) lie in the rectangle
+    auto value = [&](int k, int e) -> float {
+        const int i = e - e_lo;
+        if (k < k_lo || k >= k_hi || (unsigned)i >= (unsigned)e_n) return 128.0f;  // the canvas, Scalar(128, 128, 128)
+        const int h0 = hrows[s_slot[k][0] * stride + i], h1 = hrows[s_slot[k][1] * stride + i];
+        const int v = (((s_coef[k][0] * h0) >> 16) + ((s_coef[k][1] * h1) >> 16) + 2) >> 2;
+        return u8_to_float_alu((uint32_t)min(max(v, 0), 255));
+    };
+    const int head = min((int)(((16u - (unsigned)(reinterpret_cast<uintptr_t>(base) & 15u)) & 15u) >> 2), total);
+    const int nvec = (total - head) >> 2, tail0 = head + 4 * nvec;
+    if ((int)threadIdx.x < head) base[threadIdx.x] = value(threadIdx.x / L, threadIdx.x % L);
+    if (tail0 + (int)threadIdx.x < total) {
+        const int f = tail0 + threadIdx.x;
+        base[f] = value(f / L, f % L);
+    }
+    int q = threadIdx.x;
+    int k = (head + 4 * q) / L, e = (head + 4 * q) % L;  // row and element of the thread's first float4
+    const int step = 4 * blockDim.x;
+    for (; q < nvec; q += blockDim.x) {
+        float v[4];
+        int kk = k, ee = e;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            v[j] = value(kk, ee);
+            if (++ee == L) ee = 0, ++kk;
+        }
+        *reinterpret_cast<float4*>(base + head + 4 * q) = make_float4(v[0], v[1], v[2], v[3]);
+        for (e += step; e >= L; e -= L) ++k;
+    }
+}
+
 }  // namespace trtx
 
 using namespace trtx;
@@ -661,6 +790,63 @@ TRTX_API int trtx_preprocess_batch_enqueue(const trtx_image_desc* images_host, i
     int rc = flush_unit();
     if (rc) return rc;
     return flush_general();
+}
+
+TRTX_API int trtx_rcnn_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
+                                          trtx_stream_t stream) {
+    if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
+    if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
+    // every descriptor is checked before the first launch, so that a rejected call writes nothing
+    size_t smem_max = 0;
+    for (int i = 0; i < batch; ++i) {
+        const trtx_image_desc& d = images_host[i];
+        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
+        int pads[4];
+        trtx_rcnn_letterbox_pads(d.width, d.height, net_w, net_h, pads);
+        const int rw = net_w - (pads[0] + pads[1]), rh = net_h - (pads[2] + pads[3]);
+        if (rw <= 0 || rh <= 0 || pads[0] < 0 || pads[2] < 0) return TRTX_ERR_UNSUPPORTED;  // cv::resize / copyTo would throw
+        const size_t smem = (size_t)kRcnnPreSlots * 3 * (size_t)rw * sizeof(int16_t);
+        if (smem > 227 * 1024) return TRTX_ERR_UNSUPPORTED;
+        smem_max = smem > smem_max ? smem : smem_max;
+    }
+    if (smem_max > 48 * 1024 &&
+        cudaFuncSetAttribute(rcnn_preprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) != cudaSuccess) {
+        g_last_cuda_error = (int)cudaGetLastError();
+        return TRTX_ERR_CUDA;
+    }
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    RcnnPreArgs a;
+    a.net_w = net_w;
+    a.net_h = net_h;
+    a.bands = (net_h + kRcnnPreBand - 1) / kRcnnPreBand;
+    for (int i0 = 0; i0 < batch; i0 += kMaxRcnnPreImages) {
+        const int n = batch - i0 < kMaxRcnnPreImages ? batch - i0 : kMaxRcnnPreImages;
+        int wmax = 0;
+        for (int j = 0; j < n; ++j) {
+            const trtx_image_desc& d = images_host[i0 + j];
+            RcnnPreImage& im = a.img[j];
+            int pads[4];
+            trtx_rcnn_letterbox_pads(d.width, d.height, net_w, net_h, pads);
+            im.src = d.data_dev;
+            im.sw = d.width;
+            im.sh = d.height;
+            im.pitch = d.pitch;
+            im.x0 = pads[0];
+            im.y0 = pads[2];
+            im.rw = net_w - (pads[0] + pads[1]);
+            im.rh = net_h - (pads[2] + pads[3]);
+            im.scale_x = 1. / ((double)im.rw / d.width);
+            im.scale_y = 1. / ((double)im.rh / d.height);
+            im.dst_idx = i0 + j;
+            wmax = im.rw > wmax ? im.rw : wmax;
+        }
+        a.stride = 3 * wmax;
+        const size_t smem = (size_t)kRcnnPreSlots * a.stride * sizeof(int16_t);
+        rcnn_preprocess_kernel<<<(unsigned)(n * a.bands), kRcnnPreThreads, smem, st>>>(a, dst_dev);
+        const int rc = check_launch();
+        if (rc) return rc;
+    }
+    return TRTX_OK;
 }
 
 }  // extern "C"

@@ -996,6 +996,29 @@ def rcnn_letterbox_pads(img_w: int, img_h: int, net_w: int, net_h: int):
     return tuple(p)
 
 
+def rcnn_preprocess(images: Sequence[torch.Tensor], net_w: int, net_h: int, out: torch.Tensor | None = None,
+                    stream=None) -> torch.Tensor:
+    """GPU drop-in for the pre-process of rcnn/rcnn.cpp:497-506 (preprocessImg, rcnn/common.hpp:79-110, then the widening
+    of every byte to float) for a batch of device frames: images[i] is a u8 HWC BGR cuda tensor [h, w, 3] with packed
+    pixels (rows may be pitched, sizes may differ) -> [B, net_h, net_w, 3] float32 BGR, 0..255, 128 around the resized
+    image: the engine input.  One launch per 64 images, no synchronisation."""
+    lib = L.load()
+    n = len(images)
+    descs = (L.ImageDesc * n)()
+    for i, im in enumerate(images):
+        if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3 or im.stride(2) != 1 or im.stride(1) != 3:
+            raise L.TrtxError("images must be u8 HWC BGR with packed pixels")
+        descs[i].data_dev = im.data_ptr()
+        descs[i].height, descs[i].width = int(im.shape[0]), int(im.shape[1])
+        descs[i].pitch = int(im.stride(0))
+    if out is None:
+        out = torch.empty((n, net_h, net_w, 3), dtype=torch.float32, device=images[0].device if n else "cuda")
+    if out.dtype != torch.float32 or tuple(out.shape) != (n, net_h, net_w, 3):
+        raise ValueError(f"out must be float32 [{n}, {net_h}, {net_w}, 3]")
+    L.check(lib.trtx_rcnn_preprocess_enqueue(descs, n, net_w, net_h, _ptr(out), _stream(stream)), "trtx_rcnn_preprocess_enqueue")
+    return out
+
+
 def rcnn_postprocess(scores: torch.Tensor, boxes: torch.Tensor, classes: torch.Tensor, masks: torch.Tensor | None = None, *,
                      img_w: int, img_h: int, net_w: int, net_h: int, score_thresh: float = 0.6, max_masks: int | None = None,
                      out=None, stream=None):
