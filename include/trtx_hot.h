@@ -101,8 +101,8 @@ typedef struct trtx_yolo_params {
      * (TensorRT calls enqueue() on clones from several threads, SURVEY 8b "Threading") with different tunings are
      * independent.  0 everywhere -- what memset / trtx_yolo_params_init_v8 leave -- selects the defaults chosen on an H100 for
      * the overlapped benchmark step (DESIGN.md section 4.1).  A combination that is not built returns TRTX_ERR_UNSUPPORTED. */
-    int32_t tune_class_slices;   /* warps of a CTA splitting the class range: 1, 2, 4, 8; 0 = 2 */
-    int32_t tune_rows_in_flight; /* channel rows loaded per group; 0 = 5 (fp16 inputs, 8 anchors per lane: 10).  Built (slices, rows): (1,8) (1,16) (2,4) (2,5)
+    int32_t tune_class_slices;   /* warps of a CTA splitting the class range: 1, 2, 4, 8; 0 = 4 (fp32 inputs, 4 anchors per lane), else 2 */
+    int32_t tune_rows_in_flight; /* channel rows loaded per group; 0 = 10 (fp32 inputs with 4 anchors per lane, fp16 inputs with 8), else 5.  Built (slices, rows): (1,8) (1,16) (2,4) (2,5)
                                     (2,8) (2,10) (2,20) (4,4) (4,5) (4,10) (4,20) (8,5) (8,10) */
     int32_t tune_tma_pipeline;   /* 1: persistent TMA-fed scan (v8 layout, 16-byte aligned levels); 0 = register scan */
     int32_t tune_tma_stages;     /* cap on its pipeline stages; 0 = as many as fit (15) */

@@ -751,8 +751,9 @@ int yolo_fill_args(const trtx_yolo_params* p, int batch, const void* const* inpu
     YoloLayout L = yolo_layout(p, batch, pipe ? 1 : vec);
     L.pipe = pipe ? 1 : 0;
     // defaults chosen on an H100 for the overlapped step, not for the scan alone (DESIGN.md section 4.1, "Defaults")
-    L.slices = p->tune_class_slices ? p->tune_class_slices : 2;
-    L.unroll = p->tune_rows_in_flight ? p->tune_rows_in_flight : (vec == 8 ? 10 : 5);
+    const bool f32x4 = p->in_dtype == TRTX_F32 && vec == 4;  // the benchmark's fp32 heads: 4 x 10
+    L.slices = p->tune_class_slices ? p->tune_class_slices : (f32x4 ? 4 : 2);
+    L.unroll = p->tune_rows_in_flight ? p->tune_rows_in_flight : (f32x4 || vec == 8 ? 10 : 5);
     L.pipe_stages = p->tune_tma_stages;
     if (workspace_bytes < L.total_bytes) return TRTX_ERR_WORKSPACE;
     if (reinterpret_cast<uintptr_t>(workspace_dev) % 16 != 0) return TRTX_ERR_INVALID;
