@@ -49,7 +49,7 @@ TRTX_API const char* trtx_version(void);
 TRTX_API int trtx_last_cuda_error(void);
 /* sizeof() of the parameter structs as THIS library was compiled, so that an FFI binding (ctypes, cgo, ...) can check its
  * mirror of the layout: which = 0 trtx_yolo_params, 1 trtx_nms_params, 2 trtx_retina_params, 3 trtx_image_desc,
- * 4 trtx_mask_params, 5 trtx_rcnn_post_params; anything else 0. */
+ * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_seg_image; anything else 0. */
 TRTX_API size_t trtx_abi_sizeof(int which);
 
 /* =====================================================================================
@@ -406,6 +406,35 @@ typedef struct trtx_mask_params {
  * masks_dev: [batch, max_masks, net_h, net_w] fp32; slots >= count are left untouched.  One launch. */
 TRTX_API int trtx_process_mask_enqueue(const trtx_mask_params* p, int batch, const float* proto_dev, const float* dets_dev,
                                        int max_rows, float* masks_dev, trtx_stream_t stream);
+
+/* The segmentation models' last host stage on the device: process_mask + scale_mask + draw_mask_bbox's mask selection
+ * (yolov8/src/postprocess.cpp:228-248, yolov5/src/postprocess.cpp:148-167), for a batch of original frames of any sizes. */
+typedef struct trtx_seg_image {
+    int32_t img_w, img_h; /* the original frame: the cv::Mat img of draw_mask_bbox */
+    uint8_t* masks_dev;   /* [max_masks, img_h, pitch] u8 canvases of this image, or NULL (rows only) */
+    int32_t pitch;        /* bytes per canvas row, >= img_w (any value, any base alignment) */
+    int32_t reserved;
+} trtx_seg_image;
+
+/* p: as for trtx_process_mask_enqueue (row_floats >= 6; with every masks_dev NULL only variant, net_w, net_h and row_floats
+ *   are read).  dets_dev [B, 1 + max_rows*row_floats]: count, rows with the box at floats 0..3 in the variant's format, conf
+ *   at 4, class at 5 (the compact NMS output with extra_floats = 32: row_floats 39, coeff_offset 7; plugin rows: 90 / 6).
+ * images_host: `batch` descriptors in HOST memory (copied into launch parameters; sizes may differ within a call).
+ * rows_dev [B, 1 + max_rows*6]: n = min(count, max_rows), then per row i < n (x, y, w, h, conf, class) with x, y, w, h =
+ *   get_rect(img, bbox) (trtx_get_rect: V8 clamped to the image, V5 not), rows past n zeroed.  A box whose get_rect is
+ *   undefined in the reference (non-finite, or corners outside the int range) gets {0, 0, 0, 0}.
+ * Canvas k < min(count, max_masks, max_rows) of image b: 255 where (x, y) lies in get_rect(img, bbox_k) clipped to the
+ *   image and !(S(y, x) <= 0.5) -- draw_mask_bbox's `if (val <= 0.5) continue;`, so a NaN S is kept -- else 0, with
+ *   S = scale_mask(M) (crop trtx_scale_mask_rect, bilinear to img_w x img_h) and M = process_mask's net_w x net_h mask.
+ *   Bit-identical to thresholding trtx_process_mask_enqueue -> trtx_scale_mask_enqueue.  Canvases at or past that count are
+ *   left untouched.
+ * proto_dev [B, num_coeffs, mask_h, mask_w] may be NULL only when every masks_dev is NULL; NULL and non-NULL masks_dev in one
+ * call is TRTX_ERR_INVALID.  Everything is checked before the first launch (a rejected call writes nothing):
+ * TRTX_ERR_INVALID for null pointers, batch / max_rows / sizes <= 0, pitch < img_w; TRTX_ERR_UNSUPPORTED for an image whose
+ * scale_mask crop is empty (e.g. 1 x 5000: the reference's cv::resize throws).  Two launches per 64 images, no workspace. */
+TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const trtx_seg_image* images_host, int batch,
+                                               const float* proto_dev, const float* dets_dev, int max_rows,
+                                               float* rows_dev, trtx_stream_t stream);
 
 /* =====================================================================================
  * 7. Mask R-CNN pre- and post-process

@@ -98,6 +98,11 @@ class RcnnPostParams(C.Structure):
                [("score_thresh", C.c_float)]
 
 
+class SegImage(C.Structure):
+    _fields_ = [("img_w", C.c_int32), ("img_h", C.c_int32), ("masks_dev", C.c_void_p), ("pitch", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
 # TRTX_LIB: another build of the same ABI (the probe build of tools/nms_probe.py); default = the in-tree release library
 LIB_PATH = Path(os.environ.get("TRTX_LIB") or Path(__file__).resolve().parent / "lib" / "libtrtx_hot.so")
 
@@ -141,6 +146,7 @@ SYMBOLS = {
     "trtx_rcnn_letterbox_pads": (_i, [_i, _i, _i, _i, C.POINTER(C.c_int)]),
     "trtx_rcnn_postprocess_enqueue": (_i, [C.POINTER(RcnnPostParams), _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "trtx_rcnn_preprocess_enqueue": (_i, [C.POINTER(ImageDesc), _i, _i, _i, _vp, _vp]),
+    "trtx_yolo_seg_postprocess_enqueue": (_i, [C.POINTER(MaskParams), C.POINTER(SegImage), _i, _vp, _vp, _i, _vp, _vp]),
     "trtx_yolo_decode_nms_gather_enqueue": (_i, [C.POINTER(YoloParams), C.POINTER(NmsParams), _i, _pp, _vp, _vp, _vp, _sz,
                                                  C.POINTER(Gather), _vp]),
     "trtx_gather_wait_enqueue": (_i, [C.POINTER(Gather), _vp]),
@@ -171,7 +177,8 @@ def load() -> C.CDLL:
         fn = getattr(lib, name)  # AttributeError if the library does not export a declared symbol
         fn.restype = res
         fn.argtypes = args
-    for which, st in enumerate((YoloParams, NmsParams, RetinaParams, ImageDesc, MaskParams, RcnnPostParams)):
+    for which, st in enumerate((YoloParams, NmsParams, RetinaParams, ImageDesc, MaskParams, RcnnPostParams,
+                                   SegImage)):
         if lib.trtx_abi_sizeof(which) != C.sizeof(st):
             raise TrtxError(f"{LIB_PATH} was built from a different trtx_hot.h: sizeof({st.__name__}) = "
                             f"{lib.trtx_abi_sizeof(which)} in the library, {C.sizeof(st)} in the binding (rebuild)")

@@ -119,6 +119,106 @@ __host__ __device__ inline LinearTap cv_linear_tap(int d, double scale, int sn, 
     return t;
 }
 
+// Rounded float arithmetic spelled once for host and device: plain operators on the host (built without contraction),
+// _rn intrinsics on the device so that nvcc cannot fuse a product into an FMA.
+__host__ __device__ inline float f_mul(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+__host__ __device__ inline float f_sub(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fsub_rn(a, b);
+#else
+    return a - b;
+#endif
+}
+__host__ __device__ inline float f_add(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+__host__ __device__ inline float f_div(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fdiv_rn(a, b);
+#else
+    return a / b;
+#endif
+}
+
+// round() of a float to int, false where the reference's int conversion is undefined (NaN, inf, outside the int range)
+__host__ __device__ inline bool round_to_int(float v, int& out) {
+    const double r = round((double)v);
+    if (!(r >= -2147483648.0 && r <= 2147483647.0)) return false;
+    out = (int)r;
+    return true;
+}
+
+// get_rect: the inverse of the letterbox for a detection box -- yolov8/src/postprocess.cpp:6-36 (TRTX_YOLO_V8: l,t,r,b,
+// clamped to the image) and yolov5/src/postprocess.cpp:4-29 (TRTX_YOLO_V5: cx,cy,w,h, not clamped).  Statement by statement:
+// the two ratios are double divisions stored to float, the rest is float, round() sees doubles.  Shared by the host
+// trtx_get_rect and the segmentation post-process kernels (mask.cu).  Returns false, with rect {0, 0, 0, 0}, where the
+// reference's float -> int conversions are undefined (a non-finite box, or rescaled corners outside the int range).
+__host__ __device__ inline bool yolo_get_rect(int variant, int net_w, int net_h, int img_w, int img_h, const float bbox[4],
+                                              int rect[4]) {
+    rect[0] = rect[1] = rect[2] = rect[3] = 0;
+#ifdef __CUDA_ARCH__
+    const float r_w = __double2float_rn(__ddiv_rn((double)net_w, (double)img_w));
+    const float r_h = __double2float_rn(__ddiv_rn((double)net_h, (double)img_h));
+#else
+    const float r_w = (float)(net_w / (img_w * 1.0));
+    const float r_h = (float)(net_h / (img_h * 1.0));
+#endif
+    const bool by_w = r_h > r_w;  // the width fills the network input: vertical padding
+    const float ratio = by_w ? r_w : r_h;
+    const float pad = by_w ? f_div(f_sub((float)net_h, f_mul(r_w, (float)img_h)), 2.0f)
+                           : f_div(f_sub((float)net_w, f_mul(r_h, (float)img_w)), 2.0f);
+    float l, r, t, b;
+    if (variant == TRTX_YOLO_V8) {
+        l = bbox[0];
+        r = bbox[2];
+        t = bbox[1];
+        b = bbox[3];
+    } else {
+        l = f_sub(bbox[0], f_div(bbox[2], 2.f));
+        r = f_add(bbox[0], f_div(bbox[2], 2.f));
+        t = f_sub(bbox[1], f_div(bbox[3], 2.f));
+        b = f_add(bbox[1], f_div(bbox[3], 2.f));
+    }
+    if (by_w) {
+        t = f_sub(t, pad);
+        b = f_sub(b, pad);
+    } else {
+        l = f_sub(l, pad);
+        r = f_sub(r, pad);
+    }
+    l = f_div(l, ratio);
+    r = f_div(r, ratio);
+    t = f_div(t, ratio);
+    b = f_div(b, ratio);
+    if (variant == TRTX_YOLO_V8) {
+        l = 0.0f > l ? 0.0f : l;
+        t = 0.0f > t ? 0.0f : t;
+    }
+    int rl, rt, rw, rh;
+    if (!round_to_int(l, rl) || !round_to_int(t, rt) || !round_to_int(f_sub(r, l), rw) || !round_to_int(f_sub(b, t), rh))
+        return false;
+    if (variant == TRTX_YOLO_V8) {  // l, t >= 0 here, so img - round(l) cannot overflow
+        const int width = rw < img_w - rl ? rw : img_w - rl, height = rh < img_h - rt ? rh : img_h - rt;
+        rw = width > 0 ? width : 0;
+        rh = height > 0 ? height : 0;
+    }
+    rect[0] = rl;
+    rect[1] = rt;
+    rect[2] = rw;
+    rect[3] = rh;
+    return true;
+}
+
 __device__ __forceinline__ int warp_excl_scan(int v, int lane, int* total) {
     int x = v;
 #pragma unroll

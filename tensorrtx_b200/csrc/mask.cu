@@ -346,6 +346,250 @@ __global__ void __launch_bounds__(kPasteThreads) rcnn_paste_kernel(const __grid_
     }
 }
 
+// YOLO segmentation post-process: process_mask (above) + draw_mask_bbox's mask selection (yolov8/src/postprocess.cpp:228-248,
+// yolov5/src/postprocess.cpp:148-167), which the reference runs on one host core per image.  For detection k of image b:
+//   M = process_mask's 640^2 mask, S = scale_mask(M) (crop trtx_scale_mask_rect, bilinear to img_w x img_h),
+//   canvas[k](y, x) = 255 where (x, y) lies in get_rect(img, bbox_k) (clipped to the image) and !(S(y, x) <= 0.5), else 0.
+// Two launches per <= 64 images, stream-ordered, no workspace:
+//   seg_rows_kernel   one warp per image: count, then (get_rect x, y, w, h, conf, class) per row, zeroes the tail;
+//   seg_canvas_kernel one CTA per (image, slot, band of kSegBand full-width canvas rows).  A band that misses get_rect's rows
+//                     stores zeros and reads nothing.  Otherwise the band's y-taps of scale_mask name the rows of M it
+//                     needs (at most 2 per canvas row) and get_rect's x-range the columns; their process_mask taps name
+//                     the low-resolution cells.  The CTA evaluates those sigmoid(dot) values once into shared memory, then
+//                     the needed M values with process_mask_kernel's expression, then S with scale_mask_kernel's, and
+//                     stores the thresholded bytes with 16-byte stores.  Neither M nor S reaches HBM; every value is the
+//                     same expression of the same inputs as in process_mask_kernel -> scale_mask_kernel, so the canvases
+//                     are bit-identical to thresholding that composition.
+constexpr int kSegMaxImages = 64;          // images per launch (launch-parameter array)
+constexpr int kSegBand = 8;                // canvas rows per CTA
+constexpr int kSegThreads = 256;
+constexpr int kSegMaxY = 2 * kSegBand;     // rows of M a band can need: two taps per canvas row
+constexpr int kSegMaxLY = 2 * kSegMaxY;    // low-resolution rows those can need
+constexpr int kSegRowFloats = 6;           // x, y, w, h, conf, class
+
+struct SegImage {
+    uint8_t* canvas;     // [max_masks, img_h, pitch] u8, or nullptr (rows only)
+    int img_w, img_h, pitch;
+    int cx, cy, cw, ch;  // scale_mask's crop of the net_w x net_h mask
+    int bands;           // canvas row bands of kSegBand rows
+    int first_cta;       // first CTA of this image in the launch
+};
+struct SegArgs {
+    SegImage img[kSegMaxImages];
+    const float* proto;  // [B, nm, mh, mw]
+    const float* dets;   // [B, 1 + max_rows * row_floats]
+    float* rows;         // [B, 1 + max_rows * 6]
+    int base, n_images;  // images [base, base + n_images) of the call
+    int max_rows, row_floats, coeff_offset, variant, nm, mw, mh, net_w, net_h, max_masks;
+    int y_cap, x_cap, ly_cap, lx_cap;  // shared-memory regions of this launch: M [y_cap][x_cap], cells [ly_cap][lx_cap]
+};
+
+__global__ void __launch_bounds__(128) seg_rows_kernel(const __grid_constant__ SegArgs a) {
+    const int j = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (j >= a.n_images) return;
+    const SegImage& im = a.img[j];
+    const int b = a.base + j;
+    const float* src = a.dets + (size_t)b * (1 + (size_t)a.max_rows * a.row_floats);
+    float* out = a.rows + (size_t)b * (1 + (size_t)a.max_rows * kSegRowFloats);
+    const int n = min(max((int)src[0], 0), a.max_rows);
+    for (int i = lane; i < a.max_rows; i += 32) {
+        float* r = out + 1 + (size_t)i * kSegRowFloats;
+        if (i < n) {
+            const float* d = src + 1 + (size_t)i * a.row_floats;
+            int rect[4];
+            yolo_get_rect(a.variant, a.net_w, a.net_h, im.img_w, im.img_h, d, rect);  // {0, 0, 0, 0} where undefined
+            r[0] = (float)rect[0];
+            r[1] = (float)rect[1];
+            r[2] = (float)rect[2];
+            r[3] = (float)rect[3];
+            r[4] = d[4];
+            r[5] = d[5];
+        } else {
+#pragma unroll
+            for (int e = 0; e < kSegRowFloats; ++e) r[e] = 0.0f;
+        }
+    }
+    if (lane == 0) out[0] = (float)n;
+}
+
+// distinct-value list of at most a few dozen entries (thread 0 only)
+__device__ __forceinline__ int seg_slot(int* list, int& n, int v) {
+    for (int i = 0; i < n; ++i)
+        if (list[i] == v) return i;
+    list[n] = v;
+    return n++;
+}
+
+__global__ void __launch_bounds__(kSegThreads) seg_canvas_kernel(const __grid_constant__ SegArgs a) {
+    extern __shared__ __align__(16) float s_dyn[];  // M values [y_cap * x_cap], then sigmoid cells [ly_cap * lx_cap]
+    __shared__ float s_coeff[kMaxCoeffs];
+    __shared__ int s_yrow[kSegMaxY];      // row of M of each y slot
+    __shared__ int s_ytap[kSegBand][2];   // y slots of the two scale_mask taps of band row k
+    __shared__ float s_fy[kSegBand];
+    __shared__ int s_lyrow[kSegMaxLY];    // low-resolution row of each cell slot
+    __shared__ int s_mtap[kSegMaxY][2];   // cell slots of the two process_mask taps of y slot i
+    __shared__ float s_mfy[kSegMaxY];
+    __shared__ int s_ny, s_nly;
+    int lo = 0, hi = a.n_images - 1;  // the image owning this CTA
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (a.img[mid].first_cta <= (int)blockIdx.x) lo = mid;
+        else hi = mid - 1;
+    }
+    const SegImage& im = a.img[lo];
+    const int local = (int)blockIdx.x - im.first_cta, k = local / im.bands, band = local - k * im.bands;
+    const int b = a.base + lo, tid = threadIdx.x;
+    const float* dets = a.dets + (size_t)b * (1 + (size_t)a.max_rows * a.row_floats);
+    const int count = min(max((int)dets[0], 0), min(a.max_rows, a.max_masks));
+    if (k >= count) return;  // slots past the image's detections are left untouched
+    const float* det = dets + 1 + (size_t)k * a.row_floats;
+    int rect[4];
+    const bool defined = yolo_get_rect(a.variant, a.net_w, a.net_h, im.img_w, im.img_h, det, rect);
+    // get_rect clipped to the image (a V5 rect may leave it; the reference's loop would read outside img_mask there)
+    const int x_lo = max(rect[0], 0), x_hi = (int)min((long long)rect[0] + rect[2], (long long)im.img_w);
+    const int y_lo = max(rect[1], 0), y_hi = (int)min((long long)rect[1] + rect[3], (long long)im.img_h);
+    const int y0 = band * kSegBand, y1 = min(y0 + kSegBand, im.img_h);
+    const int ya = max(y_lo, y0), yb = min(y_hi, y1);
+    const bool touches = defined && x_lo < x_hi && ya < yb;  // uniform over the CTA
+    const double sx_scale = (double)im.cw / (double)im.img_w, sy_scale = (double)im.ch / (double)im.img_h;  // scale_mask
+    const double mx_scale = (double)a.mw / (double)a.net_w, my_scale = (double)a.mh / (double)a.net_h;      // process_mask
+    float* s_M = s_dyn;
+    int Xa = 0, nX = 1;
+    if (touches) {
+        if (tid == 0) {
+            int ny = 0, nly = 0;
+            for (int y = ya; y < yb; ++y) {
+                int sy;
+                float fy;
+                resize_tap(y, sy_scale, im.ch, sy, fy);
+                s_ytap[y - y0][0] = seg_slot(s_yrow, ny, im.cy + sy);
+                s_ytap[y - y0][1] = seg_slot(s_yrow, ny, im.cy + min(sy + 1, im.ch - 1));
+                s_fy[y - y0] = fy;
+            }
+            for (int i = 0; i < ny; ++i) {
+                int ly;
+                float fy;
+                resize_tap(s_yrow[i], my_scale, a.mh, ly, fy);
+                s_mtap[i][0] = seg_slot(s_lyrow, nly, ly);
+                s_mtap[i][1] = seg_slot(s_lyrow, nly, min(ly + 1, a.mh - 1));
+                s_mfy[i] = fy;
+            }
+            s_ny = ny;
+            s_nly = nly;
+        }
+        if (tid < a.nm) s_coeff[tid] = det[a.coeff_offset + tid];
+        // columns of M under get_rect's x-range and the low-resolution columns they need (the taps are monotonic)
+        int s0, s1;
+        float f;
+        resize_tap(x_lo, sx_scale, im.cw, s0, f);
+        resize_tap(x_hi - 1, sx_scale, im.cw, s1, f);
+        Xa = im.cx + s0;
+        nX = im.cx + min(s1 + 1, im.cw - 1) - Xa + 1;
+        int lxa, lxb;
+        resize_tap(Xa, mx_scale, a.mw, lxa, f);
+        resize_tap(Xa + nX - 1, mx_scale, a.mw, lxb, f);
+        const int nLX = min(lxb + 1, a.mw - 1) - lxa + 1;
+        float* s_cell = s_dyn + a.y_cap * a.x_cap;
+        __syncthreads();
+        const int ny = s_ny, nly = s_nly;
+        // low-resolution cells: sigmoid(coeffs . proto) inside get_downscale_rect, 0 outside (process_mask_kernel)
+        int rx, ry, rw, rh;
+        downscale_rect(a.variant, det, a.net_w, a.net_h, rx, ry, rw, rh);
+        const int dx_lo = max(rx, 0), dx_hi = min(rx + rw, a.mw), dy_lo = max(ry, 0), dy_hi = min(ry + rh, a.mh);
+        const size_t plane = (size_t)a.mh * a.mw;
+        const float* proto = a.proto + (size_t)b * a.nm * plane;
+        for (int c = tid; c < nly * nLX; c += blockDim.x) {
+            const int i = c / nLX, x = lxa + (c - i * nLX), y = s_lyrow[i];
+            float v = 0.0f;
+            if (x >= dx_lo && x < dx_hi && y >= dy_lo && y < dy_hi) {
+                const float* p = proto + (size_t)y * a.mw + x;
+                float e = 0.0f;
+                for (int j = 0; j < a.nm; ++j) e = __fadd_rn(e, __fmul_rn(s_coeff[j], __ldg(p + (size_t)j * plane)));
+                v = 1.0f / (1.0f + expf(-e));
+            }
+            s_cell[c] = v;
+        }
+        __syncthreads();
+        // the needed values of M: process_mask_kernel's horizontal then vertical pass
+        for (int c = tid; c < ny * nX; c += blockDim.x) {
+            const int i = c / nX, X = Xa + (c - i * nX);
+            int lx0;
+            float fx;
+            resize_tap(X, mx_scale, a.mw, lx0, fx);
+            const int lx1 = min(lx0 + 1, a.mw - 1) - lxa;
+            lx0 -= lxa;
+            const float* c0 = s_cell + s_mtap[i][0] * nLX;
+            const float* c1 = s_cell + s_mtap[i][1] * nLX;
+            const float a0 = 1.0f - fx, a1 = fx, fy = s_mfy[i];
+            const float b0 = 1.0f - fy, b1 = fy;
+            const float h0 = __fadd_rn(__fmul_rn(c0[lx0], a0), __fmul_rn(c0[lx1], a1));  // HResizeLinear
+            const float h1 = __fadd_rn(__fmul_rn(c1[lx0], a0), __fmul_rn(c1[lx1], a1));
+            s_M[c] = __fadd_rn(__fmul_rn(h0, b0), __fmul_rn(h1, b1));                   // VResizeLinear
+        }
+        __syncthreads();
+    }
+    // S = scale_mask_kernel's expression over M, thresholded; each thread owns 16-column chunks of the band's rows
+    const int chunks = (im.img_w + 15) / 16;
+    const int tx = min(chunks, kSegThreads), ty = kSegThreads / tx;
+    const int tcol = tid % tx, trow = tid / tx;
+    if (trow >= ty) return;
+    uint8_t* plane = im.canvas + (size_t)k * im.img_h * im.pitch;
+    for (int c = tcol; c < chunks; c += tx) {
+        const int x0 = c * 16;
+        int key[16];  // 2 * (first M column - Xa) + (second column != first), or -1 outside get_rect
+        float fx[16];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            key[j] = -1;
+            fx[j] = 0.0f;
+            const int x = x0 + j;
+            if (touches && x >= x_lo && x < x_hi) {
+                int sx;
+                resize_tap(x, sx_scale, im.cw, sx, fx[j]);
+                key[j] = 2 * (im.cx + sx - Xa) + (sx + 1 < im.cw ? 1 : 0);
+            }
+        }
+        for (int y = y0 + trow; y < y1; y += ty) {
+            uint32_t w[4] = {0u, 0u, 0u, 0u};
+            if (touches && y >= ya && y < yb) {
+                const float* r0 = s_M + s_ytap[y - y0][0] * nX;
+                const float* r1 = s_M + s_ytap[y - y0][1] * nX;
+                const float fy = s_fy[y - y0];
+                const float b0 = 1.0f - fy, b1 = fy;
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    if (key[j] < 0) continue;
+                    const int m0 = key[j] >> 1, m1 = m0 + (key[j] & 1);
+                    const float a0 = 1.0f - fx[j], a1 = fx[j];
+                    const float h0 = __fadd_rn(__fmul_rn(r0[m0], a0), __fmul_rn(r0[m1], a1));
+                    const float h1 = __fadd_rn(__fmul_rn(r1[m0], a0), __fmul_rn(r1[m1], a1));
+                    const float v = __fadd_rn(__fmul_rn(h0, b0), __fmul_rn(h1, b1));
+                    if (!(v <= 0.5f)) w[j >> 2] |= 0xffu << (8 * (j & 3));  // draw_mask_bbox: `if (val <= 0.5) continue;`
+                }
+            }
+            uint8_t* dst = plane + (size_t)y * im.pitch + x0;
+            if (x0 + 16 <= im.img_w && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+                *reinterpret_cast<uint4*>(dst) = make_uint4(w[0], w[1], w[2], w[3]);
+            } else {  // unaligned rows (odd pitch or base) and the last chunk of a row
+#pragma unroll
+                for (int j = 0; j < 16; ++j)
+                    if (x0 + j < im.img_w) dst[j] = (uint8_t)(w[j >> 2] >> (8 * (j & 3)));
+            }
+        }
+    }
+}
+
+// Upper bounds of the y slots and cell slots a band can need (seg_canvas_kernel's lists), for a scale_mask row scale s:
+// the band's kSegBand row taps span (kSegBand - 1) * s (+ float rounding), so they take at most floor(7 s) + 2 values, + 1
+// for the upper taps; the rows of M they name span <= 7 s + 2, and process_mask's scale of 1/4 maps that onto at most
+// floor((7 s + 2) / 4) + 3 low-resolution rows.  One more of slack each, capped by the hard limits.
+static void seg_caps(double s, int& y_cap, int& ly_cap) {
+    const double span = (kSegBand - 1) * s;
+    y_cap = span + 4.0 < (double)kSegMaxY ? (int)span + 4 : kSegMaxY;
+    ly_cap = (span + 3.0) / 4.0 + 4.0 < (double)kSegMaxLY ? (int)((span + 3.0) / 4.0) + 4 : kSegMaxLY;
+    if (ly_cap > 2 * y_cap) ly_cap = 2 * y_cap;
+}
+
 }  // namespace trtx
 
 using namespace trtx;
@@ -494,6 +738,115 @@ TRTX_API int trtx_rcnn_postprocess_enqueue(const trtx_rcnn_post_params* p, int b
     pa.band_rows = band_rows;
     rcnn_paste_kernel<<<(unsigned)ctas, dim3(tx, ty), 0, s>>>(pa);
     return check_launch();
+}
+
+TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const trtx_seg_image* images_host, int batch,
+                                               const float* proto_dev, const float* dets_dev, int max_rows,
+                                               float* rows_dev, trtx_stream_t stream) {
+    if (!p || !images_host || batch <= 0 || !dets_dev || !rows_dev || max_rows <= 0) return TRTX_ERR_INVALID;
+    if (p->variant != TRTX_YOLO_V8 && p->variant != TRTX_YOLO_V5) return TRTX_ERR_INVALID;
+    if (p->net_w <= 0 || p->net_h <= 0 || p->row_floats < kSegRowFloats) return TRTX_ERR_INVALID;
+    // canvases for every image or for none
+    const bool masks = images_host[0].masks_dev != nullptr;
+    for (int i = 0; i < batch; ++i) {
+        const trtx_seg_image& d = images_host[i];
+        if ((d.masks_dev != nullptr) != masks || d.img_w <= 0 || d.img_h <= 0) return TRTX_ERR_INVALID;
+        if (masks && d.pitch < d.img_w) return TRTX_ERR_INVALID;
+    }
+    if (masks) {  // trtx_process_mask_enqueue's checks
+        if (!proto_dev) return TRTX_ERR_INVALID;
+        if (p->num_coeffs <= 0 || p->num_coeffs > kMaxCoeffs || p->max_masks <= 0) return TRTX_ERR_INVALID;
+        if (p->coeff_offset < 0 || p->coeff_offset + p->num_coeffs > p->row_floats) return TRTX_ERR_INVALID;
+        if (p->mask_w <= 0 || p->mask_h <= 0) return TRTX_ERR_INVALID;
+        if (p->net_w != 4 * p->mask_w || p->net_h != 4 * p->mask_h) return TRTX_ERR_UNSUPPORTED;
+    }
+    // every image is checked before the first launch, so that a rejected call writes nothing
+    size_t smem_max = 0;
+    for (int i0 = 0; masks && i0 < batch; i0 += kSegMaxImages) {
+        const int n = min(batch - i0, kSegMaxImages);
+        long long ctas = 0;
+        int y_cap = 1, ly_cap = 1, x_cap = 1;
+        for (int j = 0; j < n; ++j) {
+            const trtx_seg_image& d = images_host[i0 + j];
+            int r[4];
+            trtx_scale_mask_rect(p->net_w, p->net_h, d.img_w, d.img_h, r);
+            // an empty crop makes the reference's cv::resize throw
+            if (r[2] <= 0 || r[3] <= 0 || r[0] < 0 || r[1] < 0 || r[0] + r[2] > p->net_w || r[1] + r[3] > p->net_h)
+                return TRTX_ERR_UNSUPPORTED;
+            int yc, lyc;
+            seg_caps((double)r[3] / (double)d.img_h, yc, lyc);
+            y_cap = max(y_cap, yc);
+            ly_cap = max(ly_cap, lyc);
+            x_cap = max(x_cap, r[2]);
+            ctas += (long long)p->max_masks * ((d.img_h + kSegBand - 1) / kSegBand);
+        }
+        if (ctas > 0x7fffffffLL) return TRTX_ERR_UNSUPPORTED;
+        const int lx_cap = min(p->mask_w, x_cap / 4 + 4);
+        const size_t smem = ((size_t)y_cap * x_cap + (size_t)ly_cap * lx_cap) * sizeof(float);
+        smem_max = smem > smem_max ? smem : smem_max;
+    }
+    if (smem_max > 48 * 1024 &&
+        cudaFuncSetAttribute(seg_canvas_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) != cudaSuccess) {
+        g_last_cuda_error = (int)cudaGetLastError();
+        return TRTX_ERR_CUDA;
+    }
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SegArgs a;
+    a.proto = proto_dev;
+    a.dets = dets_dev;
+    a.rows = rows_dev;
+    a.max_rows = max_rows;
+    a.row_floats = p->row_floats;
+    a.coeff_offset = p->coeff_offset;
+    a.variant = p->variant;
+    a.nm = p->num_coeffs;
+    a.mw = p->mask_w;
+    a.mh = p->mask_h;
+    a.net_w = p->net_w;
+    a.net_h = p->net_h;
+    a.max_masks = p->max_masks;
+    for (int i0 = 0; i0 < batch; i0 += kSegMaxImages) {
+        const int n = min(batch - i0, kSegMaxImages);
+        a.base = i0;
+        a.n_images = n;
+        int ctas = 0;
+        a.y_cap = a.ly_cap = a.x_cap = 1;
+        for (int j = 0; j < n; ++j) {
+            const trtx_seg_image& d = images_host[i0 + j];
+            SegImage& im = a.img[j];
+            im.canvas = d.masks_dev;
+            im.img_w = d.img_w;
+            im.img_h = d.img_h;
+            im.pitch = d.pitch;
+            im.bands = (d.img_h + kSegBand - 1) / kSegBand;
+            im.first_cta = ctas;
+            if (!masks) continue;
+            int r[4];
+            trtx_scale_mask_rect(p->net_w, p->net_h, d.img_w, d.img_h, r);
+            im.cx = r[0];
+            im.cy = r[1];
+            im.cw = r[2];
+            im.ch = r[3];
+            int yc, lyc;
+            seg_caps((double)r[3] / (double)d.img_h, yc, lyc);
+            a.y_cap = max(a.y_cap, yc);
+            a.ly_cap = max(a.ly_cap, lyc);
+            a.x_cap = max(a.x_cap, r[2]);
+            ctas += p->max_masks * im.bands;
+        }
+        a.lx_cap = min(p->mask_w, a.x_cap / 4 + 4);
+        seg_rows_kernel<<<(n + 3) / 4, 128, 0, st>>>(a);
+        int rc = check_launch();
+        if (rc || !masks) {
+            if (rc) return rc;
+            continue;
+        }
+        const size_t smem = ((size_t)a.y_cap * a.x_cap + (size_t)a.ly_cap * a.lx_cap) * sizeof(float);
+        seg_canvas_kernel<<<(unsigned)ctas, kSegThreads, smem, st>>>(a);
+        rc = check_launch();
+        if (rc) return rc;
+    }
+    return TRTX_OK;
 }
 
 }  // extern "C"

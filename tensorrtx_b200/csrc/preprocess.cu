@@ -567,56 +567,12 @@ TRTX_API void trtx_letterbox_matrix(int sw, int sh, int dw, int dh, float d2s[6]
     d2s[5] = (float)b2;
 }
 
-// get_rect: the inverse of the letterbox for a detection box -- yolov8/src/postprocess.cpp:6-36 (TRTX_YOLO_V8: l,t,r,b,
-// clamped to the image) and yolov5/src/postprocess.cpp:4-29 (TRTX_YOLO_V5: cx,cy,w,h).  Host arithmetic, statement
-// by statement: the two ratios are double divisions stored to float, the rest is float, round() sees doubles.
+// get_rect: the inverse of the letterbox for a detection box (yolo_get_rect in common.cuh, which the segmentation
+// post-process kernels share).  Host function.
 TRTX_API int trtx_get_rect(int variant, int net_w, int net_h, int img_w, int img_h, const float bbox[4], int rect[4]) {
     if (!bbox || !rect || net_w <= 0 || net_h <= 0 || img_w <= 0 || img_h <= 0) return TRTX_ERR_INVALID;
     if (variant != TRTX_YOLO_V8 && variant != TRTX_YOLO_V5) return TRTX_ERR_INVALID;
-    float l, r, t, b;
-    const float r_w = (float)(net_w / (img_w * 1.0));
-    const float r_h = (float)(net_h / (img_h * 1.0));
-    const bool by_w = r_h > r_w;  // the width fills the network input: vertical padding
-    const float ratio = by_w ? r_w : r_h;
-    const float pad = by_w ? (net_h - r_w * img_h) / 2 : (net_w - r_h * img_w) / 2;
-    if (variant == TRTX_YOLO_V8) {
-        l = bbox[0];
-        r = bbox[2];
-        t = bbox[1];
-        b = bbox[3];
-    } else {
-        l = bbox[0] - bbox[2] / 2.f;
-        r = bbox[0] + bbox[2] / 2.f;
-        t = bbox[1] - bbox[3] / 2.f;
-        b = bbox[1] + bbox[3] / 2.f;
-    }
-    if (by_w) {
-        t = t - pad;
-        b = b - pad;
-    } else {
-        l = l - pad;
-        r = r - pad;
-    }
-    l = l / ratio;
-    r = r / ratio;
-    t = t / ratio;
-    b = b / ratio;
-    if (variant == TRTX_YOLO_V8) {
-        l = 0.0f > l ? 0.0f : l;
-        t = 0.0f > t ? 0.0f : t;
-        const int rw = (int)round((double)(r - l)), rl = (int)round((double)l);
-        const int rh = (int)round((double)(b - t)), rt = (int)round((double)t);
-        const int width = rw < img_w - rl ? rw : img_w - rl, height = rh < img_h - rt ? rh : img_h - rt;
-        rect[0] = rl;
-        rect[1] = rt;
-        rect[2] = width > 0 ? width : 0;
-        rect[3] = height > 0 ? height : 0;
-    } else {
-        rect[0] = (int)round((double)l);
-        rect[1] = (int)round((double)t);
-        rect[2] = (int)round((double)(r - l));
-        rect[3] = (int)round((double)(b - t));
-    }
+    yolo_get_rect(variant, net_w, net_h, img_w, img_h, bbox, rect);
     return TRTX_OK;
 }
 

@@ -894,6 +894,7 @@ TRTX_API size_t trtx_abi_sizeof(int which) {
         case 3: return sizeof(trtx_image_desc);
         case 4: return sizeof(trtx_mask_params);
         case 5: return sizeof(trtx_rcnn_post_params);
+        case 6: return sizeof(trtx_seg_image);
         default: return 0;
     }
 }

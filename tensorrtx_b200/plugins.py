@@ -594,6 +594,45 @@ def process_mask(proto: torch.Tensor, dets: torch.Tensor, max_rows: int, row_flo
     return out
 
 
+def yolo_seg_postprocess(proto: torch.Tensor | None, dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]], *,
+                         variant: int, max_rows: int, row_floats: int = 39, coeff_offset: int = 7, max_masks: int,
+                         net_w: int = 640, net_h: int = 640, masks: bool = True, rows_out: torch.Tensor | None = None,
+                         canvases_out: Sequence[torch.Tensor] | None = None, stream=None):
+    """GPU drop-in for the segmentation models' post-process after NMS: process_mask + scale_mask + draw_mask_bbox's mask
+    selection (yolov8/src/postprocess.cpp:228-248, yolov5/src/postprocess.cpp:148-167) for a batch of frames of any sizes.
+    proto [B, 32, net_h/4, net_w/4] (may be None with masks=False); dets [B, 1 + max_rows*row_floats] (count, rows);
+    image_sizes[b] = (img_w, img_h) of frame b ->
+    (rows [B, 1 + max_rows*6] fp32: count, then (x, y, w, h, conf, class) with x, y, w, h = get_rect(img, bbox);
+     per-image u8 canvases [max_masks, img_h, img_w]: 255 where draw_mask_bbox would colour the pixel, or None with masks=False).
+    `canvases_out[b]` may be any u8 cuda tensor [max_masks, img_h, img_w] with contiguous rows and slots (e.g. a view
+    [..., :img_w] of a pitched buffer);
+    canvases at or past an image's count are not written (new ones start zeroed).  Two launches per 64 images."""
+    lib = L.load()
+    B = len(image_sizes)
+    if dets.dim() != 2 or dets.shape[0] != B or dets.shape[1] < 1 + max_rows * row_floats:
+        raise ValueError(f"dets must be [{B}, >= {1 + max_rows * row_floats}]")
+    nm, mh, mw = (proto.shape[1], proto.shape[2], proto.shape[3]) if proto is not None else (32, net_h // 4, net_w // 4)
+    q = L.MaskParams(variant, net_w, net_h, mw, mh, nm, row_floats, coeff_offset, max_masks)
+    if rows_out is None:
+        rows_out = torch.empty((B, 1 + max_rows * 6), dtype=torch.float32, device=dets.device)
+    if masks and canvases_out is None:
+        canvases_out = [torch.zeros((max_masks, h, w), dtype=torch.uint8, device=dets.device) for w, h in image_sizes]
+    descs = (L.SegImage * B)()
+    for b, (w, h) in enumerate(image_sizes):
+        descs[b].img_w, descs[b].img_h = int(w), int(h)
+        if masks:
+            c = canvases_out[b]
+            if c.dtype != torch.uint8 or tuple(c.shape) != (max_masks, h, w) or c.stride(2) != 1 or \
+                    c.stride(0) != h * c.stride(1):
+                raise ValueError(f"canvas {b} must be u8 [{max_masks}, {h}, {w}] with contiguous rows and slots")
+            descs[b].masks_dev = c.data_ptr()
+            descs[b].pitch = int(c.stride(1))
+    L.check(lib.trtx_yolo_seg_postprocess_enqueue(C.byref(q), descs, B, None if proto is None else _ptr(proto), _ptr(dets),
+                                                  max_rows, _ptr(rows_out), _stream(stream)),
+            "trtx_yolo_seg_postprocess_enqueue")
+    return rows_out, (list(canvases_out) if masks else None)
+
+
 class FusedYoloDecodeNms:
     """YoloLayer inputs -> compact detections in two launches (scan + NMS), no plugin-format round trip.
     Owns its workspace/output buffers (allocated once; enqueue itself allocates nothing)."""
