@@ -49,7 +49,7 @@ TRTX_API const char* trtx_version(void);
 TRTX_API int trtx_last_cuda_error(void);
 /* sizeof() of the parameter structs as THIS library was compiled, so that an FFI binding (ctypes, cgo, ...) can check its
  * mirror of the layout: which = 0 trtx_yolo_params, 1 trtx_nms_params, 2 trtx_retina_params, 3 trtx_image_desc,
- * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_seg_image; anything else 0. */
+ * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_seg_image, 7 trtx_pose_obb_params; anything else 0. */
 TRTX_API size_t trtx_abi_sizeof(int which);
 
 /* =====================================================================================
@@ -330,9 +330,18 @@ TRTX_API void trtx_letterbox_matrix(int src_w, int src_h, int dst_w, int dst_h, 
 TRTX_API int trtx_get_rect(int variant, int net_w, int net_h, int img_w, int img_h, const float bbox[4], int rect[4]);
 
 /* get_rect_adapt_landmark (yolov8/src/postprocess.cpp:38-69): like get_rect for the pose models -- the box (l,t,r,b) becomes
- * a cv::Rect in the original image and the num_kpts keypoints (x, y, conf triplets, `lmk`) are mapped IN PLACE.  Host function. */
+ * a cv::Rect in the original image (trtx_get_rect's V8 result, {0, 0, 0, 0} where that is undefined) and the num_kpts
+ * keypoints (x, y, conf triplets, `lmk`) are mapped IN PLACE, the confidences untouched.  Host function; the device form is
+ * trtx_yolo_pose_obb_postprocess_enqueue. */
 TRTX_API int trtx_get_rect_adapt_landmark(int net_w, int net_h, int img_w, int img_h, const float bbox[4], float* lmk,
                                           int num_kpts, int rect[4]);
+/* get_corner (yolov8/src/postprocess.cpp:395-472 with net 640; yolo11/src/postprocess.cpp:425-502, whose get_rect_obb is
+ * get_rect with net 1024): the four corners of an oriented box (cx, cy, w, h in network pixels, angle in radians) in the
+ * original image, corners = {x0, y0, x1, y1, x2, y2, x3, y3} in get_corner's order, each clamped to the image.  A corner
+ * whose float -> int conversion is undefined in the reference (NaN, out of range) is 0, as the compiled reference gives on
+ * x86-64 after its clamp; a box whose get_rect is undefined gets four (0, 0) corners.  The reference's debug prints are
+ * not reproduced.  Host function; the device form is trtx_yolo_pose_obb_postprocess_enqueue. */
+TRTX_API int trtx_get_corner(int net_w, int net_h, int img_w, int img_h, const float cxcywh[4], float angle, int corners[8]);
 /* RetinaFace's own get_rect_adapt_landmark (retinaface/common.hpp:65-89): 5 landmarks as x, y pairs, modified in place; the box
  * corners are truncated to int and not clamped; rect = {x, y, w, h} in the original image. */
 TRTX_API int trtx_retina_get_rect_adapt_landmark(int input_w, int input_h, int img_w, int img_h, const float bbox[4], float lmk[10],
@@ -435,6 +444,38 @@ typedef struct trtx_seg_image {
 TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const trtx_seg_image* images_host, int batch,
                                                const float* proto_dev, const float* dets_dev, int max_rows,
                                                float* rows_dev, trtx_stream_t stream);
+
+/* The pose and oriented-box models' last host stage on the device: draw_bbox_keypoints_line's get_rect_adapt_landmark
+ * (yolov8/src/postprocess.cpp:173-205) and draw_bbox_obb's get_corner (:474-507; yolo11/src/postprocess.cpp:504-537), for a
+ * batch of original frames of any sizes.  The drawing itself stays with the caller. */
+enum {
+    TRTX_TASK_POSE = 1, /* keypoints: rectangle + num_kpts (x, y, conf) mapped to the frame */
+    TRTX_TASK_OBB = 2,  /* oriented boxes: four corners in the frame */
+};
+typedef struct trtx_pose_obb_params {
+    int32_t task;         /* TRTX_TASK_* */
+    int32_t net_w, net_h; /* network input: kInputW / kInputH (640), or kObbInputW / kObbInputH (1024) of yolo11-obb */
+    int32_t row_floats;   /* floats per row of dets_dev, >= 7 (box4, conf, class, keep, extras...) */
+    int32_t extra_offset; /* POSE: first keypoint float in a row; OBB: the angle (radians) */
+    int32_t num_kpts;     /* POSE: keypoints per row, 0..64 (kNumberOfPoints = 17); OBB: not read */
+} trtx_pose_obb_params;
+
+/* dets_dev [B, 1 + max_rows*row_floats]: count, then rows (box4, conf, class, keep, extras...) -- the compact NMS output:
+ *   pose: trtx_nms_enqueue(det_floats 90, extra_floats 51, extra_offset 38): row_floats 58, extra_offset 7, box l, t, r, b;
+ *   OBB : batch_nms_obb (TRTX_BOX_OBB, greedy or one-shot): row_floats 8, extra_offset 7, box cx, cy, w, h.
+ *   Of the first min(count, max_rows) rows only those with (int)keep == 1 are used (process_decode_ptr_host(_obb)): every
+ *   greedy row, the kept rows of a one-shot output.
+ * frame_wh_host: `batch` (img_w, img_h) pairs in HOST memory (copied into launch parameters; sizes may differ in a call).
+ * rows_dev [B, 1 + max_rows*F]: n kept rows in input order, then zeros up to max_rows:
+ *   pose, F = 6 + 3*num_kpts: (x, y, w, h, conf, class, kx, ky, kc, ...) = trtx_get_rect_adapt_landmark;
+ *   OBB,  F = 10: (x0, y0, x1, y1, x2, y2, x3, y3, conf, class) = trtx_get_corner.
+ * Bit-identical to those host functions (the device's double cos / sin are not correctly rounded, see trtx_get_corner).
+ * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
+ * batch / max_rows / sizes <= 0, an unknown task, row_floats < 7 or extras outside the row, num_kpts outside 0..64.  One
+ * launch per 64 frames, one CTA per frame, no atomics (deterministic), no workspace; can be captured in a CUDA graph. */
+TRTX_API int trtx_yolo_pose_obb_postprocess_enqueue(const trtx_pose_obb_params* p, const int32_t* frame_wh_host, int batch,
+                                                    const float* dets_dev, int max_rows, float* rows_dev,
+                                                    trtx_stream_t stream);
 
 /* =====================================================================================
  * 7. Mask R-CNN pre- and post-process

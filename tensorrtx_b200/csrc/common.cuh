@@ -158,14 +158,15 @@ __host__ __device__ inline bool round_to_int(float v, int& out) {
     return true;
 }
 
-// get_rect: the inverse of the letterbox for a detection box -- yolov8/src/postprocess.cpp:6-36 (TRTX_YOLO_V8: l,t,r,b,
-// clamped to the image) and yolov5/src/postprocess.cpp:4-29 (TRTX_YOLO_V5: cx,cy,w,h, not clamped).  Statement by statement:
-// the two ratios are double divisions stored to float, the rest is float, round() sees doubles.  Shared by the host
-// trtx_get_rect and the segmentation post-process kernels (mask.cu).  Returns false, with rect {0, 0, 0, 0}, where the
-// reference's float -> int conversions are undefined (a non-finite box, or rescaled corners outside the int range).
-__host__ __device__ inline bool yolo_get_rect(int variant, int net_w, int net_h, int img_w, int img_h, const float bbox[4],
-                                              int rect[4]) {
-    rect[0] = rect[1] = rect[2] = rect[3] = 0;
+// The letterbox of an img_w x img_h frame inside the net_w x net_h input, as get_rect and get_rect_adapt_landmark
+// (yolov8/src/postprocess.cpp:6-69) spell it: `kInputW / (img.cols * 1.0)` is a double division stored to float, the pad
+// `(kInputH - r_w * img.rows) / 2` is float.
+struct YoloLetterbox {
+    float ratio;  // r_w where the width fills the input (by_w), else r_h
+    float pad;    // the padding on the other axis, in network pixels
+    bool by_w;    // r_h > r_w: vertical padding
+};
+__host__ __device__ inline YoloLetterbox yolo_letterbox(int net_w, int net_h, int img_w, int img_h) {
 #ifdef __CUDA_ARCH__
     const float r_w = __double2float_rn(__ddiv_rn((double)net_w, (double)img_w));
     const float r_h = __double2float_rn(__ddiv_rn((double)net_h, (double)img_h));
@@ -173,10 +174,32 @@ __host__ __device__ inline bool yolo_get_rect(int variant, int net_w, int net_h,
     const float r_w = (float)(net_w / (img_w * 1.0));
     const float r_h = (float)(net_h / (img_h * 1.0));
 #endif
-    const bool by_w = r_h > r_w;  // the width fills the network input: vertical padding
-    const float ratio = by_w ? r_w : r_h;
-    const float pad = by_w ? f_div(f_sub((float)net_h, f_mul(r_w, (float)img_h)), 2.0f)
-                           : f_div(f_sub((float)net_w, f_mul(r_h, (float)img_w)), 2.0f);
+    YoloLetterbox lb;
+    lb.by_w = r_h > r_w;
+    lb.ratio = lb.by_w ? r_w : r_h;
+    lb.pad = lb.by_w ? f_div(f_sub((float)net_h, f_mul(r_w, (float)img_h)), 2.0f)
+                     : f_div(f_sub((float)net_w, f_mul(r_h, (float)img_w)), 2.0f);
+    return lb;
+}
+
+// One keypoint coordinate of get_rect_adapt_landmark (yolov8/src/postprocess.cpp:47-61): axis 0 = x, 1 = y.  The padded axis
+// loses the pad first, then both are divided by the ratio, all in float; the keypoint's confidence is not touched.
+__host__ __device__ inline float yolo_map_landmark(const YoloLetterbox& lb, int axis, float v) {
+    return (axis == 0) == lb.by_w ? f_div(v, lb.ratio) : f_div(f_sub(v, lb.pad), lb.ratio);
+}
+
+// get_rect: the inverse of the letterbox for a detection box -- yolov8/src/postprocess.cpp:6-36 (TRTX_YOLO_V8: l,t,r,b,
+// clamped to the image) and yolov5/src/postprocess.cpp:4-29 (TRTX_YOLO_V5: cx,cy,w,h, not clamped).  Statement by statement:
+// the two ratios are double divisions stored to float, the rest is float, round() sees doubles.  Shared by the host
+// trtx_get_rect and trtx_get_rect_adapt_landmark (whose rectangle is the same float expressions as the V8 branch), the
+// segmentation post-process kernels (mask.cu) and yolo_get_corner.  Returns false, with rect {0, 0, 0, 0}, where the
+// reference's float -> int conversions are undefined (a non-finite box, or rescaled corners outside the int range).
+__host__ __device__ inline bool yolo_get_rect(int variant, int net_w, int net_h, int img_w, int img_h, const float bbox[4],
+                                              int rect[4]) {
+    rect[0] = rect[1] = rect[2] = rect[3] = 0;
+    const YoloLetterbox lb = yolo_letterbox(net_w, net_h, img_w, img_h);
+    const bool by_w = lb.by_w;
+    const float ratio = lb.ratio, pad = lb.pad;
     float l, r, t, b;
     if (variant == TRTX_YOLO_V8) {
         l = bbox[0];
@@ -217,6 +240,67 @@ __host__ __device__ inline bool yolo_get_rect(int variant, int net_w, int net_h,
     rect[2] = rw;
     rect[3] = rh;
     return true;
+}
+
+// get_corner: the four corners of an oriented box in the original frame -- yolov8/src/postprocess.cpp:395-472 (net 640) and
+// yolo11/src/postprocess.cpp:425-502 (get_rect_obb: net 1024), statement by statement without the debug prints:
+//   angle = box.angle * 180.0f / CV_PI        float product, DOUBLE division, stored to float
+//   h >= w: swap w, h and angle = fmod(angle + 90.0f, 180.0f) (float; fmod is exact); then angle < 0: += 360, > 180: -= 180
+//   cos / sin of angle * CV_PI / 180.0f       double expression and double cos / sin, stored to float
+//   rect = get_rect of the axis-aligned l, t, r, b (cx -/+ w / 2, cy -/+ h / 2)
+//   x_ = (rect.x + rect.x + rect.width) / 2   INTEGER division (the sum wraps as the compiled x86-64 reference does)
+//   corner = int(round(x_ +/- vec1x +/- vec2x)) (float sums in source order), clamped to [0, cols - 1] x [0, rows - 1].
+// corners = {x0, y0, x1, y1, x2, y2, x3, y3} in get_corner's order.  Undefined cases of the reference, defined here as the
+// compiled reference behaves on x86-64: a corner whose float -> int conversion is undefined (NaN, out of range) converts to
+// INT_MIN there, which the clamp makes 0; a box whose get_rect is undefined gets four (0, 0) corners.  The device's double
+// cos / sin are within 2 ulp of glibc's, not correctly rounded: a float can differ only where the double lies that close
+// to a float rounding boundary.
+__host__ __device__ inline void yolo_get_corner(int net_w, int net_h, int img_w, int img_h, const float box[4], float box_angle,
+                                                int corners[8]) {
+    constexpr double kPi = 3.1415926535897932384626433832795;  // CV_PI
+    for (int k = 0; k < 8; ++k) corners[k] = 0;
+    float w = box[2], h = box[3];
+#ifdef __CUDA_ARCH__
+    float angle = __double2float_rn(__ddiv_rn((double)__fmul_rn(box_angle, 180.0f), kPi));
+#else
+    float angle = (float)((double)(box_angle * 180.0f) / kPi);
+#endif
+    if (h >= w) {
+        const float s = w;
+        w = h;
+        h = s;
+        angle = fmodf(f_add(angle, 90.0f), 180.0f);
+    }
+    if (angle < 0) angle = f_add(angle, 360.0f);
+    if (angle > 180.0f) angle = f_sub(angle, 180.0f);
+#ifdef __CUDA_ARCH__
+    const double rad = __ddiv_rn(__dmul_rn((double)angle, kPi), 180.0);
+    const float cos_value = __double2float_rn(cos(rad)), sin_value = __double2float_rn(sin(rad));
+#else
+    const double rad = (double)angle * kPi / 180.0;
+    const float cos_value = (float)cos(rad), sin_value = (float)sin(rad);
+#endif
+    const float bbox[4] = {f_sub(box[0], f_div(w, 2.0f)), f_sub(box[1], f_div(h, 2.0f)), f_add(box[0], f_div(w, 2.0f)),
+                           f_add(box[1], f_div(h, 2.0f))};
+    int rect[4];
+    if (!yolo_get_rect(TRTX_YOLO_V8, net_w, net_h, img_w, img_h, bbox, rect)) return;
+    const float x_ = (float)((int)((unsigned)rect[0] + (unsigned)rect[0] + (unsigned)rect[2]) / 2);
+    const float y_ = (float)((int)((unsigned)rect[1] + (unsigned)rect[1] + (unsigned)rect[3]) / 2);
+    const float width = (float)rect[2], height = (float)rect[3];
+    const float vec1x = f_mul(f_div(width, 2.0f), cos_value);
+    const float vec1y = f_mul(f_div(width, 2.0f), sin_value);
+    const float vec2x = f_mul(f_div(-height, 2.0f), sin_value);
+    const float vec2y = f_mul(f_div(height, 2.0f), cos_value);
+    const float v[8] = {f_add(f_add(x_, vec1x), vec2x), f_add(f_add(y_, vec1y), vec2y),
+                        f_sub(f_add(x_, vec1x), vec2x), f_sub(f_add(y_, vec1y), vec2y),
+                        f_sub(f_sub(x_, vec1x), vec2x), f_sub(f_sub(y_, vec1y), vec2y),
+                        f_add(f_sub(x_, vec1x), vec2x), f_add(f_sub(y_, vec1y), vec2y)};
+    for (int k = 0; k < 8; ++k) {
+        const int hi = (k & 1) ? img_h - 1 : img_w - 1;
+        int c;
+        if (!round_to_int(v[k], c)) c = 0;  // INT_MIN in the reference, then its clamp
+        corners[k] = c < 0 ? 0 : (c > hi ? hi : c);
+    }
 }
 
 __device__ __forceinline__ int warp_excl_scan(int v, int lane, int* total) {

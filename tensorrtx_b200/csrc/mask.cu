@@ -590,6 +590,93 @@ static void seg_caps(double s, int& y_cap, int& ly_cap) {
     if (ly_cap > 2 * y_cap) ly_cap = 2 * y_cap;
 }
 
+// Pose and oriented-box post-process: the per-detection geometry of draw_bbox_keypoints_line (get_rect_adapt_landmark,
+// yolov8/src/postprocess.cpp:173-205) and draw_bbox_obb (get_corner, :474-507), which the reference runs on one host core
+// after a D2H copy.  One CTA of kPoseObbThreads per frame, one launch per <= 64 frames, no workspace, no atomics:
+//   the CTA walks the first min(count, max_rows) rows in passes of kPoseObbThreads, one row per thread; a ballot per warp
+//   over the keep column and a scan of the warps' counts give each kept row its output slot (input order); the owning
+//   thread computes the rectangle (yolo_get_rect) or the four corners (yolo_get_corner) into shared memory; then the whole
+//   CTA writes the pass's kept rows as one contiguous run of floats (coalesced), mapping each keypoint coordinate with
+//   yolo_map_landmark on the way.  Rows past the kept count are zeroed.
+constexpr int kPoseObbMaxImages = 64;  // frames per launch (launch-parameter array)
+constexpr int kPoseObbThreads = 256;   // rows per pass
+constexpr int kPoseObbWarps = kPoseObbThreads / kWarp;
+constexpr int kPoseMaxKpts = 64;
+
+struct PoseObbArgs {
+    int img_w[kPoseObbMaxImages], img_h[kPoseObbMaxImages];
+    const float* dets;  // [B, 1 + max_rows * row_floats]
+    float* rows;        // [B, 1 + max_rows * out_floats]
+    int base;           // frames [base, base + gridDim.x) of the call
+    int pose, net_w, net_h, row_floats, extra_offset, num_kpts, out_floats, max_rows;
+};
+
+__global__ void __launch_bounds__(kPoseObbThreads) pose_obb_rows_kernel(const __grid_constant__ PoseObbArgs a) {
+    __shared__ int s_src[kPoseObbThreads];      // input row of each kept row of the pass, by output slot
+    __shared__ int s_geo[kPoseObbThreads * 8];  // its rectangle (pose: 4 ints) or corners (OBB: 8 ints)
+    __shared__ int s_warp[kPoseObbWarps];       // kept rows per warp of the pass
+    const int j = blockIdx.x, tid = threadIdx.x, lane = tid & (kWarp - 1), warp = tid / kWarp, b = a.base + j;
+    const int img_w = a.img_w[j], img_h = a.img_h[j];
+    const size_t R = (size_t)a.row_floats, F = (size_t)a.out_floats;
+    const float* src = a.dets + (size_t)b * (1 + (size_t)a.max_rows * R);
+    float* out = a.rows + (size_t)b * (1 + (size_t)a.max_rows * F);
+    const int n = min(max((int)src[0], 0), a.max_rows);
+    const YoloLetterbox lb = yolo_letterbox(a.net_w, a.net_h, img_w, img_h);
+    const int geo = a.pose ? 4 : 8;  // floats of the row before conf and class
+    int kept = 0;                    // rows written by the earlier passes
+    for (int i0 = 0; i0 < n; i0 += kPoseObbThreads) {
+        const int i = i0 + tid;
+        const float* d = src + 1 + (size_t)i * R;
+        const bool keep = i < n && (int)d[6] == 1;  // process_decode_ptr_host: `int keep_flag = ...; if (keep_flag == 1)`
+        const unsigned m = __ballot_sync(0xffffffffu, keep);
+        if (lane == 0) s_warp[warp] = __popc(m);
+        __syncthreads();
+        int before = 0, total = 0;
+#pragma unroll
+        for (int w = 0; w < kPoseObbWarps; ++w) {
+            const int c = s_warp[w];
+            before += w < warp ? c : 0;
+            total += c;
+        }
+        if (keep) {
+            const int slot = before + __popc(m & ((1u << lane) - 1u));
+            int g[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+            if (a.pose)
+                yolo_get_rect(TRTX_YOLO_V8, a.net_w, a.net_h, img_w, img_h, d, g);  // {0, 0, 0, 0} where undefined
+            else
+                yolo_get_corner(a.net_w, a.net_h, img_w, img_h, d, d[a.extra_offset], g);
+            s_src[slot] = i;
+#pragma unroll
+            for (int e = 0; e < 8; ++e) s_geo[slot * 8 + e] = g[e];
+        }
+        __syncthreads();
+        const size_t run = (size_t)total * F;
+        float* o = out + 1 + (size_t)kept * F;
+#pragma unroll 4
+        for (size_t f = tid; f < run; f += kPoseObbThreads) {
+            const int r = (int)(f / F), e = (int)(f - (size_t)r * F);
+            const float* d2 = src + 1 + (size_t)s_src[r] * R;
+            float v;
+            if (e < geo) {
+                v = (float)s_geo[r * 8 + e];
+            } else if (e < geo + 2) {
+                v = d2[4 + e - geo];  // conf, class
+            } else {
+                const int k = e - 6;  // keypoint float: x, y, conf
+                const int c = k % 3;
+                const float x = d2[a.extra_offset + k];
+                v = c == 2 ? x : yolo_map_landmark(lb, c, x);
+            }
+            o[f] = v;
+        }
+        kept += total;
+        __syncthreads();  // the next pass reuses the shared arrays
+    }
+    const size_t end = 1 + (size_t)a.max_rows * F;
+    for (size_t f = 1 + (size_t)kept * F + tid; f < end; f += kPoseObbThreads) out[f] = 0.0f;
+    if (tid == 0) out[0] = (float)kept;
+}
+
 }  // namespace trtx
 
 using namespace trtx;
@@ -844,6 +931,45 @@ TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const 
         const size_t smem = ((size_t)a.y_cap * a.x_cap + (size_t)a.ly_cap * a.lx_cap) * sizeof(float);
         seg_canvas_kernel<<<(unsigned)ctas, kSegThreads, smem, st>>>(a);
         rc = check_launch();
+        if (rc) return rc;
+    }
+    return TRTX_OK;
+}
+
+TRTX_API int trtx_yolo_pose_obb_postprocess_enqueue(const trtx_pose_obb_params* p, const int32_t* frame_wh_host, int batch,
+                                                    const float* dets_dev, int max_rows, float* rows_dev,
+                                                    trtx_stream_t stream) {
+    if (!p || !frame_wh_host || batch <= 0 || !dets_dev || !rows_dev || max_rows <= 0) return TRTX_ERR_INVALID;
+    if (p->task != TRTX_TASK_POSE && p->task != TRTX_TASK_OBB) return TRTX_ERR_INVALID;
+    if (p->net_w <= 0 || p->net_h <= 0 || p->row_floats < 7 || p->extra_offset < 0) return TRTX_ERR_INVALID;
+    const bool pose = p->task == TRTX_TASK_POSE;
+    if (pose && (p->num_kpts < 0 || p->num_kpts > kPoseMaxKpts || p->extra_offset + 3 * p->num_kpts > p->row_floats))
+        return TRTX_ERR_INVALID;
+    if (!pose && p->extra_offset >= p->row_floats) return TRTX_ERR_INVALID;
+    // every frame is checked before the first launch, so that a rejected call writes nothing
+    for (int i = 0; i < batch; ++i)
+        if (frame_wh_host[2 * i] <= 0 || frame_wh_host[2 * i + 1] <= 0) return TRTX_ERR_INVALID;
+    PoseObbArgs a;
+    a.dets = dets_dev;
+    a.rows = rows_dev;
+    a.pose = pose;
+    a.net_w = p->net_w;
+    a.net_h = p->net_h;
+    a.row_floats = p->row_floats;
+    a.extra_offset = p->extra_offset;
+    a.num_kpts = pose ? p->num_kpts : 0;
+    a.out_floats = pose ? 6 + 3 * p->num_kpts : 10;
+    a.max_rows = max_rows;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    for (int i0 = 0; i0 < batch; i0 += kPoseObbMaxImages) {
+        const int n = min(batch - i0, kPoseObbMaxImages);
+        a.base = i0;
+        for (int j = 0; j < n; ++j) {
+            a.img_w[j] = frame_wh_host[2 * (i0 + j)];
+            a.img_h[j] = frame_wh_host[2 * (i0 + j) + 1];
+        }
+        pose_obb_rows_kernel<<<n, kPoseObbThreads, 0, st>>>(a);
+        const int rc = check_launch();
         if (rc) return rc;
     }
     return TRTX_OK;

@@ -576,43 +576,26 @@ TRTX_API int trtx_get_rect(int variant, int net_w, int net_h, int img_w, int img
     return TRTX_OK;
 }
 
-// get_rect_adapt_landmark, yolov8/src/postprocess.cpp:38-69, statement by statement (ratios: double division stored to float;
-// `(kInputH - r_w * img.rows) / 2`: int - float*int in float, then / 2).
+// get_rect_adapt_landmark, yolov8/src/postprocess.cpp:38-69: its rectangle is get_rect's V8 branch (the same float
+// expressions), its keypoints yolo_map_landmark (common.cuh, shared with the pose post-process kernel of mask.cu).
 TRTX_API int trtx_get_rect_adapt_landmark(int net_w, int net_h, int img_w, int img_h, const float bbox[4], float* lmk,
                                           int num_kpts, int rect[4]) {
     if (!bbox || !rect || (num_kpts > 0 && !lmk) || num_kpts < 0 || net_w <= 0 || net_h <= 0 || img_w <= 0 || img_h <= 0)
         return TRTX_ERR_INVALID;
-    float l, r, t, b;
-    const float r_w = (float)(net_w / (img_w * 1.0));
-    const float r_h = (float)(net_h / (img_h * 1.0));
-    if (r_h > r_w) {
-        l = bbox[0] / r_w;
-        r = bbox[2] / r_w;
-        t = (bbox[1] - (net_h - r_w * img_h) / 2) / r_w;
-        b = (bbox[3] - (net_h - r_w * img_h) / 2) / r_w;
-        for (int i = 0; i < num_kpts * 3; i += 3) {
-            lmk[i] /= r_w;
-            lmk[i + 1] = (lmk[i + 1] - (net_h - r_w * img_h) / 2) / r_w;
-        }
-    } else {
-        l = (bbox[0] - (net_w - r_h * img_w) / 2) / r_h;
-        r = (bbox[2] - (net_w - r_h * img_w) / 2) / r_h;
-        t = bbox[1] / r_h;
-        b = bbox[3] / r_h;
-        for (int i = 0; i < num_kpts * 3; i += 3) {
-            lmk[i] = (lmk[i] - (net_w - r_h * img_w) / 2) / r_h;
-            lmk[i + 1] /= r_h;
-        }
+    const YoloLetterbox lb = yolo_letterbox(net_w, net_h, img_w, img_h);
+    for (int i = 0; i < num_kpts * 3; i += 3) {
+        lmk[i] = yolo_map_landmark(lb, 0, lmk[i]);
+        lmk[i + 1] = yolo_map_landmark(lb, 1, lmk[i + 1]);
     }
-    l = 0.0f > l ? 0.0f : l;
-    t = 0.0f > t ? 0.0f : t;
-    const int rw = (int)round((double)(r - l)), rl = (int)round((double)l);
-    const int rh = (int)round((double)(b - t)), rt = (int)round((double)t);
-    const int width = rw < img_w - rl ? rw : img_w - rl, height = rh < img_h - rt ? rh : img_h - rt;
-    rect[0] = rl;
-    rect[1] = rt;
-    rect[2] = width > 0 ? width : 0;
-    rect[3] = height > 0 ? height : 0;
+    yolo_get_rect(TRTX_YOLO_V8, net_w, net_h, img_w, img_h, bbox, rect);  // {0, 0, 0, 0} where undefined
+    return TRTX_OK;
+}
+
+// get_corner, yolov8/src/postprocess.cpp:395-472 / yolo11/src/postprocess.cpp:425-502 (yolo_get_corner in common.cuh, shared
+// with the oriented-box post-process kernel of mask.cu).
+TRTX_API int trtx_get_corner(int net_w, int net_h, int img_w, int img_h, const float cxcywh[4], float angle, int corners[8]) {
+    if (!cxcywh || !corners || net_w <= 0 || net_h <= 0 || img_w <= 0 || img_h <= 0) return TRTX_ERR_INVALID;
+    yolo_get_corner(net_w, net_h, img_w, img_h, cxcywh, angle, corners);
     return TRTX_OK;
 }
 

@@ -633,6 +633,37 @@ def yolo_seg_postprocess(proto: torch.Tensor | None, dets: torch.Tensor, image_s
     return rows_out, (list(canvases_out) if masks else None)
 
 
+def yolo_pose_obb_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]], *, task: int, max_rows: int,
+                              row_floats: int | None = None, extra_offset: int = 7, num_kpts: int = 17, net_w: int = 640,
+                              net_h: int = 640, rows_out: torch.Tensor | None = None, stream=None) -> torch.Tensor:
+    """GPU drop-in for the pose and oriented-box models' geometry after NMS: get_rect_adapt_landmark of
+    draw_bbox_keypoints_line (task TASK_POSE, yolov8/src/postprocess.cpp:173-205) or get_corner of draw_bbox_obb (task
+    TASK_OBB, :474-507; yolo11-obb: net_w = net_h = 1024) for a batch of frames of any sizes.
+    dets [B, 1 + max_rows*row_floats]: count, then (box4, conf, class, keep, extras...) rows -- the compact NMS output (pose:
+    extra_floats 51, row_floats 58; OBB: batch_nms_obb, row_floats 8); only rows with (int)keep == 1 are used.
+    image_sizes[b] = (img_w, img_h) of frame b -> rows [B, 1 + max_rows*F] fp32: the kept count, then per kept row (input
+    order) pose (x, y, w, h, conf, class, kx, ky, kc, ...), F = 6 + 3*num_kpts, or OBB (x0, y0, ..., x3, y3, conf, class),
+    F = 10; rows past the count are zero.  One launch per 64 frames, no workspace."""
+    lib = L.load()
+    B = len(image_sizes)
+    if row_floats is None:
+        row_floats = 7 + 3 * num_kpts if task == L.TASK_POSE else 8
+    if dets.dim() != 2 or dets.shape[0] != B or dets.shape[1] < 1 + max_rows * row_floats:
+        raise ValueError(f"dets must be [{B}, >= {1 + max_rows * row_floats}]")
+    if dets.dtype != torch.float32 or dets.stride(1) != 1 or dets.stride(0) != dets.shape[1]:
+        raise ValueError("dets must be contiguous float32")
+    F = 6 + 3 * num_kpts if task == L.TASK_POSE else 10
+    q = L.PoseObbParams(task, net_w, net_h, row_floats, extra_offset, num_kpts)
+    if rows_out is None:
+        rows_out = torch.empty((B, 1 + max_rows * F), dtype=torch.float32, device=dets.device)
+    if tuple(rows_out.shape) != (B, 1 + max_rows * F) or rows_out.dtype != torch.float32 or not rows_out.is_contiguous():
+        raise ValueError(f"rows_out must be contiguous float32 [{B}, {1 + max_rows * F}]")
+    wh = (C.c_int32 * (2 * B))(*[int(v) for s in image_sizes for v in s])
+    L.check(lib.trtx_yolo_pose_obb_postprocess_enqueue(C.byref(q), wh, B, _ptr(dets), max_rows, _ptr(rows_out),
+                                                       _stream(stream)), "trtx_yolo_pose_obb_postprocess_enqueue")
+    return rows_out
+
+
 class FusedYoloDecodeNms:
     """YoloLayer inputs -> compact detections in two launches (scan + NMS), no plugin-format round trip.
     Owns its workspace/output buffers (allocated once; enqueue itself allocates nothing)."""
@@ -1014,6 +1045,15 @@ def get_rect_adapt_landmark(img_w: int, img_h: int, bbox, lmk, net_w: int = 640,
     r = (C.c_int * 4)()
     L.check(lib.trtx_get_rect_adapt_landmark(net_w, net_h, img_w, img_h, b, k, len(lmk) // 3, r), "trtx_get_rect_adapt_landmark")
     return tuple(r), list(k)
+
+
+def get_corner(img_w: int, img_h: int, cxcywh, angle: float, net_w: int = 640, net_h: int = 640):
+    """get_corner(img, box) of yolov8/src/postprocess.cpp:395-472 (net_w = net_h = 1024: yolo11's get_rect_obb) ->
+    ((x0, y0), (x1, y1), (x2, y2), (x3, y3)) in the original image."""
+    b = (C.c_float * 4)(*[float(v) for v in cxcywh])
+    c = (C.c_int * 8)()
+    L.check(L.load().trtx_get_corner(net_w, net_h, img_w, img_h, b, float(angle), c), "trtx_get_corner")
+    return tuple((c[2 * k], c[2 * k + 1]) for k in range(4))
 
 
 def scale_mask(masks: torch.Tensor, img_w: int, img_h: int, out=None, stream=None) -> torch.Tensor:
