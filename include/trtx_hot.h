@@ -49,7 +49,7 @@ TRTX_API const char* trtx_version(void);
 TRTX_API int trtx_last_cuda_error(void);
 /* sizeof() of the parameter structs as THIS library was compiled, so that an FFI binding (ctypes, cgo, ...) can check its
  * mirror of the layout: which = 0 trtx_yolo_params, 1 trtx_nms_params, 2 trtx_retina_params, 3 trtx_image_desc,
- * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_seg_image, 7 trtx_pose_obb_params; anything else 0. */
+ * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_seg_image, 7 trtx_pose_obb_params, 8 trtx_rcnn_image; anything else 0. */
 TRTX_API size_t trtx_abi_sizeof(int which);
 
 /* =====================================================================================
@@ -501,7 +501,8 @@ TRTX_API int trtx_rcnn_preprocess_enqueue(const trtx_image_desc* images_host, in
 
 typedef struct trtx_rcnn_post_params {
     int32_t net_w, net_h;      /* INPUT_W, INPUT_H */
-    int32_t img_w, img_h;      /* w_ori, h_ori: one original size per call (mixed sizes: one call each, offset pointers) */
+    int32_t img_w, img_h;      /* w_ori, h_ori: one original size per call; frames of mixed sizes go through
+                                  trtx_rcnn_postprocess_frames_enqueue, which does not read these two */
     int32_t detections_per_im; /* DETECTIONS_PER_IMAGE (100): rows of BatchedNms's outputs */
     int32_t mask_size;         /* POOLER_RESOLUTION (14): masks are [S, S]; at most 32 */
     int32_t max_masks;         /* canvases written per image: the first min(count, max_masks) kept rows */
@@ -520,6 +521,31 @@ typedef struct trtx_rcnn_post_params {
 TRTX_API int trtx_rcnn_postprocess_enqueue(const trtx_rcnn_post_params* p, int batch, const float* scores_dev,
                                            const float* boxes_dev, const float* classes_dev, const float* masks_dev,
                                            float* rows_dev, uint8_t* masks_out_dev, trtx_stream_t stream);
+
+/* The same post-process for a batch of frames of mixed original sizes, one descriptor per frame. */
+typedef struct trtx_rcnn_image {
+    int32_t img_w, img_h; /* w_ori, h_ori of this frame */
+    uint8_t* masks_dev;   /* [max_masks, img_h, pitch] u8 canvases of this frame, or NULL (rows only) */
+    int32_t pitch;        /* bytes per canvas row, >= img_w; any value, any base alignment */
+    int32_t reserved;
+} trtx_rcnn_image;
+
+/* p: as for trtx_rcnn_postprocess_enqueue except img_w / img_h, which are not read.  images_host: `batch` descriptors in
+ *   HOST memory (copied into launch parameters).  scores_dev, boxes_dev, classes_dev, masks_dev and rows_dev: the layouts of
+ *   trtx_rcnn_postprocess_enqueue (the engine input net_w x net_h is one size per call).
+ * Image b is rescaled with its own pads, trtx_rcnn_letterbox_pads(img_w_b, img_h_b, net_w, net_h), and its own ratios, and
+ *   its canvas k starts at masks_dev_b + k * img_h_b * pitch_b: image b of a call equals a batch-1
+ *   trtx_rcnn_postprocess_enqueue of image b with its size.  Pixel rule, threshold and untouched canvases as there; the
+ *   bytes of a row past img_w are never written.
+ * Canvases for every frame or for none: NULL and non-NULL masks_dev in one call, or canvases with a NULL masks_dev input,
+ *   is TRTX_ERR_INVALID (with no canvases masks_dev is not read).  Everything is checked before the first launch (a
+ *   rejected call writes nothing): TRTX_ERR_INVALID for null pointers, batch / sizes <= 0, pitch < img_w, mask_size > 32;
+ *   TRTX_ERR_UNSUPPORTED for more than INT_MAX paste CTAs in one launch.  Two launches per 64 frames, no workspace, no
+ *   atomics; can be captured in a CUDA graph. */
+TRTX_API int trtx_rcnn_postprocess_frames_enqueue(const trtx_rcnn_post_params* p, const trtx_rcnn_image* images_host,
+                                                  int batch, const float* scores_dev, const float* boxes_dev,
+                                                  const float* classes_dev, const float* masks_dev, float* rows_dev,
+                                                  trtx_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -108,6 +108,11 @@ class PoseObbParams(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("task", "net_w", "net_h", "row_floats", "extra_offset", "num_kpts")]
 
 
+class RcnnImage(C.Structure):
+    _fields_ = [("img_w", C.c_int32), ("img_h", C.c_int32), ("masks_dev", C.c_void_p), ("pitch", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
 # TRTX_LIB: another build of the same ABI (the probe build of tools/nms_probe.py); default = the in-tree release library
 LIB_PATH = Path(os.environ.get("TRTX_LIB") or Path(__file__).resolve().parent / "lib" / "libtrtx_hot.so")
 
@@ -150,6 +155,8 @@ SYMBOLS = {
     "trtx_scale_mask_enqueue": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "trtx_rcnn_letterbox_pads": (_i, [_i, _i, _i, _i, C.POINTER(C.c_int)]),
     "trtx_rcnn_postprocess_enqueue": (_i, [C.POINTER(RcnnPostParams), _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "trtx_rcnn_postprocess_frames_enqueue": (_i, [C.POINTER(RcnnPostParams), C.POINTER(RcnnImage), _i, _vp, _vp, _vp, _vp,
+                                                  _vp, _vp]),
     "trtx_rcnn_preprocess_enqueue": (_i, [C.POINTER(ImageDesc), _i, _i, _i, _vp, _vp]),
     "trtx_yolo_seg_postprocess_enqueue": (_i, [C.POINTER(MaskParams), C.POINTER(SegImage), _i, _vp, _vp, _i, _vp, _vp]),
     "trtx_get_corner": (_i, [_i, _i, _i, _i, C.POINTER(C.c_float), _f, C.POINTER(C.c_int)]),
@@ -185,7 +192,7 @@ def load() -> C.CDLL:
         fn.restype = res
         fn.argtypes = args
     for which, st in enumerate((YoloParams, NmsParams, RetinaParams, ImageDesc, MaskParams, RcnnPostParams,
-                                   SegImage, PoseObbParams)):
+                                   SegImage, PoseObbParams, RcnnImage)):
         if lib.trtx_abi_sizeof(which) != C.sizeof(st):
             raise TrtxError(f"{LIB_PATH} was built from a different trtx_hot.h: sizeof({st.__name__}) = "
                             f"{lib.trtx_abi_sizeof(which)} in the library, {C.sizeof(st)} in the binding (rebuild)")

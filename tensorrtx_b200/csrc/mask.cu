@@ -211,10 +211,14 @@ __global__ void __launch_bounds__(256) scale_mask_kernel(const __grid_constant__
 //                     cv::resize(mask, r.size()) > 0.5 inside the paste rectangle r (:543-550), 0 elsewhere.
 // The paste is bound by HBM writes (one byte per canvas pixel).  Each thread owns 16 adjacent columns (one 16-byte store per
 // row) and computes their horizontal taps once for all the rows of its band; a band that misses r's rows stores zeros only.
+// The per-frame entry (trtx_rcnn_postprocess_frames_enqueue) runs the same two steps, rcnn_rows_frames_kernel and
+// rcnn_paste_frames_kernel, with each frame's size, pads, canvases and pitch in the launch parameters; both pairs of kernels
+// call the same per-image (rcnn_rows_image) and per-band (rcnn_paste_band) device functions.
 constexpr int kRcnnRowFloats = 7;      // x1, y1, x2, y2, score, class, slot
 constexpr int kRcnnMaxMask = 32;       // largest mask_size the shared-memory stage holds
 constexpr int kPasteThreads = 256;
-constexpr int kPastePasses = 8;        // row passes per CTA: band = kPastePasses * blockDim.y rows (~30 KB)
+constexpr int kPastePasses = 8;        // row passes per CTA: band = kPastePasses * ty rows (~30 KB)
+constexpr int kRcnnMaxImages = 64;     // frames per launch of the per-frame entry (launch-parameter array)
 
 struct RcnnRowsArgs {
     const float* scores;   // [B, D]
@@ -227,32 +231,40 @@ struct RcnnRowsArgs {
     float w_ratio, h_ratio;
 };
 
-__global__ void __launch_bounds__(128) rcnn_rows_kernel(const __grid_constant__ RcnnRowsArgs a) {
-    const int b = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (b >= a.batch) return;
-    const size_t base = (size_t)b * a.dets;
-    float* out = a.rows + (size_t)b * (1 + (size_t)a.dets * kRcnnRowFloats);
+// One warp: the rows of image b (scores / boxes / classes / out already offset to it).
+__device__ __forceinline__ void rcnn_rows_image(const float* scores, const float* boxes, const float* classes, float* out,
+                                                int dets, float thresh, int pad_l, int pad_t, float w_ratio, float h_ratio,
+                                                int lane) {
     int n = 0;
-    for (int i0 = 0; i0 < a.dets; i0 += 32) {
+    for (int i0 = 0; i0 < dets; i0 += 32) {
         const int i = i0 + lane;
-        const float s = i < a.dets ? a.scores[base + i] : 0.0f;
-        const bool keep = i < a.dets && s > a.thresh;  // :522; a NaN score is not kept
+        const float s = i < dets ? scores[i] : 0.0f;
+        const bool keep = i < dets && s > thresh;  // :522; a NaN score is not kept
         const unsigned m = __ballot_sync(0xffffffffu, keep);
         if (keep) {
             float* r = out + 1 + (size_t)(n + __popc(m & ((1u << lane) - 1u))) * kRcnnRowFloats;
-            const float* bx = a.boxes + (base + i) * 4;
-            r[0] = __fmul_rn(__fsub_rn(bx[0], (float)a.pad_l), a.w_ratio);
-            r[1] = __fmul_rn(__fsub_rn(bx[1], (float)a.pad_t), a.h_ratio);
-            r[2] = __fmul_rn(__fsub_rn(bx[2], (float)a.pad_l), a.w_ratio);
-            r[3] = __fmul_rn(__fsub_rn(bx[3], (float)a.pad_t), a.h_ratio);
+            const float* bx = boxes + (size_t)i * 4;
+            r[0] = __fmul_rn(__fsub_rn(bx[0], (float)pad_l), w_ratio);
+            r[1] = __fmul_rn(__fsub_rn(bx[1], (float)pad_t), h_ratio);
+            r[2] = __fmul_rn(__fsub_rn(bx[2], (float)pad_l), w_ratio);
+            r[3] = __fmul_rn(__fsub_rn(bx[3], (float)pad_t), h_ratio);
             r[4] = s;
-            r[5] = a.classes[base + i];
+            r[5] = classes[i];
             r[6] = (float)i;
         }
         n += __popc(m);
     }
-    for (int e = n * kRcnnRowFloats + lane; e < a.dets * kRcnnRowFloats; e += 32) out[1 + e] = 0.0f;
+    for (int e = n * kRcnnRowFloats + lane; e < dets * kRcnnRowFloats; e += 32) out[1 + e] = 0.0f;
     if (lane == 0) out[0] = (float)n;
+}
+
+__global__ void __launch_bounds__(128) rcnn_rows_kernel(const __grid_constant__ RcnnRowsArgs a) {
+    const int b = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (b >= a.batch) return;
+    const size_t base = (size_t)b * a.dets;
+    rcnn_rows_image(a.scores + base, a.boxes + base * 4, a.classes + base,
+                    a.rows + (size_t)b * (1 + (size_t)a.dets * kRcnnRowFloats), a.dets, a.thresh, a.pad_l, a.pad_t, a.w_ratio,
+                    a.h_ratio, lane);
 }
 
 // One axis of the paste rectangle (:543-546): floor(lo) - 1 clamped at 0, ceil(hi) + 1 clamped at `size`, then cv::Rect's
@@ -276,35 +288,34 @@ __device__ __forceinline__ bool rcnn_mask_rect(const float* r, int img_w, int im
     return rcnn_rect_axis(r[0], r[2], img_w, rx, rw) && rcnn_rect_axis(r[1], r[3], img_h, ry, rh);
 }
 
-struct RcnnPasteArgs {
-    const float* rows;   // [B, 1 + D * 7], written by rcnn_rows_kernel
-    const float* masks;  // [B, D, S, S]
-    uint8_t* out;        // [B, max_masks, img_h, img_w]
-    int dets, S, img_w, img_h, max_masks;
-    int chunks, bands, band_rows;  // 16-column chunks per row; bands per canvas; rows per band
-};
-
-__global__ void __launch_bounds__(kPasteThreads) rcnn_paste_kernel(const __grid_constant__ RcnnPasteArgs a) {
-    __shared__ float s_m[kRcnnMaxMask * kRcnnMaxMask];
-    const int item = blockIdx.x / a.bands, band = blockIdx.x - item * a.bands;
-    const int b = item / a.max_masks, k = item - b * a.max_masks;
-    const float* img = a.rows + (size_t)b * (1 + (size_t)a.dets * kRcnnRowFloats);
-    const int count = min((int)img[0], min(a.dets, a.max_masks));
+// Band `band` of canvas k of image b.  rows [B, 1 + D * 7] and masks [B, D, S, S] are the whole call's; the canvas is
+// canvases + (canvas_image * max_masks + k) * img_h * pitch (the single-size entry passes the batch's canvases and b, the
+// per-frame one the frame's own canvases and 0; computing the address here, after the barrier, keeps the single-size kernel at
+// its 64 registers).  The CTA's threads form a tx x ty grid (tcol, trow): tx over the `chunks` 16-column chunks of a row, ty
+// rows per pass, band_rows = kPastePasses * ty; threads with trow >= ty (a fixed block larger than tx * ty) only help stage
+// the mask.  Every thread of the CTA calls this, since it may synchronise.
+__device__ __forceinline__ void rcnn_paste_band(float* s_m, const float* rows, const float* masks, int b, int dets, int S,
+                                                int max_masks, int k, int band, int img_w, int img_h, uint8_t* canvases,
+                                                int canvas_image, int pitch, int tx, int ty, int tcol, int trow, int chunks,
+                                                int band_rows) {
+    const float* img = rows + (size_t)b * (1 + (size_t)dets * kRcnnRowFloats);
+    const int count = min((int)img[0], min(dets, max_masks));
     if (k >= count) return;  // slots past the image's kept rows are left untouched
     const float* row = img + 1 + (size_t)k * kRcnnRowFloats;
     int rx = 0, ry = 0, rw = 1, rh = 1;
-    const bool pasted = rcnn_mask_rect(row, a.img_w, a.img_h, rx, ry, rw, rh);
-    const int y0 = band * a.band_rows, y1 = min(y0 + a.band_rows, a.img_h);
+    const bool pasted = rcnn_mask_rect(row, img_w, img_h, rx, ry, rw, rh);
+    const int y0 = band * band_rows, y1 = min(y0 + band_rows, img_h);
     const bool touches = pasted && ry < y1 && ry + rh > y0;  // uniform over the CTA
-    const int S = a.S;
     if (touches) {
-        const float* m = a.masks + ((size_t)b * a.dets + (int)row[6]) * S * S;
-        for (int e = threadIdx.y * blockDim.x + threadIdx.x; e < S * S; e += blockDim.x * blockDim.y) s_m[e] = m[e];
+        const float* m = masks + ((size_t)b * dets + (int)row[6]) * S * S;
+        const int nthreads = blockDim.x * blockDim.y;
+        for (int e = threadIdx.y * blockDim.x + threadIdx.x; e < S * S; e += nthreads) s_m[e] = m[e];
         __syncthreads();
     }
+    if (trow >= ty) return;
     const double scale_x = (double)S / (double)rw, scale_y = (double)S / (double)rh;
-    uint8_t* plane = a.out + ((size_t)b * a.max_masks + k) * (size_t)a.img_h * a.img_w;
-    for (int c = threadIdx.x; c < a.chunks; c += blockDim.x) {
+    uint8_t* plane = canvases + ((size_t)canvas_image * max_masks + k) * (size_t)img_h * pitch;
+    for (int c = tcol; c < chunks; c += tx) {
         const int x0 = c * 16;
         int sx[16];
         float fx[16];
@@ -314,7 +325,7 @@ __global__ void __launch_bounds__(kPasteThreads) rcnn_paste_kernel(const __grid_
             fx[j] = 0.0f;
             if (touches && x0 + j >= rx && x0 + j < rx + rw) resize_tap(x0 + j - rx, scale_x, S, sx[j], fx[j]);
         }
-        for (int y = y0 + threadIdx.y; y < y1; y += blockDim.y) {
+        for (int y = y0 + trow; y < y1; y += ty) {
             uint32_t w[4] = {0u, 0u, 0u, 0u};
             if (touches && y >= ry && y < ry + rh) {
                 int sy;
@@ -334,16 +345,82 @@ __global__ void __launch_bounds__(kPasteThreads) rcnn_paste_kernel(const __grid_
                     if (v > 0.5f) w[j >> 2] |= 0xffu << (8 * (j & 3));                               // :549 threshold
                 }
             }
-            uint8_t* dst = plane + (size_t)y * a.img_w + x0;
-            if (x0 + 16 <= a.img_w && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+            uint8_t* dst = plane + (size_t)y * pitch + x0;
+            if (x0 + 16 <= img_w && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
                 *reinterpret_cast<uint4*>(dst) = make_uint4(w[0], w[1], w[2], w[3]);
-            } else {  // unaligned rows (width not a multiple of 16) and the last chunk of a row
+            } else {  // unaligned rows (odd width, pitch or base) and the last chunk of a row; pitch bytes are never written
 #pragma unroll
                 for (int j = 0; j < 16; ++j)
-                    if (x0 + j < a.img_w) dst[j] = (uint8_t)(w[j >> 2] >> (8 * (j & 3)));
+                    if (x0 + j < img_w) dst[j] = (uint8_t)(w[j >> 2] >> (8 * (j & 3)));
             }
         }
     }
+}
+
+struct RcnnPasteArgs {
+    const float* rows;   // [B, 1 + D * 7], written by rcnn_rows_kernel
+    const float* masks;  // [B, D, S, S]
+    uint8_t* out;        // [B, max_masks, img_h, img_w]
+    int dets, S, img_w, img_h, max_masks;
+    int chunks, bands, band_rows;  // 16-column chunks per row; bands per canvas; rows per band
+};
+
+// One CTA of blockDim (tx, ty) per (image, mask slot, band); the host sizes the block to the image width.
+__global__ void __launch_bounds__(kPasteThreads) rcnn_paste_kernel(const __grid_constant__ RcnnPasteArgs a) {
+    __shared__ float s_m[kRcnnMaxMask * kRcnnMaxMask];
+    const int item = blockIdx.x / a.bands, band = blockIdx.x - item * a.bands;
+    const int b = item / a.max_masks, k = item - b * a.max_masks;
+    rcnn_paste_band(s_m, a.rows, a.masks, b, a.dets, a.S, a.max_masks, k, band, a.img_w, a.img_h, a.out, b, a.img_w,
+                    blockDim.x, blockDim.y, threadIdx.x, threadIdx.y, a.chunks, a.band_rows);
+}
+
+// The per-frame entry: frames [base, base + n_images) of the call, each with its own size, pads and canvases.
+struct RcnnFrame {
+    uint8_t* canvas;          // [max_masks, img_h, pitch] u8, or nullptr (rows only)
+    int img_w, img_h, pitch;
+    int pad_l, pad_t;
+    float w_ratio, h_ratio;
+    int tx, ty;               // paste threads over a row's 16-column chunks (min(chunks, 256)) and over rows (256 / tx)
+    int bands;                // bands of kPastePasses * ty rows per canvas
+};
+struct RcnnFramesArgs {
+    int first_cta[kRcnnMaxImages];  // first CTA of each frame in the paste launch: prefix of max_masks * bands (searched
+                                    // by every CTA, so kept apart from the rest of the frame's parameters)
+    RcnnFrame f[kRcnnMaxImages];
+    const float* scores;   // [B, D]
+    const float* boxes;    // [B, D, 4]
+    const float* classes;  // [B, D]
+    const float* masks;    // [B, D, S, S]
+    float* rows;           // [B, 1 + D * 7]
+    int base, n_images, dets, S, max_masks;
+    float thresh;
+};
+
+__global__ void __launch_bounds__(128) rcnn_rows_frames_kernel(const __grid_constant__ RcnnFramesArgs a) {
+    const int j = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (j >= a.n_images) return;
+    const RcnnFrame& f = a.f[j];
+    const size_t base = (size_t)(a.base + j) * a.dets;
+    rcnn_rows_image(a.scores + base, a.boxes + base * 4, a.classes + base,
+                    a.rows + (size_t)(a.base + j) * (1 + (size_t)a.dets * kRcnnRowFloats), a.dets, a.thresh, f.pad_l, f.pad_t,
+                    f.w_ratio, f.h_ratio, lane);
+}
+
+// Flat grid over (frame, slot, band), kPasteThreads threads per CTA.  Each frame keeps the band decomposition the
+// single-size entry would launch for it (the host's tx, ty), the thread's place in it derived here from threadIdx.x.
+__global__ void __launch_bounds__(kPasteThreads) rcnn_paste_frames_kernel(const __grid_constant__ RcnnFramesArgs a) {
+    __shared__ float s_m[kRcnnMaxMask * kRcnnMaxMask];
+    int lo = 0, hi = a.n_images - 1;  // the frame owning this CTA
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (a.first_cta[mid] <= (int)blockIdx.x) lo = mid;
+        else hi = mid - 1;
+    }
+    const RcnnFrame& f = a.f[lo];
+    const int local = (int)blockIdx.x - a.first_cta[lo], k = local / f.bands, band = local - k * f.bands;
+    const int tx = f.tx, ty = f.ty;
+    rcnn_paste_band(s_m, a.rows, a.masks, a.base + lo, a.dets, a.S, a.max_masks, k, band, f.img_w, f.img_h, f.canvas, 0,
+                    f.pitch, tx, ty, (int)threadIdx.x % tx, (int)threadIdx.x / tx, (f.img_w + 15) / 16, ty * kPastePasses);
 }
 
 // YOLO segmentation post-process: process_mask (above) + draw_mask_bbox's mask selection (yolov8/src/postprocess.cpp:228-248,
@@ -825,6 +902,81 @@ TRTX_API int trtx_rcnn_postprocess_enqueue(const trtx_rcnn_post_params* p, int b
     pa.band_rows = band_rows;
     rcnn_paste_kernel<<<(unsigned)ctas, dim3(tx, ty), 0, s>>>(pa);
     return check_launch();
+}
+
+TRTX_API int trtx_rcnn_postprocess_frames_enqueue(const trtx_rcnn_post_params* p, const trtx_rcnn_image* images_host,
+                                                  int batch, const float* scores_dev, const float* boxes_dev,
+                                                  const float* classes_dev, const float* masks_dev, float* rows_dev,
+                                                  trtx_stream_t stream) {
+    if (!p || !images_host || batch <= 0 || !scores_dev || !boxes_dev || !classes_dev || !rows_dev) return TRTX_ERR_INVALID;
+    if (p->net_w <= 0 || p->net_h <= 0 || p->detections_per_im <= 0 || p->mask_size <= 0 || p->max_masks <= 0)
+        return TRTX_ERR_INVALID;
+    if (p->mask_size > kRcnnMaxMask) return TRTX_ERR_INVALID;
+    // canvases for every frame or for none; every frame is checked before the first launch, so a rejected call writes nothing
+    const bool canvases = images_host[0].masks_dev != nullptr;
+    if (canvases && !masks_dev) return TRTX_ERR_INVALID;
+    for (int i = 0; i < batch; ++i) {
+        const trtx_rcnn_image& d = images_host[i];
+        if ((d.masks_dev != nullptr) != canvases || d.img_w <= 0 || d.img_h <= 0) return TRTX_ERR_INVALID;
+        if (canvases && d.pitch < d.img_w) return TRTX_ERR_INVALID;
+    }
+    auto ty_of = [](int img_w) { return kPasteThreads / min((img_w + 15) / 16, kPasteThreads); };
+    auto bands_of = [&](int img_w, int img_h) {  // the band decomposition of trtx_rcnn_postprocess_enqueue
+        const int band_rows = ty_of(img_w) * kPastePasses;
+        return (img_h + band_rows - 1) / band_rows;
+    };
+    for (int i0 = 0; canvases && i0 < batch; i0 += kRcnnMaxImages) {
+        long long ctas = 0;
+        for (int j = 0; j < min(batch - i0, kRcnnMaxImages); ++j) {
+            const trtx_rcnn_image& d = images_host[i0 + j];
+            ctas += (long long)p->max_masks * bands_of(d.img_w, d.img_h);  // each term < 2^62: checked before the next
+            if (ctas > 0x7fffffffLL) return TRTX_ERR_UNSUPPORTED;
+        }
+    }
+    RcnnFramesArgs a;
+    a.scores = scores_dev;
+    a.boxes = boxes_dev;
+    a.classes = classes_dev;
+    a.masks = masks_dev;
+    a.rows = rows_dev;
+    a.dets = p->detections_per_im;
+    a.S = p->mask_size;
+    a.max_masks = p->max_masks;
+    a.thresh = p->score_thresh;
+    const cudaStream_t s = static_cast<cudaStream_t>(stream);
+    for (int i0 = 0; i0 < batch; i0 += kRcnnMaxImages) {
+        const int n = min(batch - i0, kRcnnMaxImages);
+        a.base = i0;
+        a.n_images = n;
+        int ctas = 0;
+        for (int j = 0; j < n; ++j) {
+            const trtx_rcnn_image& d = images_host[i0 + j];
+            RcnnFrame& f = a.f[j];
+            int pads[4];
+            trtx_rcnn_letterbox_pads(d.img_w, d.img_h, p->net_w, p->net_h, pads);
+            f.canvas = d.masks_dev;
+            f.img_w = d.img_w;
+            f.img_h = d.img_h;
+            f.pitch = d.pitch;
+            f.pad_l = pads[0];
+            f.pad_t = pads[2];
+            f.h_ratio = (float)d.img_h / (float)(p->net_h - (pads[2] + pads[3]));  // as trtx_rcnn_postprocess_enqueue
+            f.w_ratio = (float)d.img_w / (float)(p->net_w - (pads[0] + pads[1]));
+            f.tx = min((d.img_w + 15) / 16, kPasteThreads);
+            f.ty = ty_of(d.img_w);
+            f.bands = bands_of(d.img_w, d.img_h);
+            a.first_cta[j] = ctas;
+            if (canvases) ctas += p->max_masks * f.bands;
+        }
+        rcnn_rows_frames_kernel<<<(n + 3) / 4, 128, 0, s>>>(a);
+        int rc = check_launch();
+        if (rc) return rc;
+        if (!canvases) continue;
+        rcnn_paste_frames_kernel<<<(unsigned)ctas, kPasteThreads, 0, s>>>(a);
+        rc = check_launch();
+        if (rc) return rc;
+    }
+    return TRTX_OK;
 }
 
 TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const trtx_seg_image* images_host, int batch,

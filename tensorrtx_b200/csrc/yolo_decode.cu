@@ -896,6 +896,7 @@ TRTX_API size_t trtx_abi_sizeof(int which) {
         case 5: return sizeof(trtx_rcnn_post_params);
         case 6: return sizeof(trtx_seg_image);
         case 7: return sizeof(trtx_pose_obb_params);
+        case 8: return sizeof(trtx_rcnn_image);
         default: return 0;
     }
 }

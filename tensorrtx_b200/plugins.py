@@ -1127,6 +1127,55 @@ def rcnn_postprocess(scores: torch.Tensor, boxes: torch.Tensor, classes: torch.T
     return rows, canvases
 
 
+def rcnn_postprocess_frames(scores: torch.Tensor, boxes: torch.Tensor, classes: torch.Tensor, masks: torch.Tensor | None = None,
+                            *, frames: Sequence[tuple[int, int]], net_w: int, net_h: int, score_thresh: float = 0.6,
+                            max_masks: int | None = None, rows: torch.Tensor | None = None,
+                            canvases: Sequence[torch.Tensor] | None = None, stream=None):
+    """rcnn_postprocess for a batch of frames of mixed original sizes: frames[b] = (img_w, img_h) of frame b, which is
+    rescaled and pasted with its own size and pads (the same as a batch-1 rcnn_postprocess of frame b).
+    -> (rows [B, 1 + D*7] fp32, per-frame u8 canvases [max_masks, img_h, img_w], or None when masks is None).
+    `canvases[b]` may be any u8 cuda tensor [max_masks, img_h, img_w] with contiguous rows and slots (e.g. a view
+    [..., :img_w] of a pitched buffer); canvases at or past a frame's count are not written (new ones start zeroed).
+    Two launches per 64 frames."""
+    lib = L.load()
+    B = len(frames)
+    if B == 0 or scores.dim() != 2 or scores.shape[0] != B:
+        raise ValueError(f"scores must be [{B}, D] for {B} frames")
+    D = scores.shape[1]
+    S = 1 if masks is None else masks.shape[-1]
+    if tuple(boxes.shape) != (B, D, 4) or tuple(classes.shape) != (B, D) or (masks is not None and tuple(masks.shape) != (B, D, S, S)):
+        raise ValueError("expected scores [B, D], boxes [B, D, 4], classes [B, D], masks [B, D, S, S]")
+    for t in (scores, boxes, classes) + (() if masks is None else (masks,)):
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            raise ValueError("scores, boxes, classes and masks must be contiguous float32")
+    max_masks = D if max_masks is None else int(max_masks)
+    q = L.RcnnPostParams(net_w, net_h, 0, 0, D, S, max_masks, score_thresh)  # img_w / img_h: per frame below
+    if rows is None:
+        rows = torch.empty((B, 1 + D * 7), dtype=torch.float32, device=scores.device)
+    if tuple(rows.shape) != (B, 1 + D * 7) or rows.dtype != torch.float32 or not rows.is_contiguous():
+        raise ValueError(f"rows must be contiguous float32 [{B}, {1 + D * 7}]")
+    if masks is None:
+        canvases = None
+    elif canvases is None:
+        canvases = [torch.zeros((max_masks, h, w), dtype=torch.uint8, device=scores.device) for w, h in frames]
+    elif len(canvases) != B:
+        raise ValueError(f"expected {B} canvases")
+    descs = (L.RcnnImage * B)()
+    for b, (w, h) in enumerate(frames):
+        descs[b].img_w, descs[b].img_h = int(w), int(h)
+        if canvases is not None:
+            c = canvases[b]
+            if c.dtype != torch.uint8 or tuple(c.shape) != (max_masks, h, w) or c.stride(2) != 1 or \
+                    c.stride(0) != h * c.stride(1):
+                raise ValueError(f"canvas {b} must be u8 [{max_masks}, {h}, {w}] with contiguous rows and slots")
+            descs[b].masks_dev = c.data_ptr()
+            descs[b].pitch = int(c.stride(1))
+    L.check(lib.trtx_rcnn_postprocess_frames_enqueue(C.byref(q), descs, B, _ptr(scores), _ptr(boxes), _ptr(classes),
+                                                     None if masks is None else _ptr(masks), _ptr(rows), _stream(stream)),
+            "trtx_rcnn_postprocess_frames_enqueue")
+    return rows, (list(canvases) if canvases is not None else None)
+
+
 def letterbox_matrix(src_w: int, src_h: int, dst_w: int, dst_h: int):
     m = (C.c_float * 6)()
     L.load().trtx_letterbox_matrix(src_w, src_h, dst_w, dst_h, m)
