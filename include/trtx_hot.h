@@ -49,7 +49,7 @@ TRTX_API const char* trtx_version(void);
 TRTX_API int trtx_last_cuda_error(void);
 /* sizeof() of the parameter structs as THIS library was compiled, so that an FFI binding (ctypes, cgo, ...) can check its
  * mirror of the layout: which = 0 trtx_yolo_params, 1 trtx_nms_params, 2 trtx_retina_params, 3 trtx_image_desc,
- * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_seg_image, 7 trtx_pose_obb_params, 8 trtx_rcnn_image; anything else 0. */
+ * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_frame, 7 trtx_pose_obb_params, 8 trtx_frame; anything else 0. */
 TRTX_API size_t trtx_abi_sizeof(int which);
 
 /* =====================================================================================
@@ -416,14 +416,19 @@ typedef struct trtx_mask_params {
 TRTX_API int trtx_process_mask_enqueue(const trtx_mask_params* p, int batch, const float* proto_dev, const float* dets_dev,
                                        int max_rows, float* masks_dev, trtx_stream_t stream);
 
-/* The segmentation models' last host stage on the device: process_mask + scale_mask + draw_mask_bbox's mask selection
- * (yolov8/src/postprocess.cpp:228-248, yolov5/src/postprocess.cpp:148-167), for a batch of original frames of any sizes. */
-typedef struct trtx_seg_image {
-    int32_t img_w, img_h; /* the original frame: the cv::Mat img of draw_mask_bbox */
-    uint8_t* masks_dev;   /* [max_masks, img_h, pitch] u8 canvases of this image, or NULL (rows only) */
+/* One original frame of a per-frame post-process call (trtx_yolo_seg_postprocess_enqueue,
+ * trtx_rcnn_postprocess_frames_enqueue): its size and its u8 canvases.  Passed in HOST memory, copied into launch parameters. */
+typedef struct trtx_frame {
+    int32_t img_w, img_h; /* the original frame (the reference's img / w_ori, h_ori) */
+    uint8_t* masks_dev;   /* [max_masks, img_h, pitch] u8 canvases of this frame, or NULL (rows only) */
     int32_t pitch;        /* bytes per canvas row, >= img_w (any value, any base alignment) */
     int32_t reserved;
-} trtx_seg_image;
+} trtx_frame;
+typedef trtx_frame trtx_seg_image;  /* earlier names of trtx_frame, same type */
+typedef trtx_frame trtx_rcnn_image;
+
+/* The segmentation models' last host stage on the device: process_mask + scale_mask + draw_mask_bbox's mask selection
+ * (yolov8/src/postprocess.cpp:228-248, yolov5/src/postprocess.cpp:148-167), for a batch of original frames of any sizes. */
 
 /* p: as for trtx_process_mask_enqueue (row_floats >= 6; with every masks_dev NULL only variant, net_w, net_h and row_floats
  *   are read).  dets_dev [B, 1 + max_rows*row_floats]: count, rows with the box at floats 0..3 in the variant's format, conf
@@ -441,7 +446,7 @@ typedef struct trtx_seg_image {
  * call is TRTX_ERR_INVALID.  Everything is checked before the first launch (a rejected call writes nothing):
  * TRTX_ERR_INVALID for null pointers, batch / max_rows / sizes <= 0, pitch < img_w; TRTX_ERR_UNSUPPORTED for an image whose
  * scale_mask crop is empty (e.g. 1 x 5000: the reference's cv::resize throws).  Two launches per 64 images, no workspace. */
-TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const trtx_seg_image* images_host, int batch,
+TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const trtx_frame* images_host, int batch,
                                                const float* proto_dev, const float* dets_dev, int max_rows,
                                                float* rows_dev, trtx_stream_t stream);
 
@@ -522,15 +527,8 @@ TRTX_API int trtx_rcnn_postprocess_enqueue(const trtx_rcnn_post_params* p, int b
                                            const float* boxes_dev, const float* classes_dev, const float* masks_dev,
                                            float* rows_dev, uint8_t* masks_out_dev, trtx_stream_t stream);
 
-/* The same post-process for a batch of frames of mixed original sizes, one descriptor per frame. */
-typedef struct trtx_rcnn_image {
-    int32_t img_w, img_h; /* w_ori, h_ori of this frame */
-    uint8_t* masks_dev;   /* [max_masks, img_h, pitch] u8 canvases of this frame, or NULL (rows only) */
-    int32_t pitch;        /* bytes per canvas row, >= img_w; any value, any base alignment */
-    int32_t reserved;
-} trtx_rcnn_image;
-
-/* p: as for trtx_rcnn_postprocess_enqueue except img_w / img_h, which are not read.  images_host: `batch` descriptors in
+/* The same post-process for a batch of frames of mixed original sizes, one trtx_frame per frame.
+ * p: as for trtx_rcnn_postprocess_enqueue except img_w / img_h, which are not read.  images_host: `batch` descriptors in
  *   HOST memory (copied into launch parameters).  scores_dev, boxes_dev, classes_dev, masks_dev and rows_dev: the layouts of
  *   trtx_rcnn_postprocess_enqueue (the engine input net_w x net_h is one size per call).
  * Image b is rescaled with its own pads, trtx_rcnn_letterbox_pads(img_w_b, img_h_b, net_w, net_h), and its own ratios, and
@@ -542,7 +540,7 @@ typedef struct trtx_rcnn_image {
  *   rejected call writes nothing): TRTX_ERR_INVALID for null pointers, batch / sizes <= 0, pitch < img_w, mask_size > 32;
  *   TRTX_ERR_UNSUPPORTED for more than INT_MAX paste CTAs in one launch.  Two launches per 64 frames, no workspace, no
  *   atomics; can be captured in a CUDA graph. */
-TRTX_API int trtx_rcnn_postprocess_frames_enqueue(const trtx_rcnn_post_params* p, const trtx_rcnn_image* images_host,
+TRTX_API int trtx_rcnn_postprocess_frames_enqueue(const trtx_rcnn_post_params* p, const trtx_frame* images_host,
                                                   int batch, const float* scores_dev, const float* boxes_dev,
                                                   const float* classes_dev, const float* masks_dev, float* rows_dev,
                                                   trtx_stream_t stream);

@@ -6,7 +6,6 @@ TEST INFRASTRUCTURE ONLY, like oracle/oracle.py: imported by tests/, never by th
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
@@ -23,9 +22,7 @@ def load():
     if _lib is not None:
         return _lib
     _base.load()   # libtrtx_oracle.so, whose bilinear resize this library uses
-    if not LIB.exists() or LIB.stat().st_mtime < (HERE / "rcnn_post_oracle.c").stat().st_mtime:
-        subprocess.run(["make", "-C", str(HERE), "-f", "rcnn_post.mk", str(LIB)], check=True, stdout=subprocess.DEVNULL)
-    _lib = C.CDLL(str(LIB))
+    _lib = _base.build_and_open(LIB, "rcnn_post_oracle.c")
     _lib.oracle_rcnn_postprocess.restype = C.c_int
     return _lib
 

@@ -6,10 +6,11 @@ TEST INFRASTRUCTURE ONLY, like oracle/oracle.py: imported by tests/, never by th
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
+
+from . import oracle as _base
 
 HERE = Path(__file__).resolve().parent
 LIB = HERE / "librcnn_pre_oracle.so"
@@ -20,9 +21,7 @@ def load():
     global _lib
     if _lib is not None:
         return _lib
-    if not LIB.exists() or LIB.stat().st_mtime < (HERE / "rcnn_pre_oracle.c").stat().st_mtime:
-        subprocess.run(["make", "-C", str(HERE), "-f", "rcnn_pre.mk", str(LIB)], check=True, stdout=subprocess.DEVNULL)
-    _lib = C.CDLL(str(LIB))
+    _lib = _base.build_and_open(LIB, "rcnn_pre_oracle.c")
     _lib.oracle_rcnn_preprocess.restype = C.c_int
     return _lib
 

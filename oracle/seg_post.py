@@ -7,7 +7,6 @@ TEST INFRASTRUCTURE ONLY, like oracle/oracle.py: imported by tests/, never by th
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
@@ -26,9 +25,7 @@ def load():
     if _lib is not None:
         return _lib
     _base.load()   # libtrtx_oracle.so: process_mask, the bilinear resize, get_rect
-    if not LIB.exists() or LIB.stat().st_mtime < (HERE / "seg_post_oracle.c").stat().st_mtime:
-        subprocess.run(["make", "-C", str(HERE), "-f", "seg_post.mk", str(LIB)], check=True, stdout=subprocess.DEVNULL)
-    _lib = C.CDLL(str(LIB))
+    _lib = _base.build_and_open(LIB, "seg_post_oracle.c")
     _lib.oracle_seg_postprocess.restype = C.c_int
     return _lib
 

@@ -99,18 +99,17 @@ class RcnnPostParams(C.Structure):
                [("score_thresh", C.c_float)]
 
 
-class SegImage(C.Structure):
+class Frame(C.Structure):
     _fields_ = [("img_w", C.c_int32), ("img_h", C.c_int32), ("masks_dev", C.c_void_p), ("pitch", C.c_int32),
                 ("reserved", C.c_int32)]
+
+
+# the earlier names of Frame, as trtx_hot.h keeps trtx_seg_image and trtx_rcnn_image as typedefs of trtx_frame
+SegImage = RcnnImage = Frame
 
 
 class PoseObbParams(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("task", "net_w", "net_h", "row_floats", "extra_offset", "num_kpts")]
-
-
-class RcnnImage(C.Structure):
-    _fields_ = [("img_w", C.c_int32), ("img_h", C.c_int32), ("masks_dev", C.c_void_p), ("pitch", C.c_int32),
-                ("reserved", C.c_int32)]
 
 
 # TRTX_LIB: another build of the same ABI (the probe build of tools/nms_probe.py); default = the in-tree release library
@@ -155,10 +154,10 @@ SYMBOLS = {
     "trtx_scale_mask_enqueue": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "trtx_rcnn_letterbox_pads": (_i, [_i, _i, _i, _i, C.POINTER(C.c_int)]),
     "trtx_rcnn_postprocess_enqueue": (_i, [C.POINTER(RcnnPostParams), _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "trtx_rcnn_postprocess_frames_enqueue": (_i, [C.POINTER(RcnnPostParams), C.POINTER(RcnnImage), _i, _vp, _vp, _vp, _vp,
-                                                  _vp, _vp]),
+    "trtx_rcnn_postprocess_frames_enqueue": (_i, [C.POINTER(RcnnPostParams), C.POINTER(Frame), _i, _vp, _vp, _vp, _vp, _vp,
+                                                  _vp]),
     "trtx_rcnn_preprocess_enqueue": (_i, [C.POINTER(ImageDesc), _i, _i, _i, _vp, _vp]),
-    "trtx_yolo_seg_postprocess_enqueue": (_i, [C.POINTER(MaskParams), C.POINTER(SegImage), _i, _vp, _vp, _i, _vp, _vp]),
+    "trtx_yolo_seg_postprocess_enqueue": (_i, [C.POINTER(MaskParams), C.POINTER(Frame), _i, _vp, _vp, _i, _vp, _vp]),
     "trtx_get_corner": (_i, [_i, _i, _i, _i, C.POINTER(C.c_float), _f, C.POINTER(C.c_int)]),
     "trtx_yolo_pose_obb_postprocess_enqueue": (_i, [C.POINTER(PoseObbParams), C.POINTER(C.c_int32), _i, _vp, _i, _vp, _vp]),
     "trtx_yolo_decode_nms_gather_enqueue": (_i, [C.POINTER(YoloParams), C.POINTER(NmsParams), _i, _pp, _vp, _vp, _vp, _sz,
@@ -192,7 +191,7 @@ def load() -> C.CDLL:
         fn.restype = res
         fn.argtypes = args
     for which, st in enumerate((YoloParams, NmsParams, RetinaParams, ImageDesc, MaskParams, RcnnPostParams,
-                                   SegImage, PoseObbParams, RcnnImage)):
+                                   Frame, PoseObbParams, Frame)):
         if lib.trtx_abi_sizeof(which) != C.sizeof(st):
             raise TrtxError(f"{LIB_PATH} was built from a different trtx_hot.h: sizeof({st.__name__}) = "
                             f"{lib.trtx_abi_sizeof(which)} in the library, {C.sizeof(st)} in the binding (rebuild)")

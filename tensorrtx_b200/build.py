@@ -90,13 +90,9 @@ def build(force: bool = False, verbose: bool = False, probe: bool = False, defin
 
 def build_oracle() -> Path:
     """Compile the CPU oracles (test infrastructure) and, when /root/reference exists, oracle/_ref."""
-    # rcnn_post.mk / rcnn_pre.mk: the Mask R-CNN post- / pre-process oracles and their reference builds;
-    # seg_post.mk: the YOLO segmentation post-process oracle and its reference build;
-    # pose_obb.mk: the reference build of the pose / oriented-box geometry (draw_bbox_keypoints_line, draw_bbox_obb)
-    for extra in ([], ["-f", "rcnn_post.mk"], ["-f", "rcnn_pre.mk"], ["-f", "seg_post.mk"], ["-f", "pose_obb.mk"]):
-        r = subprocess.run(["make", "-C", str(ROOT / "oracle"), *extra], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-        if r.returncode != 0:
-            raise RuntimeError(f"oracle build failed:\n{r.stdout}")
+    r = subprocess.run(["make", "-C", str(ROOT / "oracle")], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    if r.returncode != 0:
+        raise RuntimeError(f"oracle build failed:\n{r.stdout}")
     return ROOT / "oracle" / "libtrtx_oracle.so"
 
 

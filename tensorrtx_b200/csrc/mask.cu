@@ -26,6 +26,7 @@ namespace trtx {
 constexpr int kMaskTile = 16;                // low-resolution cells per CTA edge
 constexpr int kMaskHalo = kMaskTile + 2;     // + one cell on each side for the bilinear taps
 constexpr int kMaxCoeffs = 64;
+constexpr int kMaxFrames = 64;               // frames per launch of the per-frame entries (launch-parameter arrays)
 
 struct MaskArgs {
     const float* proto;  // [B, nm, mh, mw]
@@ -91,6 +92,37 @@ __device__ __forceinline__ void resize_tap(int d, double scale, int src, int& s0
     f = fx;
 }
 
+// OpenCV's float bilinear blend of the taps v00 v01 (upper row) and v10 v11 (lower row): HResizeLinear with the weights
+// a0, a1, then VResizeLinear with b0, b1, every product and sum rounded to float.
+__device__ __forceinline__ float bilinear(float v00, float v01, float v10, float v11, float a0, float a1, float b0, float b1) {
+    const float h0 = __fadd_rn(__fmul_rn(v00, a0), __fmul_rn(v01, a1));  // HResizeLinear
+    const float h1 = __fadd_rn(__fmul_rn(v10, a0), __fmul_rn(v11, a1));
+    return __fadd_rn(__fmul_rn(h0, b0), __fmul_rn(h1, b1));             // VResizeLinear
+}
+
+// Bytes x0 .. x0 + 15 of a u8 canvas row (w[k]: bytes 4k .. 4k + 3): one 16-byte store when whole and aligned, else byte
+// by byte up to img_w (odd width, pitch or base; the last chunk of a row), so a pitch byte is never written.
+__device__ __forceinline__ void store_canvas_chunk(uint8_t* dst, const uint32_t w[4], int x0, int img_w) {
+    if (x0 + 16 <= img_w && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+        *reinterpret_cast<uint4*>(dst) = make_uint4(w[0], w[1], w[2], w[3]);
+    } else {
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+            if (x0 + j < img_w) dst[j] = (uint8_t)(w[j >> 2] >> (8 * (j & 3)));
+    }
+}
+
+// The frame owning this CTA in a flat grid over frames: the last j < n with first_cta[j] <= blockIdx.x (ascending, [0] = 0).
+__device__ __forceinline__ int frame_of_cta(const int* first_cta, int n) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (first_cta[mid] <= (int)blockIdx.x) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
 __global__ void __launch_bounds__(256) process_mask_kernel(const __grid_constant__ MaskArgs a) {
     __shared__ float s_m[kMaskHalo][kMaskHalo + 1];
     __shared__ float s_coeff[kMaxCoeffs];
@@ -147,6 +179,8 @@ __global__ void __launch_bounds__(256) process_mask_kernel(const __grid_constant
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
                 const int lx0 = sx[k] - cx0, lx1 = min(sx[k] + 1, a.mw - 1) - cx0;
+                // bilinear() written out: as a call, its tap loads move ahead of the arithmetic and ptxas schedules the
+                // kernel differently (0.15% slower measured on an H100 80GB HBM3, 700 W)
                 const float a0 = 1.0f - fx[k], a1 = fx[k];
                 const float h0 = __fadd_rn(__fmul_rn(s_m[ly0][lx0], a0), __fmul_rn(s_m[ly0][lx1], a1));  // HResizeLinear
                 const float h1 = __fadd_rn(__fmul_rn(s_m[ly1][lx0], a0), __fmul_rn(s_m[ly1][lx1], a1));
@@ -192,9 +226,7 @@ __global__ void __launch_bounds__(256) scale_mask_kernel(const __grid_constant__
         resize_tap(min(ox0 + k, a.img_w - 1), scale_x, a.rw, sx, fx);
         const int sx1 = min(sx + 1, a.rw - 1);
         const float a0 = 1.0f - fx, a1 = fx;
-        const float h0 = __fadd_rn(__fmul_rn(__ldg(r0 + sx), a0), __fmul_rn(__ldg(r0 + sx1), a1));
-        const float h1 = __fadd_rn(__fmul_rn(__ldg(r1 + sx), a0), __fmul_rn(__ldg(r1 + sx1), a1));
-        o[k] = __fadd_rn(__fmul_rn(h0, b0), __fmul_rn(h1, b1));
+        o[k] = bilinear(__ldg(r0 + sx), __ldg(r0 + sx1), __ldg(r1 + sx), __ldg(r1 + sx1), a0, a1, b0, b1);
     }
     float* dst = a.out + (size_t)blockIdx.z * a.img_h * a.img_w + (size_t)oy * a.img_w + ox0;
     if (ox0 + 3 < a.img_w && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
@@ -218,7 +250,6 @@ constexpr int kRcnnRowFloats = 7;      // x1, y1, x2, y2, score, class, slot
 constexpr int kRcnnMaxMask = 32;       // largest mask_size the shared-memory stage holds
 constexpr int kPasteThreads = 256;
 constexpr int kPastePasses = 8;        // row passes per CTA: band = kPastePasses * ty rows (~30 KB)
-constexpr int kRcnnMaxImages = 64;     // frames per launch of the per-frame entry (launch-parameter array)
 
 struct RcnnRowsArgs {
     const float* scores;   // [B, D]
@@ -339,20 +370,11 @@ __device__ __forceinline__ void rcnn_paste_band(float* s_m, const float* rows, c
                     if (sx[j] < 0) continue;
                     const int sx1 = min(sx[j] + 1, S - 1);
                     const float a0 = 1.0f - fx[j], a1 = fx[j];
-                    const float h0 = __fadd_rn(__fmul_rn(r0[sx[j]], a0), __fmul_rn(r0[sx1], a1));  // HResizeLinear
-                    const float h1 = __fadd_rn(__fmul_rn(r1[sx[j]], a0), __fmul_rn(r1[sx1], a1));
-                    const float v = __fadd_rn(__fmul_rn(h0, b0), __fmul_rn(h1, b1));                // VResizeLinear
-                    if (v > 0.5f) w[j >> 2] |= 0xffu << (8 * (j & 3));                               // :549 threshold
+                    const float v = bilinear(r0[sx[j]], r0[sx1], r1[sx[j]], r1[sx1], a0, a1, b0, b1);
+                    if (v > 0.5f) w[j >> 2] |= 0xffu << (8 * (j & 3));  // :549 threshold
                 }
             }
-            uint8_t* dst = plane + (size_t)y * pitch + x0;
-            if (x0 + 16 <= img_w && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
-                *reinterpret_cast<uint4*>(dst) = make_uint4(w[0], w[1], w[2], w[3]);
-            } else {  // unaligned rows (odd width, pitch or base) and the last chunk of a row; pitch bytes are never written
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                    if (x0 + j < img_w) dst[j] = (uint8_t)(w[j >> 2] >> (8 * (j & 3)));
-            }
+            store_canvas_chunk(plane + (size_t)y * pitch + x0, w, x0, img_w);
         }
     }
 }
@@ -384,9 +406,9 @@ struct RcnnFrame {
     int bands;                // bands of kPastePasses * ty rows per canvas
 };
 struct RcnnFramesArgs {
-    int first_cta[kRcnnMaxImages];  // first CTA of each frame in the paste launch: prefix of max_masks * bands (searched
-                                    // by every CTA, so kept apart from the rest of the frame's parameters)
-    RcnnFrame f[kRcnnMaxImages];
+    int first_cta[kMaxFrames];  // first CTA of each frame in the paste launch: prefix of max_masks * bands (searched by
+                                // every CTA, so kept apart from the rest of the frame's parameters)
+    RcnnFrame f[kMaxFrames];
     const float* scores;   // [B, D]
     const float* boxes;    // [B, D, 4]
     const float* classes;  // [B, D]
@@ -410,17 +432,57 @@ __global__ void __launch_bounds__(128) rcnn_rows_frames_kernel(const __grid_cons
 // single-size entry would launch for it (the host's tx, ty), the thread's place in it derived here from threadIdx.x.
 __global__ void __launch_bounds__(kPasteThreads) rcnn_paste_frames_kernel(const __grid_constant__ RcnnFramesArgs a) {
     __shared__ float s_m[kRcnnMaxMask * kRcnnMaxMask];
-    int lo = 0, hi = a.n_images - 1;  // the frame owning this CTA
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (a.first_cta[mid] <= (int)blockIdx.x) lo = mid;
-        else hi = mid - 1;
-    }
+    const int lo = frame_of_cta(a.first_cta, a.n_images);
     const RcnnFrame& f = a.f[lo];
     const int local = (int)blockIdx.x - a.first_cta[lo], k = local / f.bands, band = local - k * f.bands;
     const int tx = f.tx, ty = f.ty;
     rcnn_paste_band(s_m, a.rows, a.masks, a.base + lo, a.dets, a.S, a.max_masks, k, band, f.img_w, f.img_h, f.canvas, 0,
                     f.pitch, tx, ty, (int)threadIdx.x % tx, (int)threadIdx.x / tx, (f.img_w + 15) / 16, ty * kPastePasses);
+}
+
+// A per-frame entry's descriptors: canvases for all frames or none (-> `canvases`), sizes > 0, with canvases pitch >= img_w.
+static int check_frames(const trtx_frame* frames, int batch, bool& canvases) {
+    canvases = frames[0].masks_dev != nullptr;
+    for (int i = 0; i < batch; ++i) {
+        const trtx_frame& d = frames[i];
+        if ((d.masks_dev != nullptr) != canvases || d.img_w <= 0 || d.img_h <= 0) return TRTX_ERR_INVALID;
+        if (canvases && d.pitch < d.img_w) return TRTX_ERR_INVALID;
+    }
+    return TRTX_OK;
+}
+
+// The launch arguments of frames [i0, i0 + n) of a trtx_rcnn_postprocess_frames_enqueue call (n <= kMaxFrames): each
+// frame's pads and ratios, and the band decomposition trtx_rcnn_postprocess_enqueue would launch for it.  ctas: the paste
+// CTAs (0 without canvases); TRTX_ERR_UNSUPPORTED past INT_MAX of them.
+static int rcnn_fill_frames(const trtx_rcnn_post_params* p, const trtx_frame* frames, int i0, int n, bool canvases,
+                            RcnnFramesArgs& a, int& ctas) {
+    a.base = i0;
+    a.n_images = n;
+    long long total = 0;
+    for (int j = 0; j < n; ++j) {
+        const trtx_frame& d = frames[i0 + j];
+        RcnnFrame& f = a.f[j];
+        int pads[4];
+        trtx_rcnn_letterbox_pads(d.img_w, d.img_h, p->net_w, p->net_h, pads);
+        f.canvas = d.masks_dev;
+        f.img_w = d.img_w;
+        f.img_h = d.img_h;
+        f.pitch = d.pitch;
+        f.pad_l = pads[0];
+        f.pad_t = pads[2];
+        f.h_ratio = (float)d.img_h / (float)(p->net_h - (pads[2] + pads[3]));  // as trtx_rcnn_postprocess_enqueue
+        f.w_ratio = (float)d.img_w / (float)(p->net_w - (pads[0] + pads[1]));
+        f.tx = min((d.img_w + 15) / 16, kPasteThreads);
+        f.ty = kPasteThreads / f.tx;
+        const int band_rows = f.ty * kPastePasses;
+        f.bands = (d.img_h + band_rows - 1) / band_rows;
+        a.first_cta[j] = (int)total;
+        if (!canvases) continue;
+        total += (long long)p->max_masks * f.bands;  // each term < 2^62: checked before the next
+        if (total > 0x7fffffffLL) return TRTX_ERR_UNSUPPORTED;
+    }
+    ctas = (int)total;
+    return TRTX_OK;
 }
 
 // YOLO segmentation post-process: process_mask (above) + draw_mask_bbox's mask selection (yolov8/src/postprocess.cpp:228-248,
@@ -437,7 +499,6 @@ __global__ void __launch_bounds__(kPasteThreads) rcnn_paste_frames_kernel(const 
 //                     stores the thresholded bytes with 16-byte stores.  Neither M nor S reaches HBM; every value is the
 //                     same expression of the same inputs as in process_mask_kernel -> scale_mask_kernel, so the canvases
 //                     are bit-identical to thresholding that composition.
-constexpr int kSegMaxImages = 64;          // images per launch (launch-parameter array)
 constexpr int kSegBand = 8;                // canvas rows per CTA
 constexpr int kSegThreads = 256;
 constexpr int kSegMaxY = 2 * kSegBand;     // rows of M a band can need: two taps per canvas row
@@ -449,10 +510,10 @@ struct SegImage {
     int img_w, img_h, pitch;
     int cx, cy, cw, ch;  // scale_mask's crop of the net_w x net_h mask
     int bands;           // canvas row bands of kSegBand rows
-    int first_cta;       // first CTA of this image in the launch
 };
 struct SegArgs {
-    SegImage img[kSegMaxImages];
+    int first_cta[kMaxFrames];  // first CTA of each image in the canvas launch: prefix of max_masks * bands
+    SegImage img[kMaxFrames];
     const float* proto;  // [B, nm, mh, mw]
     const float* dets;   // [B, 1 + max_rows * row_floats]
     float* rows;         // [B, 1 + max_rows * 6]
@@ -507,14 +568,9 @@ __global__ void __launch_bounds__(kSegThreads) seg_canvas_kernel(const __grid_co
     __shared__ int s_mtap[kSegMaxY][2];   // cell slots of the two process_mask taps of y slot i
     __shared__ float s_mfy[kSegMaxY];
     __shared__ int s_ny, s_nly;
-    int lo = 0, hi = a.n_images - 1;  // the image owning this CTA
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (a.img[mid].first_cta <= (int)blockIdx.x) lo = mid;
-        else hi = mid - 1;
-    }
+    const int lo = frame_of_cta(a.first_cta, a.n_images);
     const SegImage& im = a.img[lo];
-    const int local = (int)blockIdx.x - im.first_cta, k = local / im.bands, band = local - k * im.bands;
+    const int local = (int)blockIdx.x - a.first_cta[lo], k = local / im.bands, band = local - k * im.bands;
     const int b = a.base + lo, tid = threadIdx.x;
     const float* dets = a.dets + (size_t)b * (1 + (size_t)a.max_rows * a.row_floats);
     const int count = min(max((int)dets[0], 0), min(a.max_rows, a.max_masks));
@@ -597,6 +653,8 @@ __global__ void __launch_bounds__(kSegThreads) seg_canvas_kernel(const __grid_co
             lx0 -= lxa;
             const float* c0 = s_cell + s_mtap[i][0] * nLX;
             const float* c1 = s_cell + s_mtap[i][1] * nLX;
+            // the blends and the canvas store of this kernel are bilinear() and store_canvas_chunk() written out: with the
+            // helpers ptxas schedules the kernel differently and the call measured ~1% slower (H100 80GB HBM3, 700 W)
             const float a0 = 1.0f - fx, a1 = fx, fy = s_mfy[i];
             const float b0 = 1.0f - fy, b1 = fy;
             const float h0 = __fadd_rn(__fmul_rn(c0[lx0], a0), __fmul_rn(c0[lx1], a1));  // HResizeLinear
@@ -647,7 +705,7 @@ __global__ void __launch_bounds__(kSegThreads) seg_canvas_kernel(const __grid_co
             uint8_t* dst = plane + (size_t)y * im.pitch + x0;
             if (x0 + 16 <= im.img_w && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
                 *reinterpret_cast<uint4*>(dst) = make_uint4(w[0], w[1], w[2], w[3]);
-            } else {  // unaligned rows (odd pitch or base) and the last chunk of a row
+            } else {
 #pragma unroll
                 for (int j = 0; j < 16; ++j)
                     if (x0 + j < im.img_w) dst[j] = (uint8_t)(w[j >> 2] >> (8 * (j & 3)));
@@ -667,6 +725,48 @@ static void seg_caps(double s, int& y_cap, int& ly_cap) {
     if (ly_cap > 2 * y_cap) ly_cap = 2 * y_cap;
 }
 
+// The launch arguments of images [i0, i0 + n) of a trtx_yolo_seg_postprocess_enqueue call (n <= kMaxFrames): sizes and
+// canvases, and with canvases each image's scale_mask crop, the launch's shared-memory caps, its canvas CTAs `ctas` and
+// dynamic shared memory `smem` (both 0 without canvases).  TRTX_ERR_UNSUPPORTED for an empty crop (the reference's
+// cv::resize throws) or more than INT_MAX CTAs.
+static int seg_fill_frames(const trtx_mask_params* p, const trtx_frame* frames, int i0, int n, bool canvases, SegArgs& a,
+                           int& ctas, size_t& smem) {
+    a.base = i0;
+    a.n_images = n;
+    a.y_cap = a.ly_cap = a.x_cap = 1;
+    long long total = 0;
+    for (int j = 0; j < n; ++j) {
+        const trtx_frame& d = frames[i0 + j];
+        SegImage& im = a.img[j];
+        im.canvas = d.masks_dev;
+        im.img_w = d.img_w;
+        im.img_h = d.img_h;
+        im.pitch = d.pitch;
+        im.bands = (d.img_h + kSegBand - 1) / kSegBand;
+        a.first_cta[j] = (int)total;
+        if (!canvases) continue;
+        int r[4];
+        trtx_scale_mask_rect(p->net_w, p->net_h, d.img_w, d.img_h, r);
+        if (r[2] <= 0 || r[3] <= 0 || r[0] < 0 || r[1] < 0 || r[0] + r[2] > p->net_w || r[1] + r[3] > p->net_h)
+            return TRTX_ERR_UNSUPPORTED;
+        im.cx = r[0];
+        im.cy = r[1];
+        im.cw = r[2];
+        im.ch = r[3];
+        int yc, lyc;
+        seg_caps((double)r[3] / (double)d.img_h, yc, lyc);
+        a.y_cap = max(a.y_cap, yc);
+        a.ly_cap = max(a.ly_cap, lyc);
+        a.x_cap = max(a.x_cap, r[2]);
+        total += (long long)p->max_masks * im.bands;  // each term < 2^59: checked before the next
+        if (total > 0x7fffffffLL) return TRTX_ERR_UNSUPPORTED;
+    }
+    a.lx_cap = min(p->mask_w, a.x_cap / 4 + 4);
+    ctas = (int)total;
+    smem = canvases ? ((size_t)a.y_cap * a.x_cap + (size_t)a.ly_cap * a.lx_cap) * sizeof(float) : 0;
+    return TRTX_OK;
+}
+
 // Pose and oriented-box post-process: the per-detection geometry of draw_bbox_keypoints_line (get_rect_adapt_landmark,
 // yolov8/src/postprocess.cpp:173-205) and draw_bbox_obb (get_corner, :474-507), which the reference runs on one host core
 // after a D2H copy.  One CTA of kPoseObbThreads per frame, one launch per <= 64 frames, no workspace, no atomics:
@@ -675,13 +775,12 @@ static void seg_caps(double s, int& y_cap, int& ly_cap) {
 //   thread computes the rectangle (yolo_get_rect) or the four corners (yolo_get_corner) into shared memory; then the whole
 //   CTA writes the pass's kept rows as one contiguous run of floats (coalesced), mapping each keypoint coordinate with
 //   yolo_map_landmark on the way.  Rows past the kept count are zeroed.
-constexpr int kPoseObbMaxImages = 64;  // frames per launch (launch-parameter array)
 constexpr int kPoseObbThreads = 256;   // rows per pass
 constexpr int kPoseObbWarps = kPoseObbThreads / kWarp;
 constexpr int kPoseMaxKpts = 64;
 
 struct PoseObbArgs {
-    int img_w[kPoseObbMaxImages], img_h[kPoseObbMaxImages];
+    int img_w[kMaxFrames], img_h[kMaxFrames];
     const float* dets;  // [B, 1 + max_rows * row_floats]
     float* rows;        // [B, 1 + max_rows * out_floats]
     int base;           // frames [base, base + gridDim.x) of the call
@@ -904,7 +1003,7 @@ TRTX_API int trtx_rcnn_postprocess_enqueue(const trtx_rcnn_post_params* p, int b
     return check_launch();
 }
 
-TRTX_API int trtx_rcnn_postprocess_frames_enqueue(const trtx_rcnn_post_params* p, const trtx_rcnn_image* images_host,
+TRTX_API int trtx_rcnn_postprocess_frames_enqueue(const trtx_rcnn_post_params* p, const trtx_frame* images_host,
                                                   int batch, const float* scores_dev, const float* boxes_dev,
                                                   const float* classes_dev, const float* masks_dev, float* rows_dev,
                                                   trtx_stream_t stream) {
@@ -912,27 +1011,10 @@ TRTX_API int trtx_rcnn_postprocess_frames_enqueue(const trtx_rcnn_post_params* p
     if (p->net_w <= 0 || p->net_h <= 0 || p->detections_per_im <= 0 || p->mask_size <= 0 || p->max_masks <= 0)
         return TRTX_ERR_INVALID;
     if (p->mask_size > kRcnnMaxMask) return TRTX_ERR_INVALID;
-    // canvases for every frame or for none; every frame is checked before the first launch, so a rejected call writes nothing
-    const bool canvases = images_host[0].masks_dev != nullptr;
+    bool canvases;
+    int rc = check_frames(images_host, batch, canvases);
+    if (rc) return rc;
     if (canvases && !masks_dev) return TRTX_ERR_INVALID;
-    for (int i = 0; i < batch; ++i) {
-        const trtx_rcnn_image& d = images_host[i];
-        if ((d.masks_dev != nullptr) != canvases || d.img_w <= 0 || d.img_h <= 0) return TRTX_ERR_INVALID;
-        if (canvases && d.pitch < d.img_w) return TRTX_ERR_INVALID;
-    }
-    auto ty_of = [](int img_w) { return kPasteThreads / min((img_w + 15) / 16, kPasteThreads); };
-    auto bands_of = [&](int img_w, int img_h) {  // the band decomposition of trtx_rcnn_postprocess_enqueue
-        const int band_rows = ty_of(img_w) * kPastePasses;
-        return (img_h + band_rows - 1) / band_rows;
-    };
-    for (int i0 = 0; canvases && i0 < batch; i0 += kRcnnMaxImages) {
-        long long ctas = 0;
-        for (int j = 0; j < min(batch - i0, kRcnnMaxImages); ++j) {
-            const trtx_rcnn_image& d = images_host[i0 + j];
-            ctas += (long long)p->max_masks * bands_of(d.img_w, d.img_h);  // each term < 2^62: checked before the next
-            if (ctas > 0x7fffffffLL) return TRTX_ERR_UNSUPPORTED;
-        }
-    }
     RcnnFramesArgs a;
     a.scores = scores_dev;
     a.boxes = boxes_dev;
@@ -943,55 +1025,32 @@ TRTX_API int trtx_rcnn_postprocess_frames_enqueue(const trtx_rcnn_post_params* p
     a.S = p->mask_size;
     a.max_masks = p->max_masks;
     a.thresh = p->score_thresh;
+    // every frame is checked before the first launch, so a rejected call writes nothing
+    int ctas;
+    for (int i0 = 0; i0 < batch; i0 += kMaxFrames)
+        if ((rc = rcnn_fill_frames(p, images_host, i0, min(batch - i0, kMaxFrames), canvases, a, ctas))) return rc;
     const cudaStream_t s = static_cast<cudaStream_t>(stream);
-    for (int i0 = 0; i0 < batch; i0 += kRcnnMaxImages) {
-        const int n = min(batch - i0, kRcnnMaxImages);
-        a.base = i0;
-        a.n_images = n;
-        int ctas = 0;
-        for (int j = 0; j < n; ++j) {
-            const trtx_rcnn_image& d = images_host[i0 + j];
-            RcnnFrame& f = a.f[j];
-            int pads[4];
-            trtx_rcnn_letterbox_pads(d.img_w, d.img_h, p->net_w, p->net_h, pads);
-            f.canvas = d.masks_dev;
-            f.img_w = d.img_w;
-            f.img_h = d.img_h;
-            f.pitch = d.pitch;
-            f.pad_l = pads[0];
-            f.pad_t = pads[2];
-            f.h_ratio = (float)d.img_h / (float)(p->net_h - (pads[2] + pads[3]));  // as trtx_rcnn_postprocess_enqueue
-            f.w_ratio = (float)d.img_w / (float)(p->net_w - (pads[0] + pads[1]));
-            f.tx = min((d.img_w + 15) / 16, kPasteThreads);
-            f.ty = ty_of(d.img_w);
-            f.bands = bands_of(d.img_w, d.img_h);
-            a.first_cta[j] = ctas;
-            if (canvases) ctas += p->max_masks * f.bands;
-        }
+    for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {
+        const int n = min(batch - i0, kMaxFrames);
+        rcnn_fill_frames(p, images_host, i0, n, canvases, a, ctas);
         rcnn_rows_frames_kernel<<<(n + 3) / 4, 128, 0, s>>>(a);
-        int rc = check_launch();
-        if (rc) return rc;
+        if ((rc = check_launch())) return rc;
         if (!canvases) continue;
         rcnn_paste_frames_kernel<<<(unsigned)ctas, kPasteThreads, 0, s>>>(a);
-        rc = check_launch();
-        if (rc) return rc;
+        if ((rc = check_launch())) return rc;
     }
     return TRTX_OK;
 }
 
-TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const trtx_seg_image* images_host, int batch,
+TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const trtx_frame* images_host, int batch,
                                                const float* proto_dev, const float* dets_dev, int max_rows,
                                                float* rows_dev, trtx_stream_t stream) {
     if (!p || !images_host || batch <= 0 || !dets_dev || !rows_dev || max_rows <= 0) return TRTX_ERR_INVALID;
     if (p->variant != TRTX_YOLO_V8 && p->variant != TRTX_YOLO_V5) return TRTX_ERR_INVALID;
     if (p->net_w <= 0 || p->net_h <= 0 || p->row_floats < kSegRowFloats) return TRTX_ERR_INVALID;
-    // canvases for every image or for none
-    const bool masks = images_host[0].masks_dev != nullptr;
-    for (int i = 0; i < batch; ++i) {
-        const trtx_seg_image& d = images_host[i];
-        if ((d.masks_dev != nullptr) != masks || d.img_w <= 0 || d.img_h <= 0) return TRTX_ERR_INVALID;
-        if (masks && d.pitch < d.img_w) return TRTX_ERR_INVALID;
-    }
+    bool masks;
+    int rc = check_frames(images_host, batch, masks);
+    if (rc) return rc;
     if (masks) {  // trtx_process_mask_enqueue's checks
         if (!proto_dev) return TRTX_ERR_INVALID;
         if (p->num_coeffs <= 0 || p->num_coeffs > kMaxCoeffs || p->max_masks <= 0) return TRTX_ERR_INVALID;
@@ -999,37 +1058,6 @@ TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const 
         if (p->mask_w <= 0 || p->mask_h <= 0) return TRTX_ERR_INVALID;
         if (p->net_w != 4 * p->mask_w || p->net_h != 4 * p->mask_h) return TRTX_ERR_UNSUPPORTED;
     }
-    // every image is checked before the first launch, so that a rejected call writes nothing
-    size_t smem_max = 0;
-    for (int i0 = 0; masks && i0 < batch; i0 += kSegMaxImages) {
-        const int n = min(batch - i0, kSegMaxImages);
-        long long ctas = 0;
-        int y_cap = 1, ly_cap = 1, x_cap = 1;
-        for (int j = 0; j < n; ++j) {
-            const trtx_seg_image& d = images_host[i0 + j];
-            int r[4];
-            trtx_scale_mask_rect(p->net_w, p->net_h, d.img_w, d.img_h, r);
-            // an empty crop makes the reference's cv::resize throw
-            if (r[2] <= 0 || r[3] <= 0 || r[0] < 0 || r[1] < 0 || r[0] + r[2] > p->net_w || r[1] + r[3] > p->net_h)
-                return TRTX_ERR_UNSUPPORTED;
-            int yc, lyc;
-            seg_caps((double)r[3] / (double)d.img_h, yc, lyc);
-            y_cap = max(y_cap, yc);
-            ly_cap = max(ly_cap, lyc);
-            x_cap = max(x_cap, r[2]);
-            ctas += (long long)p->max_masks * ((d.img_h + kSegBand - 1) / kSegBand);
-        }
-        if (ctas > 0x7fffffffLL) return TRTX_ERR_UNSUPPORTED;
-        const int lx_cap = min(p->mask_w, x_cap / 4 + 4);
-        const size_t smem = ((size_t)y_cap * x_cap + (size_t)ly_cap * lx_cap) * sizeof(float);
-        smem_max = smem > smem_max ? smem : smem_max;
-    }
-    if (smem_max > 48 * 1024 &&
-        cudaFuncSetAttribute(seg_canvas_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) != cudaSuccess) {
-        g_last_cuda_error = (int)cudaGetLastError();
-        return TRTX_ERR_CUDA;
-    }
-    const cudaStream_t st = static_cast<cudaStream_t>(stream);
     SegArgs a;
     a.proto = proto_dev;
     a.dets = dets_dev;
@@ -1044,46 +1072,27 @@ TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const 
     a.net_w = p->net_w;
     a.net_h = p->net_h;
     a.max_masks = p->max_masks;
-    for (int i0 = 0; i0 < batch; i0 += kSegMaxImages) {
-        const int n = min(batch - i0, kSegMaxImages);
-        a.base = i0;
-        a.n_images = n;
-        int ctas = 0;
-        a.y_cap = a.ly_cap = a.x_cap = 1;
-        for (int j = 0; j < n; ++j) {
-            const trtx_seg_image& d = images_host[i0 + j];
-            SegImage& im = a.img[j];
-            im.canvas = d.masks_dev;
-            im.img_w = d.img_w;
-            im.img_h = d.img_h;
-            im.pitch = d.pitch;
-            im.bands = (d.img_h + kSegBand - 1) / kSegBand;
-            im.first_cta = ctas;
-            if (!masks) continue;
-            int r[4];
-            trtx_scale_mask_rect(p->net_w, p->net_h, d.img_w, d.img_h, r);
-            im.cx = r[0];
-            im.cy = r[1];
-            im.cw = r[2];
-            im.ch = r[3];
-            int yc, lyc;
-            seg_caps((double)r[3] / (double)d.img_h, yc, lyc);
-            a.y_cap = max(a.y_cap, yc);
-            a.ly_cap = max(a.ly_cap, lyc);
-            a.x_cap = max(a.x_cap, r[2]);
-            ctas += p->max_masks * im.bands;
-        }
-        a.lx_cap = min(p->mask_w, a.x_cap / 4 + 4);
+    // every image is checked before the first launch, so that a rejected call writes nothing
+    int ctas;
+    size_t smem, smem_max = 0;
+    for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {
+        if ((rc = seg_fill_frames(p, images_host, i0, min(batch - i0, kMaxFrames), masks, a, ctas, smem))) return rc;
+        smem_max = max(smem_max, smem);
+    }
+    if (smem_max > 48 * 1024 &&
+        cudaFuncSetAttribute(seg_canvas_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) != cudaSuccess) {
+        g_last_cuda_error = (int)cudaGetLastError();
+        return TRTX_ERR_CUDA;
+    }
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {
+        const int n = min(batch - i0, kMaxFrames);
+        seg_fill_frames(p, images_host, i0, n, masks, a, ctas, smem);
         seg_rows_kernel<<<(n + 3) / 4, 128, 0, st>>>(a);
-        int rc = check_launch();
-        if (rc || !masks) {
-            if (rc) return rc;
-            continue;
-        }
-        const size_t smem = ((size_t)a.y_cap * a.x_cap + (size_t)a.ly_cap * a.lx_cap) * sizeof(float);
+        if ((rc = check_launch())) return rc;
+        if (!masks) continue;
         seg_canvas_kernel<<<(unsigned)ctas, kSegThreads, smem, st>>>(a);
-        rc = check_launch();
-        if (rc) return rc;
+        if ((rc = check_launch())) return rc;
     }
     return TRTX_OK;
 }
@@ -1113,8 +1122,8 @@ TRTX_API int trtx_yolo_pose_obb_postprocess_enqueue(const trtx_pose_obb_params* 
     a.out_floats = pose ? 6 + 3 * p->num_kpts : 10;
     a.max_rows = max_rows;
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
-    for (int i0 = 0; i0 < batch; i0 += kPoseObbMaxImages) {
-        const int n = min(batch - i0, kPoseObbMaxImages);
+    for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {
+        const int n = min(batch - i0, kMaxFrames);
         a.base = i0;
         for (int j = 0; j < n; ++j) {
             a.img_w[j] = frame_wh_host[2 * (i0 + j)];

@@ -894,9 +894,9 @@ TRTX_API size_t trtx_abi_sizeof(int which) {
         case 3: return sizeof(trtx_image_desc);
         case 4: return sizeof(trtx_mask_params);
         case 5: return sizeof(trtx_rcnn_post_params);
-        case 6: return sizeof(trtx_seg_image);
+        case 6: return sizeof(trtx_frame);
         case 7: return sizeof(trtx_pose_obb_params);
-        case 8: return sizeof(trtx_rcnn_image);
+        case 8: return sizeof(trtx_frame);
         default: return 0;
     }
 }

@@ -594,6 +594,31 @@ def process_mask(proto: torch.Tensor, dets: torch.Tensor, max_rows: int, row_flo
     return out
 
 
+def _frames(sizes: Sequence[tuple[int, int]], canvases: Sequence[torch.Tensor] | None, max_masks: int, device,
+            with_canvases: bool):
+    """trtx_frame descriptors for frames of sizes[b] = (img_w, img_h) and, with_canvases, their u8 canvases
+    [max_masks, img_h, img_w]: the caller's `canvases` (any u8 tensors with contiguous rows and slots, e.g. views
+    [..., :img_w] of pitched buffers) or new zeroed ones.  -> (descriptors, list of canvases or None)"""
+    B = len(sizes)
+    if not with_canvases:
+        canvases = None
+    elif canvases is None:
+        canvases = [torch.zeros((max_masks, h, w), dtype=torch.uint8, device=device) for w, h in sizes]
+    elif len(canvases) != B:
+        raise ValueError(f"expected {B} canvases")
+    descs = (L.Frame * B)()
+    for b, (w, h) in enumerate(sizes):
+        descs[b].img_w, descs[b].img_h = int(w), int(h)
+        if canvases is not None:
+            c = canvases[b]
+            if c.dtype != torch.uint8 or tuple(c.shape) != (max_masks, h, w) or c.stride(2) != 1 or \
+                    c.stride(0) != h * c.stride(1):
+                raise ValueError(f"canvas {b} must be u8 [{max_masks}, {h}, {w}] with contiguous rows and slots")
+            descs[b].masks_dev = c.data_ptr()
+            descs[b].pitch = int(c.stride(1))
+    return descs, (list(canvases) if canvases is not None else None)
+
+
 def yolo_seg_postprocess(proto: torch.Tensor | None, dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]], *,
                          variant: int, max_rows: int, row_floats: int = 39, coeff_offset: int = 7, max_masks: int,
                          net_w: int = 640, net_h: int = 640, masks: bool = True, rows_out: torch.Tensor | None = None,
@@ -615,22 +640,11 @@ def yolo_seg_postprocess(proto: torch.Tensor | None, dets: torch.Tensor, image_s
     q = L.MaskParams(variant, net_w, net_h, mw, mh, nm, row_floats, coeff_offset, max_masks)
     if rows_out is None:
         rows_out = torch.empty((B, 1 + max_rows * 6), dtype=torch.float32, device=dets.device)
-    if masks and canvases_out is None:
-        canvases_out = [torch.zeros((max_masks, h, w), dtype=torch.uint8, device=dets.device) for w, h in image_sizes]
-    descs = (L.SegImage * B)()
-    for b, (w, h) in enumerate(image_sizes):
-        descs[b].img_w, descs[b].img_h = int(w), int(h)
-        if masks:
-            c = canvases_out[b]
-            if c.dtype != torch.uint8 or tuple(c.shape) != (max_masks, h, w) or c.stride(2) != 1 or \
-                    c.stride(0) != h * c.stride(1):
-                raise ValueError(f"canvas {b} must be u8 [{max_masks}, {h}, {w}] with contiguous rows and slots")
-            descs[b].masks_dev = c.data_ptr()
-            descs[b].pitch = int(c.stride(1))
+    descs, canvases_out = _frames(image_sizes, canvases_out, max_masks, dets.device, masks)
     L.check(lib.trtx_yolo_seg_postprocess_enqueue(C.byref(q), descs, B, None if proto is None else _ptr(proto), _ptr(dets),
                                                   max_rows, _ptr(rows_out), _stream(stream)),
             "trtx_yolo_seg_postprocess_enqueue")
-    return rows_out, (list(canvases_out) if masks else None)
+    return rows_out, canvases_out
 
 
 def yolo_pose_obb_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]], *, task: int, max_rows: int,
@@ -1154,26 +1168,11 @@ def rcnn_postprocess_frames(scores: torch.Tensor, boxes: torch.Tensor, classes: 
         rows = torch.empty((B, 1 + D * 7), dtype=torch.float32, device=scores.device)
     if tuple(rows.shape) != (B, 1 + D * 7) or rows.dtype != torch.float32 or not rows.is_contiguous():
         raise ValueError(f"rows must be contiguous float32 [{B}, {1 + D * 7}]")
-    if masks is None:
-        canvases = None
-    elif canvases is None:
-        canvases = [torch.zeros((max_masks, h, w), dtype=torch.uint8, device=scores.device) for w, h in frames]
-    elif len(canvases) != B:
-        raise ValueError(f"expected {B} canvases")
-    descs = (L.RcnnImage * B)()
-    for b, (w, h) in enumerate(frames):
-        descs[b].img_w, descs[b].img_h = int(w), int(h)
-        if canvases is not None:
-            c = canvases[b]
-            if c.dtype != torch.uint8 or tuple(c.shape) != (max_masks, h, w) or c.stride(2) != 1 or \
-                    c.stride(0) != h * c.stride(1):
-                raise ValueError(f"canvas {b} must be u8 [{max_masks}, {h}, {w}] with contiguous rows and slots")
-            descs[b].masks_dev = c.data_ptr()
-            descs[b].pitch = int(c.stride(1))
+    descs, canvases = _frames(frames, canvases, max_masks, scores.device, masks is not None)
     L.check(lib.trtx_rcnn_postprocess_frames_enqueue(C.byref(q), descs, B, _ptr(scores), _ptr(boxes), _ptr(classes),
                                                      None if masks is None else _ptr(masks), _ptr(rows), _stream(stream)),
             "trtx_rcnn_postprocess_frames_enqueue")
-    return rows, (list(canvases) if canvases is not None else None)
+    return rows, canvases
 
 
 def letterbox_matrix(src_w: int, src_h: int, dst_w: int, dst_h: int):

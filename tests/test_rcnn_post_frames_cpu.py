@@ -1,5 +1,5 @@
 """Mask R-CNN post-process for frames of mixed sizes (trtx_rcnn_postprocess_frames_enqueue) without a GPU: every argument
-check returns its error before anything is launched, and the ctypes mirror of trtx_rcnn_image has the C layout."""
+check returns its error before anything is launched, and the ctypes mirror of trtx_frame has the C layout."""
 import ctypes as C
 import subprocess
 from pathlib import Path
@@ -16,7 +16,7 @@ PTRS = (16, 32, 48, 64, 80)
 
 
 def _frames(sizes, canvases=True, pitch_extra=0):
-    d = (L.RcnnImage * len(sizes))()
+    d = (L.Frame * len(sizes))()
     for i, (w, h) in enumerate(sizes):
         d[i].img_w, d[i].img_h = w, h
         d[i].masks_dev = (4096 * (i + 1)) if canvases else None
@@ -107,16 +107,19 @@ def test_python_wrapper_validates_shapes():
 
 
 def test_rcnn_image_layout_equals_the_mirror(tmp_path):
-    assert L.load().trtx_abi_sizeof(8) == C.sizeof(L.RcnnImage)
+    """trtx_frame has the layout of the ctypes mirror, and the earlier names trtx_seg_image and trtx_rcnn_image are the
+    same type (a pointer to one assigns to a pointer to the other under -Werror)."""
+    assert L.load().trtx_abi_sizeof(8) == L.load().trtx_abi_sizeof(6) == C.sizeof(L.Frame) == 24
     src = tmp_path / "layout.c"
     src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "trtx_hot.h"\nint main(void) {\n'
-                   '  printf("%zu %zu %zu %zu %zu %zu\\n", sizeof(trtx_rcnn_image), offsetof(trtx_rcnn_image, img_w),\n'
-                   '         offsetof(trtx_rcnn_image, img_h), offsetof(trtx_rcnn_image, masks_dev),\n'
-                   '         offsetof(trtx_rcnn_image, pitch), offsetof(trtx_rcnn_image, reserved));\n  return 0;\n}\n')
+                   '  trtx_rcnn_image r = {0};\n  trtx_seg_image* s = &r;\n  trtx_frame* f = s;\n  (void)f;\n'
+                   '  printf("%zu %zu %zu %zu %zu %zu\\n", sizeof(trtx_frame), offsetof(trtx_frame, img_w),\n'
+                   '         offsetof(trtx_frame, img_h), offsetof(trtx_frame, masks_dev),\n'
+                   '         offsetof(trtx_frame, pitch), offsetof(trtx_frame, reserved));\n  return 0;\n}\n')
     exe = tmp_path / "layout"
     r = subprocess.run(["gcc", "-std=c99", "-Wall", "-Werror", "-I", str(ROOT / "include"), str(src), "-o", str(exe)],
                        capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
     got = [int(v) for v in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
-    want = [C.sizeof(L.RcnnImage)] + [getattr(L.RcnnImage, n).offset for n in ("img_w", "img_h", "masks_dev", "pitch", "reserved")]
+    want = [C.sizeof(L.Frame)] + [getattr(L.Frame, n).offset for n in ("img_w", "img_h", "masks_dev", "pitch", "reserved")]
     assert got == want

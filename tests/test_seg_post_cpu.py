@@ -183,7 +183,7 @@ def _fake(n):
 def test_argument_validation():
     """Rejected before anything is launched (the device pointers here are never dereferenced)."""
     lib = L.load()
-    assert lib.trtx_abi_sizeof(6) == C.sizeof(L.SegImage) == 24
+    assert lib.trtx_abi_sizeof(6) == C.sizeof(L.Frame) == 24
 
     def call(p=None, imgs=None, batch=1, proto=_fake(1), dets=_fake(2), max_rows=10, rows=_fake(3), **kw):
         q = L.MaskParams(0, 640, 640, 160, 160, 32, 39, 7, 20)
@@ -191,7 +191,7 @@ def test_argument_validation():
             setattr(q, k, v)
         if imgs is None:
             imgs = [(1920, 1080, _fake(4).value, 1920)]
-        arr = (L.SegImage * max(len(imgs), 1))()
+        arr = (L.Frame * max(len(imgs), 1))()
         for i, (w, h, m, pitch) in enumerate(imgs):
             arr[i].img_w, arr[i].img_h, arr[i].masks_dev, arr[i].pitch = w, h, m, pitch
         return lib.trtx_yolo_seg_postprocess_enqueue(C.byref(q) if p is None else p, arr, batch, proto, dets, max_rows,
@@ -219,3 +219,9 @@ def test_argument_validation():
     assert call(imgs=[(5000, 1, _fake(4).value, 5000)]) == UNS
     # rows only: the mask fields are not read, and any frame size works
     assert call(imgs=[(1, 5000, None, 0)], proto=None, num_coeffs=0, mask_w=0, dets=None) == INV
+    # the Python wrapper: one canvas per frame
+    import torch
+    for n in (1, 3):
+        with pytest.raises(ValueError, match="expected 2 canvases"):
+            P.yolo_seg_postprocess(torch.zeros((2, 1, 160, 160)), torch.zeros((2, 1 + 39)), [(64, 48), (48, 64)], variant=0,
+                                   max_rows=1, max_masks=1, canvases_out=[torch.zeros((1, 48, 64), dtype=torch.uint8)] * n)

@@ -1,5 +1,5 @@
 """Write tests/golden/ref_pose_obb_host.npz: what the reference's own draw_bbox_obb and draw_bbox_keypoints_line
-(oracle/_ref/libref_pose_obb_host.so, built by oracle/pose_obb.mk where the reference tree is present) produce for the cases
+(oracle/_ref/libref_pose_obb_host.so, built by oracle/Makefile where the reference tree is present) produce for the cases
 of tests/test_pose_obb_post_cpu.py, as one sha256 per frame size (corners of the boxes whose get_rect is defined; rectangles
 and mapped keypoints), so that machines without the reference still pin trtx_get_corner and trtx_get_rect_adapt_landmark."""
 import sys

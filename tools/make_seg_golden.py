@@ -1,5 +1,5 @@
 """Write tests/golden/ref_seg_post_host.npz: what the reference's own draw_mask_bbox (oracle/_ref/libref_seg_host.so, built by
-oracle/seg_post.mk where the reference tree is present) selects for the cases of tests/test_seg_post_cpu.py, as a sha256 of
+oracle/Makefile where the reference tree is present) selects for the cases of tests/test_seg_post_cpu.py, as a sha256 of
 each packed selection and its pixel count, so that machines without the reference still pin the oracle to it."""
 import hashlib
 import sys
