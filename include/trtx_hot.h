@@ -49,7 +49,8 @@ TRTX_API const char* trtx_version(void);
 TRTX_API int trtx_last_cuda_error(void);
 /* sizeof() of the parameter structs as THIS library was compiled, so that an FFI binding (ctypes, cgo, ...) can check its
  * mirror of the layout: which = 0 trtx_yolo_params, 1 trtx_nms_params, 2 trtx_retina_params, 3 trtx_image_desc,
- * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_frame, 7 trtx_pose_obb_params, 8 trtx_frame; anything else 0. */
+ * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_frame, 7 trtx_pose_obb_params, 8 trtx_frame,
+ * 9 trtx_face_post_params; anything else 0. */
 TRTX_API size_t trtx_abi_sizeof(int which);
 
 /* =====================================================================================
@@ -342,8 +343,11 @@ TRTX_API int trtx_get_rect_adapt_landmark(int net_w, int net_h, int img_w, int i
  * x86-64 after its clamp; a box whose get_rect is undefined gets four (0, 0) corners.  The reference's debug prints are
  * not reproduced.  Host function; the device form is trtx_yolo_pose_obb_postprocess_enqueue. */
 TRTX_API int trtx_get_corner(int net_w, int net_h, int img_w, int img_h, const float cxcywh[4], float angle, int corners[8]);
-/* RetinaFace's own get_rect_adapt_landmark (retinaface/common.hpp:65-89): 5 landmarks as x, y pairs, modified in place; the box
- * corners are truncated to int and not clamped; rect = {x, y, w, h} in the original image. */
+/* RetinaFace's own get_rect_adapt_landmark (retinaface/common.hpp:65-89; retinafaceAntiCov's copy is the same statements with
+ * input_w = input_h = 640): 5 landmarks as x, y pairs, modified in place; the box corners are truncated to int and not
+ * clamped; rect = {x, y, w, h} in the original image.  Defined where the reference is not, as the compiled x86-64 reference
+ * behaves: a corner that is NaN, infinite or outside [-2^31, 2^31) converts to INT_MIN, and w = r - l, h = b - t wrap
+ * modulo 2^32.  Host function; the device form is trtx_retina_postprocess_enqueue. */
 TRTX_API int trtx_retina_get_rect_adapt_landmark(int input_w, int input_h, int img_w, int img_h, const float bbox[4], float lmk[10],
                                                  int rect[4]);
 /* process_decode_ptr_host (yolov8/src/postprocess.cpp:131-147): rows of a compact buffer [1 + K*bbox_element] (the output
@@ -454,15 +458,17 @@ TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const 
  * (yolov8/src/postprocess.cpp:173-205) and draw_bbox_obb's get_corner (:474-507; yolo11/src/postprocess.cpp:504-537), for a
  * batch of original frames of any sizes.  The drawing itself stays with the caller. */
 enum {
-    TRTX_TASK_POSE = 1, /* keypoints: rectangle + num_kpts (x, y, conf) mapped to the frame */
-    TRTX_TASK_OBB = 2,  /* oriented boxes: four corners in the frame */
+    TRTX_TASK_POSE = 1,         /* keypoints: rectangle + num_kpts (x, y, conf) mapped to the frame */
+    TRTX_TASK_OBB = 2,          /* oriented boxes: four corners in the frame */
+    TRTX_TASK_OBB_NMS_FREE = 3, /* the same corners from yolo26-obb's NMS-free plugin rows, which have no keep column */
 };
 typedef struct trtx_pose_obb_params {
     int32_t task;         /* TRTX_TASK_* */
-    int32_t net_w, net_h; /* network input: kInputW / kInputH (640), or kObbInputW / kObbInputH (1024) of yolo11-obb */
+    int32_t net_w, net_h; /* network input: kInputW / kInputH (640), or kObbInputW / kObbInputH (1024) of yolo11 / yolo26-obb */
     int32_t row_floats;   /* floats per row of dets_dev, >= 7 (box4, conf, class, keep, extras...) */
-    int32_t extra_offset; /* POSE: first keypoint float in a row; OBB: the angle (radians) */
-    int32_t num_kpts;     /* POSE: keypoints per row, 0..64 (kNumberOfPoints = 17); OBB: not read */
+    int32_t extra_offset; /* POSE: first keypoint float in a row; OBB: the angle (radians); OBB_NMS_FREE: the angle,
+                             which ends the row (row_floats - 1) */
+    int32_t num_kpts;     /* POSE: keypoints per row, 0..64 (kNumberOfPoints = 17); OBB, OBB_NMS_FREE: not read */
 } trtx_pose_obb_params;
 
 /* dets_dev [B, 1 + max_rows*row_floats]: count, then rows (box4, conf, class, keep, extras...) -- the compact NMS output:
@@ -470,17 +476,49 @@ typedef struct trtx_pose_obb_params {
  *   OBB : batch_nms_obb (TRTX_BOX_OBB, greedy or one-shot): row_floats 8, extra_offset 7, box cx, cy, w, h.
  *   Of the first min(count, max_rows) rows only those with (int)keep == 1 are used (process_decode_ptr_host(_obb)): every
  *   greedy row, the kept rows of a one-shot output.
+ *   OBB_NMS_FREE: the output of YoloLayerPlugin26 with is_obb (TRTX_YOLO_V26, det_floats 90): row_floats 90,
+ *   extra_offset 89, box cx, cy, w, h; every one of the first min(count, max_rows) rows is used (yolo26's
+ *   batch_decode_obb, yolo26/src/postprocess.cpp:310-326).
  * frame_wh_host: `batch` (img_w, img_h) pairs in HOST memory (copied into launch parameters; sizes may differ in a call).
  * rows_dev [B, 1 + max_rows*F]: n kept rows in input order, then zeros up to max_rows:
  *   pose, F = 6 + 3*num_kpts: (x, y, w, h, conf, class, kx, ky, kc, ...) = trtx_get_rect_adapt_landmark;
- *   OBB,  F = 10: (x0, y0, x1, y1, x2, y2, x3, y3, conf, class) = trtx_get_corner.
+ *   OBB and OBB_NMS_FREE, F = 10: (x0, y0, x1, y1, x2, y2, x3, y3, conf, class) = trtx_get_corner.
  * Bit-identical to those host functions (the device's double cos / sin are not correctly rounded, see trtx_get_corner).
  * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
- * batch / max_rows / sizes <= 0, an unknown task, row_floats < 7 or extras outside the row, num_kpts outside 0..64.  One
- * launch per 64 frames, one CTA per frame, no atomics (deterministic), no workspace; can be captured in a CUDA graph. */
+ * batch / max_rows / sizes <= 0, an unknown task, row_floats < 7 or extras outside the row, num_kpts outside 0..64, an
+ * OBB_NMS_FREE angle that is not the row's last float.  One launch per 64 frames, one CTA per frame, no atomics
+ * (deterministic), no workspace; can be captured in a CUDA graph. */
 TRTX_API int trtx_yolo_pose_obb_postprocess_enqueue(const trtx_pose_obb_params* p, const int32_t* frame_wh_host, int batch,
                                                     const float* dets_dev, int max_rows, float* rows_dev,
                                                     trtx_stream_t stream);
+
+/* RetinaFace's last host stage on the device: the loop of retinaface/retina_r50.cpp:373-388 (CONF_THRESH, then
+ * get_rect_adapt_landmark) and of retinafaceAntiCov/retinafaceAntiCov.cpp:540-552 (no threshold), for a batch of frames of
+ * any sizes.  The drawing stays with the caller. */
+typedef struct trtx_face_post_params {
+    int32_t variant;    /* TRTX_RETINA_FACE: 15-float output rows | TRTX_RETINA_ANTICOV: 16 (+ mask_confidence) */
+    int32_t in_w, in_h; /* decodeplugin::INPUT_W / INPUT_H (640x480 compiled into retinaface, 640x640 in AntiCov / config 3) */
+    int32_t row_floats; /* floats per input row: 17 (compact NMS rows, extra_floats 10) / 18 (AntiCov, extra_floats 11) */
+    int32_t lmk_offset; /* first landmark float of a row: 7; AntiCov's mask_confidence follows the 10 landmarks */
+    float conf_thresh;  /* a row is skipped when conf < conf_thresh (retina_r50.cpp:381); -INFINITY = no filter (AntiCov).
+                           For the reference's double threshold T, pass the smallest float >= T: a float c satisfies
+                           c < T exactly when c < that float (0.75 is exact). */
+} trtx_face_post_params;
+
+/* dets_dev [B, 1 + max_rows*row_floats]: count, then (x1, y1, x2, y2, conf, class, keep, extras...) rows -- the compact
+ *   output of trtx_nms_enqueue with TRTX_BOX_RETINA, extra_offset 5 (the landmarks, then AntiCov's mask_confidence).  Of the
+ *   first min(count, max_rows) rows those with (int)keep == 1 and !(conf < conf_thresh) are used (a NaN conf is kept, as in
+ *   the reference).
+ * frame_wh_host: `batch` (img_w, img_h) pairs in HOST memory (copied into launch parameters; sizes may differ in a call).
+ * rows_dev [B, 1 + max_rows*F], F = 15 (FACE) or 16 (ANTICOV): the used count, then per used row in input order
+ *   (x, y, w, h, conf, lx0, ly0, ..., lx4, ly4[, mask_conf]): the rectangle of trtx_retina_get_rect_adapt_landmark as
+ *   floats (exact for |v| <= 2^24) and its mapped landmarks, bit-identical to that host function; rows past the count are
+ *   zeroed.
+ * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
+ * batch / max_rows / sizes <= 0, an unknown variant, row_floats < 7, landmarks or mask_confidence outside the row.  One
+ * launch per 64 frames, one CTA per frame, no atomics, no workspace; can be captured in a CUDA graph. */
+TRTX_API int trtx_retina_postprocess_enqueue(const trtx_face_post_params* p, const int32_t* frame_wh_host, int batch,
+                                             const float* dets_dev, int max_rows, float* rows_dev, trtx_stream_t stream);
 
 /* =====================================================================================
  * 7. Mask R-CNN pre- and post-process

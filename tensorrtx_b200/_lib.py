@@ -18,7 +18,7 @@ BOX_LTRB, BOX_CXCYWH, BOX_RETINA, BOX_OBB = 0, 1, 2, 3
 NMS_GREEDY, NMS_ONESHOT = 0, 1
 ROI_WINDOW, ROI_DIRECT = 0, 1
 RETINA_FACE, RETINA_ANTICOV = 0, 1
-TASK_POSE, TASK_OBB = 1, 2
+TASK_POSE, TASK_OBB, TASK_OBB_NMS_FREE = 1, 2, 3
 
 _ERR = {1: "TRTX_ERR_INVALID", 2: "TRTX_ERR_WORKSPACE", 3: "TRTX_ERR_CUDA", 4: "TRTX_ERR_UNSUPPORTED"}
 
@@ -112,6 +112,10 @@ class PoseObbParams(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("task", "net_w", "net_h", "row_floats", "extra_offset", "num_kpts")]
 
 
+class FacePostParams(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("variant", "in_w", "in_h", "row_floats", "lmk_offset")] + [("conf_thresh", C.c_float)]
+
+
 # TRTX_LIB: another build of the same ABI (the probe build of tools/nms_probe.py); default = the in-tree release library
 LIB_PATH = Path(os.environ.get("TRTX_LIB") or Path(__file__).resolve().parent / "lib" / "libtrtx_hot.so")
 
@@ -160,6 +164,7 @@ SYMBOLS = {
     "trtx_yolo_seg_postprocess_enqueue": (_i, [C.POINTER(MaskParams), C.POINTER(Frame), _i, _vp, _vp, _i, _vp, _vp]),
     "trtx_get_corner": (_i, [_i, _i, _i, _i, C.POINTER(C.c_float), _f, C.POINTER(C.c_int)]),
     "trtx_yolo_pose_obb_postprocess_enqueue": (_i, [C.POINTER(PoseObbParams), C.POINTER(C.c_int32), _i, _vp, _i, _vp, _vp]),
+    "trtx_retina_postprocess_enqueue": (_i, [C.POINTER(FacePostParams), C.POINTER(C.c_int32), _i, _vp, _i, _vp, _vp]),
     "trtx_yolo_decode_nms_gather_enqueue": (_i, [C.POINTER(YoloParams), C.POINTER(NmsParams), _i, _pp, _vp, _vp, _vp, _sz,
                                                  C.POINTER(Gather), _vp]),
     "trtx_gather_wait_enqueue": (_i, [C.POINTER(Gather), _vp]),
@@ -191,7 +196,7 @@ def load() -> C.CDLL:
         fn.restype = res
         fn.argtypes = args
     for which, st in enumerate((YoloParams, NmsParams, RetinaParams, ImageDesc, MaskParams, RcnnPostParams,
-                                   Frame, PoseObbParams, Frame)):
+                                   Frame, PoseObbParams, Frame, FacePostParams)):
         if lib.trtx_abi_sizeof(which) != C.sizeof(st):
             raise TrtxError(f"{LIB_PATH} was built from a different trtx_hot.h: sizeof({st.__name__}) = "
                             f"{lib.trtx_abi_sizeof(which)} in the library, {C.sizeof(st)} in the binding (rebuild)")

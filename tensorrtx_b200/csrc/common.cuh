@@ -303,6 +303,33 @@ __host__ __device__ inline void yolo_get_corner(int net_w, int net_h, int img_w,
     }
 }
 
+// A float -> int conversion as the compiled x86-64 reference performs it (cvttss2si): truncation toward zero, and INT_MIN
+// for NaN, +-inf and values outside [-2^31, 2^31), where C++ leaves the conversion undefined.  Spelled out because the
+// device's __float2int_rz saturates instead and maps NaN to 0.
+__host__ __device__ inline int trunc_to_int_x86(float v) {
+    return v >= -2147483648.0f && v < 2147483648.0f ? (int)v : INT32_MIN;
+}
+
+// RetinaFace's get_rect_adapt_landmark (retinaface/common.hpp:65-89; retinafaceAntiCov/retinafaceAntiCov.cpp:63-87 is the
+// same statements at 640 x 640): every coordinate of the box and of the 5 landmarks is mapped as yolo_map_landmark maps it
+// (the letterbox expressions are get_rect's), then the box corners are TRUNCATED to int (trunc_to_int_x86) and not clamped;
+// w = r - l and h = b - t are int differences, which wrap modulo 2^32 as on x86-64.  rect = {l, t, w, h}; lmk (x, y pairs)
+// is mapped in place.
+__host__ __device__ inline void retina_get_rect(const YoloLetterbox& lb, const float bbox[4], int rect[4]) {
+    const int l = trunc_to_int_x86(yolo_map_landmark(lb, 0, bbox[0])), t = trunc_to_int_x86(yolo_map_landmark(lb, 1, bbox[1]));
+    const int r = trunc_to_int_x86(yolo_map_landmark(lb, 0, bbox[2])), b = trunc_to_int_x86(yolo_map_landmark(lb, 1, bbox[3]));
+    rect[0] = l;
+    rect[1] = t;
+    rect[2] = (int)((uint32_t)r - (uint32_t)l);
+    rect[3] = (int)((uint32_t)b - (uint32_t)t);
+}
+__host__ __device__ inline void retina_get_rect_adapt_landmark(int input_w, int input_h, int img_w, int img_h,
+                                                               const float bbox[4], float lmk[10], int rect[4]) {
+    const YoloLetterbox lb = yolo_letterbox(input_w, input_h, img_w, img_h);
+    retina_get_rect(lb, bbox, rect);
+    for (int i = 0; i < 10; ++i) lmk[i] = yolo_map_landmark(lb, i & 1, lmk[i]);
+}
+
 __device__ __forceinline__ int warp_excl_scan(int v, int lane, int* total) {
     int x = v;
 #pragma unroll

@@ -767,90 +767,175 @@ static int seg_fill_frames(const trtx_mask_params* p, const trtx_frame* frames, 
     return TRTX_OK;
 }
 
-// Pose and oriented-box post-process: the per-detection geometry of draw_bbox_keypoints_line (get_rect_adapt_landmark,
-// yolov8/src/postprocess.cpp:173-205) and draw_bbox_obb (get_corner, :474-507), which the reference runs on one host core
-// after a D2H copy.  One CTA of kPoseObbThreads per frame, one launch per <= 64 frames, no workspace, no atomics:
-//   the CTA walks the first min(count, max_rows) rows in passes of kPoseObbThreads, one row per thread; a ballot per warp
-//   over the keep column and a scan of the warps' counts give each kept row its output slot (input order); the owning
-//   thread computes the rectangle (yolo_get_rect) or the four corners (yolo_get_corner) into shared memory; then the whole
-//   CTA writes the pass's kept rows as one contiguous run of floats (coalesced), mapping each keypoint coordinate with
-//   yolo_map_landmark on the way.  Rows past the kept count are zeroed.
-constexpr int kPoseObbThreads = 256;   // rows per pass
-constexpr int kPoseObbWarps = kPoseObbThreads / kWarp;
+// Per-row geometry post-processes: the per-detection host stage the reference runs on one core after a D2H copy, for a
+// batch of frames of any sizes.  One CTA of kRowsThreads per frame, one launch per <= 64 frames, no workspace, no atomics.
+// frame_rows() is the pass both kernels share; a small row policy says what differs:
+//   Row::pass(d)            whether row d is used;
+//   Row::geometry(d, g)     its integer geometry, Row::kGeo ints;
+//   Row::value(d, g, e)     output float e of the row, from the row and its geometry.
+// The CTA walks the first min(count, max_rows) rows in passes of kRowsThreads, one row per thread; a ballot per warp over
+// pass() and a scan of the warps' counts give each used row its output slot (input order); the owning thread computes the
+// geometry into shared memory; then the whole CTA writes the pass's rows as one contiguous run of floats (coalesced),
+// calling value() per float.  Rows past the used count are zeroed, and float 0 gets the count.
+constexpr int kRowsThreads = 256;  // rows per pass
+constexpr int kRowsWarps = kRowsThreads / kWarp;
 constexpr int kPoseMaxKpts = 64;
 
-struct PoseObbArgs {
+// What every launch of a per-row post-process carries besides the policy's own parameters.
+struct RowFrames {
     int img_w[kMaxFrames], img_h[kMaxFrames];
     const float* dets;  // [B, 1 + max_rows * row_floats]
     float* rows;        // [B, 1 + max_rows * out_floats]
     int base;           // frames [base, base + gridDim.x) of the call
-    int pose, net_w, net_h, row_floats, extra_offset, num_kpts, out_floats, max_rows;
+    int row_floats, out_floats, max_rows;
 };
 
-__global__ void __launch_bounds__(kPoseObbThreads) pose_obb_rows_kernel(const __grid_constant__ PoseObbArgs a) {
-    __shared__ int s_src[kPoseObbThreads];      // input row of each kept row of the pass, by output slot
-    __shared__ int s_geo[kPoseObbThreads * 8];  // its rectangle (pose: 4 ints) or corners (OBB: 8 ints)
-    __shared__ int s_warp[kPoseObbWarps];       // kept rows per warp of the pass
-    const int j = blockIdx.x, tid = threadIdx.x, lane = tid & (kWarp - 1), warp = tid / kWarp, b = a.base + j;
-    const int img_w = a.img_w[j], img_h = a.img_h[j];
+template <class Row, class Args>
+__device__ __forceinline__ void frame_rows(const Args& args) {
+    const RowFrames& a = args.f;
+    __shared__ int s_src[kRowsThreads];               // input row of each used row of the pass, by output slot
+    __shared__ int s_geo[kRowsThreads * Row::kGeo];   // its geometry
+    __shared__ int s_warp[kRowsWarps];                // used rows per warp of the pass
+    const int tid = threadIdx.x, lane = tid & (kWarp - 1), warp = tid / kWarp, b = a.base + blockIdx.x;
     const size_t R = (size_t)a.row_floats, F = (size_t)a.out_floats;
     const float* src = a.dets + (size_t)b * (1 + (size_t)a.max_rows * R);
     float* out = a.rows + (size_t)b * (1 + (size_t)a.max_rows * F);
     const int n = min(max((int)src[0], 0), a.max_rows);
-    const YoloLetterbox lb = yolo_letterbox(a.net_w, a.net_h, img_w, img_h);
-    const int geo = a.pose ? 4 : 8;  // floats of the row before conf and class
-    int kept = 0;                    // rows written by the earlier passes
-    for (int i0 = 0; i0 < n; i0 += kPoseObbThreads) {
+    const Row row(args, blockIdx.x);  // after the count's load, so that the policy's set-up overlaps it
+    int kept = 0;                     // rows written by the earlier passes
+    for (int i0 = 0; i0 < n; i0 += kRowsThreads) {
         const int i = i0 + tid;
         const float* d = src + 1 + (size_t)i * R;
-        const bool keep = i < n && (int)d[6] == 1;  // process_decode_ptr_host: `int keep_flag = ...; if (keep_flag == 1)`
+        const bool keep = i < n && row.pass(d);
         const unsigned m = __ballot_sync(0xffffffffu, keep);
         if (lane == 0) s_warp[warp] = __popc(m);
         __syncthreads();
         int before = 0, total = 0;
 #pragma unroll
-        for (int w = 0; w < kPoseObbWarps; ++w) {
+        for (int w = 0; w < kRowsWarps; ++w) {
             const int c = s_warp[w];
             before += w < warp ? c : 0;
             total += c;
         }
         if (keep) {
             const int slot = before + __popc(m & ((1u << lane) - 1u));
-            int g[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-            if (a.pose)
-                yolo_get_rect(TRTX_YOLO_V8, a.net_w, a.net_h, img_w, img_h, d, g);  // {0, 0, 0, 0} where undefined
-            else
-                yolo_get_corner(a.net_w, a.net_h, img_w, img_h, d, d[a.extra_offset], g);
+            int g[Row::kGeo];
+            row.geometry(d, g);
             s_src[slot] = i;
 #pragma unroll
-            for (int e = 0; e < 8; ++e) s_geo[slot * 8 + e] = g[e];
+            for (int e = 0; e < Row::kGeo; ++e) s_geo[slot * Row::kGeo + e] = g[e];
         }
         __syncthreads();
         const size_t run = (size_t)total * F;
         float* o = out + 1 + (size_t)kept * F;
 #pragma unroll 4
-        for (size_t f = tid; f < run; f += kPoseObbThreads) {
+        for (size_t f = tid; f < run; f += kRowsThreads) {
             const int r = (int)(f / F), e = (int)(f - (size_t)r * F);
-            const float* d2 = src + 1 + (size_t)s_src[r] * R;
-            float v;
-            if (e < geo) {
-                v = (float)s_geo[r * 8 + e];
-            } else if (e < geo + 2) {
-                v = d2[4 + e - geo];  // conf, class
-            } else {
-                const int k = e - 6;  // keypoint float: x, y, conf
-                const int c = k % 3;
-                const float x = d2[a.extra_offset + k];
-                v = c == 2 ? x : yolo_map_landmark(lb, c, x);
-            }
-            o[f] = v;
+            o[f] = row.value(src + 1 + (size_t)s_src[r] * R, s_geo + r * Row::kGeo, e);
         }
         kept += total;
         __syncthreads();  // the next pass reuses the shared arrays
     }
     const size_t end = 1 + (size_t)a.max_rows * F;
-    for (size_t f = 1 + (size_t)kept * F + tid; f < end; f += kPoseObbThreads) out[f] = 0.0f;
+    for (size_t f = 1 + (size_t)kept * F + tid; f < end; f += kRowsThreads) out[f] = 0.0f;
     if (tid == 0) out[0] = (float)kept;
+}
+
+// Pose and oriented boxes: draw_bbox_keypoints_line's get_rect_adapt_landmark (yolov8/src/postprocess.cpp:173-205) and
+// draw_bbox_obb's get_corner (:474-507).  Pose rows: the rectangle (yolo_get_rect), conf, class, each keypoint coordinate
+// mapped with yolo_map_landmark; OBB rows: the four corners (yolo_get_corner), conf, class.  The NMS-free yolo26 rows have
+// no keep column and use every row.
+struct PoseObbArgs {
+    RowFrames f;
+    int pose, nms_free, net_w, net_h, extra_offset, num_kpts;
+};
+
+struct PoseObbRow {
+    static constexpr int kGeo = 8;  // the rectangle (pose: 4 ints) or the corners (OBB: 8 ints)
+    const PoseObbArgs& a;
+    int img_w, img_h;
+    YoloLetterbox lb;
+    int geo;  // floats of the output row before conf and class
+    __device__ PoseObbRow(const PoseObbArgs& args, int j)
+        : a(args), img_w(args.f.img_w[j]), img_h(args.f.img_h[j]),
+          lb(yolo_letterbox(args.net_w, args.net_h, img_w, img_h)), geo(args.pose ? 4 : 8) {}
+    // process_decode_ptr_host: `int keep_flag = ...; if (keep_flag == 1)`; yolo26's batch_decode_obb takes every row
+    __device__ bool pass(const float* d) const { return a.nms_free || (int)d[6] == 1; }
+    __device__ void geometry(const float* d, int g[8]) const {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) g[e] = 0;
+        if (a.pose)
+            yolo_get_rect(TRTX_YOLO_V8, a.net_w, a.net_h, img_w, img_h, d, g);  // {0, 0, 0, 0} where undefined
+        else
+            yolo_get_corner(a.net_w, a.net_h, img_w, img_h, d, d[a.extra_offset], g);
+    }
+    __device__ float value(const float* d, const int* g, int e) const {
+        if (e < geo) return (float)g[e];
+        if (e < geo + 2) return d[4 + e - geo];  // conf, class
+        const int k = e - 6;                     // keypoint float: x, y, conf
+        const int c = k % 3;
+        const float x = d[a.extra_offset + k];
+        return c == 2 ? x : yolo_map_landmark(lb, c, x);
+    }
+};
+
+__global__ void __launch_bounds__(kRowsThreads) pose_obb_rows_kernel(const __grid_constant__ PoseObbArgs a) {
+    frame_rows<PoseObbRow>(a);
+}
+
+// Faces: the loop of retinaface/retina_r50.cpp:373-388 (retinafaceAntiCov/retinafaceAntiCov.cpp:540-552 without its
+// threshold) over the compact NMS rows (box4, conf, class, keep, extras...): kept rows with !(conf < conf_thresh) become
+// (x, y, w, h, conf, 10 landmark floats[, mask_conf]) by retina_get_rect_adapt_landmark.
+struct FaceArgs {
+    RowFrames f;
+    int in_w, in_h, lmk_offset;
+    float conf_thresh;
+};
+
+struct FaceRow {
+    static constexpr int kGeo = 4;  // the rectangle
+    const FaceArgs& a;
+    YoloLetterbox lb;
+    __device__ FaceRow(const FaceArgs& args, int j)
+        : a(args), lb(yolo_letterbox(args.in_w, args.in_h, args.f.img_w[j], args.f.img_h[j])) {}
+    // `if (res[j].class_confidence < CONF_THRESH) continue;`: a NaN confidence is kept
+    __device__ bool pass(const float* d) const { return (int)d[6] == 1 && !(d[4] < a.conf_thresh); }
+    __device__ void geometry(const float* d, int g[4]) const { retina_get_rect(lb, d, g); }
+    __device__ float value(const float* d, const int* g, int e) const {
+        if (e < 4) return (float)g[e];
+        if (e == 4) return d[4];
+        const int k = e - 5;  // landmark float, then mask_conf
+        const float x = d[a.lmk_offset + k];
+        return k < 10 ? yolo_map_landmark(lb, k & 1, x) : x;
+    }
+};
+
+__global__ void __launch_bounds__(kRowsThreads) face_rows_kernel(const __grid_constant__ FaceArgs a) {
+    frame_rows<FaceRow>(a);
+}
+
+// Every frame size of a per-row call is checked before the first launch, so that a rejected call writes nothing.
+inline bool frames_valid(const int32_t* frame_wh_host, int batch) {
+    for (int i = 0; i < batch; ++i)
+        if (frame_wh_host[2 * i] <= 0 || frame_wh_host[2 * i + 1] <= 0) return false;
+    return true;
+}
+
+// One launch of `kernel` per <= kMaxFrames frames, each with its frames' sizes in the launch parameters.
+template <class Args>
+int launch_frame_rows(void (*kernel)(Args), Args& a, const int32_t* frame_wh_host, int batch, cudaStream_t st) {
+    for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {
+        const int n = min(batch - i0, kMaxFrames);
+        a.f.base = i0;
+        for (int j = 0; j < n; ++j) {
+            a.f.img_w[j] = frame_wh_host[2 * (i0 + j)];
+            a.f.img_h[j] = frame_wh_host[2 * (i0 + j) + 1];
+        }
+        kernel<<<n, kRowsThreads, 0, st>>>(a);
+        const int rc = check_launch();
+        if (rc) return rc;
+    }
+    return TRTX_OK;
 }
 
 }  // namespace trtx
@@ -1101,39 +1186,49 @@ TRTX_API int trtx_yolo_pose_obb_postprocess_enqueue(const trtx_pose_obb_params* 
                                                     const float* dets_dev, int max_rows, float* rows_dev,
                                                     trtx_stream_t stream) {
     if (!p || !frame_wh_host || batch <= 0 || !dets_dev || !rows_dev || max_rows <= 0) return TRTX_ERR_INVALID;
-    if (p->task != TRTX_TASK_POSE && p->task != TRTX_TASK_OBB) return TRTX_ERR_INVALID;
+    if (p->task != TRTX_TASK_POSE && p->task != TRTX_TASK_OBB && p->task != TRTX_TASK_OBB_NMS_FREE) return TRTX_ERR_INVALID;
     if (p->net_w <= 0 || p->net_h <= 0 || p->row_floats < 7 || p->extra_offset < 0) return TRTX_ERR_INVALID;
-    const bool pose = p->task == TRTX_TASK_POSE;
+    const bool pose = p->task == TRTX_TASK_POSE, nms_free = p->task == TRTX_TASK_OBB_NMS_FREE;
     if (pose && (p->num_kpts < 0 || p->num_kpts > kPoseMaxKpts || p->extra_offset + 3 * p->num_kpts > p->row_floats))
         return TRTX_ERR_INVALID;
     if (!pose && p->extra_offset >= p->row_floats) return TRTX_ERR_INVALID;
-    // every frame is checked before the first launch, so that a rejected call writes nothing
-    for (int i = 0; i < batch; ++i)
-        if (frame_wh_host[2 * i] <= 0 || frame_wh_host[2 * i + 1] <= 0) return TRTX_ERR_INVALID;
+    // the NMS-free plugin row ends with the angle (yolo26/include/types.h: Detection::angle)
+    if (nms_free && p->extra_offset != p->row_floats - 1) return TRTX_ERR_INVALID;
+    if (!frames_valid(frame_wh_host, batch)) return TRTX_ERR_INVALID;
     PoseObbArgs a;
-    a.dets = dets_dev;
-    a.rows = rows_dev;
+    a.f.dets = dets_dev;
+    a.f.rows = rows_dev;
+    a.f.row_floats = p->row_floats;
+    a.f.out_floats = pose ? 6 + 3 * p->num_kpts : 10;
+    a.f.max_rows = max_rows;
     a.pose = pose;
+    a.nms_free = nms_free;
     a.net_w = p->net_w;
     a.net_h = p->net_h;
-    a.row_floats = p->row_floats;
     a.extra_offset = p->extra_offset;
     a.num_kpts = pose ? p->num_kpts : 0;
-    a.out_floats = pose ? 6 + 3 * p->num_kpts : 10;
-    a.max_rows = max_rows;
-    const cudaStream_t st = static_cast<cudaStream_t>(stream);
-    for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {
-        const int n = min(batch - i0, kMaxFrames);
-        a.base = i0;
-        for (int j = 0; j < n; ++j) {
-            a.img_w[j] = frame_wh_host[2 * (i0 + j)];
-            a.img_h[j] = frame_wh_host[2 * (i0 + j) + 1];
-        }
-        pose_obb_rows_kernel<<<n, kPoseObbThreads, 0, st>>>(a);
-        const int rc = check_launch();
-        if (rc) return rc;
-    }
-    return TRTX_OK;
+    return launch_frame_rows(pose_obb_rows_kernel, a, frame_wh_host, batch, static_cast<cudaStream_t>(stream));
+}
+
+TRTX_API int trtx_retina_postprocess_enqueue(const trtx_face_post_params* p, const int32_t* frame_wh_host, int batch,
+                                             const float* dets_dev, int max_rows, float* rows_dev, trtx_stream_t stream) {
+    if (!p || !frame_wh_host || batch <= 0 || !dets_dev || !rows_dev || max_rows <= 0) return TRTX_ERR_INVALID;
+    if (p->variant != TRTX_RETINA_FACE && p->variant != TRTX_RETINA_ANTICOV) return TRTX_ERR_INVALID;
+    const int extras = p->variant == TRTX_RETINA_ANTICOV ? 11 : 10;  // the landmarks (+ mask_confidence)
+    if (p->in_w <= 0 || p->in_h <= 0 || p->row_floats < 7 || p->lmk_offset < 0 || p->lmk_offset > p->row_floats - extras)
+        return TRTX_ERR_INVALID;
+    if (!frames_valid(frame_wh_host, batch)) return TRTX_ERR_INVALID;
+    FaceArgs a;
+    a.f.dets = dets_dev;
+    a.f.rows = rows_dev;
+    a.f.row_floats = p->row_floats;
+    a.f.out_floats = 5 + extras;
+    a.f.max_rows = max_rows;
+    a.in_w = p->in_w;
+    a.in_h = p->in_h;
+    a.lmk_offset = p->lmk_offset;
+    a.conf_thresh = p->conf_thresh;
+    return launch_frame_rows(face_rows_kernel, a, frame_wh_host, batch, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

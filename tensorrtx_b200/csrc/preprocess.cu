@@ -599,35 +599,12 @@ TRTX_API int trtx_get_corner(int net_w, int net_h, int img_w, int img_h, const f
     return TRTX_OK;
 }
 
-// get_rect_adapt_landmark of RetinaFace, retinaface/common.hpp:65-89, statement by statement: box AND the 5 landmarks (x, y pairs) of
-// a face mapped from the letterboxed network input back to the original image; the box corners are TRUNCATED to int (`int l =
-// bbox[0] / r_w`), not rounded, and not clamped to the image.
+// get_rect_adapt_landmark of RetinaFace, retinaface/common.hpp:65-89 (retina_get_rect_adapt_landmark in common.cuh, shared
+// with the face post-process kernel of mask.cu).
 TRTX_API int trtx_retina_get_rect_adapt_landmark(int input_w, int input_h, int img_w, int img_h, const float bbox[4], float lmk[10],
                                                  int rect[4]) {
     if (!bbox || !lmk || !rect || input_w <= 0 || input_h <= 0 || img_w <= 0 || img_h <= 0) return TRTX_ERR_INVALID;
-    int l, r, t, b;
-    float r_w = input_w / (img_w * 1.0);
-    float r_h = input_h / (img_h * 1.0);
-    if (r_h > r_w) {
-        l = bbox[0] / r_w;
-        r = bbox[2] / r_w;
-        t = (bbox[1] - (input_h - r_w * img_h) / 2) / r_w;
-        b = (bbox[3] - (input_h - r_w * img_h) / 2) / r_w;
-        for (int i = 0; i < 10; i += 2) {
-            lmk[i] /= r_w;
-            lmk[i + 1] = (lmk[i + 1] - (input_h - r_w * img_h) / 2) / r_w;
-        }
-    } else {
-        l = (bbox[0] - (input_w - r_h * img_w) / 2) / r_h;
-        r = (bbox[2] - (input_w - r_h * img_w) / 2) / r_h;
-        t = bbox[1] / r_h;
-        b = bbox[3] / r_h;
-        for (int i = 0; i < 10; i += 2) {
-            lmk[i] = (lmk[i] - (input_w - r_h * img_w) / 2) / r_h;
-            lmk[i + 1] /= r_h;
-        }
-    }
-    rect[0] = l, rect[1] = t, rect[2] = r - l, rect[3] = b - t;
+    retina_get_rect_adapt_landmark(input_w, input_h, img_w, img_h, bbox, lmk, rect);
     return TRTX_OK;
 }
 

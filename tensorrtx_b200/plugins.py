@@ -58,6 +58,14 @@ def float_le_threshold(x: float) -> float:
     return t
 
 
+def float_ge_threshold(x: float) -> float:
+    """Smallest fp32 t with t >= x: `(double)conf < x`  <=>  `conf < t` in fp32 (retinaface's CONF_THRESH literal)."""
+    t = struct.unpack("f", struct.pack("f", x))[0]
+    if t < x:
+        t = float(torch.nextafter(torch.tensor(t, dtype=torch.float32), torch.tensor(math.inf)).item())
+    return t
+
+
 # --------------------------------------------------------------------------------------------------
 # YoloLayer_TRT, anchor-free (yolov8 / yolo11 / yolov12 / yolov13 ...)
 # --------------------------------------------------------------------------------------------------
@@ -648,20 +656,27 @@ def yolo_seg_postprocess(proto: torch.Tensor | None, dets: torch.Tensor, image_s
 
 
 def yolo_pose_obb_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]], *, task: int, max_rows: int,
-                              row_floats: int | None = None, extra_offset: int = 7, num_kpts: int = 17, net_w: int = 640,
-                              net_h: int = 640, rows_out: torch.Tensor | None = None, stream=None) -> torch.Tensor:
+                              row_floats: int | None = None, extra_offset: int | None = None, num_kpts: int = 17,
+                              net_w: int = 640, net_h: int = 640, rows_out: torch.Tensor | None = None,
+                              stream=None) -> torch.Tensor:
     """GPU drop-in for the pose and oriented-box models' geometry after NMS: get_rect_adapt_landmark of
     draw_bbox_keypoints_line (task TASK_POSE, yolov8/src/postprocess.cpp:173-205) or get_corner of draw_bbox_obb (task
     TASK_OBB, :474-507; yolo11-obb: net_w = net_h = 1024) for a batch of frames of any sizes.
     dets [B, 1 + max_rows*row_floats]: count, then (box4, conf, class, keep, extras...) rows -- the compact NMS output (pose:
     extra_floats 51, row_floats 58; OBB: batch_nms_obb, row_floats 8); only rows with (int)keep == 1 are used.
+    Task TASK_OBB_NMS_FREE: dets is yolo26-obb's NMS-free plugin output (YoloLayerPlugin26 with is_obb, row_floats 90, the
+    angle last; net_w = net_h = 1024) and every row is used, as yolo26's batch_decode_obb + draw_bbox_obb do.
+    extra_offset defaults to 7 (the first keypoint, or the angle of a compact OBB row), and to row_floats - 1 for
+    TASK_OBB_NMS_FREE.
     image_sizes[b] = (img_w, img_h) of frame b -> rows [B, 1 + max_rows*F] fp32: the kept count, then per kept row (input
     order) pose (x, y, w, h, conf, class, kx, ky, kc, ...), F = 6 + 3*num_kpts, or OBB (x0, y0, ..., x3, y3, conf, class),
     F = 10; rows past the count are zero.  One launch per 64 frames, no workspace."""
     lib = L.load()
     B = len(image_sizes)
     if row_floats is None:
-        row_floats = 7 + 3 * num_kpts if task == L.TASK_POSE else 8
+        row_floats = {L.TASK_POSE: 7 + 3 * num_kpts, L.TASK_OBB_NMS_FREE: YoloLayerPlugin26.DET_FLOATS}.get(task, 8)
+    if extra_offset is None:
+        extra_offset = row_floats - 1 if task == L.TASK_OBB_NMS_FREE else 7
     if dets.dim() != 2 or dets.shape[0] != B or dets.shape[1] < 1 + max_rows * row_floats:
         raise ValueError(f"dets must be [{B}, >= {1 + max_rows * row_floats}]")
     if dets.dtype != torch.float32 or dets.stride(1) != 1 or dets.stride(0) != dets.shape[1]:
@@ -675,6 +690,41 @@ def yolo_pose_obb_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[in
     wh = (C.c_int32 * (2 * B))(*[int(v) for s in image_sizes for v in s])
     L.check(lib.trtx_yolo_pose_obb_postprocess_enqueue(C.byref(q), wh, B, _ptr(dets), max_rows, _ptr(rows_out),
                                                        _stream(stream)), "trtx_yolo_pose_obb_postprocess_enqueue")
+    return rows_out
+
+
+def retina_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]], *, variant: int, max_rows: int,
+                       conf_thresh: float, in_w: int, in_h: int, row_floats: int | None = None, lmk_offset: int = 7,
+                       rows_out: torch.Tensor | None = None, stream=None) -> torch.Tensor:
+    """GPU drop-in for RetinaFace's last host stage after NMS: retinaface/retina_r50.cpp:373-388 (skip a face with
+    class_confidence < CONF_THRESH, then get_rect_adapt_landmark; in_w x in_h = decodeplugin::INPUT_W x INPUT_H) and
+    retinafaceAntiCov/retinafaceAntiCov.cpp:540-552 (variant RETINA_ANTICOV, no threshold: conf_thresh = -math.inf, 640 x 640)
+    for a batch of frames of any sizes.
+    dets [B, 1 + max_rows*row_floats]: count, then (x1, y1, x2, y2, conf, class, keep, landmarks[, mask_conf]) rows -- the
+    output of batch_nms(..., box_format=BOX_RETINA, extra_floats=10 (AntiCov 11), extra_offset=5); row_floats defaults to
+    17 (AntiCov 18).  Rows with (int)keep == 1 and !(conf < conf_thresh) are used (a NaN conf is kept); conf_thresh is the
+    reference's double literal, passed to the library as the smallest float >= it, which selects the same faces.
+    image_sizes[b] = (img_w, img_h) of frame b -> rows [B, 1 + max_rows*F] fp32, F = 15 (AntiCov 16): the used count, then
+    per used row (input order) (x, y, w, h, conf, lx0, ly0, ..., lx4, ly4[, mask_conf]) = retina_get_rect_adapt_landmark;
+    rows past the count are zero.  One launch per 64 frames, no workspace."""
+    lib = L.load()
+    B = len(image_sizes)
+    extras = 11 if variant == L.RETINA_ANTICOV else 10
+    if row_floats is None:
+        row_floats = 7 + extras
+    if dets.dim() != 2 or tuple(dets.shape) != (B, 1 + max_rows * row_floats):
+        raise ValueError(f"dets must be [{B}, {1 + max_rows * row_floats}]")
+    if dets.dtype != torch.float32 or dets.stride(1) != 1 or dets.stride(0) != dets.shape[1]:
+        raise ValueError("dets must be contiguous float32")
+    F = 5 + extras
+    q = L.FacePostParams(variant, in_w, in_h, row_floats, lmk_offset, float_ge_threshold(conf_thresh))
+    if rows_out is None:
+        rows_out = torch.empty((B, 1 + max_rows * F), dtype=torch.float32, device=dets.device)
+    if tuple(rows_out.shape) != (B, 1 + max_rows * F) or rows_out.dtype != torch.float32 or not rows_out.is_contiguous():
+        raise ValueError(f"rows_out must be contiguous float32 [{B}, {1 + max_rows * F}]")
+    wh = (C.c_int32 * (2 * B))(*[int(v) for s in image_sizes for v in s])
+    L.check(lib.trtx_retina_postprocess_enqueue(C.byref(q), wh, B, _ptr(dets), max_rows, _ptr(rows_out), _stream(stream)),
+            "trtx_retina_postprocess_enqueue")
     return rows_out
 
 
