@@ -583,6 +583,40 @@ TRTX_API int trtx_rcnn_postprocess_frames_enqueue(const trtx_rcnn_post_params* p
                                                   const float* classes_dev, const float* masks_dev, float* rows_dev,
                                                   trtx_stream_t stream);
 
+/* The outlines of the pasted masks: cv::findContours(curMask, contours, RETR_EXTERNAL, CHAIN_APPROX_NONE) of
+ * rcnn/rcnn.cpp:551-552 for every canvas k < min(count, max_masks) of every frame, bit for bit as cv2 4.13 returns it
+ * (8-connected components of the nonzero pixels, the outer border of each component not inside a hole of another, each
+ * starting at its component's first pixel in raster order and going down its left side first, the contours in descending
+ * raster order of their starts).  The drawing (cv::drawContours) stays with the caller.
+ * p: the parameters of the post-process call that wrote rows and canvases; only detections_per_im and max_masks are read.
+ * images_host: `batch` descriptors in HOST memory, each with its canvases (the single-size entry's dense canvases are frames
+ *   of equal size with pitch = img_w).  rows_dev [B, 1 + D*7]: that call's rows.
+ * The call reads only the paste rectangle r of each row (trtx_rcnn_postprocess_enqueue's), where the post-process writes;
+ *   it returns the contours of the canvas restricted to r, which are those of the whole canvas, since the post-process
+ *   leaves 0 outside r.  Where the reference throws (empty r, r leaving the image, a non-finite box) the canvas is all zeros
+ *   and the call reports 0 contours.
+ * Outputs, with C = max_contours and P = max_points capacities per canvas:
+ *   counts_dev  [B, max_masks, 2] int32: (n_contours, n_points), the true totals even past the capacities; written for
+ *               every slot, (0, 0) at or past the frame's min(count, max_masks);
+ *   lengths_dev [B, max_masks, C] int32: the point counts of the first min(n_contours, C) contours;
+ *   points_dev  [B, max_masks, P, 2] int32: (x, y) in frame pixels, the first min(n_points, P) points of the contours
+ *               concatenated in order.
+ *   Entries past those counts are not written.
+ * Workspace: trtx_rcnn_contours_workspace_size(p, images_host, batch) bytes, 16-byte aligned; it depends on the arguments
+ *   only: min(min(batch, 64) * max_masks, 128) slots of (W + 2)(H + 2) + 8 ceil(W/2) ceil(H/2) + 256 ceil(W/2) bytes
+ *   (each term the largest over the frames, the sum rounded up to 256), about 3 bytes per frame pixel.  0 when the
+ *   arguments are rejected.
+ * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
+ *   batch / sizes / detections_per_im / max_masks / max_contours / max_points <= 0, a frame without canvases, pitch < img_w,
+ *   a misaligned workspace; TRTX_ERR_WORKSPACE for a smaller workspace_bytes; TRTX_ERR_UNSUPPORTED for a frame of more
+ *   than 2^29 pixels.  One launch per 64 frames of at most 128 CTAs with 200 KB of dynamic shared memory each, no atomics
+ *   (deterministic); can be captured in a CUDA graph. */
+TRTX_API size_t trtx_rcnn_contours_workspace_size(const trtx_rcnn_post_params* p, const trtx_frame* images_host, int batch);
+TRTX_API int trtx_rcnn_contours_enqueue(const trtx_rcnn_post_params* p, const trtx_frame* images_host, int batch,
+                                        const float* rows_dev, int max_contours, int max_points, int32_t* counts_dev,
+                                        int32_t* lengths_dev, int32_t* points_dev, void* workspace_dev,
+                                        size_t workspace_bytes, trtx_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -90,7 +90,7 @@ def build(force: bool = False, verbose: bool = False, probe: bool = False, defin
 
 def build_oracle() -> Path:
     """Compile the CPU oracles (test infrastructure) and, when /root/reference exists, oracle/_ref."""
-    for extra in ([], ["-f", "face_obb26.mk"]):
+    for extra in ([], ["-f", "face_obb26.mk"], ["-f", "contours.mk"]):
         r = subprocess.run(["make", "-C", str(ROOT / "oracle"), *extra], stdout=subprocess.PIPE, stderr=subprocess.STDOUT,
                            text=True)
         if r.returncode != 0:

@@ -485,6 +485,268 @@ static int rcnn_fill_frames(const trtx_rcnn_post_params* p, const trtx_frame* fr
     return TRTX_OK;
 }
 
+// Outlines of the Mask R-CNN canvases: cv::findContours(curMask, RETR_EXTERNAL, CHAIN_APPROX_NONE) of rcnn/rcnn.cpp:551-552,
+// OpenCV's Suzuki-Abe border following restated bit for bit (oracle_find_contours_external spells out the scan).  By the
+// post-process's contract a canvas is 0 outside the paste rectangle r of its row, so the kernel reads r only.  A persistent
+// grid: CTA i owns workspace slot i and walks canvases i, i + gridDim.x, ... of the launch.  Per canvas:
+//   A. r -> the slot's padded int8 map (1 where nonzero, a zero frame around it), all threads;
+//   B. bands of kContourBand rows: all warps list the band's runs of nonzero pixels (start, end) in raster order; warp 0 then
+//      walks them in order.  A run start with value 1 (unvisited) is an outer-border start, followed by lane 0 unless the
+//      value at lnbd (the last place in the row where the value changed to a mark) is positive; following marks the map and
+//      appends (start, length) to the slot's contour list.  The lanes hold 32 runs' start / end values at a time (reloaded
+//      after a trace), so the walk costs a few instructions per run;
+//   C. contours in descending start order (cv2's): a suffix scan of the lengths gives each contour's first point, and one
+//      thread per contour follows it again (the path reads zero / nonzero only) to write its points up to max_points.
+// No atomics: the output depends only on the canvas.
+constexpr int kContourThreads = 256;
+constexpr int kContourWarps = kContourThreads / kWarp;
+constexpr int kContourBand = 32;     // map rows per run-listing band
+constexpr int kContourCtas = 128;    // CTAs (workspace slots) per launch at most
+constexpr int kContourSmem = 200 * 1024;  // dynamic shared memory per CTA: the map of an r that fits goes here
+
+struct ContourFrame {
+    const uint8_t* canvas;  // [max_masks, img_h, pitch]
+    int img_w, img_h, pitch;
+};
+struct ContourArgs {
+    ContourFrame f[kMaxFrames];
+    const float* rows;  // [B, 1 + D * 7]
+    int32_t* counts;    // [B, max_masks, 2]
+    int32_t* lengths;   // [B, max_masks, C]
+    int32_t* points;    // [B, max_masks, P, 2]
+    uint8_t* work;      // gridDim.x slots of slot_bytes
+    size_t slot_bytes;
+    long long map_bytes, list_bytes;  // offsets in a slot: map at 0, contour list at map_bytes, band runs at + list_bytes
+    int base, n_images, dets, max_masks, max_contours, max_points;
+};
+
+// The regions of a workspace slot for a frame of w x h: the padded map; the contour list (at most ceil(w/2) * ceil(h/2)
+// contours: a component and the zero pixels that part it from the next take 2 x 2 pixels); the runs of one band (at most
+// ceil(w/2) per row).  A call's slot holds the largest of each region over its frames.
+static void contour_regions(int w, int h, long long& map_bytes, long long& list_bytes, long long& band_bytes) {
+    map_bytes = ((long long)(w + 2) * (h + 2) + 15) / 16 * 16;
+    list_bytes = (long long)((w + 1) / 2) * ((h + 1) / 2) * 8;
+    band_bytes = (long long)kContourBand * ((w + 1) / 2) * 8;
+}
+
+// Step s of the 3 x 3 neighbourhood (0 east, 1 north-east, ... counter-clockwise, y down), OpenCV's CV_INIT_3X3_DELTAS
+__device__ __forceinline__ int code_dx(int s) { return ((36890 >> (2 * s)) & 3) - 1; }  // {1, 1, 0, -1, -1, -1, 0, 1}
+__device__ __forceinline__ int code_dy(int s) { return ((43265 >> (2 * s)) & 3) - 1; }  // {0, -1, -1, -1, 0, 1, 1, 1}
+
+// OpenCV's icvFetchContour for the outer border starting at map index i0 (map coordinates x, y): returns the number of
+// points.  mark: write the visit marks (-2 where the search passed the right neighbour as 0, else 2 over a 1).  out: when not
+// null, point q < limit goes to out[2q], out[2q + 1] as (x + ox, y + oy).
+__device__ int contour_follow(int8_t* m, int stride, int i0, int x, int y, bool mark, int32_t* out, int limit, int ox, int oy) {
+    int s = 4, i1;
+    do {
+        s = (s - 1) & 7;
+        i1 = i0 + code_dx(s) + code_dy(s) * stride;
+    } while (m[i1] == 0 && s != 4);
+    if (s == 4) {  // a lone pixel
+        if (mark) m[i0] = -2;
+        if (out && limit > 0) out[0] = x + ox, out[1] = y + oy;
+        return 1;
+    }
+    int i3 = i0, i4, n = 0;
+    for (;;) {
+        const int s_end = s;
+        do {
+            ++s;
+            i4 = i3 + code_dx(s & 7) + code_dy(s & 7) * stride;
+        } while (m[i4] == 0);
+        s &= 7;
+        if (mark) {
+            if ((unsigned)(s - 1) < (unsigned)s_end) m[i3] = -2;
+            else if (m[i3] == 1) m[i3] = 2;
+        }
+        if (out && n < limit) {
+            out[2 * n] = x + ox;
+            out[2 * n + 1] = y + oy;
+        }
+        ++n;
+        x += code_dx(s);
+        y += code_dy(s);
+        if (i4 == i0 && i3 == i1) break;
+        i3 = i4;
+        s = (s + 4) & 7;
+    }
+    return n;
+}
+
+__device__ __forceinline__ bool is_mark(int v) { return (v & -2) != 0; }
+
+__global__ void __launch_bounds__(kContourThreads) rcnn_contours_kernel(const __grid_constant__ ContourArgs a) {
+    __shared__ int s_off[kContourBand + 1];  // first run of each band row in the band list
+    __shared__ long long s_wsum[kContourWarps];
+    __shared__ int s_n;                      // contours in the slot's list
+    __shared__ long long s_carry;
+    const int tid = threadIdx.x, lane = tid & (kWarp - 1), warp = tid / kWarp;
+    uint8_t* slot = a.work + (size_t)blockIdx.x * a.slot_bytes;
+    extern __shared__ __align__(16) int8_t s_map[];
+    int2* list = reinterpret_cast<int2*>(slot + a.map_bytes);                 // (map index, length) in trace order
+    int2* runs = reinterpret_cast<int2*>(slot + a.map_bytes + a.list_bytes);  // (start, end) of the band's runs
+    for (int c = blockIdx.x; c < a.n_images * a.max_masks; c += gridDim.x) {
+        const int j = c / a.max_masks, k = c - j * a.max_masks, b = a.base + j;
+        const ContourFrame& f = a.f[j];
+        const size_t canvas_id = (size_t)b * a.max_masks + k;
+        const float* img = a.rows + (size_t)b * (1 + (size_t)a.dets * kRcnnRowFloats);
+        const int count = min((int)img[0], min(a.dets, a.max_masks));  // as rcnn_paste_band
+        int rx = 0, ry = 0, W = 0, H = 0;
+        if (k >= count || !rcnn_mask_rect(img + 1 + (size_t)k * kRcnnRowFloats, f.img_w, f.img_h, rx, ry, W, H)) {
+            if (tid == 0) a.counts[2 * canvas_id] = a.counts[2 * canvas_id + 1] = 0;
+            continue;  // uniform over the CTA
+        }
+        const int stride = W + 2;
+        // the map in shared memory when it fits (the follower's loads and marks then stay on chip), else in the slot
+        int8_t* m = (long long)stride * (H + 2) <= kContourSmem ? s_map : reinterpret_cast<int8_t*>(slot);
+        // A. the padded map of r
+        const uint8_t* src = f.canvas + (size_t)k * f.img_h * f.pitch;
+        for (int y = warp; y < H + 2; y += kContourWarps) {
+            const uint8_t* row = src + (size_t)(ry + y - 1) * f.pitch + rx - 1;
+            int8_t* dst = m + (size_t)y * stride;
+            const bool inner = y >= 1 && y <= H;
+            for (int x = lane; x < stride; x += kWarp) dst[x] = inner && x >= 1 && x <= W && row[x] != 0;
+        }
+        if (tid == 0) s_n = 0;
+        __syncthreads();
+        // B. bands of rows 1 .. H
+        for (int y0 = 1; y0 <= H; y0 += kContourBand) {
+            const int nrows = min(kContourBand, H + 1 - y0);
+            // runs of each row: starts where a nonzero follows a zero, ends before a zero that follows a nonzero (the
+            // map's frame closes every run); counted, then written at the row's offset
+            for (int pass = 0; pass < 2; ++pass) {
+                for (int r = warp; r < nrows; r += kContourWarps) {
+                    const int8_t* row = m + (size_t)(y0 + r) * stride;
+                    int n = pass ? s_off[r] : 0;
+                    int ne = n;
+                    unsigned carry = 0;
+                    for (int x0 = 1; x0 <= W + 1; x0 += kWarp) {
+                        const int x = x0 + lane;
+                        const unsigned bits = __ballot_sync(0xffffffffu, x <= W + 1 && row[x] != 0);
+                        const unsigned left = (bits << 1) | carry;
+                        const unsigned st = bits & ~left, en = ~bits & left;
+                        if (pass) {
+                            const unsigned lt = (1u << lane) - 1u;
+                            if (st >> lane & 1) runs[n + __popc(st & lt)].x = x;
+                            if (en >> lane & 1) runs[ne + __popc(en & lt)].y = x - 1;
+                        }
+                        n += __popc(st);
+                        ne += __popc(en);
+                        carry = bits >> 31;
+                    }
+                    if (!pass && lane == 0) s_off[r + 1] = n;  // counts, summed below
+                }
+                __syncthreads();
+                if (!pass) {
+                    if (tid == 0) {
+                        s_off[0] = 0;
+                        for (int r = 0; r < nrows; ++r) s_off[r + 1] += s_off[r];
+                    }
+                    __syncthreads();
+                }
+            }
+            // warp 0 walks the band's runs in raster order
+            if (warp == 0) {
+                const int nruns = s_off[nrows];
+                int cur = -1, mval = 0, nc = s_n;
+                for (int i0 = 0; i0 < nruns; i0 += kWarp) {
+                    const int i = i0 + lane;
+                    int ry_i = 0, s = 0, e = 0;
+                    if (i < nruns) {
+                        const int2 run = runs[i];
+                        s = run.x;
+                        e = run.y;
+                        while (s_off[ry_i + 1] <= i) ++ry_i;
+                    }
+                    const int8_t* row = m + (size_t)(y0 + ry_i) * stride;
+                    int vs = 0, ve = 0, ve1 = 0;
+                    if (i < nruns) vs = row[s], ve = row[e], ve1 = row[e - 1];
+                    const int cnt = min(kWarp, nruns - i0);
+                    for (int q = 0; q < cnt; ++q) {
+                        const int yq = __shfl_sync(0xffffffffu, ry_i, q), sq = __shfl_sync(0xffffffffu, s, q),
+                                  eq = __shfl_sync(0xffffffffu, e, q);
+                        if (yq != cur) cur = yq, mval = 0;  // lnbd starts on the frame at each row
+                        int vsq = __shfl_sync(0xffffffffu, vs, q);
+                        const bool traced = vsq == 1 && mval <= 0;
+                        if (traced) {
+                            const int y = y0 + yq, i0m = y * stride + sq;
+                            if (lane == 0) {
+                                const int len = contour_follow(m, stride, i0m, sq, y, true, nullptr, 0, 0, 0);
+                                list[nc] = make_int2(i0m, len);
+                            }
+                            ++nc;
+                            __syncwarp();
+                            if (i < nruns) vs = row[s], ve = row[e], ve1 = row[e - 1];  // the trace marked the map
+                            vsq = __shfl_sync(0xffffffffu, vs, q);
+                        }
+                        const int veq = __shfl_sync(0xffffffffu, ve, q), ve1q = __shfl_sync(0xffffffffu, ve1, q);
+                        // lnbd: the last x of the run with a mark and a value change (the traced start itself excluded)
+                        if (eq > sq && is_mark(veq) && veq != ve1q) {
+                            mval = veq;
+                        } else if (eq == sq) {
+                            if (!traced && is_mark(vsq)) mval = vsq;
+                        } else {
+                            const int8_t* rq = m + (size_t)(y0 + yq) * stride;
+                            const int lo = traced ? sq + 1 : sq;
+                            for (int xh = eq; xh >= lo; xh -= kWarp) {
+                                const int x = xh - lane;
+                                const int v = x >= lo ? rq[x] : 0;
+                                const bool hit = x >= lo && is_mark(v) && v != rq[x - 1];
+                                const unsigned h = __ballot_sync(0xffffffffu, hit);
+                                if (h) {
+                                    mval = __shfl_sync(0xffffffffu, v, __ffs(h) - 1);
+                                    break;
+                                }
+                            }
+                        }
+                    }
+                }
+                if (lane == 0) s_n = nc;
+            }
+            __syncthreads();
+        }
+        // C. outputs in descending start order: contour q of the output is list[n - 1 - q]
+        const int n = s_n;
+        if (tid == 0) s_carry = 0;
+        __syncthreads();
+        for (int q0 = 0; q0 < n; q0 += kContourThreads) {
+            const int q = q0 + tid;
+            const int2 cq = q < n ? list[n - 1 - q] : make_int2(0, 0);
+            // exclusive prefix of the lengths over the output order
+            long long v = cq.y;
+#pragma unroll
+            for (int d = 1; d < kWarp; d <<= 1) {
+                const long long u = __shfl_up_sync(0xffffffffu, v, d);
+                if (lane >= d) v += u;
+            }
+            if (lane == kWarp - 1) s_wsum[warp] = v;
+            __syncthreads();
+            long long before = s_carry, chunk = 0;
+            for (int w = 0; w < kContourWarps; ++w) {
+                before += w < warp ? s_wsum[w] : 0;
+                chunk += s_wsum[w];
+            }
+            const long long off = before + v - cq.y;
+            if (q < n) {
+                if (q < a.max_contours) a.lengths[canvas_id * a.max_contours + q] = cq.y;
+                if (off < a.max_points) {
+                    const int y = cq.x / stride, x = cq.x - y * stride;
+                    contour_follow(m, stride, cq.x, x, y, false, a.points + (canvas_id * a.max_points + off) * 2,
+                                   (int)min((long long)cq.y, a.max_points - off), rx - 1, ry - 1);
+                }
+            }
+            __syncthreads();
+            if (tid == 0) s_carry += chunk;
+            __syncthreads();
+        }
+        if (tid == 0) {
+            a.counts[2 * canvas_id] = n;
+            a.counts[2 * canvas_id + 1] = (int)s_carry;
+        }
+        __syncthreads();  // the slot is reused by the next canvas
+    }
+}
+
 // YOLO segmentation post-process: process_mask (above) + draw_mask_bbox's mask selection (yolov8/src/postprocess.cpp:228-248,
 // yolov5/src/postprocess.cpp:148-167), which the reference runs on one host core per image.  For detection k of image b:
 //   M = process_mask's 640^2 mask, S = scale_mask(M) (crop trtx_scale_mask_rect, bilinear to img_w x img_h),
@@ -1123,6 +1385,81 @@ TRTX_API int trtx_rcnn_postprocess_frames_enqueue(const trtx_rcnn_post_params* p
         if (!canvases) continue;
         rcnn_paste_frames_kernel<<<(unsigned)ctas, kPasteThreads, 0, s>>>(a);
         if ((rc = check_launch())) return rc;
+    }
+    return TRTX_OK;
+}
+
+// The slots of a trtx_rcnn_contours_enqueue call and the bytes of one (sized for its largest frame); TRTX_ERR_INVALID /
+// TRTX_ERR_UNSUPPORTED as documented there.
+static int contour_plan(const trtx_rcnn_post_params* p, const trtx_frame* frames, int batch, int& slots,
+                        long long& map_bytes, long long& list_bytes, long long& slot_bytes) {
+    if (!p || !frames || batch <= 0 || p->detections_per_im <= 0 || p->max_masks <= 0) return TRTX_ERR_INVALID;
+    long long band_bytes = 0;
+    map_bytes = list_bytes = 0;
+    for (int i = 0; i < batch; ++i) {
+        const trtx_frame& d = frames[i];
+        if (!d.masks_dev || d.img_w <= 0 || d.img_h <= 0 || d.pitch < d.img_w) return TRTX_ERR_INVALID;
+        if ((long long)(d.img_w + 2) * (d.img_h + 2) > (1LL << 29)) return TRTX_ERR_UNSUPPORTED;
+        long long mb, lb, bb;
+        contour_regions(d.img_w, d.img_h, mb, lb, bb);
+        map_bytes = max(map_bytes, mb);
+        list_bytes = max(list_bytes, lb);
+        band_bytes = max(band_bytes, bb);
+    }
+    slot_bytes = (map_bytes + list_bytes + band_bytes + 255) / 256 * 256;
+    slots = (int)min((long long)min(batch, kMaxFrames) * p->max_masks, (long long)kContourCtas);
+    return TRTX_OK;
+}
+
+TRTX_API size_t trtx_rcnn_contours_workspace_size(const trtx_rcnn_post_params* p, const trtx_frame* images_host, int batch) {
+    int slots;
+    long long map_bytes, list_bytes, slot_bytes;
+    if (contour_plan(p, images_host, batch, slots, map_bytes, list_bytes, slot_bytes)) return 0;
+    return (size_t)slots * (size_t)slot_bytes;
+}
+
+TRTX_API int trtx_rcnn_contours_enqueue(const trtx_rcnn_post_params* p, const trtx_frame* images_host, int batch,
+                                        const float* rows_dev, int max_contours, int max_points, int32_t* counts_dev,
+                                        int32_t* lengths_dev, int32_t* points_dev, void* workspace_dev,
+                                        size_t workspace_bytes, trtx_stream_t stream) {
+    if (!rows_dev || !counts_dev || !lengths_dev || !points_dev || !workspace_dev || max_contours <= 0 || max_points <= 0)
+        return TRTX_ERR_INVALID;
+    if (reinterpret_cast<uintptr_t>(workspace_dev) & 15) return TRTX_ERR_INVALID;
+    int slots;
+    long long map_bytes, list_bytes, slot_bytes;
+    const int rc = contour_plan(p, images_host, batch, slots, map_bytes, list_bytes, slot_bytes);
+    if (rc) return rc;
+    if (workspace_bytes < (size_t)slots * (size_t)slot_bytes) return TRTX_ERR_WORKSPACE;
+    ContourArgs a;
+    a.rows = rows_dev;
+    a.counts = counts_dev;
+    a.lengths = lengths_dev;
+    a.points = points_dev;
+    a.work = static_cast<uint8_t*>(workspace_dev);
+    a.slot_bytes = (size_t)slot_bytes;
+    a.map_bytes = map_bytes;
+    a.list_bytes = list_bytes;
+    a.dets = p->detections_per_im;
+    a.max_masks = p->max_masks;
+    a.max_contours = max_contours;
+    a.max_points = max_points;
+    if (cudaFuncSetAttribute(rcnn_contours_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kContourSmem) !=
+        cudaSuccess) {
+        g_last_cuda_error = (int)cudaGetLastError();
+        return TRTX_ERR_CUDA;
+    }
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {
+        const int n = min(batch - i0, kMaxFrames);
+        for (int j = 0; j < n; ++j) {
+            const trtx_frame& d = images_host[i0 + j];
+            a.f[j] = ContourFrame{d.masks_dev, d.img_w, d.img_h, d.pitch};
+        }
+        a.base = i0;
+        a.n_images = n;
+        rcnn_contours_kernel<<<(unsigned)min(n * p->max_masks, kContourCtas), kContourThreads, kContourSmem, st>>>(a);
+        const int r = check_launch();
+        if (r) return r;
     }
     return TRTX_OK;
 }

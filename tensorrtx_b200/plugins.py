@@ -1225,6 +1225,36 @@ def rcnn_postprocess_frames(scores: torch.Tensor, boxes: torch.Tensor, classes: 
     return rows, canvases
 
 
+def rcnn_contours(rows: torch.Tensor, canvases: Sequence[torch.Tensor], *, frames: Sequence[tuple[int, int]],
+                  detections_per_im: int, max_masks: int, max_contours: int, max_points: int, out=None, stream=None):
+    """cv2.findContours(canvas, RETR_EXTERNAL, CHAIN_APPROX_NONE) of every kept canvas of an rcnn_postprocess(_frames) call
+    (rcnn/rcnn.cpp:551-552), read inside each row's paste rectangle.  rows [B, 1 + D*7] and canvases[b] [max_masks, img_h,
+    img_w] u8 as that call returned them (or views with contiguous rows and slots); frames[b] = (img_w, img_h).
+    -> (counts [B, max_masks, 2] int32: (n_contours, n_points), true totals; lengths [B, max_masks, max_contours] int32;
+    points [B, max_masks, max_points, 2] int32 (x, y)), contours in cv2's order.  Entries past the counts are not written
+    (new tensors start zeroed); `out` = (counts, lengths, points) reuses tensors.  Allocates the workspace."""
+    lib = L.load()
+    B = len(frames)
+    D = int(detections_per_im)
+    if B == 0 or tuple(rows.shape) != (B, 1 + D * 7) or rows.dtype != torch.float32 or not rows.is_contiguous():
+        raise ValueError(f"rows must be contiguous float32 [{B}, {1 + D * 7}]")
+    q = L.RcnnPostParams(0, 0, 0, 0, D, 1, int(max_masks), 0.0)  # only detections_per_im and max_masks are read
+    descs, _ = _frames(frames, canvases, int(max_masks), rows.device, True)
+    shapes = ((B, max_masks, 2), (B, max_masks, max_contours), (B, max_masks, max_points, 2))
+    if out is None:
+        out = tuple(torch.zeros(s, dtype=torch.int32, device=rows.device) for s in shapes)
+    for t, s in zip(out, shapes):
+        if tuple(t.shape) != tuple(s) or t.dtype != torch.int32 or not t.is_contiguous():
+            raise ValueError(f"out tensors must be contiguous int32 {shapes}")
+    n = lib.trtx_rcnn_contours_workspace_size(C.byref(q), descs, B)
+    if n == 0:
+        raise ValueError("trtx_rcnn_contours_workspace_size rejected the arguments")
+    work = torch.empty(n, dtype=torch.uint8, device=rows.device)
+    L.check(lib.trtx_rcnn_contours_enqueue(C.byref(q), descs, B, _ptr(rows), int(max_contours), int(max_points),
+                                           _ptr(out[0]), _ptr(out[1]), _ptr(out[2]), _ptr(work), n, _stream(stream)),
+            "trtx_rcnn_contours_enqueue")
+    return tuple(out)
+
 def letterbox_matrix(src_w: int, src_h: int, dst_w: int, dst_h: int):
     m = (C.c_float * 6)()
     L.load().trtx_letterbox_matrix(src_w, src_h, dst_w, dst_h, m)
