@@ -282,6 +282,10 @@ TRTX_API int trtx_retina_decode_enqueue(const trtx_retina_params* p, int batch, 
  * 4. Faster R-CNN plugins -- same "null workspace returns the size" idiom as the reference
  *    free functions (rcnn/RpnNms.cu:63-80): call with workspace_dev == NULL to get bytes.
  *    All images of the batch are processed in one launch (the reference loops on the host).
+ *    Outputs are the first entries of a stable descending sort of the scores: equal scores (-0.0 and +0.0 included)
+ *    keep ascending input index.  Limits, beyond which a call returns -TRTX_ERR_UNSUPPORTED and writes nothing:
+ *    num_anchors <= 64 and top_n <= 8192 (rpnDecode), pre_nms_topk <= 8192 (rpnNms), num_boxes <= 8192
+ *    (predictorDecode), count <= 4096 (batchedNms).
  * ===================================================================================== */
 /* rpnDecode, rcnn/RpnDecode.cu:27-143.  inputs: scores [B,A,H,W], deltas [B,A*4,H,W];
  * outputs: scores [B,top_n], boxes [B,top_n,4].  anchors_host: A*4 floats (host memory, copied

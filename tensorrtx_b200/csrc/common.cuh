@@ -78,9 +78,12 @@ struct Elem<__half> {
 // (yolov8/plugin/yololayer.cu:174-176).  No fast-math anywhere in this library.
 __device__ __forceinline__ float logist(float x) { return 1.0f / (1.0f + expf(-x)); }
 
-// order-preserving float -> uint32 (larger float => larger key); -0.0 < +0.0 like cub's radix twiddle
+// order-preserving float -> uint32 (larger float => larger key).  -0.0 is mapped to +0.0 first, so the two zeros are one
+// key and tie on the index like any other equal scores -- as in cub's radix sort ("positive and negative zeros are
+// considered equivalent") and the reference's float comparisons.  Keys are only compared, never turned back into floats.
 __device__ __forceinline__ uint32_t float_key(float f) {
     uint32_t b = __float_as_uint(f);
+    b = b == 0x80000000u ? 0u : b;
     return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 

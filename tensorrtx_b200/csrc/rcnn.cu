@@ -190,7 +190,8 @@ __global__ void __launch_bounds__(kSelThreads, 1) rpn_nms_kernel(const __grid_co
     unsigned long long* keys = reinterpret_cast<unsigned long long*>(smem_raw);
     float4* s_box = reinterpret_cast<float4*>(smem_raw + a.key_area);
     float4* s_kbox = reinterpret_cast<float4*>(smem_raw);
-    unsigned char* s_state = reinterpret_cast<unsigned char*>(s_kbox + a.post);  // 0 alive-candidate, 1 kept, 2 dead
+    // 0 alive-candidate, 1 kept, 2 dead, 3 born below -FLT_MAX (-inf) and not yet overlapped by a kept box
+    unsigned char* s_state = reinterpret_cast<unsigned char*>(s_kbox + a.post);
     __shared__ unsigned s_rem, s_sup[32];
     __shared__ int s_nkept;
 
@@ -215,7 +216,7 @@ __global__ void __launch_bounds__(kSelThreads, 1) rpn_nms_kernel(const __grid_co
     }
     __syncthreads();  // keys are dead: the area becomes kept boxes + state
     cnt = 0;
-    for (int r = tid; r < n; r += kSelThreads) s_state[r] = (my_sc[cnt++] > -FLT_MAX) ? 0 : 2;
+    for (int r = tid; r < n; r += kSelThreads, ++cnt) s_state[r] = my_sc[cnt] > -FLT_MAX ? 0 : (my_sc[cnt] < -FLT_MAX ? 3 : 2);
     if (tid == 0) {
         s_nkept = 0;
         s_rem = 0;
@@ -270,25 +271,38 @@ __global__ void __launch_bounds__(kSelThreads, 1) rpn_nms_kernel(const __grid_co
         __syncthreads();
         n_kept = s_nkept;
     }
-    // re-sort + gather (:111-117): kept boxes first (score order), then everything else in sorted position
-    // order (their keys are all -FLT_MAX; the radix sort is stable), truncated to post_nms_topk.
+    // re-sort + gather (:111-117): kept boxes first (score order), then the entries whose score is now -FLT_MAX in
+    // sorted position order (the radix sort is stable), then the -inf entries no kept box overlaps, truncated to
+    // post_nms_topk.  The reference's kernel writes -FLT_MAX into every later entry a kept box overlaps, a -inf one
+    // included, which moves that entry ahead of the other -inf entries in the re-sort.
     const int n_out = min(a.post, n);
     for (int r = tid; r < n_kept; r += kSelThreads) ob[r] = s_kbox[r];
-    if (n_kept < n_out) {
-        // rank of each non-kept entry among non-kept entries = position - #kept before it
-        // (sequential prefix by warp 0 over <= pre entries; only reached when fewer than `post` survive)
+    if (n_kept < n_out) {  // only reached when fewer than `post` survive: the NMS loop above has seen every entry
+        for (int r = tid; r < n; r += kSelThreads) {
+            if (s_state[r] != 3) continue;
+            for (int k = 0; k < n_kept; ++k) {
+                if (iou_plain(s_box[r], s_kbox[k]) > a.thresh) {
+                    s_state[r] = 2;
+                    break;
+                }
+            }
+        }
+        __syncthreads();
+        // rank of each non-kept entry among non-kept entries of its group (sequential prefix by warp 0)
         if (warp == 0) {
             int carry = 0;
-            for (int base = 0; base < n; base += 32) {
-                const int r = base + lane;
-                const bool nk = r < n && s_state[r] != 1;
-                const unsigned m = __ballot_sync(0xffffffffu, nk);
-                if (nk) {
-                    const int pos = n_kept + carry + __popc(m & ((1u << lane) - 1u));
-                    if (pos < n_out) ob[pos] = s_box[r];
+            for (int group = 2; group <= 3 && n_kept + carry < n_out; ++group) {
+                for (int base = 0; base < n; base += 32) {
+                    const int r = base + lane;
+                    const bool nk = r < n && s_state[r] == group;
+                    const unsigned m = __ballot_sync(0xffffffffu, nk);
+                    if (nk) {
+                        const int pos = n_kept + carry + __popc(m & ((1u << lane) - 1u));
+                        if (pos < n_out) ob[pos] = s_box[r];
+                    }
+                    carry += __popc(m);
+                    if (n_kept + carry >= n_out) break;
                 }
-                carry += __popc(m);
-                if (n_kept + carry >= n_out) break;
             }
         }
     }

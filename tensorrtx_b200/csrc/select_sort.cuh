@@ -1,8 +1,8 @@
 // select_sort.cuh -- block-level radix top-k select + bitonic sort, for one 1024-thread CTA.
 //
 // The reference sorts EVERYTHING with cub::DeviceRadixSort::SortPairsDescending (a stable descending
-// sort of fp32 keys with an iota payload: ties keep ascending index) and then uses the first k entries
-// (rcnn/RpnDecode.cu:82, PredictorDecode.cu:75, RpnNms.cu:100, BatchedNms.cu:134).  The same ordered
+// sort of fp32 keys with an iota payload: ties keep ascending index; -0.0 and +0.0 are equal keys) and then uses the
+// first k entries (rcnn/RpnDecode.cu:82, PredictorDecode.cu:75, RpnNms.cu:100, BatchedNms.cu:134).  The same ordered
 // prefix is obtained here by (1) an exact radix SELECT of the k largest (key, lower index first) --
 // 4 histogram passes over the keys plus 4 over the indices of the elements tied at the cut -- and
 // (2) a bitonic SORT of only those k elements in shared memory, keyed by (~key << 32 | index).
