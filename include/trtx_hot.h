@@ -621,6 +621,41 @@ TRTX_API int trtx_rcnn_contours_enqueue(const trtx_rcnn_post_params* p, const tr
                                         int32_t* lengths_dev, int32_t* points_dev, void* workspace_dev,
                                         size_t workspace_bytes, trtx_stream_t stream);
 
+/* =====================================================================================
+ * 8. YOLO classification pre- and post-process
+ *    replaces the HOST batch_preprocess of the cls drivers (yolov8/yolov8_cls.cpp:19-46, the same code in yolo11_cls.cpp and
+ *    yolo26/yolo26_cls.cpp; yolov5/yolov5_cls.cpp:19-36) and the H2D copy of its fp32 batch, and the HOST softmax + topk
+ *    (yolov8_cls.cpp:48-78, yolov5_cls.cpp:38-68, yolo26_cls.cpp:120-135) that run after a D2H copy of every logit.
+ * ===================================================================================== */
+/* batch_preprocess for a whole batch, one launch per <= 64 images: images_host = `batch` u8 HWC BGR descriptors in HOST memory
+ * (trtx_image_desc, any pitch and base alignment, mixed sizes allowed); dst_dev = [batch, 3, net_h, net_w] fp32 planar RGB,
+ * the engine input.  The resize is OpenCV 4.x's 8-bit INTER_LINEAR, bit for bit.
+ *   variant TRTX_YOLO_V8 (yolov8, yolo11, yolo26): the centre square crop Rect((w - m) / 2, (h - m) / 2, m, m), m = min(w, h),
+ *     resized to net_w x net_h, then (float)u * (float)(1 / 255.0) per byte (convertTo(CV_32F, 1 / 255.0));
+ *   variant TRTX_YOLO_V5: preprocess_img's letterbox (the rectangle of trtx_calib_letterbox_rect on a 128-grey canvas), then
+ *     (float)(((float)u / 255.0 - mean) / std) in double with mean = 0.485, 0.456, 0.406 and std = 0.229, 0.224, 0.225 for
+ *     R, G, B.
+ * Every descriptor is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
+ * batch / net sizes <= 0, pitch < 3 * width, an unknown variant or a dst_dev that is not 4-byte aligned; TRTX_ERR_UNSUPPORTED
+ * for a V5 rectangle that is empty (cv::resize throws there, e.g. 1 x 5000) or wider than 4 757 pixels (the kernel's
+ * shared-memory rows; V8 rectangles are net_w wide).  No workspace; can be captured in a CUDA graph. */
+TRTX_API int trtx_cls_preprocess_enqueue(int variant, const trtx_image_desc* images_host, int batch, int net_w, int net_h,
+                                         float* dst_dev, trtx_stream_t stream);
+
+/* softmax + topk per image: logits_dev [batch, num_classes], the engine output.
+ *   softmax = 1 (yolov8, yolo11, yolov5): res_i = expf(x_i) / sum, the sum in float in ascending i (softmax's loop);
+ *   softmax = 0 (yolo26, whose output is already a sigmoid): res_i = x_i.
+ * Outputs: index_dev [batch, k] int32, the first min(k, num_classes) indices in descending res; value_dev [batch, k], res at
+ *   those indices; probs_dev [batch, num_classes], the whole res, or NULL.  Entries past min(k, num_classes) are not written.
+ * Order: descending res with -0.0 == +0.0 and ties in ascending index; +NaN ranks above +inf and -NaN below -inf (an
+ *   overflowing expf gives inf / inf = NaN, an all-underflow row 0 / 0).  The reference's std::sort is unstable there, and
+ *   undefined with a NaN.  expf is CUDA's (within 2 ulp), so res is within a relative 2e-6 of the host's.
+ * TRTX_ERR_INVALID for a null logits / index / value pointer, batch / num_classes / k <= 0 or softmax outside {0, 1};
+ * TRTX_ERR_UNSUPPORTED for num_classes > 8 192; nothing is written then.  One launch, one 1024-thread CTA per image with up
+ * to 96 KB of shared memory, no workspace; can be captured in a CUDA graph. */
+TRTX_API int trtx_cls_postprocess_enqueue(int softmax, int batch, int num_classes, const float* logits_dev, int k,
+                                          int32_t* index_dev, float* value_dev, float* probs_dev, trtx_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

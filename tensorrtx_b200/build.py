@@ -18,7 +18,7 @@ CSRC = PKG / "csrc"
 LIBDIR = PKG / "lib"
 LIB = LIBDIR / "libtrtx_hot.so"
 
-SOURCES = ["yolo_decode.cu", "yolo_scan_pipe.cu", "nms.cu", "retina_decode.cu", "rcnn.cu", "preprocess.cu", "mask.cu", "roi_align.cu", "calib_host.cu"]
+SOURCES = ["yolo_decode.cu", "yolo_scan_pipe.cu", "nms.cu", "retina_decode.cu", "rcnn.cu", "preprocess.cu", "mask.cu", "roi_align.cu", "calib_host.cu", "cls.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -90,7 +90,7 @@ def build(force: bool = False, verbose: bool = False, probe: bool = False, defin
 
 def build_oracle() -> Path:
     """Compile the CPU oracles (test infrastructure) and, when /root/reference exists, oracle/_ref."""
-    for extra in ([], ["-f", "face_obb26.mk"], ["-f", "contours.mk"]):
+    for extra in ([], ["-f", "face_obb26.mk"], ["-f", "contours.mk"], ["-f", "cls.mk"]):
         r = subprocess.run(["make", "-C", str(ROOT / "oracle"), *extra], stdout=subprocess.PIPE, stderr=subprocess.STDOUT,
                            text=True)
         if r.returncode != 0:

@@ -436,8 +436,11 @@ struct RcnnPreArgs {
     int stride;               // int16 per staged row: 3 * the widest rectangle of the launch
 };
 
-__global__ void __launch_bounds__(kRcnnPreThreads) rcnn_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
-                                                                          float* __restrict__ dst) {
+// Stages 1 and 2 of a band, shared by the R-CNN and the classification pre-process kernels; Store is stage 3:
+// Store::run(a, im, y0, rows, k_lo, k_hi, pix, dst) writes band rows [0, rows), and pix(k, i), k_lo <= k < k_hi, is the
+// resized byte i (B, G, R interleaved) of the rectangle's row under band row k.
+template <class Store>
+__device__ __forceinline__ void resize_band(const RcnnPreArgs& a, float* __restrict__ dst) {
     constexpr int R = kRcnnPreBand;
     extern __shared__ __align__(16) int16_t hrows[];  // [slots][a.stride]
     __shared__ int s_row[kRcnnPreSlots];              // source row of each slot
@@ -495,17 +498,19 @@ __global__ void __launch_bounds__(kRcnnPreThreads) rcnn_preprocess_kernel(const 
         }
         __syncthreads();
     }
-    const int L = 3 * a.net_w;  // floats per canvas row
-    const int total = rows * L;
-    float* base = dst + ((size_t)im.dst_idx * a.net_h + y0) * (size_t)L;
-    const int e_lo = 3 * im.x0, e_n = 3 * im.rw;  // row elements [e_lo, e_lo + e_n) lie in the rectangle
-    auto value = [&](int k, int e) -> float {
-        const int i = e - e_lo;
-        if (k < k_lo || k >= k_hi || (unsigned)i >= (unsigned)e_n) return 128.0f;  // the canvas, Scalar(128, 128, 128)
+    auto pix = [&](int k, int i) -> uint32_t {
         const int h0 = hrows[s_slot[k][0] * stride + i], h1 = hrows[s_slot[k][1] * stride + i];
         const int v = (((s_coef[k][0] * h0) >> 16) + ((s_coef[k][1] * h1) >> 16) + 2) >> 2;
-        return u8_to_float_alu((uint32_t)min(max(v, 0), 255));
+        return (uint32_t)min(max(v, 0), 255);
     };
+    Store::run(a, im, y0, rows, k_lo, k_hi, pix, dst);
+}
+
+// Stage 3's stores: the run base[0, total) of a band, float f = element e of band row k of rows of L floats, value(k, e),
+// with 16-byte stores (a head of 0..3 floats up to the first 16-byte boundary and a tail of 0..3 floats are scalar: dst may be
+// only 4-byte aligned).
+template <class Value>
+__device__ __forceinline__ void store_band_run(float* __restrict__ base, int total, int L, Value value) {
     const int head = min((int)(((16u - (unsigned)(reinterpret_cast<uintptr_t>(base) & 15u)) & 15u) >> 2), total);
     const int nvec = (total - head) >> 2, tail0 = head + 4 * nvec;
     if ((int)threadIdx.x < head) base[threadIdx.x] = value(threadIdx.x / L, threadIdx.x % L);
@@ -527,6 +532,133 @@ __global__ void __launch_bounds__(kRcnnPreThreads) rcnn_preprocess_kernel(const 
         *reinterpret_cast<float4*>(base + head + 4 * q) = make_float4(v[0], v[1], v[2], v[3]);
         for (e += step; e >= L; e -= L) ++k;
     }
+}
+
+// R-CNN: HWC, so the band is ONE contiguous run of band * net_w * 3 floats; 128.0f outside the rectangle.
+struct RcnnHwcStore {
+    template <class Pix>
+    static __device__ __forceinline__ void run(const RcnnPreArgs& a, const RcnnPreImage& im, int y0, int rows, int k_lo, int k_hi,
+                                               Pix pix, float* __restrict__ dst) {
+        const int L = 3 * a.net_w;  // floats per canvas row
+        float* base = dst + ((size_t)im.dst_idx * a.net_h + y0) * (size_t)L;
+        const int e_lo = 3 * im.x0, e_n = 3 * im.rw;  // row elements [e_lo, e_lo + e_n) lie in the rectangle
+        store_band_run(base, rows * L, L, [&](int k, int e) -> float {
+            const int i = e - e_lo;
+            if (k < k_lo || k >= k_hi || (unsigned)i >= (unsigned)e_n) return 128.0f;  // the canvas, Scalar(128, 128, 128)
+            return u8_to_float_alu(pix(k, i));
+        });
+    }
+};
+
+__global__ void __launch_bounds__(kRcnnPreThreads) rcnn_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
+                                                                          float* __restrict__ dst) {
+    resize_band<RcnnHwcStore>(a, dst);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// YOLO classification pre-process: batch_preprocess of the cls drivers (yolov8/yolov8_cls.cpp:19-46, the same code in yolo11 and
+// yolo26; yolov5/yolov5_cls.cpp:19-36) into the engine's [B, 3, net_h, net_w] fp32 planar RGB input.  The resize is the band
+// kernel's above, over RcnnPreImage descriptors that the host fills per variant:
+//   TRTX_YOLO_V8: the centre square crop Rect((w - m) / 2, (h - m) / 2, m, m), m = min(w, h), as a descriptor offset (cv::resize
+//                 of a ROI reads only the ROI), resized over the whole net_w x net_h;
+//   TRTX_YOLO_V5: preprocess_img's letterbox (trtx_calib_letterbox_rect) on a 128-grey canvas.
+// Only the store stage is new: the band is three contiguous planar runs of band * net_w floats, R, G, B, each written by
+// store_band_run.  The value of byte u in plane c comes from a per-CTA table of 3 x 256 floats (cls_input_value).
+// dynamic shared memory left beside the table and the band's other static arrays: rectangles up to 4 757 pixels wide
+constexpr size_t kClsMaxDynamicSmem = 227 * 1024 - 3 * 256 * sizeof(float) - 1024;
+
+// The engine input value of byte u in plane c (0 = R, 1 = G, 2 = B).
+//   V8: convertTo(CV_32F, 1 / 255.0), i.e. (float)u * (float)(1 / 255.0), one rounded float product;
+//   V5: ((float)u / 255.0 - mean_c) / std_c in double with the driver's literals (yolov5_cls.cpp:28-30), stored to float.
+// _rn intrinsics: both are IEEE operations that nvcc must not contract.
+__device__ __forceinline__ float cls_input_value(int variant, int c, uint32_t u) {
+    if (variant == TRTX_YOLO_V8) return __fmul_rn((float)u, (float)(1 / 255.0));
+    const double mean = c == 0 ? 0.485 : (c == 1 ? 0.456 : 0.406), std = c == 0 ? 0.229 : (c == 1 ? 0.224 : 0.225);
+    return __double2float_rn(__ddiv_rn(__dsub_rn(__ddiv_rn((double)(float)u, 255.0), mean), std));
+}
+
+template <int kVariant>
+struct ClsPlanarStore {
+    template <class Pix>
+    static __device__ __forceinline__ void run(const RcnnPreArgs& a, const RcnnPreImage& im, int y0, int rows, int k_lo, int k_hi,
+                                               Pix pix, float* __restrict__ dst) {
+        __shared__ float lut[3][256];
+        for (int j = threadIdx.x; j < 3 * 256; j += blockDim.x) lut[j >> 8][j & 255] = cls_input_value(kVariant, j >> 8, j & 255);
+        __syncthreads();
+        const int W = a.net_w;
+#pragma unroll 1
+        for (int c = 0; c < 3; ++c) {
+            const int ch = 2 - c;  // cvtColor BGR2RGB / the driver's planes R, G, B
+            float* base = dst + (((size_t)im.dst_idx * 3 + c) * a.net_h + y0) * (size_t)W;
+            store_band_run(base, rows * W, W, [&](int k, int x) -> float {
+                const int i = x - im.x0;
+                const bool in = k >= k_lo && k < k_hi && (unsigned)i < (unsigned)im.rw;
+                return lut[c][in ? pix(k, 3 * i + ch) : 128u];  // the V5 canvas, Scalar(128, 128, 128)
+            });
+        }
+    }
+};
+
+template <int kVariant>
+__global__ void __launch_bounds__(kRcnnPreThreads) cls_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
+                                                                         float* __restrict__ dst) {
+    resize_band<ClsPlanarStore<kVariant>>(a, dst);
+}
+
+// One launch of `kernel` per kMaxRcnnPreImages frames: make(i, im) fills the band descriptor of frame i (validated before).
+template <class Make>
+static int launch_bands(void (*kernel)(RcnnPreArgs, float*), int batch, int net_w, int net_h, float* dst_dev, size_t smem_max,
+                        cudaStream_t st, Make make) {
+    if (smem_max > 48 * 1024 &&
+        cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) != cudaSuccess) {
+        g_last_cuda_error = (int)cudaGetLastError();
+        return TRTX_ERR_CUDA;
+    }
+    RcnnPreArgs a;
+    a.net_w = net_w;
+    a.net_h = net_h;
+    a.bands = (net_h + kRcnnPreBand - 1) / kRcnnPreBand;
+    for (int i0 = 0; i0 < batch; i0 += kMaxRcnnPreImages) {
+        const int n = batch - i0 < kMaxRcnnPreImages ? batch - i0 : kMaxRcnnPreImages;
+        int wmax = 0;
+        for (int j = 0; j < n; ++j) {
+            RcnnPreImage& im = a.img[j];
+            make(i0 + j, im);
+            im.dst_idx = i0 + j;
+            wmax = im.rw > wmax ? im.rw : wmax;
+        }
+        a.stride = 3 * wmax;
+        const size_t smem = (size_t)kRcnnPreSlots * a.stride * sizeof(int16_t);
+        kernel<<<(unsigned)(n * a.bands), kRcnnPreThreads, smem, st>>>(a, dst_dev);
+        const int rc = check_launch();
+        if (rc) return rc;
+    }
+    return TRTX_OK;
+}
+
+// The band descriptor of frame d for the classification pre-process; false where the reference's cv::resize or copyTo throws
+// (an empty letterbox rectangle, or one that leaves the canvas).
+static bool cls_band_image(int variant, const trtx_image_desc& d, int net_w, int net_h, RcnnPreImage& im) {
+    im.src = d.data_dev;
+    im.sw = d.width;
+    im.sh = d.height;
+    im.pitch = d.pitch;
+    im.x0 = im.y0 = 0;
+    im.rw = net_w;
+    im.rh = net_h;
+    if (variant == TRTX_YOLO_V8) {  // imgs[b](cv::Rect(left, top, m, m)), yolov8_cls.cpp:21-26
+        const int m = d.width < d.height ? d.width : d.height;
+        im.src += (size_t)((d.height - m) / 2) * (size_t)d.pitch + 3 * (size_t)((d.width - m) / 2);
+        im.sw = im.sh = m;
+    } else {
+        int r[4];
+        trtx_calib_letterbox_rect(d.width, d.height, net_w, net_h, r);
+        im.x0 = r[0], im.y0 = r[1], im.rw = r[2], im.rh = r[3];
+        if (im.rw <= 0 || im.rh <= 0 || im.x0 < 0 || im.y0 < 0 || im.x0 + im.rw > net_w || im.y0 + im.rh > net_h) return false;
+    }
+    im.scale_x = 1. / ((double)im.rw / im.sw);
+    im.scale_y = 1. / ((double)im.rh / im.sh);
+    return true;
 }
 
 }  // namespace trtx
@@ -725,44 +857,43 @@ TRTX_API int trtx_rcnn_preprocess_enqueue(const trtx_image_desc* images_host, in
         if (smem > 227 * 1024) return TRTX_ERR_UNSUPPORTED;
         smem_max = smem > smem_max ? smem : smem_max;
     }
-    if (smem_max > 48 * 1024 &&
-        cudaFuncSetAttribute(rcnn_preprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) != cudaSuccess) {
-        g_last_cuda_error = (int)cudaGetLastError();
-        return TRTX_ERR_CUDA;
+    return launch_bands(rcnn_preprocess_kernel, batch, net_w, net_h, dst_dev, smem_max, static_cast<cudaStream_t>(stream),
+                        [&](int i, RcnnPreImage& im) {
+                            const trtx_image_desc& d = images_host[i];
+                            int pads[4];
+                            trtx_rcnn_letterbox_pads(d.width, d.height, net_w, net_h, pads);
+                            im.src = d.data_dev;
+                            im.sw = d.width;
+                            im.sh = d.height;
+                            im.pitch = d.pitch;
+                            im.x0 = pads[0];
+                            im.y0 = pads[2];
+                            im.rw = net_w - (pads[0] + pads[1]);
+                            im.rh = net_h - (pads[2] + pads[3]);
+                            im.scale_x = 1. / ((double)im.rw / d.width);
+                            im.scale_y = 1. / ((double)im.rh / d.height);
+                        });
+}
+
+TRTX_API int trtx_cls_preprocess_enqueue(int variant, const trtx_image_desc* images_host, int batch, int net_w, int net_h,
+                                         float* dst_dev, trtx_stream_t stream) {
+    if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
+    if (variant != TRTX_YOLO_V8 && variant != TRTX_YOLO_V5) return TRTX_ERR_INVALID;
+    if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
+    // every descriptor is checked before the first launch, so that a rejected call writes nothing
+    size_t smem_max = 0;
+    for (int i = 0; i < batch; ++i) {
+        const trtx_image_desc& d = images_host[i];
+        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
+        RcnnPreImage im;
+        if (!cls_band_image(variant, d, net_w, net_h, im)) return TRTX_ERR_UNSUPPORTED;
+        const size_t smem = (size_t)kRcnnPreSlots * 3 * (size_t)im.rw * sizeof(int16_t);
+        if (smem > kClsMaxDynamicSmem) return TRTX_ERR_UNSUPPORTED;
+        smem_max = smem > smem_max ? smem : smem_max;
     }
-    const cudaStream_t st = static_cast<cudaStream_t>(stream);
-    RcnnPreArgs a;
-    a.net_w = net_w;
-    a.net_h = net_h;
-    a.bands = (net_h + kRcnnPreBand - 1) / kRcnnPreBand;
-    for (int i0 = 0; i0 < batch; i0 += kMaxRcnnPreImages) {
-        const int n = batch - i0 < kMaxRcnnPreImages ? batch - i0 : kMaxRcnnPreImages;
-        int wmax = 0;
-        for (int j = 0; j < n; ++j) {
-            const trtx_image_desc& d = images_host[i0 + j];
-            RcnnPreImage& im = a.img[j];
-            int pads[4];
-            trtx_rcnn_letterbox_pads(d.width, d.height, net_w, net_h, pads);
-            im.src = d.data_dev;
-            im.sw = d.width;
-            im.sh = d.height;
-            im.pitch = d.pitch;
-            im.x0 = pads[0];
-            im.y0 = pads[2];
-            im.rw = net_w - (pads[0] + pads[1]);
-            im.rh = net_h - (pads[2] + pads[3]);
-            im.scale_x = 1. / ((double)im.rw / d.width);
-            im.scale_y = 1. / ((double)im.rh / d.height);
-            im.dst_idx = i0 + j;
-            wmax = im.rw > wmax ? im.rw : wmax;
-        }
-        a.stride = 3 * wmax;
-        const size_t smem = (size_t)kRcnnPreSlots * a.stride * sizeof(int16_t);
-        rcnn_preprocess_kernel<<<(unsigned)(n * a.bands), kRcnnPreThreads, smem, st>>>(a, dst_dev);
-        const int rc = check_launch();
-        if (rc) return rc;
-    }
-    return TRTX_OK;
+    auto* kernel = variant == TRTX_YOLO_V8 ? cls_preprocess_kernel<TRTX_YOLO_V8> : cls_preprocess_kernel<TRTX_YOLO_V5>;
+    return launch_bands(kernel, batch, net_w, net_h, dst_dev, smem_max, static_cast<cudaStream_t>(stream),
+                        [&](int i, RcnnPreImage& im) { cls_band_image(variant, images_host[i], net_w, net_h, im); });
 }
 
 }  // extern "C"

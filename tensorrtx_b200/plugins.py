@@ -1162,6 +1162,47 @@ def rcnn_preprocess(images: Sequence[torch.Tensor], net_w: int, net_h: int, out:
     return out
 
 
+def cls_preprocess(images: Sequence[torch.Tensor], variant: int, net_w: int, net_h: int, out: torch.Tensor | None = None,
+                   stream=None) -> torch.Tensor:
+    """GPU drop-in for batch_preprocess of the YOLO cls drivers for a batch of device frames: images[i] is a u8 HWC BGR cuda
+    tensor [h, w, 3] with packed pixels (rows may be pitched, sizes may differ) -> [B, 3, net_h, net_w] float32 planar RGB, the
+    engine input.  variant _lib.YOLO_V8 (yolov8, yolo11, yolo26): centre square crop, resize, / 255; _lib.YOLO_V5 (yolov5): the
+    letterbox on a 128-grey canvas, ImageNet mean / std.  One launch per 64 images, no synchronisation."""
+    lib = L.load()
+    n = len(images)
+    descs = (L.ImageDesc * n)()
+    for i, im in enumerate(images):
+        if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3 or im.stride(2) != 1 or im.stride(1) != 3:
+            raise L.TrtxError("images must be u8 HWC BGR with packed pixels")
+        descs[i].data_dev = im.data_ptr()
+        descs[i].height, descs[i].width = int(im.shape[0]), int(im.shape[1])
+        descs[i].pitch = int(im.stride(0))
+    if out is None:
+        out = torch.empty((n, 3, net_h, net_w), dtype=torch.float32, device=images[0].device if n else "cuda")
+    if out.dtype != torch.float32 or tuple(out.shape) != (n, 3, net_h, net_w):
+        raise ValueError(f"out must be float32 [{n}, 3, {net_h}, {net_w}]")
+    L.check(lib.trtx_cls_preprocess_enqueue(variant, descs, n, net_w, net_h, _ptr(out), _stream(stream)),
+            "trtx_cls_preprocess_enqueue")
+    return out
+
+
+def cls_postprocess(logits: torch.Tensor, k: int, softmax: bool, probs: bool = False, stream=None):
+    """GPU drop-in for the cls drivers' softmax (softmax=True: yolov8, yolo11, yolov5) or raw output (softmax=False: yolo26)
+    and topk(res, k): logits [B, C] float32 cuda -> (index [B, k] int32, value [B, k] float32[, probs [B, C] float32]).  The
+    first min(k, C) entries of each row are written, in descending probability with ties in ascending index; with k > C the
+    rest keep their initial zeros.  One launch, no synchronisation."""
+    if logits.dtype != torch.float32 or logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError("logits must be a contiguous float32 [B, C] tensor")
+    b, c = logits.shape
+    index = torch.zeros((b, k), dtype=torch.int32, device=logits.device)
+    value = torch.zeros((b, k), dtype=torch.float32, device=logits.device)
+    p = torch.empty((b, c), dtype=torch.float32, device=logits.device) if probs else None
+    L.check(L.load().trtx_cls_postprocess_enqueue(int(softmax), b, c, _ptr(logits), k, _ptr(index), _ptr(value),
+                                                  _ptr(p) if p is not None else None, _stream(stream)),
+            "trtx_cls_postprocess_enqueue")
+    return (index, value, p) if probs else (index, value)
+
+
 def rcnn_postprocess(scores: torch.Tensor, boxes: torch.Tensor, classes: torch.Tensor, masks: torch.Tensor | None = None, *,
                      img_w: int, img_h: int, net_w: int, net_h: int, score_thresh: float = 0.6, max_masks: int | None = None,
                      out=None, stream=None):
