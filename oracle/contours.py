@@ -1,4 +1,4 @@
-"""ctypes/numpy wrapper around oracle/libcontours_oracle.so (oracle/contours.mk): the CPU oracle of
+"""ctypes/numpy wrapper around oracle/libcontours_oracle.so: the CPU oracle of
 cv::findContours(img, RETR_EXTERNAL, CHAIN_APPROX_NONE), the outlines the Mask R-CNN driver takes of each pasted canvas
 (rcnn/rcnn.cpp:551-552).
 
@@ -7,10 +7,11 @@ TEST INFRASTRUCTURE ONLY, like oracle/oracle.py: imported by tests/ and tools/, 
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
+
+from . import oracle as _base
 
 HERE = Path(__file__).resolve().parent
 LIB = HERE / "libcontours_oracle.so"
@@ -18,12 +19,9 @@ _lib = None
 
 
 def load():
-    """Open the oracle, first (re)building it with oracle/contours.mk when it is missing or older than its C source."""
     global _lib
     if _lib is None:
-        if not LIB.exists() or LIB.stat().st_mtime < (HERE / "contours_oracle.c").stat().st_mtime:
-            subprocess.run(["make", "-C", str(HERE), "-f", "contours.mk", str(LIB)], check=True, stdout=subprocess.DEVNULL)
-        _lib = C.CDLL(str(LIB))
+        _lib = _base.build_and_open(LIB, "contours_oracle.c")
     return _lib
 
 

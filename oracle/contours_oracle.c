@@ -1,7 +1,7 @@
 /*
  * contours_oracle.c -- CPU ORACLE of cv::findContours(img, RETR_EXTERNAL, CHAIN_APPROX_NONE), the outlines the Mask R-CNN
  * driver takes of each pasted canvas (rcnn/rcnn.cpp:551-552).  TEST INFRASTRUCTURE ONLY, like trtx_oracle.c: plain C,
- * single thread.  Pinned to cv2 by tests/test_rcnn_contours_cpu.py; built by oracle/contours.mk.
+ * single thread.  Pinned to cv2 by tests/test_rcnn_contours_cpu.py; built by oracle/Makefile.
  */
 #include <stdint.h>
 #include <stdlib.h>

@@ -1,4 +1,4 @@
-"""ctypes/numpy wrappers around the reference builds of oracle/face_obb26.mk (present where the reference tree was at build
+"""ctypes/numpy wrappers around two reference builds of oracle/Makefile (present where the reference tree was at build
 time): yolo26's own draw_bbox_obb (oracle/_ref/libref_obb26_host.so) and retina_r50.cpp:373-388's host loop
 (oracle/_ref/libref_retina_rows_host.so).
 
@@ -7,30 +7,23 @@ TEST INFRASTRUCTURE ONLY, like oracle/oracle.py: imported by tests/ and tools/, 
 from __future__ import annotations
 
 import ctypes as C
-from pathlib import Path
+import functools
 
 import numpy as np
 
-HERE = Path(__file__).resolve().parent
-OBB26_LIB = HERE / "_ref" / "libref_obb26_host.so"
-RETINA_ROWS_LIB = HERE / "_ref" / "libref_retina_rows_host.so"
-_libs: dict = {}
+from .golden import RefOutputs
 
 
-def _load(path):
-    if path not in _libs and path.exists():
-        _libs[path] = C.CDLL(str(path))
-    return _libs.get(path)
-
-
+@functools.cache
 def load_obb26():
     """yolo26's compiled draw_bbox_obb (None where oracle/_ref was not built)."""
-    return _load(OBB26_LIB)
+    return RefOutputs.lib("libref_obb26_host.so")
 
 
+@functools.cache
 def load_retina_rows():
     """retina_r50.cpp:373-388's compiled loop, ref_retina_rows (None where oracle/_ref was not built)."""
-    lib = _load(RETINA_ROWS_LIB)
+    lib = RefOutputs.lib("libref_retina_rows_host.so")
     if lib is not None:
         lib.ref_retina_rows.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_double,
                                         C.c_void_p, C.c_void_p]

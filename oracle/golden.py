@@ -73,13 +73,17 @@ class RefOutputs:
         return self._get(key)
 
     def equal(self, key: str, got, ref=None, nan_ok: bool = False, msg="") -> None:
-        """got == the reference output `ref` (computed live) or the stored one, bit for bit."""
+        """got == the reference output `ref` (computed live) or the stored one, bit for bit.  A live `ref` must also match
+        the stored digest, if there is one, so that a stale file fails where it can be recorded again."""
         got = np.asarray(got)
         if ref is not None:
             ref = np.asarray(ref)
             assert np.array_equal(got, ref, equal_nan=nan_ok), (key, msg)
             if self.record is not None:
                 self.record[key] = digest(ref)
+            elif key in self.stored:
+                assert np.array_equal(digest(ref), self.stored[key]), \
+                    f"{key}: the reference's output differs from tests/golden/{self.name}.npz {msg}"
             return
         assert nan_ok or not np.isnan(got.astype(np.float64)).any(), (key, msg)
         assert np.array_equal(digest(got), self._get(key)), f"{key}: differs from the reference's output {msg}"

@@ -7,25 +7,24 @@ TEST INFRASTRUCTURE ONLY, like oracle/oracle.py: imported by tests/, never by th
 from __future__ import annotations
 
 import ctypes as C
-from pathlib import Path
+import functools
 
 import numpy as np
 
-HERE = Path(__file__).resolve().parent
-REF_LIB = HERE / "_ref" / "libref_pose_obb_host.so"
+from .golden import RefOutputs
+
 NUM_KPTS = 17   # kNumberOfPoints of both reference trees
-_ref = None
 
 
+@functools.cache
 def load_ref():
     """The reference's compiled drawing functions (None where oracle/_ref was not built)."""
-    global _ref
-    if _ref is None and REF_LIB.exists():
-        _ref = C.CDLL(str(REF_LIB))
+    ref = RefOutputs.lib("libref_pose_obb_host.so")
+    if ref is not None:
         for fn in ("ref_v8_draw_bbox_obb", "ref_v11_draw_bbox_obb", "ref_v8_draw_bbox_keypoints_line",
                    "ref_v11_draw_bbox_keypoints_line"):
-            getattr(_ref, fn).restype = C.c_int
-    return _ref
+            getattr(ref, fn).restype = C.c_int
+    return ref
 
 
 def _p(a):

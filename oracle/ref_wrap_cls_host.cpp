@@ -1,5 +1,5 @@
 // ref_wrap_cls_host.cpp -- TEST INFRASTRUCTURE.  CPU-only wrapper around one YOLO cls driver compiled where it lies
-// (oracle/cls.mk: -DREF_CLS_DRIVER=<the driver's .cpp> -Dmain=ref_cls_driver_main, against oracle/shim_cls): its own
+// (oracle/Makefile: -DREF_CLS_DRIVER=<the driver's .cpp> -Dmain=ref_cls_driver_main, against oracle/shim_cls): its own
 // batch_preprocess, softmax and topk, called with the test's arguments.
 //   REF_CLS_V5       yolov5_cls.cpp: batch_preprocess calls preprocess_img (yolov5/src/calibrator.cpp, not compiled here); it is
 //                    defined below as the identity, so that the driver's mean / std loop runs over the caller's bytes.

@@ -1,6 +1,6 @@
 // ref_wrap_obb26_host.cpp -- TEST INFRASTRUCTURE.  yolo26's own draw_bbox_obb (get_corner over get_rect_obb, net 1024), run
 // whole on the CPU: yolo26/src/postprocess.cpp is compiled into a namespace of its own against the header shim
-// oracle/shim_pose_obb, whose cv::polylines records the points it is handed.  oracle/face_obb26.mk builds it into
+// oracle/shim_pose_obb, whose cv::polylines records the points it is handed.  oracle/Makefile builds it into
 // oracle/_ref/libref_obb26_host.so.
 #include <cstdint>
 #include <cstring>

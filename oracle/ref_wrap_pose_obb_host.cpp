@@ -3,7 +3,7 @@
 // net 640) or yolo11/src/postprocess.cpp (REF_POSE_OBB_V11: get_corner calls get_rect_obb, net 1024) is compiled into a
 // namespace of its own (the two files define the same names; the namespace also reaches the static get_corner's caller),
 // against the header shim oracle/shim_pose_obb, whose cv::polylines / cv::rectangle record what they are handed.
-// oracle/pose_obb.mk builds this file once per variant and links both objects into oracle/_ref/libref_pose_obb_host.so.
+// oracle/Makefile builds this file once per variant and links both objects into oracle/_ref/libref_pose_obb_host.so.
 #include <dirent.h>
 
 #include <cstdint>

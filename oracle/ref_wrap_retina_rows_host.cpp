@@ -1,6 +1,6 @@
 // ref_wrap_retina_rows_host.cpp -- TEST INFRASTRUCTURE.  The host loop of retinaface/retina_r50.cpp:373-388 over the compact
 // NMS rows of one frame, on the reference's own get_rect_adapt_landmark (retinaface/common.hpp:65-89), for timing against
-// the device face post-process.  oracle/face_obb26.mk builds it into oracle/_ref/libref_retina_rows_host.so.
+// the device face post-process.  oracle/Makefile builds it into oracle/_ref/libref_retina_rows_host.so.
 #include <cstring>
 #include <vector>
 

@@ -1,6 +1,6 @@
 // ref_wrap_seg_host.cpp -- TEST INFRASTRUCTURE.  The reference's own draw_mask_bbox + scale_mask + get_rect, run on the CPU:
 // yolov8/src/postprocess.cpp (REF_SEG_V8) or yolov5/src/postprocess.cpp (REF_SEG_V5) is compiled into a namespace of its
-// own (the two files define the same names), against the header shim oracle/shim_seg; oracle/seg_post.mk builds this file
+// own (the two files define the same names), against the header shim oracle/shim_seg; oracle/Makefile builds this file
 // once per variant and links both objects into oracle/_ref/libref_seg_host.so.
 #include <dirent.h>
 

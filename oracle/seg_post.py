@@ -7,17 +7,17 @@ TEST INFRASTRUCTURE ONLY, like oracle/oracle.py: imported by tests/, never by th
 from __future__ import annotations
 
 import ctypes as C
+import functools
 from pathlib import Path
 
 import numpy as np
 
 from . import oracle as _base
+from .golden import RefOutputs
 
 HERE = Path(__file__).resolve().parent
 LIB = HERE / "libseg_post_oracle.so"
-REF_LIB = HERE / "_ref" / "libref_seg_host.so"
 _lib = None
-_ref = None
 
 
 def load():
@@ -61,13 +61,11 @@ def seg_postprocess(variant, proto, dets, img_w, img_h, *, max_rows, row_floats=
     return rows, canvases, S
 
 
+@functools.cache
 def load_ref():
     """The reference's compiled draw_mask_bbox (None where oracle/_ref was not built)."""
-    global _ref
-    if _ref is None and REF_LIB.exists():
-        _base.load()
-        _ref = C.CDLL(str(REF_LIB))
-    return _ref
+    _base.load()   # libref_seg_host.so links libtrtx_oracle.so through $ORIGIN/..
+    return RefOutputs.lib("libref_seg_host.so")
 
 
 def ref_draw_mask_select(variant, mask, bbox, img_w, img_h):

@@ -1,6 +1,6 @@
 // SHIM, not OpenCV -- TEST INFRASTRUCTURE.  The cv:: names that the YOLO cls drivers (yolov8/yolov8_cls.cpp, yolo11/yolo11_cls.cpp,
 // yolov5/yolov5_cls.cpp, yolo26/yolo26_cls.cpp) and the headers they include mention, so that their batch_preprocess, softmax
-// and topk compile where they lie (oracle/cls.mk, target `ref`).  An image is a (rows, cols, type) header; only a Mat made over
+// and topk compile where they lie (oracle/Makefile, target `ref`).  An image is a (rows, cols, type) header; only a Mat made over
 // caller memory has pixels.  resize, cvtColor, convertTo and split do no pixel work: the shim records the crop rectangle taken
 // from an image and the size cv::resize is asked for (ref_cls_crop_geometry reads them back), and at<T> reads a dummy element.
 #pragma once

@@ -1,4 +1,4 @@
-// SHIM, not OpenCV -- TEST INFRASTRUCTURE for oracle/pose_obb.mk.  Declares the cv:: names the reference's
+// SHIM, not OpenCV -- TEST INFRASTRUCTURE (oracle/Makefile).  Declares the cv:: names the reference's
 // yolov8/src/postprocess.cpp and yolo11/src/postprocess.cpp mention, so that their draw_bbox_keypoints_line and draw_bbox_obb
 // run whole from where they lie.  Only the geometry those functions hand to the drawing calls matters here, so
 // cv::rectangle(img, Rect, ...), cv::circle and cv::polylines RECORD their arguments (cv::shim_record(), cleared by the

@@ -1,5 +1,5 @@
 // SHIM, not OpenCV -- TEST INFRASTRUCTURE.  The cv:: names that the reference's rcnn/common.hpp mentions, so that its
-// preprocessImg (:79-102) compiles where it lies (oracle/rcnn_post.mk, target `ref`) and can be called for its four pads.
+// preprocessImg (:79-102) compiles where it lies (oracle/Makefile, target `ref`) and can be called for its four pads.
 // An image is a (rows, cols, type) header without pixels: resize, the 128-grey canvas and the copy into it do no pixel
 // work, since only the int& pad outputs are read back.
 #pragma once

@@ -1,5 +1,5 @@
 // SHIM, not OpenCV -- TEST INFRASTRUCTURE.  The cv:: names that the reference's rcnn/common.hpp mentions, so that its
-// preprocessImg (:79-110) compiles where it lies (oracle/rcnn_pre.mk, target `ref`).  An image is a (rows, cols, type) header
+// preprocessImg (:79-110) compiles where it lies (oracle/Makefile, target `ref`).  An image is a (rows, cols, type) header
 // without pixels: resize, the 128-grey canvas and the copy into it do no pixel work.  The shim records the size cv::resize is
 // asked for and the rectangle of the canvas that is taken for the copy (ref_rcnn_preprocess_geometry reads them back).
 #pragma once

@@ -1,4 +1,4 @@
-// SHIM, not OpenCV -- TEST INFRASTRUCTURE for oracle/seg_post.mk.  Declares the cv:: names the reference's
+// SHIM, not OpenCV -- TEST INFRASTRUCTURE (oracle/Makefile).  Declares the cv:: names the reference's
 // yolov8/src/postprocess.cpp and yolov5/src/postprocess.cpp mention, so that their draw_mask_bbox + scale_mask + get_rect run
 // from where they lie.  Unlike oracle/shim, the cv::Mat here has real, shared (reference-counted) storage and ROI views with
 // the parent's row step, and cv::resize of a CV_32F image is the oracle's restatement of OpenCV's float bilinear resize

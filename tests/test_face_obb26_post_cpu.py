@@ -8,9 +8,7 @@
 Both live where oracle/_ref was built, else through tests/golden/ref_face_obb26_host.npz.  Also the argument validation of
 trtx_retina_postprocess_enqueue and of the NMS-free OBB task, without a device."""
 import ctypes as C
-import hashlib
 import math
-from pathlib import Path
 
 import numpy as np
 import pytest
@@ -23,7 +21,7 @@ from tensorrtx_b200 import plugins as P
 import test_pose_obb_post_cpu as T
 
 F = np.float32
-GOLDEN = Path(__file__).resolve().parent / "golden" / "ref_face_obb26_host.npz"
+G = RefOutputs("ref_face_obb26_host")
 INPUTS = [(640, 480), (640, 640)]   # retinaface's decodeplugin::INPUT_W x INPUT_H; retinafaceAntiCov's
 SIZES = T.SIZES                     # 11 frame sizes: portrait, landscape, square, extreme aspect, a single pixel
 N_FACE = 600
@@ -76,28 +74,6 @@ def ref_faces(lib, in_w, in_h, img_w, img_h, bb, lmk):
     return rects, mapped
 
 
-def _digest(*arrays):
-    h = hashlib.sha256()
-    for a in arrays:
-        h.update(np.ascontiguousarray(a).tobytes())
-    return np.frombuffer(h.digest(), np.uint8)
-
-
-def face_digests(in_w, in_h, result_of):
-    """sha256 of the rectangles and the landmark bits per frame size; result_of(img_w, img_h, bb, lmk)."""
-    return np.stack([_digest(*result_of(w, h, *face_cases(in_w, in_h, w, h))) for w, h in SIZES])
-
-
-def obb26_digests(corners_of):
-    """sha256 of the corners of every box whose get_rect is defined, per frame size (the cases of
-    test_pose_obb_post_cpu at net 1024); corners_of(img_w, img_h, boxes5)."""
-    return T.obb_digests("v26", 1024, corners_of)
-
-
-def _gold():
-    return np.load(GOLDEN) if GOLDEN.exists() else None
-
-
 def _ref_retina():
     return [(opt, RefOutputs.lib(name)) for opt, name in (("O2", "libref_retina_host.so"), ("O0", "libref_retina_host_O0.so"))
             if RefOutputs.lib(name) is not None]
@@ -108,27 +84,25 @@ def test_retina_get_rect_adapt_landmark_equals_reference_undefined_cases(in_w, i
     """trtx_retina_get_rect_adapt_landmark = the reference's compiled get_rect_adapt_landmark at -O2 and at -O0 on 600 faces
     x 11 frame sizes, every rectangle and every landmark bit, including the corners the reference cannot convert (INT_MIN
     on x86-64) and the widths and heights that overflow (wrap): live where oracle/_ref was built, else the stored digests."""
-    refs, gold = _ref_retina(), _gold()
-    if not refs and gold is None:
-        pytest.skip("neither the reference build nor tests/golden/ref_face_obb26_host.npz")
+    refs = _ref_retina()
     undefined = wrapped = 0
-    for opt, ref in refs:
-        for w, h in SIZES:
-            bb, lmk = face_cases(in_w, in_h, w, h)
+    for w, h in SIZES:
+        bb, lmk = face_cases(in_w, in_h, w, h)
+        got_r, got_k = lib_faces(in_w, in_h, w, h, bb, lmk)
+        key = f"face.{in_w}x{in_h}.{w}x{h}"
+        if not refs:
+            G.equal(key + ".rect", got_r)
+            G.equal(key + ".lmk", got_k.view(np.int32))
+        for opt, ref in refs:
             want_r, want_k = ref_faces(ref, in_w, in_h, w, h, bb, lmk)
-            got_r, got_k = lib_faces(in_w, in_h, w, h, bb, lmk)
-            bad = np.nonzero((want_r != got_r).any(1))[0]
-            assert len(bad) == 0, [(opt, w, h, bb[i].tolist(), want_r[i].tolist(), got_r[i].tolist()) for i in bad[:5]]
-            assert np.array_equal(want_k.view(np.int32), got_k.view(np.int32)), (opt, w, h)
+            G.equal(key + ".rect", got_r, ref=want_r, msg=opt)
+            G.equal(key + ".lmk", got_k.view(np.int32), ref=want_k.view(np.int32), msg=opt)   # bit for bit, NaN payloads too
             undefined += int((got_r[:, :2] == INT_MIN).sum())
             l, t, wd, ht = (got_r[:, k].astype(np.int64) for k in range(4))
             r, b = l + wd, t + ht
             wrapped += int(((r < INT_MIN) | (r > 2 ** 31 - 1) | (b < INT_MIN) | (b > 2 ** 31 - 1)).sum())
     if refs:
         assert undefined > 100 and wrapped > 10, (undefined, wrapped)
-    if gold is not None:
-        assert np.array_equal(gold[f"face_{in_w}x{in_h}"],
-                              face_digests(in_w, in_h, lambda w, h, b, k: lib_faces(in_w, in_h, w, h, b, k)))
 
 
 def test_retina_definitions():
@@ -154,31 +128,18 @@ def test_get_corner_equals_yolo26_draw_bbox_obb():
     cv::polylines, for every box of test_pose_obb_post_cpu's 2,500 x 11 frame sizes whose get_rect is defined (NaN and
     infinite angles, wrapping centres and h >= w swaps included): live where oracle/_ref was built (also yolo26's 3 debug
     lines per box), else the stored digests."""
-    ref, gold = FO.load_obb26(), _gold()
-    if ref is None and gold is None:
-        pytest.skip("neither the reference build nor tests/golden/ref_face_obb26_host.npz")
-    compared = 0
-    if ref is not None:
-        for w, h in SIZES:
-            b = T.obb_boxes(1024, w, h)
-            keep = np.array([T.obb_rect_defined(1024, w, h, x) for x in b])
-            want, log = FO.ref_draw_bbox_obb_v26(w, h, b)
-            got = T.lib_corners(1024, w, h, b)
-            bad = np.nonzero((want != got).any(1) & keep)[0]
-            assert len(bad) == 0, [(w, h, b[i].tolist(), want[i].tolist(), got[i].tolist()) for i in bad[:5]]
-            assert log.count("Original angle: ") == log.count("Adjusted angle: ") == log.count("Normal angle: ") == len(b)
-            compared += int(keep.sum())
-        assert compared > 0.9 * len(SIZES) * T.N_OBB
-    if gold is not None:
-        assert np.array_equal(gold["obb_v26"], obb26_digests(lambda w, h, b: T.lib_corners(1024, w, h, b)))
+    ref = FO.load_obb26()
+    T.check_corners(G, "v26", 1024, None if ref is None else lambda w, h, b: FO.ref_draw_bbox_obb_v26(w, h, b))
 
 
-def test_golden_covers_every_set():
-    gold = _gold()
-    assert gold is not None, "tests/golden/ref_face_obb26_host.npz is missing (tools/make_face_obb26_golden.py)"
-    for key in ("face_640x480", "face_640x640", "obb_v26"):
-        assert gold[key].shape == (len(SIZES), 32)
-    assert not np.array_equal(gold["face_640x480"], gold["face_640x640"])
+def test_inputs_640x480_and_640x640_give_different_faces():
+    """The two input sizes pin different mappings: on the same faces, trtx_retina_get_rect_adapt_landmark at 640x480 and at
+    640x640 differs on every frame size."""
+    for w, h in SIZES:
+        bb, lmk = face_cases(640, 480, w, h)
+        a_r, a_k = lib_faces(640, 480, w, h, bb, lmk)
+        b_r, b_k = lib_faces(640, 640, w, h, bb, lmk)
+        assert not (np.array_equal(a_r, b_r) and np.array_equal(a_k.view(np.int32), b_k.view(np.int32))), (w, h)
 
 
 def test_conf_threshold_as_float():

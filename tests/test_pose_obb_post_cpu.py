@@ -5,18 +5,17 @@ calls record their points: live where oracle/_ref was built, else through tests/
 reference's undefined cases as the library defines them, and the argument validation of
 trtx_yolo_pose_obb_postprocess_enqueue."""
 import ctypes as C
-import hashlib
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 from oracle import pose_obb as PO
+from oracle.golden import RefOutputs
 from tensorrtx_b200 import _lib as L
 from tensorrtx_b200 import plugins as P
 
 F = np.float32
-GOLDEN = Path(__file__).resolve().parent / "golden" / "ref_pose_obb_host.npz"
+G = RefOutputs("ref_pose_obb_host")
 # portrait, landscape, square, extreme aspect, a single pixel
 SIZES = [(1920, 1080), (1080, 1920), (1280, 720), (640, 480), (480, 640), (640, 640), (1024, 1024), (333, 1001),
          (5000, 20), (17, 3000), (1, 1)]
@@ -121,35 +120,20 @@ def lib_landmarks(img_w, img_h, ltrb, kpts, net=640):
     return rects, mapped
 
 
-def _digest(*arrays):
-    h = hashlib.sha256()
-    for a in arrays:
-        h.update(np.ascontiguousarray(a).tobytes())
-    return np.frombuffer(h.digest(), np.uint8)
-
-
-def obb_digests(tree, net, corners_of):
-    """sha256 of the corners of every box whose get_rect is defined, per frame size; corners_of(img_w, img_h, boxes5)."""
-    out = []
+def check_corners(g, tree, net, ref_draw):
+    """trtx_get_corner at `net` = the corners `ref_draw(img_w, img_h, boxes5) -> (corners, printed text)` hands to
+    cv::polylines, for every box whose get_rect is defined, on every frame size: live when ref_draw is given (also the 3
+    debug lines printed per box), else g's stored digests."""
     for w, h in SIZES:
         b = obb_boxes(net, w, h)
         keep = np.array([obb_rect_defined(net, w, h, x) for x in b])
-        out.append(_digest(corners_of(w, h, b)[keep]))
-    return np.stack(out)
-
-
-def pose_digests(tree, result_of):
-    out = []
-    for w, h in SIZES:
-        ltrb, k = pose_boxes(w, h)
-        keep = np.array([rect_defined(640, w, h, x) for x in ltrb])
-        rects, mapped = result_of(w, h, ltrb, k)
-        out.append(_digest(rects[keep], mapped))
-    return np.stack(out)
-
-
-def _gold():
-    return np.load(GOLDEN) if GOLDEN.exists() else None
+        want = None
+        if ref_draw is not None:
+            want, log = ref_draw(w, h, b)
+            want = want[keep]
+            assert log.count("Original angle: ") == log.count("Adjusted angle: ") == log.count("Normal angle: ") == len(b)
+            assert keep.sum() > 0.9 * len(b)
+        g.equal(f"obb.{tree}.{w}x{h}", lib_corners(net, w, h, b)[keep], ref=want)
 
 
 @pytest.mark.parametrize("tree,net", TREES)
@@ -158,24 +142,7 @@ def test_get_corner_equals_reference_draw_bbox_obb(tree, net):
     defined, on 11 frame sizes: live where oracle/_ref was built (also the 3 debug lines printed per box), else the
     stored digests."""
     ref = PO.load_ref()
-    gold = _gold()
-    if ref is None and gold is None:
-        pytest.skip("neither the reference build nor tests/golden/ref_pose_obb_host.npz")
-    compared = 0
-    if ref is not None:
-        for w, h in SIZES:
-            b = obb_boxes(net, w, h)
-            keep = np.array([obb_rect_defined(net, w, h, x) for x in b])
-            want, log = PO.ref_draw_bbox_obb(tree, w, h, b)
-            got = lib_corners(net, w, h, b)
-            bad = np.nonzero((want != got).any(1) & keep)[0]
-            assert len(bad) == 0, [(w, h, b[i].tolist(), want[i].tolist(), got[i].tolist()) for i in bad[:5]]
-            assert log.count("Original angle: ") == log.count("Adjusted angle: ") == log.count("Normal angle: ") == len(b)
-            assert keep.sum() > 0.9 * len(b)
-            compared += int(keep.sum())
-    if gold is not None:
-        assert np.array_equal(gold[f"obb_{tree}"], obb_digests(tree, net, lambda w, h, b: lib_corners(net, w, h, b)))
-    print(f"{tree}: {compared or 'digests of'} boxes equal to the reference's draw_bbox_obb")
+    check_corners(G, tree, net, None if ref is None else lambda w, h, b: PO.ref_draw_bbox_obb(tree, w, h, b))
 
 
 @pytest.mark.parametrize("tree", ["v8", "v11"])
@@ -183,21 +150,18 @@ def test_get_rect_adapt_landmark_equals_reference_draw_bbox_keypoints_line(tree)
     """trtx_get_rect_adapt_landmark = draw_bbox_keypoints_line's rectangle (for boxes whose get_rect is defined) and its
     in-place keypoint mapping (all, NaN and inf included), on 11 frame sizes."""
     ref = PO.load_ref()
-    gold = _gold()
-    if ref is None and gold is None:
-        pytest.skip("neither the reference build nor tests/golden/ref_pose_obb_host.npz")
-    if ref is not None:
-        for w, h in SIZES:
-            ltrb, k = pose_boxes(w, h)
-            keep = np.array([rect_defined(640, w, h, x) for x in ltrb])
+    for w, h in SIZES:
+        ltrb, k = pose_boxes(w, h)
+        keep = np.array([rect_defined(640, w, h, x) for x in ltrb])
+        got_r, got_k = lib_landmarks(w, h, ltrb, k)
+        want_r = want_k = None
+        if ref is not None:
             want_r, want_k = PO.ref_draw_bbox_keypoints_line(tree, w, h, ltrb, k)
-            got_r, got_k = lib_landmarks(w, h, ltrb, k)
-            assert np.array_equal(want_r[keep], got_r[keep]), (w, h)
-            assert np.array_equal(want_k.view(np.int32), got_k.view(np.int32)), (w, h)   # bit for bit, NaN payloads too
+            want_r, want_k = want_r[keep], want_k.view(np.int32)
             # the rectangle is get_rect's V8 branch
             assert all(tuple(got_r[i]) == P.get_rect(w, h, ltrb[i]) for i in range(0, len(ltrb), 7))
-    if gold is not None:
-        assert np.array_equal(gold[f"pose_{tree}"], pose_digests(tree, lib_landmarks))
+        G.equal(f"rect.{tree}.{w}x{h}", got_r[keep], ref=want_r)
+        G.equal(f"kpts.{tree}.{w}x{h}", got_k.view(np.int32), ref=want_k)   # bit for bit, NaN payloads too
 
 
 def test_undefined_cases():
@@ -220,12 +184,12 @@ def test_undefined_cases():
     assert rect == (0, 0, 0, 0) and k == [F(320) / r_w, (F(300) - pad) / r_w, F(0.7)]
 
 
-def test_golden_covers_both_nets():
-    gold = _gold()
-    assert gold is not None, "tests/golden/ref_pose_obb_host.npz is missing (tools/make_pose_obb_golden.py)"
-    for key in ("obb_v8", "obb_v11", "pose_v8", "pose_v11"):
-        assert gold[key].shape == (len(SIZES), 32)
-    assert not np.array_equal(gold["obb_v8"], gold["obb_v11"])   # 640 and 1024 really differ
+def test_nets_640_and_1024_give_different_corners():
+    """The two trees pin different mappings: on the same boxes, get_corner at net 640 and at net 1024 differ (except at
+    1 x 1, where every corner is clamped to (0, 0))."""
+    for w, h in SIZES:
+        b = obb_boxes(640, w, h)
+        assert np.array_equal(lib_corners(640, w, h, b), lib_corners(1024, w, h, b)) == (w * h == 1), (w, h)
 
 
 def _fake(n):
