@@ -16,7 +16,6 @@ of the logits and a synchronise, then softmax + topk per image on one core: the 
 (oracle/_ref/libref_cls_yolov8.so) where they were built, else the C oracle, which restates them."""
 import ctypes as C
 import json
-import subprocess
 import sys
 import time
 from pathlib import Path
@@ -27,43 +26,12 @@ import torch
 ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
 from oracle import cls as CO  # noqa: E402
+from probe_timing import alternating, graph_us, probe_main  # noqa: E402
 from tensorrtx_b200 import _lib as L  # noqa: E402
 from tensorrtx_b200 import plugins as P  # noqa: E402
 
 dev = torch.device("cuda", 0)
 B, NET = 32, 224
-
-
-def graph_us(fn, n=20, reps=20):
-    st = torch.cuda.Stream()
-    with torch.cuda.stream(st):
-        fn()
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            for _ in range(n):
-                fn()
-        for _ in range(3):
-            g.replay()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(reps):
-            g.replay()
-        e1.record()
-        torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / (n * reps) * 1e3
-
-
-def alternating(fns, rounds=3, **kw):
-    """Median over `rounds` of each function's graph time, the functions alternating within a round."""
-    t = [[] for _ in fns]
-    for _ in range(rounds):
-        for i, f in enumerate(fns):
-            t[i].append(graph_us(f, **kw))
-    return [float(np.median(x)) for x in t]
-
-
 MEAN, STD = np.array([0.485, 0.456, 0.406]), np.array([0.229, 0.224, 0.225])
 V5_LUT = ((np.arange(256.0)[:, None] / 255.0 - MEAN[None, :]) / STD[None, :]).astype(np.float32)   # [byte, R/G/B]
 
@@ -109,11 +77,7 @@ def pre_workloads():
 
 
 def main(outdir: Path):
-    outdir.mkdir(parents=True, exist_ok=True)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    res = {"card": torch.cuda.get_device_name(0), "nvidia_smi": q[0] if q else "unavailable",
-           "timing": "20 graph-captured calls x 20 replays between CUDA events, median of 3 alternating rounds",
+    res = {"timing": "20 graph-captured calls x 20 replays between CUDA events, median of 3 alternating rounds",
            "pre": [], "post": []}
     rng = np.random.default_rng(1)
     for name, sizes in pre_workloads():
@@ -135,8 +99,9 @@ def main(outdir: Path):
             out = torch.empty((B, 3, NET, NET), dtype=torch.float32, device=dev)
             nbytes = out.numel() * 4
             fill = torch.empty(nbytes // 4, dtype=torch.float32, device=dev)
-            us, floor_us = alternating([lambda: P.cls_preprocess(d_frames, variant, NET, NET, out=out),
-                                        lambda: fill.fill_(0.5)])
+            tm = alternating({"call": lambda: P.cls_preprocess(d_frames, variant, NET, NET, out=out),
+                              "floor": lambda: fill.fill_(0.5)})
+            us, floor_us = tm["call"], tm["floor"]
             del fill
 
             def device_path():
@@ -191,11 +156,8 @@ def main(outdir: Path):
              "host_over_device": round(best / us, 1)}
         res["post"].append(w)
         print(json.dumps(w), flush=True)
-    (outdir / "cls_probe.json").write_text(json.dumps(res, indent=1) + "\n")
-    print(json.dumps({"card": res["card"], "nvidia_smi": res["nvidia_smi"]}))
+    return res
 
 
 if __name__ == "__main__":
-    if len(sys.argv) != 2:
-        sys.exit("usage: python tools/cls_probe.py OUTDIR")
-    main(Path(sys.argv[1]))
+    probe_main("cls_probe", main)

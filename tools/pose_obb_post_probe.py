@@ -14,7 +14,6 @@ the angle at 7), all frames 1920 x 1080 or a mix of sizes.  Timed:
 The call is latency-bound (a few hundred KB at most), so the figures are microseconds, not a bandwidth share."""
 import json
 import statistics
-import subprocess
 import sys
 import time
 from pathlib import Path
@@ -25,33 +24,13 @@ import torch
 ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
 from oracle import pose_obb as PO  # noqa: E402
+from probe_timing import d2h_sync_us, graph_us, probe_main  # noqa: E402
 from tensorrtx_b200 import _lib as L  # noqa: E402
 from tensorrtx_b200 import plugins as P  # noqa: E402
 
 dev = torch.device("cuda", 0)
 B = 32
 MIXED = [(1920, 1080), (1280, 720), (640, 480), (1080, 1920), (3840, 2160), (333, 1001), (720, 1280), (1024, 1024)]
-
-
-def graph_us(fn, n=20, reps=20):
-    st = torch.cuda.Stream()
-    with torch.cuda.stream(st):
-        fn()
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            for _ in range(n):
-                fn()
-        for _ in range(3):
-            g.replay()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(reps):
-            g.replay()
-        e1.record()
-        torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / (n * reps) * 1e3
 
 
 def inputs(task, K, seed=3):
@@ -74,18 +53,6 @@ def inputs(task, K, seed=3):
     return d, R
 
 
-def d2h_us(dets_d):
-    host = torch.empty(dets_d.shape, dtype=torch.float32, pin_memory=True)
-    ts = []
-    for _ in range(200):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        host.copy_(dets_d, non_blocking=True)
-        torch.cuda.synchronize()
-        ts.append((time.perf_counter() - t0) * 1e6)
-    return statistics.median(ts)
-
-
 def ref_us(task, dets, R, K, sizes):
     if PO.load_ref() is None:
         return None
@@ -103,11 +70,7 @@ def ref_us(task, dets, R, K, sizes):
 
 
 def main(outdir: Path):
-    outdir.mkdir(parents=True, exist_ok=True)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    res = {"card": torch.cuda.get_device_name(0), "nvidia_smi": q[0] if q else "unavailable",
-           "timing": "call: 20 graph-captured launches x 20 replays between CUDA events; d2h: median of 200 host-timed",
+    res = {"timing": "call: 20 graph-captured launches x 20 replays between CUDA events; d2h: median of 200 host-timed",
            "workloads": []}
     for task, name in ((L.TASK_POSE, "pose"), (L.TASK_OBB, "obb")):
         for K in (20, 100):
@@ -119,17 +82,14 @@ def main(outdir: Path):
                 us = graph_us(lambda: P.yolo_pose_obb_postprocess(dets_d, sizes, task=task, max_rows=K, row_floats=R,
                                                                    rows_out=rows))
                 w = {"task": name, "frames": label, "batch": B, "rows_per_frame": K, "in_bytes": dets.nbytes,
-                     "out_bytes": rows.numel() * 4, "call_us": round(us, 2), "d2h_sync_us": round(d2h_us(dets_d), 2)}
+                     "out_bytes": rows.numel() * 4, "call_us": round(us, 2), "d2h_sync_us": round(d2h_sync_us(dets_d), 2)}
                 r = ref_us(task, dets, R, K, sizes)
                 if r is not None:
                     w["ref_host_us"] = round(r, 1)
                 res["workloads"].append(w)
                 print(json.dumps(w), flush=True)
-    (outdir / "pose_obb_post_probe.json").write_text(json.dumps(res, indent=1) + "\n")
-    print(json.dumps({"card": res["card"], "nvidia_smi": res["nvidia_smi"]}))
+    return res
 
 
 if __name__ == "__main__":
-    if len(sys.argv) != 2:
-        sys.exit("usage: python tools/pose_obb_post_probe.py OUTDIR")
-    main(Path(sys.argv[1]))
+    probe_main("pose_obb_post_probe", main)

@@ -13,7 +13,6 @@ CHAIN_APPROX_NONE) per kept canvas on one host thread; median of three.
 Every canvas's counts, lengths and points are checked against the CPU oracle (oracle_find_contours_external)."""
 import ctypes as C
 import json
-import subprocess
 import sys
 import time
 from pathlib import Path
@@ -25,6 +24,7 @@ import torch
 ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
 from oracle import contours as CO  # noqa: E402
+from probe_timing import alternating, probe_main  # noqa: E402
 from tensorrtx_b200 import _lib as L  # noqa: E402
 from tensorrtx_b200 import plugins as P  # noqa: E402
 
@@ -32,27 +32,6 @@ dev = torch.device("cuda", 0)
 B, D, S = 8, 100, 14
 MAX_CONTOURS, MAX_POINTS = 64, 16384
 MIXED = [(640, 480), (480, 640), (1280, 720), (1920, 1080), (1333, 750), (800, 800), (3000, 200), (64, 48)]
-
-
-def graph_us(fn, n=20, reps=20):
-    st = torch.cuda.Stream()
-    with torch.cuda.stream(st):
-        fn()
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            for _ in range(n):
-                fn()
-        for _ in range(3):
-            g.replay()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(reps):
-            g.replay()
-        e1.record()
-        torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / (n * reps) * 1e3
 
 
 def inputs(seed, net_w, net_h, kept):
@@ -112,11 +91,7 @@ def workload(name, frames, net_w, net_h, kept, seed):
     post_call()
     contour_call()
     torch.cuda.synchronize()
-    tm = {"contours": [], "post": []}
-    for _ in range(3):
-        tm["contours"].append(graph_us(contour_call))
-        tm["post"].append(graph_us(post_call))
-    us = {k: float(np.median(v)) for k, v in tm.items()}
+    us = alternating({"contours": contour_call, "post": post_call})
     counts = [min(int(v), D) for v in rows[:, 0].tolist()]
     # every canvas against the oracle
     cnt, ln, pt = (x.cpu().numpy() for x in out)
@@ -140,11 +115,8 @@ def workload(name, frames, net_w, net_h, kept, seed):
 
 
 def main(outdir: Path):
-    outdir.mkdir(parents=True, exist_ok=True)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
     cv2.setNumThreads(1)
-    res = {"card": torch.cuda.get_device_name(0), "nvidia_smi": q[0] if q else "unavailable", "cv2": cv2.__version__,
+    res = {"cv2": cv2.__version__,
            "timing": "20 graph-captured calls x 20 replays between CUDA events, median of 3 alternating rounds",
            "workloads": []}
     for args in (("b8_640x480_kept20", [(640, 480)] * B, 1067, 800, 20, 2),
@@ -154,11 +126,8 @@ def main(outdir: Path):
         w = workload(*args)
         res["workloads"].append(w)
         print(json.dumps(w), flush=True)
-    (outdir / "rcnn_contours_probe.json").write_text(json.dumps(res, indent=1) + "\n")
-    print(json.dumps({"card": res["card"], "nvidia_smi": res["nvidia_smi"]}))
+    return res
 
 
 if __name__ == "__main__":
-    if len(sys.argv) != 2:
-        sys.exit("usage: python tools/rcnn_contours_probe.py OUTDIR")
-    main(Path(sys.argv[1]))
+    probe_main("rcnn_contours_probe", main)

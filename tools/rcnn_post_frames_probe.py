@@ -12,7 +12,6 @@ Timing: 20 calls (or 20 groups of eight calls) captured in one CUDA graph, repla
 variant is timed three times, alternating, and the median is reported.  The floor is a device fill (torch fill_) of the
 canvas bytes the call writes, timed the same way in the same process.  Outputs of the compared variants are checked equal."""
 import json
-import subprocess
 import sys
 from pathlib import Path
 
@@ -21,41 +20,12 @@ import torch
 
 ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
+from probe_timing import alternating, graph_us, probe_main  # noqa: E402
 from tensorrtx_b200 import plugins as P  # noqa: E402
 
 dev = torch.device("cuda", 0)
 B, D, S, KEPT = 8, 100, 14, 20
 MIXED = [(640, 480), (480, 640), (1280, 720), (1920, 1080), (1333, 750), (800, 800), (3000, 200), (64, 48)]
-
-
-def graph_us(fn, n=20, reps=20):
-    st = torch.cuda.Stream()
-    with torch.cuda.stream(st):
-        fn()
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            for _ in range(n):
-                fn()
-        for _ in range(3):
-            g.replay()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(reps):
-            g.replay()
-        e1.record()
-        torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / (n * reps) * 1e3
-
-
-def alternating(fns, rounds=3):
-    """Median over `rounds` of each fn's graph time, the fns timed in turn within each round."""
-    t = {k: [] for k in fns}
-    for _ in range(rounds):
-        for k, fn in fns.items():
-            t[k].append(graph_us(fn))
-    return {k: float(np.median(v)) for k, v in t.items()}
 
 
 def inputs(seed, net_w, net_h):
@@ -133,19 +103,12 @@ def uniform_workload(img_w, img_h, net_w, net_h):
 
 
 def main(outdir: Path):
-    outdir.mkdir(parents=True, exist_ok=True)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    res = {"card": torch.cuda.get_device_name(0), "nvidia_smi": q[0] if q else "unavailable",
-           "timing": "20 graph-captured calls x 20 replays between CUDA events, median of 3 alternating", "workloads": []}
+    res = {"timing": "20 graph-captured calls x 20 replays between CUDA events, median of 3 alternating", "workloads": []}
     for w in (mixed_workload(), uniform_workload(640, 480, 1067, 800), uniform_workload(1920, 1080, 1333, 750)):
         res["workloads"].append(w)
         print(json.dumps(w), flush=True)
-    (outdir / "rcnn_post_frames_probe.json").write_text(json.dumps(res, indent=1) + "\n")
-    print(json.dumps({"card": res["card"], "nvidia_smi": res["nvidia_smi"]}))
+    return res
 
 
 if __name__ == "__main__":
-    if len(sys.argv) != 2:
-        sys.exit("usage: python tools/rcnn_post_frames_probe.py OUTDIR")
-    main(Path(sys.argv[1]))
+    probe_main("rcnn_post_frames_probe", main)

@@ -7,7 +7,6 @@ network input.  Timing: 20 launches captured in one CUDA graph, replayed between
 device fill (torch fill_) of the same byte count, timed the same way in the same process.  The host path's time per batch
 (cv2 per kept detection, one process, as rcnn.cpp:543-550 does it) is given for context and is a CPU number."""
 import json
-import subprocess
 import sys
 import time
 from pathlib import Path
@@ -17,31 +16,11 @@ import torch
 
 ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
+from probe_timing import graph_us, probe_main  # noqa: E402
 from tensorrtx_b200 import plugins as P  # noqa: E402
 
 dev = torch.device("cuda", 0)
 B, D, S = 8, 100, 14
-
-
-def graph_us(fn, n=20, reps=20):
-    st = torch.cuda.Stream()
-    with torch.cuda.stream(st):
-        fn()
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            for _ in range(n):
-                fn()
-        for _ in range(3):
-            g.replay()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(reps):
-            g.replay()
-        e1.record()
-        torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / (n * reps) * 1e3
 
 
 def inputs(seed, kept, net_w, net_h):
@@ -80,11 +59,7 @@ def host_us_per_batch(scores, boxes, masks, img_w, img_h, net_w, net_h):
 
 
 def main(outdir: Path):
-    outdir.mkdir(parents=True, exist_ok=True)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    res = {"card": torch.cuda.get_device_name(0), "nvidia_smi": q[0] if q else "unavailable",
-           "timing": "20 graph-captured launches x 20 replays between CUDA events", "workloads": []}
+    res = {"timing": "20 graph-captured launches x 20 replays between CUDA events", "workloads": []}
     for name, img_w, img_h, net_w, net_h, kept, with_masks in (
             ("b8_640x480_kept20", 640, 480, 1067, 800, 20, True),
             ("b8_640x480_kept100", 640, 480, 1067, 800, 100, True),
@@ -120,11 +95,8 @@ def main(outdir: Path):
     for w in res["workloads"][:-1]:
         w["paste_us_est"] = round(w["us"] - rows_us, 2)
         w["paste_ratio_to_floor_est"] = round(w["paste_us_est"] / w["fill_floor_us"], 3)
-    (outdir / "rcnn_post_probe.json").write_text(json.dumps(res, indent=1) + "\n")
-    print(json.dumps({"card": res["card"], "nvidia_smi": res["nvidia_smi"]}))
+    return res
 
 
 if __name__ == "__main__":
-    if len(sys.argv) != 2:
-        sys.exit("usage: python tools/rcnn_post_probe.py OUTDIR")
-    main(Path(sys.argv[1]))
+    probe_main("rcnn_post_probe", main)

@@ -10,7 +10,6 @@ same way in the same process.  End to end, per batch:
   host path:   what rcnn.cpp:497-506 + :330 do, in one process: cv2.resize, the 128 canvas, astype(float32), then the H2D
                copy of the fp32 batch from pageable memory, timed with a host clock around a device synchronise."""
 import json
-import subprocess
 import sys
 import time
 from pathlib import Path
@@ -20,31 +19,11 @@ import torch
 
 ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
+from probe_timing import graph_us, probe_main  # noqa: E402
 from tensorrtx_b200 import plugins as P  # noqa: E402
 
 dev = torch.device("cuda", 0)
 B = 8
-
-
-def graph_us(fn, n=20, reps=20):
-    st = torch.cuda.Stream()
-    with torch.cuda.stream(st):
-        fn()
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            for _ in range(n):
-                fn()
-        for _ in range(3):
-            g.replay()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(reps):
-            g.replay()
-        e1.record()
-        torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / (n * reps) * 1e3
 
 
 def host_path_us(frames, net_w, net_h, reps=5):
@@ -71,11 +50,7 @@ def host_path_us(frames, net_w, net_h, reps=5):
 
 
 def main(outdir: Path):
-    outdir.mkdir(parents=True, exist_ok=True)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    res = {"card": torch.cuda.get_device_name(0), "nvidia_smi": q[0] if q else "unavailable",
-           "timing": "20 graph-captured calls x 20 replays between CUDA events", "workloads": []}
+    res = {"timing": "20 graph-captured calls x 20 replays between CUDA events", "workloads": []}
     rng = np.random.default_rng(1)
     for name, img_w, img_h, net_w, net_h in (("b8_640x480_to_1067x800", 640, 480, 1067, 800),
                                              ("b8_1920x1080_to_1333x750", 1920, 1080, 1333, 750),
@@ -104,11 +79,8 @@ def main(outdir: Path):
              "host_path_us_per_batch": round(host_us, 1)}
         res["workloads"].append(w)
         print(json.dumps(w), flush=True)
-    (outdir / "rcnn_pre_probe.json").write_text(json.dumps(res, indent=1) + "\n")
-    print(json.dumps({"card": res["card"], "nvidia_smi": res["nvidia_smi"]}))
+    return res
 
 
 if __name__ == "__main__":
-    if len(sys.argv) != 2:
-        sys.exit("usage: python tools/rcnn_pre_probe.py OUTDIR")
-    main(Path(sys.argv[1]))
+    probe_main("rcnn_pre_probe", main)

@@ -12,7 +12,6 @@ two events:
   fill_floor   a device fill (torch fill_) of the canvas bytes."""
 import ctypes as C
 import json
-import subprocess
 import sys
 from pathlib import Path
 
@@ -21,32 +20,12 @@ import torch
 
 ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
+from probe_timing import graph_us, probe_main  # noqa: E402
 from tensorrtx_b200 import _lib as L  # noqa: E402
 from tensorrtx_b200 import plugins as P  # noqa: E402
 
 dev = torch.device("cuda", 0)
 B, K, R, OFF = 8, 20, 39, 7
-
-
-def graph_us(fn, n=20, reps=20):
-    st = torch.cuda.Stream()
-    with torch.cuda.stream(st):
-        fn()
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            for _ in range(n):
-                fn()
-        for _ in range(3):
-            g.replay()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(reps):
-            g.replay()
-        e1.record()
-        torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / (n * reps) * 1e3
 
 
 def inputs(seed, img_w, img_h):
@@ -68,11 +47,7 @@ def inputs(seed, img_w, img_h):
 
 
 def main(outdir: Path):
-    outdir.mkdir(parents=True, exist_ok=True)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    res = {"card": torch.cuda.get_device_name(0), "nvidia_smi": q[0] if q else "unavailable",
-           "timing": "20 graph-captured launches x 20 replays between CUDA events", "workloads": []}
+    res = {"timing": "20 graph-captured launches x 20 replays between CUDA events", "workloads": []}
     for img_w, img_h in ((1920, 1080), (1280, 720), (640, 480)):
         proto, dets = inputs(3, img_w, img_h)
         proto_d, dets_d = torch.from_numpy(proto).to(dev), torch.from_numpy(dets).to(dev)
@@ -117,11 +92,8 @@ def main(outdir: Path):
         res["workloads"].append(w)
         print(json.dumps(w), flush=True)
         del canv
-    (outdir / "seg_post_probe.json").write_text(json.dumps(res, indent=1) + "\n")
-    print(json.dumps({"card": res["card"], "nvidia_smi": res["nvidia_smi"]}))
+    return res
 
 
 if __name__ == "__main__":
-    if len(sys.argv) != 2:
-        sys.exit("usage: python tools/seg_post_probe.py OUTDIR")
-    main(Path(sys.argv[1]))
+    probe_main("seg_post_probe", main)

@@ -24,19 +24,12 @@ import torch
 
 ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
+from probe_timing import card  # noqa: E402
 from tensorrtx_b200 import _lib as L  # noqa: E402
 from tensorrtx_b200 import synth  # noqa: E402
 from tensorrtx_b200.pipeline import DetectionPipeline  # noqa: E402
 
 NET, NC, STRIDES, MAX_OUT, B, R = 640, 80, (8, 16, 32), 1000, 32, 4
-
-
-def card() -> str:
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                              capture_output=True, text=True, timeout=30).stdout.strip()
-    except Exception as e:
-        return f"unknown ({type(e).__name__})"
 
 
 def tune_all(pipes, cand) -> None:
@@ -142,7 +135,7 @@ def main():
         print(line, flush=True)
         log.write(line + "\n")
         log.flush()
-    emit({"card": card(), "head_dtype": args.head_dtype})
+    emit({**card(), "head_dtype": args.head_dtype})
     ceiling = ROOT / "tools" / "lb_ceiling"
     if ceiling.exists():
         r = subprocess.run([str(ceiling)], capture_output=True, text=True, timeout=300)
