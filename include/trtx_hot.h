@@ -105,8 +105,6 @@ typedef struct trtx_yolo_params {
     int32_t tune_class_slices;   /* warps of a CTA splitting the class range: 1, 2, 4, 8; 0 = 4 (fp32 inputs, 4 anchors per lane), else 2 */
     int32_t tune_rows_in_flight; /* channel rows loaded per group; 0 = 10 (fp32 inputs with 4 anchors per lane, fp16 inputs with 8), else 5.  Built (slices, rows): (1,8) (1,16) (2,4) (2,5)
                                     (2,8) (2,10) (2,20) (4,4) (4,5) (4,10) (4,20) (8,5) (8,10) */
-    int32_t tune_tma_pipeline;   /* 1: persistent TMA-fed scan (v8 layout, 16-byte aligned levels); 0 = register scan */
-    int32_t tune_tma_stages;     /* cap on its pipeline stages; 0 = as many as fit (15) */
     int32_t tune_box_prefetch;   /* box rows of a tile: 1 on demand, 2 L2 prefetch, 3 into registers up front; 0 = 2 */
 } trtx_yolo_params;
 
@@ -371,20 +369,14 @@ TRTX_API int trtx_scale_mask_enqueue(const float* masks_dev, int n, int net_w, i
 /* RoIAlign and MaskRcnnInference (SURVEY 8f rank 2): replace roiAlign (rcnn/RoiAlign.cu:150-183) and maskRcnnInference
  * (rcnn/MaskRcnnInference.cu:35-63); same argument meaning, whole batch in one launch, no cudaDeviceSynchronize().
  * rois_dev [batch, num_proposals, 4] x1,y1,x2,y2; features_dev [batch, out_channels, feature_h, feature_w];
- * out_dev [batch, num_proposals, out_channels, pooler_resolution, pooler_resolution].  sampling_ratio <= 0: adaptive. */
+ * out_dev [batch, num_proposals, out_channels, pooler_resolution, pooler_resolution].  sampling_ratio <= 0: adaptive.
+ * The library picks the kernel from the shape; both are bit-identical to the reference's roiAlign.  The reference's
+ * configuration class (pooler_resolution 14, out_channels % 4 == 0, feature_h * feature_w <= 4096) stages each proposal's
+ * feature-map window in shared memory and takes the bilinear taps from there; any other shape takes every tap from global
+ * memory. */
 TRTX_API int trtx_roi_align(int batch, const float* rois_dev, const float* features_dev, float* out_dev, int pooler_resolution,
                             float spatial_scale, int sampling_ratio, int num_proposals, int out_channels, int feature_h,
                             int feature_w, trtx_stream_t stream);
-/* The same with the kernel chosen by the caller (both are bit-identical to the reference's roiAlign):
- * TRTX_ROI_WINDOW (what trtx_roi_align uses) stages each proposal's feature-map window in shared memory and takes the
- * bilinear taps from there -- for the reference's configuration class: pooler_resolution 14, out_channels % 4 == 0,
- * feature_h * feature_w <= 4096; any other shape runs TRTX_ROI_DIRECT, which takes every tap from global memory (the
- * round-1 kernel). */
-#define TRTX_ROI_WINDOW 0
-#define TRTX_ROI_DIRECT 1
-TRTX_API int trtx_roi_align_ex(int batch, const float* rois_dev, const float* features_dev, float* out_dev, int pooler_resolution,
-                               float spatial_scale, int sampling_ratio, int num_proposals, int out_channels, int feature_h,
-                               int feature_w, int mode, trtx_stream_t stream);
 /* indices_dev [batch, detections_per_im] class index as float; masks_dev [batch, detections_per_im, num_classes, S, S];
  * out_dev [batch, detections_per_im, S, S] = sigmoid of the predicted class' mask (rows with an index outside
  * [0, num_classes) are left untouched, as in the reference). */

@@ -16,7 +16,6 @@ YOLO_V8, YOLO_V5, YOLO_V3, YOLO_V26 = 0, 1, 2, 3
 F32, F16 = 0, 1
 BOX_LTRB, BOX_CXCYWH, BOX_RETINA, BOX_OBB = 0, 1, 2, 3
 NMS_GREEDY, NMS_ONESHOT = 0, 1
-ROI_WINDOW, ROI_DIRECT = 0, 1
 RETINA_FACE, RETINA_ANTICOV = 0, 1
 TASK_POSE, TASK_OBB, TASK_OBB_NMS_FREE = 1, 2, 3
 
@@ -50,8 +49,6 @@ class YoloParams(C.Structure):
         # per-call launch tuning (0 = default); the library holds no global knobs
         ("tune_class_slices", C.c_int32),
         ("tune_rows_in_flight", C.c_int32),
-        ("tune_tma_pipeline", C.c_int32),
-        ("tune_tma_stages", C.c_int32),
         ("tune_box_prefetch", C.c_int32),
     ]
 
@@ -145,7 +142,6 @@ SYMBOLS = {
     "trtx_roi_align": (_i, [_i, _vp, _vp, _vp, _i, C.c_float, _i, _i, _i, _i, _i, _vp]),
     "trtx_calib_letterbox_rect": (_i, [_i, _i, _i, _i, C.POINTER(C.c_int)]),
     "trtx_calib_letterbox_host": (_i, [_vp, _i, _i, C.c_size_t, _i, _i, _vp]),
-    "trtx_roi_align_ex": (_i, [_i, _vp, _vp, _vp, _i, C.c_float, _i, _i, _i, _i, _i, _i, _vp]),
     "trtx_mask_rcnn_inference": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "trtx_process_mask_enqueue": (_i, [C.POINTER(MaskParams), _i, _vp, _vp, _i, _vp, _vp]),
     "trtx_letterbox_matrix": (None, [_i, _i, _i, _i, C.POINTER(C.c_float)]),

@@ -18,7 +18,7 @@ CSRC = PKG / "csrc"
 LIBDIR = PKG / "lib"
 LIB = LIBDIR / "libtrtx_hot.so"
 
-SOURCES = ["yolo_decode.cu", "yolo_scan_pipe.cu", "nms.cu", "retina_decode.cu", "rcnn.cu", "preprocess.cu", "mask.cu", "roi_align.cu", "calib_host.cu", "cls.cu"]
+SOURCES = ["yolo_decode.cu", "nms.cu", "retina_decode.cu", "rcnn.cu", "preprocess.cu", "mask.cu", "roi_align.cu", "calib_host.cu", "cls.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -44,23 +44,20 @@ def _stamp(sources: list[Path]) -> str:
     return h.hexdigest()
 
 
-def build(force: bool = False, verbose: bool = False, probe: bool = False, defines: tuple = (), suffix: str = "") -> Path:
+def build(force: bool = False, verbose: bool = False, probe: bool = False) -> Path:
     """Compile every CUDA source for sm_90a into tensorrtx_b200/lib/libtrtx_hot.so.
     probe=True builds libtrtx_hot_probe.so instead: the same sources with -DTRTX_NMS_PROBE (clock64 phase stamps in
-    nms_kernel + trtx_probe_set_nms_stamps), used by tools/nms_probe.py only.  `defines` + `suffix`: further experiment
-    builds (tools/scan_probe.py), never loaded by the product path."""
+    nms_kernel + trtx_probe_set_nms_stamps), used by tools/nms_probe.py only."""
     srcs = [CSRC / s for s in SOURCES if (CSRC / s).exists()]
     LIBDIR.mkdir(exist_ok=True)
-    if defines:
-        probe = True
-    lib = LIBDIR / f"libtrtx_hot_probe{suffix}.so" if probe else LIB
+    lib = LIBDIR / "libtrtx_hot_probe.so" if probe else LIB
     stamp_file = lib.with_suffix(".stamp")
-    stamp = _stamp(srcs) + "|" + ",".join(defines)
+    stamp = _stamp(srcs)
     if not force and lib.exists() and stamp_file.exists() and stamp_file.read_text() == stamp:
         return lib
     nvcc = _nvcc()
     objs = []
-    objdir = LIBDIR / (f"obj_probe{suffix}" if probe else "obj")
+    objdir = LIBDIR / ("obj_probe" if probe else "obj")
     objdir.mkdir(exist_ok=True)
     procs = []
     for s in srcs:
@@ -68,8 +65,6 @@ def build(force: bool = False, verbose: bool = False, probe: bool = False, defin
         cmd = [nvcc, *NVCC_FLAGS, "-I", str(ROOT / "include"), "-I", str(CSRC), "-c", str(s), "-o", str(o)]
         if probe:
             cmd.insert(1, "-DTRTX_NMS_PROBE")
-            for d in defines:
-                cmd.insert(1, "-D" + d)
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
         procs.append((s, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))

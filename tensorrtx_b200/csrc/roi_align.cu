@@ -153,8 +153,7 @@ __device__ __forceinline__ void roi_build_tables(const RoiArgs& a, const RoiGeom
     }
 }
 
-// round-1 kernel: every tap is a global load (kept as `mode = 1` of trtx_roi_align_ex and for proposals the window
-// kernel does not tabulate)
+// round-1 kernel: every tap is a global load (the shapes the window kernel does not cover)
 __global__ void __launch_bounds__(256) roi_align_kernel(const __grid_constant__ RoiArgs a) {
     __shared__ AxisTap s_y[kRoiMaxTable], s_x[kRoiMaxTable];
     const int n = blockIdx.x, b = blockIdx.z;
@@ -401,14 +400,13 @@ using namespace trtx;
 
 extern "C" {
 
-TRTX_API int trtx_roi_align_ex(int batch, const float* rois_dev, const float* features_dev, float* out_dev, int pooler_resolution,
-                               float spatial_scale, int sampling_ratio, int num_proposals, int out_channels, int feature_h,
-                               int feature_w, int mode, trtx_stream_t stream) {
+TRTX_API int trtx_roi_align(int batch, const float* rois_dev, const float* features_dev, float* out_dev, int pooler_resolution,
+                            float spatial_scale, int sampling_ratio, int num_proposals, int out_channels, int feature_h,
+                            int feature_w, trtx_stream_t stream) {
     if (batch <= 0 || !rois_dev || !features_dev || !out_dev) return TRTX_ERR_INVALID;
     if (pooler_resolution <= 0 || num_proposals <= 0 || out_channels <= 0 || feature_h <= 0 || feature_w <= 0) return TRTX_ERR_INVALID;
     if (pooler_resolution > kRoiMaxPooled || pooler_resolution * pooler_resolution > 256) return TRTX_ERR_UNSUPPORTED;
     if (batch > 65535) return TRTX_ERR_UNSUPPORTED;
-    if (mode != TRTX_ROI_WINDOW && mode != TRTX_ROI_DIRECT) return TRTX_ERR_INVALID;
     RoiArgs a;
     a.rois = reinterpret_cast<const float4*>(rois_dev);
     a.feat = features_dev;
@@ -422,11 +420,11 @@ TRTX_API int trtx_roi_align_ex(int batch, const float* rois_dev, const float* fe
     a.spatial_scale = spatial_scale;
     dim3 grid(num_proposals, (out_channels + kRoiChannelsPerCta - 1) / kRoiChannelsPerCta, batch);
     if (grid.y > 65535) return TRTX_ERR_UNSUPPORTED;
-    // the window kernel is built (and was validated on hardware) for the 14 x 14 pooler of the reference's heads (rcnn.cpp:43) and
-    // needs a map whose single-channel window fits its shared memory; every other shape (other poolers, channel counts that are
-    // not a multiple of 4 -- code paths no test has run on a GPU) takes the direct kernel
+    // the window kernel is built for the 14 x 14 pooler of the reference's heads (rcnn.cpp:43), takes four channels per
+    // shared-memory load and needs a map whose single-channel window fits its shared memory; every other shape (other
+    // poolers, channel counts that are not a multiple of 4, larger maps) takes the direct kernel
     const bool window_ok = pooler_resolution == 14 && out_channels % 4 == 0 && (long long)feature_h * feature_w <= kRoiWindowFloats / 4;
-    if (mode == TRTX_ROI_DIRECT || !window_ok) {
+    if (!window_ok) {
         roi_align_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
         return check_launch();
     }
@@ -439,13 +437,6 @@ TRTX_API int trtx_roi_align_ex(int batch, const float* rois_dev, const float* fe
     }
     kernel<<<grid, kRoiWindowThreads, smem, static_cast<cudaStream_t>(stream)>>>(a);
     return check_launch();
-}
-
-TRTX_API int trtx_roi_align(int batch, const float* rois_dev, const float* features_dev, float* out_dev, int pooler_resolution,
-                            float spatial_scale, int sampling_ratio, int num_proposals, int out_channels, int feature_h,
-                            int feature_w, trtx_stream_t stream) {
-    return trtx_roi_align_ex(batch, rois_dev, features_dev, out_dev, pooler_resolution, spatial_scale, sampling_ratio, num_proposals,
-                             out_channels, feature_h, feature_w, TRTX_ROI_WINDOW, stream);
 }
 
 TRTX_API int trtx_mask_rcnn_inference(int batch, const float* indices_dev, const float* masks_dev, float* out_dev,

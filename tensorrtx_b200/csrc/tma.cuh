@@ -1,5 +1,5 @@
 // tma.cuh -- mbarrier / TMA (cp.async.bulk.tensor) PTX wrappers and the host-side tensor-map encoder (sm_90a).
-// Shared by the YoloLayer TMA pipeline (yolo_scan_pipe.cu) and the TMA-staged letterbox (preprocess.cu).
+// Used by the TMA-staged letterbox (preprocess.cu).
 #pragma once
 #include <cuda.h>  // CUtensorMap (types only; the encoder is fetched through cudaGetDriverEntryPoint -- no -lcuda)
 
@@ -14,9 +14,6 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t tx) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(tx) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     const uint32_t addr = smem_u32(bar);
@@ -40,9 +37,6 @@ __device__ __forceinline__ void tma_load_3d(void* dst_smem, const CUtensorMap* m
                     smem_u32(dst_smem)),
             "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar))
             : "memory");
-}
-__device__ __forceinline__ void tma_prefetch_map(const CUtensorMap* map) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,

@@ -53,13 +53,6 @@ __device__ __forceinline__ void scan_classes(const T* __restrict__ row0, size_t 
             }
             // replay only the anchors whose running maximum rises (usually one of the four, around a real candidate):
             // U sequential updates for that anchor instead of 4*U for the quad; ONE branch in the common (no hit) case
-#if defined(TRTX_SCAN_PROBE) && TRTX_SCAN_PROBE == 2  // experiment build: streaming + maxima only
-            if (true) {
-                s.bx[0] = fmaxf(s.bx[0], m.x), s.bx[1] = fmaxf(s.bx[1], m.y), s.bx[2] = fmaxf(s.bx[2], m.z), s.bx[3] = fmaxf(s.bx[3], m.w);
-                p += (size_t)U * g;
-                continue;
-            }
-#endif
             if (!((m.x > s.bx[0]) | (m.y > s.bx[1]) | (m.z > s.bx[2]) | (m.w > s.bx[3]))) {
                 p += (size_t)U * g;
                 continue;
@@ -278,9 +271,6 @@ __global__ void __launch_bounds__(32 * SLICES) yolo_v8_scan_kernel(const __grid_
     int total;
     int off = warp_excl_scan(__popc(flags), lane, &total);
     if (lane == 0) a.tile_count[(size_t)b * a.tiles_per_image + t] = total;
-#if defined(TRTX_SCAN_PROBE) && TRTX_SCAN_PROBE == 1  // experiment build: no box decode / record stores
-    flags = 0;
-#endif
     if (flags) {
         if (a.prefetch_box != 3) load_box();
         const size_t slot0 = (size_t)b * a.slots_per_image + L.slot_begin + (size_t)tile * TILE;
@@ -742,19 +732,13 @@ int yolo_fill_args(const trtx_yolo_params* p, int batch, const void* const* inpu
     for (int l = 0; l < p->num_levels; ++l)
         if (!inputs_dev[l]) return TRTX_ERR_INVALID;
     const int vec = p->variant == TRTX_YOLO_V26 ? 1 : yolo_pick_vec(p, inputs_dev);  // V26: 32-anchor tiles
-    // The TMA pipeline scan splits every 128-anchor stage over four warps of 32 anchors, i.e. it runs on the
-    // 32-cell tile layout (the same one as the scalar kernels, which are its fallback).
-    if (p->tune_class_slices < 0 || p->tune_rows_in_flight < 0 || p->tune_tma_stages < 0 || p->tune_box_prefetch < 0 ||
-        p->tune_box_prefetch > 3 || (p->tune_tma_pipeline != 0 && p->tune_tma_pipeline != 1))
+    if (p->tune_class_slices < 0 || p->tune_rows_in_flight < 0 || p->tune_box_prefetch < 0 || p->tune_box_prefetch > 3)
         return TRTX_ERR_INVALID;
-    const bool pipe = p->tune_tma_pipeline && p->variant == TRTX_YOLO_V8 && vec >= 4 && yolo_pipe_supported(p, inputs_dev);
-    YoloLayout L = yolo_layout(p, batch, pipe ? 1 : vec);
-    L.pipe = pipe ? 1 : 0;
+    YoloLayout L = yolo_layout(p, batch, vec);
     // defaults chosen on an H100 for the overlapped step, not for the scan alone (DESIGN.md section 4.1, "Defaults")
     const bool f32x4 = p->in_dtype == TRTX_F32 && vec == 4;  // the benchmark's fp32 heads: 4 x 10
     L.slices = p->tune_class_slices ? p->tune_class_slices : (f32x4 ? 4 : 2);
     L.unroll = p->tune_rows_in_flight ? p->tune_rows_in_flight : (f32x4 || vec == 8 ? 10 : 5);
-    L.pipe_stages = p->tune_tma_stages;
     if (workspace_bytes < L.total_bytes) return TRTX_ERR_WORKSPACE;
     if (reinterpret_cast<uintptr_t>(workspace_dev) % 16 != 0) return TRTX_ERR_INVALID;
     memset(a, 0, sizeof(*a));
@@ -840,10 +824,6 @@ static int launch_v8(const YoloArgs& a, const YoloLayout& L, int grid, cudaStrea
 
 int yolo_scan_launch(const YoloArgs& a, const YoloLayout& L, int in_dtype, int batch, cudaStream_t st) {
     const int grid = batch * L.tiles_per_image;
-    if (L.pipe) {
-        const int rc = yolo_scan_pipe_launch(a, L, in_dtype, batch, st);
-        if (rc != TRTX_ERR_UNSUPPORTED) return rc;  // else: scalar kernels on the same 32-cell layout
-    }
     if (a.variant == TRTX_YOLO_V26) {
         const int Cp = a.C | 1;
         int wpc = 4;

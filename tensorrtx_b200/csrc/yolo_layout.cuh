@@ -51,8 +51,7 @@ struct YoloArgs {
 
 struct YoloLayout {
     int vec;
-    int pipe;  // 1: the TMA pipeline scan runs on this layout (tile_cells = 32, four tiles per 128-anchor stage)
-    int slices, unroll, pipe_stages;  // launch tuning resolved from trtx_yolo_params.tune_* (per call, no global state)
+    int slices, unroll;  // launch tuning resolved from trtx_yolo_params.tune_* (per call, no global state)
     int tile_cells;
     int apc;
     int tiles_per_image;
@@ -158,8 +157,5 @@ int yolo_pick_vec(const trtx_yolo_params* p, const void* const* inputs_dev);
 int yolo_fill_args(const trtx_yolo_params* p, int batch, const void* const* inputs_dev, void* workspace_dev,
                    size_t workspace_bytes, YoloArgs* a, YoloLayout* L);
 int yolo_scan_launch(const YoloArgs& a, const YoloLayout& L, int in_dtype, int batch, cudaStream_t stream);
-// TMA-pipelined scan (yolo_scan_pipe.cu); returns TRTX_ERR_UNSUPPORTED when the shape does not fit it
-int yolo_scan_pipe_launch(const YoloArgs& a, const YoloLayout& L, int in_dtype, int batch, cudaStream_t stream);
-bool yolo_pipe_supported(const trtx_yolo_params* p, const void* const* inputs_dev);
 
 }  // namespace trtx

@@ -43,11 +43,10 @@ def _stream(stream=None) -> int:
     return int(stream)
 
 
-def _tune(params, slices: int = 0, rows: int = 0, tma: int = 0, stages: int = 0, box: int = 0) -> None:
+def _tune(params, slices: int = 0, rows: int = 0, box: int = 0) -> None:
     """Per-plugin launch tuning of the scan kernel (trtx_yolo_params.tune_*; 0 = default).  Plain data inside the
     plugin's own parameter block -- nothing global, clones / other plugins are unaffected."""
-    params.tune_class_slices, params.tune_rows_in_flight = int(slices), int(rows)
-    params.tune_tma_pipeline, params.tune_tma_stages, params.tune_box_prefetch = int(tma), int(stages), int(box)
+    params.tune_class_slices, params.tune_rows_in_flight, params.tune_box_prefetch = int(slices), int(rows), int(box)
 
 
 def float_le_threshold(x: float) -> float:
@@ -1011,15 +1010,10 @@ class RoiAlignPlugin:
     def getWorkspaceSize(self, maxBatchSize: int) -> int:
         return 0
 
-    def enqueue(self, batchSize, inputs, outputs, workspace=None, stream=None, mode: int | None = None) -> int:
-        """mode: None = trtx_roi_align (the window kernel); L.ROI_WINDOW / L.ROI_DIRECT pick the kernel (trtx_roi_align_ex)."""
-        if mode is None:
-            return int(self._lib.trtx_roi_align(batchSize, _ptr(inputs[0]), _ptr(inputs[1]), _ptr(outputs[0]), self._pooler_resolution,
-                                                self._spatial_scale, self._sampling_ratio, self._num_proposals, self._out_channels,
-                                                self._feature_h, self._feature_w, _stream(stream)))
-        return int(self._lib.trtx_roi_align_ex(batchSize, _ptr(inputs[0]), _ptr(inputs[1]), _ptr(outputs[0]), self._pooler_resolution,
-                                               self._spatial_scale, self._sampling_ratio, self._num_proposals, self._out_channels,
-                                               self._feature_h, self._feature_w, int(mode), _stream(stream)))
+    def enqueue(self, batchSize, inputs, outputs, workspace=None, stream=None) -> int:
+        return int(self._lib.trtx_roi_align(batchSize, _ptr(inputs[0]), _ptr(inputs[1]), _ptr(outputs[0]), self._pooler_resolution,
+                                            self._spatial_scale, self._sampling_ratio, self._num_proposals, self._out_channels,
+                                            self._feature_h, self._feature_w, _stream(stream)))
 
 
 class MaskRcnnInferencePlugin:

@@ -77,7 +77,7 @@ def test_yolov8_plugin_vs_reference_kernel(dev, seed, B):
 def test_yolov8_near_ulp_sigmoid_collisions_vs_reference_kernel(dev):
     """Logits a few ulps apart: whether two of them round to the same probability (-> the EARLIER class wins the
     reference's strict `p > max`) depends on expf itself, so this is checked against the reference kernel (same CUDA
-    expf), for every scan variant (class slices merge their running state; the TMA pipeline replays from smem)."""
+    expf), for several scan variants (class slices merge their running state)."""
     lib = G.lib("libref_yolov8.so")
     heads = synth.yolov8_heads(1, seed=430, n_obj=0)
     h = heads[0]
@@ -97,12 +97,12 @@ def test_yolov8_near_ulp_sigmoid_collisions_vs_reference_kernel(dev):
     ref = _ref_v8(lib, hd, 1, dev)
     r = _rows(ref, 0, 90, slice(0, 6))
     plug = P.YoloLayerPlugin(80, 17, 0.0, 640, 640, 1000, False, False, False, (8, 16, 32))
-    for pipe, slices, unroll in ((1, 2, 5), (0, 2, 5), (0, 4, 10), (0, 1, 8), (0, 8, 5)):
-        plug.tune(tma=pipe, slices=slices, rows=unroll)
+    for slices, unroll in ((2, 5), (4, 10), (1, 8), (8, 5)):
+        plug.tune(slices=slices, rows=unroll)
         got = _ours_decode(plug, hd, 1, dev)
         G.equal("v8_ulp.count", got[:, 0], None if ref is None else ref[:, 0])
         g = _rows(got, 0, 90, slice(0, 6))
-        G.equal("v8_ulp.rows", g, r, msg=(pipe, slices, unroll))
+        G.equal("v8_ulp.rows", g, r, msg=(slices, unroll))
         assert len(g) >= 6 * 24
         assert (g[:, 5] == 60).any() and (g[:, 5] != 60).any()     # both outcomes occur
 
@@ -308,20 +308,25 @@ def test_roi_align_and_mask_rcnn_inference_vs_reference_functions(dev, oracle):
     rois[1, 1] = [0, 0, 1067, 800]           # the whole map: the window of a channel is 50 x 67 cells (several passes)
     rois[1, 2] = [5, 5, 9, 9]                # a fraction of one cell
     rois[1, 3] = [1060, 790, 1200, 900]      # hangs over the bottom-right corner
+    # trtx_roi_align picks the kernel from the shape: 80 channels of the 50 x 67 map take the shared-memory window kernel,
+    # 78 channels (not a multiple of 4) and a 70 x 67 map (more than 4096 cells) the direct kernel
+    feat70 = np.random.default_rng(471).standard_normal((B, Cc, 70, W)).astype(np.float32)
+    shapes = {"": fd, ".c78": fd[:, :78].contiguous(), ".70x67": torch.from_numpy(feat70).to(dev)}
     for sampling in (0, 2, 5, 19):           # 19: 14 * 19 = 266 table entries per axis > 256 -> coordinates on the fly
-        r = None
-        if lib is not None:
-            ref = torch.zeros((B, N, Cc, Pp, Pp), device=dev)
-            assert lib.ref_roi_align(B, C.c_void_p(rd.data_ptr()), C.c_void_p(fd.data_ptr()), C.c_void_p(ref.data_ptr()), Pp,
-                                     C.c_float(1 / 16), sampling, N, Cc, H, W) == 0
-            r = ref.cpu().numpy()
-        plug = P.RoiAlignPlugin(Pp, 1 / 16, sampling, N, Cc)
-        plug.configurePlugin([(N, 4), (Cc, H, W)])
-        for mode in (None, L.ROI_WINDOW, L.ROI_DIRECT):  # the shared-memory window kernel (default) and the round-1 kernel
-            got = torch.full((B, N, Cc, Pp, Pp), -3.0, device=dev)
-            assert plug.enqueue(B, [rd, fd], [got], mode=mode) == 0
+        for tag, f in shapes.items():
+            _, c, fh, fw = f.shape
+            r = None
+            if lib is not None:
+                ref = torch.zeros((B, N, c, Pp, Pp), device=dev)
+                assert lib.ref_roi_align(B, C.c_void_p(rd.data_ptr()), C.c_void_p(f.data_ptr()), C.c_void_p(ref.data_ptr()), Pp,
+                                         C.c_float(1 / 16), sampling, N, c, fh, fw) == 0
+                r = ref.cpu().numpy()
+            plug = P.RoiAlignPlugin(Pp, 1 / 16, sampling, N, c)
+            plug.configurePlugin([(N, 4), (c, fh, fw)])
+            got = torch.full((B, N, c, Pp, Pp), -3.0, device=dev)
+            assert plug.enqueue(B, [rd, f], [got]) == 0
             torch.cuda.synchronize()
-            G.equal(f"roi_align.{sampling}", got.cpu().numpy(), r, nan_ok=True, msg=(sampling, mode))   # bit-identical, NaNs included
+            G.equal(f"roi_align{tag}.{sampling}", got.cpu().numpy(), r, nan_ok=True, msg=(sampling, tag))   # bit-identical, NaNs included
         if sampling > 2:
             continue
         # CPU restatement (no FMA contraction) on proposals inside the feature map: at the `x > width -> 0` border of
@@ -329,6 +334,7 @@ def test_roi_align_and_mask_rcnn_inference_vs_reference_functions(dev, oracle):
         # comparison above can pin
         orc = oracle.roi_align(rois_in, feat[1], Pp, 1 / 16, sampling)
         got_in = torch.empty((1, N, Cc, Pp, Pp), device=dev)
+        plug = P.RoiAlignPlugin(Pp, 1 / 16, sampling, N, Cc, H, W)
         assert plug.enqueue(1, [torch.from_numpy(rois_in).to(dev), fd[1:2].contiguous()], [got_in]) == 0
         np.testing.assert_allclose(got_in[0].cpu().numpy(), orc, rtol=0, atol=2e-5)
     # MaskRcnnInference

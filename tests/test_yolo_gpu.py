@@ -159,24 +159,9 @@ def test_v8_unbuilt_tuning_is_refused_and_tunings_are_per_plugin(oracle, dev):
     ws = torch.empty(bad.getWorkspaceSize(2), dtype=torch.uint8, device=dev)
     assert bad.enqueue(2, hd, [out], ws) == L.ERR_UNSUPPORTED
     a = P.YoloLayerPlugin(80, 17, 0.0, 640, 640, 1000, False, False, False, (8, 16, 32)).tune(slices=4, rows=10, box=3)
-    b = P.YoloLayerPlugin(80, 17, 0.0, 640, 640, 1000, False, False, False, (8, 16, 32)).tune(tma=1, stages=3)
+    b = P.YoloLayerPlugin(80, 17, 0.0, 640, 640, 1000, False, False, False, (8, 16, 32)).tune(slices=2, rows=5, box=1)
     for plug in (a, b, a, b):
         _check_rows(_decode_gpu(plug, hd, 2, dev), ref, 2, 90, 6, 1000)
-
-
-@pytest.mark.parametrize("consumers", [2, 3, 15])  # cap on pipeline stages
-@pytest.mark.parametrize("dtype", ["f32", "f16"])
-@pytest.mark.parametrize("B", [1, 7, 40])
-def test_v8_tma_pipeline_scan(oracle, dev, consumers, dtype, B):
-    """The persistent TMA-fed scan (yolo_scan_pipe.cu): every CTA loops over many tiles, stages wrap around."""
-    heads = synth.yolov8_heads(B, seed=13 + B, n_obj=40)
-    if dtype == "f16":
-        heads = [h.astype(np.float16).astype(np.float32) for h in heads]
-    ref, _ = oracle.yolov8_decode(heads)
-    plug = P.YoloLayerPlugin(80, 17, 0.0, 640, 640, 1000, False, False, False, (8, 16, 32),
-                             in_dtype=L.F16 if dtype == "f16" else L.F32).tune(tma=1, stages=consumers)
-    got = _decode_gpu(plug, _to_dev(heads, dev, torch.float16 if dtype == "f16" else torch.float32), B, dev)
-    _check_rows(got, ref, B, 90, 6, 1000)
 
 
 def test_first_argmax_on_sigmoid_collisions(oracle, dev):
@@ -189,8 +174,8 @@ def test_first_argmax_on_sigmoid_collisions(oracle, dev):
     h[0, 4 + 20, 200] = 6.0000  # exact tie -> first class wins
     ref, _ = oracle.yolov8_decode(heads)
     plug = P.YoloLayerPlugin(80, 17, 0.0, 640, 640, 1000, False, False, False, (8, 16, 32))
-    for pipe, slices, unroll in ((1, 2, 5), (0, 2, 5), (0, 4, 10), (0, 1, 8)):
-        plug.tune(tma=pipe, slices=slices, rows=unroll)
+    for slices, unroll in ((2, 5), (4, 10), (1, 8)):
+        plug.tune(slices=slices, rows=unroll)
         got = _decode_gpu(plug, _to_dev(heads, dev), 1, dev)
         assert got[0, 0] == ref[0, 0] == 2
         g = got[0, 1:181].reshape(2, 90)

@@ -46,12 +46,9 @@ for data, nobj in (("dense", 64), ("background", 0)):
     for dt, ss, nb in ((L.F32, sets, nbytes), (L.F16, sets16, nbytes // 2)):
         plug = P.YoloLayerPlugin(80, 17, 0.0, 640, 640, 1000, False, False, False, (8, 16, 32), in_dtype=dt)
         fused = P.FusedYoloDecodeNms(plug, B, device=dev)
-        for slices, unroll in [(-1, 15), (-1, 10), (1, 8), (1, 16), (2, 4), (2, 5), (2, 8), (2, 10), (2, 20), (4, 4), (4, 5), (4, 10), (4, 20), (8, 5), (8, 10)]:
+        for slices, unroll in [(1, 8), (1, 16), (2, 4), (2, 5), (2, 8), (2, 10), (2, 20), (4, 4), (4, 5), (4, 10), (4, 20), (8, 5), (8, 10)]:
             for box in ((2, 3) if slices == 2 and unroll == 5 else (0,)):
-                if slices < 0:   # TMA pipeline kernel, `unroll` = cap on stages (= consumer warps)
-                    plug.tune(tma=1, stages=unroll)
-                else:
-                    plug.tune(slices=slices, rows=unroll, box=box)
+                plug.tune(slices=slices, rows=unroll, box=box)
                 us = graph_us(lambda i: fused.enqueue_scan(B, ss[i % R]))
                 print(json.dumps({"data": data, "dtype": "f32" if dt == L.F32 else "f16", "slices": slices, "rows": unroll, "box": box,
                                   "us": round(us, 2), "GBps": round(nb / us / 1e3, 1)}), flush=True)
