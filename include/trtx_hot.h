@@ -155,7 +155,9 @@ typedef struct trtx_nms_params {
                             so that the float compare equals the reference's double compare) */
     float nms_thresh;    /* kNmsThresh 0.45 / 0.4 */
     int32_t max_det;     /* K: rows of the compact output per image (kMaxNumOutputBbox) */
-    int32_t class_aware; /* 1: only same-class rows interact (yolo); 0: single class (retinaface) */
+    int32_t class_aware; /* 1: only same-class rows interact (yolo); 0: single class (retinaface).  Class ids are
+                            compared as floats, like the reference's std::map<float, ...> (-0.0 == +0.0; 2.0 and 2.5 are
+                            two classes) and every row keeps its own class float; the order of NaN ids is unspecified. */
     int32_t tie_break_x0; /* 1: equal conf ordered by box[0] ascending (yolov8 cmp, postprocess.cpp:87-92); 0: none */
     int32_t extra_floats; /* floats copied verbatim from each source row into the output row after `keep`
                              (retinaface: 10 landmarks; yolo seg: 32 mask coefficients); 0 for plain det */

@@ -457,11 +457,15 @@ ORACLE_API void oracle_anticov_decode(const float* const* inputs, int batch, int
  * the double literal 0.1.
  * returns number of kept rows.
  * ------------------------------------------------------------------------------------------ */
+/* The four max / min of each IoU take their operands in the reference's order: std::max(a, b) is `a < b ? b : a` and
+ * std::min(a, b) is `b < a ? b : a`, so a NaN in the later row `r` is ignored and one in the kept row `l` propagates. */
+#define STD_MAX(a, b) ((a) < (b) ? (b) : (a))
+#define STD_MIN(a, b) ((b) < (a) ? (b) : (a))
 static float iou_ltrb(const float* l, const float* r) { /* yolov8/src/postprocess.cpp:71-85 */
-    float ib0 = l[0] > r[0] ? l[0] : r[0];
-    float ib1 = l[2] < r[2] ? l[2] : r[2];
-    float ib2 = l[1] > r[1] ? l[1] : r[1];
-    float ib3 = l[3] < r[3] ? l[3] : r[3];
+    float ib0 = STD_MAX(l[0], r[0]);
+    float ib1 = STD_MIN(l[2], r[2]);
+    float ib2 = STD_MAX(l[1], r[1]);
+    float ib3 = STD_MIN(l[3], r[3]);
     if (ib2 > ib3 || ib0 > ib1) return 0.0f;
     float inter = (ib1 - ib0) * (ib3 - ib2);
     float uni = (l[2] - l[0]) * (l[3] - l[1]) + (r[2] - r[0]) * (r[3] - r[1]) - inter;
@@ -472,19 +476,19 @@ static float iou_cxcywh(const float* l, const float* r) { /* yolov5/src/postproc
     float a1 = l[0] + l[2] / 2.f, b1 = r[0] + r[2] / 2.f;
     float a2 = l[1] - l[3] / 2.f, b2 = r[1] - r[3] / 2.f;
     float a3 = l[1] + l[3] / 2.f, b3 = r[1] + r[3] / 2.f;
-    float ib0 = a0 > b0 ? a0 : b0;
-    float ib1 = a1 < b1 ? a1 : b1;
-    float ib2 = a2 > b2 ? a2 : b2;
-    float ib3 = a3 < b3 ? a3 : b3;
+    float ib0 = STD_MAX(a0, b0);
+    float ib1 = STD_MIN(a1, b1);
+    float ib2 = STD_MAX(a2, b2);
+    float ib3 = STD_MIN(a3, b3);
     if (ib2 > ib3 || ib0 > ib1) return 0.0f;
     float inter = (ib1 - ib0) * (ib3 - ib2);
     return inter / (l[2] * l[3] + r[2] * r[3] - inter);
 }
 static float iou_retina(const float* l, const float* r) { /* retinaface/common.hpp:91-104 */
-    float ib0 = l[0] > r[0] ? l[0] : r[0];
-    float ib1 = l[2] < r[2] ? l[2] : r[2];
-    float ib2 = l[1] > r[1] ? l[1] : r[1];
-    float ib3 = l[3] < r[3] ? l[3] : r[3];
+    float ib0 = STD_MAX(l[0], r[0]);
+    float ib1 = STD_MIN(l[2], r[2]);
+    float ib2 = STD_MAX(l[1], r[1]);
+    float ib3 = STD_MIN(l[3], r[3]);
     if (ib2 > ib3 || ib0 > ib1) return 0.0f;
     float inter = (ib1 - ib0) * (ib3 - ib2);
     return inter / ((l[2] - l[0]) * (l[3] - l[1]) + (r[2] - r[0]) * (r[3] - r[1]) - inter + 0.000001f);

@@ -248,6 +248,12 @@ __device__ __forceinline__ void pick_bucket(const int* hist, bool descending, in
     *bucket_out = d;
 }
 
+// Class ids are grouped and ordered as floats, like the reference's std::map<float, ...>: float_key(cls) (-0.0 == +0.0).
+// Only ids that are integers in [0, 65535] fit the packed 64-bit sort keys; any other id (negative, fractional, huge,
+// NaN) sends the image to the generic 128-bit sort, which keys on float_key.
+__device__ __forceinline__ bool packed_class(float c) { return c >= 0.0f && c <= 65535.0f && c == truncf(c); }
+__device__ __forceinline__ bool same_class(float x, float y) { return float_key(x) == float_key(y); }
+
 // IoU work units of a segment of m rows: row li (0-based inside the segment) needs ceil(li/8) of them
 __device__ __forceinline__ int seg_units(int m) {
     const int G = (m + 6) >> 3;
@@ -262,10 +268,10 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
     float4* s_box = u_box + S;                                                   // S  sorted rows
     unsigned long long* k64 = reinterpret_cast<unsigned long long*>(s_box + S);  // S  64-bit sort keys (fast path)
     float* u_conf = reinterpret_cast<float*>(k64 + S);                           // S
-    int* u_cls = reinterpret_cast<int*>(u_conf + S);                             // S
+    float* u_cls = u_conf + S;                                                   // S   the source row's class float
     uint32_t* u_id = reinterpret_cast<uint32_t*>(u_cls + S);                     // S
     float* s_conf = reinterpret_cast<float*>(u_id + S);                          // S
-    int* s_cls = reinterpret_cast<int*>(s_conf + S);                             // S
+    float* s_cls = s_conf + S;                                                   // S
     uint32_t* s_id = reinterpret_cast<uint32_t*>(s_cls + S);                     // S
     int* s_seg = reinterpret_cast<int*>(s_id + S);                               // S   short class segments (start<<16 | len)
     int* s_long = s_seg + S;                                                     // S/2 long class segments
@@ -304,12 +310,12 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
         const int pos = atomicAdd(&s_n, 1);
         list[pos] = make_uint2(float_key(r.conf), id);  // only read back if more than pre_topk rows survive
         if (pos < S) {
-            const int c = a.class_aware ? (int)r.cls : 0;
+            const float c = a.class_aware ? r.cls : 0.0f;
             u_box[pos] = r.box;
             u_conf[pos] = r.conf;
             u_cls[pos] = c;
             u_id[pos] = id;
-            if (c < 0 || c > 0xffff) s_bad = 1;  // class does not fit the packed 64-bit key: generic sort
+            if (!packed_class(c)) s_bad = 1;  // class does not fit the packed 64-bit key: generic sort
         }
     };
     if (a.from_tiles) {
@@ -428,12 +434,12 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
             if (e.x > key_cut || (e.x == key_cut && e.y <= id_cut)) {
                 const Row r = fetch_row(a, b, e.y);
                 const int pos = atomicAdd(&s_n, 1);
-                const int c = a.class_aware ? (int)r.cls : 0;
+                const float c = a.class_aware ? r.cls : 0.0f;
                 u_box[pos] = r.box;
                 u_conf[pos] = r.conf;
                 u_cls[pos] = c;
                 u_id[pos] = e.y;
-                if (c < 0 || c > 0xffff) s_bad = 1;
+                if (!packed_class(c)) s_bad = 1;
             }
         }
         __syncthreads();
@@ -458,7 +464,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
         for (int base = 0; base < M; base += kNmsThreads) {
             // rows arrive in tile order, so neighbouring lanes often share a class: one atomic per (warp, class)
             const int i = base + tid;
-            const int c = i < M ? u_cls[i] : -1;
+            const int c = i < M ? (int)u_cls[i] : -1;
             const unsigned peers = __match_any_sync(0xffffffffu, c);
             const int leader = __ffs(peers) - 1;
             int first = 0;
@@ -482,7 +488,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
             s_cstart[tid] = s_wsum[warp] + ex;
             __syncthreads();
             for (int i = tid; i < M; i += kNmsThreads) {
-                const int c = u_cls[i];
+                const int c = (int)u_cls[i];
                 kb[s_cstart[c] + s_pos[i]] =
                     ((unsigned long long)(uint32_t)c << 48) | ((unsigned long long)(uint32_t)(~float_key(u_conf[i])) << 16) | (uint32_t)i;
             }
@@ -507,7 +513,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
     }
     if (!generic && !bucketed) {
         for (int i = tid; i < S_eff; i += kNmsThreads)
-            k64[i] = i < M ? ((unsigned long long)(uint32_t)u_cls[i] << 48) | ((unsigned long long)(uint32_t)(~float_key(u_conf[i])) << 16) | (uint32_t)i
+            k64[i] = i < M ? ((unsigned long long)(uint32_t)(int)u_cls[i] << 48) | ((unsigned long long)(uint32_t)(~float_key(u_conf[i])) << 16) | (uint32_t)i
                            : ~0ull;
         __syncthreads();
         if (S_eff <= kNmsThreads) {
@@ -558,7 +564,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
     if (generic) {
         for (int i = tid; i < S_eff; i += kNmsThreads) {
             if (i < M) {
-                k_hi[i] = ((unsigned long long)(uint32_t)u_cls[i] << 32) | (uint32_t)(~float_key(u_conf[i]));
+                k_hi[i] = ((unsigned long long)float_key(u_cls[i]) << 32) | (uint32_t)(~float_key(u_conf[i]));
                 k_lo[i] = ((unsigned long long)(a.tie_break_x0 ? float_key(u_box[i].x) : 0u) << 32) | u_id[i];
             } else {
                 k_hi[i] = ~0ull;
@@ -649,7 +655,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
         if (bucketed) {
             // the class histogram already is the segment table
             for (int i = tid; i < M; i += kNmsThreads) {
-                const int c = s_cls[i], m = s_chist[c];
+                const int c = (int)s_cls[i], m = s_chist[c];
                 s_rowseg[i] = m > kShortSeg ? 0 : ((s_cstart[c] << 16) | m);
             }
             const int m = s_chist[tid], p0 = s_cstart[tid];
@@ -662,9 +668,9 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
             if (m > 1 && m <= kShortSeg) s_pos[p0] = (unsigned short)atomicAdd(&s_nunit, seg_units(m));
         } else
         for (int i = tid; i < M; i += kNmsThreads) {
-            if (i == 0 || s_cls[i] != s_cls[i - 1]) {
+            if (i == 0 || !same_class(s_cls[i], s_cls[i - 1])) {
                 int e = i + 1;
-                while (e < M && s_cls[e] == s_cls[i]) ++e;
+                while (e < M && same_class(s_cls[e], s_cls[i])) ++e;
                 const int m = e - i;
                 // every row learns its segment (start << 16 | length; 0 = long segment, handled by the whole CTA)
                 for (int r = i; r < e; ++r) s_rowseg[r] = m > kShortSeg ? 0 : ((i << 16) | m);
@@ -803,10 +809,10 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
     } else {
         // one-shot: dropped iff some earlier same-class row (higher conf) overlaps (postprocess.cu:89-111)
         for (int i = tid; i < M; i += kNmsThreads) {
-            const int ci = s_cls[i];
+            const float ci = s_cls[i];
             const float4 bi = s_box[i];
             bool keep = true;
-            for (int jx = i - 1; jx >= 0 && s_cls[jx] == ci; --jx) {
+            for (int jx = i - 1; jx >= 0 && same_class(s_cls[jx], ci); --jx) {
                 if (iq.obb ? obb_probiou_dev(bi, s_area[i], s_box[jx], s_area[jx]) > a.nms_thresh
                            : iou_oneshot(bi, s_box[jx]) > a.nms_thresh) {
                     keep = false;
@@ -847,7 +853,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
             row[2] = bx.z;
             row[3] = bx.w;
             row[4] = s_conf[i];
-            row[5] = (float)s_cls[i];
+            row[5] = s_cls[i];  // the source row's own class float (the reference pushes a copy of the row)
             row[6] = s_keep[i] ? 1.0f : 0.0f;
             if (oidx) oidx[k] = a.from_tiles ? __float_as_int(a.cand[2 * ((size_t)b * a.slots_per_image + s_id[i]) + 1].z)
                                              : (int)s_id[i];
