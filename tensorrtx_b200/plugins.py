@@ -43,10 +43,18 @@ def _stream(stream=None) -> int:
     return int(stream)
 
 
-def _tune(params, slices: int = 0, rows: int = 0, box: int = 0) -> None:
-    """Per-plugin launch tuning of the scan kernel (trtx_yolo_params.tune_*; 0 = default).  Plain data inside the
-    plugin's own parameter block -- nothing global, clones / other plugins are unaffected."""
-    params.tune_class_slices, params.tune_rows_in_flight, params.tune_box_prefetch = int(slices), int(rows), int(box)
+def _nbytes(workspace: torch.Tensor) -> int:
+    return workspace.numel() * workspace.element_size()
+
+
+def _out_tensor(t, shape: tuple, dtype, device, what: str, alloc=torch.empty, contiguous: bool = True) -> torch.Tensor:
+    """`t`, or a new tensor from alloc (torch.empty or torch.zeros) when t is None.  A given t of another shape or dtype
+    raises ValueError(what), and so does a non-contiguous one when `contiguous` (else _ptr rejects it with TrtxError)."""
+    if t is None:
+        return alloc(shape, dtype=dtype, device=device)
+    if tuple(t.shape) != tuple(shape) or t.dtype != dtype or (contiguous and not t.is_contiguous()):
+        raise ValueError(what)
+    return t
 
 
 def float_le_threshold(x: float) -> float:
@@ -66,11 +74,58 @@ def float_ge_threshold(x: float) -> float:
 
 
 # --------------------------------------------------------------------------------------------------
-# YoloLayer_TRT, anchor-free (yolov8 / yolo11 / yolov12 / yolov13 ...)
+# YoloLayer_TRT: what every variant's mirror shares
 # --------------------------------------------------------------------------------------------------
-class YoloLayerPlugin:
+class _YoloLayerBase:
+    """The YoloLayer_TRT surface common to all variants: one output of 1 + rows*DET_FLOATS floats per image, the workspace
+    trtx_yolo_workspace_size asks for, and the trtx_yolo_decode_enqueue call on the subclass' `params` block."""
     PLUGIN_TYPE = "YoloLayer_TRT"
     PLUGIN_VERSION = "1"
+    mThreadCount = 256  # serialized by the reference (yololayer.cu:80); unused here
+    mPluginNamespace = ""
+
+    @property
+    def _max_rows(self) -> int:
+        return self.mMaxOutObject
+
+    def getNbOutputs(self) -> int:
+        return 1
+
+    def output_elems(self) -> int:
+        return 1 + self._max_rows * self.DET_FLOATS
+
+    def getWorkspaceSize(self, maxBatchSize: int) -> int:
+        return int(self._lib.trtx_yolo_workspace_size(C.byref(self.params), int(maxBatchSize)))
+
+    def getPluginType(self) -> str:
+        return self.PLUGIN_TYPE
+
+    def getPluginVersion(self) -> str:
+        return self.PLUGIN_VERSION
+
+    def _decode(self, batch: int, inputs, output, workspace, stream, ws_bytes: int | None = None) -> int:
+        """trtx_yolo_decode_enqueue of `inputs` (device tensors, one per level) into `output`; ws_bytes defaults to the size
+        of the workspace tensor.  Returns the library's status, 0 on success."""
+        ptrs = L.ptr_array([_ptr(t) for t in inputs])
+        return int(self._lib.trtx_yolo_decode_enqueue(C.byref(self.params), int(batch), ptrs, _ptr(output), _ptr(workspace),
+                                                      _nbytes(workspace) if ws_bytes is None else ws_bytes, _stream(stream)))
+
+
+class _TunableYoloLayer(_YoloLayerBase):
+    """The YoloLayer mirrors with tune(): all but YoloLayerPlugin26."""
+
+    def tune(self, *, slices: int = 0, rows: int = 0, box: int = 0):
+        """Per-plugin launch tuning of the scan kernel (trtx_yolo_params.tune_*; 0 = default).  Plain data inside the
+        plugin's own parameter block -- nothing global, clones / other plugins are unaffected."""
+        p = self.params
+        p.tune_class_slices, p.tune_rows_in_flight, p.tune_box_prefetch = int(slices), int(rows), int(box)
+        return self
+
+
+# --------------------------------------------------------------------------------------------------
+# YoloLayer_TRT, anchor-free (yolov8 / yolo11 / yolov12 / yolov13 ...)
+# --------------------------------------------------------------------------------------------------
+class YoloLayerPlugin(_TunableYoloLayer):
     DET_FLOATS = 90  # sizeof(Detection)/4, yolov8/include/types.h:4-12
 
     def __init__(self, classCount: int, numberofpoints: int, confthreshkeypoints: float, netWidth: int,
@@ -86,8 +141,6 @@ class YoloLayerPlugin:
         self.is_pose_ = bool(is_pose)
         self.is_obb_ = bool(is_obb)
         self.mStrides = [int(s) for s in strides]
-        self.mThreadCount = 256  # serialized by the reference (yololayer.cu:80); unused here
-        self.mPluginNamespace = ""
         self.in_dtype = in_dtype
         self._lib = L.load()
         p = L.YoloParams()
@@ -104,19 +157,9 @@ class YoloLayerPlugin:
         self.params = p
 
     # ---- IPluginV2 surface ----
-    def tune(self, **kw) -> "YoloLayerPlugin":
-        _tune(self.params, **kw)
-        return self
-
-    def getNbOutputs(self) -> int:
-        return 1
-
     def getOutputDimensions(self, index=0, inputs=None, nbInputDims=0):
         total = self.mMaxOutObject * self.DET_FLOATS  # yololayer.cu:107-111
         return (total + 1, 1, 1)
-
-    def output_elems(self) -> int:
-        return 1 + self.mMaxOutObject * self.DET_FLOATS
 
     def initialize(self) -> int:
         return 0
@@ -124,27 +167,17 @@ class YoloLayerPlugin:
     def terminate(self) -> None:
         pass
 
-    def getWorkspaceSize(self, maxBatchSize: int) -> int:
-        return int(self._lib.trtx_yolo_workspace_size(C.byref(self.params), int(maxBatchSize)))
-
     def enqueue(self, batchSize: int, inputs, outputs, workspace, stream=None) -> int:
-        """inputs: one device tensor per stride [B, C, g]; outputs[0]: [B, 1+maxOut*90] fp32; returns 0 on success."""
-        ptrs = L.ptr_array([_ptr(t) for t in inputs])
-        ws_bytes = workspace.numel() * workspace.element_size() if isinstance(workspace, torch.Tensor) else self.getWorkspaceSize(batchSize)
-        return int(self._lib.trtx_yolo_decode_enqueue(C.byref(self.params), int(batchSize), ptrs, _ptr(outputs[0]),
-                                                      _ptr(workspace), ws_bytes, _stream(stream)))
+        """inputs: one device tensor per stride [B, C, g]; outputs[0]: [B, 1+maxOut*90] fp32; workspace: a device tensor or
+        a raw pointer to getWorkspaceSize(batchSize) bytes; returns 0 on success."""
+        ws_bytes = None if isinstance(workspace, torch.Tensor) else self.getWorkspaceSize(batchSize)
+        return self._decode(batchSize, inputs, outputs[0], workspace, stream, ws_bytes)
 
     def supportsFormatCombination(self, pos, inOut, nbInputs, nbOutputs) -> bool:
         fmt, dtype = inOut[pos]
         if pos < nbInputs:
             return fmt == "kLINEAR" and dtype in (("kFLOAT",) if self.in_dtype == L.F32 else ("kHALF",))
         return fmt == "kLINEAR" and dtype == "kFLOAT"
-
-    def getPluginType(self) -> str:
-        return self.PLUGIN_TYPE
-
-    def getPluginVersion(self) -> str:
-        return self.PLUGIN_VERSION
 
     def getOutputDataType(self, index, inputTypes, nbInputs) -> str:
         return "kFLOAT"
@@ -239,9 +272,7 @@ class YoloKernel:
         assert len(self.anchors) == 6
 
 
-class YoloLayerPluginV5:
-    PLUGIN_TYPE = "YoloLayer_TRT"
-    PLUGIN_VERSION = "1"
+class YoloLayerPluginV5(_TunableYoloLayer):
     DET_FLOATS = 38  # yolov5/src/types.h:11-16
 
     def __init__(self, classCount: int, netWidth: int, netHeight: int, maxOut: int, is_segmentation: bool,
@@ -251,8 +282,6 @@ class YoloLayerPluginV5:
         self.is_segmentation_ = bool(is_segmentation)
         self.mYoloKernel = list(vYoloKernel)
         self.mKernelCount = len(self.mYoloKernel)
-        self.mThreadCount = 256
-        self.mPluginNamespace = ""
         self._lib = L.load()
         p = L.YoloParams()
         p.variant = L.YOLO_V5
@@ -270,33 +299,11 @@ class YoloLayerPluginV5:
         p.in_dtype = in_dtype
         self.params = p
 
-    def tune(self, **kw) -> "YoloLayerPlugin":
-        _tune(self.params, **kw)
-        return self
-
-    def getNbOutputs(self) -> int:
-        return 1
-
-    def output_elems(self) -> int:
-        return 1 + self.mMaxOutObject * self.DET_FLOATS
-
     def getOutputDimensions(self, index=0, inputs=None, nbInputDims=0):
         return (self.mMaxOutObject * self.DET_FLOATS + 1, 1, 1)
 
-    def getWorkspaceSize(self, maxBatchSize: int) -> int:
-        return int(self._lib.trtx_yolo_workspace_size(C.byref(self.params), int(maxBatchSize)))
-
     def enqueue(self, batchSize: int, inputs, outputs, workspace, stream=None) -> int:
-        ptrs = L.ptr_array([_ptr(t) for t in inputs])
-        ws_bytes = workspace.numel() * workspace.element_size()
-        return int(self._lib.trtx_yolo_decode_enqueue(C.byref(self.params), int(batchSize), ptrs, _ptr(outputs[0]),
-                                                      _ptr(workspace), ws_bytes, _stream(stream)))
-
-    def getPluginType(self) -> str:
-        return self.PLUGIN_TYPE
-
-    def getPluginVersion(self) -> str:
-        return self.PLUGIN_VERSION
+        return self._decode(batchSize, inputs, outputs[0], workspace, stream)
 
     def clone(self) -> "YoloLayerPluginV5":
         p = YoloLayerPluginV5(self.mClassCount, self.mYoloV5NetWidth, self.mYoloV5NetHeight, self.mMaxOutObject,
@@ -384,19 +391,17 @@ YOLOV3_KERNELS = (YoloKernelV3(-1, -1, 32, (116, 90, 156, 198, 373, 326)),
                   YoloKernelV3(-1, -1, 8, (10, 13, 16, 30, 33, 23)))
 
 
-class YoloLayerPluginV3:
+class YoloLayerPluginV3(_TunableYoloLayer):
     """yolov3-spp/yololayer.h:58-121 (IPluginV2DynamicExt "YoloLayer_TRT" v1; yolov3 / yolov4 carry the same plugin).
     The reference compiles CLASS_NUM, the kernels and MAX_OUTPUT_BBOX_COUNT in; here they are constructor arguments with
     the reference's values as defaults.  enqueue() takes the grids from the input tensors like the reference
     (yololayer.cu:207-216)."""
-    PLUGIN_TYPE = "YoloLayer_TRT"
-    PLUGIN_VERSION = "1"
     DET_FLOATS = 7  # x,y,w,h, det_confidence, class_id, class_confidence (yololayer.h:47-53)
 
     def __init__(self, classCount: int = 80, kernels: Sequence[YoloKernelV3] = YOLOV3_KERNELS, maxOut: int = 1000,
                  in_dtype: int = L.F32):
         self.mClassCount, self.mYoloKernel, self.mMaxOutObject = int(classCount), list(kernels), int(maxOut)
-        self.mKernelCount, self.mThreadCount, self.mPluginNamespace = len(self.mYoloKernel), 256, ""
+        self.mKernelCount = len(self.mYoloKernel)
         self._lib = L.load()
         p = L.YoloParams()
         p.variant = L.YOLO_V3
@@ -410,23 +415,10 @@ class YoloLayerPluginV3:
         p.in_dtype = in_dtype
         self.params = p
 
-    def tune(self, **kw) -> "YoloLayerPluginV3":
-        _tune(self.params, **kw)
-        return self
-
-    def getNbOutputs(self) -> int:
-        return 1
-
-    def output_elems(self) -> int:
-        return 1 + self.mMaxOutObject * self.DET_FLOATS
-
     def configure(self, inputs) -> None:
         """grid = dims 2, 3 of every input tensor [B, 3*(5+nc), gh, gw] (yololayer.cu:209-212)."""
         for i, t in enumerate(inputs):
             self.params.grid_h[i], self.params.grid_w[i] = int(t.shape[2]), int(t.shape[3])
-
-    def getWorkspaceSize(self, maxBatchSize: int) -> int:
-        return int(self._lib.trtx_yolo_workspace_size(C.byref(self.params), int(maxBatchSize)))
 
     def enqueue(self, inputs, outputs, workspace=None, stream=None) -> int:
         """IPluginV2DynamicExt::enqueue: batch = inputs[0].shape[0]."""
@@ -434,15 +426,7 @@ class YoloLayerPluginV3:
         batch = int(inputs[0].shape[0])
         if workspace is None:
             workspace = torch.empty(self.getWorkspaceSize(batch), dtype=torch.uint8, device=inputs[0].device)
-        ptrs = L.ptr_array([_ptr(t) for t in inputs])
-        return int(self._lib.trtx_yolo_decode_enqueue(C.byref(self.params), batch, ptrs, _ptr(outputs[0]), _ptr(workspace),
-                                                      workspace.numel() * workspace.element_size(), _stream(stream)))
-
-    def getPluginType(self) -> str:
-        return self.PLUGIN_TYPE
-
-    def getPluginVersion(self) -> str:
-        return self.PLUGIN_VERSION
+        return self._decode(batch, inputs, outputs[0], workspace, stream)
 
     def clone(self) -> "YoloLayerPluginV3":
         p = YoloLayerPluginV3(self.mClassCount, self.mYoloKernel, self.mMaxOutObject, self.params.in_dtype)
@@ -473,19 +457,17 @@ class YoloLayerPluginV3:
         return p
 
 
-class YoloLayerPlugin26:
+class YoloLayerPlugin26(_YoloLayerBase):
     """yolo26/plugin/yololayer.h:10-77 ("YoloLayer_TRT" v1 of the NMS-free yolo26 heads): ctor (classCount, numberOfPoints,
     maxDetections, isDetection, isSegmentation, isPose, isObb, anchor_count); setPluginDeviceParams(confThreshold) of the
     reference is the `conf_thresh` argument here (no device global).  One input [B, anchor_count, 4+nc(+1)]."""
-    PLUGIN_TYPE = "YoloLayer_TRT"
-    PLUGIN_VERSION = "1"
     DET_FLOATS = 90  # yolo26/include/types.h
 
     def __init__(self, classCount: int, numberOfPoints: int, maxDetections: int, isDetection: bool, isSegmentation: bool,
                  isPose: bool, isObb: bool, anchor_count: int, conf_thresh: float = 0.4):
         self.mClassCount, self.mNumberOfPoints, self.mMaxDetections = int(classCount), int(numberOfPoints), int(maxDetections)
         self.mIsDetection, self.mIsSegmentation, self.mIsPose, self.mIsObb = bool(isDetection), bool(isSegmentation), bool(isPose), bool(isObb)
-        self.mAnchorCount, self.mThreadCount, self.mPluginNamespace = int(anchor_count), 256, ""
+        self.mAnchorCount = int(anchor_count)
         self._lib = L.load()
         p = L.YoloParams()
         p.variant = L.YOLO_V26
@@ -497,25 +479,12 @@ class YoloLayerPlugin26:
         p.in_dtype = L.F32
         self.params = p
 
-    def getNbOutputs(self) -> int:
-        return 1
-
-    def output_elems(self) -> int:
-        return 1 + self.mMaxDetections * self.DET_FLOATS
-
-    def getWorkspaceSize(self, maxBatchSize: int) -> int:
-        return int(self._lib.trtx_yolo_workspace_size(C.byref(self.params), int(maxBatchSize)))
+    @property
+    def _max_rows(self) -> int:
+        return self.mMaxDetections
 
     def enqueue(self, batchSize: int, inputs, outputs, workspace, stream=None) -> int:
-        ptrs = L.ptr_array([_ptr(inputs[0])])
-        return int(self._lib.trtx_yolo_decode_enqueue(C.byref(self.params), int(batchSize), ptrs, _ptr(outputs[0]), _ptr(workspace),
-                                                      workspace.numel() * workspace.element_size(), _stream(stream)))
-
-    def getPluginType(self) -> str:
-        return self.PLUGIN_TYPE
-
-    def getPluginVersion(self) -> str:
-        return self.PLUGIN_VERSION
+        return self._decode(batchSize, (inputs[0],), outputs[0], workspace, stream)
 
     def clone(self) -> "YoloLayerPlugin26":
         p = YoloLayerPlugin26(self.mClassCount, self.mNumberOfPoints, self.mMaxDetections, self.mIsDetection, self.mIsSegmentation,
@@ -626,6 +595,17 @@ def _frames(sizes: Sequence[tuple[int, int]], canvases: Sequence[torch.Tensor] |
     return descs, (list(canvases) if canvases is not None else None)
 
 
+def _f32_rows(dets: torch.Tensor) -> None:
+    """Per-row entries read dets [B, 1 + rows*F] as dense float32 rows."""
+    if dets.dtype != torch.float32 or dets.stride(1) != 1 or dets.stride(0) != dets.shape[1]:
+        raise ValueError("dets must be contiguous float32")
+
+
+def _frame_wh(image_sizes: Sequence[tuple[int, int]]):
+    """The per-row entries' host int32 array (img_w, img_h) of every frame."""
+    return (C.c_int32 * (2 * len(image_sizes)))(*[int(v) for s in image_sizes for v in s])
+
+
 def yolo_seg_postprocess(proto: torch.Tensor | None, dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]], *,
                          variant: int, max_rows: int, row_floats: int = 39, coeff_offset: int = 7, max_masks: int,
                          net_w: int = 640, net_h: int = 640, masks: bool = True, rows_out: torch.Tensor | None = None,
@@ -678,17 +658,13 @@ def yolo_pose_obb_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[in
         extra_offset = row_floats - 1 if task == L.TASK_OBB_NMS_FREE else 7
     if dets.dim() != 2 or dets.shape[0] != B or dets.shape[1] < 1 + max_rows * row_floats:
         raise ValueError(f"dets must be [{B}, >= {1 + max_rows * row_floats}]")
-    if dets.dtype != torch.float32 or dets.stride(1) != 1 or dets.stride(0) != dets.shape[1]:
-        raise ValueError("dets must be contiguous float32")
+    _f32_rows(dets)
     F = 6 + 3 * num_kpts if task == L.TASK_POSE else 10
     q = L.PoseObbParams(task, net_w, net_h, row_floats, extra_offset, num_kpts)
-    if rows_out is None:
-        rows_out = torch.empty((B, 1 + max_rows * F), dtype=torch.float32, device=dets.device)
-    if tuple(rows_out.shape) != (B, 1 + max_rows * F) or rows_out.dtype != torch.float32 or not rows_out.is_contiguous():
-        raise ValueError(f"rows_out must be contiguous float32 [{B}, {1 + max_rows * F}]")
-    wh = (C.c_int32 * (2 * B))(*[int(v) for s in image_sizes for v in s])
-    L.check(lib.trtx_yolo_pose_obb_postprocess_enqueue(C.byref(q), wh, B, _ptr(dets), max_rows, _ptr(rows_out),
-                                                       _stream(stream)), "trtx_yolo_pose_obb_postprocess_enqueue")
+    rows_out = _out_tensor(rows_out, (B, 1 + max_rows * F), torch.float32, dets.device,
+                           f"rows_out must be contiguous float32 [{B}, {1 + max_rows * F}]")
+    L.check(lib.trtx_yolo_pose_obb_postprocess_enqueue(C.byref(q), _frame_wh(image_sizes), B, _ptr(dets), max_rows,
+                                                       _ptr(rows_out), _stream(stream)), "trtx_yolo_pose_obb_postprocess_enqueue")
     return rows_out
 
 
@@ -713,17 +689,13 @@ def retina_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]
         row_floats = 7 + extras
     if dets.dim() != 2 or tuple(dets.shape) != (B, 1 + max_rows * row_floats):
         raise ValueError(f"dets must be [{B}, {1 + max_rows * row_floats}]")
-    if dets.dtype != torch.float32 or dets.stride(1) != 1 or dets.stride(0) != dets.shape[1]:
-        raise ValueError("dets must be contiguous float32")
+    _f32_rows(dets)
     F = 5 + extras
     q = L.FacePostParams(variant, in_w, in_h, row_floats, lmk_offset, float_ge_threshold(conf_thresh))
-    if rows_out is None:
-        rows_out = torch.empty((B, 1 + max_rows * F), dtype=torch.float32, device=dets.device)
-    if tuple(rows_out.shape) != (B, 1 + max_rows * F) or rows_out.dtype != torch.float32 or not rows_out.is_contiguous():
-        raise ValueError(f"rows_out must be contiguous float32 [{B}, {1 + max_rows * F}]")
-    wh = (C.c_int32 * (2 * B))(*[int(v) for s in image_sizes for v in s])
-    L.check(lib.trtx_retina_postprocess_enqueue(C.byref(q), wh, B, _ptr(dets), max_rows, _ptr(rows_out), _stream(stream)),
-            "trtx_retina_postprocess_enqueue")
+    rows_out = _out_tensor(rows_out, (B, 1 + max_rows * F), torch.float32, dets.device,
+                           f"rows_out must be contiguous float32 [{B}, {1 + max_rows * F}]")
+    L.check(lib.trtx_retina_postprocess_enqueue(C.byref(q), _frame_wh(image_sizes), B, _ptr(dets), max_rows, _ptr(rows_out),
+                                                _stream(stream)), "trtx_retina_postprocess_enqueue")
     return rows_out
 
 
@@ -813,8 +785,7 @@ class DecodePlugin:
     def enqueue(self, batchSize: int, inputs, outputs, workspace, stream=None) -> int:
         ptrs = L.ptr_array([_ptr(t) for t in inputs])
         return int(self._lib.trtx_retina_decode_enqueue(C.byref(self.params), int(batchSize), ptrs, _ptr(outputs[0]),
-                                                        _ptr(workspace), workspace.numel() * workspace.element_size(),
-                                                        _stream(stream)))
+                                                        _ptr(workspace), _nbytes(workspace), _stream(stream)))
 
     def getPluginType(self) -> str:
         return self.PLUGIN_TYPE
@@ -845,6 +816,11 @@ def _rc64(rc: int, what: str) -> int:
     return rc
 
 
+def _status(rc: int) -> int:
+    """enqueue()'s return value from a call that returns -error or a non-negative count: the error code, or 0."""
+    return int(-rc if rc < 0 else 0)
+
+
 class RpnDecodePlugin:
     def __init__(self, top_n: int, anchors: Sequence[float], stride: float, image_height: int, image_width: int,
                  height: int = 0, width: int = 0):
@@ -871,9 +847,9 @@ class RpnDecodePlugin:
     def enqueue(self, batchSize, inputs, outputs, workspace, stream=None) -> int:
         rc = self._lib.trtx_rpn_decode(batchSize, _ptr(inputs[0]), _ptr(inputs[1]), _ptr(outputs[0]), _ptr(outputs[1]),
                                        self._height, self._width, self._image_height, self._image_width, self._stride,
-                                       self._anc, len(self._anchors) // 4, self._top_n, _ptr(workspace),
-                                       workspace.numel() * workspace.element_size(), _stream(stream))
-        return int(-rc if rc < 0 else 0)
+                                       self._anc, len(self._anchors) // 4, self._top_n, _ptr(workspace), _nbytes(workspace),
+                                       _stream(stream))
+        return _status(rc)
 
 
 class RpnNmsPlugin:
@@ -896,9 +872,8 @@ class RpnNmsPlugin:
 
     def enqueue(self, batchSize, inputs, outputs, workspace, stream=None) -> int:
         rc = self._lib.trtx_rpn_nms(batchSize, _ptr(inputs[0]), _ptr(inputs[1]), _ptr(outputs[0]), self._pre_nms_topk,
-                                    self._post_nms_topk, self._nms_thresh, _ptr(workspace),
-                                    workspace.numel() * workspace.element_size(), _stream(stream))
-        return int(-rc if rc < 0 else 0)
+                                    self._post_nms_topk, self._nms_thresh, _ptr(workspace), _nbytes(workspace), _stream(stream))
+        return _status(rc)
 
 
 class PredictorDecodePlugin:
@@ -924,8 +899,8 @@ class PredictorDecodePlugin:
         rc = self._lib.trtx_predictor_decode(batchSize, _ptr(inputs[0]), _ptr(inputs[1]), _ptr(inputs[2]),
                                              _ptr(outputs[0]), _ptr(outputs[1]), _ptr(outputs[2]), self._num_boxes,
                                              self._num_classes, self._image_height, self._image_width, self._w,
-                                             _ptr(workspace), workspace.numel() * workspace.element_size(), _stream(stream))
-        return int(-rc if rc < 0 else 0)
+                                             _ptr(workspace), _nbytes(workspace), _stream(stream))
+        return _status(rc)
 
 
 class BatchedNmsPlugin:
@@ -951,9 +926,9 @@ class BatchedNmsPlugin:
     def enqueue(self, batchSize, inputs, outputs, workspace, stream=None) -> int:
         rc = self._lib.trtx_batched_nms(self._nms_method, batchSize, _ptr(inputs[0]), _ptr(inputs[1]), _ptr(inputs[2]),
                                         _ptr(outputs[0]), _ptr(outputs[1]), _ptr(outputs[2]), self._count,
-                                        self._detections_per_im, self._nms_thresh, _ptr(workspace),
-                                        workspace.numel() * workspace.element_size(), _stream(stream))
-        return int(-rc if rc < 0 else 0)
+                                        self._detections_per_im, self._nms_thresh, _ptr(workspace), _nbytes(workspace),
+                                        _stream(stream))
+        return _status(rc)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -1042,22 +1017,27 @@ class MaskRcnnInferencePlugin:
                                                       _stream(stream)))
 
 
+def _image_descs(images: Sequence[torch.Tensor]):
+    """trtx_image_desc array of u8 HWC BGR device frames [h, w, 3]: rows may be pitched, pixels may not."""
+    descs = (L.ImageDesc * len(images))()
+    for i, im in enumerate(images):
+        if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3 or im.stride(2) != 1 or im.stride(1) != 3:
+            raise L.TrtxError("images must be u8 HWC BGR with packed pixels")
+        descs[i].data_dev = im.data_ptr()
+        descs[i].height, descs[i].width = int(im.shape[0]), int(im.shape[1])
+        descs[i].pitch = int(im.stride(0))
+    return descs
+
+
 def cuda_batch_preprocess(img_batch: Sequence[torch.Tensor], dst: torch.Tensor, dst_width: int, dst_height: int,
                           stream=None) -> None:
     """Drop-in for cuda_batch_preprocess (yolov8/src/preprocess.cu:119-127) with DEVICE images:
     img_batch[i] is a u8 HWC BGR cuda tensor [h, w, 3] (row-contiguous); dst is [B, 3, dst_h, dst_w] fp32/fp16.
     One launch for the whole batch, no synchronisation."""
     lib = L.load()
-    n = len(img_batch)
-    descs = (L.ImageDesc * n)()
-    for i, im in enumerate(img_batch):
-        if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3 or im.stride(2) != 1 or im.stride(1) != 3:
-            raise L.TrtxError("images must be u8 HWC BGR with packed pixels")
-        descs[i].data_dev = im.data_ptr()
-        descs[i].height, descs[i].width = int(im.shape[0]), int(im.shape[1])
-        descs[i].pitch = int(im.stride(0))
+    descs = _image_descs(img_batch)
     dt = L.F32 if dst.dtype == torch.float32 else L.F16
-    L.check(lib.trtx_preprocess_batch_enqueue(descs, n, _ptr(dst), dst_width, dst_height, dt, _stream(stream)),
+    L.check(lib.trtx_preprocess_batch_enqueue(descs, len(img_batch), _ptr(dst), dst_width, dst_height, dt, _stream(stream)),
             "trtx_preprocess_batch_enqueue")
 
 
@@ -1069,14 +1049,8 @@ class PreprocessPlan:
     def __init__(self, img_batch: Sequence[torch.Tensor], dst: torch.Tensor, dst_width: int, dst_height: int):
         self._lib = L.load()
         self.n = len(img_batch)
-        self.descs = (L.ImageDesc * self.n)()
+        self.descs = _image_descs(img_batch)
         self._keep = list(img_batch)
-        for i, im in enumerate(img_batch):
-            if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3 or im.stride(2) != 1 or im.stride(1) != 3:
-                raise L.TrtxError("images must be u8 HWC BGR with packed pixels")
-            self.descs[i].data_dev = im.data_ptr()
-            self.descs[i].height, self.descs[i].width = int(im.shape[0]), int(im.shape[1])
-            self.descs[i].pitch = int(im.stride(0))
         self.dst, self.dw, self.dh = dst, int(dst_width), int(dst_height)
         self.dt = L.F32 if dst.dtype == torch.float32 else L.F16
 
@@ -1141,17 +1115,9 @@ def rcnn_preprocess(images: Sequence[torch.Tensor], net_w: int, net_h: int, out:
     image: the engine input.  One launch per 64 images, no synchronisation."""
     lib = L.load()
     n = len(images)
-    descs = (L.ImageDesc * n)()
-    for i, im in enumerate(images):
-        if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3 or im.stride(2) != 1 or im.stride(1) != 3:
-            raise L.TrtxError("images must be u8 HWC BGR with packed pixels")
-        descs[i].data_dev = im.data_ptr()
-        descs[i].height, descs[i].width = int(im.shape[0]), int(im.shape[1])
-        descs[i].pitch = int(im.stride(0))
-    if out is None:
-        out = torch.empty((n, net_h, net_w, 3), dtype=torch.float32, device=images[0].device if n else "cuda")
-    if out.dtype != torch.float32 or tuple(out.shape) != (n, net_h, net_w, 3):
-        raise ValueError(f"out must be float32 [{n}, {net_h}, {net_w}, 3]")
+    descs = _image_descs(images)
+    out = _out_tensor(out, (n, net_h, net_w, 3), torch.float32, images[0].device if n else "cuda",
+                      f"out must be float32 [{n}, {net_h}, {net_w}, 3]", contiguous=False)
     L.check(lib.trtx_rcnn_preprocess_enqueue(descs, n, net_w, net_h, _ptr(out), _stream(stream)), "trtx_rcnn_preprocess_enqueue")
     return out
 
@@ -1164,17 +1130,9 @@ def cls_preprocess(images: Sequence[torch.Tensor], variant: int, net_w: int, net
     letterbox on a 128-grey canvas, ImageNet mean / std.  One launch per 64 images, no synchronisation."""
     lib = L.load()
     n = len(images)
-    descs = (L.ImageDesc * n)()
-    for i, im in enumerate(images):
-        if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3 or im.stride(2) != 1 or im.stride(1) != 3:
-            raise L.TrtxError("images must be u8 HWC BGR with packed pixels")
-        descs[i].data_dev = im.data_ptr()
-        descs[i].height, descs[i].width = int(im.shape[0]), int(im.shape[1])
-        descs[i].pitch = int(im.stride(0))
-    if out is None:
-        out = torch.empty((n, 3, net_h, net_w), dtype=torch.float32, device=images[0].device if n else "cuda")
-    if out.dtype != torch.float32 or tuple(out.shape) != (n, 3, net_h, net_w):
-        raise ValueError(f"out must be float32 [{n}, 3, {net_h}, {net_w}]")
+    descs = _image_descs(images)
+    out = _out_tensor(out, (n, 3, net_h, net_w), torch.float32, images[0].device if n else "cuda",
+                      f"out must be float32 [{n}, 3, {net_h}, {net_w}]", contiguous=False)
     L.check(lib.trtx_cls_preprocess_enqueue(variant, descs, n, net_w, net_h, _ptr(out), _stream(stream)),
             "trtx_cls_preprocess_enqueue")
     return out
@@ -1249,10 +1207,7 @@ def rcnn_postprocess_frames(scores: torch.Tensor, boxes: torch.Tensor, classes: 
             raise ValueError("scores, boxes, classes and masks must be contiguous float32")
     max_masks = D if max_masks is None else int(max_masks)
     q = L.RcnnPostParams(net_w, net_h, 0, 0, D, S, max_masks, score_thresh)  # img_w / img_h: per frame below
-    if rows is None:
-        rows = torch.empty((B, 1 + D * 7), dtype=torch.float32, device=scores.device)
-    if tuple(rows.shape) != (B, 1 + D * 7) or rows.dtype != torch.float32 or not rows.is_contiguous():
-        raise ValueError(f"rows must be contiguous float32 [{B}, {1 + D * 7}]")
+    rows = _out_tensor(rows, (B, 1 + D * 7), torch.float32, scores.device, f"rows must be contiguous float32 [{B}, {1 + D * 7}]")
     descs, canvases = _frames(frames, canvases, max_masks, scores.device, masks is not None)
     L.check(lib.trtx_rcnn_postprocess_frames_enqueue(C.byref(q), descs, B, _ptr(scores), _ptr(boxes), _ptr(classes),
                                                      None if masks is None else _ptr(masks), _ptr(rows), _stream(stream)),
@@ -1276,11 +1231,8 @@ def rcnn_contours(rows: torch.Tensor, canvases: Sequence[torch.Tensor], *, frame
     q = L.RcnnPostParams(0, 0, 0, 0, D, 1, int(max_masks), 0.0)  # only detections_per_im and max_masks are read
     descs, _ = _frames(frames, canvases, int(max_masks), rows.device, True)
     shapes = ((B, max_masks, 2), (B, max_masks, max_contours), (B, max_masks, max_points, 2))
-    if out is None:
-        out = tuple(torch.zeros(s, dtype=torch.int32, device=rows.device) for s in shapes)
-    for t, s in zip(out, shapes):
-        if tuple(t.shape) != tuple(s) or t.dtype != torch.int32 or not t.is_contiguous():
-            raise ValueError(f"out tensors must be contiguous int32 {shapes}")
+    out = tuple(_out_tensor(t, s, torch.int32, rows.device, f"out tensors must be contiguous int32 {shapes}", torch.zeros)
+                for t, s in zip((None,) * 3 if out is None else out, shapes))
     n = lib.trtx_rcnn_contours_workspace_size(C.byref(q), descs, B)
     if n == 0:
         raise ValueError("trtx_rcnn_contours_workspace_size rejected the arguments")
