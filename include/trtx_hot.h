@@ -255,7 +255,7 @@ TRTX_API int trtx_peer_free(void* dev_ptr);
 
 /* =====================================================================================
  * 3. Decode_TRT (RetinaFace) -- replaces retinaface/decode.cu:110-199
- *    inputs_dev[l] : [batch, 32, (in_h/s)*(in_w/s)] fp32, s = 8,16,32, channels [bbox 2x4 | cls 2x2 | lmk 2x10]
+ *    inputs_dev[l] : [batch, 32, (in_h/s)*(in_w/s)] fp32 (or fp16: in_dtype), s = 8,16,32, channels [bbox 2x4 | cls 2x2 | lmk 2x10]
  *    output_dev    : [batch, 1 + total_priors*15] fp32, rows x1,y1,x2,y2,conf,lmk[10]
  *    (TRTX_RETINA_ANTICOV: [batch, 38, g] inputs, [batch, 1 + total_priors*16] output)
  * ===================================================================================== */
@@ -270,10 +270,18 @@ typedef struct trtx_retina_params {
     int32_t in_h, in_w; /* decodeplugin::INPUT_H / INPUT_W (compile-time 480x640 in decode.h:16-17) */
     float gate;         /* 0.02 (decode.cu:131); compared as `conf <= gate`.  Unused by TRTX_RETINA_ANTICOV */
     int32_t variant;    /* TRTX_RETINA_FACE (0, what a zeroed struct selects) | TRTX_RETINA_ANTICOV */
+    int32_t in_dtype;   /* element type of all three inputs: TRTX_F32 (0, what a zeroed struct selects; the reference's only
+                           mode) | TRTX_F16.  A half is widened to float (exact) where the reference reads a float; the
+                           arithmetic and the fp32 output rows are the same code, so the rows are those of the fp32 call on
+                           the widened inputs */
 } trtx_retina_params;
 
 TRTX_API int trtx_retina_total_priors(const trtx_retina_params* p);
 TRTX_API size_t trtx_retina_workspace_size(const trtx_retina_params* p, int batch);
+/* TRTX_ERR_INVALID, before the first launch and with nothing written: a null argument, in_h or in_w < 32, an unknown variant
+ * or in_dtype, an input pointer that is not a multiple of its element size (4 / 2 bytes), an output pointer that is not a
+ * multiple of 4.  Inputs that are 16-byte (fp32) / 8-byte (fp16) aligned with grids of a multiple of 4 cells are read four
+ * cells per load, any other one cell per load; the rows do not depend on which. */
 TRTX_API int trtx_retina_decode_enqueue(const trtx_retina_params* p, int batch, const void* const* inputs_dev,
                                         float* output_dev, void* workspace_dev, size_t workspace_bytes,
                                         trtx_stream_t stream);
@@ -379,11 +387,33 @@ TRTX_API int trtx_scale_mask_enqueue(const float* masks_dev, int n, int net_w, i
 TRTX_API int trtx_roi_align(int batch, const float* rois_dev, const float* features_dev, float* out_dev, int pooler_resolution,
                             float spatial_scale, int sampling_ratio, int num_proposals, int out_channels, int feature_h,
                             int feature_w, trtx_stream_t stream);
+/* The same with the element type of features_dev AND out_dev chosen by dtype: TRTX_F32 (= trtx_roi_align, byte for byte) or
+ * TRTX_F16, so that an FP16 engine hands the plugin its half feature map and takes half bins without a reformat copy on
+ * either side.  rois_dev stays fp32 in both modes (a half holds a coordinate up to 1067 to 0.5 px only).
+ * The half result is DEFINED: every tap is widened to float (exact), sampled and summed exactly as in the fp32 mode, and
+ * only the finished bin is rounded, once, to nearest-even (overflow to +-inf, NaN stays NaN):
+ *     out = half(trtx_roi_align(float(features))), bit for bit.
+ * In the half mode the shared-memory window kernel takes out_channels % 8 == 0 (pooler 14, feature_h * feature_w <= 4096 as
+ * before); other shapes take every tap from global memory.
+ * TRTX_ERR_INVALID, before any launch and with nothing written: dtype not TRTX_F32 / TRTX_F16; a null pointer or a
+ * non-positive size; rois_dev not a multiple of 16 bytes (a proposal is one 16-byte load); features_dev or out_dev not a
+ * multiple of the element size (4 / 2 bytes). */
+TRTX_API int trtx_roi_align_typed(int dtype, int batch, const float* rois_dev, const void* features_dev, void* out_dev,
+                                  int pooler_resolution, float spatial_scale, int sampling_ratio, int num_proposals,
+                                  int out_channels, int feature_h, int feature_w, trtx_stream_t stream);
 /* indices_dev [batch, detections_per_im] class index as float; masks_dev [batch, detections_per_im, num_classes, S, S];
  * out_dev [batch, detections_per_im, S, S] = sigmoid of the predicted class' mask (rows with an index outside
  * [0, num_classes) are left untouched, as in the reference). */
 TRTX_API int trtx_mask_rcnn_inference(int batch, const float* indices_dev, const float* masks_dev, float* out_dev,
                                       int detections_per_im, int output_size, int num_classes, trtx_stream_t stream);
+/* The same with masks_dev of element type in_dtype: TRTX_F32 (= trtx_mask_rcnn_inference) or TRTX_F16 (the mask head of an
+ * FP16 engine).  A half is widened to float (exact) before the sigmoid; indices_dev and out_dev are fp32 in both modes
+ * (out_dev feeds trtx_rcnn_postprocess*).  TRTX_ERR_INVALID, before the launch and with nothing written: in_dtype not
+ * TRTX_F32 / TRTX_F16; a null pointer or a non-positive size; indices_dev or out_dev not a multiple of 4 bytes, masks_dev
+ * not a multiple of its element size. */
+TRTX_API int trtx_mask_rcnn_inference_typed(int in_dtype, int batch, const float* indices_dev, const void* masks_dev,
+                                            float* out_dev, int detections_per_im, int output_size, int num_classes,
+                                            trtx_stream_t stream);
 
 /* The INT8 calibrator's host pre-process (SURVEY 8f rank 4): Int8EntropyCalibrator2::getBatch, yolov8/src/calibrator.cpp:33-52
  * = preprocess_img (yolov8/include/utils.h:6-26: cv::resize INTER_LINEAR of the 8-bit image into the letterbox rectangle, 128-grey

@@ -350,8 +350,10 @@ class DecodePluginDynamic : public nvinfer1::IPluginV2DynamicExt {
     int enqueue(const nvinfer1::PluginTensorDesc* in, const nvinfer1::PluginTensorDesc*, const void* const* inputs, void* const* outputs,
                 void* workspace, cudaStream_t stream) TRTX_NOEXCEPT override {
         const int batch = in[0].dims.d[0];
-        return trtx_retina_decode_enqueue(&p_, batch, inputs, static_cast<float*>(outputs[0]), workspace,
-                                          trtx_retina_workspace_size(&p_, batch), stream);
+        trtx_retina_params p = p_;  // per-call copy: enqueue never mutates the plugin
+        p.in_dtype = in[0].type == nvinfer1::DataType::kHALF ? TRTX_F16 : TRTX_F32;
+        return trtx_retina_decode_enqueue(&p, batch, inputs, static_cast<float*>(outputs[0]), workspace,
+                                          trtx_retina_workspace_size(&p, batch), stream);
     }
     size_t getSerializationSize() const TRTX_NOEXCEPT override { return 8; }
     void serialize(void* buffer) const TRTX_NOEXCEPT override {
@@ -359,8 +361,11 @@ class DecodePluginDynamic : public nvinfer1::IPluginV2DynamicExt {
         detail::write(d, p_.in_h);
         detail::write(d, p_.in_w);
     }
-    bool supportsFormatCombination(int pos, const nvinfer1::PluginTensorDesc* io, int, int) TRTX_NOEXCEPT override {
-        return io[pos].format == nvinfer1::TensorFormat::kLINEAR && io[pos].type == nvinfer1::DataType::kFLOAT;
+    bool supportsFormatCombination(int pos, const nvinfer1::PluginTensorDesc* io, int nbInputs, int) TRTX_NOEXCEPT override {
+        if (io[pos].format != nvinfer1::TensorFormat::kLINEAR) return false;
+        if (pos < nbInputs)  // the three heads: all fp32 (the reference's only mode) or all fp16, as YoloLayerPluginDynamic
+            return (io[pos].type == nvinfer1::DataType::kFLOAT || io[pos].type == nvinfer1::DataType::kHALF) && io[pos].type == io[0].type;
+        return io[pos].type == nvinfer1::DataType::kFLOAT;
     }
     const char* getPluginType() const TRTX_NOEXCEPT override { return "Decode_TRT"; }
     const char* getPluginVersion() const TRTX_NOEXCEPT override { return "1"; }
@@ -422,7 +427,8 @@ class DecodePluginCreator : public nvinfer1::IPluginCreator {
 
 // ================================================================================================
 // Faster R-CNN plugins: IPluginV2Ext with the reference's constructors (rcnn/*Plugin.h), names "RpnDecode",
-// "RpnNms", "PredictorDecode", "BatchedNms", version "1", namespace "".  Implicit batch, fp32 linear only.
+// "RpnNms", "PredictorDecode", "BatchedNms", version "1", namespace "".  Implicit batch, fp32 linear only
+// (RoiAlignPluginIOExt / MaskRcnnInferencePluginIOExt below also take fp16 feature maps / masks).
 // ================================================================================================
 class RcnnPluginBase : public nvinfer1::IPluginV2Ext {
    public:
@@ -752,6 +758,192 @@ struct BatchedNmsPluginCreator : RcnnCreator<BatchedNmsPlugin> { BatchedNmsPlugi
 struct RoiAlignPluginCreator : RcnnCreator<RoiAlignPlugin> { RoiAlignPluginCreator() : RcnnCreator("RoiAlign") {} };
 struct MaskRcnnInferencePluginCreator : RcnnCreator<MaskRcnnInferencePlugin> { MaskRcnnInferencePluginCreator() : RcnnCreator("MaskRcnnInference") {} };
 
+// ------------------------------------------------------------------------------------------------
+// RoiAlign and MaskRcnnInference for an FP16 engine.  RoIAlign needs fp32 proposals next to half features, which
+// IPluginV2Ext::supportsFormat (one type for every tensor) cannot say; IPluginV2IOExt::supportsFormatCombination can.
+// Same plugin names, version, constructor arguments and namespace as the IPluginV2Ext classes above, which stay as they
+// are.  The element type TensorRT chose arrives in configurePlugin, is carried through clone() and is appended to the
+// serialized blob as one int32 (TRTX_F32 | TRTX_F16); a blob of the reference's length deserializes as fp32.
+// Exercised against tests/mock_trt only: how a real TensorRT builder drives these two classes is NOT verified.
+// ------------------------------------------------------------------------------------------------
+class RcnnIOExtBase : public nvinfer1::IPluginV2IOExt {
+   public:
+    int initialize() TRTX_NOEXCEPT override { return 0; }
+    void terminate() TRTX_NOEXCEPT override {}
+    void destroy() TRTX_NOEXCEPT override { delete this; }
+    size_t getWorkspaceSize(int) const TRTX_NOEXCEPT override { return 0; }
+    int getNbOutputs() const TRTX_NOEXCEPT override { return 1; }
+    const char* getPluginVersion() const TRTX_NOEXCEPT override { return "1"; }
+    const char* getPluginNamespace() const TRTX_NOEXCEPT override { return ""; }
+    void setPluginNamespace(const char*) TRTX_NOEXCEPT override {}
+    bool isOutputBroadcastAcrossBatch(int, const bool*, int) const TRTX_NOEXCEPT override { return false; }
+    bool canBroadcastInputAcrossBatch(int) const TRTX_NOEXCEPT override { return false; }
+    void attachToContext(cudnnContext*, cublasContext*, nvinfer1::IGpuAllocator*) TRTX_NOEXCEPT override {}
+    void detachFromContext() TRTX_NOEXCEPT override {}
+    int dtype() const { return dtype_; }
+
+   protected:
+    static bool float_or_half(nvinfer1::DataType t) { return t == nvinfer1::DataType::kFLOAT || t == nvinfer1::DataType::kHALF; }
+    // the trailing int32 of a blob that is 4 bytes longer than the reference's; false: an unknown type
+    bool read_dtype(const char* d, size_t length, size_t reference_length) {
+        if (length == reference_length) return true;
+        int32_t v;
+        detail::read(d, v);
+        if (v != TRTX_F32 && v != TRTX_F16) return false;
+        dtype_ = v;
+        return true;
+    }
+    int32_t dtype_ = TRTX_F32;  // of input 1: the feature map / the masks
+};
+
+class RoiAlignPluginIOExt : public RcnnIOExtBase {
+   public:
+    RoiAlignPluginIOExt(int pooler_resolution, float spatial_scale, int sampling_ratio, int num_proposals, int out_channels,
+                        int feature_h = 0, int feature_w = 0)
+        : pooler_(pooler_resolution), scale_(spatial_scale), sampling_(sampling_ratio), proposals_(num_proposals),
+          channels_(out_channels), fh_(feature_h), fw_(feature_w) {}
+    RoiAlignPluginIOExt(const void* data, size_t length) {  // RoiAlignPlugin.h:37-46 (+ the element type)
+        if (length != kReferenceBlob && length != kReferenceBlob + sizeof(int32_t)) {
+            valid_ = false;
+            return;
+        }
+        const char* d = static_cast<const char*>(data);
+        detail::read(d, pooler_);
+        detail::read(d, scale_);
+        detail::read(d, sampling_);
+        detail::read(d, proposals_);
+        detail::read(d, channels_);
+        detail::read(d, fh_);
+        detail::read(d, fw_);
+        valid_ = read_dtype(d, length, kReferenceBlob);
+    }
+    bool valid() const { return valid_; }  // false: the blob had neither the reference's length nor that + 4
+    const char* getPluginType() const TRTX_NOEXCEPT override { return "RoiAlign"; }
+    nvinfer1::Dims getOutputDimensions(int, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override {
+        return nvinfer1::Dims4(proposals_, channels_, pooler_, pooler_);
+    }
+    // proposals fp32; features fp32 or fp16; the bins in the features' type
+    bool supportsFormatCombination(int pos, const nvinfer1::PluginTensorDesc* io, int, int) const TRTX_NOEXCEPT override {
+        if (io[pos].format != nvinfer1::TensorFormat::kLINEAR) return false;
+        if (pos == 0) return io[0].type == nvinfer1::DataType::kFLOAT;
+        if (pos == 1) return float_or_half(io[1].type);
+        return io[pos].type == io[1].type;
+    }
+    nvinfer1::DataType getOutputDataType(int, const nvinfer1::DataType* inputTypes, int nbInputs) const TRTX_NOEXCEPT override {
+        return nbInputs > 1 ? inputTypes[1] : nvinfer1::DataType::kFLOAT;
+    }
+    void configurePlugin(const nvinfer1::PluginTensorDesc* in, int, const nvinfer1::PluginTensorDesc*, int) TRTX_NOEXCEPT override {
+        fh_ = in[1].dims.d[1];  // RoiAlignPlugin.h:151-152
+        fw_ = in[1].dims.d[2];
+        dtype_ = in[1].type == nvinfer1::DataType::kHALF ? TRTX_F16 : TRTX_F32;
+    }
+    int enqueue(int batchSize, const void* const* inputs, void* TRTX_CONST_ENQUEUE* outputs, void*, cudaStream_t stream) TRTX_NOEXCEPT override {
+        return trtx_roi_align_typed(dtype_, batchSize, static_cast<const float*>(inputs[0]), inputs[1], outputs[0], pooler_, scale_,
+                                    sampling_, proposals_, channels_, fh_, fw_, stream);
+    }
+    size_t getSerializationSize() const TRTX_NOEXCEPT override { return kReferenceBlob + sizeof(int32_t); }
+    void serialize(void* buffer) const TRTX_NOEXCEPT override {
+        char* d = static_cast<char*>(buffer);
+        detail::write(d, pooler_);
+        detail::write(d, scale_);
+        detail::write(d, sampling_);
+        detail::write(d, proposals_);
+        detail::write(d, channels_);
+        detail::write(d, fh_);
+        detail::write(d, fw_);
+        detail::write(d, dtype_);
+    }
+    nvinfer1::IPluginV2IOExt* clone() const TRTX_NOEXCEPT override {
+        auto* c = new RoiAlignPluginIOExt(pooler_, scale_, sampling_, proposals_, channels_, fh_, fw_);
+        c->dtype_ = dtype_;
+        return c;
+    }
+
+   private:
+    static constexpr size_t kReferenceBlob = 6 * sizeof(int) + sizeof(float);
+    int pooler_ = 0;
+    float scale_ = 0.f;
+    int sampling_ = 0, proposals_ = 0, channels_ = 0, fh_ = 0, fw_ = 0;
+    bool valid_ = true;
+};
+
+class MaskRcnnInferencePluginIOExt : public RcnnIOExtBase {
+   public:
+    MaskRcnnInferencePluginIOExt(int detections_per_im, int output_size, int num_classes = 1)
+        : dets_(detections_per_im), size_(output_size), classes_(num_classes) {}
+    MaskRcnnInferencePluginIOExt(const void* data, size_t length) {  // MaskRcnnInferencePlugin.h:32-37 (+ the element type)
+        if (length != kReferenceBlob && length != kReferenceBlob + sizeof(int32_t)) {
+            valid_ = false;
+            return;
+        }
+        const char* d = static_cast<const char*>(data);
+        detail::read(d, dets_);
+        detail::read(d, size_);
+        detail::read(d, classes_);
+        valid_ = read_dtype(d, length, kReferenceBlob);
+    }
+    bool valid() const { return valid_; }
+    const char* getPluginType() const TRTX_NOEXCEPT override { return "MaskRcnnInference"; }
+    nvinfer1::Dims getOutputDimensions(int, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override { return nvinfer1::Dims4(dets_, 1, size_, size_); }
+    // class indices fp32; masks fp32 or fp16; the probabilities fp32 (they feed trtx_rcnn_postprocess*)
+    bool supportsFormatCombination(int pos, const nvinfer1::PluginTensorDesc* io, int, int) const TRTX_NOEXCEPT override {
+        if (io[pos].format != nvinfer1::TensorFormat::kLINEAR) return false;
+        if (pos == 1) return float_or_half(io[1].type);
+        return io[pos].type == nvinfer1::DataType::kFLOAT;
+    }
+    nvinfer1::DataType getOutputDataType(int, const nvinfer1::DataType*, int) const TRTX_NOEXCEPT override { return nvinfer1::DataType::kFLOAT; }
+    void configurePlugin(const nvinfer1::PluginTensorDesc* in, int, const nvinfer1::PluginTensorDesc*, int) TRTX_NOEXCEPT override {
+        classes_ = in[1].dims.d[1];  // MaskRcnnInferencePlugin.h:119
+        dtype_ = in[1].type == nvinfer1::DataType::kHALF ? TRTX_F16 : TRTX_F32;
+    }
+    int enqueue(int batchSize, const void* const* inputs, void* TRTX_CONST_ENQUEUE* outputs, void*, cudaStream_t stream) TRTX_NOEXCEPT override {
+        return trtx_mask_rcnn_inference_typed(dtype_, batchSize, static_cast<const float*>(inputs[0]), inputs[1],
+                                              static_cast<float*>(outputs[0]), dets_, size_, classes_, stream);
+    }
+    size_t getSerializationSize() const TRTX_NOEXCEPT override { return kReferenceBlob + sizeof(int32_t); }
+    void serialize(void* buffer) const TRTX_NOEXCEPT override {
+        char* d = static_cast<char*>(buffer);
+        detail::write(d, dets_);
+        detail::write(d, size_);
+        detail::write(d, classes_);
+        detail::write(d, dtype_);
+    }
+    nvinfer1::IPluginV2IOExt* clone() const TRTX_NOEXCEPT override {
+        auto* c = new MaskRcnnInferencePluginIOExt(dets_, size_, classes_);
+        c->dtype_ = dtype_;
+        return c;
+    }
+
+   private:
+    static constexpr size_t kReferenceBlob = 3 * sizeof(int);
+    int dets_ = 0, size_ = 0, classes_ = 0;
+    bool valid_ = true;
+};
+
+// deserializePlugin for the two classes above: a blob of neither accepted length is refused (nullptr)
+template <typename P>
+class RcnnIOExtCreator : public nvinfer1::IPluginCreator {
+   public:
+    explicit RcnnIOExtCreator(const char* name) : name_(name) {}
+    const char* getPluginName() const TRTX_NOEXCEPT override { return name_; }
+    const char* getPluginVersion() const TRTX_NOEXCEPT override { return "1"; }
+    const char* getPluginNamespace() const TRTX_NOEXCEPT override { return ""; }
+    void setPluginNamespace(const char*) TRTX_NOEXCEPT override {}
+    const nvinfer1::PluginFieldCollection* getFieldNames() TRTX_NOEXCEPT override { return nullptr; }
+    nvinfer1::IPluginV2* createPlugin(const char*, const nvinfer1::PluginFieldCollection*) TRTX_NOEXCEPT override { return nullptr; }  // as the reference
+    nvinfer1::IPluginV2* deserializePlugin(const char*, const void* data, size_t len) TRTX_NOEXCEPT override {
+        P* p = new P(data, len);
+        if (p->valid()) return p;
+        delete p;
+        return nullptr;
+    }
+
+   private:
+    const char* name_;
+};
+struct RoiAlignPluginIOExtCreator : RcnnIOExtCreator<RoiAlignPluginIOExt> { RoiAlignPluginIOExtCreator() : RcnnIOExtCreator("RoiAlign") {} };
+struct MaskRcnnInferencePluginIOExtCreator : RcnnIOExtCreator<MaskRcnnInferencePluginIOExt> { MaskRcnnInferencePluginIOExtCreator() : RcnnIOExtCreator("MaskRcnnInference") {} };
+
 }  // namespace trtx
 
 #ifdef TRTX_REGISTER_PLUGINS
@@ -766,8 +958,13 @@ REGISTER_TENSORRT_PLUGIN(RpnDecodePluginCreator);
 REGISTER_TENSORRT_PLUGIN(RpnNmsPluginCreator);
 REGISTER_TENSORRT_PLUGIN(PredictorDecodePluginCreator);
 REGISTER_TENSORRT_PLUGIN(BatchedNmsPluginCreator);
+#ifdef TRTX_RCNN_HALF_IO_PLUGINS  // "RoiAlign" / "MaskRcnnInference" that also accept fp16 feature maps / masks
+REGISTER_TENSORRT_PLUGIN(RoiAlignPluginIOExtCreator);
+REGISTER_TENSORRT_PLUGIN(MaskRcnnInferencePluginIOExtCreator);
+#else
 REGISTER_TENSORRT_PLUGIN(RoiAlignPluginCreator);
 REGISTER_TENSORRT_PLUGIN(MaskRcnnInferencePluginCreator);
+#endif
 }  // namespace trtx
 #endif
 

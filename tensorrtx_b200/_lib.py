@@ -73,7 +73,7 @@ class Gather(C.Structure):
 
 
 class RetinaParams(C.Structure):
-    _fields_ = [("in_h", C.c_int32), ("in_w", C.c_int32), ("gate", C.c_float), ("variant", C.c_int32)]
+    _fields_ = [("in_h", C.c_int32), ("in_w", C.c_int32), ("gate", C.c_float), ("variant", C.c_int32), ("in_dtype", C.c_int32)]
 
 
 class ImageDesc(C.Structure):
@@ -140,9 +140,11 @@ SYMBOLS = {
     "trtx_preprocess_batch_enqueue": (_i, [C.POINTER(ImageDesc), _i, _vp, _i, _i, _i, _vp]),
     "trtx_get_rect": (_i, [_i, _i, _i, _i, _i, C.POINTER(C.c_float), C.POINTER(C.c_int)]),
     "trtx_roi_align": (_i, [_i, _vp, _vp, _vp, _i, C.c_float, _i, _i, _i, _i, _i, _vp]),
+    "trtx_roi_align_typed": (_i, [_i, _i, _vp, _vp, _vp, _i, C.c_float, _i, _i, _i, _i, _i, _vp]),
     "trtx_calib_letterbox_rect": (_i, [_i, _i, _i, _i, C.POINTER(C.c_int)]),
     "trtx_calib_letterbox_host": (_i, [_vp, _i, _i, C.c_size_t, _i, _i, _vp]),
     "trtx_mask_rcnn_inference": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "trtx_mask_rcnn_inference_typed": (_i, [_i, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "trtx_process_mask_enqueue": (_i, [C.POINTER(MaskParams), _i, _vp, _vp, _i, _vp, _vp]),
     "trtx_letterbox_matrix": (None, [_i, _i, _i, _i, C.POINTER(C.c_float)]),
     "trtx_abi_sizeof": (_sz, [_i]),

@@ -20,7 +20,7 @@
 namespace trtx {
 
 struct RetinaLevel {
-    const float* in;
+    const void* in;  // [B, 32 | 38, g] of the scan's element type
     int g, w, h;
     int tile_begin;
     int slot_begin;
@@ -37,7 +37,9 @@ struct RetinaArgs {
     int total_priors;
 };
 
-template <int VEC>
+// T: the heads' element type (float | __half).  Every read goes through Elem<T>, which widens a half to float exactly, so
+// the decode below -- the double-precision literals included -- is the same code on the same floats in both modes.
+template <typename T, int VEC>
 __global__ void __launch_bounds__(128) retina_scan_kernel(const __grid_constant__ RetinaArgs a, int batch) {
     constexpr int TILE = 32 * VEC;
     const int lane = threadIdx.x & 31;
@@ -52,8 +54,8 @@ __global__ void __launch_bounds__(128) retina_scan_kernel(const __grid_constant_
     const int a0 = tile * TILE + lane * VEC;
     const size_t g = (size_t)L.g;
     const bool active = a0 < L.g;
-    const float* cur = L.in + (size_t)b * 32 * g;
-    const float* cls_reg = cur + 8 * g;
+    const T* cur = static_cast<const T*>(L.in) + (size_t)b * 32 * g;
+    const T* cls_reg = cur + 8 * g;
 
     float c[4][VEC];
 #pragma unroll
@@ -62,13 +64,13 @@ __global__ void __launch_bounds__(128) retina_scan_kernel(const __grid_constant_
         for (int j = 0; j < VEC; ++j) c[r][j] = 0.0f;
         if (active) {
             if constexpr (VEC == 4) {
-                float4 v = ldg_stream_f4(cls_reg + (size_t)r * g + a0);
+                float4 v = Elem<T>::ld4(cls_reg + (size_t)r * g + a0);
                 c[r][0] = v.x;
                 c[r][1] = v.y;
                 c[r][2] = v.z;
                 c[r][3] = v.w;
             } else {
-                c[r][0] = ldg_stream_f1(cls_reg + (size_t)r * g + a0);
+                c[r][0] = Elem<T>::ld1(cls_reg + (size_t)r * g + a0);
             }
         }
     }
@@ -91,8 +93,8 @@ __global__ void __launch_bounds__(128) retina_scan_kernel(const __grid_constant_
     if (lane == 0) a.tile_count[(size_t)b * a.tiles_per_image + t] = total;
     if (!flags) return;
     const size_t slot0 = (size_t)b * a.slots_per_image + L.slot_begin + (size_t)tile * TILE * 2;
-    const float* bbox_reg = cur;
-    const float* lmk_reg = cur + 12 * g;
+    const T* bbox_reg = cur;
+    const T* lmk_reg = cur + 12 * g;
 #pragma unroll
     for (int j = 0; j < VEC; ++j) {
 #pragma unroll
@@ -106,11 +108,11 @@ __global__ void __launch_bounds__(128) retina_scan_kernel(const __grid_constant_
             prior[2] = (float)L.anchor * (k + 1) / a.in_w;
             prior[3] = (float)L.anchor * (k + 1) / a.in_h;
             float d[15];
-            const float* br = bbox_reg + idx + (size_t)k * 4 * g;
-            d[0] = (float)(prior[0] + (double)__ldg(br) * 0.1 * prior[2]);  // :145-156
-            d[1] = (float)(prior[1] + (double)__ldg(br + g) * 0.1 * prior[3]);
-            d[2] = prior[2] * expf((float)((double)__ldg(br + 2 * g) * 0.2));
-            d[3] = prior[3] * expf((float)((double)__ldg(br + 3 * g) * 0.2));
+            const T* br = bbox_reg + idx + (size_t)k * 4 * g;
+            d[0] = (float)(prior[0] + (double)Elem<T>::ld1_cached(br) * 0.1 * prior[2]);  // :145-156
+            d[1] = (float)(prior[1] + (double)Elem<T>::ld1_cached(br + g) * 0.1 * prior[3]);
+            d[2] = prior[2] * expf((float)((double)Elem<T>::ld1_cached(br + 2 * g) * 0.2));
+            d[3] = prior[3] * expf((float)((double)Elem<T>::ld1_cached(br + 3 * g) * 0.2));
             d[0] -= d[2] / 2;
             d[1] -= d[3] / 2;
             d[2] += d[0];
@@ -120,11 +122,11 @@ __global__ void __launch_bounds__(128) retina_scan_kernel(const __grid_constant_
             d[2] *= a.in_w;
             d[3] *= a.in_h;
             d[4] = conf[j][k];
-            const float* lr = lmk_reg + idx + (size_t)k * 10 * g;
+            const T* lr = lmk_reg + idx + (size_t)k * 10 * g;
 #pragma unroll
             for (int i = 0; i < 10; i += 2) {  // :158-163
-                d[5 + i] = (float)(prior[0] + (double)__ldg(lr + (size_t)i * g) * 0.1 * prior[2]);
-                d[5 + i + 1] = (float)(prior[1] + (double)__ldg(lr + (size_t)(i + 1) * g) * 0.1 * prior[3]);
+                d[5 + i] = (float)(prior[0] + (double)Elem<T>::ld1_cached(lr + (size_t)i * g) * 0.1 * prior[2]);
+                d[5 + i + 1] = (float)(prior[1] + (double)Elem<T>::ld1_cached(lr + (size_t)(i + 1) * g) * 0.1 * prior[3]);
                 d[5 + i] *= a.in_w;
                 d[5 + i + 1] *= a.in_h;
             }
@@ -139,7 +141,7 @@ __global__ void __launch_bounds__(128) retina_scan_kernel(const __grid_constant_
 }
 
 // retinafaceAntiCov/decode.cu:110-155.  Same tiling; the face probability of prior k is channel 2+k as it comes.
-template <int VEC>
+template <typename T, int VEC>
 __global__ void __launch_bounds__(128) anticov_scan_kernel(const __grid_constant__ RetinaArgs a, int batch) {
     constexpr int TILE = 32 * VEC;
     const int lane = threadIdx.x & 31;
@@ -154,8 +156,8 @@ __global__ void __launch_bounds__(128) anticov_scan_kernel(const __grid_constant
     const int a0 = tile * TILE + lane * VEC;
     const size_t g = (size_t)L.g;
     const bool active = a0 < L.g;
-    const float* cur = L.in + (size_t)b * 38 * g;
-    const float* cls_reg = cur + 2 * g;  // :120
+    const T* cur = static_cast<const T*>(L.in) + (size_t)b * 38 * g;
+    const T* cls_reg = cur + 2 * g;  // :120
     float c[2][VEC];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -163,13 +165,13 @@ __global__ void __launch_bounds__(128) anticov_scan_kernel(const __grid_constant
         for (int j = 0; j < VEC; ++j) c[r][j] = 0.0f;
         if (active) {
             if constexpr (VEC == 4) {
-                float4 v = ldg_stream_f4(cls_reg + (size_t)r * g + a0);
+                float4 v = Elem<T>::ld4(cls_reg + (size_t)r * g + a0);
                 c[r][0] = v.x;
                 c[r][1] = v.y;
                 c[r][2] = v.z;
                 c[r][3] = v.w;
             } else {
-                c[r][0] = ldg_stream_f1(cls_reg + (size_t)r * g + a0);
+                c[r][0] = Elem<T>::ld1(cls_reg + (size_t)r * g + a0);
             }
         }
     }
@@ -184,9 +186,9 @@ __global__ void __launch_bounds__(128) anticov_scan_kernel(const __grid_constant
     if (lane == 0) a.tile_count[(size_t)b * a.tiles_per_image + t] = total;
     if (!flags) return;
     const size_t slot0 = (size_t)b * a.slots_per_image + L.slot_begin + (size_t)tile * TILE * 2;
-    const float* bbox_reg = cur + 4 * g;
-    const float* lmk_reg = cur + 12 * g;
-    const float* mask_reg = cur + 36 * g;
+    const T* bbox_reg = cur + 4 * g;
+    const T* lmk_reg = cur + 12 * g;
+    const T* mask_reg = cur + 36 * g;
     const int step = a.in_w / L.w;  // 8, 16, 32 (:162-170)
 #pragma unroll
     for (int j = 0; j < VEC; ++j) {
@@ -201,23 +203,23 @@ __global__ void __launch_bounds__(128) anticov_scan_kernel(const __grid_constant
             prior[2] = (float)(L.anchor * 2 / (k + 1));
             prior[3] = prior[2];
             float d[16];
-            const float* br = bbox_reg + idx + (size_t)k * 4 * g;
-            d[0] = prior[0] + __ldg(br) * prior[2];  // :141-148 (float; contracted like the reference build)
-            d[1] = prior[1] + __ldg(br + g) * prior[3];
-            d[2] = prior[2] * expf(__ldg(br + 2 * g));
-            d[3] = prior[3] * expf(__ldg(br + 3 * g));
+            const T* br = bbox_reg + idx + (size_t)k * 4 * g;
+            d[0] = prior[0] + Elem<T>::ld1_cached(br) * prior[2];  // :141-148 (float; contracted like the reference build)
+            d[1] = prior[1] + Elem<T>::ld1_cached(br + g) * prior[3];
+            d[2] = prior[2] * expf(Elem<T>::ld1_cached(br + 2 * g));
+            d[3] = prior[3] * expf(Elem<T>::ld1_cached(br + 3 * g));
             d[0] -= (d[2] - 1) / 2;
             d[1] -= (d[3] - 1) / 2;
             d[2] += d[0];
             d[3] += d[1];
             d[4] = c[k][j];
-            const float* lr = lmk_reg + idx + (size_t)k * 10 * g;
+            const T* lr = lmk_reg + idx + (size_t)k * 10 * g;
 #pragma unroll
             for (int i = 0; i < 10; i += 2) {  // :150-153: `* 0.2` promotes to double
-                d[5 + i] = (float)(prior[0] + (double)__ldg(lr + (size_t)i * g) * 0.2 * prior[2]);
-                d[5 + i + 1] = (float)(prior[1] + (double)__ldg(lr + (size_t)(i + 1) * g) * 0.2 * prior[3]);
+                d[5 + i] = (float)(prior[0] + (double)Elem<T>::ld1_cached(lr + (size_t)i * g) * 0.2 * prior[2]);
+                d[5 + i + 1] = (float)(prior[1] + (double)Elem<T>::ld1_cached(lr + (size_t)(i + 1) * g) * 0.2 * prior[3]);
             }
-            d[15] = __ldg(mask_reg + idx + (size_t)k * g);  // :154
+            d[15] = Elem<T>::ld1_cached(mask_reg + idx + (size_t)k * g);  // :154
             float4* rec = reinterpret_cast<float4*>(a.cand + (slot0 + off) * 16);
             rec[0] = make_float4(d[0], d[1], d[2], d[3]);
             rec[1] = make_float4(d[4], d[5], d[6], d[7]);
@@ -287,6 +289,19 @@ static RetinaLayout retina_layout(const trtx_retina_params* p, int batch, int ve
     return L;
 }
 
+template <typename T>
+static void retina_scan_launch(bool anticov, int vec, const RetinaArgs& a, int batch, int warps, cudaStream_t st) {
+    if (anticov) {
+        if (vec == 4)
+            anticov_scan_kernel<T, 4><<<(warps + 3) / 4, 128, 0, st>>>(a, batch);
+        else
+            anticov_scan_kernel<T, 1><<<(warps + 3) / 4, 128, 0, st>>>(a, batch);
+    } else if (vec == 4)
+        retina_scan_kernel<T, 4><<<(warps + 3) / 4, 128, 0, st>>>(a, batch);
+    else
+        retina_scan_kernel<T, 1><<<(warps + 3) / 4, 128, 0, st>>>(a, batch);
+}
+
 }  // namespace trtx
 
 using namespace trtx;
@@ -311,11 +326,14 @@ TRTX_API int trtx_retina_decode_enqueue(const trtx_retina_params* p, int batch, 
     if (!p || batch <= 0 || !inputs_dev || !output_dev || !workspace_dev) return TRTX_ERR_INVALID;
     if (p->in_h < 32 || p->in_w < 32) return TRTX_ERR_INVALID;
     if (p->variant != TRTX_RETINA_FACE && p->variant != TRTX_RETINA_ANTICOV) return TRTX_ERR_INVALID;
+    if (p->in_dtype != TRTX_F32 && p->in_dtype != TRTX_F16) return TRTX_ERR_INVALID;
+    const size_t elem = p->in_dtype == TRTX_F16 ? sizeof(__half) : sizeof(float);
+    if (reinterpret_cast<uintptr_t>(output_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
     int vec = 4, step = 8;
     for (int l = 0; l < 3; ++l, step *= 2) {
-        if (!inputs_dev[l]) return TRTX_ERR_INVALID;
+        if (!inputs_dev[l] || reinterpret_cast<uintptr_t>(inputs_dev[l]) % elem != 0) return TRTX_ERR_INVALID;
         int g = (p->in_h / step) * (p->in_w / step);
-        if (g % 4 != 0 || reinterpret_cast<uintptr_t>(inputs_dev[l]) % 16 != 0) vec = 1;
+        if (g % 4 != 0 || reinterpret_cast<uintptr_t>(inputs_dev[l]) % (4 * elem) != 0) vec = 1;  // four cells per load
     }
     RetinaLayout L = retina_layout(p, batch, vec);
     if (workspace_bytes < L.total) return TRTX_ERR_WORKSPACE;
@@ -323,7 +341,7 @@ TRTX_API int trtx_retina_decode_enqueue(const trtx_retina_params* p, int batch, 
     step = 8;
     int anchor = 16;
     for (int l = 0; l < 3; ++l, step *= 2, anchor *= 4) {
-        a.lv[l].in = static_cast<const float*>(inputs_dev[l]);
+        a.lv[l].in = inputs_dev[l];
         a.lv[l].h = p->in_h / step;
         a.lv[l].w = p->in_w / step;
         a.lv[l].g = a.lv[l].h * a.lv[l].w;
@@ -343,15 +361,11 @@ TRTX_API int trtx_retina_decode_enqueue(const trtx_retina_params* p, int batch, 
     a.det_floats = p->variant == TRTX_RETINA_ANTICOV ? 16 : 15;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int warps = batch * L.tiles;
-    if (p->variant == TRTX_RETINA_ANTICOV) {
-        if (vec == 4)
-            anticov_scan_kernel<4><<<(warps + 3) / 4, 128, 0, st>>>(a, batch);
-        else
-            anticov_scan_kernel<1><<<(warps + 3) / 4, 128, 0, st>>>(a, batch);
-    } else if (vec == 4)
-        retina_scan_kernel<4><<<(warps + 3) / 4, 128, 0, st>>>(a, batch);
+    const bool anticov = p->variant == TRTX_RETINA_ANTICOV;
+    if (p->in_dtype == TRTX_F16)
+        retina_scan_launch<__half>(anticov, vec, a, batch, warps, st);
     else
-        retina_scan_kernel<1><<<(warps + 3) / 4, 128, 0, st>>>(a, batch);
+        retina_scan_launch<float>(anticov, vec, a, batch, warps, st);
     int rc = check_launch();
     if (rc) return rc;
     const size_t smem = sizeof(int) * (size_t)(L.tiles + 1);

@@ -145,7 +145,8 @@ class DetectionPipeline:
 class RetinaPipeline:
     """retina_r50.cpp's per-batch loop on the device: letterbox of the frames, Decode_TRT over the three head tensors,
     nms() with landmarks (retinaface/retina_r50.cpp:320-360, common.hpp:110-130).  Same structure as DetectionPipeline:
-    decode + NMS on a high-priority side stream next to the letterbox."""
+    decode + NMS on a high-priority side stream next to the letterbox.  The heads may be torch.float32 or torch.float16 (an
+    FP16 engine's outputs), all three alike: DecodePlugin.enqueue takes the element type from them."""
 
     def __init__(self, batch: int, in_h: int = 640, in_w: int = 640, max_det: int = 2048, device="cuda"):
         from .plugins import DecodePlugin, float_le_threshold, nms_params

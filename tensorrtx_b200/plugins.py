@@ -35,6 +35,28 @@ def _ptr(t) -> int:
     return int(t)
 
 
+def _elem_dtype(tensors, what: str, only=None) -> int:
+    """TRTX_F32 / TRTX_F16 of tensors that share one element type: the tensors' dtype is the selector, no option to set.  A raw
+    integer address carries no dtype and means fp32.  Another dtype, a mix, or a dtype other than `only` raises TrtxError,
+    before the library is called with a pointer it would read as the wrong type."""
+    codes = set()
+    for t in tensors:
+        if not isinstance(t, torch.Tensor):
+            codes.add(L.F32)
+        elif t.dtype == torch.float32:
+            codes.add(L.F32)
+        elif t.dtype == torch.float16:
+            codes.add(L.F16)
+        else:
+            raise L.TrtxError(f"{what}: {t.dtype} tensors are not accepted (torch.float32 or torch.float16)")
+    if len(codes) != 1:
+        raise L.TrtxError(f"{what}: tensors of mixed dtypes (all torch.float32 or all torch.float16)")
+    code = codes.pop()
+    if only is not None and code != only:
+        raise L.TrtxError(f"{what}: must be torch.float32")
+    return code
+
+
 def _stream(stream=None) -> int:
     if stream is None:
         return torch.cuda.current_stream().cuda_stream
@@ -783,8 +805,12 @@ class DecodePlugin:
         return int(self._lib.trtx_retina_workspace_size(C.byref(self.params), int(maxBatchSize)))
 
     def enqueue(self, batchSize: int, inputs, outputs, workspace, stream=None) -> int:
+        """The heads may be torch.float32 (the reference's mode) or torch.float16, all three alike; the rows are fp32."""
+        p = L.RetinaParams.from_buffer_copy(self.params)  # per-call copy: enqueue never mutates the plugin
+        p.in_dtype = _elem_dtype(inputs, "Decode_TRT inputs")
+        _elem_dtype(outputs[:1], "Decode_TRT output", only=L.F32)
         ptrs = L.ptr_array([_ptr(t) for t in inputs])
-        return int(self._lib.trtx_retina_decode_enqueue(C.byref(self.params), int(batchSize), ptrs, _ptr(outputs[0]),
+        return int(self._lib.trtx_retina_decode_enqueue(C.byref(p), int(batchSize), ptrs, _ptr(outputs[0]),
                                                         _ptr(workspace), _nbytes(workspace), _stream(stream)))
 
     def getPluginType(self) -> str:
@@ -986,9 +1012,14 @@ class RoiAlignPlugin:
         return 0
 
     def enqueue(self, batchSize, inputs, outputs, workspace=None, stream=None) -> int:
-        return int(self._lib.trtx_roi_align(batchSize, _ptr(inputs[0]), _ptr(inputs[1]), _ptr(outputs[0]), self._pooler_resolution,
-                                            self._spatial_scale, self._sampling_ratio, self._num_proposals, self._out_channels,
-                                            self._feature_h, self._feature_w, _stream(stream)))
+        """Features and output share one dtype, torch.float32 or torch.float16 (the bins are then the fp32 bins of the widened
+        features, rounded once); the proposals are torch.float32 in both modes."""
+        _elem_dtype(inputs[:1], "RoiAlign proposals", only=L.F32)
+        dt = _elem_dtype([inputs[1], outputs[0]], "RoiAlign features and output")
+        return int(self._lib.trtx_roi_align_typed(dt, batchSize, _ptr(inputs[0]), _ptr(inputs[1]), _ptr(outputs[0]),
+                                                  self._pooler_resolution, self._spatial_scale, self._sampling_ratio,
+                                                  self._num_proposals, self._out_channels, self._feature_h, self._feature_w,
+                                                  _stream(stream)))
 
 
 class MaskRcnnInferencePlugin:
@@ -1012,9 +1043,12 @@ class MaskRcnnInferencePlugin:
         return 0
 
     def enqueue(self, batchSize, inputs, outputs, workspace=None, stream=None) -> int:
-        return int(self._lib.trtx_mask_rcnn_inference(batchSize, _ptr(inputs[0]), _ptr(inputs[1]), _ptr(outputs[0]),
-                                                      self._detections_per_im, self._output_size, self._num_classes,
-                                                      _stream(stream)))
+        """The masks may be torch.float32 or torch.float16; indices and output are torch.float32 in both modes."""
+        _elem_dtype([inputs[0], outputs[0]], "MaskRcnnInference indices and output", only=L.F32)
+        dt = _elem_dtype(inputs[1:2], "MaskRcnnInference masks")
+        return int(self._lib.trtx_mask_rcnn_inference_typed(dt, batchSize, _ptr(inputs[0]), _ptr(inputs[1]), _ptr(outputs[0]),
+                                                            self._detections_per_im, self._output_size, self._num_classes,
+                                                            _stream(stream)))
 
 
 def _image_descs(images: Sequence[torch.Tensor]):
