@@ -313,6 +313,27 @@ TRTX_API int64_t trtx_predictor_decode(int batch, const float* scores_dev, const
                                        float* out_classes_dev, int num_boxes, int num_classes, int image_height,
                                        int image_width, const float* bbox_reg_weights_host, void* workspace_dev,
                                        size_t workspace_bytes, trtx_stream_t stream);
+/* rpnDecode and predictorDecode with scores_dev AND deltas_dev of element type in_dtype: TRTX_F32 (= the untyped call, byte for
+ * byte) or TRTX_F16, so that an FP16 engine hands both plugins the heads' half tensors without a reformat copy.  Every output
+ * stays fp32 in both modes (scores, boxes up to the image size -- a half holds 1067 to 0.5 px only -- and classes: they feed
+ * rpnNms, batchedNms and trtx_rcnn_postprocess*), and so do proposals_dev (rpnNms's output).  The half result is DEFINED as
+ * the fp32 call on the widened tensors, bit for bit:
+ *     trtx_*_decode_typed(TRTX_F16, h, ...) == trtx_*_decode(float(h), ...)
+ * where float() is the device's exact widening; the order is the fp32 order (stable descending, -0.0 == +0.0, a NaN where its
+ * widened value ranks).  The half select ranks 16-bit keys (two radix passes over 2-byte loads instead of four over 4-byte
+ * ones).  The workspace query, limits and return codes are those of the untyped calls; the size does not depend on the type.
+ * -TRTX_ERR_INVALID, before any launch and with nothing written: in_dtype not TRTX_F32 / TRTX_F16 (workspace query
+ * included); in the half mode a scores_dev or deltas_dev not a multiple of 2 bytes, in predictorDecode a deltas_dev not a
+ * multiple of 8 bytes (a candidate's 4 deltas are one load).  The fp32 mode checks what the untyped call checks, no more. */
+TRTX_API int64_t trtx_rpn_decode_typed(int in_dtype, int batch, const void* scores_dev, const void* deltas_dev,
+                                       float* out_scores_dev, float* out_boxes_dev, int height, int width, int image_height,
+                                       int image_width, float stride, const float* anchors_host, int num_anchors, int top_n,
+                                       void* workspace_dev, size_t workspace_bytes, trtx_stream_t stream);
+TRTX_API int64_t trtx_predictor_decode_typed(int in_dtype, int batch, const void* scores_dev, const void* deltas_dev,
+                                             const float* proposals_dev, float* out_scores_dev, float* out_boxes_dev,
+                                             float* out_classes_dev, int num_boxes, int num_classes, int image_height,
+                                             int image_width, const float* bbox_reg_weights_host, void* workspace_dev,
+                                             size_t workspace_bytes, trtx_stream_t stream);
 /* batchedNms, rcnn/BatchedNms.cu:92-162.  nms_method 0 hard / 1 soft-linear / 2 soft-gaussian. */
 TRTX_API int64_t trtx_batched_nms(int nms_method, int batch, const float* scores_dev, const float* boxes_dev,
                                   const float* classes_dev, float* out_scores_dev, float* out_boxes_dev,

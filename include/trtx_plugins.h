@@ -428,7 +428,7 @@ class DecodePluginCreator : public nvinfer1::IPluginCreator {
 // ================================================================================================
 // Faster R-CNN plugins: IPluginV2Ext with the reference's constructors (rcnn/*Plugin.h), names "RpnDecode",
 // "RpnNms", "PredictorDecode", "BatchedNms", version "1", namespace "".  Implicit batch, fp32 linear only
-// (RoiAlignPluginIOExt / MaskRcnnInferencePluginIOExt below also take fp16 feature maps / masks).
+// (the *PluginIOExt classes below also take fp16 feature maps / masks / scores and deltas).
 // ================================================================================================
 class RcnnPluginBase : public nvinfer1::IPluginV2Ext {
    public:
@@ -759,12 +759,13 @@ struct RoiAlignPluginCreator : RcnnCreator<RoiAlignPlugin> { RoiAlignPluginCreat
 struct MaskRcnnInferencePluginCreator : RcnnCreator<MaskRcnnInferencePlugin> { MaskRcnnInferencePluginCreator() : RcnnCreator("MaskRcnnInference") {} };
 
 // ------------------------------------------------------------------------------------------------
-// RoiAlign and MaskRcnnInference for an FP16 engine.  RoIAlign needs fp32 proposals next to half features, which
-// IPluginV2Ext::supportsFormat (one type for every tensor) cannot say; IPluginV2IOExt::supportsFormatCombination can.
-// Same plugin names, version, constructor arguments and namespace as the IPluginV2Ext classes above, which stay as they
-// are.  The element type TensorRT chose arrives in configurePlugin, is carried through clone() and is appended to the
-// serialized blob as one int32 (TRTX_F32 | TRTX_F16); a blob of the reference's length deserializes as fp32.
-// Exercised against tests/mock_trt only: how a real TensorRT builder drives these two classes is NOT verified.
+// RoiAlign, MaskRcnnInference, RpnDecode and PredictorDecode for an FP16 engine.  Each needs fp32 tensors next to half
+// ones (proposals, class indices, fp32 outputs), which IPluginV2Ext::supportsFormat (one type for every tensor) cannot say;
+// IPluginV2IOExt::supportsFormatCombination can.  Same plugin names, version, constructor arguments and namespace as the
+// IPluginV2Ext classes above, which stay as they are.  The element type TensorRT chose arrives in configurePlugin, is
+// carried through clone() and is appended to the serialized blob as one int32 (TRTX_F32 | TRTX_F16); a blob of the
+// reference's length deserializes as fp32, a blob of any other length is refused.
+// Exercised against tests/mock_trt only: how a real TensorRT builder drives these four classes is NOT verified.
 // ------------------------------------------------------------------------------------------------
 class RcnnIOExtBase : public nvinfer1::IPluginV2IOExt {
    public:
@@ -793,7 +794,7 @@ class RcnnIOExtBase : public nvinfer1::IPluginV2IOExt {
         dtype_ = v;
         return true;
     }
-    int32_t dtype_ = TRTX_F32;  // of input 1: the feature map / the masks
+    int32_t dtype_ = TRTX_F32;  // of the half-capable inputs: the feature map / the masks / the scores and deltas
 };
 
 class RoiAlignPluginIOExt : public RcnnIOExtBase {
@@ -920,7 +921,170 @@ class MaskRcnnInferencePluginIOExt : public RcnnIOExtBase {
     bool valid_ = true;
 };
 
-// deserializePlugin for the two classes above: a blob of neither accepted length is refused (nullptr)
+// RpnDecode and PredictorDecode for an FP16 engine: scores and deltas fp32 or fp16 (one type for both), PredictorDecode's
+// proposals and every output fp32 (trtx_rpn_decode_typed / trtx_predictor_decode_typed).  Same names, version, constructor
+// arguments and namespace as RpnDecodePlugin / PredictorDecodePlugin, same blob + the trailing int32 element type.
+class RpnDecodePluginIOExt : public RcnnIOExtBase {
+   public:
+    RpnDecodePluginIOExt(int top_n, const std::vector<float>& anchors, float stride, size_t image_height, size_t image_width)
+        : top_n_(top_n), anchors_(anchors), stride_(stride), height_(0), width_(0), image_height_(image_height), image_width_(image_width) {}
+    RpnDecodePluginIOExt(int top_n, const std::vector<float>& anchors, float stride, size_t height, size_t width, size_t image_height,
+                         size_t image_width)
+        : top_n_(top_n), anchors_(anchors), stride_(stride), height_(height), width_(width), image_height_(image_height), image_width_(image_width) {}
+    RpnDecodePluginIOExt(const void* data, size_t length) {  // RpnDecodePlugin.h:42-58 (+ the element type)
+        const char* d = static_cast<const char*>(data);
+        size_t n = 0;
+        valid_ = length >= sizeof(top_n_) + sizeof(size_t);
+        if (valid_) {
+            detail::read(d, top_n_);
+            detail::read(d, n);
+            valid_ = n <= length / sizeof(float) &&
+                     (length == reference_length(n) || length == reference_length(n) + sizeof(int32_t));
+        }
+        if (!valid_) return;
+        anchors_.resize(n);
+        for (size_t i = 0; i < n; ++i) detail::read(d, anchors_[i]);
+        detail::read(d, stride_);
+        detail::read(d, height_);
+        detail::read(d, width_);
+        detail::read(d, image_height_);
+        detail::read(d, image_width_);
+        valid_ = read_dtype(d, length, reference_length(n));
+    }
+    bool valid() const { return valid_; }  // false: the blob had neither the reference's length nor that + 4
+    const char* getPluginType() const TRTX_NOEXCEPT override { return "RpnDecode"; }
+    int getNbOutputs() const TRTX_NOEXCEPT override { return 2; }
+    nvinfer1::Dims getOutputDimensions(int index, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override { return nvinfer1::Dims2(top_n_, index == 1 ? 4 : 1); }
+    size_t getWorkspaceSize(int maxBatchSize) const TRTX_NOEXCEPT override {
+        return (size_t)trtx_rpn_decode_typed(dtype_, maxBatchSize, nullptr, nullptr, nullptr, nullptr, (int)height_, (int)width_,
+                                             (int)image_height_, (int)image_width_, stride_, anchors_.data(), (int)anchors_.size() / 4,
+                                             top_n_, nullptr, 0, nullptr);
+    }
+    // scores and deltas fp32 or fp16, one type; the scores and boxes fp32
+    bool supportsFormatCombination(int pos, const nvinfer1::PluginTensorDesc* io, int nbInputs, int) const TRTX_NOEXCEPT override {
+        if (io[pos].format != nvinfer1::TensorFormat::kLINEAR) return false;
+        if (pos < nbInputs) return float_or_half(io[pos].type) && io[pos].type == io[0].type;
+        return io[pos].type == nvinfer1::DataType::kFLOAT;
+    }
+    nvinfer1::DataType getOutputDataType(int, const nvinfer1::DataType*, int) const TRTX_NOEXCEPT override { return nvinfer1::DataType::kFLOAT; }
+    void configurePlugin(const nvinfer1::PluginTensorDesc* in, int, const nvinfer1::PluginTensorDesc*, int) TRTX_NOEXCEPT override {
+        height_ = in[0].dims.d[1];  // RpnDecodePlugin.h:148-157: scores dims {A, H, W}
+        width_ = in[0].dims.d[2];
+        dtype_ = in[0].type == nvinfer1::DataType::kHALF ? TRTX_F16 : TRTX_F32;
+    }
+    int enqueue(int batchSize, const void* const* inputs, void* TRTX_CONST_ENQUEUE* outputs, void* workspace, cudaStream_t stream) TRTX_NOEXCEPT override {
+        const int64_t rc = trtx_rpn_decode_typed(dtype_, batchSize, inputs[0], inputs[1], static_cast<float*>(outputs[0]),
+                                                 static_cast<float*>(outputs[1]), (int)height_, (int)width_, (int)image_height_,
+                                                 (int)image_width_, stride_, anchors_.data(), (int)anchors_.size() / 4, top_n_, workspace,
+                                                 getWorkspaceSize(batchSize), stream);
+        return detail::rcnn_rc(rc);
+    }
+    size_t getSerializationSize() const TRTX_NOEXCEPT override { return reference_length(anchors_.size()) + sizeof(int32_t); }
+    void serialize(void* buffer) const TRTX_NOEXCEPT override {
+        char* d = static_cast<char*>(buffer);
+        detail::write(d, top_n_);
+        detail::write(d, anchors_.size());
+        for (float v : anchors_) detail::write(d, v);
+        detail::write(d, stride_);
+        detail::write(d, height_);
+        detail::write(d, width_);
+        detail::write(d, image_height_);
+        detail::write(d, image_width_);
+        detail::write(d, dtype_);
+    }
+    nvinfer1::IPluginV2IOExt* clone() const TRTX_NOEXCEPT override {
+        auto* c = new RpnDecodePluginIOExt(top_n_, anchors_, stride_, height_, width_, image_height_, image_width_);
+        c->dtype_ = dtype_;
+        return c;
+    }
+
+   private:
+    static size_t reference_length(size_t num_anchor_floats) {
+        return sizeof(int) + sizeof(size_t) + sizeof(float) * num_anchor_floats + sizeof(float) + 4 * sizeof(size_t);
+    }
+    int top_n_ = 0;
+    std::vector<float> anchors_;
+    float stride_ = 0.f;
+    size_t height_ = 0, width_ = 0, image_height_ = 0, image_width_ = 0;
+    bool valid_ = true;
+};
+
+class PredictorDecodePluginIOExt : public RcnnIOExtBase {
+   public:
+    PredictorDecodePluginIOExt(unsigned num_boxes, unsigned image_height, unsigned image_width, const std::vector<float>& w)
+        : num_boxes_(num_boxes), num_classes_(0), image_height_(image_height), image_width_(image_width), w_(w) {}
+    PredictorDecodePluginIOExt(unsigned num_boxes, unsigned num_classes, unsigned image_height, unsigned image_width, const std::vector<float>& w)
+        : num_boxes_(num_boxes), num_classes_(num_classes), image_height_(image_height), image_width_(image_width), w_(w) {}
+    PredictorDecodePluginIOExt(const void* data, size_t length) {  // PredictorDecodePlugin.h:40-54 (+ the element type)
+        const char* d = static_cast<const char*>(data);
+        size_t n = 0;
+        valid_ = length >= 4 * sizeof(unsigned) + sizeof(size_t);
+        if (valid_) {
+            detail::read(d, num_boxes_);
+            detail::read(d, num_classes_);
+            detail::read(d, image_height_);
+            detail::read(d, image_width_);
+            detail::read(d, n);
+            valid_ = n <= length / sizeof(float) &&
+                     (length == reference_length(n) || length == reference_length(n) + sizeof(int32_t));
+        }
+        if (!valid_) return;
+        w_.resize(n);
+        for (size_t i = 0; i < n; ++i) detail::read(d, w_[i]);
+        valid_ = read_dtype(d, length, reference_length(n));
+    }
+    bool valid() const { return valid_; }  // false: the blob had neither the reference's length nor that + 4
+    const char* getPluginType() const TRTX_NOEXCEPT override { return "PredictorDecode"; }
+    int getNbOutputs() const TRTX_NOEXCEPT override { return 3; }
+    nvinfer1::Dims getOutputDimensions(int index, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override { return nvinfer1::Dims2(num_boxes_, index == 1 ? 4 : 1); }
+    size_t getWorkspaceSize(int maxBatchSize) const TRTX_NOEXCEPT override {
+        return (size_t)trtx_predictor_decode_typed(dtype_, maxBatchSize, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, (int)num_boxes_,
+                                                   (int)num_classes_, (int)image_height_, (int)image_width_, w_.data(), nullptr, 0, nullptr);
+    }
+    // scores and deltas fp32 or fp16, one type; the proposals and the scores, boxes and classes fp32
+    bool supportsFormatCombination(int pos, const nvinfer1::PluginTensorDesc* io, int, int) const TRTX_NOEXCEPT override {
+        if (io[pos].format != nvinfer1::TensorFormat::kLINEAR) return false;
+        if (pos < 2) return float_or_half(io[pos].type) && io[pos].type == io[0].type;
+        return io[pos].type == nvinfer1::DataType::kFLOAT;
+    }
+    nvinfer1::DataType getOutputDataType(int, const nvinfer1::DataType*, int) const TRTX_NOEXCEPT override { return nvinfer1::DataType::kFLOAT; }
+    void configurePlugin(const nvinfer1::PluginTensorDesc* in, int, const nvinfer1::PluginTensorDesc*, int) TRTX_NOEXCEPT override {
+        num_classes_ = in[0].dims.d[1];  // scores dims {N, C, 1, 1}
+        dtype_ = in[0].type == nvinfer1::DataType::kHALF ? TRTX_F16 : TRTX_F32;
+    }
+    int enqueue(int batchSize, const void* const* inputs, void* TRTX_CONST_ENQUEUE* outputs, void* workspace, cudaStream_t stream) TRTX_NOEXCEPT override {
+        if (w_.size() < 4) return TRTX_ERR_INVALID;
+        const int64_t rc = trtx_predictor_decode_typed(dtype_, batchSize, inputs[0], inputs[1], static_cast<const float*>(inputs[2]),
+                                                       static_cast<float*>(outputs[0]), static_cast<float*>(outputs[1]),
+                                                       static_cast<float*>(outputs[2]), (int)num_boxes_, (int)num_classes_, (int)image_height_,
+                                                       (int)image_width_, w_.data(), workspace, getWorkspaceSize(batchSize), stream);
+        return detail::rcnn_rc(rc);
+    }
+    size_t getSerializationSize() const TRTX_NOEXCEPT override { return reference_length(w_.size()) + sizeof(int32_t); }
+    void serialize(void* buffer) const TRTX_NOEXCEPT override {
+        char* d = static_cast<char*>(buffer);
+        detail::write(d, num_boxes_);
+        detail::write(d, num_classes_);
+        detail::write(d, image_height_);
+        detail::write(d, image_width_);
+        detail::write(d, w_.size());
+        for (float v : w_) detail::write(d, v);
+        detail::write(d, dtype_);
+    }
+    nvinfer1::IPluginV2IOExt* clone() const TRTX_NOEXCEPT override {
+        auto* c = new PredictorDecodePluginIOExt(num_boxes_, num_classes_, image_height_, image_width_, w_);
+        c->dtype_ = dtype_;
+        return c;
+    }
+
+   private:
+    static size_t reference_length(size_t num_weights) { return 4 * sizeof(unsigned) + sizeof(size_t) + sizeof(float) * num_weights; }
+    unsigned num_boxes_ = 0, num_classes_ = 0, image_height_ = 0, image_width_ = 0;
+    std::vector<float> w_;
+    bool valid_ = true;
+};
+
+// deserializePlugin for the four classes above: a blob of neither accepted length is refused (nullptr)
 template <typename P>
 class RcnnIOExtCreator : public nvinfer1::IPluginCreator {
    public:
@@ -943,6 +1107,8 @@ class RcnnIOExtCreator : public nvinfer1::IPluginCreator {
 };
 struct RoiAlignPluginIOExtCreator : RcnnIOExtCreator<RoiAlignPluginIOExt> { RoiAlignPluginIOExtCreator() : RcnnIOExtCreator("RoiAlign") {} };
 struct MaskRcnnInferencePluginIOExtCreator : RcnnIOExtCreator<MaskRcnnInferencePluginIOExt> { MaskRcnnInferencePluginIOExtCreator() : RcnnIOExtCreator("MaskRcnnInference") {} };
+struct RpnDecodePluginIOExtCreator : RcnnIOExtCreator<RpnDecodePluginIOExt> { RpnDecodePluginIOExtCreator() : RcnnIOExtCreator("RpnDecode") {} };
+struct PredictorDecodePluginIOExtCreator : RcnnIOExtCreator<PredictorDecodePluginIOExt> { PredictorDecodePluginIOExtCreator() : RcnnIOExtCreator("PredictorDecode") {} };
 
 }  // namespace trtx
 
@@ -954,14 +1120,17 @@ REGISTER_TENSORRT_PLUGIN(YoloPluginCreatorImplicitBatch);
 REGISTER_TENSORRT_PLUGIN(YoloPluginCreator);
 #endif
 REGISTER_TENSORRT_PLUGIN(DecodePluginCreator);
-REGISTER_TENSORRT_PLUGIN(RpnDecodePluginCreator);
 REGISTER_TENSORRT_PLUGIN(RpnNmsPluginCreator);
-REGISTER_TENSORRT_PLUGIN(PredictorDecodePluginCreator);
 REGISTER_TENSORRT_PLUGIN(BatchedNmsPluginCreator);
-#ifdef TRTX_RCNN_HALF_IO_PLUGINS  // "RoiAlign" / "MaskRcnnInference" that also accept fp16 feature maps / masks
+#ifdef TRTX_RCNN_HALF_IO_PLUGINS  // the R-CNN plugins of an FP16 engine: "RpnDecode", "PredictorDecode", "RoiAlign" and
+                                  // "MaskRcnnInference" that also accept fp16 scores and deltas / feature maps / masks
+REGISTER_TENSORRT_PLUGIN(RpnDecodePluginIOExtCreator);
+REGISTER_TENSORRT_PLUGIN(PredictorDecodePluginIOExtCreator);
 REGISTER_TENSORRT_PLUGIN(RoiAlignPluginIOExtCreator);
 REGISTER_TENSORRT_PLUGIN(MaskRcnnInferencePluginIOExtCreator);
 #else
+REGISTER_TENSORRT_PLUGIN(RpnDecodePluginCreator);
+REGISTER_TENSORRT_PLUGIN(PredictorDecodePluginCreator);
 REGISTER_TENSORRT_PLUGIN(RoiAlignPluginCreator);
 REGISTER_TENSORRT_PLUGIN(MaskRcnnInferencePluginCreator);
 #endif

@@ -136,6 +136,9 @@ SYMBOLS = {
     "trtx_rpn_decode": (C.c_int64, [_i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, C.POINTER(C.c_float), _i, _i, _vp, _sz, _vp]),
     "trtx_rpn_nms": (C.c_int64, [_i, _vp, _vp, _vp, _i, _i, _f, _vp, _sz, _vp]),
     "trtx_predictor_decode": (C.c_int64, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, C.POINTER(C.c_float), _vp, _sz, _vp]),
+    "trtx_rpn_decode_typed": (C.c_int64, [_i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, C.POINTER(C.c_float), _i, _i, _vp, _sz, _vp]),
+    "trtx_predictor_decode_typed": (C.c_int64, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, C.POINTER(C.c_float), _vp, _sz,
+                                                _vp]),
     "trtx_batched_nms": (C.c_int64, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _vp, _sz, _vp]),
     "trtx_preprocess_batch_enqueue": (_i, [C.POINTER(ImageDesc), _i, _vp, _i, _i, _i, _vp]),
     "trtx_get_rect": (_i, [_i, _i, _i, _i, _i, C.POINTER(C.c_float), C.POINTER(C.c_int)]),

@@ -34,9 +34,13 @@ __device__ __forceinline__ float iou_plain(const float4 i, const float4 m) {
 
 constexpr int kMaxAnchors = 64;
 
+// T: the element type of the scores and deltas, float or __half.  A half is widened exactly (widen) wherever the fp32 kernel
+// reads a float, and the select ranks halves by half_key, which orders as float_key of the widened value: the half result
+// is the fp32 result on the widened tensors, bit for bit.  Outputs are fp32 in both modes.
+template <typename T>
 struct RpnDecodeArgs {
-    const float* scores;
-    const float* deltas;
+    const T* scores;
+    const T* deltas;
     float* out_scores;
     float* out_boxes;
     int height, width, image_height, image_width;
@@ -48,7 +52,8 @@ struct RpnDecodeArgs {
 // ---------------------------------------------------------------------------------------------
 // RpnDecode (rcnn/RpnDecode.cu:27-143)
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kSelThreads, 1) rpn_decode_kernel(const __grid_constant__ RpnDecodeArgs a) {
+template <typename T>
+__global__ void __launch_bounds__(kSelThreads, 1) rpn_decode_kernel(const __grid_constant__ RpnDecodeArgs<T> a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     unsigned long long* keys = reinterpret_cast<unsigned long long*>(smem_raw);
     __shared__ SelectScratch sc;
@@ -56,8 +61,8 @@ __global__ void __launch_bounds__(kSelThreads, 1) rpn_decode_kernel(const __grid
     const int b = blockIdx.x, tid = threadIdx.x;
     const int hw = a.height * a.width;
     const int n = a.num_anchors * hw;
-    const float* in_scores = a.scores + (size_t)b * n;
-    const float* in_boxes = a.deltas + (size_t)b * n * 4;
+    const T* in_scores = a.scores + (size_t)b * n;
+    const T* in_boxes = a.deltas + (size_t)b * n * 4;
     float* out_scores = a.out_scores + (size_t)b * a.top_n;
     float4* out_boxes = reinterpret_cast<float4*>(a.out_boxes) + (size_t)b * a.top_n;
 
@@ -65,14 +70,14 @@ __global__ void __launch_bounds__(kSelThreads, 1) rpn_decode_kernel(const __grid
     const bool sorted = n > a.top_n;  // RpnDecode.cu:79-86
     if (sorted) {
         uint32_t kc, ic;
-        block_select_topk([&](int i) { return float_key(in_scores[i]); }, n, a.top_n, sc, &kc, &ic);
+        block_select_topk<SelectKey<T>::kBits>([&](int i) { return SelectKey<T>::of(in_scores[i]); }, n, a.top_n, sc, &kc, &ic);
         if (tid == 0) s_cnt = 0;
         for (int i = tid; i < a.sort_cap; i += kSelThreads) keys[i] = ~0ull;
         __syncthreads();
         for (int i = tid; i < n; i += kSelThreads) {
-            const float s = in_scores[i];
-            const uint32_t k = float_key(s);
-            if (k > kc || (k == kc && (uint32_t)i <= ic)) keys[atomicAdd(&s_cnt, 1)] = desc_key(s, (uint32_t)i);
+            const T s = in_scores[i];
+            const uint32_t k = SelectKey<T>::of(s);
+            if (k > kc || (k == kc && (uint32_t)i <= ic)) keys[atomicAdd(&s_cnt, 1)] = desc_key(widen(s), (uint32_t)i);
         }
         __syncthreads();
         block_bitonic_sort_u64(keys, a.sort_cap);
@@ -83,10 +88,10 @@ __global__ void __launch_bounds__(kSelThreads, 1) rpn_decode_kernel(const __grid
         const int x = i % a.width;
         const int y = (i / a.width) % a.height;
         const int an = (i / a.height / a.width) % a.num_anchors;
-        float4 box = make_float4(in_boxes[((size_t)(an * 4 + 0) * a.height + y) * a.width + x],
-                                 in_boxes[((size_t)(an * 4 + 1) * a.height + y) * a.width + x],
-                                 in_boxes[((size_t)(an * 4 + 2) * a.height + y) * a.width + x],
-                                 in_boxes[((size_t)(an * 4 + 3) * a.height + y) * a.width + x]);
+        float4 box = make_float4(widen(in_boxes[((size_t)(an * 4 + 0) * a.height + y) * a.width + x]),
+                                 widen(in_boxes[((size_t)(an * 4 + 1) * a.height + y) * a.width + x]),
+                                 widen(in_boxes[((size_t)(an * 4 + 2) * a.height + y) * a.width + x]),
+                                 widen(in_boxes[((size_t)(an * 4 + 3) * a.height + y) * a.width + x]));
         if (a.num_anchors > 0) {  // has_anchors, :107-131
             const float fx = __fmul_rn((float)x, a.stride);
             const float fy = __fmul_rn((float)y, a.stride);
@@ -104,7 +109,7 @@ __global__ void __launch_bounds__(kSelThreads, 1) rpn_decode_kernel(const __grid
         }
         out_boxes[r] = box;
         // filter empty boxes, :129-132
-        out_scores[r] = (box.z - box.x <= 0.0f || box.w - box.y <= 0.0f) ? -FLT_MAX : in_scores[i];
+        out_scores[r] = (box.z - box.x <= 0.0f || box.w - box.y <= 0.0f) ? -FLT_MAX : widen(in_scores[i]);
     }
     for (int r = num_det + tid; r < a.top_n; r += kSelThreads) out_scores[r] = -FLT_MAX;  // :136-139
 }
@@ -112,9 +117,10 @@ __global__ void __launch_bounds__(kSelThreads, 1) rpn_decode_kernel(const __grid
 // ---------------------------------------------------------------------------------------------
 // PredictorDecode (rcnn/PredictorDecode.cu:24-110)
 // ---------------------------------------------------------------------------------------------
+template <typename T>
 struct PredictorArgs {
-    const float* scores;
-    const float* deltas;
+    const T* scores;
+    const T* deltas;
     const float* proposals;
     float* out_scores;
     float* out_boxes;
@@ -123,15 +129,31 @@ struct PredictorArgs {
     float w[4];
 };
 
-__global__ void __launch_bounds__(kSelThreads, 1) predictor_decode_kernel(const __grid_constant__ PredictorArgs a) {
+// a candidate's 4 deltas: one 16-byte load of floats, or one 8-byte load of 4 halves, widened
+template <typename T>
+struct Deltas4 {
+    using Vec = float4;
+};
+template <>
+struct Deltas4<__half> {
+    using Vec = uint2;
+};
+__device__ __forceinline__ float4 widen4(float4 v) { return v; }
+__device__ __forceinline__ float4 widen4(uint2 u) {
+    return make_float4(widen(__ushort_as_half((unsigned short)(u.x & 0xffffu))), widen(__ushort_as_half((unsigned short)(u.x >> 16))),
+                       widen(__ushort_as_half((unsigned short)(u.y & 0xffffu))), widen(__ushort_as_half((unsigned short)(u.y >> 16))));
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kSelThreads, 1) predictor_decode_kernel(const __grid_constant__ PredictorArgs<T> a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     unsigned long long* keys = reinterpret_cast<unsigned long long*>(smem_raw);
     __shared__ SelectScratch sc;
     __shared__ int s_cnt;
     const int b = blockIdx.x, tid = threadIdx.x;
     const int n = a.num_boxes * a.num_classes;
-    const float* in_scores = a.scores + (size_t)b * n;
-    const float4* in_boxes = reinterpret_cast<const float4*>(a.deltas) + (size_t)b * n;
+    const T* in_scores = a.scores + (size_t)b * n;
+    const typename Deltas4<T>::Vec* in_boxes = reinterpret_cast<const typename Deltas4<T>::Vec*>(a.deltas) + (size_t)b * n;
     const float4* in_prop = reinterpret_cast<const float4*>(a.proposals) + (size_t)b * a.num_boxes;
     const int k = a.num_boxes;  // the reference sorts all n scores and keeps the first num_boxes (:75-79)
 
@@ -140,14 +162,14 @@ __global__ void __launch_bounds__(kSelThreads, 1) predictor_decode_kernel(const 
     __syncthreads();
     if (n > k) {
         uint32_t kc, ic;
-        block_select_topk([&](int i) { return float_key(in_scores[i]); }, n, k, sc, &kc, &ic);
+        block_select_topk<SelectKey<T>::kBits>([&](int i) { return SelectKey<T>::of(in_scores[i]); }, n, k, sc, &kc, &ic);
         for (int i = tid; i < n; i += kSelThreads) {
-            const float s = in_scores[i];
-            const uint32_t kk = float_key(s);
-            if (kk > kc || (kk == kc && (uint32_t)i <= ic)) keys[atomicAdd(&s_cnt, 1)] = desc_key(s, (uint32_t)i);
+            const T s = in_scores[i];
+            const uint32_t kk = SelectKey<T>::of(s);
+            if (kk > kc || (kk == kc && (uint32_t)i <= ic)) keys[atomicAdd(&s_cnt, 1)] = desc_key(widen(s), (uint32_t)i);
         }
     } else {
-        for (int i = tid; i < n; i += kSelThreads) keys[i] = desc_key(in_scores[i], (uint32_t)i);
+        for (int i = tid; i < n; i += kSelThreads) keys[i] = desc_key(widen(in_scores[i]), (uint32_t)i);
     }
     __syncthreads();
     block_bitonic_sort_u64(keys, a.sort_cap);
@@ -155,7 +177,7 @@ __global__ void __launch_bounds__(kSelThreads, 1) predictor_decode_kernel(const 
         const int i = (int)(keys[r] & 0xffffffffull);
         const int cls = i % a.num_classes;
         const int nb = i / a.num_classes;
-        const float4 d = in_boxes[i];
+        const float4 d = widen4(in_boxes[i]);
         const float4 p = in_prop[nb];
         const float w = __fsub_rn(p.z, p.x), h = __fsub_rn(p.w, p.y);
         const float pcx = __fadd_rn(__fadd_rn(__fmul_rn(__fdiv_rn(d.x, a.w[0]), w), p.x), __fmul_rn(0.5f, w));
@@ -166,7 +188,7 @@ __global__ void __launch_bounds__(kSelThreads, 1) predictor_decode_kernel(const 
                                        fminf(__fadd_rn(pcx, __fmul_rn(0.5f, pw)), (float)a.image_width),
                                        fminf(__fadd_rn(pcy, __fmul_rn(0.5f, ph)), (float)a.image_width));  // sic: :99 uses image_width
         reinterpret_cast<float4*>(a.out_boxes)[(size_t)b * a.num_boxes + r] = box;
-        a.out_scores[(size_t)b * a.num_boxes + r] = (box.z - box.x <= 0.0f || box.w - box.y <= 0.0f) ? 0.0f : in_scores[i];
+        a.out_scores[(size_t)b * a.num_boxes + r] = (box.z - box.x <= 0.0f || box.w - box.y <= 0.0f) ? 0.0f : widen(in_scores[i]);
         a.out_classes[(size_t)b * a.num_boxes + r] = (float)cls;
     }
 }
@@ -427,30 +449,13 @@ static int pow2_at_least(int v) {
 }
 constexpr int kMaxSortCap = 8192;
 
-}  // namespace trtx
-
-using namespace trtx;
-
-extern "C" {
-
-// Workspace: none of these kernels needs global scratch (everything lives in shared memory); the
-// "null workspace -> size" idiom is kept and reports a nominal 256 bytes so that TensorRT's
-// allocation path is exercised exactly as with the reference plugins.
-static const int64_t kNominalWorkspace = 256;
-
-TRTX_API int64_t trtx_rpn_decode(int batch, const float* scores_dev, const float* deltas_dev, float* out_scores_dev,
-                                 float* out_boxes_dev, int height, int width, int image_height, int image_width,
-                                 float stride, const float* anchors_host, int num_anchors, int top_n,
-                                 void* workspace_dev, size_t workspace_bytes, trtx_stream_t stream) {
-    if (!workspace_dev || !workspace_bytes) return kNominalWorkspace;
-    if (batch <= 0 || !scores_dev || !deltas_dev || !out_scores_dev || !out_boxes_dev) return -TRTX_ERR_INVALID;
-    if (height <= 0 || width <= 0 || top_n <= 0 || num_anchors < 0 || (num_anchors > 0 && !anchors_host))
-        return -TRTX_ERR_INVALID;
-    if (num_anchors > kMaxAnchors || top_n > kMaxSortCap) return -TRTX_ERR_UNSUPPORTED;
-    if (num_anchors == 0) return -TRTX_ERR_UNSUPPORTED;  // scores_size would be 0 in the reference too
-    RpnDecodeArgs a{};
-    a.scores = scores_dev;
-    a.deltas = deltas_dev;
+template <typename T>
+static int rpn_decode_launch(int batch, const void* scores_dev, const void* deltas_dev, float* out_scores_dev, float* out_boxes_dev,
+                             int height, int width, int image_height, int image_width, float stride, const float* anchors_host,
+                             int num_anchors, int top_n, cudaStream_t stream) {
+    RpnDecodeArgs<T> a{};
+    a.scores = static_cast<const T*>(scores_dev);
+    a.deltas = static_cast<const T*>(deltas_dev);
     a.out_scores = out_scores_dev;
     a.out_boxes = out_boxes_dev;
     a.height = height;
@@ -463,9 +468,75 @@ TRTX_API int64_t trtx_rpn_decode(int batch, const float* scores_dev, const float
     a.sort_cap = pow2_at_least(top_n);
     for (int i = 0; i < num_anchors * 4; ++i) a.anchors[i] = anchors_host[i];
     const size_t smem = sizeof(unsigned long long) * a.sort_cap;
-    cudaFuncSetAttribute(rpn_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(unsigned long long) * kMaxSortCap));
-    rpn_decode_kernel<<<batch, kSelThreads, smem, static_cast<cudaStream_t>(stream)>>>(a);
-    return -(int64_t)check_launch();
+    cudaFuncSetAttribute(rpn_decode_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(unsigned long long) * kMaxSortCap));
+    rpn_decode_kernel<T><<<batch, kSelThreads, smem, stream>>>(a);
+    return check_launch();
+}
+
+template <typename T>
+static int predictor_decode_launch(int batch, const void* scores_dev, const void* deltas_dev, const float* proposals_dev,
+                                   float* out_scores_dev, float* out_boxes_dev, float* out_classes_dev, int num_boxes, int num_classes,
+                                   int image_height, int image_width, const float* bbox_reg_weights_host, cudaStream_t stream) {
+    PredictorArgs<T> a{};
+    a.scores = static_cast<const T*>(scores_dev);
+    a.deltas = static_cast<const T*>(deltas_dev);
+    a.proposals = proposals_dev;
+    a.out_scores = out_scores_dev;
+    a.out_boxes = out_boxes_dev;
+    a.out_classes = out_classes_dev;
+    a.num_boxes = num_boxes;
+    a.num_classes = num_classes;
+    a.image_height = image_height;
+    a.image_width = image_width;
+    a.sort_cap = pow2_at_least(num_boxes);
+    for (int i = 0; i < 4; ++i) a.w[i] = bbox_reg_weights_host[i];
+    const size_t smem = sizeof(unsigned long long) * a.sort_cap;
+    cudaFuncSetAttribute(predictor_decode_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)(sizeof(unsigned long long) * kMaxSortCap));
+    predictor_decode_kernel<T><<<batch, kSelThreads, smem, stream>>>(a);
+    return check_launch();
+}
+
+static bool aligned_to(const void* p, size_t n) { return reinterpret_cast<uintptr_t>(p) % n == 0; }
+
+}  // namespace trtx
+
+using namespace trtx;
+
+extern "C" {
+
+// Workspace: none of these kernels needs global scratch (everything lives in shared memory); the
+// "null workspace -> size" idiom is kept and reports a nominal 256 bytes so that TensorRT's
+// allocation path is exercised exactly as with the reference plugins.
+static const int64_t kNominalWorkspace = 256;
+
+TRTX_API int64_t trtx_rpn_decode_typed(int in_dtype, int batch, const void* scores_dev, const void* deltas_dev,
+                                       float* out_scores_dev, float* out_boxes_dev, int height, int width, int image_height,
+                                       int image_width, float stride, const float* anchors_host, int num_anchors, int top_n,
+                                       void* workspace_dev, size_t workspace_bytes, trtx_stream_t stream) {
+    if (in_dtype != TRTX_F32 && in_dtype != TRTX_F16) return -TRTX_ERR_INVALID;
+    if (!workspace_dev || !workspace_bytes) return kNominalWorkspace;
+    if (batch <= 0 || !scores_dev || !deltas_dev || !out_scores_dev || !out_boxes_dev) return -TRTX_ERR_INVALID;
+    if (height <= 0 || width <= 0 || top_n <= 0 || num_anchors < 0 || (num_anchors > 0 && !anchors_host))
+        return -TRTX_ERR_INVALID;
+    if (in_dtype == TRTX_F16 && (!aligned_to(scores_dev, sizeof(__half)) || !aligned_to(deltas_dev, sizeof(__half))))
+        return -TRTX_ERR_INVALID;
+    if (num_anchors > kMaxAnchors || top_n > kMaxSortCap) return -TRTX_ERR_UNSUPPORTED;
+    if (num_anchors == 0) return -TRTX_ERR_UNSUPPORTED;  // scores_size would be 0 in the reference too
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (in_dtype == TRTX_F16)
+        return -(int64_t)rpn_decode_launch<__half>(batch, scores_dev, deltas_dev, out_scores_dev, out_boxes_dev, height, width,
+                                                   image_height, image_width, stride, anchors_host, num_anchors, top_n, st);
+    return -(int64_t)rpn_decode_launch<float>(batch, scores_dev, deltas_dev, out_scores_dev, out_boxes_dev, height, width,
+                                              image_height, image_width, stride, anchors_host, num_anchors, top_n, st);
+}
+
+TRTX_API int64_t trtx_rpn_decode(int batch, const float* scores_dev, const float* deltas_dev, float* out_scores_dev,
+                                 float* out_boxes_dev, int height, int width, int image_height, int image_width,
+                                 float stride, const float* anchors_host, int num_anchors, int top_n,
+                                 void* workspace_dev, size_t workspace_bytes, trtx_stream_t stream) {
+    return trtx_rpn_decode_typed(TRTX_F32, batch, scores_dev, deltas_dev, out_scores_dev, out_boxes_dev, height, width, image_height,
+                                 image_width, stride, anchors_host, num_anchors, top_n, workspace_dev, workspace_bytes, stream);
 }
 
 TRTX_API int64_t trtx_rpn_nms(int batch, const float* scores_dev, const float* boxes_dev, float* out_boxes_dev,
@@ -493,33 +564,38 @@ TRTX_API int64_t trtx_rpn_nms(int batch, const float* scores_dev, const float* b
     return -(int64_t)check_launch();
 }
 
+TRTX_API int64_t trtx_predictor_decode_typed(int in_dtype, int batch, const void* scores_dev, const void* deltas_dev,
+                                             const float* proposals_dev, float* out_scores_dev, float* out_boxes_dev,
+                                             float* out_classes_dev, int num_boxes, int num_classes, int image_height,
+                                             int image_width, const float* bbox_reg_weights_host, void* workspace_dev,
+                                             size_t workspace_bytes, trtx_stream_t stream) {
+    if (in_dtype != TRTX_F32 && in_dtype != TRTX_F16) return -TRTX_ERR_INVALID;
+    if (!workspace_dev || !workspace_bytes) return kNominalWorkspace;
+    if (batch <= 0 || !scores_dev || !deltas_dev || !proposals_dev || !out_scores_dev || !out_boxes_dev ||
+        !out_classes_dev || num_boxes <= 0 || num_classes <= 0 || !bbox_reg_weights_host)
+        return -TRTX_ERR_INVALID;
+    // half scores are read one by one, a candidate's 4 half deltas as one 8-byte load
+    if (in_dtype == TRTX_F16 && (!aligned_to(scores_dev, sizeof(__half)) || !aligned_to(deltas_dev, 4 * sizeof(__half))))
+        return -TRTX_ERR_INVALID;
+    if (num_boxes > kMaxSortCap) return -TRTX_ERR_UNSUPPORTED;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (in_dtype == TRTX_F16)
+        return -(int64_t)predictor_decode_launch<__half>(batch, scores_dev, deltas_dev, proposals_dev, out_scores_dev, out_boxes_dev,
+                                                         out_classes_dev, num_boxes, num_classes, image_height, image_width,
+                                                         bbox_reg_weights_host, st);
+    return -(int64_t)predictor_decode_launch<float>(batch, scores_dev, deltas_dev, proposals_dev, out_scores_dev, out_boxes_dev,
+                                                    out_classes_dev, num_boxes, num_classes, image_height, image_width,
+                                                    bbox_reg_weights_host, st);
+}
+
 TRTX_API int64_t trtx_predictor_decode(int batch, const float* scores_dev, const float* deltas_dev,
                                        const float* proposals_dev, float* out_scores_dev, float* out_boxes_dev,
                                        float* out_classes_dev, int num_boxes, int num_classes, int image_height,
                                        int image_width, const float* bbox_reg_weights_host, void* workspace_dev,
                                        size_t workspace_bytes, trtx_stream_t stream) {
-    if (!workspace_dev || !workspace_bytes) return kNominalWorkspace;
-    if (batch <= 0 || !scores_dev || !deltas_dev || !proposals_dev || !out_scores_dev || !out_boxes_dev ||
-        !out_classes_dev || num_boxes <= 0 || num_classes <= 0 || !bbox_reg_weights_host)
-        return -TRTX_ERR_INVALID;
-    if (num_boxes > kMaxSortCap) return -TRTX_ERR_UNSUPPORTED;
-    PredictorArgs a{};
-    a.scores = scores_dev;
-    a.deltas = deltas_dev;
-    a.proposals = proposals_dev;
-    a.out_scores = out_scores_dev;
-    a.out_boxes = out_boxes_dev;
-    a.out_classes = out_classes_dev;
-    a.num_boxes = num_boxes;
-    a.num_classes = num_classes;
-    a.image_height = image_height;
-    a.image_width = image_width;
-    a.sort_cap = pow2_at_least(num_boxes);
-    for (int i = 0; i < 4; ++i) a.w[i] = bbox_reg_weights_host[i];
-    const size_t smem = sizeof(unsigned long long) * a.sort_cap;
-    cudaFuncSetAttribute(predictor_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(unsigned long long) * kMaxSortCap));
-    predictor_decode_kernel<<<batch, kSelThreads, smem, static_cast<cudaStream_t>(stream)>>>(a);
-    return -(int64_t)check_launch();
+    return trtx_predictor_decode_typed(TRTX_F32, batch, scores_dev, deltas_dev, proposals_dev, out_scores_dev, out_boxes_dev,
+                                       out_classes_dev, num_boxes, num_classes, image_height, image_width, bbox_reg_weights_host,
+                                       workspace_dev, workspace_bytes, stream);
 }
 
 TRTX_API int64_t trtx_batched_nms(int nms_method, int batch, const float* scores_dev, const float* boxes_dev,

@@ -4,8 +4,8 @@
 // sort of fp32 keys with an iota payload: ties keep ascending index; -0.0 and +0.0 are equal keys) and then uses the
 // first k entries (rcnn/RpnDecode.cu:82, PredictorDecode.cu:75, RpnNms.cu:100, BatchedNms.cu:134).  The same ordered
 // prefix is obtained here by (1) an exact radix SELECT of the k largest (key, lower index first) --
-// 4 histogram passes over the keys plus 4 over the indices of the elements tied at the cut -- and
-// (2) a bitonic SORT of only those k elements in shared memory, keyed by (~key << 32 | index).
+// 4 histogram passes over the keys (2 over the 16-bit keys of half scores) plus 4 over the indices of the elements tied
+// at the cut -- and (2) a bitonic SORT of only those k elements in shared memory, keyed by (~key << 32 | index).
 #pragma once
 #include "common.cuh"
 
@@ -38,14 +38,16 @@ __device__ __forceinline__ void pick_bucket_dev(const int* hist, bool descending
 
 // Exact cut for "the k largest of key(i), i in [0,n), ties -> smaller i":
 // element i is selected  <=>  key(i) > key_cut || (key(i) == key_cut && i <= id_cut).   Requires n > k > 0.
-template <typename KeyFn>
+// kKeyBits: the width of the keys (32 or 16), one 8-bit histogram pass per byte.
+template <int kKeyBits = 32, typename KeyFn>
 __device__ void block_select_topk(KeyFn key, int n, int k, SelectScratch& sc, uint32_t* key_cut_out, uint32_t* id_cut_out) {
+    static_assert(kKeyBits == 32 || kKeyBits == 16, "keys of 4 or 2 bytes");
     const int tid = threadIdx.x;
     uint32_t prefix = 0, mask = 0;
     __syncthreads();
     if (tid == 0) sc.need = k;
-    for (int pass = 0; pass < 4; ++pass) {
-        const int shift = 24 - 8 * pass;
+    for (int pass = 0; pass < kKeyBits / 8; ++pass) {
+        const int shift = kKeyBits - 8 - 8 * pass;
         if (tid < 256) sc.hist[tid] = 0;
         __syncthreads();
         for (int i = tid; i < n; i += kSelThreads) {
@@ -112,5 +114,37 @@ __device__ __forceinline__ void block_bitonic_sort_u64(unsigned long long* keys,
 __device__ __forceinline__ unsigned long long desc_key(float score, uint32_t idx) {
     return ((unsigned long long)(~float_key(score)) << 32) | idx;
 }
+
+// 16-bit key of a half that orders and ties exactly as float_key(__half2float(h)): widening is exact and monotonic, so every
+// pattern that is not a NaN takes float_key's transform on its own 16 bits (-0 -> +0, then the sign flip).  A NaN takes the
+// key of the half whose sign, exponent and top 10 mantissa bits are those of the float the device widens it to, so NaNs
+// rank among themselves and against +-inf as their widened floats do, whether the conversion keeps the payload or returns
+// one canonical NaN (a widened NaN's low 13 mantissa bits are then all zero or all one, the same for every NaN).
+__device__ __forceinline__ uint32_t half_key(__half h) {
+    uint32_t b = __half_as_ushort(h);
+    if ((b & 0x7fffu) > 0x7c00u) {
+        const uint32_t w = __float_as_uint(__half2float(h));
+        b = ((w >> 16) & 0x8000u) | 0x7c00u | ((w >> 13) & 0x3ffu);
+    }
+    b = b == 0x8000u ? 0u : b;
+    return (b & 0x8000u) ? (~b & 0xffffu) : (b | 0x8000u);
+}
+
+// The select key of an input element type: the 32-bit float_key, or the 16-bit half_key (two histogram passes, not four).
+template <typename T>
+struct SelectKey;
+template <>
+struct SelectKey<float> {
+    static constexpr int kBits = 32;
+    static __device__ __forceinline__ uint32_t of(float s) { return float_key(s); }
+};
+template <>
+struct SelectKey<__half> {
+    static constexpr int kBits = 16;
+    static __device__ __forceinline__ uint32_t of(__half s) { return half_key(s); }
+};
+
+__device__ __forceinline__ float widen(float v) { return v; }
+__device__ __forceinline__ float widen(__half v) { return __half2float(v); }
 
 }  // namespace trtx

@@ -204,7 +204,9 @@ class RetinaPipeline:
 class RcnnHeadChain:
     """The four Faster R-CNN plugins chained on one stream exactly as rcnn.cpp wires them (rcnn/rcnn.cpp:134-195):
     RpnDecode -> RpnNms -> [RoIAlign + box head: TensorRT, not on this path; its outputs are inputs here] ->
-    PredictorDecode -> BatchedNms.  All images of the batch per launch."""
+    PredictorDecode -> BatchedNms.  All images of the batch per launch.  run_device takes the heads of an FP32 or an FP16
+    engine: rpn_scores / rpn_deltas, and cls_scores / box_deltas, each pair torch.float32 or torch.float16; what RpnNms and
+    BatchedNms read stays fp32, and a half pair gives the result of the widened pair, bit for bit."""
 
     def __init__(self, batch: int, anchors, device="cuda", H: int = 50, W: int = 67, image_h: int = 800, image_w: int = 1067,
                  pre: int = 6000, post: int = 1000, classes: int = 80, dets: int = 100, nms_method: int = 1):

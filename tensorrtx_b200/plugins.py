@@ -871,10 +871,14 @@ class RpnDecodePlugin:
                                                len(self._anchors) // 4, self._top_n, None, 0, None), "trtx_rpn_decode(size)")
 
     def enqueue(self, batchSize, inputs, outputs, workspace, stream=None) -> int:
-        rc = self._lib.trtx_rpn_decode(batchSize, _ptr(inputs[0]), _ptr(inputs[1]), _ptr(outputs[0]), _ptr(outputs[1]),
-                                       self._height, self._width, self._image_height, self._image_width, self._stride,
-                                       self._anc, len(self._anchors) // 4, self._top_n, _ptr(workspace), _nbytes(workspace),
-                                       _stream(stream))
+        """Scores and deltas share one dtype, torch.float32 or torch.float16 (the result is then the fp32 result of the
+        widened tensors, bit for bit); the output scores and boxes are torch.float32 in both modes."""
+        dt = _elem_dtype(inputs[:2], "RpnDecode scores and deltas")
+        _elem_dtype(outputs[:2], "RpnDecode outputs", only=L.F32)
+        rc = self._lib.trtx_rpn_decode_typed(dt, batchSize, _ptr(inputs[0]), _ptr(inputs[1]), _ptr(outputs[0]), _ptr(outputs[1]),
+                                             self._height, self._width, self._image_height, self._image_width, self._stride,
+                                             self._anc, len(self._anchors) // 4, self._top_n, _ptr(workspace), _nbytes(workspace),
+                                             _stream(stream))
         return _status(rc)
 
 
@@ -922,10 +926,15 @@ class PredictorDecodePlugin:
                                                      None, 0, None), "trtx_predictor_decode(size)")
 
     def enqueue(self, batchSize, inputs, outputs, workspace, stream=None) -> int:
-        rc = self._lib.trtx_predictor_decode(batchSize, _ptr(inputs[0]), _ptr(inputs[1]), _ptr(inputs[2]),
-                                             _ptr(outputs[0]), _ptr(outputs[1]), _ptr(outputs[2]), self._num_boxes,
-                                             self._num_classes, self._image_height, self._image_width, self._w,
-                                             _ptr(workspace), _nbytes(workspace), _stream(stream))
+        """Scores and deltas share one dtype, torch.float32 or torch.float16 (the result is then the fp32 result of the
+        widened tensors, bit for bit); the proposals and the output scores, boxes and classes are torch.float32 in both modes."""
+        dt = _elem_dtype(inputs[:2], "PredictorDecode scores and deltas")
+        _elem_dtype(inputs[2:3], "PredictorDecode proposals", only=L.F32)
+        _elem_dtype(outputs[:3], "PredictorDecode outputs", only=L.F32)
+        rc = self._lib.trtx_predictor_decode_typed(dt, batchSize, _ptr(inputs[0]), _ptr(inputs[1]), _ptr(inputs[2]),
+                                                   _ptr(outputs[0]), _ptr(outputs[1]), _ptr(outputs[2]), self._num_boxes,
+                                                   self._num_classes, self._image_height, self._image_width, self._w,
+                                                   _ptr(workspace), _nbytes(workspace), _stream(stream))
         return _status(rc)
 
 
