@@ -5,7 +5,8 @@ compares in full.  Elsewhere it compares against tests/golden/<name>.npz, which 
 a SHA-256 of the canonical bytes for a bit-exact comparison (the same verdict as comparing the arrays), the values -- or a
 fixed, seeded sample of them -- for a comparison within a tolerance.  The inputs are not stored: the tests rebuild them from
 seeds.  With TRTX_GOLDEN_RECORD=<dir> in the environment, a pytest run against oracle/_ref writes <dir>/<name>.npz
-(ref_gpu.npz on a GPU: `pytest -m gpu tests/test_vs_reference_gpu.py tests/test_variants_gpu.py`)."""
+(ref_gpu.npz on a GPU: `pytest -m gpu tests/test_vs_reference_gpu.py tests/test_variants_gpu.py
+tests/test_yolo_scan_paths_gpu.py`)."""
 from __future__ import annotations
 
 import atexit

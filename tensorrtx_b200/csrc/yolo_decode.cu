@@ -311,7 +311,7 @@ template <typename T, int VEC, int U>
 __global__ void __launch_bounds__(128) yolo_v5_scan_kernel(const __grid_constant__ YoloArgs a) {
     constexpr int TILE = 32 * VEC;
     constexpr int SLICES = 4;
-    __shared__ float s_obj[3][TILE];            // objectness prob (0 if not passing)
+    __shared__ float s_obj[3][TILE];            // objectness prob, NaN included; -1 if not passing (test: !(v < 0))
     __shared__ float s_m[SLICES - 1][TILE];     // class slices 1..3: max logit, max logit before its class, its class
     __shared__ float s_m2[SLICES - 1][TILE];
     __shared__ int s_c[SLICES - 1][TILE];
@@ -357,7 +357,8 @@ __global__ void __launch_bounds__(128) yolo_v5_scan_kernel(const __grid_constant
         for (int j = 0; j < VEC; ++j) {
             float pr = 0.0f;
             bool pass = false;
-            if (active && (a0 + j < L.g) && x[j] > a.x_lo) {
+            // a NaN logit is evaluated too: its box_prob is NaN, which `box_prob < kIgnoreThresh` does not skip
+            if (active && (a0 + j < L.g) && !(x[j] <= a.x_lo)) {
                 pr = logist(x[j]);
                 pass = !(pr < a.gate);  // yololayer.cu:177 `if (box_prob < kIgnoreThresh) continue;`
             }
@@ -384,7 +385,7 @@ __global__ void __launch_bounds__(128) yolo_v5_scan_kernel(const __grid_constant
 #pragma unroll
         for (int j = 0; j < VEC; ++j) {
             // anchors that failed the objectness gate never update; passing ones see every running max
-            s.bx[j] = (s_obj[k][lane * VEC + j] >= 0.0f) ? -INFINITY : INFINITY;
+            s.bx[j] = !(s_obj[k][lane * VEC + j] < 0.0f) ? -INFINITY : INFINITY;
             s.b2[j] = s.bx[j];
             s.bc[j] = 0;
         }
@@ -410,7 +411,7 @@ __global__ void __launch_bounds__(128) yolo_v5_scan_kernel(const __grid_constant
             for (int j = 0; j < VEC; ++j) {
                 // one sigmoid per passing anchor; the v5 class probability has no gate of its own (yololayer.cu:178-186)
                 float P = 0.0f;
-                if (s_obj[k][lane * VEC + j] >= 0.0f && s.bx[j] > -INFINITY) {
+                if (!(s_obj[k][lane * VEC + j] < 0.0f) && s.bx[j] > -INFINITY) {
                     const T* cls_row0 = base + ((size_t)k * ilen + 5) * g + a0 + j;
                     P = finish_best(s.bx[j], s.b2[j], s.bc[j], 0.0f, [&](int i) { return Elem<T>::ld1(cls_row0 + (size_t)i * g); });
                 }
@@ -428,7 +429,7 @@ __global__ void __launch_bounds__(128) yolo_v5_scan_kernel(const __grid_constant
     for (int j = 0; j < VEC; ++j)
 #pragma unroll
         for (int k = 0; k < 3; ++k)  // v3: `max_cls_prob < IGNORE_THRESH || box_prob < IGNORE_THRESH` -> skip
-            if (s_obj[k][lane * VEC + j] >= 0.0f && !(v3 && s_fp[k][lane * VEC + j] < a.gate)) flags |= 1u << (j * 3 + k);
+            if (!(s_obj[k][lane * VEC + j] < 0.0f) && !(v3 && s_fp[k][lane * VEC + j] < a.gate)) flags |= 1u << (j * 3 + k);
     int total;
     int off = warp_excl_scan(__popc(flags), lane, &total);
     if (lane == 0) a.tile_count[(size_t)b * a.tiles_per_image + t] = total;
