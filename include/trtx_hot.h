@@ -50,7 +50,7 @@ TRTX_API int trtx_last_cuda_error(void);
 /* sizeof() of the parameter structs as THIS library was compiled, so that an FFI binding (ctypes, cgo, ...) can check its
  * mirror of the layout: which = 0 trtx_yolo_params, 1 trtx_nms_params, 2 trtx_retina_params, 3 trtx_image_desc,
  * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_frame, 7 trtx_pose_obb_params, 8 trtx_frame,
- * 9 trtx_face_post_params; anything else 0. */
+ * 9 trtx_face_post_params, 10 trtx_yolop_post_params; anything else 0. */
 TRTX_API size_t trtx_abi_sizeof(int which);
 
 /* =====================================================================================
@@ -700,6 +700,61 @@ TRTX_API int trtx_cls_preprocess_enqueue(int variant, const trtx_image_desc* ima
  * to 96 KB of shared memory, no workspace; can be captured in a CUDA graph. */
 TRTX_API int trtx_cls_postprocess_enqueue(int softmax, int batch, int num_classes, const float* logits_dev, int k,
                                           int32_t* index_dev, float* value_dev, float* probs_dev, trtx_stream_t stream);
+
+/* =====================================================================================
+ * 9. YOLOP pre- and post-process
+ *    replaces the HOST preprocess_img of yolop/utils.h:11-36 with the driver's plane loop and H2D copy
+ *    (yolop/yolop.cpp:110-127), and the HOST stages after inference: nms() + get_rect (yolop/common.hpp:13-83) on a D2H
+ *    copy of the plugin rows, and the per-pixel loop over the drivable-area and lane maps (yolop/yolop.cpp:148-169).
+ *    The detection head itself is YoloLayer_TRT with 6-float rows (TRTX_YOLO_V5, det_floats 6); its NMS is
+ *    trtx_nms_enqueue with TRTX_BOX_CXCYWH, greedy.
+ * ===================================================================================== */
+/* preprocess_img + the plane loop for a whole batch, one launch per <= 64 images: images_host = `batch` u8 HWC BGR descriptors
+ * in HOST memory (trtx_image_desc, any pitch and base alignment, mixed sizes allowed); dst_dev = [batch, 3, net_h, net_w] fp32
+ * planes in the driver's B, G, R order (Yolo::INPUT_W x INPUT_H = 640 x 384), the engine input.  The resize is OpenCV 4.x's
+ * 8-bit INTER_LINEAR into the rectangle of trtx_calib_letterbox_rect on a 114-grey canvas, bit for bit; byte u of plane c
+ * (mean = 0.485, 0.456, 0.406 and std = 0.229, 0.224, 0.225 for planes 0, 1, 2) becomes
+ *     s = (float)u * (1.f / 255.f) - (float)mean_c  (float),   (float)((double)s / std_c),
+ * cv2 4.13's convertTo / subtract / divide chain.  Every descriptor is checked before the first launch (a rejected call writes
+ * nothing): TRTX_ERR_INVALID for a null pointer, batch / net sizes <= 0, pitch < 3 * width or a dst_dev that is not 4-byte
+ * aligned; TRTX_ERR_UNSUPPORTED for a rectangle that is empty (cv::resize throws there) or wider than 4 757 pixels.  No
+ * workspace; can be captured in a CUDA graph. */
+TRTX_API int trtx_yolop_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
+                                           trtx_stream_t stream);
+
+/* YOLOP's get_rect (yolop/common.hpp:13-37): box cx, cy, w, h in network pixels (net_w x net_h = Yolo::INPUT_W x INPUT_H,
+ * 640 x 384) -> rect = {x, y, w, h} in the img_w x img_h frame; each statement truncates to int, nothing is clamped.
+ * Defined where the reference is not, as the compiled x86-64 reference behaves: a value that is NaN, infinite or outside
+ * [-2^31, 2^31) converts to INT_MIN, and w = r - l, h = b - t wrap modulo 2^32.  Host function; the device form is
+ * trtx_yolop_postprocess_enqueue. */
+TRTX_API int trtx_yolop_get_rect(int net_w, int net_h, int img_w, int img_h, const float bbox[4], int rect[4]);
+
+typedef struct trtx_yolop_post_params {
+    int32_t net_w, net_h; /* Yolo::INPUT_W x INPUT_H (640 x 384): get_rect's letterbox */
+    int32_t map_w, map_h; /* Yolo::IMG_W x IMG_H (640 x 360): the drivable-area and lane maps */
+    int32_t row_floats;   /* floats per input row, >= 7: the compact NMS rows (cx, cy, w, h, conf, class, keep) */
+} trtx_yolop_post_params;
+
+/* dets_dev [B, 1 + max_rows*row_floats]: count, then (cx, cy, w, h, conf, class, keep, ...) rows -- the compact output of
+ *   trtx_nms_enqueue (TRTX_BOX_CXCYWH, greedy, det_floats 6) over the plugin rows.  Of the first min(count, max_rows) rows
+ *   those with (int)keep == 1 are used: every row of a greedy output.
+ * frames_host: `batch` trtx_frame in HOST memory (copied into launch parameters; sizes may differ in a call).
+ * rows_dev [B, 1 + max_rows*6]: the used count, then per used row in input order (x, y, w, h, conf, class) with x, y, w, h =
+ *   trtx_yolop_get_rect as floats (exact for |v| <= 2^24); rows past the count are zeroed.
+ * Labels, where frames_host[b].masks_dev is an [img_h, pitch] u8 canvas: pixel (x, y) of frame b gets 2 where
+ *   lane_dev[b][sy][sx] != 0, else 1 where seg_dev[b][sy][sx] != 0, else 0 (yolop.cpp:148-169: `if (lane_idx) ... else if
+ *   (seg_idx)`), with sx = min(floor(x * (1 / ((double)img_w / map_w))), map_w - 1) and sy likewise: cv::resize's
+ *   INTER_NEAREST of OpenCV 4.x.  Bytes of a row past img_w are not written.  seg_dev and lane_dev are the engine's
+ *   [B, map_h, map_w] int32 index maps.  Frame b reads maps b; the reference reads the first image's maps for every frame
+ *   (yolop.cpp:90-92), which is the same at its BATCH_SIZE 1.  Colouring the frame stays with the caller.
+ * Canvases for every frame or for none (then seg_dev and lane_dev may be NULL and are not read).  Everything is checked before
+ * the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer, batch / max_rows / sizes <= 0,
+ * row_floats < 7, NULL and non-NULL masks_dev in one call, pitch < img_w; TRTX_ERR_UNSUPPORTED where a CTA's shared-memory
+ * tables, 10 bytes per pixel of the widest frame's row + 8 * map_w bytes, exceed 227 KB (with 640-wide maps: frames wider
+ * than about 22 000 pixels).  Two launches per 64 frames, no workspace, no atomics; can be captured in a CUDA graph. */
+TRTX_API int trtx_yolop_postprocess_enqueue(const trtx_yolop_post_params* p, const trtx_frame* frames_host, int batch,
+                                            const float* dets_dev, int max_rows, const int32_t* seg_dev,
+                                            const int32_t* lane_dev, float* rows_dev, trtx_stream_t stream);
 
 #ifdef __cplusplus
 }

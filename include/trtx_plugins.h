@@ -70,15 +70,19 @@ struct YoloCore {
         p.is_pose = pose;
         p.is_obb = obb;
     }
-    // yolov5: YoloLayerPlugin(classCount, netW, netH, maxOut, is_seg, vector<YoloKernel>) (yolov5 yololayer.cu:22-39)
-    void init_v5(int nc, int w, int h, int max_out, bool seg, const void* kernels /* {int w,h; float a[6]}[] */, int n) {
+    // yolov5: YoloLayerPlugin(classCount, netW, netH, maxOut, is_seg, vector<YoloKernel>) (yolov5 yololayer.cu:22-39).
+    // yolov7 and YOLOP: the same arithmetic with 6-float rows, YoloLayerPlugin(classCount, netW, netH, maxOut,
+    // vector<YoloKernel>) (yolov7/plugin/yololayer.cu:21-36, yolop/yololayer.cu:28-44), det_floats = kV7Floats.
+    static constexpr int kV5Floats = 38, kV7Floats = 6;
+    void init_v5(int nc, int w, int h, int max_out, bool seg, const void* kernels /* {int w,h; float a[6]}[] */, int n,
+                 int det_floats = kV5Floats) {
         std::memset(&p, 0, sizeof(p));
         p.variant = TRTX_YOLO_V5;
         p.num_classes = nc;
         p.net_w = w;
         p.net_h = h;
         p.max_out = max_out;
-        p.det_floats = 38;
+        p.det_floats = det_floats;
         p.num_levels = n;
         p.is_seg = seg;
         p.gate = 0.1f;
@@ -90,10 +94,13 @@ struct YoloCore {
         }
     }
     int out_elems() const { return 1 + p.max_out * p.det_floats; }  // yololayer.cu:107-111
+    // the yolov7 / YOLOP blob: the yolov5 one without the is_seg byte (yolov7/plugin/yololayer.cu:62-77,
+    // yolop/yololayer.cu:81-101)
+    bool v7_layout() const { return p.variant == TRTX_YOLO_V5 && p.det_floats == kV7Floats; }
 
     size_t serial_size() const {
         if (p.variant == TRTX_YOLO_V8) return 4 * 8 + 4 * (size_t)p.num_levels + 3;  // yololayer.cu:97-101
-        return 25 + 32 * (size_t)p.num_levels;                                      // yolov5 yololayer.cu:72-83
+        return (v7_layout() ? 24 : 25) + 32 * (size_t)p.num_levels;                 // yolov5 yololayer.cu:72-83
     }
     void serialize(void* buffer) const {
         char* d = static_cast<char*>(buffer);
@@ -117,7 +124,7 @@ struct YoloCore {
             detail::write(d, p.net_w);
             detail::write(d, p.net_h);
             detail::write(d, p.max_out);
-            detail::write(d, (bool)p.is_seg);
+            if (!v7_layout()) detail::write(d, (bool)p.is_seg);
             for (int i = 0; i < p.num_levels; ++i) {
                 detail::write(d, p.grid_w[i]);
                 detail::write(d, p.grid_h[i]);
@@ -125,8 +132,9 @@ struct YoloCore {
             }
         }
     }
-    // returns false on a malformed blob (the reference asserts, yololayer.cu:72)
-    bool deserialize(const void* data, size_t length, int variant) {
+    // returns false on a malformed blob (the reference asserts, yololayer.cu:72).  variant TRTX_YOLO_V5 with v7 = true reads
+    // the yolov7 / YOLOP layout.
+    bool deserialize(const void* data, size_t length, int variant, bool v7 = false) {
         const char* d = static_cast<const char*>(data);
         if (variant == TRTX_YOLO_V8) {
             if (length < 35) return false;
@@ -150,41 +158,83 @@ struct YoloCore {
             init_v8(nc, nk, kt, w, h, mo, seg, pose, obb, st, ns);
             thread_count = tc;
         } else {
-            if (length < 25) return false;
+            const size_t header = v7 ? 24 : 25;
+            if (length < header) return false;
             int nc, tc, kc, w, h, mo;
-            bool seg;
+            bool seg = false;
             detail::read(d, nc);
             detail::read(d, tc);
             detail::read(d, kc);
             detail::read(d, w);
             detail::read(d, h);
             detail::read(d, mo);
-            detail::read(d, seg);
-            if (kc <= 0 || kc > TRTX_MAX_LEVELS || length != 25 + 32 * (size_t)kc) return false;
-            init_v5(nc, w, h, mo, seg, d, kc);
+            if (!v7) detail::read(d, seg);
+            if (kc <= 0 || kc > TRTX_MAX_LEVELS || length != header + 32 * (size_t)kc) return false;
+            init_v5(nc, w, h, mo, seg, d, kc, v7 ? kV7Floats : kV5Floats);
             thread_count = tc;
         }
         return true;
     }
-    // createPlugin field parsing: v8 "combinedInfo" (block.cpp:264-296), v5 "netinfo" + "kernels" (model.cpp:249-277)
+    // createPlugin field parsing: v8 "combinedInfo" (block.cpp:264-296); "netinfo" + "kernels" with a netinfo of 5 ints
+    // (yolov5, model.cpp:249-277) or of 4 (yolov7, yolov7/src/block.cpp:224-241: 6-float rows); YOLOP's "netdata" +
+    // "yolodata1".."yolodataN" (yolop/common.hpp:318-356).  Every field's declared length is checked before it is read,
+    // except netdata's, whose fourth int lies past the declared 3 (below).
     bool from_fields(const nvinfer1::PluginFieldCollection* fc) {
-        if (!fc) return false;
-        if (fc->nbFields == 1 && fc->fields[0].name && std::strcmp(fc->fields[0].name, "combinedInfo") == 0) {
-            const int* ci = static_cast<const int*>(fc->fields[0].data);
-            const int n = fc->fields[0].length - 9;
-            if (!ci || n <= 0 || n > TRTX_MAX_LEVELS) return false;
+        if (!fc || fc->nbFields <= 0 || !fc->fields) return false;
+        const nvinfer1::PluginField* f = fc->fields;
+        for (int i = 0; i < fc->nbFields; ++i)
+            if (!f[i].name || !f[i].data) return false;
+        if (fc->nbFields == 1 && std::strcmp(f[0].name, "combinedInfo") == 0) {
+            const int* ci = static_cast<const int*>(f[0].data);
+            const int n = f[0].length - 9;
+            if (n <= 0 || n > TRTX_MAX_LEVELS) return false;
             init_v8(ci[0], ci[1], (float)ci[2], ci[3], ci[4], ci[5], ci[6] != 0, ci[7] != 0, ci[8] != 0, ci + 9, n);
             return true;
         }
-        if (fc->nbFields == 2 && fc->fields[0].name && fc->fields[1].name && std::strcmp(fc->fields[0].name, "netinfo") == 0 &&
-            std::strcmp(fc->fields[1].name, "kernels") == 0) {
-            const int* ni = static_cast<const int*>(fc->fields[0].data);
-            const int n = fc->fields[1].length;
-            if (!ni || !fc->fields[1].data || n <= 0 || n > TRTX_MAX_LEVELS) return false;
-            init_v5(ni[0], ni[1], ni[2], ni[3], ni[4] != 0, fc->fields[1].data, n);
+        if (fc->nbFields == 2 && std::strcmp(f[0].name, "netinfo") == 0 && std::strcmp(f[1].name, "kernels") == 0) {
+            const int* ni = static_cast<const int*>(f[0].data);
+            const int n = f[1].length;
+            if (f[0].length < 4 || n <= 0 || n > TRTX_MAX_LEVELS) return false;
+            if (f[0].length == 4)
+                init_v5(ni[0], ni[1], ni[2], ni[3], false, f[1].data, n, kV7Floats);
+            else
+                init_v5(ni[0], ni[1], ni[2], ni[3], ni[4] != 0, f[1].data, n);
             return true;
         }
-        return false;
+        return yolop_fields(fc);
+    }
+    // YOLOP, parsed as yolop/yololayer.cu:289-320 parses it: fields in any order; "netdata" = {classCount, netW, netH,
+    // maxOut}, declared with length 3 by YOLOP's builder (common.hpp:328-336) but read as 4 ints, as the reference reads
+    // it; "yolodata1".."yolodata3" = {grid w, grid h, 6 anchors} as ints, each converted to a float anchor, yolodataK into
+    // kernel slot 3 - K (the builder passes its stride-32 head first).  Rejected: a field of another name, a netdata
+    // shorter than 3, a yolodataK whose length is not 8, a K outside 1..3 or given twice, a missing field.
+    bool yolop_fields(const nvinfer1::PluginFieldCollection* fc) {
+        constexpr int n = 3;  // the reference's yolo_kernels(3)
+        if (fc->nbFields != n + 1) return false;
+        const int* nd = nullptr;
+        char kernels[n][32];
+        bool seen[n] = {};
+        for (int i = 0; i < fc->nbFields; ++i) {
+            const nvinfer1::PluginField& f = fc->fields[i];
+            if (std::strcmp(f.name, "netdata") == 0) {
+                if (nd || f.length < 3) return false;
+                nd = static_cast<const int*>(f.data);
+                continue;
+            }
+            const int k = std::strncmp(f.name, "yolodata", 8) == 0 && f.name[9] == '\0' ? f.name[8] - '0' : 0;
+            if (k < 1 || k > n || seen[k - 1] || f.length != 8) return false;
+            seen[k - 1] = true;
+            const int* v = static_cast<const int*>(f.data);
+            char* o = kernels[n - k];
+            std::memcpy(o, v, 8);  // grid w, h
+            for (int j = 0; j < 6; ++j) {
+                const float a = (float)v[2 + j];
+                std::memcpy(o + 8 + 4 * j, &a, 4);
+            }
+        }
+        if (!nd) return false;
+        init_v5(nd[0], nd[1], nd[2], nd[3], false, kernels, n, kV7Floats);
+        return true;
     }
 };
 
@@ -308,8 +358,10 @@ class YoloPluginCreatorT : public nvinfer1::IPluginCreator {
     }
     nvinfer1::IPluginV2* deserializePlugin(const char*, const void* data, size_t len) TRTX_NOEXCEPT override {
         YoloCore c;
-        // the two layouts differ in size: v8 = 35 + 4n bytes, v5 = 25 + 32n bytes
-        if (!c.deserialize(data, len, TRTX_YOLO_V8) && !c.deserialize(data, len, TRTX_YOLO_V5)) return nullptr;
+        // the three layouts differ in size modulo 4: v8 = 35 + 4n bytes (3), v5 = 25 + 32n (1), yolov7 / YOLOP = 24 + 32n (0)
+        if (!c.deserialize(data, len, TRTX_YOLO_V8) && !c.deserialize(data, len, TRTX_YOLO_V5) &&
+            !c.deserialize(data, len, TRTX_YOLO_V5, true))
+            return nullptr;
         return make(c);
     }
     void setPluginNamespace(const char* n) TRTX_NOEXCEPT override { ns_ = n ? n : ""; }

@@ -113,6 +113,10 @@ class FacePostParams(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("variant", "in_w", "in_h", "row_floats", "lmk_offset")] + [("conf_thresh", C.c_float)]
 
 
+class YolopPostParams(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("net_w", "net_h", "map_w", "map_h", "row_floats")]
+
+
 # TRTX_LIB: another build of the same ABI (the probe build of tools/nms_probe.py); default = the in-tree release library
 LIB_PATH = Path(os.environ.get("TRTX_LIB") or Path(__file__).resolve().parent / "lib" / "libtrtx_hot.so")
 
@@ -171,6 +175,9 @@ SYMBOLS = {
     "trtx_get_corner": (_i, [_i, _i, _i, _i, C.POINTER(C.c_float), _f, C.POINTER(C.c_int)]),
     "trtx_yolo_pose_obb_postprocess_enqueue": (_i, [C.POINTER(PoseObbParams), C.POINTER(C.c_int32), _i, _vp, _i, _vp, _vp]),
     "trtx_retina_postprocess_enqueue": (_i, [C.POINTER(FacePostParams), C.POINTER(C.c_int32), _i, _vp, _i, _vp, _vp]),
+    "trtx_yolop_preprocess_enqueue": (_i, [C.POINTER(ImageDesc), _i, _i, _i, _vp, _vp]),
+    "trtx_yolop_get_rect": (_i, [_i, _i, _i, _i, C.POINTER(C.c_float), C.POINTER(C.c_int)]),
+    "trtx_yolop_postprocess_enqueue": (_i, [C.POINTER(YolopPostParams), C.POINTER(Frame), _i, _vp, _i, _vp, _vp, _vp, _vp]),
     "trtx_yolo_decode_nms_gather_enqueue": (_i, [C.POINTER(YoloParams), C.POINTER(NmsParams), _i, _pp, _vp, _vp, _vp, _sz,
                                                  C.POINTER(Gather), _vp]),
     "trtx_gather_wait_enqueue": (_i, [C.POINTER(Gather), _vp]),
@@ -202,7 +209,7 @@ def load() -> C.CDLL:
         fn.restype = res
         fn.argtypes = args
     for which, st in enumerate((YoloParams, NmsParams, RetinaParams, ImageDesc, MaskParams, RcnnPostParams,
-                                   Frame, PoseObbParams, Frame, FacePostParams)):
+                                   Frame, PoseObbParams, Frame, FacePostParams, YolopPostParams)):
         if lib.trtx_abi_sizeof(which) != C.sizeof(st):
             raise TrtxError(f"{LIB_PATH} was built from a different trtx_hot.h: sizeof({st.__name__}) = "
                             f"{lib.trtx_abi_sizeof(which)} in the library, {C.sizeof(st)} in the binding (rebuild)")

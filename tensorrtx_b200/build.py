@@ -85,9 +85,11 @@ def build(force: bool = False, verbose: bool = False, probe: bool = False) -> Pa
 
 def build_oracle() -> Path:
     """Compile the CPU oracles (test infrastructure) and, when /root/reference exists, oracle/_ref."""
-    r = subprocess.run(["make", "-C", str(ROOT / "oracle")], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    if r.returncode != 0:
-        raise RuntimeError(f"oracle build failed:\n{r.stdout}")
+    for makefile in ("Makefile", "yolop.mk"):
+        r = subprocess.run(["make", "-C", str(ROOT / "oracle"), "-f", makefile], stdout=subprocess.PIPE, stderr=subprocess.STDOUT,
+                           text=True)
+        if r.returncode != 0:
+            raise RuntimeError(f"oracle build failed ({makefile}):\n{r.stdout}")
     return ROOT / "oracle" / "libtrtx_oracle.so"
 
 

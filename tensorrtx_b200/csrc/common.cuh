@@ -333,6 +333,25 @@ __host__ __device__ inline void retina_get_rect_adapt_landmark(int input_w, int 
     for (int i = 0; i < 10; ++i) lmk[i] = yolo_map_landmark(lb, i & 1, lmk[i]);
 }
 
+// YOLOP's get_rect (yolop/common.hpp:13-37): box cx, cy, w, h; the letterbox expressions are get_rect's (yolo_letterbox).
+// Every statement stores to an int, so a corner is truncated twice: after `bbox[0] - bbox[2] / 2.f` (minus the pad on the
+// padded axis, all float) and after its division by the ratio (int / float: a float division).  No clamp; rect =
+// {l, t, r - l, b - t}.  Undefined cases as the compiled x86-64 reference behaves: trunc_to_int_x86, and int differences
+// that wrap modulo 2^32.
+__host__ __device__ inline void yolop_get_rect(const YoloLetterbox& lb, const float bbox[4], int rect[4]) {
+    float c[4] = {f_sub(bbox[0], f_div(bbox[2], 2.f)), f_sub(bbox[1], f_div(bbox[3], 2.f)), f_add(bbox[0], f_div(bbox[2], 2.f)),
+                  f_add(bbox[1], f_div(bbox[3], 2.f))};  // l, t, r, b
+    const int padded = lb.by_w ? 1 : 0;                 // the axis that carries the pad: y when the width fills the input
+    c[padded] = f_sub(c[padded], lb.pad);
+    c[padded + 2] = f_sub(c[padded + 2], lb.pad);
+    int v[4];
+    for (int k = 0; k < 4; ++k) v[k] = trunc_to_int_x86(f_div((float)trunc_to_int_x86(c[k]), lb.ratio));
+    rect[0] = v[0];
+    rect[1] = v[1];
+    rect[2] = (int)((uint32_t)v[2] - (uint32_t)v[0]);
+    rect[3] = (int)((uint32_t)v[3] - (uint32_t)v[1]);
+}
+
 __device__ __forceinline__ int warp_excl_scan(int v, int lane, int* total) {
     int x = v;
 #pragma unroll

@@ -1176,6 +1176,109 @@ __global__ void __launch_bounds__(kRowsThreads) face_rows_kernel(const __grid_co
     frame_rows<FaceRow>(a);
 }
 
+// YOLOP: the driver's nms() result mapped by YOLOP's own get_rect (yolop/common.hpp:13-37, yolop.cpp:129-146) into
+// (x, y, w, h, conf, class) rows.
+struct YolopRowsArgs {
+    RowFrames f;
+    int net_w, net_h;
+};
+
+struct YolopRow {
+    static constexpr int kGeo = 4;  // the rectangle
+    YoloLetterbox lb;
+    __device__ YolopRow(const YolopRowsArgs& args, int j) : lb(yolo_letterbox(args.net_w, args.net_h, args.f.img_w[j], args.f.img_h[j])) {}
+    __device__ bool pass(const float* d) const { return (int)d[6] == 1; }  // every row of a greedy NMS output
+    __device__ void geometry(const float* d, int g[4]) const { yolop_get_rect(lb, d, g); }
+    __device__ float value(const float* d, const int* g, int e) const { return e < 4 ? (float)g[e] : d[e]; }  // conf, class
+};
+
+__global__ void __launch_bounds__(kRowsThreads) yolop_rows_kernel(const __grid_constant__ YolopRowsArgs a) {
+    frame_rows<YolopRow>(a);
+}
+
+// YOLOP's labels (yolop/yolop.cpp:148-169): the drivable-area and lane maps resized to the frame with cv::resize(INTER_NEAREST)
+// and combined per pixel, 2 = lane, else 1 = drivable area, else 0, into the frame's u8 canvas.  Bound by the canvas writes.
+// A CTA owns a band of kLabelBand canvas rows of one frame (grid: bands x frames):
+//   1. the nearest source column of every canvas column (sx, uint16 in shared memory) and the map row of every band row;
+//      sy is non-decreasing in y, so the band's distinct map rows are consecutive;
+//   2. the label of every map pixel of those rows, from the two int32 maps (small enough to stay in L2), as bytes in shared
+//      memory;
+//   3. each warp stages its row's bytes in shared memory, then writes the row with 16-byte stores (a head of 0..15 bytes up to
+//      the first 16-byte boundary and a tail of 0..15 bytes are scalar: pitch and base may be anything); bytes past img_w are
+//      not touched.
+constexpr int kLabelBand = 8;  // canvas rows per CTA: small bands keep every SM busy at b8
+constexpr int kLabelThreads = 256;
+constexpr int kLabelWarps = kLabelThreads / kWarp;
+
+struct YolopLabelFrame {
+    uint8_t* canvas;
+    double ifx, ify;  // cv::resize: 1. / ((double)dsize / ssize) per axis
+    int img_w, img_h, pitch;
+};
+struct YolopLabelArgs {
+    YolopLabelFrame fr[kMaxFrames];
+    const int32_t* seg;   // [B, map_h, map_w]
+    const int32_t* lane;
+    int map_w, map_h, base;
+    int sx_bytes;         // the sx table's bytes in dynamic shared memory (the widest frame, rounded to 16)
+    int stage_bytes;      // bytes of a warp's staged row: the widest frame + 15, rounded to 16
+};
+
+__global__ void __launch_bounds__(kLabelThreads) yolop_label_kernel(const __grid_constant__ YolopLabelArgs a) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    __shared__ int s_srow[kLabelBand];  // map row of each distinct slot
+    __shared__ int s_slot[kLabelBand];  // slot of each band row
+    __shared__ int s_nslots;
+    const YolopLabelFrame& f = a.fr[blockIdx.y];
+    const int y0 = blockIdx.x * kLabelBand;
+    if (y0 >= f.img_h) return;  // uniform: a band past this frame's height (bands are sized for the tallest frame)
+    const int rows = min(kLabelBand, f.img_h - y0), tid = threadIdx.x;
+    const int warp = tid / kWarp, l = tid & (kWarp - 1);
+    uint16_t* sx = reinterpret_cast<uint16_t*>(smem);
+    uint8_t* lab = smem + a.sx_bytes;  // [slots][map_w], then the warps' staged rows
+    if (warp == 0) {  // lane k: band row k; sy is non-decreasing, so a new slot starts where it changes
+        const int sy = l < rows ? min((int)floor(__dmul_rn((double)(y0 + l), f.ify)), a.map_h - 1) : INT_MAX;
+        const int prev = __shfl_up_sync(0xffffffffu, sy, 1);
+        const unsigned starts = __ballot_sync(0xffffffffu, l < rows && (l == 0 || sy != prev));
+        const int slot = __popc(starts & (0xffffffffu >> (31 - l))) - 1;
+        if (l < rows) {
+            s_slot[l] = slot;
+            if ((starts >> l) & 1u) s_srow[slot] = sy;
+        }
+        if (l == 0) s_nslots = __popc(starts);
+    }
+    for (int x = tid; x < f.img_w; x += kLabelThreads) sx[x] = (uint16_t)min((int)floor(__dmul_rn((double)x, f.ifx)), a.map_w - 1);
+    __syncthreads();
+    const size_t map = (size_t)a.map_w * a.map_h, b = (size_t)(a.base + blockIdx.y);
+    const int32_t* seg = a.seg + b * map;
+    const int32_t* lane = a.lane + b * map;
+    const int items = s_nslots * a.map_w;
+#pragma unroll 4
+    for (int i = tid; i < items; i += kLabelThreads) {
+        const int s = i / a.map_w, m = i - s * a.map_w;
+        const size_t o = (size_t)s_srow[s] * a.map_w + m;
+        lab[i] = __ldg(lane + o) != 0 ? 2 : (__ldg(seg + o) != 0 ? 1 : 0);
+    }
+    __syncthreads();
+    // each warp writes rows warp, warp + kLabelWarps, ...: its bytes staged so that the 16-byte runs of the canvas row are
+    // 16-byte aligned in shared memory too (byte x at x + pad)
+    uint8_t* stage = lab + ((kLabelBand * a.map_w + 15) & ~15) + warp * a.stage_bytes;
+    const int w = f.img_w;
+    for (int k = warp; k < rows; k += kLabelWarps) {
+        const uint8_t* L = lab + s_slot[k] * a.map_w;
+        uint8_t* row = f.canvas + (size_t)(y0 + k) * (size_t)f.pitch;
+        const int head = min((int)((16u - (unsigned)(reinterpret_cast<uintptr_t>(row) & 15u)) & 15u), w);
+        const int nvec = (w - head) >> 4, tail0 = head + 16 * nvec, pad = (16 - head) & 15;
+        for (int x = l; x < w; x += kWarp) stage[x + pad] = L[sx[x]];  // consecutive lanes, consecutive x: no bank conflicts
+        __syncwarp();
+        if (l < head) row[l] = stage[l + pad];
+        if (tail0 + l < w) row[tail0 + l] = stage[tail0 + l + pad];
+        for (int q = l; q < nvec; q += kWarp)
+            *reinterpret_cast<uint4*>(row + head + 16 * q) = *reinterpret_cast<const uint4*>(stage + head + pad + 16 * q);
+        __syncwarp();  // the next row reuses the stage
+    }
+}
+
 // Every frame size of a per-row call is checked before the first launch, so that a rejected call writes nothing.
 inline bool frames_valid(const int32_t* frame_wh_host, int batch) {
     for (int i = 0; i < batch; ++i)
@@ -1183,21 +1286,24 @@ inline bool frames_valid(const int32_t* frame_wh_host, int batch) {
     return true;
 }
 
-// One launch of `kernel` per <= kMaxFrames frames, each with its frames' sizes in the launch parameters.
-template <class Args>
-int launch_frame_rows(void (*kernel)(Args), Args& a, const int32_t* frame_wh_host, int batch, cudaStream_t st) {
+// One launch of `kernel` per <= kMaxFrames frames, each with its frames' sizes in the launch parameters: size(i, w, h) gives
+// frame i's.
+template <class Args, class Size>
+int launch_frame_rows(void (*kernel)(Args), Args& a, Size size, int batch, cudaStream_t st) {
     for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {
         const int n = min(batch - i0, kMaxFrames);
         a.f.base = i0;
-        for (int j = 0; j < n; ++j) {
-            a.f.img_w[j] = frame_wh_host[2 * (i0 + j)];
-            a.f.img_h[j] = frame_wh_host[2 * (i0 + j) + 1];
-        }
+        for (int j = 0; j < n; ++j) size(i0 + j, a.f.img_w[j], a.f.img_h[j]);
         kernel<<<n, kRowsThreads, 0, st>>>(a);
         const int rc = check_launch();
         if (rc) return rc;
     }
     return TRTX_OK;
+}
+template <class Args>
+int launch_frame_rows(void (*kernel)(Args), Args& a, const int32_t* frame_wh_host, int batch, cudaStream_t st) {
+    return launch_frame_rows(kernel, a, [&](int i, int& w, int& h) { w = frame_wh_host[2 * i], h = frame_wh_host[2 * i + 1]; },
+                             batch, st);
 }
 
 }  // namespace trtx
@@ -1566,6 +1672,69 @@ TRTX_API int trtx_retina_postprocess_enqueue(const trtx_face_post_params* p, con
     a.lmk_offset = p->lmk_offset;
     a.conf_thresh = p->conf_thresh;
     return launch_frame_rows(face_rows_kernel, a, frame_wh_host, batch, static_cast<cudaStream_t>(stream));
+}
+
+TRTX_API int trtx_yolop_postprocess_enqueue(const trtx_yolop_post_params* p, const trtx_frame* frames_host, int batch,
+                                            const float* dets_dev, int max_rows, const int32_t* seg_dev,
+                                            const int32_t* lane_dev, float* rows_dev, trtx_stream_t stream) {
+    if (!p || !frames_host || batch <= 0 || !dets_dev || !rows_dev || max_rows <= 0) return TRTX_ERR_INVALID;
+    if (p->net_w <= 0 || p->net_h <= 0 || p->map_w <= 0 || p->map_h <= 0 || p->row_floats < 7) return TRTX_ERR_INVALID;
+    const bool labels = frames_host[0].masks_dev != nullptr;
+    if (labels && (!seg_dev || !lane_dev)) return TRTX_ERR_INVALID;
+    int w_max = 0;
+    for (int i = 0; i < batch; ++i) {
+        const trtx_frame& d = frames_host[i];
+        if (d.img_w <= 0 || d.img_h <= 0 || (d.masks_dev != nullptr) != labels) return TRTX_ERR_INVALID;
+        if (labels && d.pitch < d.img_w) return TRTX_ERR_INVALID;
+        w_max = max(w_max, d.img_w);
+    }
+    // the sx table (uint16, so map_w <= 65536), the label rows of a band and the warps' staged rows in shared memory
+    const int sx_bytes = (int)align_up(2 * (size_t)w_max, 16), stage_bytes = (int)align_up((size_t)w_max + 15, 16);
+    const size_t smem = (size_t)sx_bytes + align_up((size_t)kLabelBand * p->map_w, 16) + (size_t)kLabelWarps * stage_bytes;
+    if (labels && smem > 227 * 1024) return TRTX_ERR_UNSUPPORTED;
+    if (labels && smem > 48 * 1024 &&
+        cudaFuncSetAttribute(yolop_label_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+        g_last_cuda_error = (int)cudaGetLastError();
+        return TRTX_ERR_CUDA;
+    }
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    YolopRowsArgs r;
+    r.f.dets = dets_dev;
+    r.f.rows = rows_dev;
+    r.f.row_floats = p->row_floats;
+    r.f.out_floats = 6;
+    r.f.max_rows = max_rows;
+    r.net_w = p->net_w;
+    r.net_h = p->net_h;
+    int rc = launch_frame_rows(yolop_rows_kernel, r, [&](int i, int& w, int& h) { w = frames_host[i].img_w, h = frames_host[i].img_h; },
+                               batch, st);
+    if (rc || !labels) return rc;
+    YolopLabelArgs a;
+    a.seg = seg_dev;
+    a.lane = lane_dev;
+    a.map_w = p->map_w;
+    a.map_h = p->map_h;
+    a.sx_bytes = sx_bytes;
+    a.stage_bytes = stage_bytes;
+    for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {
+        const int n = min(batch - i0, kMaxFrames);
+        int bands = 0;
+        a.base = i0;
+        for (int j = 0; j < n; ++j) {
+            const trtx_frame& d = frames_host[i0 + j];
+            YolopLabelFrame& f = a.fr[j];
+            f.canvas = d.masks_dev;
+            f.img_w = d.img_w;
+            f.img_h = d.img_h;
+            f.pitch = d.pitch;
+            f.ifx = 1. / ((double)d.img_w / p->map_w);
+            f.ify = 1. / ((double)d.img_h / p->map_h);
+            bands = max(bands, (d.img_h + kLabelBand - 1) / kLabelBand);
+        }
+        yolop_label_kernel<<<dim3(bands, n), kLabelThreads, smem, st>>>(a);
+        if ((rc = check_launch())) return rc;
+    }
+    return TRTX_OK;
 }
 
 }  // extern "C"

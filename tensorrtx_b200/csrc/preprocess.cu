@@ -577,23 +577,51 @@ __device__ __forceinline__ float cls_input_value(int variant, int c, uint32_t u)
     return __double2float_rn(__ddiv_rn(__dsub_rn(__ddiv_rn((double)(float)u, 255.0), mean), std));
 }
 
+// YOLOP's preprocess_img (yolop/utils.h:11-36) after the resize, the value of byte u in plane c (0 = B, 1 = G, 2 = R: the
+// driver copies the planes in BGR order, yolop/yolop.cpp:110-127, so Scalar(0.485, ...) meets B first):
+//   convertTo(CV_32FC3, 1.f / 255.f)       t = (float)u * (1.f / 255.f)
+//   cv::subtract(tensor, Scalar(mean))     s = t - (float)mean_c, in float
+//   cv::divide(tensor, Scalar(std))        (float)((double)s / std_c), in double
+// Pinned against cv2 4.13 on all 3 x 256 bytes (tests/test_yolop_cpu.py).
+__device__ __forceinline__ float yolop_input_value(int c, uint32_t u) {
+    const double mean = c == 0 ? 0.485 : (c == 1 ? 0.456 : 0.406), std = c == 0 ? 0.229 : (c == 1 ? 0.224 : 0.225);
+    const float s = __fsub_rn(__fmul_rn((float)u, 1.f / 255.f), (float)mean);
+    return __double2float_rn(__ddiv_rn((double)s, std));
+}
+
+// The input conventions of the planar stores: In::kCanvas is the byte of the letterbox canvas, In::channel(c) the BGR
+// channel that plane c takes, In::value(c, u) the engine input value of byte u in plane c.
 template <int kVariant>
-struct ClsPlanarStore {
+struct ClsInput {
+    static constexpr uint32_t kCanvas = 128u;  // the V5 canvas, Scalar(128, 128, 128); V8 has none
+    static __device__ __forceinline__ int channel(int c) { return 2 - c; }  // cvtColor BGR2RGB / the driver's planes R, G, B
+    static __device__ __forceinline__ float value(int c, uint32_t u) { return cls_input_value(kVariant, c, u); }
+};
+struct YolopInput {
+    static constexpr uint32_t kCanvas = 114u;  // Scalar(114, 114, 114)
+    static __device__ __forceinline__ int channel(int c) { return c; }
+    static __device__ __forceinline__ float value(int c, uint32_t u) { return yolop_input_value(c, u); }
+};
+
+// [B, 3, net_h, net_w] planes: the band is three contiguous runs of band * net_w floats, each written by store_band_run; the
+// value of a byte comes from a per-CTA table of 3 x 256 floats.
+template <class In>
+struct PlanarStore {
     template <class Pix>
     static __device__ __forceinline__ void run(const RcnnPreArgs& a, const RcnnPreImage& im, int y0, int rows, int k_lo, int k_hi,
                                                Pix pix, float* __restrict__ dst) {
         __shared__ float lut[3][256];
-        for (int j = threadIdx.x; j < 3 * 256; j += blockDim.x) lut[j >> 8][j & 255] = cls_input_value(kVariant, j >> 8, j & 255);
+        for (int j = threadIdx.x; j < 3 * 256; j += blockDim.x) lut[j >> 8][j & 255] = In::value(j >> 8, j & 255);
         __syncthreads();
         const int W = a.net_w;
 #pragma unroll 1
         for (int c = 0; c < 3; ++c) {
-            const int ch = 2 - c;  // cvtColor BGR2RGB / the driver's planes R, G, B
+            const int ch = In::channel(c);
             float* base = dst + (((size_t)im.dst_idx * 3 + c) * a.net_h + y0) * (size_t)W;
             store_band_run(base, rows * W, W, [&](int k, int x) -> float {
                 const int i = x - im.x0;
                 const bool in = k >= k_lo && k < k_hi && (unsigned)i < (unsigned)im.rw;
-                return lut[c][in ? pix(k, 3 * i + ch) : 128u];  // the V5 canvas, Scalar(128, 128, 128)
+                return lut[c][in ? pix(k, 3 * i + ch) : In::kCanvas];
             });
         }
     }
@@ -602,7 +630,12 @@ struct ClsPlanarStore {
 template <int kVariant>
 __global__ void __launch_bounds__(kRcnnPreThreads) cls_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
                                                                          float* __restrict__ dst) {
-    resize_band<ClsPlanarStore<kVariant>>(a, dst);
+    resize_band<PlanarStore<ClsInput<kVariant>>>(a, dst);
+}
+
+__global__ void __launch_bounds__(kRcnnPreThreads) yolop_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
+                                                                           float* __restrict__ dst) {
+    resize_band<PlanarStore<YolopInput>>(a, dst);
 }
 
 // One launch of `kernel` per kMaxRcnnPreImages frames: make(i, im) fills the band descriptor of frame i (validated before).
@@ -737,6 +770,13 @@ TRTX_API int trtx_retina_get_rect_adapt_landmark(int input_w, int input_h, int i
                                                  int rect[4]) {
     if (!bbox || !lmk || !rect || input_w <= 0 || input_h <= 0 || img_w <= 0 || img_h <= 0) return TRTX_ERR_INVALID;
     retina_get_rect_adapt_landmark(input_w, input_h, img_w, img_h, bbox, lmk, rect);
+    return TRTX_OK;
+}
+
+// get_rect of YOLOP, yolop/common.hpp:13-37 (yolop_get_rect in common.cuh, shared with the YOLOP post-process kernel of mask.cu).
+TRTX_API int trtx_yolop_get_rect(int net_w, int net_h, int img_w, int img_h, const float bbox[4], int rect[4]) {
+    if (!bbox || !rect || net_w <= 0 || net_h <= 0 || img_w <= 0 || img_h <= 0) return TRTX_ERR_INVALID;
+    yolop_get_rect(yolo_letterbox(net_w, net_h, img_w, img_h), bbox, rect);
     return TRTX_OK;
 }
 
@@ -894,6 +934,27 @@ TRTX_API int trtx_cls_preprocess_enqueue(int variant, const trtx_image_desc* ima
     auto* kernel = variant == TRTX_YOLO_V8 ? cls_preprocess_kernel<TRTX_YOLO_V8> : cls_preprocess_kernel<TRTX_YOLO_V5>;
     return launch_bands(kernel, batch, net_w, net_h, dst_dev, smem_max, static_cast<cudaStream_t>(stream),
                         [&](int i, RcnnPreImage& im) { cls_band_image(variant, images_host[i], net_w, net_h, im); });
+}
+
+// YOLOP's preprocess_img letterbox is yolov5-cls's (the same statements, yolop/utils.h:13-25), so its band descriptor is
+// cls_band_image's V5 one; only the store differs (canvas 114, BGR planes, its own value chain).
+TRTX_API int trtx_yolop_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
+                                           trtx_stream_t stream) {
+    if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
+    if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
+    // every descriptor is checked before the first launch, so that a rejected call writes nothing
+    size_t smem_max = 0;
+    for (int i = 0; i < batch; ++i) {
+        const trtx_image_desc& d = images_host[i];
+        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
+        RcnnPreImage im;
+        if (!cls_band_image(TRTX_YOLO_V5, d, net_w, net_h, im)) return TRTX_ERR_UNSUPPORTED;
+        const size_t smem = (size_t)kRcnnPreSlots * 3 * (size_t)im.rw * sizeof(int16_t);
+        if (smem > kClsMaxDynamicSmem) return TRTX_ERR_UNSUPPORTED;
+        smem_max = smem > smem_max ? smem : smem_max;
+    }
+    return launch_bands(yolop_preprocess_kernel, batch, net_w, net_h, dst_dev, smem_max, static_cast<cudaStream_t>(stream),
+                        [&](int i, RcnnPreImage& im) { cls_band_image(TRTX_YOLO_V5, images_host[i], net_w, net_h, im); });
 }
 
 }  // extern "C"

@@ -361,7 +361,8 @@ class YoloLayerPluginV5(_TunableYoloLayer):
 class YoloLayerPluginV7(YoloLayerPluginV5):
     """yolov7/plugin/yololayer.h:9-73 (same kernel arithmetic as yolov5, yolov7/plugin/yololayer.cu:152-200, but
     Detection = 6 floats, yolov7/include/types.h:11-16; also yolov10 / yolov13 style rows).  No segmentation flag:
-    ctor (classCount, netWidth, netHeight, maxOut, vYoloKernel), serialization without the bool."""
+    ctor (classCount, netWidth, netHeight, maxOut, vYoloKernel), serialization without the bool.  YOLOP's plugin
+    (yolop/yololayer.h) is this one with YOLOP's arguments: (1, 640, 384, 1000, kernels with the stride-32 one first)."""
     DET_FLOATS = 6
 
     def __init__(self, classCount: int, netWidth: int, netHeight: int, maxOut: int, vYoloKernel: Sequence[YoloKernel],
@@ -1179,6 +1180,73 @@ def cls_preprocess(images: Sequence[torch.Tensor], variant: int, net_w: int, net
     L.check(lib.trtx_cls_preprocess_enqueue(variant, descs, n, net_w, net_h, _ptr(out), _stream(stream)),
             "trtx_cls_preprocess_enqueue")
     return out
+
+
+YOLOP_NET = (640, 384)  # Yolo::INPUT_W, INPUT_H (yolop/yololayer.h)
+YOLOP_MAP = (640, 360)  # Yolo::IMG_W, IMG_H: the drivable-area and lane maps
+
+
+def yolop_preprocess(images: Sequence[torch.Tensor], out: torch.Tensor | None = None, net_w: int = YOLOP_NET[0],
+                     net_h: int = YOLOP_NET[1], stream=None) -> torch.Tensor:
+    """GPU drop-in for YOLOP's preprocess_img (yolop/utils.h:11-36) and the driver's plane copy (yolop/yolop.cpp:110-127)
+    for a batch of device frames: images[i] is a u8 HWC BGR cuda tensor [h, w, 3] with packed pixels (rows may be pitched,
+    sizes may differ) -> [B, 3, net_h, net_w] float32 planes in B, G, R order, the engine input: the letterbox on a 114-grey
+    canvas, / 255, minus the ImageNet mean, over its std.  One launch per 64 images, no synchronisation."""
+    lib = L.load()
+    n = len(images)
+    descs = _image_descs(images)
+    out = _out_tensor(out, (n, 3, net_h, net_w), torch.float32, images[0].device if n else "cuda",
+                      f"out must be float32 [{n}, 3, {net_h}, {net_w}]", contiguous=False)
+    L.check(lib.trtx_yolop_preprocess_enqueue(descs, n, net_w, net_h, _ptr(out), _stream(stream)), "trtx_yolop_preprocess_enqueue")
+    return out
+
+
+def yolop_get_rect(img_w: int, img_h: int, bbox, net_w: int = YOLOP_NET[0], net_h: int = YOLOP_NET[1]):
+    """get_rect(img, bbox) of yolop/common.hpp:13-37: bbox cx, cy, w, h in network pixels -> (x, y, w, h) in the frame."""
+    b = (C.c_float * 4)(*[float(v) for v in bbox])
+    r = (C.c_int * 4)()
+    L.check(L.load().trtx_yolop_get_rect(net_w, net_h, img_w, img_h, b, r), "trtx_yolop_get_rect")
+    return tuple(r)
+
+
+def yolop_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]], *, max_rows: int,
+                      seg: torch.Tensor | None = None, lane: torch.Tensor | None = None, labels: bool = True,
+                      row_floats: int = 7, net_w: int = YOLOP_NET[0], net_h: int = YOLOP_NET[1],
+                      rows_out: torch.Tensor | None = None, canvases_out: Sequence[torch.Tensor] | None = None, stream=None):
+    """GPU drop-in for YOLOP's host stages after NMS: get_rect per box (yolop/common.hpp:13-37) and the per-pixel label loop
+    over the drivable-area and lane maps (yolop/yolop.cpp:148-169), for a batch of frames of any sizes.
+    dets [B, 1 + max_rows*row_floats]: count, then (cx, cy, w, h, conf, class, keep) rows -- batch_nms(..., box_format=
+    BOX_CXCYWH, det_floats=6); seg, lane [B, map_h, map_w] int32: the engine's TopK index maps; image_sizes[b] = (img_w,
+    img_h) of frame b -> (rows [B, 1 + max_rows*6] fp32: the count, then (x, y, w, h, conf, class), rows past the count zero;
+    per-frame u8 canvases [img_h, img_w]: 2 on a lane, else 1 on the drivable area, else 0 -- or None with labels=False).
+    `canvases_out[b]` may be any u8 cuda tensor [img_h, img_w] with contiguous rows (e.g. a view [:, :img_w] of a pitched
+    buffer); bytes past img_w are not written.  Frame b reads maps b.  Two launches per 64 frames."""
+    lib = L.load()
+    B = len(image_sizes)
+    if dets.dim() != 2 or tuple(dets.shape) != (B, 1 + max_rows * row_floats):
+        raise ValueError(f"dets must be [{B}, {1 + max_rows * row_floats}]")
+    _f32_rows(dets)
+    rows_out = _out_tensor(rows_out, (B, 1 + max_rows * 6), torch.float32, dets.device,
+                           f"rows_out must be contiguous float32 [{B}, {1 + max_rows * 6}]")
+    map_w, map_h = YOLOP_MAP
+    if labels:
+        if seg is None or lane is None or seg.shape != lane.shape or seg.dim() != 3 or seg.shape[0] != B:
+            raise ValueError(f"seg and lane must be int32 [{B}, map_h, map_w]")
+        for t in (seg, lane):
+            if t.dtype != torch.int32 or not t.is_contiguous():
+                raise ValueError("seg and lane must be contiguous int32")
+        map_h, map_w = int(seg.shape[1]), int(seg.shape[2])
+        if canvases_out is None:
+            canvases_out = [torch.zeros((h, w), dtype=torch.uint8, device=dets.device) for w, h in image_sizes]
+        descs, canvases = _frames(image_sizes, [c.unsqueeze(0) for c in canvases_out], 1, dets.device, True)
+        canvases_out = [c.squeeze(0) for c in canvases]
+    else:
+        descs, canvases_out = _frames(image_sizes, None, 1, dets.device, False)
+    q = L.YolopPostParams(net_w, net_h, map_w, map_h, row_floats)
+    L.check(lib.trtx_yolop_postprocess_enqueue(C.byref(q), descs, B, _ptr(dets), max_rows,
+                                               _ptr(seg) if labels else None, _ptr(lane) if labels else None,
+                                               _ptr(rows_out), _stream(stream)), "trtx_yolop_postprocess_enqueue")
+    return rows_out, canvases_out
 
 
 def cls_postprocess(logits: torch.Tensor, k: int, softmax: bool, probs: bool = False, stream=None):
