@@ -478,689 +478,509 @@ class DecodePluginCreator : public nvinfer1::IPluginCreator {
 };
 
 // ================================================================================================
-// Faster R-CNN plugins: IPluginV2Ext with the reference's constructors (rcnn/*Plugin.h), names "RpnDecode",
-// "RpnNms", "PredictorDecode", "BatchedNms", version "1", namespace "".  Implicit batch, fp32 linear only
-// (the *PluginIOExt classes below also take fp16 feature maps / masks / scores and deltas).
+// Faster / Mask R-CNN plugins (rcnn/*Plugin.h): names "RpnDecode", "RpnNms", "PredictorDecode", "BatchedNms", "RoiAlign",
+// "MaskRcnnInference", version "1", namespace "", implicit batch.  Each plugin is one parameter block (RpnDecodeParams, ...):
+// the reference's fields with the reference's types (they fix the blob layout), its constructors, its blob, its output dims,
+// its configurePlugin rule (on the dims of input kInput) and its C call.  RcnnPlugin<P> puts a block behind IPluginV2Ext (the
+// reference's classes: RpnDecodePlugin, ...), RcnnPluginIOExt<P> behind IPluginV2IOExt (RpnDecodePluginIOExt, ...).
 // ================================================================================================
-class RcnnPluginBase : public nvinfer1::IPluginV2Ext {
+namespace detail {
+inline bool float_or_half(nvinfer1::DataType t) { return t == nvinfer1::DataType::kFLOAT || t == nvinfer1::DataType::kHALF; }
+
+// A blob read front to back.  A read that does not fit in what is left fails the reader, and every read after it.
+class BlobReader {
    public:
+    BlobReader(const void* data, size_t length) : d_(static_cast<const char*>(data)), left_(data ? length : 0) {}
+    // the next count * size bytes; nullptr when they do not fit
+    const char* take(size_t count, size_t size) {
+        if (!ok_ || count > left_ / size) {
+            ok_ = false;
+            return nullptr;
+        }
+        const char* p = d_;
+        d_ += count * size;
+        left_ -= count * size;
+        return p;
+    }
+    template <typename T>
+    void get(T& v) {
+        if (const char* p = take(1, sizeof(T))) std::memcpy(&v, p, sizeof(T));
+    }
+    // every read fitted and no byte is left over
+    bool done() const { return ok_ && left_ == 0; }
+
+   private:
+    const char* d_;
+    size_t left_;
+    bool ok_ = true;
+};
+// n floats that BlobReader::take has found in the blob
+inline void assign(std::vector<float>& v, const char* p, size_t n) {
+    v.resize(n);
+    if (n) std::memcpy(v.data(), p, n * sizeof(float));
+}
+
+// Reads an R-CNN blob into p: the reference's blob (element type TRTX_F32) or, where tagged, the reference's blob followed by
+// its element type as one int32 (TRTX_F32 | TRTX_F16).  False for any other blob.
+template <class P>
+bool read_dtype(P& p, const void* data, size_t length, bool tagged, int32_t& dtype) {
+    int32_t t = TRTX_F32;
+    if (!p.read(data, length)) {
+        if (!tagged || length < sizeof(t) || !p.read(data, length - sizeof(t))) return false;
+        std::memcpy(&t, static_cast<const char*>(data) + length - sizeof(t), sizeof(t));
+        if (t != TRTX_F32 && t != TRTX_F16) return false;
+    }
+    dtype = t;
+    return true;
+}
+}  // namespace detail
+
+// rcnn/RpnDecodePlugin.h: scores [A, H, W] and deltas [4A, H, W] -> top_n scores [top_n, 1] and boxes [top_n, 4]
+struct RpnDecodeParams {
+    int top_n = 0;
+    std::vector<float> anchors;
+    float stride = 0.f;
+    size_t height = 0, width = 0, image_height = 0, image_width = 0;
+
+    RpnDecodeParams() = default;
+    RpnDecodeParams(int top_n, const std::vector<float>& anchors, float stride, size_t image_height, size_t image_width)
+        : RpnDecodeParams(top_n, anchors, stride, 0, 0, image_height, image_width) {}
+    RpnDecodeParams(int top_n, const std::vector<float>& anchors, float stride, size_t height, size_t width, size_t image_height,
+                    size_t image_width)
+        : top_n(top_n), anchors(anchors), stride(stride), height(height), width(width), image_height(image_height),
+          image_width(image_width) {}
+
+    static const char* type() { return "RpnDecode"; }
+    static constexpr int kOutputs = 2, kInput = 0;
+    static constexpr bool kHasIOExt = true;
+    size_t blob_size() const { return sizeof(int) + sizeof(size_t) + sizeof(float) * anchors.size() + sizeof(float) + 4 * sizeof(size_t); }
+    void write(char*& d) const {  // RpnDecodePlugin.h:64-75
+        detail::write(d, top_n);
+        detail::write(d, anchors.size());
+        for (float v : anchors) detail::write(d, v);
+        detail::write(d, stride);
+        detail::write(d, height);
+        detail::write(d, width);
+        detail::write(d, image_height);
+        detail::write(d, image_width);
+    }
+    bool read(const void* data, size_t length) {  // RpnDecodePlugin.h:42-58
+        detail::BlobReader r(data, length);
+        size_t n = 0;
+        r.get(top_n);
+        r.get(n);
+        const char* a = r.take(n, sizeof(float));
+        r.get(stride);
+        r.get(height);
+        r.get(width);
+        r.get(image_height);
+        r.get(image_width);
+        if (!r.done()) return false;
+        detail::assign(anchors, a, n);
+        return true;
+    }
+    nvinfer1::Dims dims(int index) const { return nvinfer1::Dims2(top_n, index == 1 ? 4 : 1); }
+    void configure(const nvinfer1::Dims& scores) {  // RpnDecodePlugin.h:148-157: scores dims {A, H, W}
+        height = scores.d[1];
+        width = scores.d[2];
+    }
+    size_t workspace(int dtype, int batch) const {
+        return (size_t)trtx_rpn_decode_typed(dtype, batch, nullptr, nullptr, nullptr, nullptr, (int)height, (int)width, (int)image_height,
+                                             (int)image_width, stride, anchors.data(), (int)anchors.size() / 4, top_n, nullptr, 0, nullptr);
+    }
+    int run(int dtype, int batch, const void* const* in, void* const* out, void* ws, cudaStream_t stream) const {
+        return detail::rcnn_rc(trtx_rpn_decode_typed(dtype, batch, in[0], in[1], static_cast<float*>(out[0]), static_cast<float*>(out[1]),
+                                                     (int)height, (int)width, (int)image_height, (int)image_width, stride, anchors.data(),
+                                                     (int)anchors.size() / 4, top_n, ws, workspace(dtype, batch), stream));
+    }
+    // IPluginV2IOExt: scores and deltas fp32 or fp16, one type; the scores and boxes fp32
+    static bool io_type_ok(int pos, const nvinfer1::PluginTensorDesc* io, int nbInputs) {
+        if (pos < nbInputs) return detail::float_or_half(io[pos].type) && io[pos].type == io[0].type;
+        return io[pos].type == nvinfer1::DataType::kFLOAT;
+    }
+    static nvinfer1::DataType io_output_type(const nvinfer1::DataType*, int) { return nvinfer1::DataType::kFLOAT; }
+};
+
+// rcnn/RpnNmsPlugin.h: scores [pre, 1] and boxes [pre, 4] -> boxes [post, 4]
+struct RpnNmsParams {
+    float nms_thresh = 0.f;
+    int post_nms_topk = 0;
+    size_t pre_nms_topk = 1;
+
+    RpnNmsParams() = default;
+    RpnNmsParams(float nms_thresh, int post_nms_topk, size_t pre_nms_topk = 1)
+        : nms_thresh(nms_thresh), post_nms_topk(post_nms_topk), pre_nms_topk(pre_nms_topk) {}
+
+    static const char* type() { return "RpnNms"; }
+    static constexpr int kOutputs = 1, kInput = 0;
+    static constexpr bool kHasIOExt = false;
+    size_t blob_size() const { return sizeof(float) + sizeof(int) + sizeof(size_t); }
+    void write(char*& d) const {  // RpnNmsPlugin.h:48-52
+        detail::write(d, nms_thresh);
+        detail::write(d, post_nms_topk);
+        detail::write(d, pre_nms_topk);
+    }
+    bool read(const void* data, size_t length) {  // RpnNmsPlugin.h:36-41
+        detail::BlobReader r(data, length);
+        r.get(nms_thresh);
+        r.get(post_nms_topk);
+        r.get(pre_nms_topk);
+        return r.done();
+    }
+    nvinfer1::Dims dims(int) const { return nvinfer1::Dims2(post_nms_topk, 4); }
+    void configure(const nvinfer1::Dims& scores) { pre_nms_topk = scores.d[0]; }
+    size_t workspace(int, int batch) const {  // fp32 only
+        return (size_t)trtx_rpn_nms(batch, nullptr, nullptr, nullptr, (int)pre_nms_topk, post_nms_topk, nms_thresh, nullptr, 0, nullptr);
+    }
+    int run(int dtype, int batch, const void* const* in, void* const* out, void* ws, cudaStream_t stream) const {
+        return detail::rcnn_rc(trtx_rpn_nms(batch, static_cast<const float*>(in[0]), static_cast<const float*>(in[1]),
+                                            static_cast<float*>(out[0]), (int)pre_nms_topk, post_nms_topk, nms_thresh, ws,
+                                            workspace(dtype, batch), stream));
+    }
+};
+
+// rcnn/RoiAlignPlugin.h:27-170: proposals [N, 4] and features [C, H, W] -> bins [N, C, P, P]
+struct RoiAlignParams {
+    int pooler_resolution = 0;
+    float spatial_scale = 0.f;
+    int sampling_ratio = 0, num_proposals = 0, out_channels = 0, feature_h = 0, feature_w = 0;
+
+    RoiAlignParams() = default;
+    RoiAlignParams(int pooler_resolution, float spatial_scale, int sampling_ratio, int num_proposals, int out_channels, int feature_h = 0,
+                   int feature_w = 0)
+        : pooler_resolution(pooler_resolution), spatial_scale(spatial_scale), sampling_ratio(sampling_ratio), num_proposals(num_proposals),
+          out_channels(out_channels), feature_h(feature_h), feature_w(feature_w) {}
+
+    static const char* type() { return "RoiAlign"; }
+    static constexpr int kOutputs = 1, kInput = 1;
+    static constexpr bool kHasIOExt = true;
+    size_t blob_size() const { return 6 * sizeof(int) + sizeof(float); }
+    void write(char*& d) const {  // RoiAlignPlugin.h:53-61
+        detail::write(d, pooler_resolution);
+        detail::write(d, spatial_scale);
+        detail::write(d, sampling_ratio);
+        detail::write(d, num_proposals);
+        detail::write(d, out_channels);
+        detail::write(d, feature_h);
+        detail::write(d, feature_w);
+    }
+    bool read(const void* data, size_t length) {  // RoiAlignPlugin.h:37-46
+        detail::BlobReader r(data, length);
+        r.get(pooler_resolution);
+        r.get(spatial_scale);
+        r.get(sampling_ratio);
+        r.get(num_proposals);
+        r.get(out_channels);
+        r.get(feature_h);
+        r.get(feature_w);
+        return r.done();
+    }
+    nvinfer1::Dims dims(int) const { return nvinfer1::Dims4(num_proposals, out_channels, pooler_resolution, pooler_resolution); }
+    void configure(const nvinfer1::Dims& features) {  // RoiAlignPlugin.h:151-152
+        feature_h = features.d[1];
+        feature_w = features.d[2];
+    }
+    size_t workspace(int, int) const { return 0; }
+    int run(int dtype, int batch, const void* const* in, void* const* out, void*, cudaStream_t stream) const {
+        return trtx_roi_align_typed(dtype, batch, static_cast<const float*>(in[0]), in[1], out[0], pooler_resolution, spatial_scale,
+                                    sampling_ratio, num_proposals, out_channels, feature_h, feature_w, stream);
+    }
+    // IPluginV2IOExt: proposals fp32; features fp32 or fp16; the bins in the features' type
+    static bool io_type_ok(int pos, const nvinfer1::PluginTensorDesc* io, int) {
+        if (pos == 0) return io[0].type == nvinfer1::DataType::kFLOAT;
+        if (pos == 1) return detail::float_or_half(io[1].type);
+        return io[pos].type == io[1].type;
+    }
+    static nvinfer1::DataType io_output_type(const nvinfer1::DataType* in, int nbInputs) {
+        return nbInputs > 1 ? in[1] : nvinfer1::DataType::kFLOAT;
+    }
+};
+
+// rcnn/MaskRcnnInferencePlugin.h:27-140: class indices [D] and masks [D, C, S, S] -> probabilities [D, 1, S, S]
+struct MaskRcnnInferenceParams {
+    int detections_per_im = 0, output_size = 0, num_classes = 1;
+
+    MaskRcnnInferenceParams() = default;
+    MaskRcnnInferenceParams(int detections_per_im, int output_size, int num_classes = 1)
+        : detections_per_im(detections_per_im), output_size(output_size), num_classes(num_classes) {}
+
+    static const char* type() { return "MaskRcnnInference"; }
+    static constexpr int kOutputs = 1, kInput = 1;
+    static constexpr bool kHasIOExt = true;
+    size_t blob_size() const { return 3 * sizeof(int); }
+    void write(char*& d) const {  // MaskRcnnInferencePlugin.h:41-45
+        detail::write(d, detections_per_im);
+        detail::write(d, output_size);
+        detail::write(d, num_classes);
+    }
+    bool read(const void* data, size_t length) {  // MaskRcnnInferencePlugin.h:32-37
+        detail::BlobReader r(data, length);
+        r.get(detections_per_im);
+        r.get(output_size);
+        r.get(num_classes);
+        return r.done();
+    }
+    nvinfer1::Dims dims(int) const { return nvinfer1::Dims4(detections_per_im, 1, output_size, output_size); }
+    void configure(const nvinfer1::Dims& masks) { num_classes = masks.d[1]; }  // MaskRcnnInferencePlugin.h:119
+    size_t workspace(int, int) const { return 0; }
+    int run(int dtype, int batch, const void* const* in, void* const* out, void*, cudaStream_t stream) const {
+        return trtx_mask_rcnn_inference_typed(dtype, batch, static_cast<const float*>(in[0]), in[1], static_cast<float*>(out[0]),
+                                              detections_per_im, output_size, num_classes, stream);
+    }
+    // IPluginV2IOExt: class indices fp32; masks fp32 or fp16; the probabilities fp32 (they feed trtx_rcnn_postprocess*)
+    static bool io_type_ok(int pos, const nvinfer1::PluginTensorDesc* io, int) {
+        if (pos == 1) return detail::float_or_half(io[1].type);
+        return io[pos].type == nvinfer1::DataType::kFLOAT;
+    }
+    static nvinfer1::DataType io_output_type(const nvinfer1::DataType*, int) { return nvinfer1::DataType::kFLOAT; }
+};
+
+// rcnn/PredictorDecodePlugin.h: scores [N, C, 1, 1], deltas [N, 4C, 1, 1] and proposals [N, 4] -> scores [N, 1], boxes [N, 4]
+// and classes [N, 1]
+struct PredictorDecodeParams {
+    unsigned num_boxes = 0, num_classes = 0, image_height = 0, image_width = 0;
+    std::vector<float> bbox_reg_weights;
+
+    PredictorDecodeParams() = default;
+    PredictorDecodeParams(unsigned num_boxes, unsigned image_height, unsigned image_width, const std::vector<float>& bbox_reg_weights)
+        : PredictorDecodeParams(num_boxes, 0, image_height, image_width, bbox_reg_weights) {}
+    PredictorDecodeParams(unsigned num_boxes, unsigned num_classes, unsigned image_height, unsigned image_width,
+                          const std::vector<float>& bbox_reg_weights)
+        : num_boxes(num_boxes), num_classes(num_classes), image_height(image_height), image_width(image_width),
+          bbox_reg_weights(bbox_reg_weights) {}
+
+    static const char* type() { return "PredictorDecode"; }
+    static constexpr int kOutputs = 3, kInput = 0;
+    static constexpr bool kHasIOExt = true;
+    size_t blob_size() const { return 4 * sizeof(unsigned) + sizeof(size_t) + sizeof(float) * bbox_reg_weights.size(); }
+    void write(char*& d) const {  // PredictorDecodePlugin.h:62-70
+        detail::write(d, num_boxes);
+        detail::write(d, num_classes);
+        detail::write(d, image_height);
+        detail::write(d, image_width);
+        detail::write(d, bbox_reg_weights.size());
+        for (float v : bbox_reg_weights) detail::write(d, v);
+    }
+    bool read(const void* data, size_t length) {  // PredictorDecodePlugin.h:40-54
+        detail::BlobReader r(data, length);
+        size_t n = 0;
+        r.get(num_boxes);
+        r.get(num_classes);
+        r.get(image_height);
+        r.get(image_width);
+        r.get(n);
+        const char* w = r.take(n, sizeof(float));
+        if (!r.done()) return false;
+        detail::assign(bbox_reg_weights, w, n);
+        return true;
+    }
+    nvinfer1::Dims dims(int index) const { return nvinfer1::Dims2(num_boxes, index == 1 ? 4 : 1); }
+    void configure(const nvinfer1::Dims& scores) { num_classes = scores.d[1]; }  // scores dims {N, C, 1, 1}
+    size_t workspace(int dtype, int batch) const {
+        return (size_t)trtx_predictor_decode_typed(dtype, batch, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, (int)num_boxes,
+                                                   (int)num_classes, (int)image_height, (int)image_width, bbox_reg_weights.data(), nullptr,
+                                                   0, nullptr);
+    }
+    int run(int dtype, int batch, const void* const* in, void* const* out, void* ws, cudaStream_t stream) const {
+        if (bbox_reg_weights.size() < 4) return TRTX_ERR_INVALID;
+        return detail::rcnn_rc(trtx_predictor_decode_typed(dtype, batch, in[0], in[1], static_cast<const float*>(in[2]),
+                                                           static_cast<float*>(out[0]), static_cast<float*>(out[1]),
+                                                           static_cast<float*>(out[2]), (int)num_boxes, (int)num_classes, (int)image_height,
+                                                           (int)image_width, bbox_reg_weights.data(), ws, workspace(dtype, batch), stream));
+    }
+    // IPluginV2IOExt: scores and deltas fp32 or fp16, one type; the proposals and the scores, boxes and classes fp32
+    static bool io_type_ok(int pos, const nvinfer1::PluginTensorDesc* io, int) {
+        if (pos < 2) return detail::float_or_half(io[pos].type) && io[pos].type == io[0].type;
+        return io[pos].type == nvinfer1::DataType::kFLOAT;
+    }
+    static nvinfer1::DataType io_output_type(const nvinfer1::DataType*, int) { return nvinfer1::DataType::kFLOAT; }
+};
+
+// rcnn/BatchedNmsPlugin.h: scores [count, 1], boxes [count, 4] and classes [count, 1] -> the same for detections_per_im
+struct BatchedNmsParams {
+    int nms_method = 0;
+    float nms_thresh = 0.f;
+    int detections_per_im = 0;
+    size_t count = 1;
+
+    BatchedNmsParams() = default;
+    BatchedNmsParams(int nms_method, float nms_thresh, int detections_per_im, size_t count = 1)
+        : nms_method(nms_method), nms_thresh(nms_thresh), detections_per_im(detections_per_im), count(count) {}
+
+    static const char* type() { return "BatchedNms"; }
+    static constexpr int kOutputs = 3, kInput = 0;
+    static constexpr bool kHasIOExt = false;
+    size_t blob_size() const { return sizeof(int) + sizeof(float) + sizeof(int) + sizeof(size_t); }
+    void write(char*& d) const {  // BatchedNmsPlugin.h:51-56
+        detail::write(d, nms_method);
+        detail::write(d, nms_thresh);
+        detail::write(d, detections_per_im);
+        detail::write(d, count);
+    }
+    bool read(const void* data, size_t length) {  // BatchedNmsPlugin.h:38-44
+        detail::BlobReader r(data, length);
+        r.get(nms_method);
+        r.get(nms_thresh);
+        r.get(detections_per_im);
+        r.get(count);
+        return r.done();
+    }
+    nvinfer1::Dims dims(int index) const { return nvinfer1::Dims2(detections_per_im, index == 1 ? 4 : 1); }
+    void configure(const nvinfer1::Dims& scores) { count = scores.d[0]; }  // BatchedNmsPlugin.h:148-157
+    size_t workspace(int, int batch) const {  // fp32 only
+        return (size_t)trtx_batched_nms(nms_method, batch, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, (int)count,
+                                        detections_per_im, nms_thresh, nullptr, 0, nullptr);
+    }
+    int run(int dtype, int batch, const void* const* in, void* const* out, void* ws, cudaStream_t stream) const {
+        return detail::rcnn_rc(trtx_batched_nms(nms_method, batch, static_cast<const float*>(in[0]), static_cast<const float*>(in[1]),
+                                                static_cast<const float*>(in[2]), static_cast<float*>(out[0]), static_cast<float*>(out[1]),
+                                                static_cast<float*>(out[2]), (int)count, detections_per_im, nms_thresh, ws,
+                                                workspace(dtype, batch), stream));
+    }
+};
+
+// IPluginV2Ext (rcnn/BatchedNmsPlugin.h:30) with the reference's constructors, fp32 linear tensors only and the reference's
+// blob.  A blob is refused (valid() false) unless it is the reference's blob or, for a plugin that has an IPluginV2IOExt twin,
+// that blob followed by a TRTX_F32 tag (what the twin writes in an fp32 engine).
+template <class P>
+class RcnnPlugin : public nvinfer1::IPluginV2Ext, private P {  // P is a base for its constructors (using P::P)
+   public:
+    using P::P;
+    using P::type;  // the plugin name, for RcnnCreator
+    RcnnPlugin(const void* data, size_t length) {
+        int32_t dtype = -1;
+        valid_ = detail::read_dtype<P>(*this, data, length, P::kHasIOExt, dtype) && dtype == TRTX_F32;
+    }
+    bool valid() const { return valid_; }
+    const char* getPluginType() const TRTX_NOEXCEPT override { return P::type(); }
+    const char* getPluginVersion() const TRTX_NOEXCEPT override { return "1"; }
+    const char* getPluginNamespace() const TRTX_NOEXCEPT override { return ""; }
+    void setPluginNamespace(const char*) TRTX_NOEXCEPT override {}
+    int getNbOutputs() const TRTX_NOEXCEPT override { return P::kOutputs; }
+    nvinfer1::Dims getOutputDimensions(int index, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override { return P::dims(index); }
     bool supportsFormat(nvinfer1::DataType t, nvinfer1::PluginFormat f) const TRTX_NOEXCEPT override {
         return t == nvinfer1::DataType::kFLOAT && f == nvinfer1::PluginFormat::kLINEAR;  // BatchedNmsPlugin.h:98-100
     }
-    int initialize() TRTX_NOEXCEPT override { return 0; }
-    void terminate() TRTX_NOEXCEPT override {}
-    void destroy() TRTX_NOEXCEPT override { delete this; }
-    const char* getPluginVersion() const TRTX_NOEXCEPT override { return "1"; }
-    const char* getPluginNamespace() const TRTX_NOEXCEPT override { return ""; }
-    void setPluginNamespace(const char*) TRTX_NOEXCEPT override {}
     nvinfer1::DataType getOutputDataType(int, const nvinfer1::DataType*, int) const TRTX_NOEXCEPT override { return nvinfer1::DataType::kFLOAT; }
     bool isOutputBroadcastAcrossBatch(int, const bool*, int) const TRTX_NOEXCEPT override { return false; }
     bool canBroadcastInputAcrossBatch(int) const TRTX_NOEXCEPT override { return false; }
-};
-
-class RpnDecodePlugin : public RcnnPluginBase {
-   public:
-    RpnDecodePlugin(int top_n, const std::vector<float>& anchors, float stride, size_t image_height, size_t image_width)
-        : top_n_(top_n), anchors_(anchors), stride_(stride), height_(0), width_(0), image_height_(image_height), image_width_(image_width) {}
-    RpnDecodePlugin(int top_n, const std::vector<float>& anchors, float stride, size_t height, size_t width, size_t image_height, size_t image_width)
-        : top_n_(top_n), anchors_(anchors), stride_(stride), height_(height), width_(width), image_height_(image_height), image_width_(image_width) {}
-    RpnDecodePlugin(const void* data, size_t) {  // RpnDecodePlugin.h:42-58
-        const char* d = static_cast<const char*>(data);
-        detail::read(d, top_n_);
-        size_t n;
-        detail::read(d, n);
-        anchors_.resize(n);
-        for (size_t i = 0; i < n; ++i) detail::read(d, anchors_[i]);
-        detail::read(d, stride_);
-        detail::read(d, height_);
-        detail::read(d, width_);
-        detail::read(d, image_height_);
-        detail::read(d, image_width_);
+    void configurePlugin(const nvinfer1::Dims* inputDims, int, const nvinfer1::Dims*, int, const nvinfer1::DataType*, const nvinfer1::DataType*,
+                         const bool*, const bool*, nvinfer1::PluginFormat, int) TRTX_NOEXCEPT override {
+        P::configure(inputDims[P::kInput]);
     }
-    const char* getPluginType() const TRTX_NOEXCEPT override { return "RpnDecode"; }
-    int getNbOutputs() const TRTX_NOEXCEPT override { return 2; }
-    nvinfer1::Dims getOutputDimensions(int index, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override { return nvinfer1::Dims2(top_n_, index == 1 ? 4 : 1); }
-    size_t getWorkspaceSize(int maxBatchSize) const TRTX_NOEXCEPT override {
-        return (size_t)trtx_rpn_decode(maxBatchSize, nullptr, nullptr, nullptr, nullptr, (int)height_, (int)width_, (int)image_height_,
-                                       (int)image_width_, stride_, anchors_.data(), (int)anchors_.size() / 4, top_n_, nullptr, 0, nullptr);
-    }
+    int initialize() TRTX_NOEXCEPT override { return 0; }
+    void terminate() TRTX_NOEXCEPT override {}
+    size_t getWorkspaceSize(int maxBatchSize) const TRTX_NOEXCEPT override { return P::workspace(TRTX_F32, maxBatchSize); }
     int enqueue(int batchSize, const void* const* inputs, void* TRTX_CONST_ENQUEUE* outputs, void* workspace, cudaStream_t stream) TRTX_NOEXCEPT override {
-        const int64_t rc = trtx_rpn_decode(batchSize, static_cast<const float*>(inputs[0]), static_cast<const float*>(inputs[1]),
-                                           static_cast<float*>(outputs[0]), static_cast<float*>(outputs[1]), (int)height_, (int)width_,
-                                           (int)image_height_, (int)image_width_, stride_, anchors_.data(), (int)anchors_.size() / 4,
-                                           top_n_, workspace, getWorkspaceSize(batchSize), stream);
-        return detail::rcnn_rc(rc);
+        return valid_ ? P::run(TRTX_F32, batchSize, inputs, outputs, workspace, stream) : TRTX_ERR_INVALID;
     }
-    size_t getSerializationSize() const TRTX_NOEXCEPT override {
-        return sizeof(top_n_) + sizeof(size_t) + sizeof(float) * anchors_.size() + sizeof(stride_) + 4 * sizeof(size_t);
-    }
+    size_t getSerializationSize() const TRTX_NOEXCEPT override { return P::blob_size(); }
     void serialize(void* buffer) const TRTX_NOEXCEPT override {
         char* d = static_cast<char*>(buffer);
-        detail::write(d, top_n_);
-        detail::write(d, anchors_.size());
-        for (float v : anchors_) detail::write(d, v);
-        detail::write(d, stride_);
-        detail::write(d, height_);
-        detail::write(d, width_);
-        detail::write(d, image_height_);
-        detail::write(d, image_width_);
+        P::write(d);
     }
-    void configurePlugin(const nvinfer1::Dims* inputDims, int, const nvinfer1::Dims*, int, const nvinfer1::DataType*, const nvinfer1::DataType*,
-                         const bool*, const bool*, nvinfer1::PluginFormat, int) TRTX_NOEXCEPT override {
-        height_ = inputDims[0].d[1];  // RpnDecodePlugin.h:148-157: scores dims {A, H, W}
-        width_ = inputDims[0].d[2];
-    }
-    nvinfer1::IPluginV2Ext* clone() const TRTX_NOEXCEPT override {
-        return new RpnDecodePlugin(top_n_, anchors_, stride_, height_, width_, image_height_, image_width_);
-    }
+    nvinfer1::IPluginV2Ext* clone() const TRTX_NOEXCEPT override { return new RcnnPlugin(*this); }
+    void destroy() TRTX_NOEXCEPT override { delete this; }
 
    private:
-    int top_n_;
-    std::vector<float> anchors_;
-    float stride_;
-    size_t height_, width_, image_height_, image_width_;
+    bool valid_ = true;
 };
-
-class RpnNmsPlugin : public RcnnPluginBase {
-   public:
-    RpnNmsPlugin(float nms_thresh, int post_nms_topk, size_t pre_nms_topk = 1) : thresh_(nms_thresh), post_(post_nms_topk), pre_(pre_nms_topk) {}
-    RpnNmsPlugin(const void* data, size_t) {  // RpnNmsPlugin.h:36-41
-        const char* d = static_cast<const char*>(data);
-        detail::read(d, thresh_);
-        detail::read(d, post_);
-        detail::read(d, pre_);
-    }
-    const char* getPluginType() const TRTX_NOEXCEPT override { return "RpnNms"; }
-    int getNbOutputs() const TRTX_NOEXCEPT override { return 1; }
-    nvinfer1::Dims getOutputDimensions(int, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override { return nvinfer1::Dims2(post_, 4); }
-    size_t getWorkspaceSize(int maxBatchSize) const TRTX_NOEXCEPT override {
-        return (size_t)trtx_rpn_nms(maxBatchSize, nullptr, nullptr, nullptr, (int)pre_, post_, thresh_, nullptr, 0, nullptr);
-    }
-    int enqueue(int batchSize, const void* const* inputs, void* TRTX_CONST_ENQUEUE* outputs, void* workspace, cudaStream_t stream) TRTX_NOEXCEPT override {
-        const int64_t rc = trtx_rpn_nms(batchSize, static_cast<const float*>(inputs[0]), static_cast<const float*>(inputs[1]),
-                                        static_cast<float*>(outputs[0]), (int)pre_, post_, thresh_, workspace, getWorkspaceSize(batchSize), stream);
-        return detail::rcnn_rc(rc);
-    }
-    size_t getSerializationSize() const TRTX_NOEXCEPT override { return sizeof(thresh_) + sizeof(post_) + sizeof(pre_); }
-    void serialize(void* buffer) const TRTX_NOEXCEPT override {
-        char* d = static_cast<char*>(buffer);
-        detail::write(d, thresh_);
-        detail::write(d, post_);
-        detail::write(d, pre_);
-    }
-    void configurePlugin(const nvinfer1::Dims* inputDims, int, const nvinfer1::Dims*, int, const nvinfer1::DataType*, const nvinfer1::DataType*,
-                         const bool*, const bool*, nvinfer1::PluginFormat, int) TRTX_NOEXCEPT override {
-        pre_ = inputDims[0].d[0];
-    }
-    nvinfer1::IPluginV2Ext* clone() const TRTX_NOEXCEPT override { return new RpnNmsPlugin(thresh_, post_, pre_); }
-
-   private:
-    float thresh_;
-    int post_;
-    size_t pre_;
-};
-
-// rcnn/RoiAlignPlugin.h:27-170
-class RoiAlignPlugin : public RcnnPluginBase {
-   public:
-    RoiAlignPlugin(int pooler_resolution, float spatial_scale, int sampling_ratio, int num_proposals, int out_channels,
-                   int feature_h = 0, int feature_w = 0)
-        : pooler_(pooler_resolution), scale_(spatial_scale), sampling_(sampling_ratio), proposals_(num_proposals),
-          channels_(out_channels), fh_(feature_h), fw_(feature_w) {}
-    RoiAlignPlugin(const void* data, size_t) {  // RoiAlignPlugin.h:37-46
-        const char* d = static_cast<const char*>(data);
-        detail::read(d, pooler_);
-        detail::read(d, scale_);
-        detail::read(d, sampling_);
-        detail::read(d, proposals_);
-        detail::read(d, channels_);
-        detail::read(d, fh_);
-        detail::read(d, fw_);
-    }
-    const char* getPluginType() const TRTX_NOEXCEPT override { return "RoiAlign"; }
-    int getNbOutputs() const TRTX_NOEXCEPT override { return 1; }
-    nvinfer1::Dims getOutputDimensions(int, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override {
-        return nvinfer1::Dims4(proposals_, channels_, pooler_, pooler_);
-    }
-    size_t getWorkspaceSize(int) const TRTX_NOEXCEPT override { return 0; }
-    int enqueue(int batchSize, const void* const* inputs, void* TRTX_CONST_ENQUEUE* outputs, void*, cudaStream_t stream) TRTX_NOEXCEPT override {
-        return trtx_roi_align(batchSize, static_cast<const float*>(inputs[0]), static_cast<const float*>(inputs[1]),
-                              static_cast<float*>(outputs[0]), pooler_, scale_, sampling_, proposals_, channels_, fh_, fw_, stream);
-    }
-    size_t getSerializationSize() const TRTX_NOEXCEPT override { return 6 * sizeof(int) + sizeof(float); }
-    void serialize(void* buffer) const TRTX_NOEXCEPT override {
-        char* d = static_cast<char*>(buffer);
-        detail::write(d, pooler_);
-        detail::write(d, scale_);
-        detail::write(d, sampling_);
-        detail::write(d, proposals_);
-        detail::write(d, channels_);
-        detail::write(d, fh_);
-        detail::write(d, fw_);
-    }
-    void configurePlugin(const nvinfer1::Dims* inputDims, int, const nvinfer1::Dims*, int, const nvinfer1::DataType*, const nvinfer1::DataType*,
-                         const bool*, const bool*, nvinfer1::PluginFormat, int) TRTX_NOEXCEPT override {
-        fh_ = inputDims[1].d[1];  // RoiAlignPlugin.h:151-152
-        fw_ = inputDims[1].d[2];
-    }
-    nvinfer1::IPluginV2Ext* clone() const TRTX_NOEXCEPT override {
-        return new RoiAlignPlugin(pooler_, scale_, sampling_, proposals_, channels_, fh_, fw_);
-    }
-
-   private:
-    int pooler_;
-    float scale_;
-    int sampling_, proposals_, channels_, fh_, fw_;
-};
-
-// rcnn/MaskRcnnInferencePlugin.h:27-140
-class MaskRcnnInferencePlugin : public RcnnPluginBase {
-   public:
-    MaskRcnnInferencePlugin(int detections_per_im, int output_size, int num_classes = 1)
-        : dets_(detections_per_im), size_(output_size), classes_(num_classes) {}
-    MaskRcnnInferencePlugin(const void* data, size_t) {  // MaskRcnnInferencePlugin.h:32-37
-        const char* d = static_cast<const char*>(data);
-        detail::read(d, dets_);
-        detail::read(d, size_);
-        detail::read(d, classes_);
-    }
-    const char* getPluginType() const TRTX_NOEXCEPT override { return "MaskRcnnInference"; }
-    int getNbOutputs() const TRTX_NOEXCEPT override { return 1; }
-    nvinfer1::Dims getOutputDimensions(int, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override { return nvinfer1::Dims4(dets_, 1, size_, size_); }
-    size_t getWorkspaceSize(int) const TRTX_NOEXCEPT override { return 0; }
-    int enqueue(int batchSize, const void* const* inputs, void* TRTX_CONST_ENQUEUE* outputs, void*, cudaStream_t stream) TRTX_NOEXCEPT override {
-        return trtx_mask_rcnn_inference(batchSize, static_cast<const float*>(inputs[0]), static_cast<const float*>(inputs[1]),
-                                        static_cast<float*>(outputs[0]), dets_, size_, classes_, stream);
-    }
-    size_t getSerializationSize() const TRTX_NOEXCEPT override { return 3 * sizeof(int); }
-    void serialize(void* buffer) const TRTX_NOEXCEPT override {
-        char* d = static_cast<char*>(buffer);
-        detail::write(d, dets_);
-        detail::write(d, size_);
-        detail::write(d, classes_);
-    }
-    void configurePlugin(const nvinfer1::Dims* inputDims, int, const nvinfer1::Dims*, int, const nvinfer1::DataType*, const nvinfer1::DataType*,
-                         const bool*, const bool*, nvinfer1::PluginFormat, int) TRTX_NOEXCEPT override {
-        classes_ = inputDims[1].d[1];  // MaskRcnnInferencePlugin.h:119
-    }
-    nvinfer1::IPluginV2Ext* clone() const TRTX_NOEXCEPT override { return new MaskRcnnInferencePlugin(dets_, size_, classes_); }
-
-   private:
-    int dets_, size_, classes_;
-};
-
-class PredictorDecodePlugin : public RcnnPluginBase {
-   public:
-    PredictorDecodePlugin(unsigned num_boxes, unsigned image_height, unsigned image_width, const std::vector<float>& w)
-        : num_boxes_(num_boxes), num_classes_(0), image_height_(image_height), image_width_(image_width), w_(w) {}
-    PredictorDecodePlugin(unsigned num_boxes, unsigned num_classes, unsigned image_height, unsigned image_width, const std::vector<float>& w)
-        : num_boxes_(num_boxes), num_classes_(num_classes), image_height_(image_height), image_width_(image_width), w_(w) {}
-    PredictorDecodePlugin(const void* data, size_t) {  // PredictorDecodePlugin.h:40-54
-        const char* d = static_cast<const char*>(data);
-        detail::read(d, num_boxes_);
-        detail::read(d, num_classes_);
-        detail::read(d, image_height_);
-        detail::read(d, image_width_);
-        size_t n;
-        detail::read(d, n);
-        w_.resize(n);
-        for (size_t i = 0; i < n; ++i) detail::read(d, w_[i]);
-    }
-    const char* getPluginType() const TRTX_NOEXCEPT override { return "PredictorDecode"; }
-    int getNbOutputs() const TRTX_NOEXCEPT override { return 3; }
-    nvinfer1::Dims getOutputDimensions(int index, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override { return nvinfer1::Dims2(num_boxes_, index == 1 ? 4 : 1); }
-    size_t getWorkspaceSize(int maxBatchSize) const TRTX_NOEXCEPT override {
-        return (size_t)trtx_predictor_decode(maxBatchSize, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, (int)num_boxes_, (int)num_classes_,
-                                             (int)image_height_, (int)image_width_, w_.data(), nullptr, 0, nullptr);
-    }
-    int enqueue(int batchSize, const void* const* inputs, void* TRTX_CONST_ENQUEUE* outputs, void* workspace, cudaStream_t stream) TRTX_NOEXCEPT override {
-        if (w_.size() < 4) return TRTX_ERR_INVALID;
-        const int64_t rc = trtx_predictor_decode(batchSize, static_cast<const float*>(inputs[0]), static_cast<const float*>(inputs[1]),
-                                                 static_cast<const float*>(inputs[2]), static_cast<float*>(outputs[0]), static_cast<float*>(outputs[1]),
-                                                 static_cast<float*>(outputs[2]), (int)num_boxes_, (int)num_classes_, (int)image_height_,
-                                                 (int)image_width_, w_.data(), workspace, getWorkspaceSize(batchSize), stream);
-        return detail::rcnn_rc(rc);
-    }
-    size_t getSerializationSize() const TRTX_NOEXCEPT override { return 4 * sizeof(unsigned) + sizeof(size_t) + sizeof(float) * w_.size(); }
-    void serialize(void* buffer) const TRTX_NOEXCEPT override {
-        char* d = static_cast<char*>(buffer);
-        detail::write(d, num_boxes_);
-        detail::write(d, num_classes_);
-        detail::write(d, image_height_);
-        detail::write(d, image_width_);
-        detail::write(d, w_.size());
-        for (float v : w_) detail::write(d, v);
-    }
-    void configurePlugin(const nvinfer1::Dims* inputDims, int, const nvinfer1::Dims*, int, const nvinfer1::DataType*, const nvinfer1::DataType*,
-                         const bool*, const bool*, nvinfer1::PluginFormat, int) TRTX_NOEXCEPT override {
-        num_classes_ = inputDims[0].d[1];  // scores dims {N, C, 1, 1}
-    }
-    nvinfer1::IPluginV2Ext* clone() const TRTX_NOEXCEPT override {
-        return new PredictorDecodePlugin(num_boxes_, num_classes_, image_height_, image_width_, w_);
-    }
-
-   private:
-    unsigned num_boxes_, num_classes_, image_height_, image_width_;
-    std::vector<float> w_;
-};
-
-class BatchedNmsPlugin : public RcnnPluginBase {
-   public:
-    BatchedNmsPlugin(int nms_method, float nms_thresh, int detections_per_im, size_t count = 1)
-        : method_(nms_method), thresh_(nms_thresh), dets_(detections_per_im), count_(count) {}
-    BatchedNmsPlugin(const void* data, size_t) {  // BatchedNmsPlugin.h:38-44
-        const char* d = static_cast<const char*>(data);
-        detail::read(d, method_);
-        detail::read(d, thresh_);
-        detail::read(d, dets_);
-        detail::read(d, count_);
-    }
-    const char* getPluginType() const TRTX_NOEXCEPT override { return "BatchedNms"; }
-    int getNbOutputs() const TRTX_NOEXCEPT override { return 3; }
-    nvinfer1::Dims getOutputDimensions(int index, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override { return nvinfer1::Dims2(dets_, index == 1 ? 4 : 1); }
-    size_t getWorkspaceSize(int maxBatchSize) const TRTX_NOEXCEPT override {
-        return (size_t)trtx_batched_nms(method_, maxBatchSize, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, (int)count_, dets_, thresh_, nullptr, 0, nullptr);
-    }
-    int enqueue(int batchSize, const void* const* inputs, void* TRTX_CONST_ENQUEUE* outputs, void* workspace, cudaStream_t stream) TRTX_NOEXCEPT override {
-        const int64_t rc = trtx_batched_nms(method_, batchSize, static_cast<const float*>(inputs[0]), static_cast<const float*>(inputs[1]),
-                                            static_cast<const float*>(inputs[2]), static_cast<float*>(outputs[0]), static_cast<float*>(outputs[1]),
-                                            static_cast<float*>(outputs[2]), (int)count_, dets_, thresh_, workspace, getWorkspaceSize(batchSize), stream);
-        return detail::rcnn_rc(rc);
-    }
-    size_t getSerializationSize() const TRTX_NOEXCEPT override { return sizeof(method_) + sizeof(thresh_) + sizeof(dets_) + sizeof(count_); }
-    void serialize(void* buffer) const TRTX_NOEXCEPT override {
-        char* d = static_cast<char*>(buffer);
-        detail::write(d, method_);
-        detail::write(d, thresh_);
-        detail::write(d, dets_);
-        detail::write(d, count_);
-    }
-    void configurePlugin(const nvinfer1::Dims* inputDims, int, const nvinfer1::Dims*, int, const nvinfer1::DataType*, const nvinfer1::DataType*,
-                         const bool*, const bool*, nvinfer1::PluginFormat, int) TRTX_NOEXCEPT override {
-        count_ = inputDims[0].d[0];  // BatchedNmsPlugin.h:148-157
-    }
-    nvinfer1::IPluginV2Ext* clone() const TRTX_NOEXCEPT override { return new BatchedNmsPlugin(method_, thresh_, dets_, count_); }
-
-   private:
-    int method_;
-    float thresh_;
-    int dets_;
-    size_t count_;
-};
-
-template <typename P>
-class RcnnCreator : public nvinfer1::IPluginCreator {
-   public:
-    explicit RcnnCreator(const char* name) : name_(name) {}
-    const char* getPluginName() const TRTX_NOEXCEPT override { return name_; }
-    const char* getPluginVersion() const TRTX_NOEXCEPT override { return "1"; }
-    const char* getPluginNamespace() const TRTX_NOEXCEPT override { return ""; }
-    void setPluginNamespace(const char*) TRTX_NOEXCEPT override {}
-    const nvinfer1::PluginFieldCollection* getFieldNames() TRTX_NOEXCEPT override { return nullptr; }
-    nvinfer1::IPluginV2* createPlugin(const char*, const nvinfer1::PluginFieldCollection*) TRTX_NOEXCEPT override { return nullptr; }  // as the reference
-    nvinfer1::IPluginV2* deserializePlugin(const char*, const void* data, size_t len) TRTX_NOEXCEPT override { return new P(data, len); }
-
-   private:
-    const char* name_;
-};
-struct RpnDecodePluginCreator : RcnnCreator<RpnDecodePlugin> { RpnDecodePluginCreator() : RcnnCreator("RpnDecode") {} };
-struct RpnNmsPluginCreator : RcnnCreator<RpnNmsPlugin> { RpnNmsPluginCreator() : RcnnCreator("RpnNms") {} };
-struct PredictorDecodePluginCreator : RcnnCreator<PredictorDecodePlugin> { PredictorDecodePluginCreator() : RcnnCreator("PredictorDecode") {} };
-struct BatchedNmsPluginCreator : RcnnCreator<BatchedNmsPlugin> { BatchedNmsPluginCreator() : RcnnCreator("BatchedNms") {} };
-struct RoiAlignPluginCreator : RcnnCreator<RoiAlignPlugin> { RoiAlignPluginCreator() : RcnnCreator("RoiAlign") {} };
-struct MaskRcnnInferencePluginCreator : RcnnCreator<MaskRcnnInferencePlugin> { MaskRcnnInferencePluginCreator() : RcnnCreator("MaskRcnnInference") {} };
 
 // ------------------------------------------------------------------------------------------------
 // RoiAlign, MaskRcnnInference, RpnDecode and PredictorDecode for an FP16 engine.  Each needs fp32 tensors next to half
 // ones (proposals, class indices, fp32 outputs), which IPluginV2Ext::supportsFormat (one type for every tensor) cannot say;
 // IPluginV2IOExt::supportsFormatCombination can.  Same plugin names, version, constructor arguments and namespace as the
-// IPluginV2Ext classes above, which stay as they are.  The element type TensorRT chose arrives in configurePlugin, is
-// carried through clone() and is appended to the serialized blob as one int32 (TRTX_F32 | TRTX_F16); a blob of the
-// reference's length deserializes as fp32, a blob of any other length is refused.
+// IPluginV2Ext classes.  The element type TensorRT chose for input kInput arrives in configurePlugin, is carried through
+// clone() and is appended to the serialized blob as one int32 (TRTX_F32 | TRTX_F16); a blob of the reference's length
+// deserializes as fp32, a blob of any other length or with another tag is refused.
 // Exercised against tests/mock_trt only: how a real TensorRT builder drives these four classes is NOT verified.
 // ------------------------------------------------------------------------------------------------
-class RcnnIOExtBase : public nvinfer1::IPluginV2IOExt {
+template <class P>
+class RcnnPluginIOExt : public nvinfer1::IPluginV2IOExt, private P {  // P is a base for its constructors (using P::P)
    public:
-    int initialize() TRTX_NOEXCEPT override { return 0; }
-    void terminate() TRTX_NOEXCEPT override {}
-    void destroy() TRTX_NOEXCEPT override { delete this; }
-    size_t getWorkspaceSize(int) const TRTX_NOEXCEPT override { return 0; }
-    int getNbOutputs() const TRTX_NOEXCEPT override { return 1; }
+    using P::P;
+    using P::type;  // the plugin name, for RcnnCreator
+    RcnnPluginIOExt(const void* data, size_t length) { valid_ = detail::read_dtype<P>(*this, data, length, true, dtype_); }
+    bool valid() const { return valid_; }
+    int dtype() const { return dtype_; }  // of input kInput: the feature map / the masks / the scores and deltas
+    const char* getPluginType() const TRTX_NOEXCEPT override { return P::type(); }
     const char* getPluginVersion() const TRTX_NOEXCEPT override { return "1"; }
     const char* getPluginNamespace() const TRTX_NOEXCEPT override { return ""; }
     void setPluginNamespace(const char*) TRTX_NOEXCEPT override {}
-    bool isOutputBroadcastAcrossBatch(int, const bool*, int) const TRTX_NOEXCEPT override { return false; }
-    bool canBroadcastInputAcrossBatch(int) const TRTX_NOEXCEPT override { return false; }
-    void attachToContext(cudnnContext*, cublasContext*, nvinfer1::IGpuAllocator*) TRTX_NOEXCEPT override {}
-    void detachFromContext() TRTX_NOEXCEPT override {}
-    int dtype() const { return dtype_; }
-
-   protected:
-    static bool float_or_half(nvinfer1::DataType t) { return t == nvinfer1::DataType::kFLOAT || t == nvinfer1::DataType::kHALF; }
-    // the trailing int32 of a blob that is 4 bytes longer than the reference's; false: an unknown type
-    bool read_dtype(const char* d, size_t length, size_t reference_length) {
-        if (length == reference_length) return true;
-        int32_t v;
-        detail::read(d, v);
-        if (v != TRTX_F32 && v != TRTX_F16) return false;
-        dtype_ = v;
-        return true;
-    }
-    int32_t dtype_ = TRTX_F32;  // of the half-capable inputs: the feature map / the masks / the scores and deltas
-};
-
-class RoiAlignPluginIOExt : public RcnnIOExtBase {
-   public:
-    RoiAlignPluginIOExt(int pooler_resolution, float spatial_scale, int sampling_ratio, int num_proposals, int out_channels,
-                        int feature_h = 0, int feature_w = 0)
-        : pooler_(pooler_resolution), scale_(spatial_scale), sampling_(sampling_ratio), proposals_(num_proposals),
-          channels_(out_channels), fh_(feature_h), fw_(feature_w) {}
-    RoiAlignPluginIOExt(const void* data, size_t length) {  // RoiAlignPlugin.h:37-46 (+ the element type)
-        if (length != kReferenceBlob && length != kReferenceBlob + sizeof(int32_t)) {
-            valid_ = false;
-            return;
-        }
-        const char* d = static_cast<const char*>(data);
-        detail::read(d, pooler_);
-        detail::read(d, scale_);
-        detail::read(d, sampling_);
-        detail::read(d, proposals_);
-        detail::read(d, channels_);
-        detail::read(d, fh_);
-        detail::read(d, fw_);
-        valid_ = read_dtype(d, length, kReferenceBlob);
-    }
-    bool valid() const { return valid_; }  // false: the blob had neither the reference's length nor that + 4
-    const char* getPluginType() const TRTX_NOEXCEPT override { return "RoiAlign"; }
-    nvinfer1::Dims getOutputDimensions(int, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override {
-        return nvinfer1::Dims4(proposals_, channels_, pooler_, pooler_);
-    }
-    // proposals fp32; features fp32 or fp16; the bins in the features' type
-    bool supportsFormatCombination(int pos, const nvinfer1::PluginTensorDesc* io, int, int) const TRTX_NOEXCEPT override {
-        if (io[pos].format != nvinfer1::TensorFormat::kLINEAR) return false;
-        if (pos == 0) return io[0].type == nvinfer1::DataType::kFLOAT;
-        if (pos == 1) return float_or_half(io[1].type);
-        return io[pos].type == io[1].type;
+    int getNbOutputs() const TRTX_NOEXCEPT override { return P::kOutputs; }
+    nvinfer1::Dims getOutputDimensions(int index, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override { return P::dims(index); }
+    bool supportsFormatCombination(int pos, const nvinfer1::PluginTensorDesc* io, int nbInputs, int) const TRTX_NOEXCEPT override {
+        return io[pos].format == nvinfer1::TensorFormat::kLINEAR && P::io_type_ok(pos, io, nbInputs);
     }
     nvinfer1::DataType getOutputDataType(int, const nvinfer1::DataType* inputTypes, int nbInputs) const TRTX_NOEXCEPT override {
-        return nbInputs > 1 ? inputTypes[1] : nvinfer1::DataType::kFLOAT;
+        return P::io_output_type(inputTypes, nbInputs);
     }
+    bool isOutputBroadcastAcrossBatch(int, const bool*, int) const TRTX_NOEXCEPT override { return false; }
+    bool canBroadcastInputAcrossBatch(int) const TRTX_NOEXCEPT override { return false; }
     void configurePlugin(const nvinfer1::PluginTensorDesc* in, int, const nvinfer1::PluginTensorDesc*, int) TRTX_NOEXCEPT override {
-        fh_ = in[1].dims.d[1];  // RoiAlignPlugin.h:151-152
-        fw_ = in[1].dims.d[2];
-        dtype_ = in[1].type == nvinfer1::DataType::kHALF ? TRTX_F16 : TRTX_F32;
+        P::configure(in[P::kInput].dims);
+        dtype_ = in[P::kInput].type == nvinfer1::DataType::kHALF ? TRTX_F16 : TRTX_F32;
     }
-    int enqueue(int batchSize, const void* const* inputs, void* TRTX_CONST_ENQUEUE* outputs, void*, cudaStream_t stream) TRTX_NOEXCEPT override {
-        return trtx_roi_align_typed(dtype_, batchSize, static_cast<const float*>(inputs[0]), inputs[1], outputs[0], pooler_, scale_,
-                                    sampling_, proposals_, channels_, fh_, fw_, stream);
-    }
-    size_t getSerializationSize() const TRTX_NOEXCEPT override { return kReferenceBlob + sizeof(int32_t); }
-    void serialize(void* buffer) const TRTX_NOEXCEPT override {
-        char* d = static_cast<char*>(buffer);
-        detail::write(d, pooler_);
-        detail::write(d, scale_);
-        detail::write(d, sampling_);
-        detail::write(d, proposals_);
-        detail::write(d, channels_);
-        detail::write(d, fh_);
-        detail::write(d, fw_);
-        detail::write(d, dtype_);
-    }
-    nvinfer1::IPluginV2IOExt* clone() const TRTX_NOEXCEPT override {
-        auto* c = new RoiAlignPluginIOExt(pooler_, scale_, sampling_, proposals_, channels_, fh_, fw_);
-        c->dtype_ = dtype_;
-        return c;
-    }
-
-   private:
-    static constexpr size_t kReferenceBlob = 6 * sizeof(int) + sizeof(float);
-    int pooler_ = 0;
-    float scale_ = 0.f;
-    int sampling_ = 0, proposals_ = 0, channels_ = 0, fh_ = 0, fw_ = 0;
-    bool valid_ = true;
-};
-
-class MaskRcnnInferencePluginIOExt : public RcnnIOExtBase {
-   public:
-    MaskRcnnInferencePluginIOExt(int detections_per_im, int output_size, int num_classes = 1)
-        : dets_(detections_per_im), size_(output_size), classes_(num_classes) {}
-    MaskRcnnInferencePluginIOExt(const void* data, size_t length) {  // MaskRcnnInferencePlugin.h:32-37 (+ the element type)
-        if (length != kReferenceBlob && length != kReferenceBlob + sizeof(int32_t)) {
-            valid_ = false;
-            return;
-        }
-        const char* d = static_cast<const char*>(data);
-        detail::read(d, dets_);
-        detail::read(d, size_);
-        detail::read(d, classes_);
-        valid_ = read_dtype(d, length, kReferenceBlob);
-    }
-    bool valid() const { return valid_; }
-    const char* getPluginType() const TRTX_NOEXCEPT override { return "MaskRcnnInference"; }
-    nvinfer1::Dims getOutputDimensions(int, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override { return nvinfer1::Dims4(dets_, 1, size_, size_); }
-    // class indices fp32; masks fp32 or fp16; the probabilities fp32 (they feed trtx_rcnn_postprocess*)
-    bool supportsFormatCombination(int pos, const nvinfer1::PluginTensorDesc* io, int, int) const TRTX_NOEXCEPT override {
-        if (io[pos].format != nvinfer1::TensorFormat::kLINEAR) return false;
-        if (pos == 1) return float_or_half(io[1].type);
-        return io[pos].type == nvinfer1::DataType::kFLOAT;
-    }
-    nvinfer1::DataType getOutputDataType(int, const nvinfer1::DataType*, int) const TRTX_NOEXCEPT override { return nvinfer1::DataType::kFLOAT; }
-    void configurePlugin(const nvinfer1::PluginTensorDesc* in, int, const nvinfer1::PluginTensorDesc*, int) TRTX_NOEXCEPT override {
-        classes_ = in[1].dims.d[1];  // MaskRcnnInferencePlugin.h:119
-        dtype_ = in[1].type == nvinfer1::DataType::kHALF ? TRTX_F16 : TRTX_F32;
-    }
-    int enqueue(int batchSize, const void* const* inputs, void* TRTX_CONST_ENQUEUE* outputs, void*, cudaStream_t stream) TRTX_NOEXCEPT override {
-        return trtx_mask_rcnn_inference_typed(dtype_, batchSize, static_cast<const float*>(inputs[0]), inputs[1],
-                                              static_cast<float*>(outputs[0]), dets_, size_, classes_, stream);
-    }
-    size_t getSerializationSize() const TRTX_NOEXCEPT override { return kReferenceBlob + sizeof(int32_t); }
-    void serialize(void* buffer) const TRTX_NOEXCEPT override {
-        char* d = static_cast<char*>(buffer);
-        detail::write(d, dets_);
-        detail::write(d, size_);
-        detail::write(d, classes_);
-        detail::write(d, dtype_);
-    }
-    nvinfer1::IPluginV2IOExt* clone() const TRTX_NOEXCEPT override {
-        auto* c = new MaskRcnnInferencePluginIOExt(dets_, size_, classes_);
-        c->dtype_ = dtype_;
-        return c;
-    }
-
-   private:
-    static constexpr size_t kReferenceBlob = 3 * sizeof(int);
-    int dets_ = 0, size_ = 0, classes_ = 0;
-    bool valid_ = true;
-};
-
-// RpnDecode and PredictorDecode for an FP16 engine: scores and deltas fp32 or fp16 (one type for both), PredictorDecode's
-// proposals and every output fp32 (trtx_rpn_decode_typed / trtx_predictor_decode_typed).  Same names, version, constructor
-// arguments and namespace as RpnDecodePlugin / PredictorDecodePlugin, same blob + the trailing int32 element type.
-class RpnDecodePluginIOExt : public RcnnIOExtBase {
-   public:
-    RpnDecodePluginIOExt(int top_n, const std::vector<float>& anchors, float stride, size_t image_height, size_t image_width)
-        : top_n_(top_n), anchors_(anchors), stride_(stride), height_(0), width_(0), image_height_(image_height), image_width_(image_width) {}
-    RpnDecodePluginIOExt(int top_n, const std::vector<float>& anchors, float stride, size_t height, size_t width, size_t image_height,
-                         size_t image_width)
-        : top_n_(top_n), anchors_(anchors), stride_(stride), height_(height), width_(width), image_height_(image_height), image_width_(image_width) {}
-    RpnDecodePluginIOExt(const void* data, size_t length) {  // RpnDecodePlugin.h:42-58 (+ the element type)
-        const char* d = static_cast<const char*>(data);
-        size_t n = 0;
-        valid_ = length >= sizeof(top_n_) + sizeof(size_t);
-        if (valid_) {
-            detail::read(d, top_n_);
-            detail::read(d, n);
-            valid_ = n <= length / sizeof(float) &&
-                     (length == reference_length(n) || length == reference_length(n) + sizeof(int32_t));
-        }
-        if (!valid_) return;
-        anchors_.resize(n);
-        for (size_t i = 0; i < n; ++i) detail::read(d, anchors_[i]);
-        detail::read(d, stride_);
-        detail::read(d, height_);
-        detail::read(d, width_);
-        detail::read(d, image_height_);
-        detail::read(d, image_width_);
-        valid_ = read_dtype(d, length, reference_length(n));
-    }
-    bool valid() const { return valid_; }  // false: the blob had neither the reference's length nor that + 4
-    const char* getPluginType() const TRTX_NOEXCEPT override { return "RpnDecode"; }
-    int getNbOutputs() const TRTX_NOEXCEPT override { return 2; }
-    nvinfer1::Dims getOutputDimensions(int index, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override { return nvinfer1::Dims2(top_n_, index == 1 ? 4 : 1); }
-    size_t getWorkspaceSize(int maxBatchSize) const TRTX_NOEXCEPT override {
-        return (size_t)trtx_rpn_decode_typed(dtype_, maxBatchSize, nullptr, nullptr, nullptr, nullptr, (int)height_, (int)width_,
-                                             (int)image_height_, (int)image_width_, stride_, anchors_.data(), (int)anchors_.size() / 4,
-                                             top_n_, nullptr, 0, nullptr);
-    }
-    // scores and deltas fp32 or fp16, one type; the scores and boxes fp32
-    bool supportsFormatCombination(int pos, const nvinfer1::PluginTensorDesc* io, int nbInputs, int) const TRTX_NOEXCEPT override {
-        if (io[pos].format != nvinfer1::TensorFormat::kLINEAR) return false;
-        if (pos < nbInputs) return float_or_half(io[pos].type) && io[pos].type == io[0].type;
-        return io[pos].type == nvinfer1::DataType::kFLOAT;
-    }
-    nvinfer1::DataType getOutputDataType(int, const nvinfer1::DataType*, int) const TRTX_NOEXCEPT override { return nvinfer1::DataType::kFLOAT; }
-    void configurePlugin(const nvinfer1::PluginTensorDesc* in, int, const nvinfer1::PluginTensorDesc*, int) TRTX_NOEXCEPT override {
-        height_ = in[0].dims.d[1];  // RpnDecodePlugin.h:148-157: scores dims {A, H, W}
-        width_ = in[0].dims.d[2];
-        dtype_ = in[0].type == nvinfer1::DataType::kHALF ? TRTX_F16 : TRTX_F32;
-    }
+    int initialize() TRTX_NOEXCEPT override { return 0; }
+    void terminate() TRTX_NOEXCEPT override {}
+    size_t getWorkspaceSize(int maxBatchSize) const TRTX_NOEXCEPT override { return P::workspace(dtype_, maxBatchSize); }
     int enqueue(int batchSize, const void* const* inputs, void* TRTX_CONST_ENQUEUE* outputs, void* workspace, cudaStream_t stream) TRTX_NOEXCEPT override {
-        const int64_t rc = trtx_rpn_decode_typed(dtype_, batchSize, inputs[0], inputs[1], static_cast<float*>(outputs[0]),
-                                                 static_cast<float*>(outputs[1]), (int)height_, (int)width_, (int)image_height_,
-                                                 (int)image_width_, stride_, anchors_.data(), (int)anchors_.size() / 4, top_n_, workspace,
-                                                 getWorkspaceSize(batchSize), stream);
-        return detail::rcnn_rc(rc);
+        return valid_ ? P::run(dtype_, batchSize, inputs, outputs, workspace, stream) : TRTX_ERR_INVALID;
     }
-    size_t getSerializationSize() const TRTX_NOEXCEPT override { return reference_length(anchors_.size()) + sizeof(int32_t); }
+    size_t getSerializationSize() const TRTX_NOEXCEPT override { return P::blob_size() + sizeof(dtype_); }
     void serialize(void* buffer) const TRTX_NOEXCEPT override {
         char* d = static_cast<char*>(buffer);
-        detail::write(d, top_n_);
-        detail::write(d, anchors_.size());
-        for (float v : anchors_) detail::write(d, v);
-        detail::write(d, stride_);
-        detail::write(d, height_);
-        detail::write(d, width_);
-        detail::write(d, image_height_);
-        detail::write(d, image_width_);
+        P::write(d);
         detail::write(d, dtype_);
     }
-    nvinfer1::IPluginV2IOExt* clone() const TRTX_NOEXCEPT override {
-        auto* c = new RpnDecodePluginIOExt(top_n_, anchors_, stride_, height_, width_, image_height_, image_width_);
-        c->dtype_ = dtype_;
-        return c;
-    }
+    nvinfer1::IPluginV2IOExt* clone() const TRTX_NOEXCEPT override { return new RcnnPluginIOExt(*this); }
+    void destroy() TRTX_NOEXCEPT override { delete this; }
 
    private:
-    static size_t reference_length(size_t num_anchor_floats) {
-        return sizeof(int) + sizeof(size_t) + sizeof(float) * num_anchor_floats + sizeof(float) + 4 * sizeof(size_t);
-    }
-    int top_n_ = 0;
-    std::vector<float> anchors_;
-    float stride_ = 0.f;
-    size_t height_ = 0, width_ = 0, image_height_ = 0, image_width_ = 0;
+    int32_t dtype_ = TRTX_F32;
     bool valid_ = true;
 };
 
-class PredictorDecodePluginIOExt : public RcnnIOExtBase {
+// The creator of an R-CNN plugin class.  No fields: createPlugin answers nullptr, as the reference's creators do; a blob the
+// class refuses deserializes to nullptr.
+template <class Plugin>
+class RcnnCreator : public nvinfer1::IPluginCreator {
    public:
-    PredictorDecodePluginIOExt(unsigned num_boxes, unsigned image_height, unsigned image_width, const std::vector<float>& w)
-        : num_boxes_(num_boxes), num_classes_(0), image_height_(image_height), image_width_(image_width), w_(w) {}
-    PredictorDecodePluginIOExt(unsigned num_boxes, unsigned num_classes, unsigned image_height, unsigned image_width, const std::vector<float>& w)
-        : num_boxes_(num_boxes), num_classes_(num_classes), image_height_(image_height), image_width_(image_width), w_(w) {}
-    PredictorDecodePluginIOExt(const void* data, size_t length) {  // PredictorDecodePlugin.h:40-54 (+ the element type)
-        const char* d = static_cast<const char*>(data);
-        size_t n = 0;
-        valid_ = length >= 4 * sizeof(unsigned) + sizeof(size_t);
-        if (valid_) {
-            detail::read(d, num_boxes_);
-            detail::read(d, num_classes_);
-            detail::read(d, image_height_);
-            detail::read(d, image_width_);
-            detail::read(d, n);
-            valid_ = n <= length / sizeof(float) &&
-                     (length == reference_length(n) || length == reference_length(n) + sizeof(int32_t));
-        }
-        if (!valid_) return;
-        w_.resize(n);
-        for (size_t i = 0; i < n; ++i) detail::read(d, w_[i]);
-        valid_ = read_dtype(d, length, reference_length(n));
-    }
-    bool valid() const { return valid_; }  // false: the blob had neither the reference's length nor that + 4
-    const char* getPluginType() const TRTX_NOEXCEPT override { return "PredictorDecode"; }
-    int getNbOutputs() const TRTX_NOEXCEPT override { return 3; }
-    nvinfer1::Dims getOutputDimensions(int index, const nvinfer1::Dims*, int) TRTX_NOEXCEPT override { return nvinfer1::Dims2(num_boxes_, index == 1 ? 4 : 1); }
-    size_t getWorkspaceSize(int maxBatchSize) const TRTX_NOEXCEPT override {
-        return (size_t)trtx_predictor_decode_typed(dtype_, maxBatchSize, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, (int)num_boxes_,
-                                                   (int)num_classes_, (int)image_height_, (int)image_width_, w_.data(), nullptr, 0, nullptr);
-    }
-    // scores and deltas fp32 or fp16, one type; the proposals and the scores, boxes and classes fp32
-    bool supportsFormatCombination(int pos, const nvinfer1::PluginTensorDesc* io, int, int) const TRTX_NOEXCEPT override {
-        if (io[pos].format != nvinfer1::TensorFormat::kLINEAR) return false;
-        if (pos < 2) return float_or_half(io[pos].type) && io[pos].type == io[0].type;
-        return io[pos].type == nvinfer1::DataType::kFLOAT;
-    }
-    nvinfer1::DataType getOutputDataType(int, const nvinfer1::DataType*, int) const TRTX_NOEXCEPT override { return nvinfer1::DataType::kFLOAT; }
-    void configurePlugin(const nvinfer1::PluginTensorDesc* in, int, const nvinfer1::PluginTensorDesc*, int) TRTX_NOEXCEPT override {
-        num_classes_ = in[0].dims.d[1];  // scores dims {N, C, 1, 1}
-        dtype_ = in[0].type == nvinfer1::DataType::kHALF ? TRTX_F16 : TRTX_F32;
-    }
-    int enqueue(int batchSize, const void* const* inputs, void* TRTX_CONST_ENQUEUE* outputs, void* workspace, cudaStream_t stream) TRTX_NOEXCEPT override {
-        if (w_.size() < 4) return TRTX_ERR_INVALID;
-        const int64_t rc = trtx_predictor_decode_typed(dtype_, batchSize, inputs[0], inputs[1], static_cast<const float*>(inputs[2]),
-                                                       static_cast<float*>(outputs[0]), static_cast<float*>(outputs[1]),
-                                                       static_cast<float*>(outputs[2]), (int)num_boxes_, (int)num_classes_, (int)image_height_,
-                                                       (int)image_width_, w_.data(), workspace, getWorkspaceSize(batchSize), stream);
-        return detail::rcnn_rc(rc);
-    }
-    size_t getSerializationSize() const TRTX_NOEXCEPT override { return reference_length(w_.size()) + sizeof(int32_t); }
-    void serialize(void* buffer) const TRTX_NOEXCEPT override {
-        char* d = static_cast<char*>(buffer);
-        detail::write(d, num_boxes_);
-        detail::write(d, num_classes_);
-        detail::write(d, image_height_);
-        detail::write(d, image_width_);
-        detail::write(d, w_.size());
-        for (float v : w_) detail::write(d, v);
-        detail::write(d, dtype_);
-    }
-    nvinfer1::IPluginV2IOExt* clone() const TRTX_NOEXCEPT override {
-        auto* c = new PredictorDecodePluginIOExt(num_boxes_, num_classes_, image_height_, image_width_, w_);
-        c->dtype_ = dtype_;
-        return c;
-    }
-
-   private:
-    static size_t reference_length(size_t num_weights) { return 4 * sizeof(unsigned) + sizeof(size_t) + sizeof(float) * num_weights; }
-    unsigned num_boxes_ = 0, num_classes_ = 0, image_height_ = 0, image_width_ = 0;
-    std::vector<float> w_;
-    bool valid_ = true;
-};
-
-// deserializePlugin for the four classes above: a blob of neither accepted length is refused (nullptr)
-template <typename P>
-class RcnnIOExtCreator : public nvinfer1::IPluginCreator {
-   public:
-    explicit RcnnIOExtCreator(const char* name) : name_(name) {}
-    const char* getPluginName() const TRTX_NOEXCEPT override { return name_; }
+    const char* getPluginName() const TRTX_NOEXCEPT override { return Plugin::type(); }
     const char* getPluginVersion() const TRTX_NOEXCEPT override { return "1"; }
     const char* getPluginNamespace() const TRTX_NOEXCEPT override { return ""; }
     void setPluginNamespace(const char*) TRTX_NOEXCEPT override {}
     const nvinfer1::PluginFieldCollection* getFieldNames() TRTX_NOEXCEPT override { return nullptr; }
-    nvinfer1::IPluginV2* createPlugin(const char*, const nvinfer1::PluginFieldCollection*) TRTX_NOEXCEPT override { return nullptr; }  // as the reference
+    nvinfer1::IPluginV2* createPlugin(const char*, const nvinfer1::PluginFieldCollection*) TRTX_NOEXCEPT override { return nullptr; }
     nvinfer1::IPluginV2* deserializePlugin(const char*, const void* data, size_t len) TRTX_NOEXCEPT override {
-        P* p = new P(data, len);
+        Plugin* p = new Plugin(data, len);
         if (p->valid()) return p;
         delete p;
         return nullptr;
     }
-
-   private:
-    const char* name_;
 };
-struct RoiAlignPluginIOExtCreator : RcnnIOExtCreator<RoiAlignPluginIOExt> { RoiAlignPluginIOExtCreator() : RcnnIOExtCreator("RoiAlign") {} };
-struct MaskRcnnInferencePluginIOExtCreator : RcnnIOExtCreator<MaskRcnnInferencePluginIOExt> { MaskRcnnInferencePluginIOExtCreator() : RcnnIOExtCreator("MaskRcnnInference") {} };
-struct RpnDecodePluginIOExtCreator : RcnnIOExtCreator<RpnDecodePluginIOExt> { RpnDecodePluginIOExtCreator() : RcnnIOExtCreator("RpnDecode") {} };
-struct PredictorDecodePluginIOExtCreator : RcnnIOExtCreator<PredictorDecodePluginIOExt> { PredictorDecodePluginIOExtCreator() : RcnnIOExtCreator("PredictorDecode") {} };
+
+using RpnDecodePlugin = RcnnPlugin<RpnDecodeParams>;
+using RpnNmsPlugin = RcnnPlugin<RpnNmsParams>;
+using PredictorDecodePlugin = RcnnPlugin<PredictorDecodeParams>;
+using BatchedNmsPlugin = RcnnPlugin<BatchedNmsParams>;
+using RoiAlignPlugin = RcnnPlugin<RoiAlignParams>;
+using MaskRcnnInferencePlugin = RcnnPlugin<MaskRcnnInferenceParams>;
+using RpnDecodePluginIOExt = RcnnPluginIOExt<RpnDecodeParams>;
+using PredictorDecodePluginIOExt = RcnnPluginIOExt<PredictorDecodeParams>;
+using RoiAlignPluginIOExt = RcnnPluginIOExt<RoiAlignParams>;
+using MaskRcnnInferencePluginIOExt = RcnnPluginIOExt<MaskRcnnInferenceParams>;
+
+using RpnDecodePluginCreator = RcnnCreator<RpnDecodePlugin>;
+using RpnNmsPluginCreator = RcnnCreator<RpnNmsPlugin>;
+using PredictorDecodePluginCreator = RcnnCreator<PredictorDecodePlugin>;
+using BatchedNmsPluginCreator = RcnnCreator<BatchedNmsPlugin>;
+using RoiAlignPluginCreator = RcnnCreator<RoiAlignPlugin>;
+using MaskRcnnInferencePluginCreator = RcnnCreator<MaskRcnnInferencePlugin>;
+using RpnDecodePluginIOExtCreator = RcnnCreator<RpnDecodePluginIOExt>;
+using PredictorDecodePluginIOExtCreator = RcnnCreator<PredictorDecodePluginIOExt>;
+using RoiAlignPluginIOExtCreator = RcnnCreator<RoiAlignPluginIOExt>;
+using MaskRcnnInferencePluginIOExtCreator = RcnnCreator<MaskRcnnInferencePluginIOExt>;
 
 }  // namespace trtx
 

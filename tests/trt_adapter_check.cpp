@@ -1,6 +1,7 @@
 // trt_adapter_check.cpp -- drives include/trtx_plugins.h through the TensorRT plugin surface exactly as an engine
 // builder / the TensorRT runtime would: registry lookup by name, createPlugin with the reference's field layouts,
-// (de)serialization, clone, getOutputDimensions, getWorkspaceSize, and (with --gpu) enqueue on the device.
+// (de)serialization, malformed R-CNN blobs refused, clone, getOutputDimensions, getWorkspaceSize, and (with --gpu) enqueue on
+// the device.
 // Compiled against tests/mock_trt/NvInfer.h (this image has no TensorRT) and linked with libtrtx_hot.so.
 #define TRTX_REGISTER_PLUGINS
 #include "trtx_plugins.h"
@@ -10,6 +11,7 @@
 #include <cassert>
 #include <cstdio>
 #include <cstdlib>
+#include <type_traits>
 #include <vector>
 
 #define CHECK(x)                                                          \
@@ -36,6 +38,48 @@ struct Builder : IExprBuilder {
     }
     const IDimensionExpr* operation(DimensionOperation, const IDimensionExpr& a, const IDimensionExpr&) TRTX_NX override { return &a; }
 };
+
+// The blobs an IPluginV2Ext R-CNN class accepts: its reference blob ref and, where the class has an IPluginV2IOExt twin
+// (f32_tag), ref + a TRTX_F32 tag; each deserializes, directly and through the registered creator, to a plugin that writes ref.
+// Refused, with the creator answering nullptr and the plugin's enqueue TRTX_ERR_INVALID: an empty blob, ref one byte short or
+// over, ref + a TRTX_F16 tag, and an anchor / weight count of 2^62 at byte count_at.
+template <class P>
+static void check_blobs(const std::vector<char>& ref, bool f32_tag, int count_at = -1) {
+    static_assert(std::is_copy_constructible<P>::value && std::is_move_constructible<P>::value, "rcnn.cpp builds the plugins by value");
+    IPluginCreator* c = getPluginRegistry()->getPluginCreator(P::type(), "1");
+    CHECK(c != nullptr);
+    auto accepted = [&](const std::vector<char>& b) {
+        P direct(b.data(), b.size());
+        IPluginV2* p = c->deserializePlugin(P::type(), b.data(), b.size());
+        CHECK((p != nullptr) == direct.valid());
+        if (!p) {
+            CHECK(direct.enqueue(1, nullptr, nullptr, nullptr, nullptr) == TRTX_ERR_INVALID);
+            return false;
+        }
+        std::vector<char> back(p->getSerializationSize());
+        p->serialize(back.data());
+        CHECK(back == ref);
+        p->destroy();
+        return true;
+    };
+    CHECK(accepted(ref));
+    CHECK(!accepted({}));
+    CHECK(!accepted(std::vector<char>(ref.begin(), ref.end() - 1)));
+    std::vector<char> b = ref;
+    b.push_back(0);
+    CHECK(!accepted(b));
+    for (int32_t tag : {TRTX_F32, TRTX_F16}) {
+        b = ref;
+        b.insert(b.end(), reinterpret_cast<const char*>(&tag), reinterpret_cast<const char*>(&tag) + sizeof(tag));
+        CHECK(accepted(b) == (f32_tag && tag == TRTX_F32));
+    }
+    if (count_at >= 0) {
+        b = ref;
+        const size_t big = (size_t)1 << 62;
+        std::memcpy(b.data() + count_at, &big, sizeof(big));
+        CHECK(!accepted(b));
+    }
+}
 
 int main(int argc, char** argv) {
     const bool gpu = argc > 1 && std::string(argv[1]) == "--gpu";
@@ -136,6 +180,7 @@ int main(int argc, char** argv) {
     rpn.serialize(rb.data());
     trtx::RpnDecodePlugin rpn2(rb.data(), rb.size());
     hex("rpn_decode", rb);
+    check_blobs<trtx::RpnDecodePlugin>(rb, true, 4);
     {
         trtx::RpnNmsPlugin rn(0.7f, 1000);
         Dims nd[2];
@@ -144,6 +189,7 @@ int main(int argc, char** argv) {
         std::vector<char> nb(rn.getSerializationSize());
         rn.serialize(nb.data());
         hex("rpn_nms", nb);
+        check_blobs<trtx::RpnNmsPlugin>(nb, false);
         trtx::PredictorDecodePlugin pd(1000, 800, 1067, std::vector<float>{10.f, 10.f, 5.f, 5.f});
         Dims pdm[3];
         pdm[0].nbDims = 4; pdm[0].d[0] = 1000; pdm[0].d[1] = 80; pdm[0].d[2] = 1; pdm[0].d[3] = 1; pdm[1] = pdm[0]; pdm[2] = pdm[0];
@@ -151,6 +197,7 @@ int main(int argc, char** argv) {
         std::vector<char> pb(pd.getSerializationSize());
         pd.serialize(pb.data());
         hex("predictor_decode", pb);
+        check_blobs<trtx::PredictorDecodePlugin>(pb, true, 16);
     }
     CHECK(rpn2.getSerializationSize() == rb.size());
     trtx::BatchedNmsPlugin bn(1, 0.5f, 100);
@@ -162,6 +209,7 @@ int main(int argc, char** argv) {
         std::vector<char> bb(bn.getSerializationSize());
         bn.serialize(bb.data());
         hex("batched_nms", bb);
+        check_blobs<trtx::BatchedNmsPlugin>(bb, false);
     }
     CHECK(getPluginRegistry()->getPluginCreator("BatchedNms", "1") != nullptr && getPluginRegistry()->getPluginCreator("RpnNms", "1") != nullptr);
     trtx::RoiAlignPlugin ra(14, 1.f / 16, 0, 1000, 1024);
@@ -173,6 +221,7 @@ int main(int argc, char** argv) {
     ra.serialize(rab.data());
     trtx::RoiAlignPlugin ra2(rab.data(), rab.size());
     hex("roi_align", rab);
+    check_blobs<trtx::RoiAlignPlugin>(rab, true);
     CHECK(rab.size() == 28 && ra2.getOutputDimensions(0, nullptr, 2).d[3] == 14 && ra2.getWorkspaceSize(8) == 0);
     CHECK(std::string(ra2.getPluginType()) == "RoiAlign" && getPluginRegistry()->getPluginCreator("RoiAlign", "1") != nullptr);
     trtx::MaskRcnnInferencePlugin mi(100, 14);
@@ -182,6 +231,7 @@ int main(int argc, char** argv) {
         std::vector<char> mb(mi.getSerializationSize());
         mi.serialize(mb.data());
         hex("mask_rcnn_inference", mb);
+        check_blobs<trtx::MaskRcnnInferencePlugin>(mb, true);
     }
 
     if (gpu) {

@@ -1,7 +1,8 @@
 // trt_adapter_half_check.cpp -- the half-accepting adapters of include/trtx_plugins.h (DecodePluginDynamic,
 // RoiAlignPluginIOExt, MaskRcnnInferencePluginIOExt) driven as a TensorRT builder / runtime drives plugins: format
 // combinations at every position, output data types, configurePlugin -> serialize -> deserialize -> clone, and (with --gpu)
-// enqueue through the adapter against the direct C call.  Compiled against tests/mock_trt/NvInfer.h (this image has no
+// enqueue through the adapter, and through the IPluginV2Ext RoiAlign / MaskRcnnInference classes in fp32, against the direct C
+// call.  Compiled against tests/mock_trt/NvInfer.h (this image has no
 // TensorRT) with the half-accepting rcnn creators registered, and linked with libtrtx_hot.so.
 #define TRTX_REGISTER_PLUGINS
 #define TRTX_RCNN_HALF_IO_PLUGINS
@@ -219,6 +220,11 @@ int main(int argc, char** argv) {
             CHECK(trtx_roi_align(B, d_rois, d_feat, static_cast<float*>(d_b), 14, 1.f / 16, 2, N, C, H, W, nullptr) == 0);
             CHECK(cudaDeviceSynchronize() == cudaSuccess);
             CHECK(download<uint32_t>(d_a, nout) == download<uint32_t>(d_b, nout));
+            trtx::RoiAlignPlugin legacy(14, 1.f / 16, 2, N, C, H, W);  // the IPluginV2Ext class == the fp32 call
+            CHECK(cudaMemset(d_a, 0x11, nout * 4) == cudaSuccess);
+            CHECK(legacy.enqueue(B, ins, outs, nullptr, nullptr) == 0);
+            CHECK(cudaDeviceSynchronize() == cudaSuccess);
+            CHECK(download<uint32_t>(d_a, nout) == download<uint32_t>(d_b, nout));
         }
         // ---- MaskRcnnInference: half masks through the adapter == the typed C call
         std::vector<float> masks((size_t)B * D * NC * S * S), idx((size_t)B * D);
@@ -238,6 +244,13 @@ int main(int argc, char** argv) {
             const std::vector<uint32_t> r = download<uint32_t>(d_a, mout);
             CHECK(r == download<uint32_t>(d_b, mout));
             CHECK(r[3 * S * S] == 0x11111111u && r[0] != 0x11111111u);  // the row of index -1 stays untouched
+            trtx::MaskRcnnInferencePlugin legacy(D, S, NC);  // the IPluginV2Ext class == the fp32 call
+            ins[1] = upload(masks);
+            CHECK(cudaMemset(d_a, 0x11, mout * 4) == cudaSuccess && cudaMemset(d_b, 0x11, mout * 4) == cudaSuccess);
+            CHECK(legacy.enqueue(B, ins, outs, nullptr, nullptr) == 0);
+            CHECK(trtx_mask_rcnn_inference(B, d_idx, static_cast<const float*>(ins[1]), static_cast<float*>(d_b), D, S, NC, nullptr) == 0);
+            CHECK(cudaDeviceSynchronize() == cudaSuccess);
+            CHECK(download<uint32_t>(d_a, mout) == download<uint32_t>(d_b, mout));
         }
         // ---- Decode_TRT: half heads through the adapter == trtx_retina_decode_enqueue with in_dtype = TRTX_F16
         trtx_retina_params rp{};

@@ -2,7 +2,7 @@
 // TensorRT builder / runtime drives plugins: format combinations at every position, output data types, configurePlugin ->
 // serialize -> deserialize -> clone with the trailing element type, a blob of the reference's length (what a plan serialized
 // with the IPluginV2Ext classes holds) deserializing through the registry as an fp32 plugin, wrong lengths refused, and (with
-// --gpu) enqueue through the adapters in both types against the direct C calls.  Compiled against tests/mock_trt/NvInfer.h
+// --gpu) enqueue through the adapters in both types, and through the IPluginV2Ext classes in fp32, against the direct C calls.  Compiled against tests/mock_trt/NvInfer.h
 // with the R-CNN plugins of an FP16 engine registered, and linked with libtrtx_hot.so.
 #define TRTX_REGISTER_PLUGINS
 #define TRTX_RCNN_HALF_IO_PLUGINS
@@ -230,6 +230,17 @@ int main(int argc, char** argv) {
             CHECK(cudaDeviceSynchronize() == cudaSuccess);
             CHECK(download(o1, B * TOP) == download(r1, B * TOP) && download(o2, B * TOP * 4) == download(r2, B * TOP * 4));
         }
+        {  // the IPluginV2Ext class configured with the same dims == the fp32 call
+            trtx::RpnDecodePlugin legacy(TOP, anchors, 16.f, 320, 432);
+            const Dims dims[2] = {rio[0].dims, rio[1].dims};
+            legacy.configurePlugin(dims, 2, nullptr, 2, nullptr, nullptr, nullptr, nullptr, PluginFormat::kLINEAR, B);
+            const void* ins[2] = {s32, d32};
+            void* outs[2] = {o1, o2};
+            CHECK(cudaMemset(o1, 0x11, B * TOP * 4) == cudaSuccess && cudaMemset(o2, 0x11, B * TOP * 16) == cudaSuccess);
+            CHECK(legacy.enqueue(B, ins, outs, ws, nullptr) == 0);
+            CHECK(cudaDeviceSynchronize() == cudaSuccess);
+            CHECK(download(o1, B * TOP) == download(r1, B * TOP) && download(o2, B * TOP * 4) == download(r2, B * TOP * 4));
+        }
         // ---- PredictorDecode through the adapter == trtx_predictor_decode_typed
         std::vector<float> ps((size_t)B * N * NC), pdl((size_t)B * N * NC * 4), props((size_t)B * N * 4);
         for (float& v : ps) v = (rnd() + 1.f) * 0.5f;
@@ -258,6 +269,17 @@ int main(int argc, char** argv) {
             CHECK(cudaDeviceSynchronize() == cudaSuccess);
             CHECK(download(a[0], B * N) == download(b[0], B * N) && download(a[1], B * N * 4) == download(b[1], B * N * 4));
             CHECK(download(a[2], B * N) == download(b[2], B * N));
+        }
+        {  // the IPluginV2Ext class configured with the same dims == the fp32 call
+            trtx::PredictorDecodePlugin legacy(N, 320, 432, w4);
+            const Dims dims[3] = {pio[0].dims, pio[1].dims, pio[2].dims};
+            legacy.configurePlugin(dims, 3, nullptr, 3, nullptr, nullptr, nullptr, nullptr, PluginFormat::kLINEAR, B);
+            const void* ins[3] = {p32, q32, dprops};
+            void* outs[3] = {a[0], a[1], a[2]};
+            for (int k = 0; k < 3; ++k) CHECK(cudaMemset(a[k], 0x11, B * N * 16) == cudaSuccess);
+            CHECK(legacy.enqueue(B, ins, outs, ws, nullptr) == 0);
+            CHECK(cudaDeviceSynchronize() == cudaSuccess);
+            for (int k = 0; k < 3; ++k) CHECK(download(a[k], B * N * (k == 1 ? 4 : 1)) == download(b[k], B * N * (k == 1 ? 4 : 1)));
         }
         std::printf("gpu rcnn half enqueue ok\n");
     }
