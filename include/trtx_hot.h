@@ -50,7 +50,7 @@ TRTX_API int trtx_last_cuda_error(void);
 /* sizeof() of the parameter structs as THIS library was compiled, so that an FFI binding (ctypes, cgo, ...) can check its
  * mirror of the layout: which = 0 trtx_yolo_params, 1 trtx_nms_params, 2 trtx_retina_params, 3 trtx_image_desc,
  * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_frame, 7 trtx_pose_obb_params, 8 trtx_frame,
- * 9 trtx_face_post_params, 10 trtx_yolop_post_params; anything else 0. */
+ * 9 trtx_face_post_params, 10 trtx_yolop_post_params, 11 trtx_detr_post_params; anything else 0. */
 TRTX_API size_t trtx_abi_sizeof(int which);
 
 /* =====================================================================================
@@ -755,6 +755,56 @@ typedef struct trtx_yolop_post_params {
 TRTX_API int trtx_yolop_postprocess_enqueue(const trtx_yolop_post_params* p, const trtx_frame* frames_host, int batch,
                                             const float* dets_dev, int max_rows, const int32_t* seg_dev,
                                             const int32_t* lane_dev, float* rows_dev, trtx_stream_t stream);
+
+/* =====================================================================================
+ * 10. DETR pre- and post-process
+ *    replaces the HOST preprocessImg of detr/common.hpp:81-89 with the driver's plane loop and H2D copy
+ *    (detr/detr.cpp:754-767, :638-641; the INT8 calibrator's getBatch, detr/calibrator.hpp:78-88, calls the same
+ *    preprocessImg), and the HOST stage after inference: the D2H copy of the engine's scores and boxes (:643-648) and the
+ *    per-query loop of detr/detr.cpp:777-806 (argmax, score threshold, no-object class, cv::Rect in the frame).
+ * ===================================================================================== */
+/* preprocessImg + the plane loop for a whole batch, one launch per <= 64 images: images_host = `batch` u8 HWC BGR descriptors
+ * in HOST memory (trtx_image_desc, any pitch and base alignment, mixed sizes allowed); dst_dev = [batch, 3, net_h, net_w] fp32
+ * planes in R, G, B order (cvtColor BGR2RGB, then the driver's planes 0, 1, 2; INPUT_W x INPUT_H = 1066 x 800), the engine
+ * input.  The whole frame is stretched over the whole net (no letterbox) by OpenCV 4.x's 8-bit INTER_LINEAR, bit for bit
+ * (an exact 2x downscale, where OpenCV takes INTER_AREA, gives the same bytes); byte u of plane c (mean = 0.485, 0.456,
+ * 0.406 and std = 0.229, 0.224, 0.225 for planes 0, 1, 2) becomes
+ *     s = (float)u * (1.f / 255.f) - (float)mean_c  (float),   (float)((double)s / std_c),
+ * the driver's convertTo / `/= 255` / `-= Scalar` / `/= Scalar` chain.  Every descriptor is checked before the first launch
+ * (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer, batch / net sizes <= 0, pitch < 3 * width or a
+ * dst_dev that is not 4-byte aligned; TRTX_ERR_UNSUPPORTED for a net wider than 4 757 pixels (the band's staged source rows
+ * in shared memory).  No workspace; can be captured in a CUDA graph. */
+TRTX_API int trtx_detr_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
+                                          trtx_stream_t stream);
+
+/* The rectangle of detr/detr.cpp:795-803 for one box cx, cy, w, h (normalised, the engine's sigmoid output) in an
+ * img_w x img_h frame: x1 = (float)(((double)cx - (double)w / 2.0) * img_w), likewise y1 (cy, h), x2 and y2 (with +);
+ * rect = {(int)x1, (int)y1, (int)(x2 - x1), (int)(y2 - y1)}, the differences in float.  Defined where the reference is
+ * not, as the compiled x86-64 reference behaves: a value that is NaN, infinite or outside [-2^31, 2^31) converts to
+ * INT_MIN.  Host function; the device form is trtx_detr_postprocess_enqueue. */
+TRTX_API int trtx_detr_get_rect(int img_w, int img_h, const float box[4], int rect[4]);
+
+typedef struct trtx_detr_post_params {
+    int32_t num_queries;  /* Q: NUM_QUERIES (100) */
+    int32_t num_classes;  /* C: NUM_CLASS (92), the last one the no-object class */
+    float score_thresh;   /* SCORE_THRESH (0.5f) */
+} trtx_detr_post_params;
+
+/* scores_dev [B, Q, C] fp32: the engine's softmax scores; boxes_dev [B, Q, 4] fp32: its (cx, cy, w, h), normalised.
+ * frame_wh_host: `batch` pairs (img_w, img_h) in HOST memory (copied into launch parameters; sizes may differ in a call).
+ * rows_dev [B, 1 + Q*6]: the kept count, then per kept query in query order (x, y, w, h, score, class) with x, y, w, h =
+ *   trtx_detr_get_rect as floats (exact for |v| <= 2^24); rows past the count are zeroed.
+ * Per query (detr.cpp:779-799): label = -1, score = -1.f; for j = 0 .. C-1 `if (score < s[j])` takes j, so the first
+ * maximum wins and a NaN is never taken; the query is kept when score > score_thresh (float) and label != C - 1.  Frame b
+ * reads queries b; the reference's loop runs over every query of the batch for every frame (detr.cpp:778), which is the
+ * same at its BATCH_SIZE 1.  Drawing and labels stay with the caller.
+ * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
+ * batch / Q / a frame size <= 0, C < 2, or a score_thresh that is NaN or below -1 (which would keep the reference's
+ * label -1 queries); TRTX_ERR_UNSUPPORTED for Q or C above 2^24 (the count and the class are stored as floats).  One CTA per
+ * frame, one launch per 64 frames, no workspace, no atomics; can be captured in a CUDA graph. */
+TRTX_API int trtx_detr_postprocess_enqueue(const trtx_detr_post_params* p, const int32_t* frame_wh_host, int batch,
+                                           const float* scores_dev, const float* boxes_dev, float* rows_dev,
+                                           trtx_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -352,6 +352,27 @@ __host__ __device__ inline void yolop_get_rect(const YoloLetterbox& lb, const fl
     rect[3] = (int)((uint32_t)v[3] - (uint32_t)v[1]);
 }
 
+// DETR's rectangle (detr/detr.cpp:795-803): box = cx, cy, w, h, normalised.  Each corner is a double expression stored to
+// float, `float x1 = (cx - w / 2.0) * img.cols`; then cv::Rect r(x1, y1, x2 - x1, y2 - y1) converts four floats to int, the
+// differences taken in float.  Undefined cases as the compiled x86-64 reference behaves: trunc_to_int_x86.  __dsub_rn /
+// __dmul_rn on the device, so that nvcc cannot contract the corner into an FMA.
+__host__ __device__ inline void detr_get_rect(int img_w, int img_h, const float box[4], int rect[4]) {
+    float c[4];  // x1, y1, x2, y2
+    for (int k = 0; k < 4; ++k) {
+        const int a = k & 1;  // 0: x, 1: y
+        const double centre = (double)box[a], half = (double)box[2 + a] / 2.0, size = (double)(a ? img_h : img_w);
+#ifdef __CUDA_ARCH__
+        c[k] = __double2float_rn(__dmul_rn(k < 2 ? __dsub_rn(centre, half) : __dadd_rn(centre, half), size));
+#else
+        c[k] = (float)((k < 2 ? centre - half : centre + half) * size);
+#endif
+    }
+    rect[0] = trunc_to_int_x86(c[0]);
+    rect[1] = trunc_to_int_x86(c[1]);
+    rect[2] = trunc_to_int_x86(f_sub(c[2], c[0]));
+    rect[3] = trunc_to_int_x86(f_sub(c[3], c[1]));
+}
+
 __device__ __forceinline__ int warp_excl_scan(int v, int lane, int* total) {
     int x = v;
 #pragma unroll

@@ -602,6 +602,14 @@ struct YolopInput {
     static __device__ __forceinline__ int channel(int c) { return c; }
     static __device__ __forceinline__ float value(int c, uint32_t u) { return yolop_input_value(c, u); }
 };
+// DETR's preprocessImg (detr/common.hpp:81-89): cvtColor BGR2RGB, so plane c (0 = R) takes BGR channel 2 - c; then
+// convertTo(CV_32FC3), `img /= 255` (convertTo(-1, 1. / 255): (float)u * (1.f / 255.f)), `img -= Scalar(mean)` (cv::subtract,
+// float) and `img /= Scalar(std)` (cv::divide, double) -- YOLOP's chain with Scalar(0.485, ...) meeting R instead of B.
+struct DetrInput {
+    static constexpr uint32_t kCanvas = 0u;  // never read: the frame is stretched over the whole net
+    static __device__ __forceinline__ int channel(int c) { return 2 - c; }
+    static __device__ __forceinline__ float value(int c, uint32_t u) { return yolop_input_value(c, u); }
+};
 
 // [B, 3, net_h, net_w] planes: the band is three contiguous runs of band * net_w floats, each written by store_band_run; the
 // value of a byte comes from a per-CTA table of 3 x 256 floats.
@@ -636,6 +644,11 @@ __global__ void __launch_bounds__(kRcnnPreThreads) cls_preprocess_kernel(const _
 __global__ void __launch_bounds__(kRcnnPreThreads) yolop_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
                                                                            float* __restrict__ dst) {
     resize_band<PlanarStore<YolopInput>>(a, dst);
+}
+
+__global__ void __launch_bounds__(kRcnnPreThreads) detr_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
+                                                                          float* __restrict__ dst) {
+    resize_band<PlanarStore<DetrInput>>(a, dst);
 }
 
 // One launch of `kernel` per kMaxRcnnPreImages frames: make(i, im) fills the band descriptor of frame i (validated before).
@@ -692,6 +705,20 @@ static bool cls_band_image(int variant, const trtx_image_desc& d, int net_w, int
     im.scale_x = 1. / ((double)im.rw / im.sw);
     im.scale_y = 1. / ((double)im.rh / im.sh);
     return true;
+}
+
+// The band descriptor of frame d for DETR's preprocessImg: cv::resize(img, img, Size(net_w, net_h)) of the whole frame, i.e.
+// cls_band_image's V8 descriptor without the crop.
+static void detr_band_image(const trtx_image_desc& d, int net_w, int net_h, RcnnPreImage& im) {
+    im.src = d.data_dev;
+    im.sw = d.width;
+    im.sh = d.height;
+    im.pitch = d.pitch;
+    im.x0 = im.y0 = 0;
+    im.rw = net_w;
+    im.rh = net_h;
+    im.scale_x = 1. / ((double)net_w / d.width);
+    im.scale_y = 1. / ((double)net_h / d.height);
 }
 
 }  // namespace trtx
@@ -955,6 +982,23 @@ TRTX_API int trtx_yolop_preprocess_enqueue(const trtx_image_desc* images_host, i
     }
     return launch_bands(yolop_preprocess_kernel, batch, net_w, net_h, dst_dev, smem_max, static_cast<cudaStream_t>(stream),
                         [&](int i, RcnnPreImage& im) { cls_band_image(TRTX_YOLO_V5, images_host[i], net_w, net_h, im); });
+}
+
+// DETR's preprocessImg stretches the whole frame over the whole net: one band descriptor per frame (detr_band_image), the
+// planar store with DETR's R, G, B planes and value chain.
+TRTX_API int trtx_detr_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
+                                          trtx_stream_t stream) {
+    if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
+    if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
+    // every descriptor is checked before the first launch, so that a rejected call writes nothing
+    for (int i = 0; i < batch; ++i) {
+        const trtx_image_desc& d = images_host[i];
+        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
+    }
+    const size_t smem = (size_t)kRcnnPreSlots * 3 * (size_t)net_w * sizeof(int16_t);  // every rectangle is net_w wide
+    if (smem > kClsMaxDynamicSmem) return TRTX_ERR_UNSUPPORTED;
+    return launch_bands(detr_preprocess_kernel, batch, net_w, net_h, dst_dev, smem, static_cast<cudaStream_t>(stream),
+                        [&](int i, RcnnPreImage& im) { detr_band_image(images_host[i], net_w, net_h, im); });
 }
 
 }  // extern "C"

@@ -880,6 +880,7 @@ TRTX_API size_t trtx_abi_sizeof(int which) {
         case 8: return sizeof(trtx_frame);
         case 9: return sizeof(trtx_face_post_params);
         case 10: return sizeof(trtx_yolop_post_params);
+        case 11: return sizeof(trtx_detr_post_params);
         default: return 0;
     }
 }

@@ -1249,6 +1249,55 @@ def yolop_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]]
     return rows_out, canvases_out
 
 
+DETR_NET = (1066, 800)  # INPUT_W, INPUT_H (detr/detr.cpp:13-14)
+
+
+def detr_preprocess(images: Sequence[torch.Tensor], out: torch.Tensor | None = None, net_w: int = DETR_NET[0],
+                    net_h: int = DETR_NET[1], stream=None) -> torch.Tensor:
+    """GPU drop-in for DETR's preprocessImg (detr/common.hpp:81-89) and the driver's plane copy (detr/detr.cpp:754-767) for a
+    batch of device frames: images[i] is a u8 HWC BGR cuda tensor [h, w, 3] with packed pixels (rows may be pitched, sizes
+    may differ) -> [B, 3, net_h, net_w] float32 planes in R, G, B order, the engine input: the whole frame resized to the
+    whole net, / 255, minus the ImageNet mean, over its std.  One launch per 64 images, no synchronisation."""
+    lib = L.load()
+    n = len(images)
+    descs = _image_descs(images)
+    out = _out_tensor(out, (n, 3, net_h, net_w), torch.float32, images[0].device if n else "cuda",
+                      f"out must be float32 [{n}, 3, {net_h}, {net_w}]", contiguous=False)
+    L.check(lib.trtx_detr_preprocess_enqueue(descs, n, net_w, net_h, _ptr(out), _stream(stream)), "trtx_detr_preprocess_enqueue")
+    return out
+
+
+def detr_get_rect(img_w: int, img_h: int, box):
+    """The cv::Rect of detr/detr.cpp:795-803: box cx, cy, w, h (normalised) -> (x, y, w, h) in the img_w x img_h frame."""
+    b = (C.c_float * 4)(*[float(v) for v in box])
+    r = (C.c_int * 4)()
+    L.check(L.load().trtx_detr_get_rect(img_w, img_h, b, r), "trtx_detr_get_rect")
+    return tuple(r)
+
+
+def detr_postprocess(scores: torch.Tensor, boxes: torch.Tensor, image_sizes: Sequence[tuple[int, int]], *,
+                     score_thresh: float = 0.5, out: torch.Tensor | None = None, stream=None) -> torch.Tensor:
+    """GPU drop-in for DETR's host loop after inference (detr/detr.cpp:777-806) for a batch of frames of any sizes.
+    scores [B, Q, C] float32: the engine's softmax scores, class C - 1 the no-object class; boxes [B, Q, 4] float32: its
+    (cx, cy, w, h), normalised; image_sizes[b] = (img_w, img_h) of frame b -> rows [B, 1 + Q*6] float32: the kept count, then
+    per kept query in query order (x, y, w, h, score, class) -- the first maximum over the classes, kept when score >
+    score_thresh (float) and the class is not C - 1, the rectangle as detr_get_rect -- rows past the count zero.  Frame b
+    reads queries b.  One launch per 64 frames, no workspace."""
+    lib = L.load()
+    B = len(image_sizes)
+    if scores.dim() != 3 or scores.shape[0] != B or tuple(boxes.shape) != (B, scores.shape[1], 4):
+        raise ValueError(f"scores must be [{B}, Q, C] and boxes [{B}, Q, 4]")
+    for t in (scores, boxes):
+        if t.dtype != torch.float32:
+            raise ValueError("scores and boxes must be float32")
+    Q, Cn = int(scores.shape[1]), int(scores.shape[2])
+    out = _out_tensor(out, (B, 1 + Q * 6), torch.float32, scores.device, f"out must be contiguous float32 [{B}, {1 + Q * 6}]")
+    q = L.DetrPostParams(Q, Cn, score_thresh)
+    L.check(lib.trtx_detr_postprocess_enqueue(C.byref(q), _frame_wh(image_sizes), B, _ptr(scores), _ptr(boxes), _ptr(out),
+                                              _stream(stream)), "trtx_detr_postprocess_enqueue")
+    return out
+
+
 def cls_postprocess(logits: torch.Tensor, k: int, softmax: bool, probs: bool = False, stream=None):
     """GPU drop-in for the cls drivers' softmax (softmax=True: yolov8, yolo11, yolov5) or raw output (softmax=False: yolo26)
     and topk(res, k): logits [B, C] float32 cuda -> (index [B, k] int32, value [B, k] float32[, probs [B, C] float32]).  The
