@@ -209,6 +209,10 @@ struct Row {
     float cls;
     int anchor;
 };
+// row `id` of image b in the plugin-format rows [B, 1 + max_rows*det_floats]
+__device__ __forceinline__ const float* plugin_row(const NmsArgs& a, int b, uint32_t id) {
+    return a.rows + (size_t)b * (1 + (size_t)a.max_rows * a.det_floats) + 1 + (size_t)id * a.det_floats;
+}
 __device__ __forceinline__ Row fetch_row(const NmsArgs& a, int b, uint32_t id) {
     Row r;
     if (a.from_tiles) {
@@ -219,7 +223,7 @@ __device__ __forceinline__ Row fetch_row(const NmsArgs& a, int b, uint32_t id) {
         r.cls = m.y;
         r.anchor = __float_as_int(m.z);
     } else {
-        const float* p = a.rows + (size_t)b * (1 + (size_t)a.max_rows * a.det_floats) + 1 + (size_t)id * a.det_floats;
+        const float* p = plugin_row(a, b, id);
         r.box = make_float4(p[0], p[1], p[2], p[3]);
         r.conf = p[4];
         r.cls = a.box_format == TRTX_BOX_RETINA ? 0.0f : p[5];
@@ -248,6 +252,82 @@ __device__ __forceinline__ void pick_bucket(const int* hist, bool descending, in
     *bucket_out = d;
 }
 
+// Block-wide radix select, 4 x 8-bit passes over the list entries e with take(e): the value digit(e) of the `*need`-th entry
+// counting from the top (descending) or the bottom; on return *need is its rank among the entries of that same value.
+template <bool kDescending, class Take, class Digit>
+__device__ __forceinline__ uint32_t radix_select(const uint2* list, int n, Take take, Digit digit, int* hist, int* need, int* bucket) {
+    uint32_t prefix = 0, mask = 0;
+    for (int pass = 0; pass < 4; ++pass) {
+        const int shift = 24 - 8 * pass;
+        if (threadIdx.x < 256) hist[threadIdx.x] = 0;
+        __syncthreads();
+        for (int i = threadIdx.x; i < n; i += kNmsThreads) {
+            const uint2 e = list[i];
+            const uint32_t v = digit(e);
+            if (take(e) && (v & mask) == prefix) atomicAdd(&hist[(v >> shift) & 255], 1);
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) pick_bucket(hist, kDescending, need, bucket);
+        __syncthreads();
+        prefix |= (uint32_t)*bucket << shift;
+        mask |= 255u << shift;
+    }
+    return prefix;
+}
+
+// Cross-warp half of a block-wide exclusive scan, entered after lane 0 of every warp has stored its warp's total in wsum[warp]
+// and the block has synchronised: warp 0 scans the 32 totals in place (and, with kTotal, stores the block total to *total);
+// after one barrier every thread returns its warp's offset.
+template <bool kTotal = true>
+__device__ __forceinline__ int block_scan_warp_offset(int* wsum, int* total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (warp == 0) {
+        int tot;
+        wsum[lane] = warp_excl_scan(wsum[lane], lane, &tot);
+        if (kTotal && lane == 0) *total = tot;
+    }
+    __syncthreads();
+    return wsum[warp];
+}
+
+// Packed 64-bit sort key class(16) | ~conf key(32) | stash position(16): ascending order = class asc, conf desc.
+__device__ __forceinline__ unsigned long long packed_key(int cls, float conf, int pos) {
+    return ((unsigned long long)(uint32_t)cls << 48) | ((unsigned long long)(uint32_t)(~float_key(conf)) << 16) | (uint32_t)pos;
+}
+// Block vote after a packed sort of M keys: does some (class, conf) occur twice?  Then the generic sort decides by (box[0], id).
+__device__ __forceinline__ bool packed_keys_tie(const unsigned long long* k64, int M) {
+    bool tie = false;
+    for (int i = threadIdx.x; i < M; i += kNmsThreads)
+        if (i > 0 && (k64[i] >> 16) == (k64[i - 1] >> 16)) tie = true;
+    return __syncthreads_or(tie ? 1 : 0) != 0;
+}
+
+// Block-wide bitonic network over n (a power of two) entries in shared memory, one barrier per step:
+// cx(i, ixj, up) puts the pair (i, ixj = i ^ j, ixj > i) in ascending order when up, descending otherwise.
+template <class CompareExchange>
+__device__ __forceinline__ void bitonic_smem(int n, CompareExchange cx) {
+    for (int k = 2; k <= n; k <<= 1) {
+        for (int jj = k >> 1; jj > 0; jj >>= 1) {
+            for (int i = threadIdx.x; i < n; i += kNmsThreads) {
+                const int ixj = i ^ jj;
+                if (ixj > i) cx(i, ixj, (i & k) == 0);
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// Greedy NMS of a 32-row chunk by one warp: `alive` = the rows still in, bit j of `mine` = row j of the chunk suppresses this
+// lane's row.  Visits surviving rows only (one ballot per kept row) and returns the kept rows.
+__device__ __forceinline__ unsigned resolve_chunk(unsigned alive, unsigned mine) {
+    for (unsigned rem = alive; rem != 0u;) {
+        const int jx = __ffs(rem) - 1;
+        alive &= ~__ballot_sync(0xffffffffu, (mine >> jx) & 1u);  // later rows that row jx suppresses
+        rem = alive & ~((2u << jx) - 1u);
+    }
+    return alive;
+}
+
 // Class ids are grouped and ordered as floats, like the reference's std::map<float, ...>: float_key(cls) (-0.0 == +0.0).
 // Only ids that are integers in [0, 65535] fit the packed 64-bit sort keys; any other id (negative, fractional, huge,
 // NaN) sends the image to the generic 128-bit sort, which keys on float_key.
@@ -260,26 +340,60 @@ __device__ __forceinline__ int seg_units(int m) {
     return G * (m - 1) - 4 * G * (G - 1);
 }
 
+// Dynamic shared memory of nms_kernel, in carve-up order.  Every array but the last holds a fixed number of bytes per row of
+// capacity S, so array x starts at byte S * NmsSmem::x; the last one, the tile count prefix of the fused path, holds
+// tiles_per_image + 1 ints, and 64 spare bytes follow it.
+struct NmsSmem {
+    static constexpr int u_box = 0;                                         // float4  stash in arrival order
+    static constexpr int s_box = u_box + sizeof(float4);                    // float4  sorted rows
+    static constexpr int k64 = s_box + sizeof(float4);                      // u64     64-bit sort keys (fast path)
+    static constexpr int u_conf = k64 + sizeof(unsigned long long);         // float
+    static constexpr int u_cls = u_conf + sizeof(float);                    // float   the source row's class float
+    static constexpr int u_id = u_cls + sizeof(float);                      // u32
+    static constexpr int s_conf = u_id + sizeof(uint32_t);                  // float
+    static constexpr int s_cls = s_conf + sizeof(float);                    // float
+    static constexpr int s_id = s_cls + sizeof(float);                      // u32
+    static constexpr int s_seg = s_id + sizeof(uint32_t);                   // int     short class segments (start<<16 | len)
+    static constexpr int s_long = s_seg + sizeof(int);                      // int     S/2 long class segments
+    static constexpr int s_pos = s_long + sizeof(int) / 2;                  // u16     slow path: stash position riding along
+    static constexpr int s_keep = s_pos + sizeof(unsigned short);           // u8      keep flags
+    static constexpr int s_unit = s_keep + 1;                               // u16 x 12 IoU work units (row << 4 | group of 8)
+    static constexpr int s_area = s_unit + sizeof(unsigned short) * (kShortSeg / 8);  // float  box areas (greedy mode)
+    static constexpr int s_tpre = s_area + sizeof(float);                   // int x (tiles_per_image + 1)
+    // row capacity S: a power of two >= pre_topk
+    __host__ __device__ static int rows(int pre_topk) { return pre_topk <= 1024 ? 1024 : kMaxSort; }
+    // what the launch reserves
+    __host__ __device__ static size_t bytes(int pre_topk, int tiles) {
+        return (size_t)rows(pre_topk) * s_tpre + sizeof(int) * (size_t)(tiles + 1) + 64;
+    }
+};
+// The array at per-row offset `to`, reached from the array `prev` at per-row offset `from` in prev's own element type: the
+// carve-up stays a chain of typed pointer steps, which nvcc keeps in fewer registers than independent byte offsets.
+template <class T, class P>
+__device__ __forceinline__ T* smem_after(P* prev, int S, int from, int to) {
+    return reinterpret_cast<T*>(prev + S * (to - from) / (int)sizeof(P));
+}
+
 __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_constant__ NmsArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    // carve-up (S = row capacity, power of two >= pre_topk)
-    const int S = a.pre_topk <= 1024 ? 1024 : kMaxSort;
-    float4* u_box = reinterpret_cast<float4*>(smem_raw);                         // S  stash in arrival order
-    float4* s_box = u_box + S;                                                   // S  sorted rows
-    unsigned long long* k64 = reinterpret_cast<unsigned long long*>(s_box + S);  // S  64-bit sort keys (fast path)
-    float* u_conf = reinterpret_cast<float*>(k64 + S);                           // S
-    float* u_cls = u_conf + S;                                                   // S   the source row's class float
-    uint32_t* u_id = reinterpret_cast<uint32_t*>(u_cls + S);                     // S
-    float* s_conf = reinterpret_cast<float*>(u_id + S);                          // S
-    float* s_cls = s_conf + S;                                                   // S
-    uint32_t* s_id = reinterpret_cast<uint32_t*>(s_cls + S);                     // S
-    int* s_seg = reinterpret_cast<int*>(s_id + S);                               // S   short class segments (start<<16 | len)
-    int* s_long = s_seg + S;                                                     // S/2 long class segments
-    unsigned short* s_pos = reinterpret_cast<unsigned short*>(s_long + S / 2);   // S   slow path: stash position riding along
-    unsigned char* s_keep = reinterpret_cast<unsigned char*>(s_pos + S);         // S   keep flags
-    unsigned short* s_unit = reinterpret_cast<unsigned short*>(s_keep + S);      // S*12 IoU work units (row << 4 | group of 8)
-    float* s_area = reinterpret_cast<float*>(s_unit + S * (kShortSeg / 8));      // S   box areas (greedy mode)
-    int* s_tpre = reinterpret_cast<int*>(s_area + S);                            // tiles_per_image + 1 (fused path)
+    // carve-up: the arrays of NmsSmem in order
+    const int S = NmsSmem::rows(a.pre_topk);
+    float4* u_box = reinterpret_cast<float4*>(smem_raw);
+    float4* s_box = smem_after<float4>(u_box, S, NmsSmem::u_box, NmsSmem::s_box);
+    unsigned long long* k64 = smem_after<unsigned long long>(s_box, S, NmsSmem::s_box, NmsSmem::k64);
+    float* u_conf = smem_after<float>(k64, S, NmsSmem::k64, NmsSmem::u_conf);
+    float* u_cls = smem_after<float>(u_conf, S, NmsSmem::u_conf, NmsSmem::u_cls);
+    uint32_t* u_id = smem_after<uint32_t>(u_cls, S, NmsSmem::u_cls, NmsSmem::u_id);
+    float* s_conf = smem_after<float>(u_id, S, NmsSmem::u_id, NmsSmem::s_conf);
+    float* s_cls = smem_after<float>(s_conf, S, NmsSmem::s_conf, NmsSmem::s_cls);
+    uint32_t* s_id = smem_after<uint32_t>(s_cls, S, NmsSmem::s_cls, NmsSmem::s_id);
+    int* s_seg = smem_after<int>(s_id, S, NmsSmem::s_id, NmsSmem::s_seg);
+    int* s_long = smem_after<int>(s_seg, S, NmsSmem::s_seg, NmsSmem::s_long);
+    unsigned short* s_pos = smem_after<unsigned short>(s_long, S, NmsSmem::s_long, NmsSmem::s_pos);
+    unsigned char* s_keep = smem_after<unsigned char>(s_pos, S, NmsSmem::s_pos, NmsSmem::s_keep);
+    unsigned short* s_unit = smem_after<unsigned short>(s_keep, S, NmsSmem::s_keep, NmsSmem::s_unit);
+    float* s_area = smem_after<float>(s_unit, S, NmsSmem::s_unit, NmsSmem::s_area);
+    int* s_tpre = smem_after<int>(s_area, S, NmsSmem::s_area, NmsSmem::s_tpre);
     unsigned short* s_krow = reinterpret_cast<unsigned short*>(u_box);  // kept rows of a long segment (the stash is dead after D)
     unsigned* s_mask = reinterpret_cast<unsigned*>(u_conf);  // 3 words per row: suppressor bitmaps (aliases u_conf/u_cls/u_id)
     int* s_rowseg = reinterpret_cast<int*>(k64);             // per row: segment start << 16 | length (aliases the sort keys)
@@ -306,17 +420,18 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
         s_n = 0;
         s_bad = 0;
     }
+    auto put = [&](int pos, const Row& r, uint32_t id) {  // row r into stash slot pos
+        const float c = a.class_aware ? r.cls : 0.0f;
+        u_box[pos] = r.box;
+        u_conf[pos] = r.conf;
+        u_cls[pos] = c;
+        u_id[pos] = id;
+        if (!packed_class(c)) s_bad = 1;  // class does not fit the packed 64-bit key: generic sort
+    };
     auto stash = [&](const Row& r, uint32_t id) {
         const int pos = atomicAdd(&s_n, 1);
         list[pos] = make_uint2(float_key(r.conf), id);  // only read back if more than pre_topk rows survive
-        if (pos < S) {
-            const float c = a.class_aware ? r.cls : 0.0f;
-            u_box[pos] = r.box;
-            u_conf[pos] = r.conf;
-            u_cls[pos] = c;
-            u_id[pos] = id;
-            if (!packed_class(c)) s_bad = 1;  // class does not fit the packed 64-bit key: generic sort
-        }
+        if (pos < S) put(pos, r, id);
     };
     if (a.from_tiles) {
         // prefix over the per-tile candidate counts, then one thread per candidate (binary search for its tile)
@@ -330,14 +445,8 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
             const int ex = warp_excl_scan(v, lane, &tot);
             if (lane == 0) s_wsum[warp] = tot;
             __syncthreads();
-            if (warp == 0) {
-                int w = s_wsum[lane], wt;
-                const int wex = warp_excl_scan(w, lane, &wt);
-                s_wsum[lane] = wex;
-                if (lane == 0) s_need = wt;
-            }
-            __syncthreads();
-            if (t < T) s_tpre[t] = carry + s_wsum[warp] + ex;
+            const int wex = block_scan_warp_offset(s_wsum, &s_need);
+            if (t < T) s_tpre[t] = carry + wex + ex;
             carry += s_need;
             __syncthreads();
         }
@@ -376,54 +485,13 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
 
     // ---------------- B: radix select when more than pre_topk rows survive (rare) ----------------
     if (n_valid > a.pre_topk) {
-        uint32_t key_cut = 0, id_cut = 0xffffffffu;  // take key > key_cut, or key == key_cut && id <= id_cut
-        uint32_t prefix = 0, mask = 0;
+        // keep the pre_topk largest conf keys, ties at the cut to the smaller ids: key > key_cut, or key == key_cut && id <= id_cut
         if (tid == 0) s_need = a.pre_topk;
-        for (int pass = 0; pass < 4; ++pass) {
-            const int shift = 24 - 8 * pass;
-            if (tid < 256) s_hist[tid] = 0;
-            __syncthreads();
-            for (int i = tid; i < n_valid; i += kNmsThreads) {
-                uint32_t k = list[i].x;
-                if ((k & mask) == prefix) atomicAdd(&s_hist[(k >> shift) & 255], 1);
-            }
-            __syncthreads();
-            if (tid == 0) {
-                int need = s_need, d;
-                pick_bucket(s_hist, true, &need, &d);
-                s_need = need;
-                s_bucket = d;
-            }
-            __syncthreads();
-            prefix |= (uint32_t)s_bucket << shift;
-            mask |= 255u << shift;
-        }
-        key_cut = prefix;
-        const int need_eq = s_need;  // how many rows with key == key_cut are taken
-        uint32_t ip = 0, im = 0;     // ties at the cut: take the need_eq smallest ids
-        __syncthreads();
-        if (tid == 0) s_need = need_eq;
-        for (int pass = 0; pass < 4; ++pass) {
-            const int shift = 24 - 8 * pass;
-            if (tid < 256) s_hist[tid] = 0;
-            __syncthreads();
-            for (int i = tid; i < n_valid; i += kNmsThreads) {
-                uint2 e = list[i];
-                if (e.x == key_cut && (e.y & im) == ip) atomicAdd(&s_hist[(e.y >> shift) & 255], 1);
-            }
-            __syncthreads();
-            if (tid == 0) {
-                int need = s_need, d;
-                pick_bucket(s_hist, false, &need, &d);
-                s_need = need;
-                s_bucket = d;
-            }
-            __syncthreads();
-            ip |= (uint32_t)s_bucket << shift;
-            im |= 255u << shift;
-        }
-        id_cut = ip;
-        // re-stash exactly the selected rows
+        const uint32_t key_cut = radix_select<true>(
+            list, n_valid, [](uint2) { return true; }, [](uint2 e) { return e.x; }, s_hist, &s_need, &s_bucket);
+        const uint32_t id_cut = radix_select<false>(
+            list, n_valid, [key_cut](uint2 e) { return e.x == key_cut; }, [](uint2 e) { return e.y; }, s_hist, &s_need, &s_bucket);
+        // re-stash exactly the selected rows (list[] is not written: other threads are still reading it)
         if (tid == 0) {
             s_n = 0;
             s_bad = 0;
@@ -431,16 +499,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
         __syncthreads();
         for (int i = tid; i < n_valid; i += kNmsThreads) {
             const uint2 e = list[i];
-            if (e.x > key_cut || (e.x == key_cut && e.y <= id_cut)) {
-                const Row r = fetch_row(a, b, e.y);
-                const int pos = atomicAdd(&s_n, 1);
-                const float c = a.class_aware ? r.cls : 0.0f;
-                u_box[pos] = r.box;
-                u_conf[pos] = r.conf;
-                u_cls[pos] = c;
-                u_id[pos] = e.y;
-                if (!packed_class(c)) s_bad = 1;
-            }
+            if (e.x > key_cut || (e.x == key_cut && e.y <= id_cut)) put(atomicAdd(&s_n, 1), fetch_row(a, b, e.y), e.y);
         }
         __syncthreads();
     }
@@ -479,18 +538,11 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
         const int ex = warp_excl_scan(h, lane, &tot);
         if (lane == 0) s_wsum[warp] = tot;
         if (!__syncthreads_or(big || h > kMaxBucket ? 1 : 0)) {
-            if (warp == 0) {
-                int w = s_wsum[lane], wt;
-                const int wex = warp_excl_scan(w, lane, &wt);
-                s_wsum[lane] = wex;
-            }
-            __syncthreads();
-            s_cstart[tid] = s_wsum[warp] + ex;
+            s_cstart[tid] = block_scan_warp_offset<false>(s_wsum, nullptr) + ex;
             __syncthreads();
             for (int i = tid; i < M; i += kNmsThreads) {
                 const int c = (int)u_cls[i];
-                kb[s_cstart[c] + s_pos[i]] =
-                    ((unsigned long long)(uint32_t)c << 48) | ((unsigned long long)(uint32_t)(~float_key(u_conf[i])) << 16) | (uint32_t)i;
+                kb[s_cstart[c] + s_pos[i]] = packed_key(c, u_conf[i], i);
             }
             __syncthreads();
             // thread p owns bucket slot p: neighbouring lanes share a bucket, so the key reads below are broadcasts
@@ -504,17 +556,12 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
                 k64[s0 + rank] = mk;
             }
             __syncthreads();
-            bool tie = false;  // same (class, conf) twice: the generic sort decides by (box[0], id)
-            for (int i = tid; i < M; i += kNmsThreads)
-                if (i > 0 && (k64[i] >> 16) == (k64[i - 1] >> 16)) tie = true;
-            generic = __syncthreads_or(tie ? 1 : 0) != 0;
+            generic = packed_keys_tie(k64, M);
             bucketed = !generic;
         }
     }
     if (!generic && !bucketed) {
-        for (int i = tid; i < S_eff; i += kNmsThreads)
-            k64[i] = i < M ? ((unsigned long long)(uint32_t)(int)u_cls[i] << 48) | ((unsigned long long)(uint32_t)(~float_key(u_conf[i])) << 16) | (uint32_t)i
-                           : ~0ull;
+        for (int i = tid; i < S_eff; i += kNmsThreads) k64[i] = i < M ? packed_key((int)u_cls[i], u_conf[i], i) : ~0ull;
         __syncthreads();
         if (S_eff <= kNmsThreads) {
             // one key per thread in registers; shuffles for partner distance < 32, smem ping-pong otherwise
@@ -540,26 +587,15 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
             if (tid < S_eff) k64[tid] = mk;
             __syncthreads();
         } else {
-            for (int k = 2; k <= S_eff; k <<= 1) {
-                for (int jj = k >> 1; jj > 0; jj >>= 1) {
-                    for (int i = tid; i < S_eff; i += kNmsThreads) {
-                        const int ixj = i ^ jj;
-                        if (ixj > i) {
-                            const unsigned long long x = k64[i], y = k64[ixj];
-                            if ((x > y) == ((i & k) == 0)) {
-                                k64[i] = y;
-                                k64[ixj] = x;
-                            }
-                        }
-                    }
-                    __syncthreads();
+            bitonic_smem(S_eff, [&](int i, int ixj, bool up) {
+                const unsigned long long x = k64[i], y = k64[ixj];
+                if ((x > y) == up) {
+                    k64[i] = y;
+                    k64[ixj] = x;
                 }
-            }
+            });
         }
-        bool tie = false;
-        for (int i = tid; i < M; i += kNmsThreads)
-            if (i > 0 && (k64[i] >> 16) == (k64[i - 1] >> 16)) tie = true;
-        generic = __syncthreads_or(tie ? 1 : 0) != 0;
+        generic = packed_keys_tie(k64, M);
     }
     if (generic) {
         for (int i = tid; i < S_eff; i += kNmsThreads) {
@@ -573,27 +609,19 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
             s_pos[i] = (unsigned short)i;
         }
         __syncthreads();
-        for (int k = 2; k <= S_eff; k <<= 1) {
-            for (int jj = k >> 1; jj > 0; jj >>= 1) {
-                for (int i = tid; i < S_eff; i += kNmsThreads) {
-                    const int ixj = i ^ jj;
-                    if (ixj > i) {
-                        const unsigned long long ah = k_hi[i], al = k_lo[i], bh = k_hi[ixj], bl = k_lo[ixj];
-                        const bool gt = ah > bh || (ah == bh && al > bl);
-                        if (gt == ((i & k) == 0)) {
-                            k_hi[i] = bh;
-                            k_lo[i] = bl;
-                            k_hi[ixj] = ah;
-                            k_lo[ixj] = al;
-                            const unsigned short t0 = s_pos[i];
-                            s_pos[i] = s_pos[ixj];
-                            s_pos[ixj] = t0;
-                        }
-                    }
-                }
-                __syncthreads();
+        bitonic_smem(S_eff, [&](int i, int ixj, bool up) {
+            const unsigned long long ah = k_hi[i], al = k_lo[i], bh = k_hi[ixj], bl = k_lo[ixj];
+            const bool gt = ah > bh || (ah == bh && al > bl);
+            if (gt == up) {
+                k_hi[i] = bh;
+                k_lo[i] = bl;
+                k_hi[ixj] = ah;
+                k_lo[ixj] = al;
+                const unsigned short t0 = s_pos[i];
+                s_pos[i] = s_pos[ixj];
+                s_pos[ixj] = t0;
             }
-        }
+        });
         for (int i = tid; i < M; i += kNmsThreads) k64[i] = s_pos[i];  // permutation in the low 16 bits, like the fast path
         __syncthreads();  // the 128-bit keys (in the sorted-row area) are dead from here on
     }
@@ -611,8 +639,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
         const int pos = (int)(k64[i] & 0xffffull);
         const float4 bx = u_box[pos];
         if (a.box_format == TRTX_BOX_OBB) {  // covariance of the row's Gaussian, once per row; the angle is the first extra float
-            const float ang = a.rows[(size_t)b * (1 + (size_t)a.max_rows * a.det_floats) + 1 + (size_t)u_id[pos] * a.det_floats +
-                                     a.extra_offset];
+            const float ang = plugin_row(a, b, u_id[pos])[a.extra_offset];
             float ca, cb, cc;
             if (greedy)
                 obb_cov_host(bx.z, bx.w, ang, ca, cb, cc);
@@ -652,35 +679,34 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
 
     if (greedy) {
         // ---------------- E: class segments ----------------
+        // segment of m >= 1 rows from sorted row p0 (M <= 2048: start and length fit 16 bits): long ones are handled by the
+        // whole CTA, medium ones are taken first (longest-first scheduling), and one of 2..kShortSeg rows reserves its
+        // IoU work units, whose base goes to s_pos[p0]
+        auto file_segment = [&](int p0, int m) {
+            if (m > kShortSeg)
+                s_long[atomicAdd(&s_nlong, 1)] = (p0 << 16) | m;
+            else if (m > 32)
+                s_seg[S - 1 - atomicAdd(&s_nmed, 1)] = (p0 << 16) | m;
+            else
+                s_seg[atomicAdd(&s_nshort, 1)] = (p0 << 16) | m;
+            if (m > 1 && m <= kShortSeg) s_pos[p0] = (unsigned short)atomicAdd(&s_nunit, seg_units(m));
+        };
+        // every row learns its segment (start << 16 | length; 0 = long segment)
         if (bucketed) {
             // the class histogram already is the segment table
             for (int i = tid; i < M; i += kNmsThreads) {
                 const int c = (int)s_cls[i], m = s_chist[c];
                 s_rowseg[i] = m > kShortSeg ? 0 : ((s_cstart[c] << 16) | m);
             }
-            const int m = s_chist[tid], p0 = s_cstart[tid];
-            if (m > kShortSeg)
-                s_long[atomicAdd(&s_nlong, 1)] = (p0 << 16) | m;
-            else if (m > 32)
-                s_seg[S - 1 - atomicAdd(&s_nmed, 1)] = (p0 << 16) | m;
-            else if (m > 0)
-                s_seg[atomicAdd(&s_nshort, 1)] = (p0 << 16) | m;
-            if (m > 1 && m <= kShortSeg) s_pos[p0] = (unsigned short)atomicAdd(&s_nunit, seg_units(m));
+            if (s_chist[tid] > 0) file_segment(s_cstart[tid], s_chist[tid]);
         } else
         for (int i = tid; i < M; i += kNmsThreads) {
             if (i == 0 || !same_class(s_cls[i], s_cls[i - 1])) {
                 int e = i + 1;
                 while (e < M && same_class(s_cls[e], s_cls[i])) ++e;
                 const int m = e - i;
-                // every row learns its segment (start << 16 | length; 0 = long segment, handled by the whole CTA)
                 for (int r = i; r < e; ++r) s_rowseg[r] = m > kShortSeg ? 0 : ((i << 16) | m);
-                if (m > kShortSeg)
-                    s_long[atomicAdd(&s_nlong, 1)] = (i << 16) | m;  // M <= 2048: start and length fit 16 bits
-                else if (m > 32)
-                    s_seg[S - 1 - atomicAdd(&s_nmed, 1)] = (i << 16) | m;  // medium segments: taken first (longest-first scheduling)
-                else
-                    s_seg[atomicAdd(&s_nshort, 1)] = (i << 16) | m;
-                if (m > 1 && m <= kShortSeg) s_pos[i] = (unsigned short)atomicAdd(&s_nunit, seg_units(m));
+                file_segment(i, m);
             }
         }
         __syncthreads();
@@ -709,14 +735,8 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
                 }
                 __syncthreads();
                 if (warp == 0) {
-                    const unsigned my = s_sup[lane];
-                    unsigned alive = ~s_rem & (nchunk == 32 ? 0xffffffffu : ((1u << nchunk) - 1u));
-                    for (unsigned rem = alive; rem != 0u;) {
-                        const int jx = __ffs(rem) - 1;
-                        const unsigned kill = __ballot_sync(0xffffffffu, (my >> jx) & 1u);
-                        alive &= ~kill;
-                        rem = alive & ~((2u << jx) - 1u);
-                    }
+                    const unsigned alive =
+                        resolve_chunk(~s_rem & (nchunk == 32 ? 0xffffffffu : ((1u << nchunk) - 1u)), s_sup[lane]);
                     if ((alive >> lane) & 1u) {
                         const int pos = n_kept + __popc(alive & ((1u << lane) - 1u));
                         s_krow[pos] = (unsigned short)(p0 + c0 + lane);
@@ -793,14 +813,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
                 bool removed = false;
 #pragma unroll
                 for (int w = 0; w < c; ++w) removed |= (mw[w] & kept[w]) != 0u;  // suppressed by a kept row of an earlier chunk
-                unsigned alive = __ballot_sync(0xffffffffu, in && !removed);
-                const unsigned mymask = mw[c];
-                for (unsigned rem = alive; rem != 0u;) {  // visit surviving rows only: one ballot per kept row
-                    const int jx = __ffs(rem) - 1;
-                    const unsigned kill = __ballot_sync(0xffffffffu, (mymask >> jx) & 1u);  // later rows that row jx suppresses
-                    alive &= ~kill;
-                    rem = alive & ~((2u << jx) - 1u);
-                }
+                const unsigned alive = resolve_chunk(__ballot_sync(0xffffffffu, in && !removed), mw[c]);
                 kept[c] = alive;
                 if ((alive >> lane) & 1u) s_keep[row] = 1;
             }
@@ -834,14 +847,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
         const unsigned bal = __ballot_sync(0xffffffffu, emit);
         if (lane == 0) s_wsum[warp] = __popc(bal);
         __syncthreads();
-        if (warp == 0) {
-            int v = s_wsum[lane], tot;
-            const int ex = warp_excl_scan(v, lane, &tot);
-            s_wsum[lane] = ex;
-            if (lane == 0) s_nkept = tot;
-        }
-        __syncthreads();
-        const int k = carry + s_wsum[warp] + __popc(bal & ((1u << lane) - 1u));
+        const int k = carry + block_scan_warp_offset(s_wsum, &s_nkept) + __popc(bal & ((1u << lane) - 1u));
         if (emit && k < a.max_det) {
             // rows that were turned into corners / covariances for the overlap tests are emitted as they came in
             const float4 bx = a.box_format == TRTX_BOX_OBB || (greedy && a.box_format == TRTX_BOX_CXCYWH)
@@ -858,8 +864,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
             if (oidx) oidx[k] = a.from_tiles ? __float_as_int(a.cand[2 * ((size_t)b * a.slots_per_image + s_id[i]) + 1].z)
                                              : (int)s_id[i];
             if (a.extra_floats && !a.from_tiles) {
-                const float* src = a.rows + (size_t)b * (1 + (size_t)a.max_rows * a.det_floats) + 1 +
-                                   (size_t)s_id[i] * a.det_floats + a.extra_offset;
+                const float* src = plugin_row(a, b, s_id[i]) + a.extra_offset;
                 for (int e = 0; e < a.extra_floats; ++e) row[7 + e] = src[e];
             }
         }
@@ -972,11 +977,6 @@ __global__ void __launch_bounds__(64) gather_publish_kernel(NmsArgs::Gather g, i
     st_relaxed_sys(g.flags[p] + fi, v);
 }
 
-static size_t nms_smem_bytes(int pre_topk, int tiles = 0) {
-    const size_t S = pre_topk <= 1024 ? 1024 : kMaxSort;
-    return S * (16 + 16 + 8 + 6 * 4 + 4 + 2 + 2 + 1 + 2 * (kShortSeg / 8) + 4) + 64 + sizeof(int) * (size_t)(tiles + 1);
-}
-
 static int nms_validate(const trtx_nms_params* q) {
     if (!q) return TRTX_ERR_INVALID;
     if (q->box_format < 0 || q->box_format > TRTX_BOX_OBB) return TRTX_ERR_INVALID;
@@ -991,7 +991,7 @@ static int nms_launch(NmsArgs& a, int batch, cudaStream_t st) {
     a.dbg = t_nms_stamps;
 #endif
     if (a.pre_topk > kMaxSort) return TRTX_ERR_UNSUPPORTED;
-    const size_t smem = nms_smem_bytes(a.pre_topk, a.from_tiles ? a.tiles_per_image : 0);
+    const size_t smem = NmsSmem::bytes(a.pre_topk, a.from_tiles ? a.tiles_per_image : 0);
     // 227 KB per CTA minus the kernel's static shared memory (histograms, ~18 KB)
     constexpr size_t kMaxDynSmem = (227 - 20) * 1024;
     if (smem > kMaxDynSmem) return TRTX_ERR_UNSUPPORTED;
@@ -1015,6 +1015,21 @@ TRTX_API int trtx_probe_set_nms_stamps(void* p) {
 }
 #endif
 
+// NMS arguments taken from trtx_nms_params as they are; the row source, pre_topk, extras and gather are the caller's
+static NmsArgs nms_args(const trtx_nms_params* q, float* compact_out_dev, int32_t* keep_index_dev) {
+    NmsArgs a{};
+    a.box_format = q->box_format;
+    a.mode = q->mode;
+    a.class_aware = q->class_aware;
+    a.tie_break_x0 = q->tie_break_x0;
+    a.conf_thresh = q->conf_thresh;
+    a.nms_thresh = q->nms_thresh;
+    a.max_det = q->max_det;
+    a.out = compact_out_dev;
+    a.keep_index = keep_index_dev;
+    return a;
+}
+
 TRTX_API size_t trtx_nms_workspace_size(const trtx_nms_params* p, int batch, int max_rows) {
     if (nms_validate(p) || batch <= 0 || max_rows <= 0) return 0;
     return align_up(sizeof(uint2) * (size_t)batch * max_rows);
@@ -1030,25 +1045,17 @@ TRTX_API int trtx_nms_enqueue(const trtx_nms_params* p, int batch, const float* 
     if (p->extra_floats && p->extra_offset + p->extra_floats > det_floats) return TRTX_ERR_INVALID;
     if (p->box_format != TRTX_BOX_RETINA && det_floats < 6) return TRTX_ERR_INVALID;
     if (workspace_bytes < trtx_nms_workspace_size(p, batch, max_rows)) return TRTX_ERR_WORKSPACE;
-    NmsArgs a{};
+    NmsArgs a = nms_args(p, compact_out_dev, keep_index_dev);
     a.rows = plugin_out_dev;
     a.max_rows = max_rows;
     a.det_floats = det_floats;
     a.from_tiles = 0;
     a.list = static_cast<uint2*>(workspace_dev);
     a.list_stride = max_rows;
-    a.box_format = p->box_format;
-    a.mode = p->mode;
-    a.class_aware = p->class_aware && p->box_format != TRTX_BOX_RETINA;
-    a.tie_break_x0 = p->tie_break_x0;
-    a.conf_thresh = p->conf_thresh;
-    a.nms_thresh = p->nms_thresh;
+    a.class_aware = p->class_aware && p->box_format != TRTX_BOX_RETINA;  // RetinaFace rows carry no class
     a.pre_topk = max_rows < kMaxSort ? max_rows : kMaxSort;
-    a.max_det = p->max_det;
     a.extra_floats = p->extra_floats;
     a.extra_offset = p->extra_offset;
-    a.out = compact_out_dev;
-    a.keep_index = keep_index_dev;
     return nms_launch(a, batch, static_cast<cudaStream_t>(stream));
 }
 
@@ -1076,7 +1083,7 @@ static int yolo_nms_tiles(const trtx_yolo_params* p, const trtx_nms_params* q, i
                           const YoloLayout& L, float* compact_out_dev, int32_t* keep_index_dev, void* workspace_dev,
                           cudaStream_t st, const trtx_gather* gather = nullptr) {
     if (q->box_format == TRTX_BOX_OBB) return TRTX_ERR_UNSUPPORTED;  // the tile records carry no angle: use the plugin-row source
-    NmsArgs a{};
+    NmsArgs a = nms_args(q, compact_out_dev, keep_index_dev);
     a.from_tiles = 1;
     a.tiles_per_image = L.tiles_per_image;
     a.slots_per_image = L.slots_per_image;
@@ -1090,34 +1097,35 @@ static int yolo_nms_tiles(const trtx_yolo_params* p, const trtx_nms_params* q, i
     a.cand = ya.cand;
     a.list = reinterpret_cast<uint2*>(static_cast<char*>(workspace_dev) + L.off_list);
     a.list_stride = L.slots_per_image;
-    a.box_format = q->box_format;
-    a.mode = q->mode;
-    a.class_aware = q->class_aware;
-    a.tie_break_x0 = q->tie_break_x0;
-    a.conf_thresh = q->conf_thresh;
-    a.nms_thresh = q->nms_thresh;
     a.pre_topk = p->max_out;  // the reference's plugin capacity bounds what reaches nms()
-    a.max_det = q->max_det;
-    a.out = compact_out_dev;
-    a.keep_index = keep_index_dev;
     const int rc = fill_gather(gather, &a.g);
     if (rc) return rc;
     return nms_launch(a, batch, st);
+}
+
+// Checks of the fused YOLO + NMS entries, in this order: the NMS parameters, the output buffer (and the gather descriptor
+// when the entry needs one), no extras (they need the plugin-format rows: use the two-stage path), the scan's arguments and
+// workspace (filling ya and L), the NMS row capacity.
+static int yolo_nms_prologue(const trtx_yolo_params* p, const trtx_nms_params* q, int batch, const void* const* inputs_dev,
+                             float* compact_out_dev, bool gather_missing, void* workspace_dev, size_t workspace_bytes,
+                             YoloArgs* ya, YoloLayout* L) {
+    int rc = nms_validate(q);
+    if (rc) return rc;
+    if (!compact_out_dev || gather_missing) return TRTX_ERR_INVALID;
+    if (q->extra_floats) return TRTX_ERR_UNSUPPORTED;
+    rc = yolo_fill_args(p, batch, inputs_dev, workspace_dev, workspace_bytes, ya, L);
+    if (rc) return rc;
+    return p->max_out > kMaxSort ? TRTX_ERR_UNSUPPORTED : TRTX_OK;
 }
 
 TRTX_API int trtx_yolo_decode_nms_enqueue(const trtx_yolo_params* p, const trtx_nms_params* q, int batch,
                                           const void* const* inputs_dev, float* compact_out_dev,
                                           int32_t* keep_index_dev, void* workspace_dev, size_t workspace_bytes,
                                           trtx_stream_t stream) {
-    int rc = nms_validate(q);
-    if (rc) return rc;
-    if (!compact_out_dev) return TRTX_ERR_INVALID;
-    if (q->extra_floats) return TRTX_ERR_UNSUPPORTED;  // extras need the plugin-format rows (use the two-stage path)
     YoloArgs ya;
     YoloLayout L;
-    rc = yolo_fill_args(p, batch, inputs_dev, workspace_dev, workspace_bytes, &ya, &L);
+    int rc = yolo_nms_prologue(p, q, batch, inputs_dev, compact_out_dev, false, workspace_dev, workspace_bytes, &ya, &L);
     if (rc) return rc;
-    if (p->max_out > kMaxSort) return TRTX_ERR_UNSUPPORTED;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     rc = yolo_scan_launch(ya, L, p->in_dtype, batch, st);
     if (rc) return rc;
@@ -1128,15 +1136,10 @@ TRTX_API int trtx_yolo_decode_nms_gather_enqueue(const trtx_yolo_params* p, cons
                                                  const void* const* inputs_dev, float* compact_out_dev, int32_t* keep_index_dev,
                                                  void* workspace_dev, size_t workspace_bytes, const trtx_gather* gather,
                                                  trtx_stream_t stream) {
-    int rc = nms_validate(q);
-    if (rc) return rc;
-    if (!compact_out_dev || !gather) return TRTX_ERR_INVALID;
-    if (q->extra_floats) return TRTX_ERR_UNSUPPORTED;
     YoloArgs ya;
     YoloLayout L;
-    rc = yolo_fill_args(p, batch, inputs_dev, workspace_dev, workspace_bytes, &ya, &L);
+    int rc = yolo_nms_prologue(p, q, batch, inputs_dev, compact_out_dev, !gather, workspace_dev, workspace_bytes, &ya, &L);
     if (rc) return rc;
-    if (p->max_out > kMaxSort) return TRTX_ERR_UNSUPPORTED;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     rc = yolo_scan_launch(ya, L, p->in_dtype, batch, st);
     if (rc) return rc;
@@ -1224,15 +1227,10 @@ TRTX_API int trtx_yolo_nms_after_scan_enqueue(const trtx_yolo_params* p, const t
                                               const void* const* inputs_dev, float* compact_out_dev,
                                               int32_t* keep_index_dev, void* workspace_dev, size_t workspace_bytes,
                                               trtx_stream_t stream) {
-    int rc = nms_validate(q);
-    if (rc) return rc;
-    if (!compact_out_dev) return TRTX_ERR_INVALID;
-    if (q->extra_floats) return TRTX_ERR_UNSUPPORTED;
     YoloArgs ya;
     YoloLayout L;
-    rc = yolo_fill_args(p, batch, inputs_dev, workspace_dev, workspace_bytes, &ya, &L);
+    const int rc = yolo_nms_prologue(p, q, batch, inputs_dev, compact_out_dev, false, workspace_dev, workspace_bytes, &ya, &L);
     if (rc) return rc;
-    if (p->max_out > kMaxSort) return TRTX_ERR_UNSUPPORTED;
     return yolo_nms_tiles(p, q, batch, ya, L, compact_out_dev, keep_index_dev, workspace_dev,
                           static_cast<cudaStream_t>(stream));
 }
