@@ -50,7 +50,8 @@ TRTX_API int trtx_last_cuda_error(void);
 /* sizeof() of the parameter structs as THIS library was compiled, so that an FFI binding (ctypes, cgo, ...) can check its
  * mirror of the layout: which = 0 trtx_yolo_params, 1 trtx_nms_params, 2 trtx_retina_params, 3 trtx_image_desc,
  * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_frame, 7 trtx_pose_obb_params, 8 trtx_frame,
- * 9 trtx_face_post_params, 10 trtx_yolop_post_params, 11 trtx_detr_post_params; anything else 0. */
+ * 9 trtx_face_post_params, 10 trtx_yolop_post_params, 11 trtx_detr_post_params, 12 trtx_centernet_params;
+ * anything else 0. */
 TRTX_API size_t trtx_abi_sizeof(int which);
 
 /* =====================================================================================
@@ -805,6 +806,66 @@ typedef struct trtx_detr_post_params {
 TRTX_API int trtx_detr_postprocess_enqueue(const trtx_detr_post_params* p, const int32_t* frame_wh_host, int batch,
                                            const float* scores_dev, const float* boxes_dev, float* rows_dev,
                                            trtx_stream_t stream);
+
+/* =====================================================================================
+ * 11. CenterNet pre-process and decode
+ *    replaces the HOST stages of centernet/sample/test.py (ctdet_coco_dla_2x): pre_process (:34-41) and the H2D copy of its
+ *    input, and after inference the D2H copy of hm, wh and reg, ctdet_decode (:44-102) and the driver loop (:126-132).
+ *    The DCNv2 plugin of the backbone is not part of this library.
+ * ===================================================================================== */
+/* pre_process for a whole batch, one launch per <= 64 images: images_host = `batch` u8 HWC BGR descriptors in HOST memory
+ * (trtx_image_desc, any pitch and base alignment, mixed sizes allowed); dst_dev = [batch, 3, net, net] fp32 planes in the
+ * frame's B, G, R order (the sample feeds cv.imread's BGR through transpose(2, 0, 1)), the engine input (net = 512).
+ * Per frame: L = max(h, w, 3) (max(image.shape) includes the channel count); a float64 L x L zero canvas holds the frame at
+ * its top-left; cv.resize(canvas, (net, net)) is OpenCV 4.x's INTER_LINEAR on float64, bit for bit: separable, weights
+ * (1 - fx, fx) in float from fx = (float)((d + 0.5) * scale - 0.5) - floor, the tap clamped with fx = 0 at both ends of both
+ * axes, each pass a0 * p0 + a1 * p1 in double; then (float)(((v / 255.) - 0.5) / 0.5) in double (the padding is -1.0f).
+ * Defined where the sample raises: for 1 < w < L its `img[:h, :L] = image` fails, and the frame is placed at the top-left
+ * with zeros elsewhere, the sample's evident intent; a frame with w == 1 fills every column of its rows, as numpy
+ * broadcasts it there.  Every descriptor is checked before the first launch (a rejected call writes nothing):
+ * TRTX_ERR_INVALID for a null pointer, batch / net <= 0, pitch < 3 * width or a dst_dev that is not 4-byte aligned;
+ * TRTX_ERR_UNSUPPORTED for net > 8192.  No workspace; can be captured in a CUDA graph. */
+TRTX_API int trtx_centernet_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net, float* dst_dev,
+                                               trtx_stream_t stream);
+
+typedef struct trtx_centernet_params {
+    int32_t num_classes;  /* C: 80 */
+    int32_t height, width; /* H, W of the heads: 128 x 128 */
+    int32_t k;            /* K: 100, ctdet_decode's default */
+    int32_t net;          /* frame rows only: the input side, 512 */
+    int32_t down;         /* frame rows only: the heads' stride, 4 */
+    float score_thresh;   /* frame rows only: 0.5f */
+} trtx_centernet_params;
+
+/* Workspace of trtx_centernet_decode_enqueue: 8 * B * C * K bytes (two 256-byte aligned halves); 0 for rejected params. */
+TRTX_API size_t trtx_centernet_workspace_size(const trtx_centernet_params* p, int batch);
+
+/* ctdet_decode(hm, wh, reg, K) for a batch: heat_dev [B, C, H, W], wh_dev [B, 2, H, W], reg_dev [B, 2, H, W], all fp32 (the
+ * engine outputs hm, wh, reg) -> dets_dev [B, K, 6] fp32 (x1, y1, x2, y2, score, class) in map units.  Per image:
+ *   1. s = 1 / (1 + expf(-x)) (the reference's CPU sigmoid may differ by a few ulps);
+ *   2. a cell is a peak iff s equals the max of s over its 3 x 3 window clipped to the map (max_pool2d pads with -inf); the
+ *      suppressed value is s at a peak and +0 elsewhere; a NaN in the window makes the max NaN, so the cell is no peak, and
+ *      a NaN cell stays NaN; a saturated plateau (s == 1.0f) is a peak in every cell;
+ *   3. the K largest suppressed values over all C * H * W cells, ordered NaN first, then by descending value, ties to the
+ *      smaller flat index c * H * W + y * W + x.  This is the reference's two-stage topk under that order (a cell outside
+ *      its class's top K has K cells above it); the reference's order among ties is implementation-defined, this one is not.  With
+ *      fewer than K positive or NaN cells the rest are zero-valued cells in flat-index order;
+ *   4. class = c, xs = x + reg[0, y, x], ys = y + reg[1, y, x], x1 = xs - wh[0] / 2, y1 = ys - wh[1] / 2, x2 = xs + wh[0] / 2,
+ *      y2 = ys + wh[1] / 2, all float without contraction.  The accepted sizes keep the reference's float index divisions
+ *      (true_divide(width), true_divide(K)) equal to integer divisions.
+ * Frame rows (the driver loop), when frame_wh_host (`batch` pairs img_w, img_h in HOST memory) and rows_dev are both given:
+ * rows_dev [B, 1 + K * 6] gets the count n of detections with score > score_thresh (a NaN score is dropped), then those
+ * rows in order as (x1 * k, y1 * k, x2 * k, y2 * k, score, class), zeros past n, with k = (float)(down * (L / (double)net)),
+ * L = max(img_h, img_w, 3) -- `i[:4] *= 4*s`, each product rounded once; int(), rectangles and text stay with the caller.
+ * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer, batch,
+ * C, H, W or K <= 0, K > H * W (the reference's topk raises), only one of frame_wh_host / rows_dev, and with rows a net or down <= 0,
+ * a NaN score_thresh or a frame size <= 0; TRTX_ERR_WORKSPACE for a short workspace; TRTX_ERR_INVALID for a workspace that is
+ * not 256-byte aligned; TRTX_ERR_UNSUPPORTED for C > 1024, H or W > 1024, H * W > 2^20 or K > 1024.  Two launches per call
+ * (one more per 64 frames past the first 64), no host sync, no allocation; can be captured in a CUDA graph. */
+TRTX_API int trtx_centernet_decode_enqueue(const trtx_centernet_params* p, int batch, const float* heat_dev,
+                                           const float* wh_dev, const float* reg_dev, void* workspace_dev,
+                                           size_t workspace_bytes, float* dets_dev, const int32_t* frame_wh_host,
+                                           float* rows_dev, trtx_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -10,6 +10,7 @@ import hashlib
 import os
 import shutil
 import subprocess
+import sys
 from pathlib import Path
 
 PKG = Path(__file__).resolve().parent
@@ -19,7 +20,7 @@ LIBDIR = PKG / "lib"
 LIB = LIBDIR / "libtrtx_hot.so"
 
 SOURCES = ["yolo_decode.cu", "nms.cu", "retina_decode.cu", "rcnn.cu", "preprocess.cu", "mask.cu", "roi_align.cu", "calib_host.cu", "cls.cu",
-           "detr.cu"]
+           "detr.cu", "centernet.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -86,15 +87,13 @@ def build(force: bool = False, verbose: bool = False, probe: bool = False) -> Pa
 
 def build_oracle() -> Path:
     """Compile the CPU oracles (test infrastructure) and, when /root/reference exists, oracle/_ref."""
-    for makefile in ("Makefile", "yolop.mk", "detr.mk"):
-        r = subprocess.run(["make", "-C", str(ROOT / "oracle"), "-f", makefile], stdout=subprocess.PIPE, stderr=subprocess.STDOUT,
-                           text=True)
+    for makefile in ("Makefile", "yolop.mk", "detr.mk", "centernet.mk"):
+        r = subprocess.run(["make", "-C", str(ROOT / "oracle"), "-f", makefile, f"PYTHON={sys.executable}"],
+                           stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"oracle build failed ({makefile}):\n{r.stdout}")
     return ROOT / "oracle" / "libtrtx_oracle.so"
 
 
 if __name__ == "__main__":
-    import sys
-
     print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))

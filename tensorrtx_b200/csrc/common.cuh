@@ -94,11 +94,13 @@ __device__ __forceinline__ uint32_t float_key(float f) {
 // only floating-point step of that resize, shared by the host calibrator (calib_host.cu) and the R-CNN pre-process kernel
 // (preprocess.cu).  The device spells the double expression with _rn intrinsics: left to itself nvcc may contract it into
 // a DFMA, which rounds once where the host rounds twice.
-struct LinearTap {
-    int s;           // low tap (x: clamped; y: not clamped)
-    short c0, c1;    // fixed-point weights, c0 + c1 = 2048
+// cv_linear_coord is the geometry alone, the low tap and its float fraction fx; the float64 resize of the CenterNet
+// pre-process (centernet.cu) weights by (1 - fx, fx) in float.
+struct LinearCoord {
+    int s;    // low tap (clamped or not, as for LinearTap)
+    float f;  // fraction, 0 where the tap was clamped
 };
-__host__ __device__ inline LinearTap cv_linear_tap(int d, double scale, int sn, bool clamp) {
+__host__ __device__ inline LinearCoord cv_linear_coord(int d, double scale, int sn, bool clamp) {
 #ifdef __CUDA_ARCH__
     float f = __double2float_rn(__dadd_rn(__dmul_rn(__dadd_rn((double)d, 0.5), scale), -0.5));
 #else
@@ -110,8 +112,17 @@ __host__ __device__ inline LinearTap cv_linear_tap(int d, double scale, int sn, 
         if (s < 0) f = 0, s = 0;
         if (s >= sn - 1) f = 0, s = sn - 1;
     }
+    return LinearCoord{s, f};
+}
+struct LinearTap {
+    int s;           // low tap (x: clamped; y: not clamped)
+    short c0, c1;    // fixed-point weights, c0 + c1 = 2048
+};
+__host__ __device__ inline LinearTap cv_linear_tap(int d, double scale, int sn, bool clamp) {
+    const LinearCoord g = cv_linear_coord(d, scale, sn, clamp);
+    const float f = g.f;
     LinearTap t;
-    t.s = s;
+    t.s = g.s;
 #ifdef __CUDA_ARCH__
     t.c0 = (short)__float2int_rn(__fmul_rn(__fsub_rn(1.f, f), 2048.f));
     t.c1 = (short)__float2int_rn(__fmul_rn(f, 2048.f));

@@ -881,6 +881,7 @@ TRTX_API size_t trtx_abi_sizeof(int which) {
         case 9: return sizeof(trtx_face_post_params);
         case 10: return sizeof(trtx_yolop_post_params);
         case 11: return sizeof(trtx_detr_post_params);
+        case 12: return sizeof(trtx_centernet_params);
         default: return 0;
     }
 }

@@ -1298,6 +1298,66 @@ def detr_postprocess(scores: torch.Tensor, boxes: torch.Tensor, image_sizes: Seq
     return out
 
 
+CENTERNET_NET, CENTERNET_DOWN = 512, 4  # centernet/sample/test.py: cv.resize(img, (512, 512)), `4*s`
+
+
+def centernet_preprocess(images: Sequence[torch.Tensor], out: torch.Tensor | None = None, net: int = CENTERNET_NET,
+                         stream=None) -> torch.Tensor:
+    """GPU drop-in for CenterNet's pre_process (centernet/sample/test.py:34-41) for a batch of device frames: images[i] is a
+    u8 HWC BGR cuda tensor [h, w, 3] with packed pixels (rows may be pitched, sizes may differ) -> [B, 3, net, net] float32
+    planes in B, G, R order, the engine input: the frame at the top-left of an L x L zero canvas (L = max(h, w, 3)), resized
+    on float64 as cv.resize does, then ((v / 255.) - 0.5) / 0.5.  One launch per 64 images, no synchronisation."""
+    lib = L.load()
+    n = len(images)
+    descs = _image_descs(images)
+    out = _out_tensor(out, (n, 3, net, net), torch.float32, images[0].device if n else "cuda",
+                      f"out must be float32 [{n}, 3, {net}, {net}]", contiguous=False)
+    L.check(lib.trtx_centernet_preprocess_enqueue(descs, n, net, _ptr(out), _stream(stream)),
+            "trtx_centernet_preprocess_enqueue")
+    return out
+
+
+def centernet_decode(heat: torch.Tensor, wh: torch.Tensor, reg: torch.Tensor, k: int = 100, *,
+                     image_sizes: Sequence[tuple[int, int]] | None = None, score_thresh: float = 0.5,
+                     net: int = CENTERNET_NET, down: int = CENTERNET_DOWN, workspace: torch.Tensor | None = None,
+                     out: torch.Tensor | None = None, rows_out: torch.Tensor | None = None, stream=None):
+    """GPU drop-in for ctdet_decode(hm, wh, reg, K=k) (centernet/sample/test.py:44-102) on the engine outputs heat
+    [B, C, H, W], wh and reg [B, 2, H, W] float32 -> dets [B, k, 6] float32 (x1, y1, x2, y2, score, class) in map units:
+    sigmoid, the 3 x 3 peak test, the k best cells of each image ordered NaN first, then by descending score, ties to the
+    smaller flat index.  With image_sizes[b] = (img_w, img_h), also the driver loop (:126-132): rows [B, 1 + k*6] with the
+    count of score > score_thresh, then those rows with the box times (float)(down * (L / net)), L = max(img_h, img_w, 3),
+    zeros past the count -> (dets, rows).  Two launches, no synchronisation."""
+    lib = L.load()
+    if heat.dim() != 4:
+        raise ValueError("heat must be [B, C, H, W]")
+    B, Cn, H, W = (int(v) for v in heat.shape)
+    for t, what in ((wh, "wh"), (reg, "reg")):
+        if tuple(t.shape) != (B, 2, H, W):
+            raise ValueError(f"{what} must be [{B}, 2, {H}, {W}]")
+    for t in (heat, wh, reg):
+        if t.dtype != torch.float32:
+            raise ValueError("heat, wh and reg must be float32")
+    q = L.CenternetParams(Cn, H, W, k, net, down, score_thresh)
+    ws_bytes = int(lib.trtx_centernet_workspace_size(C.byref(q), B))
+    if ws_bytes == 0:
+        L.check(L.ERR_INVALID if B <= 0 or k <= 0 or k > H * W else L.ERR_UNSUPPORTED, "trtx_centernet_workspace_size")
+    if workspace is None:
+        workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=heat.device)
+    out = _out_tensor(out, (B, k, 6), torch.float32, heat.device, f"out must be contiguous float32 [{B}, {k}, 6]")
+    wh_arr = None
+    if image_sizes is not None:
+        if len(image_sizes) != B:
+            raise ValueError(f"expected {B} image sizes")
+        wh_arr = _frame_wh(image_sizes)
+        rows_out = _out_tensor(rows_out, (B, 1 + k * 6), torch.float32, heat.device,
+                               f"rows_out must be contiguous float32 [{B}, {1 + k * 6}]")
+    L.check(lib.trtx_centernet_decode_enqueue(C.byref(q), B, _ptr(heat), _ptr(wh), _ptr(reg), _ptr(workspace),
+                                              _nbytes(workspace), _ptr(out), wh_arr,
+                                              _ptr(rows_out) if wh_arr is not None else None, _stream(stream)),
+            "trtx_centernet_decode_enqueue")
+    return (out, rows_out) if wh_arr is not None else out
+
+
 def cls_postprocess(logits: torch.Tensor, k: int, softmax: bool, probs: bool = False, stream=None):
     """GPU drop-in for the cls drivers' softmax (softmax=True: yolov8, yolo11, yolov5) or raw output (softmax=False: yolo26)
     and topk(res, k): logits [B, C] float32 cuda -> (index [B, k] int32, value [B, k] float32[, probs [B, C] float32]).  The
