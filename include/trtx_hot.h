@@ -354,7 +354,10 @@ typedef struct trtx_image_desc {
 } trtx_image_desc;
 
 /* images_host: array of `batch` descriptors in HOST memory (copied into launch parameters);
- * dst_dev: [batch, 3, dst_h, dst_w] fp32 or fp16 (out_dtype TRTX_F32 | TRTX_F16). One launch. */
+ * dst_dev: [batch, 3, dst_h, dst_w] fp32 or fp16 (out_dtype TRTX_F32 | TRTX_F16). One launch per kernel and per
+ * <= 64 scale-1 images / <= 128 other images.  Every argument is checked before the first launch (a rejected call writes
+ * nothing): TRTX_ERR_INVALID for a null pointer, batch / dst sizes <= 0, an unknown out_dtype, pitch < 3 * width or a
+ * dst_dev that is not aligned to its element size (4 bytes for TRTX_F32, 2 for TRTX_F16). */
 TRTX_API int trtx_preprocess_batch_enqueue(const trtx_image_desc* images_host, int batch, void* dst_dev, int dst_w,
                                            int dst_h, int out_dtype, trtx_stream_t stream);
 /* The reference's d2s matrix (preprocess.cu:98-110): scale, centre, cv::invertAffineTransform. */

@@ -218,12 +218,20 @@ def letterbox_matrix(sw, sh, dw, dh):
     return m
 
 
-def warpaffine(src_hwc_u8, dw, dh):
+def warpaffine(src_hwc_u8, dw, dh, contracted=False):
+    """Letterbox of one u8 HWC BGR frame [sh, sw, 3] -> fp32 [3, dh, dw].  The frame may be a view with pitched rows (packed
+    pixels).  contracted=False sums the four bilinear taps with every product rounded; contracted=True evaluates the sum as
+    the device kernels do, fmaf(w4, v4, fmaf(w3, v3, fmaf(w1, v1, w2 * v2))): the exact fp32 expectation for
+    trtx_preprocess_batch_enqueue, whose fp16 output is that value rounded to nearest (.astype(np.float16))."""
     lib = load()
-    src = np.ascontiguousarray(src_hwc_u8, np.uint8)
+    src = np.asarray(src_hwc_u8)
+    assert src.dtype == np.uint8 and src.ndim == 3 and src.shape[2] == 3
+    if src.strides[1:] != (3, 1) or src.strides[0] < 3 * src.shape[1]:
+        src = np.ascontiguousarray(src)
     sh, sw = src.shape[:2]
     dst = np.zeros((3, dh, dw), np.float32)
-    lib.oracle_warpaffine(src.ctypes.data_as(C.c_void_p), sw, sh, dst.ctypes.data_as(C.c_void_p), dw, dh)
+    lib.oracle_warpaffine(C.c_void_p(src.ctypes.data), sw, sh, src.strides[0], dst.ctypes.data_as(C.c_void_p), dw, dh,
+                          int(contracted))
     return dst
 
 

@@ -758,10 +758,21 @@ ORACLE_API void oracle_letterbox_matrix(int sw, int sh, int dw, int dh, float* d
     d2s[5] = (float)b2;
 }
 
-ORACLE_API void oracle_warpaffine(const uint8_t* src, int sw, int sh, float* dst, int dw, int dh) {
+/* The bilinear sum w1 * v1 + w2 * v2 + w3 * v3 + w4 * v4 (:59-61) as nvcc's default FMA contraction evaluates it in
+ * the reference's compiled warpaffine_kernel and in both paths of letterbox_kernel (one FMUL, three FFMA in the SASS of
+ * each): the product w2 * v2 is rounded, every other product is fused into the running sum. */
+static float bilinear_contracted(float w1, float v1, float w2, float v2, float w3, float v3, float w4, float v4) {
+    return fmaf(w4, v4, fmaf(w3, v3, fmaf(w1, v1, w2 * v2)));
+}
+
+/* src rows are `pitch` bytes apart.  contracted = 0: the sum evaluated left to right with every product rounded (the
+ * plain IEEE restatement); contracted = 1: bilinear_contracted, the exact expectation for the device kernels (fp32
+ * output; an fp16 output is this value rounded to nearest). */
+ORACLE_API void oracle_warpaffine(const uint8_t* src, int sw, int sh, int pitch, float* dst, int dw, int dh,
+                                  int contracted) {
     float m[6];
     oracle_letterbox_matrix(sw, sh, dw, dh, m);
-    const int line = sw * 3;
+    const size_t line = (size_t)pitch;
     const uint8_t cv = 128; /* :115 */
     const int area = dw * dh;
     for (int pos = 0; pos < area; ++pos) {
@@ -787,9 +798,15 @@ ORACLE_API void oracle_warpaffine(const uint8_t* src, int sw, int sh, float* dst
                 if (x_low >= 0) v3 = src + (size_t)y_high * line + x_low * 3;
                 if (x_high < sw) v4 = src + (size_t)y_high * line + x_high * 3;
             }
-            c0 = w1 * v1[0] + w2 * v2[0] + w3 * v3[0] + w4 * v4[0];
-            c1 = w1 * v1[1] + w2 * v2[1] + w3 * v3[1] + w4 * v4[1];
-            c2 = w1 * v1[2] + w2 * v2[2] + w3 * v3[2] + w4 * v4[2];
+            if (contracted) {
+                c0 = bilinear_contracted(w1, v1[0], w2, v2[0], w3, v3[0], w4, v4[0]);
+                c1 = bilinear_contracted(w1, v1[1], w2, v2[1], w3, v3[1], w4, v4[1]);
+                c2 = bilinear_contracted(w1, v1[2], w2, v2[2], w3, v3[2], w4, v4[2]);
+            } else {
+                c0 = w1 * v1[0] + w2 * v2[0] + w3 * v3[0] + w4 * v4[0];
+                c1 = w1 * v1[1] + w2 * v2[1] + w3 * v3[1] + w4 * v4[1];
+                c2 = w1 * v1[2] + w2 * v2[2] + w3 * v3[2] + w4 * v4[2];
+            }
         }
         float t = c2; /* bgr -> rgb :66-69 */
         c2 = c0;

@@ -13,7 +13,10 @@
 //
 // Arithmetic follows the reference kernel statement by statement (including its `+0.5f` source
 // offset without a matching `-0.5f`, preprocess.cu:22-23) and, like the reference's own nvcc build,
-// leaves the bilinear sums to the default FMA contraction (<= 1 ulp from the uncontracted oracle).
+// leaves the bilinear sums to the default FMA contraction, which both paths of letterbox_kernel and the reference
+// evaluate as fmaf(w4, v4, fmaf(w3, v3, fmaf(w1, v1, w2 * v2))).  The CPU oracle's contracted warpaffine
+// (oracle/trtx_oracle.c) restates exactly that: it is the bit-exact expectation for every output of this file's
+// letterbox (tests/test_letterbox_paths_gpu.py), fp16 outputs being its fp32 value rounded to nearest.
 #include <limits.h>
 #include <math.h>
 #include <string.h>
@@ -841,6 +844,7 @@ TRTX_API int trtx_preprocess_batch_enqueue(const trtx_image_desc* images_host, i
                                            int dst_h, int out_dtype, trtx_stream_t stream) {
     if (!images_host || batch <= 0 || !dst_dev || dst_w <= 0 || dst_h <= 0) return TRTX_ERR_INVALID;
     if (out_dtype != TRTX_F32 && out_dtype != TRTX_F16) return TRTX_ERR_INVALID;
+    if (reinterpret_cast<uintptr_t>(dst_dev) % (out_dtype == TRTX_F32 ? sizeof(float) : sizeof(__half)) != 0) return TRTX_ERR_INVALID;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     for (int i = 0; i < batch; ++i) {
         const trtx_image_desc& d = images_host[i];

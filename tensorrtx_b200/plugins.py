@@ -1073,6 +1073,15 @@ def _image_descs(images: Sequence[torch.Tensor]):
     return descs
 
 
+def _letterbox_dst(dst: torch.Tensor, n: int, dst_width: int, dst_height: int) -> int:
+    """TRTX_F32 / TRTX_F16 of the letterbox output dst, which must be a float32 or float16 tensor [n, 3, dst_h, dst_w]:
+    TrtxError for another dtype, ValueError for another shape, both before the library is called."""
+    dt = _elem_dtype([dst], "letterbox dst")
+    _out_tensor(dst, (n, 3, int(dst_height), int(dst_width)), dst.dtype, dst.device,
+                f"dst must be float32 or float16 [{n}, 3, {dst_height}, {dst_width}]", contiguous=False)
+    return dt
+
+
 def cuda_batch_preprocess(img_batch: Sequence[torch.Tensor], dst: torch.Tensor, dst_width: int, dst_height: int,
                           stream=None) -> None:
     """Drop-in for cuda_batch_preprocess (yolov8/src/preprocess.cu:119-127) with DEVICE images:
@@ -1080,7 +1089,7 @@ def cuda_batch_preprocess(img_batch: Sequence[torch.Tensor], dst: torch.Tensor, 
     One launch for the whole batch, no synchronisation."""
     lib = L.load()
     descs = _image_descs(img_batch)
-    dt = L.F32 if dst.dtype == torch.float32 else L.F16
+    dt = _letterbox_dst(dst, len(img_batch), dst_width, dst_height)
     L.check(lib.trtx_preprocess_batch_enqueue(descs, len(img_batch), _ptr(dst), dst_width, dst_height, dt, _stream(stream)),
             "trtx_preprocess_batch_enqueue")
 
@@ -1096,7 +1105,7 @@ class PreprocessPlan:
         self.descs = _image_descs(img_batch)
         self._keep = list(img_batch)
         self.dst, self.dw, self.dh = dst, int(dst_width), int(dst_height)
-        self.dt = L.F32 if dst.dtype == torch.float32 else L.F16
+        self.dt = _letterbox_dst(dst, self.n, self.dw, self.dh)
 
     def enqueue(self, stream=None) -> None:
         L.check(self._lib.trtx_preprocess_batch_enqueue(self.descs, self.n, _ptr(self.dst), self.dw, self.dh, self.dt,
