@@ -50,7 +50,8 @@ TRTX_API int trtx_last_cuda_error(void);
 /* sizeof() of the parameter structs as THIS library was compiled, so that an FFI binding (ctypes, cgo, ...) can check its
  * mirror of the layout: which = 0 trtx_yolo_params, 1 trtx_nms_params, 2 trtx_retina_params, 3 trtx_image_desc,
  * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_frame, 7 trtx_pose_obb_params, 8 trtx_frame,
- * 9 trtx_face_post_params, 10 trtx_yolop_post_params, 11 trtx_detr_post_params, 12 trtx_centernet_params;
+ * 9 trtx_face_post_params, 10 trtx_yolop_post_params, 11 trtx_detr_post_params, 12 trtx_centernet_params,
+ * 13 trtx_ufld_post_params;
  * anything else 0. */
 TRTX_API size_t trtx_abi_sizeof(int which);
 
@@ -869,6 +870,61 @@ TRTX_API int trtx_centernet_decode_enqueue(const trtx_centernet_params* p, int b
                                            const float* wh_dev, const float* reg_dev, void* workspace_dev,
                                            size_t workspace_bytes, float* dets_dev, const int32_t* frame_wh_host,
                                            float* rows_dev, trtx_stream_t stream);
+
+/* =====================================================================================
+ * 12. UFLD lane detection pre- and post-process
+ *    replaces the HOST stages of ufld/lane_det.cpp (the Ultra-Fast Lane Detection row-anchor model): prepareImage (:194-221)
+ *    and the H2D copy of its input, and after inference the D2H copy of `prob` and the driver's loops (:358-410: the row flip,
+ *    argmax and softmax_mul of :223-270, the "no lane" zeroing, the lane choice and the points).  Drawing stays with the caller.
+ * ===================================================================================== */
+/* prepareImage for a whole batch, one launch per <= 64 images: images_host = `batch` u8 HWC BGR descriptors in HOST memory
+ * (trtx_image_desc, any pitch and base alignment, mixed sizes allowed); dst_dev = [batch, 3, net_h, net_w] fp32 planes in R, G,
+ * B order (cvtColor BGR2RGB, then cv::split; INPUT_W x INPUT_H = 800 x 288), the engine input.  The whole frame is stretched
+ * over the whole net by OpenCV 4.x's 8-bit INTER_LINEAR, bit for bit (an exact 2x downscale, where OpenCV takes INTER_AREA,
+ * gives the same bytes); byte u of plane c (the driver's `static float` mean = 0.485f, 0.456f, 0.406f and std = 0.229f,
+ * 0.224f, 0.225f for planes 0, 1, 2) becomes
+ *     s = (float)u * (float)(1. / 255.),   fmaf(s, (float)(1. / std_c), (float)(-mean_c / std_c))  (quotients in double),
+ * the one convertTo that OpenCV 4.x makes of `(channel - mean[c]) / std[c]`, with the fused multiply-add of its AVX2 kernel.
+ * The caller's frame is not converted in place, as the driver's cvtColor(img, img) does.  Every descriptor is checked before
+ * the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer, batch / net sizes <= 0, pitch <
+ * 3 * width or a dst_dev that is not 4-byte aligned; TRTX_ERR_UNSUPPORTED for a net wider than 4 757 pixels (the band's staged
+ * source rows in shared memory).  No workspace; can be captured in a CUDA graph. */
+TRTX_API int trtx_ufld_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
+                                          trtx_stream_t stream);
+
+typedef struct trtx_ufld_post_params {
+    int32_t num_cells;    /* C: OUTPUT_C = 101 (griding_num + 1); cell C - 1 is "no lane" (the driver's literal 100) */
+    int32_t num_rows;     /* H: OUTPUT_H = 56 row anchors */
+    int32_t num_lanes;    /* W: OUTPUT_W = 4 */
+    int32_t net_w, net_h; /* INPUT_W 800, INPUT_H 288 */
+    int32_t col_sample_w; /* 8 */
+} trtx_ufld_post_params;
+
+/* prob_dev [B, C, H, W] fp32: the engine output `prob`.  row_anchor_host: H ints in HOST memory (tusimple_row_anchor);
+ * frame_wh_host: `batch` pairs (w, h) in HOST memory, the size of the picture the points are for ((1280, 720) is the driver's
+ * `vis`; a frame's own size gives the points on that frame); both are copied into launch parameters.
+ * rows_dev [B, 1 + H*W*3]: the point count n, then n rows (x, y, lane) as floats in the driver's draw order -- engine rows
+ * j = H - 1 .. 0 (the driver flips the rows and indexes the anchors with H - 1 - k), the chosen lanes ascending in each --
+ * then zeros.  Per cell (row j, lane l), reading prob[b, :, j, l], each statement of the driver rounded as there:
+ *   argmax: int max = -10000000, max_ind = -1; for c: if (v > (float)max) max = (int)v, max_ind = c -- truncated, so a later
+ *     value above the truncated running maximum wins ([3.7, 3.2] gives 1); (int)v is INT_MIN where the x86-64 conversion
+ *     gives it (v >= 2^31 or +inf); a NaN is never taken; max_ind may stay -1;
+ *   softmax_mul: e_c = (float)exp((double)v_c) for c < C - 1 (no max subtraction; the correctly rounded expf except within
+ *     about 2^-29 of a rounding boundary), sum += e_c in float in c order, then expect += (e_c / sum) * (float)(c + 1) in c
+ *     order; overflow and underflow give NaN as in the driver (inf / inf, 0 / 0);
+ *   expect = 0 where max_ind == C - 1.
+ * Per frame: lane l is chosen when more than 2 of its H cells have expect != 0 (a NaN counts); each chosen cell with
+ * expect > 0 (NaN excluded) gives x = (int)(((expect * (float)col_sample_w) * (float)w) / (float)net_w) - 1 (float, left to
+ * right; (int) as x86-64 converts, the - 1 wrapping) and y = h * anchor[j] / net_h - 1 in int; rows hold (float)x, exact for
+ * |x| <= 2^24 (C * col_sample_w * w <= 2^24 * net_w suffices).
+ * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer, batch,
+ * H, W, net_w, net_h, col_sample_w or a frame side <= 0, or C < 2; TRTX_ERR_UNSUPPORTED for H * W > 1024 or
+ * (C - 1) * H * W > 53 248 (one CTA per frame: a thread per cell, the exponentials in shared memory), a frame side above 2^24,
+ * or a frame and anchor where h * anchor overflows int32 or |y| > 2^24.  One launch per 64 frames, no workspace, no atomics;
+ * can be captured in a CUDA graph. */
+TRTX_API int trtx_ufld_postprocess_enqueue(const trtx_ufld_post_params* p, const int32_t* row_anchor_host,
+                                           const int32_t* frame_wh_host, int batch, const float* prob_dev, float* rows_dev,
+                                           trtx_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -384,6 +384,21 @@ __host__ __device__ inline void detr_get_rect(int img_w, int img_h, const float 
     rect[3] = trunc_to_int_x86(f_sub(c[3], c[1]));
 }
 
+// UFLD's prepareImage after the resize (ufld/lane_det.cpp:194-221), the value of byte u in plane c (0 = R, 1 = G, 2 = B:
+// cvtColor BGR2RGB, then cv::split), with the driver's `static float` mean and std:
+//   convertTo(CV_32FC3, 1. / 255.)        s = (float)u * (float)(1. / 255.)
+//   (channel - mean[c]) / std[c]          one convertTo(-1, 1 / std, -mean / std): OpenCV 4.x folds the MatExpr
+//                                         (MatOp_AddEx), and cvtScale32f casts both coefficients to float and fuses them with
+//                                         v_fma: fmaf(s, (float)(1 / std), (float)(-mean / std)), the quotients in double.
+// The folding is read from OpenCV's source, not run (DESIGN §4.8); the fused product is pinned against cv2 4.13 on all
+// 3 x 256 bytes (tests/test_ufld_cpu.py).
+__device__ __forceinline__ float ufld_input_value(int c, uint32_t u) {
+    const double mean = (double)(c == 0 ? 0.485f : (c == 1 ? 0.456f : 0.406f));
+    const double sd = (double)(c == 0 ? 0.229f : (c == 1 ? 0.224f : 0.225f));
+    const float s = __fmul_rn((float)u, (float)(1. / 255.));
+    return __fmaf_rn(s, __double2float_rn(__ddiv_rn(1.0, sd)), __double2float_rn(__ddiv_rn(-mean, sd)));
+}
+
 __device__ __forceinline__ int warp_excl_scan(int v, int lane, int* total) {
     int x = v;
 #pragma unroll

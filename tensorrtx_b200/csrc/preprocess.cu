@@ -613,6 +613,13 @@ struct DetrInput {
     static __device__ __forceinline__ int channel(int c) { return 2 - c; }
     static __device__ __forceinline__ float value(int c, uint32_t u) { return yolop_input_value(c, u); }
 };
+// UFLD's prepareImage (ufld/lane_det.cpp:194-221): cvtColor BGR2RGB and cv::split, so plane c (0 = R) takes BGR channel
+// 2 - c; the value chain is ufld_input_value (common.cuh).
+struct UfldInput {
+    static constexpr uint32_t kCanvas = 0u;  // never read: the frame is stretched over the whole net
+    static __device__ __forceinline__ int channel(int c) { return 2 - c; }
+    static __device__ __forceinline__ float value(int c, uint32_t u) { return ufld_input_value(c, u); }
+};
 
 // [B, 3, net_h, net_w] planes: the band is three contiguous runs of band * net_w floats, each written by store_band_run; the
 // value of a byte comes from a per-CTA table of 3 x 256 floats.
@@ -652,6 +659,11 @@ __global__ void __launch_bounds__(kRcnnPreThreads) yolop_preprocess_kernel(const
 __global__ void __launch_bounds__(kRcnnPreThreads) detr_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
                                                                           float* __restrict__ dst) {
     resize_band<PlanarStore<DetrInput>>(a, dst);
+}
+
+__global__ void __launch_bounds__(kRcnnPreThreads) ufld_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
+                                                                          float* __restrict__ dst) {
+    resize_band<PlanarStore<UfldInput>>(a, dst);
 }
 
 // One launch of `kernel` per kMaxRcnnPreImages frames: make(i, im) fills the band descriptor of frame i (validated before).
@@ -710,9 +722,9 @@ static bool cls_band_image(int variant, const trtx_image_desc& d, int net_w, int
     return true;
 }
 
-// The band descriptor of frame d for DETR's preprocessImg: cv::resize(img, img, Size(net_w, net_h)) of the whole frame, i.e.
-// cls_band_image's V8 descriptor without the crop.
-static void detr_band_image(const trtx_image_desc& d, int net_w, int net_h, RcnnPreImage& im) {
+// The band descriptor of frame d for a whole frame stretched over the whole net, cv::resize(img, dst, Size(net_w, net_h))
+// (DETR's preprocessImg, UFLD's prepareImage), i.e. cls_band_image's V8 descriptor without the crop.
+static void stretch_band_image(const trtx_image_desc& d, int net_w, int net_h, RcnnPreImage& im) {
     im.src = d.data_dev;
     im.sw = d.width;
     im.sh = d.height;
@@ -722,6 +734,22 @@ static void detr_band_image(const trtx_image_desc& d, int net_w, int net_h, Rcnn
     im.rh = net_h;
     im.scale_x = 1. / ((double)net_w / d.width);
     im.scale_y = 1. / ((double)net_h / d.height);
+}
+
+// The whole-frame pre-processes (DETR, UFLD): one band descriptor per frame (stretch_band_image) into `kernel`'s planar store.
+static int stretch_preprocess(void (*kernel)(RcnnPreArgs, float*), const trtx_image_desc* images_host, int batch, int net_w,
+                              int net_h, float* dst_dev, cudaStream_t st) {
+    if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
+    if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
+    // every descriptor is checked before the first launch, so that a rejected call writes nothing
+    for (int i = 0; i < batch; ++i) {
+        const trtx_image_desc& d = images_host[i];
+        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
+    }
+    const size_t smem = (size_t)kRcnnPreSlots * 3 * (size_t)net_w * sizeof(int16_t);  // every rectangle is net_w wide
+    if (smem > kClsMaxDynamicSmem) return TRTX_ERR_UNSUPPORTED;
+    return launch_bands(kernel, batch, net_w, net_h, dst_dev, smem, st,
+                        [&](int i, RcnnPreImage& im) { stretch_band_image(images_host[i], net_w, net_h, im); });
 }
 
 }  // namespace trtx
@@ -988,21 +1016,19 @@ TRTX_API int trtx_yolop_preprocess_enqueue(const trtx_image_desc* images_host, i
                         [&](int i, RcnnPreImage& im) { cls_band_image(TRTX_YOLO_V5, images_host[i], net_w, net_h, im); });
 }
 
-// DETR's preprocessImg stretches the whole frame over the whole net: one band descriptor per frame (detr_band_image), the
-// planar store with DETR's R, G, B planes and value chain.
+// DETR's preprocessImg stretches the whole frame over the whole net: the planar store with DETR's R, G, B planes and value
+// chain.
 TRTX_API int trtx_detr_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
                                           trtx_stream_t stream) {
-    if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
-    if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
-    // every descriptor is checked before the first launch, so that a rejected call writes nothing
-    for (int i = 0; i < batch; ++i) {
-        const trtx_image_desc& d = images_host[i];
-        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
-    }
-    const size_t smem = (size_t)kRcnnPreSlots * 3 * (size_t)net_w * sizeof(int16_t);  // every rectangle is net_w wide
-    if (smem > kClsMaxDynamicSmem) return TRTX_ERR_UNSUPPORTED;
-    return launch_bands(detr_preprocess_kernel, batch, net_w, net_h, dst_dev, smem, static_cast<cudaStream_t>(stream),
-                        [&](int i, RcnnPreImage& im) { detr_band_image(images_host[i], net_w, net_h, im); });
+    return stretch_preprocess(detr_preprocess_kernel, images_host, batch, net_w, net_h, dst_dev,
+                              static_cast<cudaStream_t>(stream));
+}
+
+// UFLD's prepareImage, likewise, with UFLD's fused value chain.
+TRTX_API int trtx_ufld_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
+                                          trtx_stream_t stream) {
+    return stretch_preprocess(ufld_preprocess_kernel, images_host, batch, net_w, net_h, dst_dev,
+                              static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -882,6 +882,7 @@ TRTX_API size_t trtx_abi_sizeof(int which) {
         case 10: return sizeof(trtx_yolop_post_params);
         case 11: return sizeof(trtx_detr_post_params);
         case 12: return sizeof(trtx_centernet_params);
+        case 13: return sizeof(trtx_ufld_post_params);
         default: return 0;
     }
 }

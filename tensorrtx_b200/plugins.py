@@ -1367,6 +1367,55 @@ def centernet_decode(heat: torch.Tensor, wh: torch.Tensor, reg: torch.Tensor, k:
     return (out, rows_out) if wh_arr is not None else out
 
 
+UFLD_NET = (800, 288)  # INPUT_W, INPUT_H (ufld/lane_det.cpp:13-14)
+UFLD_SHAPE = (101, 56, 4)  # OUTPUT_C, OUTPUT_H, OUTPUT_W
+UFLD_COL_SAMPLE_W = 8
+UFLD_TUSIMPLE_ROW_ANCHOR = tuple(range(64, 288, 4))  # tusimple_row_anchor (ufld/lane_det.cpp:358-363)
+UFLD_VIS = (1280, 720)  # vis_w, vis_h: the driver's drawing frame
+
+
+def ufld_preprocess(images: Sequence[torch.Tensor], out: torch.Tensor | None = None, net_w: int = UFLD_NET[0],
+                    net_h: int = UFLD_NET[1], stream=None) -> torch.Tensor:
+    """GPU drop-in for UFLD's prepareImage (ufld/lane_det.cpp:194-221) for a batch of device frames: images[i] is a u8 HWC BGR
+    cuda tensor [h, w, 3] with packed pixels (rows may be pitched, sizes may differ) -> [B, 3, net_h, net_w] float32 planes in
+    R, G, B order, the engine input: the whole frame resized to the whole net, then fmaf(u * (1 / 255.), 1 / std, -mean / std)
+    as OpenCV folds the driver's `(c - mean) / std`.  The frames are not written.  One launch per 64 images, no
+    synchronisation."""
+    lib = L.load()
+    n = len(images)
+    descs = _image_descs(images)
+    out = _out_tensor(out, (n, 3, net_h, net_w), torch.float32, images[0].device if n else "cuda",
+                      f"out must be float32 [{n}, 3, {net_h}, {net_w}]", contiguous=False)
+    L.check(lib.trtx_ufld_preprocess_enqueue(descs, n, net_w, net_h, _ptr(out), _stream(stream)), "trtx_ufld_preprocess_enqueue")
+    return out
+
+
+def ufld_postprocess(prob: torch.Tensor, image_sizes: Sequence[tuple[int, int]] | None = None, *,
+                     row_anchor: Sequence[int] = UFLD_TUSIMPLE_ROW_ANCHOR, col_sample_w: int = UFLD_COL_SAMPLE_W,
+                     net_w: int = UFLD_NET[0], net_h: int = UFLD_NET[1], out: torch.Tensor | None = None,
+                     stream=None) -> torch.Tensor:
+    """GPU drop-in for UFLD's host stages after inference (ufld/lane_det.cpp:358-410) for a batch: prob [B, C, H, W] float32,
+    the engine output (C = 101 cells, the last one "no lane"; H = 56 row anchors; W = 4 lanes); image_sizes[b] = (w, h) of the
+    picture frame b's points are for (default: the driver's 1280 x 720 `vis` for every frame); row_anchor: H ints ->
+    rows [B, 1 + H*W*3] float32: the point count, then (x, y, lane) per point in the driver's draw order (engine rows H - 1
+    .. 0, lanes ascending), zeros past the count.  One launch per 64 frames, no workspace."""
+    lib = L.load()
+    if prob.dim() != 4 or prob.dtype != torch.float32:
+        raise ValueError("prob must be float32 [B, C, H, W]")
+    B, Cn, H, W = (int(v) for v in prob.shape)
+    if image_sizes is None:
+        image_sizes = [UFLD_VIS] * B
+    if len(image_sizes) != B or len(row_anchor) != H:
+        raise ValueError(f"expected {B} image sizes and {H} row anchors")
+    out = _out_tensor(out, (B, 1 + H * W * 3), torch.float32, prob.device,
+                      f"out must be contiguous float32 [{B}, {1 + H * W * 3}]")
+    q = L.UfldPostParams(Cn, H, W, net_w, net_h, col_sample_w)
+    anchors = (C.c_int32 * H)(*[int(v) for v in row_anchor])
+    L.check(lib.trtx_ufld_postprocess_enqueue(C.byref(q), anchors, _frame_wh(image_sizes), B, _ptr(prob), _ptr(out),
+                                              _stream(stream)), "trtx_ufld_postprocess_enqueue")
+    return out
+
+
 def cls_postprocess(logits: torch.Tensor, k: int, softmax: bool, probs: bool = False, stream=None):
     """GPU drop-in for the cls drivers' softmax (softmax=True: yolov8, yolo11, yolov5) or raw output (softmax=False: yolo26)
     and topk(res, k): logits [B, C] float32 cuda -> (index [B, k] int32, value [B, k] float32[, probs [B, C] float32]).  The
