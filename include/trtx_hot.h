@@ -409,7 +409,11 @@ TRTX_API int trtx_scale_mask_enqueue(const float* masks_dev, int n, int net_w, i
  * The library picks the kernel from the shape; both are bit-identical to the reference's roiAlign.  The reference's
  * configuration class (pooler_resolution 14, out_channels % 4 == 0, feature_h * feature_w <= 4096) stages each proposal's
  * feature-map window in shared memory and takes the bilinear taps from there; any other shape takes every tap from global
- * memory. */
+ * memory.
+ * Adaptive sampling (sampling_ratio <= 0) takes ceil(side / pooler_resolution) samples per bin and axis, as the reference
+ * does: a proposal side of s feature cells costs about (s / pooler_resolution)^2 samples per bin, so a huge proposal does
+ * that much work, and one with an infinite side an unbounded amount (its grid saturates at 2^31 - 1 per axis).  Pass finite
+ * proposals of bounded size, or a fixed sampling_ratio. */
 TRTX_API int trtx_roi_align(int batch, const float* rois_dev, const float* features_dev, float* out_dev, int pooler_resolution,
                             float spatial_scale, int sampling_ratio, int num_proposals, int out_channels, int feature_h,
                             int feature_w, trtx_stream_t stream);
