@@ -930,6 +930,37 @@ TRTX_API int trtx_ufld_postprocess_enqueue(const trtx_ufld_post_params* p, const
                                            const int32_t* frame_wh_host, int batch, const float* prob_dev, float* rows_dev,
                                            trtx_stream_t stream);
 
+/* =====================================================================================
+ * 13. Bicubic letterbox pre-process (yolov3-tiny, retinafaceAntiCov)
+ *    replaces the HOST preprocess_img with cv::resize(INTER_CUBIC) of yolov3-tiny/yolov3-tiny.cpp:40-60 and
+ *    retinafaceAntiCov/retinafaceAntiCov.cpp:41-61, the drivers' plane loops (:441-445, :528-532) and the H2D copy of their
+ *    fp32 input.
+ * ===================================================================================== */
+enum {
+    TRTX_CUBIC_YOLOV3_TINY = 0, /* data = u / 255.0 (double), stored to float */
+    TRTX_CUBIC_ANTICOV = 1,     /* data = ((float)u - 127.5) * 0.0078125 (double), stored to float: exact */
+};
+
+/* preprocess_img + the plane loop for a whole batch, one launch per <= 64 images: images_host = `batch` u8 HWC BGR descriptors
+ * in HOST memory (trtx_image_desc, any pitch and base alignment, mixed sizes allowed); dst_dev = [batch, 3, net_h, net_w] fp32
+ * planes in R, G, B order (INPUT_W x INPUT_H = 608 x 608 for yolov3-tiny, 640 x 640 for retinafaceAntiCov), the engine input.
+ * The frame is resized into the rectangle of trtx_calib_letterbox_rect on a 128-grey canvas by OpenCV 4.x's own 8-bit
+ * INTER_CUBIC (the build without IPP, which every non-x86 build runs), bit for bit:
+ *   taps      fx = (float)((d + 0.5) * scale - 0.5), scale = 1. / ((double)dsize / ssize), s = floor(fx), fx -= s; taps
+ *             s - 1 .. s + 2 clamped into the frame; weights saturate_cast<short>(interpolateCubic(fx) * 2048), A = -0.75;
+ *   passes    horizontal: h = sum of the 4 products in int; vertical, for byte i of the 3 * w bytes of a resized row:
+ *             i < (3 * w) & ~7: h0 * b0' + (h1 * b1' + (h2 * b2' + h3 * b3')) in float, b' = b / 2048^2, rounded half to even;
+ *             otherwise (sum h_k * b_k + 2^21) >> 22; saturated to 0..255.
+ * OpenCV with IPP (the default of x86 wheels) differs from this by 1 in a few % of the bytes of a non-integer-ratio resize.
+ * Byte u then becomes the variant's value.  Every descriptor is checked before the first launch (a rejected call writes
+ * nothing): TRTX_ERR_INVALID for a null pointer, batch / net sizes <= 0, pitch < 3 * width, an unknown variant or a dst_dev
+ * that is not 4-byte aligned; TRTX_ERR_UNSUPPORTED for a rectangle that is empty (cv::resize throws there, e.g. 1 x 5000) or
+ * whose staged source rows exceed the kernel's shared memory (4 bytes per byte of the rectangle's row times at most 16 rows:
+ * rectangles up to 1 189 pixels wide at any scale, 2 378 when enlarging).  No workspace; can be captured in a CUDA
+ * graph. */
+TRTX_API int trtx_cubic_preprocess_enqueue(int variant, const trtx_image_desc* images_host, int batch, int net_w, int net_h,
+                                           float* dst_dev, trtx_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

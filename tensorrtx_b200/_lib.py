@@ -18,6 +18,7 @@ BOX_LTRB, BOX_CXCYWH, BOX_RETINA, BOX_OBB = 0, 1, 2, 3
 NMS_GREEDY, NMS_ONESHOT = 0, 1
 RETINA_FACE, RETINA_ANTICOV = 0, 1
 TASK_POSE, TASK_OBB, TASK_OBB_NMS_FREE = 1, 2, 3
+CUBIC_YOLOV3_TINY, CUBIC_ANTICOV = 0, 1
 
 _ERR = {1: "TRTX_ERR_INVALID", 2: "TRTX_ERR_WORKSPACE", 3: "TRTX_ERR_CUDA", 4: "TRTX_ERR_UNSUPPORTED"}
 
@@ -200,6 +201,7 @@ SYMBOLS = {
     "trtx_ufld_preprocess_enqueue": (_i, [C.POINTER(ImageDesc), _i, _i, _i, _vp, _vp]),
     "trtx_ufld_postprocess_enqueue": (_i, [C.POINTER(UfldPostParams), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _i, _vp,
                                            _vp, _vp]),
+    "trtx_cubic_preprocess_enqueue": (_i, [_i, C.POINTER(ImageDesc), _i, _i, _i, _vp, _vp]),
     "trtx_yolo_decode_nms_gather_enqueue": (_i, [C.POINTER(YoloParams), C.POINTER(NmsParams), _i, _pp, _vp, _vp, _vp, _sz,
                                                  C.POINTER(Gather), _vp]),
     "trtx_gather_wait_enqueue": (_i, [C.POINTER(Gather), _vp]),

@@ -752,6 +752,150 @@ static int stretch_preprocess(void (*kernel)(RcnnPreArgs, float*), const trtx_im
                         [&](int i, RcnnPreImage& im) { stretch_band_image(images_host[i], net_w, net_h, im); });
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Bicubic letterbox pre-process: preprocess_img of yolov3-tiny (yolov3-tiny/yolov3-tiny.cpp:40-60) and retinafaceAntiCov
+// (retinafaceAntiCov/retinafaceAntiCov.cpp:41-61) -- cv::resize(INTER_CUBIC) into trtx_calib_letterbox_rect's rectangle on a
+// 128-grey canvas -- and the drivers' loops into R, G, B planes (:441-445, :528-532).  The resize is OpenCV 4.x's own 8-bit
+// INTER_CUBIC (resizeGeneric_ with HResizeCubic and VResizeCubic; IPP's differs by 1 in a few % of the bytes, DESIGN §7):
+//   taps:       fx = (float)((d + 0.5) * scale - 0.5), s = floor(fx), fx -= s (kept at the borders: cv_linear_coord without
+//               clamp); taps s - 1 .. s + 2, clamped into the image; weights interpolateCubic(fx) (A = -0.75, float) and
+//               saturate_cast<short>(c * 2048);
+//   horizontal: h = the int sum of the 4 products (|h| reaches 2^19.3, so nothing is staged in int16);
+//   vertical:   of the 3 * rw bytes of a destination row, the first (3 * rw) & ~7 are VResizeCubicVec_32s8u's 8-lane float loop:
+//               h0 * b0' + (h1 * b1' + (h2 * b2' + h3 * b3')), b' = b / 2048^2 (exact), every product and sum rounded (no FMA),
+//               then rounded half to even; the rest are the scalar tail's (sum h_k * b_k + 2^21) >> 22; both saturated to 0..255.
+// The band structure is resize_band's with 4 y taps per destination row, the staged rows in int32 and up to 4 slots per row.
+// The horizontal pass is shared by the band rows that read the same source row; stage 3 is PlanarStore.
+constexpr int kCubicMaxSlots = 4 * kRcnnPreBand;
+
+// interpolateCubic (imgproc/src/resize.cpp) statement by statement in float, then saturate_cast<short>(c * 2048)
+__device__ __forceinline__ void cv_cubic_coeffs(float x, int (&c)[4]) {
+    constexpr float A = -0.75f;
+    const float x1 = __fadd_rn(x, 1.f), mx = __fsub_rn(1.f, x);
+    const float c0 = __fsub_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fsub_rn(__fmul_rn(A, x1), 5 * A), x1), 8 * A), x1), 4 * A);
+    const float c1 = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(A + 2, x), A + 3), x), x), 1.f);
+    const float c2 = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(A + 2, mx), A + 3), mx), mx), 1.f);
+    const float c3 = __fsub_rn(__fsub_rn(__fsub_rn(1.f, c0), c1), c2);
+    c[0] = __float2int_rn(__fmul_rn(c0, 2048.f));
+    c[1] = __float2int_rn(__fmul_rn(c1, 2048.f));
+    c[2] = __float2int_rn(__fmul_rn(c2, 2048.f));
+    c[3] = __float2int_rn(__fmul_rn(c3, 2048.f));
+}
+
+// Source rows a band of kRcnnPreBand destination rows can read at y scale `scale`: the low taps of its first and last rows are
+// at most ceil(3 * scale) + 1 apart (the float rounding of fy moves a difference by far less than 1), and each row reads 4 rows
+// from its low tap on.
+static int cubic_band_slots(double scale) {
+    return (int)fmin((double)kCubicMaxSlots, ceil((kRcnnPreBand - 1) * scale) + 5);
+}
+
+template <class Store>
+__device__ __forceinline__ void cubic_band(const RcnnPreArgs& a, float* __restrict__ dst) {
+    constexpr int R = kRcnnPreBand;
+    extern __shared__ __align__(16) int hcub[];  // [slots][a.stride]
+    __shared__ int s_row[kCubicMaxSlots];
+    __shared__ int s_slot[R][4];
+    __shared__ int s_coef[R][4];
+    __shared__ int s_nslots;
+    const int item = blockIdx.x / a.bands, band = blockIdx.x - item * a.bands;
+    const RcnnPreImage& im = a.img[item];
+    const int y0 = band * R, rows = min(R, a.net_h - y0);
+    const int k_lo = max(im.y0 - y0, 0), k_hi = min(im.y0 + im.rh - y0, rows);
+    const int stride = a.stride;
+    if (k_lo < k_hi) {  // uniform over the CTA
+        if (threadIdx.x == 0) {
+            int n = 0;
+            for (int k = k_lo; k < k_hi; ++k) {
+                const LinearCoord g = cv_linear_coord(y0 + k - im.y0, im.scale_y, im.sh, false);
+                int c[4];
+                cv_cubic_coeffs(g.f, c);
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int sy = min(max(g.s - 1 + j, 0), im.sh - 1);
+                    int slot = -1;
+                    for (int i = 0; i < n; ++i) slot = s_row[i] == sy ? i : slot;
+                    if (slot < 0) {
+                        s_row[n] = sy;
+                        slot = n++;
+                    }
+                    s_slot[k][j] = slot;
+                    s_coef[k][j] = c[j];
+                }
+            }
+            s_nslots = n;
+        }
+        __syncthreads();
+        const int n = s_nslots;
+        for (int x = threadIdx.x; x < im.rw; x += blockDim.x) {
+            const LinearCoord g = cv_linear_coord(x, im.scale_x, im.sw, false);
+            int c[4], o[4];
+            cv_cubic_coeffs(g.f, c);
+#pragma unroll
+            for (int t = 0; t < 4; ++t) o[t] = 3 * min(max(g.s - 1 + t, 0), im.sw - 1);
+            for (int j0 = 0; j0 < n; j0 += 4) {
+                uint32_t px[4][12];  // the loads of 4 slot rows are in flight before the first use
+#pragma unroll
+                for (int j = 0; j < 4; ++j)
+                    if (j0 + j < n) {
+                        const uint8_t* S = im.src + (size_t)s_row[j0 + j] * (size_t)im.pitch;
+#pragma unroll
+                        for (int t = 0; t < 4; ++t)
+#pragma unroll
+                            for (int ch = 0; ch < 3; ++ch) px[j][3 * t + ch] = __ldg(S + o[t] + ch);
+                    }
+#pragma unroll
+                for (int j = 0; j < 4; ++j)
+                    if (j0 + j < n) {
+                        int* h = hcub + (j0 + j) * stride + 3 * x;
+#pragma unroll
+                        for (int ch = 0; ch < 3; ++ch)
+                            h[ch] = (int)px[j][ch] * c[0] + (int)px[j][3 + ch] * c[1] + (int)px[j][6 + ch] * c[2] +
+                                    (int)px[j][9 + ch] * c[3];
+                    }
+            }
+        }
+        __syncthreads();
+    }
+    const int nvec = (3 * im.rw) & ~7;  // bytes of a row that the 8-lane vector loop produces
+    auto pix = [&](int k, int i) -> uint32_t {
+        int h[4], b[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) h[j] = hcub[s_slot[k][j] * stride + i], b[j] = s_coef[k][j];
+        int v;
+        if (i < nvec) {
+            constexpr float sc = 1.f / (2048.f * 2048.f);
+            float t = __fmul_rn((float)h[3], (float)b[3] * sc);
+            t = __fadd_rn(__fmul_rn((float)h[2], (float)b[2] * sc), t);
+            t = __fadd_rn(__fmul_rn((float)h[1], (float)b[1] * sc), t);
+            t = __fadd_rn(__fmul_rn((float)h[0], (float)b[0] * sc), t);
+            v = __float2int_rn(t);
+        } else {
+            v = (h[0] * b[0] + h[1] * b[1] + h[2] * b[2] + h[3] * b[3] + (1 << 21)) >> 22;
+        }
+        return (uint32_t)min(max(v, 0), 255);
+    };
+    Store::run(a, im, y0, rows, k_lo, k_hi, pix, dst);
+}
+
+// The drivers' plane loops: data[i + c * H * W] = byte 2 - c of pixel i, as
+//   TRTX_CUBIC_YOLOV3_TINY   u / 255.0 in double, stored to float;
+//   TRTX_CUBIC_ANTICOV       ((float)u - 127.5) * 0.0078125 in double, stored to float (exact in float).
+template <int kVariant>
+struct CubicInput {
+    static constexpr uint32_t kCanvas = 128u;  // Scalar(128, 128, 128)
+    static __device__ __forceinline__ int channel(int c) { return 2 - c; }
+    static __device__ __forceinline__ float value(int, uint32_t u) {
+        if (kVariant == TRTX_CUBIC_YOLOV3_TINY) return __double2float_rn(__ddiv_rn((double)u, 255.0));
+        return __double2float_rn(__dmul_rn(__dsub_rn((double)u, 127.5), 0.0078125));
+    }
+};
+
+template <int kVariant>
+__global__ void __launch_bounds__(kRcnnPreThreads) cubic_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
+                                                                           float* __restrict__ dst) {
+    cubic_band<PlanarStore<CubicInput<kVariant>>>(a, dst);
+}
+
 }  // namespace trtx
 
 using namespace trtx;
@@ -1029,6 +1173,64 @@ TRTX_API int trtx_ufld_preprocess_enqueue(const trtx_image_desc* images_host, in
                                           trtx_stream_t stream) {
     return stretch_preprocess(ufld_preprocess_kernel, images_host, batch, net_w, net_h, dst_dev,
                               static_cast<cudaStream_t>(stream));
+}
+
+// preprocess_img with INTER_CUBIC (yolov3-tiny, retinafaceAntiCov): cls_band_image's V5 rectangle, the bicubic band kernel.
+// A launch's dynamic shared memory is its widest rectangle times its most slots, so every launch is sized (and checked against
+// the budget) before the first one.
+TRTX_API int trtx_cubic_preprocess_enqueue(int variant, const trtx_image_desc* images_host, int batch, int net_w, int net_h,
+                                           float* dst_dev, trtx_stream_t stream) {
+    if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
+    if (variant != TRTX_CUBIC_YOLOV3_TINY && variant != TRTX_CUBIC_ANTICOV) return TRTX_ERR_INVALID;
+    if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
+    // every descriptor is checked before the first launch, so that a rejected call writes nothing
+    for (int i = 0; i < batch; ++i) {
+        const trtx_image_desc& d = images_host[i];
+        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
+    }
+    size_t smem_max = 0;
+    for (int i0 = 0; i0 < batch; i0 += kMaxRcnnPreImages) {
+        int wmax = 0, slots = 0;
+        for (int i = i0; i < batch && i < i0 + kMaxRcnnPreImages; ++i) {
+            RcnnPreImage im;
+            if (!cls_band_image(TRTX_YOLO_V5, images_host[i], net_w, net_h, im)) return TRTX_ERR_UNSUPPORTED;
+            wmax = im.rw > wmax ? im.rw : wmax;
+            const int s = cubic_band_slots(im.scale_y);
+            slots = s > slots ? s : slots;
+        }
+        const size_t smem = (size_t)slots * 3 * (size_t)wmax * sizeof(int);
+        if (smem > kClsMaxDynamicSmem) return TRTX_ERR_UNSUPPORTED;
+        smem_max = smem > smem_max ? smem : smem_max;
+    }
+    auto* kernel = variant == TRTX_CUBIC_YOLOV3_TINY ? cubic_preprocess_kernel<TRTX_CUBIC_YOLOV3_TINY>
+                                                     : cubic_preprocess_kernel<TRTX_CUBIC_ANTICOV>;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (smem_max > 48 * 1024 &&
+        cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) != cudaSuccess) {
+        g_last_cuda_error = (int)cudaGetLastError();
+        return TRTX_ERR_CUDA;
+    }
+    RcnnPreArgs a;
+    a.net_w = net_w;
+    a.net_h = net_h;
+    a.bands = (net_h + kRcnnPreBand - 1) / kRcnnPreBand;
+    for (int i0 = 0; i0 < batch; i0 += kMaxRcnnPreImages) {
+        const int n = batch - i0 < kMaxRcnnPreImages ? batch - i0 : kMaxRcnnPreImages;
+        int wmax = 0, slots = 0;
+        for (int j = 0; j < n; ++j) {
+            RcnnPreImage& im = a.img[j];
+            cls_band_image(TRTX_YOLO_V5, images_host[i0 + j], net_w, net_h, im);
+            im.dst_idx = i0 + j;
+            wmax = im.rw > wmax ? im.rw : wmax;
+            const int s = cubic_band_slots(im.scale_y);
+            slots = s > slots ? s : slots;
+        }
+        a.stride = 3 * wmax;
+        kernel<<<(unsigned)(n * a.bands), kRcnnPreThreads, (size_t)slots * a.stride * sizeof(int), st>>>(a, dst_dev);
+        const int rc = check_launch();
+        if (rc) return rc;
+    }
+    return TRTX_OK;
 }
 
 }  // extern "C"

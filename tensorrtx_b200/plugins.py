@@ -1416,6 +1416,25 @@ def ufld_postprocess(prob: torch.Tensor, image_sizes: Sequence[tuple[int, int]] 
     return out
 
 
+def cubic_preprocess(images: Sequence[torch.Tensor], variant: int, out: torch.Tensor | None = None, net_w: int = 608,
+                     net_h: int = 608, stream=None) -> torch.Tensor:
+    """GPU drop-in for preprocess_img with cv::resize(INTER_CUBIC) and the driver's plane loop of yolov3-tiny
+    (yolov3-tiny/yolov3-tiny.cpp:40-60, :441-445; variant _lib.CUBIC_YOLOV3_TINY, u / 255.0) and retinafaceAntiCov
+    (retinafaceAntiCov/retinafaceAntiCov.cpp:41-61, :528-532; variant _lib.CUBIC_ANTICOV, (u - 127.5) * 0.0078125, net
+    640 x 640) for a batch of device frames: images[i] is a u8 HWC BGR cuda tensor [h, w, 3] with packed pixels (rows may be
+    pitched, sizes may differ) -> [B, 3, net_h, net_w] float32 planes in R, G, B order, the engine input: the letterbox on a
+    128-grey canvas, resized as OpenCV's own 8-bit INTER_CUBIC (without IPP) does, bit for bit.  One launch per 64 images,
+    no synchronisation."""
+    lib = L.load()
+    n = len(images)
+    descs = _image_descs(images)
+    out = _out_tensor(out, (n, 3, net_h, net_w), torch.float32, images[0].device if n else "cuda",
+                      f"out must be float32 [{n}, 3, {net_h}, {net_w}]", contiguous=False)
+    L.check(lib.trtx_cubic_preprocess_enqueue(variant, descs, n, net_w, net_h, _ptr(out), _stream(stream)),
+            "trtx_cubic_preprocess_enqueue")
+    return out
+
+
 def cls_postprocess(logits: torch.Tensor, k: int, softmax: bool, probs: bool = False, stream=None):
     """GPU drop-in for the cls drivers' softmax (softmax=True: yolov8, yolo11, yolov5) or raw output (softmax=False: yolo26)
     and topk(res, k): logits [B, C] float32 cuda -> (index [B, k] int32, value [B, k] float32[, probs [B, C] float32]).  The
