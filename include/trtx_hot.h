@@ -474,7 +474,10 @@ typedef struct trtx_mask_params {
 /* proto_dev: [batch, num_coeffs, mask_h, mask_w] fp32 (the engine's "proto" output);
  * dets_dev : [batch, 1 + max_rows*row_floats] fp32 = count, rows (e.g. the compact NMS output with
  *            extra_floats = 32, extra_offset = 6: row_floats = 39, coeff_offset = 7);
- * masks_dev: [batch, max_masks, net_h, net_w] fp32; slots >= count are left untouched.  One launch. */
+ * masks_dev: [batch, max_masks, net_h, net_w] fp32; slots >= count are left untouched.  One launch.
+ * A box for which one of get_downscale_rect's float -> int conversions is undefined in the reference (a non-finite box, or
+ * a corner or size outside the int range in mask cells) gets an all-zero mask, as get_rect gives it {0, 0, 0, 0}.
+ * TRTX_ERR_UNSUPPORTED for net != 4 * mask, or batch * max_masks > 65535 (nothing is launched). */
 TRTX_API int trtx_process_mask_enqueue(const trtx_mask_params* p, int batch, const float* proto_dev, const float* dets_dev,
                                        int max_rows, float* masks_dev, trtx_stream_t stream);
 
@@ -507,10 +510,21 @@ typedef trtx_frame trtx_rcnn_image;
  * proto_dev [B, num_coeffs, mask_h, mask_w] may be NULL only when every masks_dev is NULL; NULL and non-NULL masks_dev in one
  * call is TRTX_ERR_INVALID.  Everything is checked before the first launch (a rejected call writes nothing):
  * TRTX_ERR_INVALID for null pointers, batch / max_rows / sizes <= 0, pitch < img_w; TRTX_ERR_UNSUPPORTED for an image whose
- * scale_mask crop is empty (e.g. 1 x 5000: the reference's cv::resize throws).  Two launches per 64 images, no workspace. */
+ * scale_mask crop is empty (e.g. 1 x 5000: the reference's cv::resize throws), and for nets whose canvas launch would need
+ * more than 226 KB of shared memory (227 KB less a 1 KB margin for the kernel's static arrays; square nets above 2408^2
+ * with a frame of a few pixels).  Two launches per 64 images, no
+ * workspace. */
 TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const trtx_frame* images_host, int batch,
                                                const float* proto_dev, const float* dets_dev, int max_rows,
                                                float* rows_dev, trtx_stream_t stream);
+
+/* Host only, no device work: the shared memory the canvas launches of trtx_yolo_seg_postprocess_enqueue would use for these
+ * frames (with canvases; masks_dev is not read), so a caller can check a set of frame sizes before enqueueing.  caps =
+ * {M rows, low-resolution rows, M columns, low-resolution columns, dynamic shared-memory bytes}, each the largest over the
+ * call's launches of 64 frames.  Returns what the enqueue would return for this geometry: TRTX_OK, TRTX_ERR_UNSUPPORTED for
+ * an empty scale_mask crop or caps above 226 KB (caps then hold the launches sized so far), TRTX_ERR_INVALID for null
+ * pointers or sizes <= 0. */
+TRTX_API int trtx_yolo_seg_launch_caps(const trtx_mask_params* p, const trtx_frame* images_host, int batch, int32_t caps[5]);
 
 /* The pose and oriented-box models' last host stage on the device: draw_bbox_keypoints_line's get_rect_adapt_landmark
  * (yolov8/src/postprocess.cpp:173-205) and draw_bbox_obb's get_corner (:474-507; yolo11/src/postprocess.cpp:504-537), for a

@@ -1042,6 +1042,8 @@ ORACLE_API int oracle_yolov8_decode_nms_image(const float* const* inputs /* per 
  * cv::resize(CV_32FC1, INTER_LINEAR) restated from OpenCV's resize.cpp (fx = (dx+0.5)*scale-0.5, floor, clamp with
  * zero fraction, horizontal pass then vertical pass in float); checked against cv2 4.13 in tests/test_oracle_cpu.py.
  * The x/y loops are clamped to the mask (the reference would index out of bounds for a yolov5 box leaving the image).
+ * Where one of get_downscale_rect's float -> int conversions is undefined (NaN, +-inf, past the int range; x86 gives
+ * INT_MIN) the mask stays all zeros, as the library documents; rx + rw is summed in 64 bits.
  * ------------------------------------------------------------------------------------------ */
 static void resize_tap(int d, double scale, int src, int* s0, float* f) {
     float fx = (float)(((double)d + 0.5) * scale - 0.5);
@@ -1078,11 +1080,17 @@ ORACLE_API void oracle_resize_bilinear(const float* src, int sh, int sw, float* 
         }
     }
 }
+/* (int)v and (int)round(v) where they are defined */
+static int trunc_fits(float v) { return v >= -2147483648.0f && v < 2147483648.0f; }
+static int round_fits(float v) {
+    double r = round((double)v);
+    return r >= -2147483648.0 && r <= 2147483647.0;
+}
 ORACLE_API void oracle_process_mask(int variant, const float* proto, int nm, int mh, int mw, int net_w, int net_h,
                                     const float* bbox, const float* coeffs, float* out) {
     float* m = (float*)calloc((size_t)mh * mw, sizeof(float)); /* cv::Mat::zeros */
     float left, top, right, bottom;
-    int rx, ry, rw, rh;
+    int rx = 0, ry = 0, rw = 0, rh = 0;
     if (variant == 0) { /* yolov8_seg.cpp:17-34 */
         left = bbox[0];
         top = bbox[1];
@@ -1096,10 +1104,12 @@ ORACLE_API void oracle_process_mask(int variant, const float* proto, int nm, int
         top /= 4.0f;
         right /= 4.0f;
         bottom /= 4.0f;
-        rx = (int)left;
-        ry = (int)top;
-        rw = (int)(right - left);
-        rh = (int)(bottom - top);
+        if (trunc_fits(left) && trunc_fits(top) && trunc_fits(right - left) && trunc_fits(bottom - top)) {
+            rx = (int)left;
+            ry = (int)top;
+            rw = (int)(right - left);
+            rh = (int)(bottom - top);
+        }
     } else { /* yolov5/src/postprocess.cpp:94-104 */
         left = bbox[0] - bbox[2] / 2;
         top = bbox[1] - bbox[3] / 2;
@@ -1109,15 +1119,18 @@ ORACLE_API void oracle_process_mask(int variant, const float* proto, int nm, int
         top /= 4.0f;
         right /= 4.0f;
         bottom /= 4.0f;
-        rx = (int)round(left);
-        ry = (int)round(top);
-        rw = (int)round(right - left);
-        rh = (int)round(bottom - top);
+        if (round_fits(left) && round_fits(top) && round_fits(right - left) && round_fits(bottom - top)) {
+            rx = (int)round(left);
+            ry = (int)round(top);
+            rw = (int)round(right - left);
+            rh = (int)round(bottom - top);
+        }
     }
     size_t plane = (size_t)mh * mw; /* proto_size / 32 */
-    for (int x = rx; x < rx + rw; ++x) {
-        for (int y = ry; y < ry + rh; ++y) {
-            if (x < 0 || x >= mw || y < 0 || y >= mh) continue;
+    const long long x_hi = (long long)rx + rw < mw ? (long long)rx + rw : mw;
+    const long long y_hi = (long long)ry + rh < mh ? (long long)ry + rh : mh;
+    for (long long x = rx > 0 ? rx : 0; x < x_hi; ++x) {
+        for (long long y = ry > 0 ? ry : 0; y < y_hi; ++y) {
             float e = 0.0f;
             for (int j = 0; j < nm; ++j) e += coeffs[j] * proto[(size_t)j * plane + (size_t)y * mw + x];
             m[(size_t)y * mw + x] = 1.0f / (1.0f + expf(-e));

@@ -185,6 +185,7 @@ SYMBOLS = {
     "trtx_cls_preprocess_enqueue": (_i, [_i, C.POINTER(ImageDesc), _i, _i, _i, _vp, _vp]),
     "trtx_cls_postprocess_enqueue": (_i, [_i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp]),
     "trtx_yolo_seg_postprocess_enqueue": (_i, [C.POINTER(MaskParams), C.POINTER(Frame), _i, _vp, _vp, _i, _vp, _vp]),
+    "trtx_yolo_seg_launch_caps": (_i, [C.POINTER(MaskParams), C.POINTER(Frame), _i, C.POINTER(C.c_int32)]),
     "trtx_get_corner": (_i, [_i, _i, _i, _i, C.POINTER(C.c_float), _f, C.POINTER(C.c_int)]),
     "trtx_yolo_pose_obb_postprocess_enqueue": (_i, [C.POINTER(PoseObbParams), C.POINTER(C.c_int32), _i, _vp, _i, _vp, _vp]),
     "trtx_retina_postprocess_enqueue": (_i, [C.POINTER(FacePostParams), C.POINTER(C.c_int32), _i, _vp, _i, _vp, _vp]),

@@ -36,12 +36,25 @@ struct MaskArgs {
     int variant, nm, mw, mh, net_w, net_h, max_masks;
 };
 
+// (int)v where it is defined: v truncated toward zero fits an int.  False for NaN, +-inf and values past the int range
+// (in float, v >= -2^31 is the same as trunc(v) >= INT_MIN).
+__device__ __forceinline__ bool trunc_to_int(float v, int& out) {
+    if (!(v >= -2147483648.0f && v < 2147483648.0f)) return false;
+    out = (int)v;
+    return true;
+}
+
 // get_downscale_rect: yolov8_seg.cpp:17-34 (bbox used as x, y, w, h; clamped to the network input; int() truncation),
-// yolov5/src/postprocess.cpp:94-104 (cx, cy, w, h; round()).  The loops of process_mask are additionally clamped to
-// the mask here (the reference would write out of bounds for a v5 box that leaves the image).
-__device__ __forceinline__ void downscale_rect(int variant, const float* bbox, int net_w, int net_h, int& rx, int& ry,
-                                               int& rw, int& rh) {
+// yolov5/src/postprocess.cpp:94-104 (cx, cy, w, h; round()), as the cells [x_lo, x_hi) x [y_lo, y_hi) of the mw x mh mask
+// that process_mask's loops visit.  The loops are clamped to the mask here (the reference would write out of bounds for a
+// v5 box that leaves the image).  Where one of the four float -> int conversions is undefined (a non-finite box, or a
+// corner or size past the int range in cells) the range is empty, so the mask is all zeros, as get_rect gives {0, 0, 0, 0}
+// for such boxes; rx + rw is summed in 64 bits.
+__device__ __forceinline__ void downscale_rect(int variant, const float* bbox, int net_w, int net_h, int mw, int mh,
+                                               int& x_lo, int& x_hi, int& y_lo, int& y_hi) {
     float left, top, right, bottom;
+    int rx, ry, rw, rh;
+    bool defined;
     if (variant == TRTX_YOLO_V8) {
         left = bbox[0];
         top = bbox[1];
@@ -55,10 +68,8 @@ __device__ __forceinline__ void downscale_rect(int variant, const float* bbox, i
         top = __fdiv_rn(top, 4.0f);
         right = __fdiv_rn(right, 4.0f);
         bottom = __fdiv_rn(bottom, 4.0f);
-        rx = (int)left;
-        ry = (int)top;
-        rw = (int)__fsub_rn(right, left);
-        rh = (int)__fsub_rn(bottom, top);
+        defined = trunc_to_int(left, rx) && trunc_to_int(top, ry) && trunc_to_int(__fsub_rn(right, left), rw) &&
+                  trunc_to_int(__fsub_rn(bottom, top), rh);
     } else {
         left = __fsub_rn(bbox[0], __fdiv_rn(bbox[2], 2.0f));
         top = __fsub_rn(bbox[1], __fdiv_rn(bbox[3], 2.0f));
@@ -68,11 +79,19 @@ __device__ __forceinline__ void downscale_rect(int variant, const float* bbox, i
         top = __fdiv_rn(top, 4.0f);
         right = __fdiv_rn(right, 4.0f);
         bottom = __fdiv_rn(bottom, 4.0f);
-        rx = (int)round((double)left);
-        ry = (int)round((double)top);
-        rw = (int)round((double)__fsub_rn(right, left));
-        rh = (int)round((double)__fsub_rn(bottom, top));
+        defined = round_to_int(left, rx) && round_to_int(top, ry) && round_to_int(__fsub_rn(right, left), rw) &&
+                  round_to_int(__fsub_rn(bottom, top), rh);
     }
+    if (!defined) {
+        x_lo = x_hi = y_lo = y_hi = 0;
+        return;
+    }
+    // the 64-bit ends are clamped to [0, mw] and [0, mh] before they narrow: a V5 box with rx and rw both near INT_MIN
+    // sums below INT_MIN, which would wrap to a large positive end
+    x_lo = max(rx, 0);
+    x_hi = (int)max(0LL, min((long long)rx + rw, (long long)mw));
+    y_lo = max(ry, 0);
+    y_hi = (int)max(0LL, min((long long)ry + rh, (long long)mh));
 }
 
 // OpenCV bilinear source coordinate for destination index d: (first tap, fraction)
@@ -131,9 +150,8 @@ __global__ void __launch_bounds__(256) process_mask_kernel(const __grid_constant
     const int count = min(max((int)img[0], 0), min(a.max_rows, a.max_masks));
     if (m >= count) return;  // slots past the image's detections are left untouched
     const float* det = img + 1 + (size_t)m * a.row_floats;
-    int rx, ry, rw, rh;
-    downscale_rect(a.variant, det, a.net_w, a.net_h, rx, ry, rw, rh);
-    const int x_lo = max(rx, 0), x_hi = min(rx + rw, a.mw), y_lo = max(ry, 0), y_hi = min(ry + rh, a.mh);
+    int x_lo, x_hi, y_lo, y_hi;
+    downscale_rect(a.variant, det, a.net_w, a.net_h, a.mw, a.mh, x_lo, x_hi, y_lo, y_hi);
     const int cx0 = blockIdx.x * kMaskTile - 1, cy0 = blockIdx.y * kMaskTile - 1;  // first halo cell
     const int tid = threadIdx.x;
     const bool touches = x_lo < x_hi && y_lo < y_hi && cx0 < x_hi && cx0 + kMaskHalo > x_lo && cy0 < y_hi && cy0 + kMaskHalo > y_lo;
@@ -766,6 +784,10 @@ constexpr int kSegThreads = 256;
 constexpr int kSegMaxY = 2 * kSegBand;     // rows of M a band can need: two taps per canvas row
 constexpr int kSegMaxLY = 2 * kSegMaxY;    // low-resolution rows those can need
 constexpr int kSegRowFloats = 6;           // x, y, w, h, conf, class
+// dynamic shared memory of a canvas launch at most: 227 KB per CTA less a 1 KB margin for the kernel's static arrays
+// (752 B today), so the limit does not move when they do.  The margin, not the hardware, makes 2408^2 the largest square
+// net for a frame of a few pixels (2412^2 would need 231 552 B + 752 B, which an H100 could still launch).
+constexpr size_t kSegMaxDynamicSmem = 227 * 1024 - 1024;
 
 struct SegImage {
     uint8_t* canvas;     // [max_masks, img_h, pitch] u8, or nullptr (rows only)
@@ -841,8 +863,8 @@ __global__ void __launch_bounds__(kSegThreads) seg_canvas_kernel(const __grid_co
     int rect[4];
     const bool defined = yolo_get_rect(a.variant, a.net_w, a.net_h, im.img_w, im.img_h, det, rect);
     // get_rect clipped to the image (a V5 rect may leave it; the reference's loop would read outside img_mask there)
-    const int x_lo = max(rect[0], 0), x_hi = (int)min((long long)rect[0] + rect[2], (long long)im.img_w);
-    const int y_lo = max(rect[1], 0), y_hi = (int)min((long long)rect[1] + rect[3], (long long)im.img_h);
+    const int x_lo = max(rect[0], 0), x_hi = (int)max(0LL, min((long long)rect[0] + rect[2], (long long)im.img_w));
+    const int y_lo = max(rect[1], 0), y_hi = (int)max(0LL, min((long long)rect[1] + rect[3], (long long)im.img_h));
     const int y0 = band * kSegBand, y1 = min(y0 + kSegBand, im.img_h);
     const int ya = max(y_lo, y0), yb = min(y_hi, y1);
     const bool touches = defined && x_lo < x_hi && ya < yb;  // uniform over the CTA
@@ -888,9 +910,8 @@ __global__ void __launch_bounds__(kSegThreads) seg_canvas_kernel(const __grid_co
         __syncthreads();
         const int ny = s_ny, nly = s_nly;
         // low-resolution cells: sigmoid(coeffs . proto) inside get_downscale_rect, 0 outside (process_mask_kernel)
-        int rx, ry, rw, rh;
-        downscale_rect(a.variant, det, a.net_w, a.net_h, rx, ry, rw, rh);
-        const int dx_lo = max(rx, 0), dx_hi = min(rx + rw, a.mw), dy_lo = max(ry, 0), dy_hi = min(ry + rh, a.mh);
+        int dx_lo, dx_hi, dy_lo, dy_hi;
+        downscale_rect(a.variant, det, a.net_w, a.net_h, a.mw, a.mh, dx_lo, dx_hi, dy_lo, dy_hi);
         const size_t plane = (size_t)a.mh * a.mw;
         const float* proto = a.proto + (size_t)b * a.nm * plane;
         for (int c = tid; c < nly * nLX; c += blockDim.x) {
@@ -990,7 +1011,8 @@ static void seg_caps(double s, int& y_cap, int& ly_cap) {
 // The launch arguments of images [i0, i0 + n) of a trtx_yolo_seg_postprocess_enqueue call (n <= kMaxFrames): sizes and
 // canvases, and with canvases each image's scale_mask crop, the launch's shared-memory caps, its canvas CTAs `ctas` and
 // dynamic shared memory `smem` (both 0 without canvases).  TRTX_ERR_UNSUPPORTED for an empty crop (the reference's
-// cv::resize throws) or more than INT_MAX CTAs.
+// cv::resize throws), more than INT_MAX CTAs, or caps that need more than kSegMaxDynamicSmem (a net of more than 2408^2
+// for a frame of a few pixels: M rows x crop width grows with the net).
 static int seg_fill_frames(const trtx_mask_params* p, const trtx_frame* frames, int i0, int n, bool canvases, SegArgs& a,
                            int& ctas, size_t& smem) {
     a.base = i0;
@@ -1026,7 +1048,7 @@ static int seg_fill_frames(const trtx_mask_params* p, const trtx_frame* frames, 
     a.lx_cap = min(p->mask_w, a.x_cap / 4 + 4);
     ctas = (int)total;
     smem = canvases ? ((size_t)a.y_cap * a.x_cap + (size_t)a.ly_cap * a.lx_cap) * sizeof(float) : 0;
-    return TRTX_OK;
+    return smem > kSegMaxDynamicSmem ? TRTX_ERR_UNSUPPORTED : TRTX_OK;
 }
 
 // Per-row geometry post-processes: the per-detection host stage the reference runs on one core after a D2H copy, for a
@@ -1621,6 +1643,29 @@ TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const 
         if (!masks) continue;
         seg_canvas_kernel<<<(unsigned)ctas, kSegThreads, smem, st>>>(a);
         if ((rc = check_launch())) return rc;
+    }
+    return TRTX_OK;
+}
+
+TRTX_API int trtx_yolo_seg_launch_caps(const trtx_mask_params* p, const trtx_frame* images_host, int batch, int32_t caps[5]) {
+    if (!p || !images_host || !caps || batch <= 0) return TRTX_ERR_INVALID;
+    if (p->net_w <= 0 || p->net_h <= 0 || p->mask_w <= 0 || p->mask_h <= 0) return TRTX_ERR_INVALID;
+    for (int i = 0; i < batch; ++i)
+        if (images_host[i].img_w <= 0 || images_host[i].img_h <= 0) return TRTX_ERR_INVALID;
+    SegArgs a;
+    int ctas, rc;
+    size_t smem;
+    caps[0] = caps[1] = caps[2] = caps[3] = caps[4] = 0;
+    for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {  // the launches trtx_yolo_seg_postprocess_enqueue makes
+        a.lx_cap = 0;  // set last: still 0 where a frame is refused before
+        smem = 0;
+        rc = seg_fill_frames(p, images_host, i0, min(batch - i0, kMaxFrames), true, a, ctas, smem);
+        caps[0] = max(caps[0], a.y_cap);
+        caps[1] = max(caps[1], a.ly_cap);
+        caps[2] = max(caps[2], a.x_cap);
+        caps[3] = max(caps[3], a.lx_cap);
+        caps[4] = max(caps[4], (int32_t)min(smem, (size_t)INT32_MAX));
+        if (rc) return rc;
     }
     return TRTX_OK;
 }

@@ -657,6 +657,17 @@ def yolo_seg_postprocess(proto: torch.Tensor | None, dets: torch.Tensor, image_s
     return rows_out, canvases_out
 
 
+def yolo_seg_launch_caps(image_sizes: Sequence[tuple[int, int]], *, net_w: int = 640, net_h: int = 640) -> tuple[int, ...]:
+    """The shared memory yolo_seg_postprocess's canvas launches would use for frames of image_sizes[b] = (img_w, img_h), from
+    the host alone: (M rows, low-resolution rows, M columns, low-resolution columns, dynamic shared-memory bytes), each the
+    largest over the call's launches.  Raises TrtxError (UNSUPPORTED) where the enqueue would refuse these frames."""
+    descs, _ = _frames(image_sizes, None, 0, None, False)
+    q = L.MaskParams(L.YOLO_V8, net_w, net_h, net_w // 4, net_h // 4, 32, 39, 7, 1)
+    caps = (C.c_int32 * 5)()
+    L.check(L.load().trtx_yolo_seg_launch_caps(C.byref(q), descs, len(image_sizes), caps), "trtx_yolo_seg_launch_caps")
+    return tuple(caps)
+
+
 def yolo_pose_obb_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]], *, task: int, max_rows: int,
                               row_floats: int | None = None, extra_offset: int | None = None, num_kpts: int = 17,
                               net_w: int = 640, net_h: int = 640, rows_out: torch.Tensor | None = None,
