@@ -51,7 +51,7 @@ TRTX_API int trtx_last_cuda_error(void);
  * mirror of the layout: which = 0 trtx_yolo_params, 1 trtx_nms_params, 2 trtx_retina_params, 3 trtx_image_desc,
  * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_frame, 7 trtx_pose_obb_params, 8 trtx_frame,
  * 9 trtx_face_post_params, 10 trtx_yolop_post_params, 11 trtx_detr_post_params, 12 trtx_centernet_params,
- * 13 trtx_ufld_post_params;
+ * 13 trtx_ufld_post_params, 14 trtx_refinedet_params;
  * anything else 0. */
 TRTX_API size_t trtx_abi_sizeof(int which);
 
@@ -974,6 +974,79 @@ enum {
  * graph. */
 TRTX_API int trtx_cubic_preprocess_enqueue(int variant, const trtx_image_desc* images_host, int batch, int net_w, int net_h,
                                            float* dst_dev, trtx_stream_t stream);
+
+/* =====================================================================================
+ * 14. RefineDet pre- and post-process
+ *    replaces base_transform of refinedet/refinedet.cpp (:822-839) and the H2D copy of its input, and the float64 tensor
+ *    post-process of doInference (:730-815: PriorBox, the two decode steps, the ARM filter, the per-class nms() and the rows)
+ *    with the driver's rectangles (:957-993 with RoiCorrect, :22-35).  Drawing and the text files stay with the caller.
+ * ===================================================================================== */
+/* base_transform for a whole batch, one launch per <= 64 images: images_host = `batch` u8 HWC BGR descriptors in HOST memory
+ * (trtx_image_desc, any pitch and base alignment, mixed sizes allowed); dst_dev = [batch, 3, net, net] fp32 planes, the
+ * engine input (INPUT_W = INPUT_H = 320; the reference indexes its planes with `i * INPUT_H + j`, right for square nets only,
+ * so the call takes one side).  The whole frame is stretched over the net by OpenCV 4.x's 8-bit INTER_LINEAR, bit for bit;
+ * plane 0 = R - 123, plane 1 = G - 117, plane 2 = B - 104 (exact in float).  Gray frames are not accepted.  Every descriptor
+ * is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer, batch / net <= 0,
+ * pitch < 3 * width or a dst_dev that is not 4-byte aligned; TRTX_ERR_UNSUPPORTED for a net above 4 757 (the band's staged
+ * source rows in shared memory).  No workspace; can be captured in a CUDA graph. */
+TRTX_API int trtx_refinedet_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net, float* dst_dev,
+                                               trtx_stream_t stream);
+
+typedef struct trtx_refinedet_params {
+    int32_t net;          /* S: the net side, 320; the priors are the four levels of side S / 8, S / 16, S / 32, S / 64 */
+    int32_t num_classes;  /* C: num_class = 25, class 0 the background */
+    float obj_thresh;     /* 0.01f: a prior keeps its ODM scores where arm_conf[p, 1] > obj_thresh */
+    float conf_thresh;    /* 0.01f: a class score is a candidate where it is > conf_thresh */
+    float nms_thresh;     /* 0.45f: overlap */
+    int32_t top_k;        /* 1000: the highest candidates of a class that enter its NMS */
+    int32_t max_det;      /* rows kept per frame; (C - 1) * top_k keeps every row the reference keeps */
+    float score_thresh;   /* frame rows only: TH = 0.2f */
+} trtx_refinedet_params;
+
+/* Workspace of trtx_refinedet_postprocess_enqueue: B * (C - 1) * (4 + 2 * top_k) bytes in two 256-byte aligned parts; 0 for
+ * rejected params. */
+TRTX_API size_t trtx_refinedet_workspace_size(const trtx_refinedet_params* p, int batch);
+
+/* doInference's post-process for a batch: arm_loc_dev [B, P, 4], arm_conf_dev [B, P, 2] (softmaxed), odm_loc_dev [B, P, 4],
+ * odm_conf_dev [B, P, C] (softmaxed), all fp32, P = 3 * ((S/8)^2 + (S/16)^2 + (S/32)^2 + (S/64)^2) (6375 at S = 320), prior
+ * index = level offset + (y * f + x) * 3 + k.
+ * dets_dev [B, 1 + max_det * 6] fp32: n = min(total, max_det), then the reference's rows (x1, y1, x2, y2, score, label) in its
+ * order -- classes ascending, each in keep order -- rounded to float as the driver's std::vector<float> holds them, zeros
+ * past n.  Everything is the reference's float64 arithmetic, each tensor op rounded on its own (no contraction):
+ *   priors   PriorBox (:553-597) in float: f_k = (float)(S / step), cx = (j + .5) / f_k, s_k = min_size / S (steps 8, 16, 32,
+ *            64, min sizes 32, 64, 128, 256), anchors (s_k, s_k), (s_k * sqrt2, s_k / sqrt2), (s_k / sqrt2, s_k * sqrt2) in
+ *            double rounded to float with sqrt2 = sqrtf(2.f), clamped to [0, 1].  The reference's headers decide which
+ *            overload its `sqrt(ar)` names (with libstdc++, any <math.h> among them makes it the float one); the double
+ *            overload gives the same table at S = 320 but differs in some anchors' last bit at S = 192, 384, 448 and
+ *            704 .. 960;
+ *   decode   d = (p01 + (l01 * v0) * p23, p23 * exp(l23 * v1)) over the prior with arm_loc, then the same over d with odm_loc,
+ *            v0 = (double)0.1f, v1 = (double)0.2f, exp the CUDA double exp (ATen's); x1 = cx - w / 2, x2 = x1 + w;
+ *   filter   score = odm_conf where arm_conf[p, 1] > obj_thresh, else odm_conf * 0.0 (inf and NaN become NaN); class c in
+ *            1 .. C-1 takes the priors with score > conf_thresh (a NaN never) in the reference's order;
+ *   nms      per class: the top_k highest candidates, then greedily the highest remaining box i is kept and every remaining j
+ *            with !(IoU < nms_thresh) dropped (a NaN IoU drops j).  IoU clamps j's corners with i's rounded to float
+ *            (`x1[i].item().toFloat()`; a finite value beyond the float range, where the reference throws, rounds to inf),
+ *            as Tensor::clamp (a NaN bound gives NaN); w, h clamped to [0, INT_MAX]; inter = w * h;
+ *            IoU = inter * 1.0 / ((area_j - inter) + area_i), areas (x2 - x1) * (y2 - y1) in double.
+ *            Ties: the reference's CUDA sort leaves the order among equal scores, and the top_k cut at a tie, open; here a lower
+ *            prior index ranks higher.
+ * The reference's `score_my[0] < conf_thresh` class skip never fires (a kept score is above conf_thresh).
+ * Frame rows, when frame_wh_host (`batch` pairs cols, rows in HOST memory, copied into launch parameters) and rows_dev
+ * [B, 1 + max_det * 6] are both given: the count, then per det row in order with score >= score_thresh (the driver's
+ * `if (score < TH) continue`) (x, y, w, h, score, label) with x = (int)(x1 * cols) (a float product), w = (int)(x2 * cols -
+ * x) in float, likewise y and h, then RoiCorrect: x < 0 -> 0, y < 0 -> 0, x >= cols - 1 -> 0, y >= rows - 1 -> 0, w <= 0 -> 1,
+ * h <= 0 -> 1, x + w > cols - 1 -> w = cols - 1 - x, likewise h.  Conversions as x86-64 performs them (INT_MIN for NaN,
+ * inf and out of range), x + w wrapping as there; zeros past the count.
+ * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
+ * batch, net, top_k or max_det <= 0, C < 2, a NaN threshold, only one of frame_wh_host / rows_dev or a frame side <= 0;
+ * TRTX_ERR_WORKSPACE for a short workspace; TRTX_ERR_INVALID for a workspace that is not 256-byte aligned;
+ * TRTX_ERR_UNSUPPORTED for S not a multiple of 64, P > 2^16 (S > 1024), top_k > 1024, C > 1024, max_det > 2^24 or a frame
+ * side above 2^24.  Two launches per call (one more per 64 frames past the first 64), no host sync, no allocation; can be
+ * captured in a CUDA graph. */
+TRTX_API int trtx_refinedet_postprocess_enqueue(const trtx_refinedet_params* p, int batch, const float* arm_loc_dev,
+                                                const float* arm_conf_dev, const float* odm_loc_dev, const float* odm_conf_dev,
+                                                void* workspace_dev, size_t workspace_bytes, float* dets_dev,
+                                                const int32_t* frame_wh_host, float* rows_dev, trtx_stream_t stream);
 
 #ifdef __cplusplus
 }

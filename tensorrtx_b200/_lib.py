@@ -130,6 +130,12 @@ class UfldPostParams(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("num_cells", "num_rows", "num_lanes", "net_w", "net_h", "col_sample_w")]
 
 
+class RefinedetParams(C.Structure):
+    _fields_ = [("net", C.c_int32), ("num_classes", C.c_int32),
+                *[(n, C.c_float) for n in ("obj_thresh", "conf_thresh", "nms_thresh")],
+                ("top_k", C.c_int32), ("max_det", C.c_int32), ("score_thresh", C.c_float)]
+
+
 # TRTX_LIB: another build of the same ABI (the probe build of tools/nms_probe.py); default = the in-tree release library
 LIB_PATH = Path(os.environ.get("TRTX_LIB") or Path(__file__).resolve().parent / "lib" / "libtrtx_hot.so")
 
@@ -203,6 +209,10 @@ SYMBOLS = {
     "trtx_ufld_postprocess_enqueue": (_i, [C.POINTER(UfldPostParams), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _i, _vp,
                                            _vp, _vp]),
     "trtx_cubic_preprocess_enqueue": (_i, [_i, C.POINTER(ImageDesc), _i, _i, _i, _vp, _vp]),
+    "trtx_refinedet_preprocess_enqueue": (_i, [C.POINTER(ImageDesc), _i, _i, _vp, _vp]),
+    "trtx_refinedet_workspace_size": (_sz, [C.POINTER(RefinedetParams), _i]),
+    "trtx_refinedet_postprocess_enqueue": (_i, [C.POINTER(RefinedetParams), _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp,
+                                                C.POINTER(C.c_int32), _vp, _vp]),
     "trtx_yolo_decode_nms_gather_enqueue": (_i, [C.POINTER(YoloParams), C.POINTER(NmsParams), _i, _pp, _vp, _vp, _vp, _sz,
                                                  C.POINTER(Gather), _vp]),
     "trtx_gather_wait_enqueue": (_i, [C.POINTER(Gather), _vp]),
@@ -235,7 +245,7 @@ def load() -> C.CDLL:
         fn.argtypes = args
     for which, st in enumerate((YoloParams, NmsParams, RetinaParams, ImageDesc, MaskParams, RcnnPostParams,
                                    Frame, PoseObbParams, Frame, FacePostParams, YolopPostParams,
-                                   DetrPostParams, CenternetParams, UfldPostParams)):
+                                   DetrPostParams, CenternetParams, UfldPostParams, RefinedetParams)):
         if lib.trtx_abi_sizeof(which) != C.sizeof(st):
             raise TrtxError(f"{LIB_PATH} was built from a different trtx_hot.h: sizeof({st.__name__}) = "
                             f"{lib.trtx_abi_sizeof(which)} in the library, {C.sizeof(st)} in the binding (rebuild)")

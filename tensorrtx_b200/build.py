@@ -20,7 +20,7 @@ LIBDIR = PKG / "lib"
 LIB = LIBDIR / "libtrtx_hot.so"
 
 SOURCES = ["yolo_decode.cu", "nms.cu", "retina_decode.cu", "rcnn.cu", "preprocess.cu", "mask.cu", "roi_align.cu", "calib_host.cu", "cls.cu",
-           "detr.cu", "centernet.cu", "ufld.cu"]
+           "detr.cu", "centernet.cu", "ufld.cu", "refinedet.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -87,7 +87,7 @@ def build(force: bool = False, verbose: bool = False, probe: bool = False) -> Pa
 
 def build_oracle() -> Path:
     """Compile the CPU oracles (test infrastructure) and, when /root/reference exists, oracle/_ref."""
-    for makefile in ("Makefile", "yolop.mk", "detr.mk", "centernet.mk", "ufld.mk", "cubic.mk"):
+    for makefile in ("Makefile", "yolop.mk", "detr.mk", "centernet.mk", "ufld.mk", "cubic.mk", "refinedet.mk"):
         r = subprocess.run(["make", "-C", str(ROOT / "oracle"), "-f", makefile, f"PYTHON={sys.executable}"],
                            stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         if r.returncode != 0:

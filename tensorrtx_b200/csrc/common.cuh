@@ -399,6 +399,12 @@ __device__ __forceinline__ float ufld_input_value(int c, uint32_t u) {
     return __fmaf_rn(s, __double2float_rn(__ddiv_rn(1.0, sd)), __double2float_rn(__ddiv_rn(-mean, sd)));
 }
 
+// RefineDet's base_transform after the resize (refinedet/refinedet.cpp:822-839), the value of byte u in plane c (0 = R,
+// 1 = G, 2 = B): (float)(u * 1.0 - mean) with mean 123, 117, 104, exact in float.
+__device__ __forceinline__ float refinedet_input_value(int c, uint32_t u) {
+    return __fsub_rn((float)u, c == 0 ? 123.f : (c == 1 ? 117.f : 104.f));
+}
+
 __device__ __forceinline__ int warp_excl_scan(int v, int lane, int* total) {
     int x = v;
 #pragma unroll

@@ -620,6 +620,13 @@ struct UfldInput {
     static __device__ __forceinline__ int channel(int c) { return 2 - c; }
     static __device__ __forceinline__ float value(int c, uint32_t u) { return ufld_input_value(c, u); }
 };
+// RefineDet's base_transform (refinedet/refinedet.cpp:822-839): plane c (0 = R) reads BGR byte 2 - c of the resized frame;
+// the value is refinedet_input_value (common.cuh).
+struct RefinedetInput {
+    static constexpr uint32_t kCanvas = 0u;  // never read: the frame is stretched over the whole net
+    static __device__ __forceinline__ int channel(int c) { return 2 - c; }
+    static __device__ __forceinline__ float value(int c, uint32_t u) { return refinedet_input_value(c, u); }
+};
 
 // [B, 3, net_h, net_w] planes: the band is three contiguous runs of band * net_w floats, each written by store_band_run; the
 // value of a byte comes from a per-CTA table of 3 x 256 floats.
@@ -664,6 +671,11 @@ __global__ void __launch_bounds__(kRcnnPreThreads) detr_preprocess_kernel(const 
 __global__ void __launch_bounds__(kRcnnPreThreads) ufld_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
                                                                           float* __restrict__ dst) {
     resize_band<PlanarStore<UfldInput>>(a, dst);
+}
+
+__global__ void __launch_bounds__(kRcnnPreThreads) refinedet_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
+                                                                               float* __restrict__ dst) {
+    resize_band<PlanarStore<RefinedetInput>>(a, dst);
 }
 
 // One launch of `kernel` per kMaxRcnnPreImages frames: make(i, im) fills the band descriptor of frame i (validated before).
@@ -1172,6 +1184,13 @@ TRTX_API int trtx_detr_preprocess_enqueue(const trtx_image_desc* images_host, in
 TRTX_API int trtx_ufld_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
                                           trtx_stream_t stream) {
     return stretch_preprocess(ufld_preprocess_kernel, images_host, batch, net_w, net_h, dst_dev,
+                              static_cast<cudaStream_t>(stream));
+}
+
+// RefineDet's base_transform, likewise, on a square net with its mean-subtracted planes.
+TRTX_API int trtx_refinedet_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net, float* dst_dev,
+                                               trtx_stream_t stream) {
+    return stretch_preprocess(refinedet_preprocess_kernel, images_host, batch, net, net, dst_dev,
                               static_cast<cudaStream_t>(stream));
 }
 

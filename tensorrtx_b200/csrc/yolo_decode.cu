@@ -883,6 +883,7 @@ TRTX_API size_t trtx_abi_sizeof(int which) {
         case 11: return sizeof(trtx_detr_post_params);
         case 12: return sizeof(trtx_centernet_params);
         case 13: return sizeof(trtx_ufld_post_params);
+        case 14: return sizeof(trtx_refinedet_params);
         default: return 0;
     }
 }

@@ -1427,6 +1427,82 @@ def ufld_postprocess(prob: torch.Tensor, image_sizes: Sequence[tuple[int, int]] 
     return out
 
 
+REFINEDET_NET = 320        # INPUT_W = INPUT_H (refinedet/configure.h)
+REFINEDET_NUM_CLASSES = 25  # num_class, the background included
+REFINEDET_TOP_K = 1000     # nms()'s top_k (refinedet/refinedet.cpp:766)
+
+
+def refinedet_num_priors(net: int = REFINEDET_NET) -> int:
+    """P = 3 * ((S/8)^2 + (S/16)^2 + (S/32)^2 + (S/64)^2): 6375 at S = 320."""
+    return 3 * sum((net >> s) ** 2 for s in (3, 4, 5, 6))
+
+
+def refinedet_preprocess(images: Sequence[torch.Tensor], out: torch.Tensor | None = None, net: int = REFINEDET_NET,
+                         stream=None) -> torch.Tensor:
+    """GPU drop-in for RefineDet's base_transform (refinedet/refinedet.cpp:822-839) for a batch of device frames: images[i]
+    is a u8 HWC BGR cuda tensor [h, w, 3] with packed pixels (rows may be pitched, sizes may differ) -> [B, 3, net, net]
+    float32 planes R - 123, G - 117, B - 104 of the whole frame resized to net x net, the engine input.  One launch per 64
+    images, no synchronisation."""
+    lib = L.load()
+    n = len(images)
+    descs = _image_descs(images)
+    out = _out_tensor(out, (n, 3, net, net), torch.float32, images[0].device if n else "cuda",
+                      f"out must be float32 [{n}, 3, {net}, {net}]", contiguous=False)
+    L.check(lib.trtx_refinedet_preprocess_enqueue(descs, n, net, _ptr(out), _stream(stream)),
+            "trtx_refinedet_preprocess_enqueue")
+    return out
+
+
+def refinedet_postprocess(arm_loc: torch.Tensor, arm_conf: torch.Tensor, odm_loc: torch.Tensor, odm_conf: torch.Tensor,
+                          image_sizes: Sequence[tuple[int, int]] | None = None, *, net: int = REFINEDET_NET,
+                          obj_thresh: float = 0.01, conf_thresh: float = 0.01, nms_thresh: float = 0.45,
+                          top_k: int = REFINEDET_TOP_K, max_det: int | None = None, score_thresh: float = 0.2,
+                          workspace: torch.Tensor | None = None, out: torch.Tensor | None = None,
+                          rows_out: torch.Tensor | None = None, stream=None):
+    """GPU drop-in for RefineDet's libtorch post-process (refinedet/refinedet.cpp:730-815) on the engine outputs arm_loc
+    [B, P, 4], arm_conf [B, P, 2], odm_loc [B, P, 4] and odm_conf [B, P, C], float32 -> dets [B, 1 + max_det*6] float32: the
+    count, then (x1, y1, x2, y2, score, label) in the reference's order (classes ascending, each in NMS keep order), zeros
+    past the count.  max_det defaults to (C - 1) * top_k, every row the reference can keep.  With image_sizes[b] = (cols,
+    rows), also the driver's rectangles after `score < TH` and RoiCorrect (:957-993): rows [B, 1 + max_det*6] of (x, y, w, h,
+    score, label) -> (dets, rows).  Two launches, no synchronisation."""
+    lib = L.load()
+    if odm_conf.dim() != 3:
+        raise ValueError("odm_conf must be [B, P, C]")
+    B, Pn, Cn = (int(v) for v in odm_conf.shape)
+    if Pn != refinedet_num_priors(net):
+        raise ValueError(f"the heads hold {Pn} priors; a {net} x {net} net has {refinedet_num_priors(net)}")
+    for t, k, what in ((arm_loc, 4, "arm_loc"), (arm_conf, 2, "arm_conf"), (odm_loc, 4, "odm_loc")):
+        if tuple(t.shape) != (B, Pn, k):
+            raise ValueError(f"{what} must be [{B}, {Pn}, {k}]")
+    for t in (arm_loc, arm_conf, odm_loc, odm_conf):
+        if t.dtype != torch.float32:
+            raise ValueError("arm_loc, arm_conf, odm_loc and odm_conf must be float32")
+    if max_det is None:
+        max_det = (Cn - 1) * top_k
+    q = L.RefinedetParams(net, Cn, obj_thresh, conf_thresh, nms_thresh, top_k, max_det, score_thresh)
+    ws_bytes = int(lib.trtx_refinedet_workspace_size(C.byref(q), B))
+    if ws_bytes == 0:
+        bad = B <= 0 or net <= 0 or Cn < 2 or top_k <= 0 or max_det <= 0 or any(
+            v != v for v in (obj_thresh, conf_thresh, nms_thresh, score_thresh))
+        L.check(L.ERR_INVALID if bad else L.ERR_UNSUPPORTED, "trtx_refinedet_workspace_size")
+    if workspace is None:
+        workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=odm_conf.device)
+    row = 1 + max_det * 6
+    out = _out_tensor(out, (B, row), torch.float32, odm_conf.device, f"out must be contiguous float32 [{B}, {row}]")
+    wh_arr = None
+    if image_sizes is not None:
+        if len(image_sizes) != B:
+            raise ValueError(f"expected {B} image sizes")
+        wh_arr = _frame_wh(image_sizes)
+        rows_out = _out_tensor(rows_out, (B, row), torch.float32, odm_conf.device,
+                               f"rows_out must be contiguous float32 [{B}, {row}]")
+    L.check(lib.trtx_refinedet_postprocess_enqueue(C.byref(q), B, _ptr(arm_loc), _ptr(arm_conf), _ptr(odm_loc),
+                                                   _ptr(odm_conf), _ptr(workspace), _nbytes(workspace), _ptr(out), wh_arr,
+                                                   _ptr(rows_out) if wh_arr is not None else None, _stream(stream)),
+            "trtx_refinedet_postprocess_enqueue")
+    return (out, rows_out) if wh_arr is not None else out
+
+
 def cubic_preprocess(images: Sequence[torch.Tensor], variant: int, out: torch.Tensor | None = None, net_w: int = 608,
                      net_h: int = 608, stream=None) -> torch.Tensor:
     """GPU drop-in for preprocess_img with cv::resize(INTER_CUBIC) and the driver's plane loop of yolov3-tiny
