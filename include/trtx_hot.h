@@ -283,7 +283,10 @@ TRTX_API size_t trtx_retina_workspace_size(const trtx_retina_params* p, int batc
 /* TRTX_ERR_INVALID, before the first launch and with nothing written: a null argument, in_h or in_w < 32, an unknown variant
  * or in_dtype, an input pointer that is not a multiple of its element size (4 / 2 bytes), an output pointer that is not a
  * multiple of 4.  Inputs that are 16-byte (fp32) / 8-byte (fp16) aligned with grids of a multiple of 4 cells are read four
- * cells per load, any other one cell per load; the rows do not depend on which. */
+ * cells per load, any other one cell per load; the rows do not depend on which, and no input size is refused for either:
+ * every in_h, in_w >= 32 decodes, with floor grids (in_h/s) x (in_w/s) per axis.  The priors are placed on the level's fixed
+ * stride s = 8, 16, 32 (TRTX_RETINA_ANTICOV: 7.5 + x*s, 7.5 + y*s; not in_w / (in_w/s), which differs from s when s does not
+ * divide in_w), as the reference's forwardGpu passes it. */
 TRTX_API int trtx_retina_decode_enqueue(const trtx_retina_params* p, int batch, const void* const* inputs_dev,
                                         float* output_dev, void* workspace_dev, size_t workspace_bytes,
                                         trtx_stream_t stream);

@@ -189,7 +189,9 @@ __global__ void __launch_bounds__(128) anticov_scan_kernel(const __grid_constant
     const T* bbox_reg = cur + 4 * g;
     const T* lmk_reg = cur + 12 * g;
     const T* mask_reg = cur + 36 * g;
-    const int step = a.in_w / L.w;  // 8, 16, 32 (:162-170)
+    // The level's fixed stride 8, 16, 32 (forwardGpu's base_step, :162-170).  Not in_w / w: with floor grids that is another
+    // number whenever the stride does not divide in_w (in_w = 660 gives 33 at level 2), and it would move x and y alike.
+    const int step = 8 << l;
 #pragma unroll
     for (int j = 0; j < VEC; ++j) {
 #pragma unroll
@@ -230,41 +232,53 @@ __global__ void __launch_bounds__(128) anticov_scan_kernel(const __grid_constant
     }
 }
 
+// Tiles whose row offsets one pass of the pack holds in shared memory.  An image of more tiles takes several passes, each
+// starting from the rows of the passes before it, so no input size is refused for the pack and its shared memory is the
+// same for every call (640x640 has 67 tiles per image: one pass).
+constexpr int kPackChunk = 1024;
+
 __global__ void __launch_bounds__(256) retina_pack_kernel(const __grid_constant__ RetinaArgs a, float* __restrict__ out) {
-    extern __shared__ int s_prefix[];
+    __shared__ int s_prefix[kPackChunk + 1];
     const int b = blockIdx.x;
     const int T_ = a.tiles_per_image;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     const int* cnt = a.tile_count + (size_t)b * T_;
-    if (warp == 0) {
-        int carry = 0;
-        for (int base = 0; base < T_; base += 32) {
-            int v = (base + lane < T_) ? cnt[base + lane] : 0;
-            int tot;
-            int ex = warp_excl_scan(v, lane, &tot);
-            if (base + lane < T_) s_prefix[base + lane] = carry + ex;
-            carry += tot;
-        }
-        if (lane == 0) s_prefix[T_] = carry;
-    }
-    __syncthreads();
     const int F = a.det_floats;
     float* o = out + (size_t)b * (1 + (size_t)a.total_priors * F);
-    if (threadIdx.x == 0) o[0] = (float)s_prefix[T_];
     const int tile_slots = a.tile_cells * 2;
-    for (int t = warp; t < T_; t += nwarps) {
-        const int n = s_prefix[t + 1] - s_prefix[t];
-        if (n == 0) continue;
-        int l = 0;
-        while (l + 1 < 3 && t >= a.lv[l + 1].tile_begin) ++l;
-        const size_t slot0 =
-                (size_t)b * a.slots_per_image + a.lv[l].slot_begin + (size_t)(t - a.lv[l].tile_begin) * tile_slots;
-        // n records x F floats, copied by the whole warp
-        for (int e = lane; e < n * F; e += 32) {
-            const int j = e / F, f = e - j * F;
-            o[1 + (size_t)(s_prefix[t] + j) * F + f] = a.cand[(slot0 + j) * 16 + f];
+    int carry = 0;  // rows of the tiles before this pass
+    for (int c0 = 0; c0 < T_; c0 += kPackChunk) {
+        const int nt = min(kPackChunk, T_ - c0);
+        if (warp == 0) {
+            int run = carry;
+            for (int base = 0; base < nt; base += 32) {
+                int v = (base + lane < nt) ? cnt[c0 + base + lane] : 0;
+                int tot;
+                int ex = warp_excl_scan(v, lane, &tot);
+                if (base + lane < nt) s_prefix[base + lane] = run + ex;
+                run += tot;
+            }
+            if (lane == 0) s_prefix[nt] = run;
         }
+        __syncthreads();
+        for (int i = warp; i < nt; i += nwarps) {
+            const int n = s_prefix[i + 1] - s_prefix[i];
+            if (n == 0) continue;
+            const int t = c0 + i;
+            int l = 0;
+            while (l + 1 < 3 && t >= a.lv[l + 1].tile_begin) ++l;
+            const size_t slot0 =
+                    (size_t)b * a.slots_per_image + a.lv[l].slot_begin + (size_t)(t - a.lv[l].tile_begin) * tile_slots;
+            // n records x F floats, copied by the whole warp
+            for (int e = lane; e < n * F; e += 32) {
+                const int j = e / F, f = e - j * F;
+                o[1 + (size_t)(s_prefix[i] + j) * F + f] = a.cand[(slot0 + j) * 16 + f];
+            }
+        }
+        carry = s_prefix[nt];
+        __syncthreads();  // the next pass rewrites s_prefix
     }
+    if (threadIdx.x == 0) o[0] = (float)carry;
 }
 
 struct RetinaLayout {
@@ -368,9 +382,7 @@ TRTX_API int trtx_retina_decode_enqueue(const trtx_retina_params* p, int batch, 
         retina_scan_launch<float>(anticov, vec, a, batch, warps, st);
     int rc = check_launch();
     if (rc) return rc;
-    const size_t smem = sizeof(int) * (size_t)(L.tiles + 1);
-    if (smem > 48 * 1024) return TRTX_ERR_UNSUPPORTED;
-    retina_pack_kernel<<<batch, 256, smem, st>>>(a, output_dev);
+    retina_pack_kernel<<<batch, 256, 0, st>>>(a, output_dev);
     return check_launch();
 }
 
