@@ -368,7 +368,19 @@ TRTX_API int trtx_preprocess_batch_enqueue(const trtx_image_desc* images_host, i
 TRTX_API void trtx_letterbox_matrix(int src_w, int src_h, int dst_w, int dst_h, float d2s[6]);
 /* get_rect (yolov8/src/postprocess.cpp:6-36, yolov5/src/postprocess.cpp:4-29): maps a detection box from network-input
  * pixels back to the original image: rect = {x, y, width, height} as cv::Rect.  variant TRTX_YOLO_V8: box l,t,r,b,
- * result clamped to the image; TRTX_YOLO_V5: box cx,cy,w,h.  Host function (no device work). */
+ * result clamped to the image; TRTX_YOLO_V5: box cx,cy,w,h.
+ * TRTX_YOLO_V3: the get_rect of yolov3, yolov4, scaled-yolov4 and yolov3-tiny (yolov3/yolov3.cpp:30-52, yolov4/yolov4.cpp:55-77,
+ *   scaled-yolov4/common.hpp:36-58, yolov3-tiny/yolov3-tiny.cpp:62-84): box cx,cy,w,h; r_w = net_w / (img_w * 1.0) stored to
+ *   float (r_h likewise), l = (int)(cx - w / 2.f) (minus the float pad (net_h - r_w * img_h) / 2 on the padded axis), then
+ *   l = (int)((float)l / r_w); every int store truncates toward zero; no clamp; rect = {l, t, r - l, b - t}.
+ * TRTX_RECT_YOLOV3_SPP: yolov3-spp's get_rect (yolov3-spp/yolov3-spp.cpp:58-75) with MAX_INPUT_SIZE = net_w = net_h: the
+ *   letterbox of trtx_yolov3spp_letterbox, l = (int)(cx - w / 2.f - dw / 2) with dw / 2 an int division, then l /= ra
+ *   (truncated); no clamp.
+ * A box whose get_rect is undefined in the reference -- a NaN, an infinity or a float outside the int range converted to int,
+ * or an r - l that overflows -- gets {0, 0, 0, 0} (TRTX_YOLO_V8 / V5: a non-finite box or rescaled corners outside the int
+ * range).  TRTX_ERR_INVALID for a null pointer, a size <= 0, another variant, or net_w != net_h with TRTX_RECT_YOLOV3_SPP.
+ * Host function (no device work). */
+enum { TRTX_RECT_YOLOV3_SPP = 16 /* a rectangle variant only: no YoloLayer decodes with it */ };
 TRTX_API int trtx_get_rect(int variant, int net_w, int net_h, int img_w, int img_h, const float bbox[4], int rect[4]);
 
 /* get_rect_adapt_landmark (yolov8/src/postprocess.cpp:38-69): like get_rect for the pose models -- the box (l,t,r,b) becomes
@@ -499,8 +511,10 @@ typedef trtx_frame trtx_rcnn_image;
  * (yolov8/src/postprocess.cpp:228-248, yolov5/src/postprocess.cpp:148-167), for a batch of original frames of any sizes. */
 
 /* p: as for trtx_process_mask_enqueue (row_floats >= 6; with every masks_dev NULL only variant, net_w, net_h and row_floats
- *   are read).  dets_dev [B, 1 + max_rows*row_floats]: count, rows with the box at floats 0..3 in the variant's format, conf
- *   at 4, class at 5 (the compact NMS output with extra_floats = 32: row_floats 39, coeff_offset 7; plugin rows: 90 / 6).
+ *   are read, and variant may also be TRTX_YOLO_V3 or TRTX_RECT_YOLOV3_SPP: the rows of yolov3 / yolov4 / scaled-yolov4 /
+ *   yolov3-tiny and yolov3-spp, whose models have no masks; with canvases those two are TRTX_ERR_INVALID).
+ * dets_dev [B, 1 + max_rows*row_floats]: count, rows with the box at floats 0..3 in the variant's format, conf at 4, class
+ *   at 5 (the compact NMS output with extra_floats = 32: row_floats 39, coeff_offset 7; plugin rows: 90 / 6).
  * images_host: `batch` descriptors in HOST memory (copied into launch parameters; sizes may differ within a call).
  * rows_dev [B, 1 + max_rows*6]: n = min(count, max_rows), then per row i < n (x, y, w, h, conf, class) with x, y, w, h =
  *   get_rect(img, bbox) (trtx_get_rect: V8 clamped to the image, V5 not), rows past n zeroed.  A box whose get_rect is
@@ -1050,6 +1064,49 @@ TRTX_API int trtx_refinedet_postprocess_enqueue(const trtx_refinedet_params* p, 
                                                 const float* arm_conf_dev, const float* odm_loc_dev, const float* odm_conf_dev,
                                                 void* workspace_dev, size_t workspace_bytes, float* dets_dev,
                                                 const int32_t* frame_wh_host, float* rows_dev, trtx_stream_t stream);
+
+/* =====================================================================================
+ * 15. Bilinear letterbox pre-process (yolov3, yolov4, scaled-yolov4, yolov3-spp, RetinaFace)
+ *    replaces the HOST preprocess_img with cv::resize(INTER_LINEAR) and the drivers' plane loops of yolov3
+ *    (yolov3/utils.h:41-61, yolov3/yolov3.cpp:477-481), yolov4 (yolov4/yolov4.cpp:33-53, :637-641), scaled-yolov4
+ *    (scaled-yolov4/common.hpp:14-34, yolov4_csp.cpp:466-468) and retina_r50 / retina_mnet (retinaface/common.hpp:21-41,
+ *    retina_r50.cpp:342-352); yolov3-spp's letterbox + cv::dnn::blobFromImage (yolov3-spp/yolov3-spp.cpp:43-56, :533-536);
+ *    and the H2D copy of their fp32 input.  The rectangles after NMS are trtx_get_rect's TRTX_YOLO_V3 and
+ *    TRTX_RECT_YOLOV3_SPP, on the device trtx_yolo_seg_postprocess_enqueue's rows-only mode.
+ * ===================================================================================== */
+enum {
+    TRTX_LINEAR_YOLOV3 = 0,     /* preprocess_img on a 128 canvas; planes R, G, B; data = u / 255.0 (double), stored to float */
+    TRTX_LINEAR_RETINA = 1,     /* preprocess_img on a 128 canvas; planes B, G, R; data = u - 104.0, u - 117.0, u - 123.0
+                                   (exact) */
+    TRTX_LINEAR_YOLOV3_SPP = 2, /* yolov3-spp's letterbox; planes R, G, B; data = (float)u * (float)(1 / 255.0), as
+                                   blobFromImage(pr, 1 / 255.0, size, Scalar(0, 0, 0), swapRB = true, crop = false) stores it */
+};
+
+/* yolov3-spp's letterbox of an img_w x img_h frame for MAX_INPUT_SIZE = max_size (608 in the reference): r = std::min(max_size /
+ * (img_w * 1.0), max_size / (img_h * 1.0)) stored to float, r = std::min(r, 1.0f), unpad = (int)(r * w) (a float product),
+ * d = (max_size - unpad) % 32 per axis.  out = {canvas_w, canvas_h, x, y, w, h}: the (unpad_w + dw) x (unpad_h + dh) canvas the
+ * engine's input shape is bound to, and the rectangle (dw / 2, dh / 2, unpad_w, unpad_h) the resized frame occupies (a frame no
+ * larger than max_size keeps its size).  A caller skips frames whose canvas is below the engine profile's minimum (128, as
+ * the driver does at :535).  TRTX_ERR_INVALID for a null out or a size <= 0; TRTX_ERR_UNSUPPORTED, with out filled, for an
+ * empty rectangle (cv::resize throws there, e.g. 1 x 5000).  Host function. */
+TRTX_API int trtx_yolov3spp_letterbox(int img_w, int img_h, int max_size, int out[6]);
+
+/* The pre-process for a whole batch, one launch per <= 64 images: images_host = `batch` u8 HWC BGR descriptors in HOST memory
+ * (trtx_image_desc, any pitch and base alignment, mixed sizes allowed); dst_dev = [batch, 3, net_h, net_w] fp32 planes, the
+ * engine input.  The frame is resized into its rectangle on a 128-grey canvas by OpenCV 4.x's 8-bit INTER_LINEAR, bit for bit
+ * (fx = (float)((d + 0.5) * scale - 0.5), weights saturate_cast<short>((1 - fx) * 2048) and (fx * 2048), horizontal pass in
+ * int, vertical pass ((b0 * (S0 >> 4)) >> 16) + ((b1 * (S1 >> 4)) >> 16) + 2) >> 2; cv2 4.13 gives these bytes with IPP on
+ * and off); a frame
+ * resized to its own size is copied.  The rectangle is trtx_calib_letterbox_rect's for TRTX_LINEAR_YOLOV3 / RETINA
+ * (INPUT_W x INPUT_H: 608 x 608 for yolov3 / yolov4, 512 x 512 for scaled-yolov4, 640 x 480 for RetinaFace) and
+ * trtx_yolov3spp_letterbox's for TRTX_LINEAR_YOLOV3_SPP.  max_size is read by TRTX_LINEAR_YOLOV3_SPP only; its engine binds
+ * one input shape per enqueue, so every frame's canvas must be net_w x net_h.
+ * Every descriptor is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
+ * batch / net sizes <= 0, pitch < 3 * width, an unknown variant, a dst_dev that is not 4-byte aligned, or (SPP) max_size <= 0
+ * or a frame whose canvas is not net_w x net_h; TRTX_ERR_UNSUPPORTED for an empty rectangle (cv::resize throws) or one wider
+ * than 4 757 pixels (the band's staged source rows in shared memory).  No workspace; can be captured in a CUDA graph. */
+TRTX_API int trtx_linear_preprocess_enqueue(int variant, const trtx_image_desc* images_host, int batch, int net_w, int net_h,
+                                            int max_size, float* dst_dev, trtx_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -19,6 +19,8 @@ NMS_GREEDY, NMS_ONESHOT = 0, 1
 RETINA_FACE, RETINA_ANTICOV = 0, 1
 TASK_POSE, TASK_OBB, TASK_OBB_NMS_FREE = 1, 2, 3
 CUBIC_YOLOV3_TINY, CUBIC_ANTICOV = 0, 1
+LINEAR_YOLOV3, LINEAR_RETINA, LINEAR_YOLOV3_SPP = 0, 1, 2
+RECT_YOLOV3_SPP = 16  # trtx_get_rect / the seg rows: yolov3-spp's get_rect
 
 _ERR = {1: "TRTX_ERR_INVALID", 2: "TRTX_ERR_WORKSPACE", 3: "TRTX_ERR_CUDA", 4: "TRTX_ERR_UNSUPPORTED"}
 
@@ -210,6 +212,8 @@ SYMBOLS = {
                                            _vp, _vp]),
     "trtx_cubic_preprocess_enqueue": (_i, [_i, C.POINTER(ImageDesc), _i, _i, _i, _vp, _vp]),
     "trtx_refinedet_preprocess_enqueue": (_i, [C.POINTER(ImageDesc), _i, _i, _vp, _vp]),
+    "trtx_yolov3spp_letterbox": (_i, [_i, _i, _i, C.POINTER(C.c_int)]),
+    "trtx_linear_preprocess_enqueue": (_i, [_i, C.POINTER(ImageDesc), _i, _i, _i, _i, _vp, _vp]),
     "trtx_refinedet_workspace_size": (_sz, [C.POINTER(RefinedetParams), _i]),
     "trtx_refinedet_postprocess_enqueue": (_i, [C.POINTER(RefinedetParams), _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp,
                                                 C.POINTER(C.c_int32), _vp, _vp]),

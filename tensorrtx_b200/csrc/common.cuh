@@ -202,14 +202,108 @@ __host__ __device__ inline float yolo_map_landmark(const YoloLetterbox& lb, int 
     return (axis == 0) == lb.by_w ? f_div(v, lb.ratio) : f_div(f_sub(v, lb.pad), lb.ratio);
 }
 
+// (int)v where it is defined: v truncated toward zero fits an int.  False for NaN, +-inf and values past the int range
+// (in float, v >= -2^31 is the same as trunc(v) >= INT_MIN).  Shared by the truncating get_rects below and process_mask (mask.cu).
+__host__ __device__ inline bool trunc_to_int(float v, int& out) {
+    if (!(v >= -2147483648.0f && v < 2147483648.0f)) return false;
+    out = (int)v;
+    return true;
+}
+
+// The corners l, t, r, b of a cx, cy, w, h box as the truncating get_rect of yolov3 / yolov4 / scaled-yolov4 / yolov3-tiny and
+// YOLOP (yolov3/yolov3.cpp:30-52, yolop/common.hpp:13-37; the same statements) compute them before their first int store:
+// `bbox[0] - bbox[2]/2.f`, minus the pad `(INPUT_H - r_w * img.rows) / 2` on the padded axis, all in float.
+__host__ __device__ inline void trunc_rect_corners(const YoloLetterbox& lb, const float bbox[4], float c[4]) {
+    c[0] = f_sub(bbox[0], f_div(bbox[2], 2.f));
+    c[1] = f_sub(bbox[1], f_div(bbox[3], 2.f));
+    c[2] = f_add(bbox[0], f_div(bbox[2], 2.f));
+    c[3] = f_add(bbox[1], f_div(bbox[3], 2.f));
+    const int padded = lb.by_w ? 1 : 0;  // the axis that carries the pad: y when the width fills the input
+    c[padded] = f_sub(c[padded], lb.pad);
+    c[padded + 2] = f_sub(c[padded + 2], lb.pad);
+}
+
+// rect = {l, t, r - l, b - t} of four truncated corners; false where r - l or b - t overflows int.
+__host__ __device__ inline bool int_rect(const int v[4], int rect[4]) {
+    const long long w = (long long)v[2] - v[0], h = (long long)v[3] - v[1];
+    if (w < INT32_MIN || w > INT32_MAX || h < INT32_MIN || h > INT32_MAX) return false;
+    rect[0] = v[0];
+    rect[1] = v[1];
+    rect[2] = (int)w;
+    rect[3] = (int)h;
+    return true;
+}
+
+// get_rect of yolov3, yolov4, scaled-yolov4 and yolov3-tiny (yolov3/yolov3.cpp:30-52, yolov4/yolov4.cpp:55-77,
+// scaled-yolov4/common.hpp:36-58, yolov3-tiny/yolov3-tiny.cpp:62-84): every assignment to `int l, r, t, b` truncates toward
+// zero, so a corner is truncated after trunc_rect_corners and again after `l = l / r_w` (int -> float, a float division); no
+// clamp.  Returns false, with rect {0, 0, 0, 0}, where the reference is undefined: a conversion of a NaN, an infinity or a
+// float outside the int range, or an r - l that overflows.
+__host__ __device__ inline bool yolov3_get_rect(const YoloLetterbox& lb, const float bbox[4], int rect[4]) {
+    rect[0] = rect[1] = rect[2] = rect[3] = 0;
+    float c[4];
+    trunc_rect_corners(lb, bbox, c);
+    int v[4];
+    for (int k = 0; k < 4; ++k) {
+        int t;
+        if (!trunc_to_int(c[k], t) || !trunc_to_int(f_div((float)t, lb.ratio), v[k])) return false;
+    }
+    return int_rect(v, rect);
+}
+
+// yolov3-spp's letterbox (yolov3-spp/yolov3-spp.cpp:43-56) and the same lines at the top of its get_rect (:58-64), for MAX =
+// max_size: r = std::min(MAX / (w * 1.0), MAX / (h * 1.0)) stored to float, r = std::min(r, 1.0f); unpad = (int)(r * w) in
+// float; d = (MAX - unpad) % 32 per axis.  The canvas is (unpad_w + dw) x (unpad_h + dh), the resized frame sits at
+// (dw / 2, dh / 2).
+struct SppLetterbox {
+    float ratio;
+    int unpad_w, unpad_h, dw, dh;
+};
+__host__ __device__ inline SppLetterbox yolov3spp_letterbox(int max_size, int img_w, int img_h) {
+#ifdef __CUDA_ARCH__
+    const double a = __ddiv_rn((double)max_size, (double)img_w), b = __ddiv_rn((double)max_size, (double)img_h);
+    float r = __double2float_rn(a < b ? a : b);
+#else
+    const double a = max_size / (img_w * 1.0), b = max_size / (img_h * 1.0);
+    float r = (float)(a < b ? a : b);
+#endif
+    r = r < 1.0f ? r : 1.0f;
+    SppLetterbox lb;
+    lb.ratio = r;
+    lb.unpad_w = (int)f_mul(r, (float)img_w);
+    lb.unpad_h = (int)f_mul(r, (float)img_h);
+    lb.dw = (max_size - lb.unpad_w) % 32;
+    lb.dh = (max_size - lb.unpad_h) % 32;
+    return lb;
+}
+
+// yolov3-spp's get_rect (yolov3-spp.cpp:58-75): `int l = bbox[0] - bbox[2]/2.f - dw / 2` (the pad an int division, the rest
+// float, truncated), then `l /= ra` (int -> float, a float division, truncated); no clamp; undefined cases as yolov3_get_rect.
+__host__ __device__ inline bool yolov3spp_get_rect(int max_size, int img_w, int img_h, const float bbox[4], int rect[4]) {
+    rect[0] = rect[1] = rect[2] = rect[3] = 0;
+    const SppLetterbox lb = yolov3spp_letterbox(max_size, img_w, img_h);
+    const float px = (float)(lb.dw / 2), py = (float)(lb.dh / 2);
+    const float c[4] = {f_sub(f_sub(bbox[0], f_div(bbox[2], 2.f)), px), f_sub(f_sub(bbox[1], f_div(bbox[3], 2.f)), py),
+                        f_sub(f_add(bbox[0], f_div(bbox[2], 2.f)), px), f_sub(f_add(bbox[1], f_div(bbox[3], 2.f)), py)};
+    int v[4];
+    for (int k = 0; k < 4; ++k) {
+        int t;
+        if (!trunc_to_int(c[k], t) || !trunc_to_int(f_div((float)t, lb.ratio), v[k])) return false;
+    }
+    return int_rect(v, rect);
+}
+
 // get_rect: the inverse of the letterbox for a detection box -- yolov8/src/postprocess.cpp:6-36 (TRTX_YOLO_V8: l,t,r,b,
 // clamped to the image) and yolov5/src/postprocess.cpp:4-29 (TRTX_YOLO_V5: cx,cy,w,h, not clamped).  Statement by statement:
 // the two ratios are double divisions stored to float, the rest is float, round() sees doubles.  Shared by the host
 // trtx_get_rect and trtx_get_rect_adapt_landmark (whose rectangle is the same float expressions as the V8 branch), the
 // segmentation post-process kernels (mask.cu) and yolo_get_corner.  Returns false, with rect {0, 0, 0, 0}, where the
 // reference's float -> int conversions are undefined (a non-finite box, or rescaled corners outside the int range).
+// TRTX_YOLO_V3 is yolov3_get_rect, TRTX_RECT_YOLOV3_SPP yolov3spp_get_rect with MAX = net_w.
 __host__ __device__ inline bool yolo_get_rect(int variant, int net_w, int net_h, int img_w, int img_h, const float bbox[4],
                                               int rect[4]) {
+    if (variant == TRTX_YOLO_V3) return yolov3_get_rect(yolo_letterbox(net_w, net_h, img_w, img_h), bbox, rect);
+    if (variant == TRTX_RECT_YOLOV3_SPP) return yolov3spp_get_rect(net_w, img_w, img_h, bbox, rect);
     rect[0] = rect[1] = rect[2] = rect[3] = 0;
     const YoloLetterbox lb = yolo_letterbox(net_w, net_h, img_w, img_h);
     const bool by_w = lb.by_w;
@@ -350,11 +444,8 @@ __host__ __device__ inline void retina_get_rect_adapt_landmark(int input_w, int 
 // {l, t, r - l, b - t}.  Undefined cases as the compiled x86-64 reference behaves: trunc_to_int_x86, and int differences
 // that wrap modulo 2^32.
 __host__ __device__ inline void yolop_get_rect(const YoloLetterbox& lb, const float bbox[4], int rect[4]) {
-    float c[4] = {f_sub(bbox[0], f_div(bbox[2], 2.f)), f_sub(bbox[1], f_div(bbox[3], 2.f)), f_add(bbox[0], f_div(bbox[2], 2.f)),
-                  f_add(bbox[1], f_div(bbox[3], 2.f))};  // l, t, r, b
-    const int padded = lb.by_w ? 1 : 0;                 // the axis that carries the pad: y when the width fills the input
-    c[padded] = f_sub(c[padded], lb.pad);
-    c[padded + 2] = f_sub(c[padded + 2], lb.pad);
+    float c[4];  // l, t, r, b
+    trunc_rect_corners(lb, bbox, c);
     int v[4];
     for (int k = 0; k < 4; ++k) v[k] = trunc_to_int_x86(f_div((float)trunc_to_int_x86(c[k]), lb.ratio));
     rect[0] = v[0];

@@ -36,14 +36,6 @@ struct MaskArgs {
     int variant, nm, mw, mh, net_w, net_h, max_masks;
 };
 
-// (int)v where it is defined: v truncated toward zero fits an int.  False for NaN, +-inf and values past the int range
-// (in float, v >= -2^31 is the same as trunc(v) >= INT_MIN).
-__device__ __forceinline__ bool trunc_to_int(float v, int& out) {
-    if (!(v >= -2147483648.0f && v < 2147483648.0f)) return false;
-    out = (int)v;
-    return true;
-}
-
 // get_downscale_rect: yolov8_seg.cpp:17-34 (bbox used as x, y, w, h; clamped to the network input; int() truncation),
 // yolov5/src/postprocess.cpp:94-104 (cx, cy, w, h; round()), as the cells [x_lo, x_hi) x [y_lo, y_hi) of the mw x mh mask
 // that process_mask's loops visit.  The loops are clamped to the mask here (the reference would write out of bounds for a
@@ -1596,13 +1588,16 @@ TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const 
                                                const float* proto_dev, const float* dets_dev, int max_rows,
                                                float* rows_dev, trtx_stream_t stream) {
     if (!p || !images_host || batch <= 0 || !dets_dev || !rows_dev || max_rows <= 0) return TRTX_ERR_INVALID;
-    if (p->variant != TRTX_YOLO_V8 && p->variant != TRTX_YOLO_V5) return TRTX_ERR_INVALID;
+    // TRTX_YOLO_V3 and TRTX_RECT_YOLOV3_SPP: rectangles only (their models have no masks)
+    const bool rect_only = p->variant == TRTX_YOLO_V3 || p->variant == TRTX_RECT_YOLOV3_SPP;
+    if (p->variant != TRTX_YOLO_V8 && p->variant != TRTX_YOLO_V5 && !rect_only) return TRTX_ERR_INVALID;
     if (p->net_w <= 0 || p->net_h <= 0 || p->row_floats < kSegRowFloats) return TRTX_ERR_INVALID;
+    if (p->variant == TRTX_RECT_YOLOV3_SPP && p->net_w != p->net_h) return TRTX_ERR_INVALID;
     bool masks;
     int rc = check_frames(images_host, batch, masks);
     if (rc) return rc;
     if (masks) {  // trtx_process_mask_enqueue's checks
-        if (!proto_dev) return TRTX_ERR_INVALID;
+        if (rect_only || !proto_dev) return TRTX_ERR_INVALID;
         if (p->num_coeffs <= 0 || p->num_coeffs > kMaxCoeffs || p->max_masks <= 0) return TRTX_ERR_INVALID;
         if (p->coeff_offset < 0 || p->coeff_offset + p->num_coeffs > p->row_floats) return TRTX_ERR_INVALID;
         if (p->mask_w <= 0 || p->mask_h <= 0) return TRTX_ERR_INVALID;

@@ -908,6 +908,46 @@ __global__ void __launch_bounds__(kRcnnPreThreads) cubic_preprocess_kernel(const
     cubic_band<PlanarStore<CubicInput<kVariant>>>(a, dst);
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Bilinear letterbox pre-process of yolov3, yolov4, scaled-yolov4, yolov3-spp and RetinaFace: resize_band with a planar store;
+// only the value conventions and the host-side rectangles are their own.
+//   TRTX_LINEAR_YOLOV3      the yolov3-tiny chain, u / 255.0 in double (CubicInput<TRTX_CUBIC_YOLOV3_TINY>), planes R, G, B;
+//   TRTX_LINEAR_RETINA      RetinaInput below;
+//   TRTX_LINEAR_YOLOV3_SPP  blobFromImage's (float)u * (float)(1 / 255.0), planes R, G, B: cls_preprocess_kernel<TRTX_YOLO_V8>,
+//                           whose value chain it is, over yolov3-spp's rectangle.
+// retina_r50.cpp:342-352: plane c (0 = B) takes BGR byte c, `pr_img.at<cv::Vec3b>(i)[c] - mean` in double with means 104, 117,
+// 123, stored to float (exact).
+struct RetinaInput {
+    static constexpr uint32_t kCanvas = 128u;  // Scalar(128, 128, 128)
+    static __device__ __forceinline__ int channel(int c) { return c; }
+    static __device__ __forceinline__ float value(int c, uint32_t u) {
+        return __fsub_rn((float)u, c == 0 ? 104.f : (c == 1 ? 117.f : 123.f));
+    }
+};
+
+template <class In>
+__global__ void __launch_bounds__(kRcnnPreThreads) linear_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
+                                                                            float* __restrict__ dst) {
+    resize_band<PlanarStore<In>>(a, dst);
+}
+
+// The band descriptor of frame d in yolov3-spp's letterbox: TRTX_ERR_UNSUPPORTED where the rectangle is empty (cv::resize
+// throws), TRTX_ERR_INVALID where the canvas is not net_w x net_h (the call binds one input shape).
+static int spp_band_image(const trtx_image_desc& d, int max_size, int net_w, int net_h, RcnnPreImage& im) {
+    int g[6];
+    const int rc = trtx_yolov3spp_letterbox(d.width, d.height, max_size, g);
+    if (rc) return rc;
+    if (g[0] != net_w || g[1] != net_h) return TRTX_ERR_INVALID;
+    im.src = d.data_dev;
+    im.sw = d.width;
+    im.sh = d.height;
+    im.pitch = d.pitch;
+    im.x0 = g[2], im.y0 = g[3], im.rw = g[4], im.rh = g[5];
+    im.scale_x = 1. / ((double)im.rw / im.sw);
+    im.scale_y = 1. / ((double)im.rh / im.sh);
+    return TRTX_OK;
+}
+
 }  // namespace trtx
 
 using namespace trtx;
@@ -950,7 +990,9 @@ TRTX_API void trtx_letterbox_matrix(int sw, int sh, int dw, int dh, float d2s[6]
 // post-process kernels share).  Host function.
 TRTX_API int trtx_get_rect(int variant, int net_w, int net_h, int img_w, int img_h, const float bbox[4], int rect[4]) {
     if (!bbox || !rect || net_w <= 0 || net_h <= 0 || img_w <= 0 || img_h <= 0) return TRTX_ERR_INVALID;
-    if (variant != TRTX_YOLO_V8 && variant != TRTX_YOLO_V5) return TRTX_ERR_INVALID;
+    if (variant != TRTX_YOLO_V8 && variant != TRTX_YOLO_V5 && variant != TRTX_YOLO_V3 && variant != TRTX_RECT_YOLOV3_SPP)
+        return TRTX_ERR_INVALID;
+    if (variant == TRTX_RECT_YOLOV3_SPP && net_w != net_h) return TRTX_ERR_INVALID;
     yolo_get_rect(variant, net_w, net_h, img_w, img_h, bbox, rect);
     return TRTX_OK;
 }
@@ -1250,6 +1292,52 @@ TRTX_API int trtx_cubic_preprocess_enqueue(int variant, const trtx_image_desc* i
         if (rc) return rc;
     }
     return TRTX_OK;
+}
+
+TRTX_API int trtx_yolov3spp_letterbox(int img_w, int img_h, int max_size, int out[6]) {
+    if (!out || img_w <= 0 || img_h <= 0 || max_size <= 0) return TRTX_ERR_INVALID;
+    const SppLetterbox lb = yolov3spp_letterbox(max_size, img_w, img_h);
+    out[0] = lb.unpad_w + lb.dw;
+    out[1] = lb.unpad_h + lb.dh;
+    out[2] = lb.dw / 2;
+    out[3] = lb.dh / 2;
+    out[4] = lb.unpad_w;
+    out[5] = lb.unpad_h;
+    return lb.unpad_w > 0 && lb.unpad_h > 0 ? TRTX_OK : TRTX_ERR_UNSUPPORTED;
+}
+
+// preprocess_img with INTER_LINEAR (yolov3, yolov4, scaled-yolov4, RetinaFace: cls_band_image's V5 rectangle) or yolov3-spp's
+// letterbox (spp_band_image), the bilinear band kernel with the variant's planar store.
+TRTX_API int trtx_linear_preprocess_enqueue(int variant, const trtx_image_desc* images_host, int batch, int net_w, int net_h,
+                                            int max_size, float* dst_dev, trtx_stream_t stream) {
+    if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
+    if (variant != TRTX_LINEAR_YOLOV3 && variant != TRTX_LINEAR_RETINA && variant != TRTX_LINEAR_YOLOV3_SPP)
+        return TRTX_ERR_INVALID;
+    if (variant == TRTX_LINEAR_YOLOV3_SPP && max_size <= 0) return TRTX_ERR_INVALID;
+    if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
+    auto make = [&](int i, RcnnPreImage& im) -> int {
+        if (variant == TRTX_LINEAR_YOLOV3_SPP) return spp_band_image(images_host[i], max_size, net_w, net_h, im);
+        return cls_band_image(TRTX_YOLO_V5, images_host[i], net_w, net_h, im) ? TRTX_OK : TRTX_ERR_UNSUPPORTED;
+    };
+    // every descriptor is checked before the first launch, so that a rejected call writes nothing
+    for (int i = 0; i < batch; ++i) {
+        const trtx_image_desc& d = images_host[i];
+        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
+    }
+    size_t smem_max = 0;
+    for (int i = 0; i < batch; ++i) {
+        RcnnPreImage im;
+        const int rc = make(i, im);
+        if (rc) return rc;
+        const size_t smem = (size_t)kRcnnPreSlots * 3 * (size_t)im.rw * sizeof(int16_t);
+        if (smem > kClsMaxDynamicSmem) return TRTX_ERR_UNSUPPORTED;
+        smem_max = smem > smem_max ? smem : smem_max;
+    }
+    auto* kernel = variant == TRTX_LINEAR_YOLOV3  ? linear_preprocess_kernel<CubicInput<TRTX_CUBIC_YOLOV3_TINY>>
+                   : variant == TRTX_LINEAR_RETINA ? linear_preprocess_kernel<RetinaInput>
+                                                   : cls_preprocess_kernel<TRTX_YOLO_V8>;
+    return launch_bands(kernel, batch, net_w, net_h, dst_dev, smem_max, static_cast<cudaStream_t>(stream),
+                        [&](int i, RcnnPreImage& im) { make(i, im); });
 }
 
 }  // extern "C"

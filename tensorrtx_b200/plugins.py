@@ -638,6 +638,8 @@ def yolo_seg_postprocess(proto: torch.Tensor | None, dets: torch.Tensor, image_s
     proto [B, 32, net_h/4, net_w/4] (may be None with masks=False); dets [B, 1 + max_rows*row_floats] (count, rows);
     image_sizes[b] = (img_w, img_h) of frame b ->
     (rows [B, 1 + max_rows*6] fp32: count, then (x, y, w, h, conf, class) with x, y, w, h = get_rect(img, bbox);
+    variant YOLO_V3 or RECT_YOLOV3_SPP, with masks=False, maps the NMS rows of yolov3 / yolov4 / scaled-yolov4 /
+    yolov3-tiny or yolov3-spp (net_w = net_h = MAX_INPUT_SIZE) by their get_rect;
      per-image u8 canvases [max_masks, img_h, img_w]: 255 where draw_mask_bbox would colour the pixel, or None with masks=False).
     `canvases_out[b]` may be any u8 cuda tensor [max_masks, img_h, img_w] with contiguous rows and slots (e.g. a view
     [..., :img_w] of a pitched buffer);
@@ -1124,8 +1126,10 @@ class PreprocessPlan:
 
 
 def get_rect(img_w: int, img_h: int, bbox, net_w: int = 640, net_h: int = 640, variant: int = L.YOLO_V8):
-    """get_rect(img, bbox) of yolov8/src/postprocess.cpp:6-36 (variant YOLO_V5: yolov5/src/postprocess.cpp:4-29):
-    -> (x, y, width, height) in the original image."""
+    """get_rect(img, bbox) of yolov8/src/postprocess.cpp:6-36 (variant YOLO_V5: yolov5/src/postprocess.cpp:4-29; YOLO_V3:
+    the truncating get_rect of yolov3, yolov4, scaled-yolov4 and yolov3-tiny; RECT_YOLOV3_SPP: yolov3-spp's, with
+    net_w = net_h = MAX_INPUT_SIZE) -> (x, y, width, height) in the original image, (0, 0, 0, 0) where the reference's
+    conversions are undefined."""
     lib = L.load()
     b = (C.c_float * 4)(*[float(v) for v in bbox])
     r = (C.c_int * 4)()
@@ -1519,6 +1523,35 @@ def cubic_preprocess(images: Sequence[torch.Tensor], variant: int, out: torch.Te
                       f"out must be float32 [{n}, 3, {net_h}, {net_w}]", contiguous=False)
     L.check(lib.trtx_cubic_preprocess_enqueue(variant, descs, n, net_w, net_h, _ptr(out), _stream(stream)),
             "trtx_cubic_preprocess_enqueue")
+    return out
+
+
+def yolov3spp_letterbox(w: int, h: int, max_size: int = 608) -> tuple[tuple[int, int], tuple[int, int, int, int]]:
+    """yolov3-spp's letterbox (yolov3-spp/yolov3-spp.cpp:43-56) of a w x h frame -> ((canvas_w, canvas_h), (x, y, w, h) of
+    the resized frame on it).  The canvas is the engine input shape of the frame; the driver skips frames whose canvas is
+    below 128 on either side."""
+    g = (C.c_int * 6)()
+    L.check(L.load().trtx_yolov3spp_letterbox(int(w), int(h), int(max_size), g), "trtx_yolov3spp_letterbox")
+    return (g[0], g[1]), (g[2], g[3], g[4], g[5])
+
+
+def linear_preprocess(images: Sequence[torch.Tensor], variant: int, out: torch.Tensor | None = None, net_w: int = 608,
+                      net_h: int = 608, max_size: int = 608, stream=None) -> torch.Tensor:
+    """GPU drop-in for preprocess_img with cv::resize(INTER_LINEAR) and the driver's plane loop of yolov3 / yolov4 /
+    scaled-yolov4 (variant _lib.LINEAR_YOLOV3: u / 255.0, planes R, G, B; net 608 x 608, scaled-yolov4 512 x 512) and
+    retina_r50 / retina_mnet (_lib.LINEAR_RETINA: u - 104, u - 117, u - 123, planes B, G, R; net 640 x 480), and for
+    yolov3-spp's letterbox + cv::dnn::blobFromImage (_lib.LINEAR_YOLOV3_SPP: (float)u * (float)(1 / 255.0), planes R, G, B;
+    every frame's canvas, yolov3spp_letterbox(w, h, max_size)[0], must be (net_w, net_h)), for a batch of device frames:
+    images[i] is a u8 HWC BGR cuda tensor [h, w, 3] with packed pixels (rows may be pitched, sizes may differ) ->
+    [B, 3, net_h, net_w] float32 planes, the engine input: the frame resized as OpenCV's 8-bit INTER_LINEAR does, bit for
+    bit, on a 128-grey canvas.  One launch per 64 images, no synchronisation."""
+    lib = L.load()
+    n = len(images)
+    descs = _image_descs(images)
+    out = _out_tensor(out, (n, 3, net_h, net_w), torch.float32, images[0].device if n else "cuda",
+                      f"out must be float32 [{n}, 3, {net_h}, {net_w}]", contiguous=False)
+    L.check(lib.trtx_linear_preprocess_enqueue(variant, descs, n, net_w, net_h, max_size, _ptr(out), _stream(stream)),
+            "trtx_linear_preprocess_enqueue")
     return out
 
 
