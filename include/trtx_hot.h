@@ -65,21 +65,33 @@ enum {
     TRTX_YOLO_V8 = 0,
     TRTX_YOLO_V5 = 1,
     /* SURVEY 8f rank 4 -- older / other YoloLayer variants through the same scan / pack / NMS kernels: */
-    TRTX_YOLO_V3 = 2,  /* yolov3, yolov3-spp, yolov4 (yolov3-spp/yololayer.cu:148-191): anchor-based like V5, but box =
+    TRTX_YOLO_V3 = 2,  /* yolov3-spp (yolov3-spp/yololayer.cu:148-191): anchor-based like V5, but box =
                           ((col + sigmoid(x)) * stride, ..., exp(w) * anchor_w, ...), class AND objectness gated, rows of 7
                           floats x,y,w,h, det_confidence, class_id, class_confidence (yololayer.h:47-53).  `strides` and
-                          `anchors` are both used; det_floats >= 7 */
+                          `anchors` are both used; det_floats >= 7.  The rectangle entry points (trtx_get_rect, the rows of
+                          trtx_yolo_seg_postprocess_enqueue) take this value for the whole family below */
     TRTX_YOLO_V26 = 3, /* yolo26 NMS-free gatherKernel (yolo26/plugin/yololayer.cu:178-245): ONE input
                           [batch, anchors, 4 + num_classes (+1 angle when is_obb)], row-major per anchor, scores are
                           probabilities already; argmax `>` from (0, class -1), rows with score < gate dropped, 90-float
                           rows, everything the kernel does not write is zero (the reference memsets the buffer).
                           num_levels = 1, grid_h[0] * grid_w[0] = anchor count.  The reference decodes image 0 only
                           (":185 TODO"); this build decodes every image of the batch */
+    /* The rest of the yolov3 family: TRTX_YOLO_V3's gates, rows, grids and anchors (`strides` unused), another box and sigmoid.
+     * Every entry point that takes TRTX_YOLO_V3 for a decode takes these too, fp16 heads included. */
+    TRTX_YOLO_V3_NET = 4, /* yolov3, yolov3-tiny (yolov3/yololayer.cu:173-176, yolov3-tiny/yololayer.cu:172-175):
+                             x = ((float)col + sigmoid(x0)) * (float)net_w / (float)grid_w, in float left to right with an IEEE
+                             divide (y with net_h, grid_h); w = expf(x2) * anchor_w.  Logist = 1.0f / (1.0f + expf(-x)) */
+    TRTX_YOLO_V4 = 5,     /* yolov4 (yolov4/yololayer.cu:154, :191-194): TRTX_YOLO_V3_NET's box, but Logist = 1. / (1. + exp(-x))
+                             in double, rounded to float -- for the gates, both confidences and the box */
+    TRTX_YOLO_V4_CSP = 6, /* scaled-yolov4 (scaled-yolov4/yololayer.cu:154, :191-194): TRTX_YOLO_V4's double Logist;
+                             x = (float)(((double)((float)col + 2.0f * sigmoid(x0)) - 0.5) * net_w / grid_w) in double (the
+                             `- 0.5` is a double literal); w = powf(2.0f * sigmoid(x2), 2.0f) * anchor_w */
 };
 enum { TRTX_F32 = 0, TRTX_F16 = 1 };
 
 typedef struct trtx_yolo_params {
-    int32_t variant;     /* TRTX_YOLO_V8 | TRTX_YOLO_V5 | TRTX_YOLO_V3 | TRTX_YOLO_V26 */
+    int32_t variant;     /* TRTX_YOLO_V8 | TRTX_YOLO_V5 | TRTX_YOLO_V3 | TRTX_YOLO_V26 | TRTX_YOLO_V3_NET | TRTX_YOLO_V4 |
+                            TRTX_YOLO_V4_CSP */
     int32_t num_classes; /* combinedInfo[0] (yolov8/src/block.cpp:268) | netinfo[0] (yolov5/src/model.cpp:249) */
     int32_t net_w;       /* kInputW */
     int32_t net_h;       /* kInputH */

@@ -93,6 +93,50 @@ struct YoloCore {
             std::memcpy(p.anchors[i], k + 8, 24);
         }
     }
+    // the yolov3 family (yolov3/yololayer.h:20-44 and its siblings): rows of 7 floats; the blob holds no net size, box formula
+    // or maxOut, they are compile-time constants of each driver.  spp: a YoloKernel with a stride (36 bytes, grids -1 until
+    // the tensors are bound); the others: {int w, h; float anchors[6]} (32 bytes).
+    static constexpr int kV3Floats = 7;
+    void init_v3(int variant, int nc, int w, int h, int max_out, const void* kernels, int n) {
+        std::memset(&p, 0, sizeof(p));
+        p.variant = variant;
+        p.num_classes = nc;
+        p.net_w = w;
+        p.net_h = h;
+        p.max_out = max_out;
+        p.det_floats = kV3Floats;
+        p.num_levels = n;
+        p.gate = 0.1f;  // IGNORE_THRESH, yolov4/yololayer.h:11
+        const int ks = v3_kernel_bytes();
+        const char* k = static_cast<const char*>(kernels);
+        for (int i = 0; i < n && i < TRTX_MAX_LEVELS; ++i, k += ks) {
+            std::memcpy(&p.grid_w[i], k, 4);
+            std::memcpy(&p.grid_h[i], k + 4, 4);
+            if (ks == 36) std::memcpy(&p.strides[i], k + 8, 4);
+            std::memcpy(p.anchors[i], k + ks - 24, 24);
+        }
+    }
+    // bytes of one serialized YoloKernel of the yolov3 family, 0 for the other variants
+    int v3_kernel_bytes() const {
+        if (p.variant == TRTX_YOLO_V3) return 36;
+        return p.variant == TRTX_YOLO_V3_NET || p.variant == TRTX_YOLO_V4 || p.variant == TRTX_YOLO_V4_CSP ? 32 : 0;
+    }
+    // the family's blob (yolov4/yololayer.cu:58-70, yolov3-spp/yololayer.cu:58-69): the variant, net size and maxOut come
+    // from the caller; any length other than 12 + kernel bytes * kernelCount is refused
+    bool deserialize_v3(const void* data, size_t length, int variant, int w, int h, int max_out) {
+        if (length < 12) return false;
+        const char* d = static_cast<const char*>(data);
+        int nc, tc, kc;
+        detail::read(d, nc);
+        detail::read(d, tc);
+        detail::read(d, kc);
+        p.variant = variant;
+        const size_t ks = (size_t)v3_kernel_bytes();
+        if (ks == 0 || kc <= 0 || kc > TRTX_MAX_LEVELS || length != 12 + ks * (size_t)kc) return false;
+        init_v3(variant, nc, w, h, max_out, d, kc);
+        thread_count = tc;
+        return true;
+    }
     int out_elems() const { return 1 + p.max_out * p.det_floats; }  // yololayer.cu:107-111
     // the yolov7 / YOLOP blob: the yolov5 one without the is_seg byte (yolov7/plugin/yololayer.cu:62-77,
     // yolop/yololayer.cu:81-101)
@@ -100,6 +144,7 @@ struct YoloCore {
 
     size_t serial_size() const {
         if (p.variant == TRTX_YOLO_V8) return 4 * 8 + 4 * (size_t)p.num_levels + 3;  // yololayer.cu:97-101
+        if (v3_kernel_bytes()) return 12 + (size_t)v3_kernel_bytes() * p.num_levels;
         return (v7_layout() ? 24 : 25) + 32 * (size_t)p.num_levels;                 // yolov5 yololayer.cu:72-83
     }
     void serialize(void* buffer) const {
@@ -117,6 +162,16 @@ struct YoloCore {
             detail::write(d, (bool)p.is_seg);
             detail::write(d, (bool)p.is_pose);
             detail::write(d, (bool)p.is_obb);
+        } else if (v3_kernel_bytes()) {
+            detail::write(d, p.num_classes);
+            detail::write(d, thread_count);
+            detail::write(d, p.num_levels);
+            for (int i = 0; i < p.num_levels; ++i) {
+                detail::write(d, p.grid_w[i]);
+                detail::write(d, p.grid_h[i]);
+                if (p.variant == TRTX_YOLO_V3) detail::write(d, p.strides[i]);
+                for (int j = 0; j < 6; ++j) detail::write(d, p.anchors[i][j]);
+            }
         } else {
             detail::write(d, p.num_classes);
             detail::write(d, thread_count);
@@ -378,6 +433,114 @@ class YoloPluginCreatorT : public nvinfer1::IPluginCreator {
 };
 using YoloPluginCreator = YoloPluginCreatorT<true>;
 using YoloPluginCreatorImplicitBatch = YoloPluginCreatorT<false>;
+
+// ------------------------------------------------------------------------------------------------
+// "YoloLayer_TRT"/"1" of the yolov3 family.  Its creators take no fields (yolov4/yololayer.cu:258-263) and its plugins carry
+// the driver's compiled-in constants, so the creator is configured with them: a traits struct of the driver's yololayer.h
+// (CLASS_NUM, INPUT_W x INPUT_H, MAX_OUTPUT_BBOX_COUNT, the YoloKernel table in the plugin's level order) and its decode
+// variant.  createPlugin ignores the field collection and returns the configured plugin, as the reference does;
+// deserializePlugin accepts this driver's blob layout only, with the driver's kernel count (and strides, for spp).  A 3-level yolov3-spp blob (12 + 36 * 3 = 120 bytes) has the
+// length of a 3-level yolov7 / YOLOP one (24 + 32 * 3): only a creator configured for the driver can tell them apart.
+// ------------------------------------------------------------------------------------------------
+struct YoloV3FamilyKernel {
+    int w, h, stride;  // stride: yolov3-spp only (its grids are -1 until the tensors are bound)
+    float anchors[6];
+};
+struct YoloV3Traits {  // yolov3/yololayer.h:11-39
+    static constexpr int variant = TRTX_YOLO_V3_NET, classes = 80, net_w = 608, net_h = 608, max_out = 1000, levels = 3;
+    static const YoloV3FamilyKernel* kernels() {
+        static const YoloV3FamilyKernel k[3] = {{19, 19, 0, {116, 90, 156, 198, 373, 326}},
+                                                {38, 38, 0, {30, 61, 62, 45, 59, 119}},
+                                                {76, 76, 0, {10, 13, 16, 30, 33, 23}}};
+        return k;
+    }
+};
+struct YoloV4Traits {  // yolov4/yololayer.h:10-34
+    static constexpr int variant = TRTX_YOLO_V4, classes = 80, net_w = 608, net_h = 608, max_out = 1000, levels = 3;
+    static const YoloV3FamilyKernel* kernels() {
+        static const YoloV3FamilyKernel k[3] = {{76, 76, 0, {12, 16, 19, 36, 40, 28}},
+                                                {38, 38, 0, {36, 75, 76, 55, 72, 146}},
+                                                {19, 19, 0, {142, 110, 192, 243, 459, 401}}};
+        return k;
+    }
+};
+struct ScaledYoloV4Traits {  // scaled-yolov4/yololayer.h:10-38
+    static constexpr int variant = TRTX_YOLO_V4_CSP, classes = 80, net_w = 512, net_h = 512, max_out = 1000, levels = 3;
+    static const YoloV3FamilyKernel* kernels() {
+        static const YoloV3FamilyKernel k[3] = {{64, 64, 0, {12, 16, 19, 36, 40, 28}},
+                                                {32, 32, 0, {36, 75, 76, 55, 72, 146}},
+                                                {16, 16, 0, {142, 110, 192, 243, 459, 401}}};
+        return k;
+    }
+};
+struct YoloV3TinyTraits {  // yolov3-tiny/yololayer.h:11-34
+    static constexpr int variant = TRTX_YOLO_V3_NET, classes = 80, net_w = 608, net_h = 608, max_out = 1000, levels = 2;
+    static const YoloV3FamilyKernel* kernels() {
+        static const YoloV3FamilyKernel k[2] = {{19, 19, 0, {81, 82, 135, 169, 344, 319}},
+                                                {38, 38, 0, {23, 27, 37, 58, 81, 82}}};
+        return k;
+    }
+};
+struct YoloV3SppTraits {  // yolov3-spp/yololayer.h:11-44: dynamic input, the stride in the kernel, no net size
+    static constexpr int variant = TRTX_YOLO_V3, classes = 80, net_w = 0, net_h = 0, max_out = 1000, levels = 3;
+    static const YoloV3FamilyKernel* kernels() {
+        static const YoloV3FamilyKernel k[3] = {{-1, -1, 32, {116, 90, 156, 198, 373, 326}},
+                                                {-1, -1, 16, {30, 61, 62, 45, 59, 119}},
+                                                {-1, -1, 8, {10, 13, 16, 30, 33, 23}}};
+        return k;
+    }
+};
+
+template <class Traits, bool Dynamic = true>
+class YoloV3FamilyCreatorT : public nvinfer1::IPluginCreator {
+   public:
+    YoloV3FamilyCreatorT() { fc_.nbFields = 0; fc_.fields = nullptr; }
+    const char* getPluginName() const TRTX_NOEXCEPT override { return "YoloLayer_TRT"; }
+    const char* getPluginVersion() const TRTX_NOEXCEPT override { return "1"; }
+    const nvinfer1::PluginFieldCollection* getFieldNames() TRTX_NOEXCEPT override { return &fc_; }
+    // the reference's default constructor: CLASS_NUM, the YoloKernel table, threadCount 256
+    static YoloCore configured() {
+        YoloCore c;
+        c.p.variant = Traits::variant;
+        const int ks = c.v3_kernel_bytes();
+        char blob[TRTX_MAX_LEVELS][36];
+        for (int i = 0; i < Traits::levels; ++i) {
+            const YoloV3FamilyKernel& k = Traits::kernels()[i];
+            std::memcpy(blob[0] + i * ks, &k.w, 4);
+            std::memcpy(blob[0] + i * ks + 4, &k.h, 4);
+            if (ks == 36) std::memcpy(blob[0] + i * ks + 8, &k.stride, 4);
+            std::memcpy(blob[0] + i * ks + ks - 24, k.anchors, 24);
+        }
+        c.init_v3(Traits::variant, Traits::classes, Traits::net_w, Traits::net_h, Traits::max_out, blob, Traits::levels);
+        return c;
+    }
+    nvinfer1::IPluginV2* createPlugin(const char*, const nvinfer1::PluginFieldCollection*) TRTX_NOEXCEPT override {
+        YoloCore c = configured();
+        return make(c);
+    }
+    nvinfer1::IPluginV2* deserializePlugin(const char*, const void* data, size_t len) TRTX_NOEXCEPT override {
+        YoloCore c;
+        if (!data || !c.deserialize_v3(data, len, Traits::variant, Traits::net_w, Traits::net_h, Traits::max_out)) return nullptr;
+        // the driver's plugin always serializes its own YoloKernel count and (spp) strides, which nothing changes: a blob
+        // with other ones is not this driver's (a 3-level yolov7 / YOLOP blob has spp's length but maxOut where the
+        // first stride lies)
+        if (c.p.num_levels != Traits::levels) return nullptr;
+        for (int i = 0; i < Traits::levels; ++i)
+            if (Traits::variant == TRTX_YOLO_V3 && c.p.strides[i] != Traits::kernels()[i].stride) return nullptr;
+        return make(c);
+    }
+    void setPluginNamespace(const char* n) TRTX_NOEXCEPT override { ns_ = n ? n : ""; }
+    const char* getPluginNamespace() const TRTX_NOEXCEPT override { return ns_.c_str(); }
+
+   private:
+    nvinfer1::IPluginV2* make(YoloCore& c) const {
+        c.ns = ns_;
+        if (Dynamic) return new YoloLayerPluginDynamic(c);
+        return new YoloLayerPluginIOExt(c);
+    }
+    std::string ns_;
+    nvinfer1::PluginFieldCollection fc_;
+};
 
 // ================================================================================================
 // Decode_TRT (RetinaFace), retinaface/decode.h:22-107.  The reference serializes nothing and bakes 480x640 in
@@ -986,7 +1149,15 @@ using MaskRcnnInferencePluginIOExtCreator = RcnnCreator<MaskRcnnInferencePluginI
 
 #ifdef TRTX_REGISTER_PLUGINS
 namespace trtx {
-#ifdef TRTX_IMPLICIT_BATCH_PLUGINS
+// TRTX_YOLO_V3_FAMILY=<traits> (YoloV3Traits, YoloV4Traits, ScaledYoloV4Traits, YoloV3TinyTraits, YoloV3SppTraits): the
+// "YoloLayer_TRT" creator is that driver's family creator instead of YoloPluginCreator (only one creator can hold the name)
+#if defined(TRTX_YOLO_V3_FAMILY) && defined(TRTX_IMPLICIT_BATCH_PLUGINS)
+using YoloV3FamilyRegisteredCreator = YoloV3FamilyCreatorT<TRTX_YOLO_V3_FAMILY, false>;
+REGISTER_TENSORRT_PLUGIN(YoloV3FamilyRegisteredCreator);
+#elif defined(TRTX_YOLO_V3_FAMILY)
+using YoloV3FamilyRegisteredCreator = YoloV3FamilyCreatorT<TRTX_YOLO_V3_FAMILY, true>;
+REGISTER_TENSORRT_PLUGIN(YoloV3FamilyRegisteredCreator);
+#elif defined(TRTX_IMPLICIT_BATCH_PLUGINS)
 REGISTER_TENSORRT_PLUGIN(YoloPluginCreatorImplicitBatch);
 #else
 REGISTER_TENSORRT_PLUGIN(YoloPluginCreator);

@@ -13,6 +13,7 @@ MAX_LEVELS = 8
 
 OK, ERR_INVALID, ERR_WORKSPACE, ERR_CUDA, ERR_UNSUPPORTED = range(5)
 YOLO_V8, YOLO_V5, YOLO_V3, YOLO_V26 = 0, 1, 2, 3
+YOLO_V3_NET, YOLO_V4, YOLO_V4_CSP = 4, 5, 6  # the rest of the yolov3 family (trtx_hot.h section 1)
 F32, F16 = 0, 1
 BOX_LTRB, BOX_CXCYWH, BOX_RETINA, BOX_OBB = 0, 1, 2, 3
 NMS_GREEDY, NMS_ONESHOT = 0, 1

@@ -300,14 +300,29 @@ __global__ void __launch_bounds__(32 * SLICES) yolo_v8_scan_kernel(const __grid_
 }
 
 // --------------------------------------------------------------------------------------------
-// Anchor-based scan (yolov5 family; variant TRTX_YOLO_V3 = yolov3 / v3-spp / v4, yolov3-spp/yololayer.cu:148-191: the
-// class probability is gated too (:171), boxes use exp() for w/h and the stride for x/y (:183-186), and the record's
+// Anchor-based scan (yolov5 family; the yolov3 family, yolo_is_v3_family: yolov3-spp/yololayer.cu:148-191 and its
+// siblings, the class probability is gated too (:171), each driver has its own box (trtx_hot.h section 1), and the record's
 // spare float carries the class confidence).  CTA = 4 warps over a tile of 32*VEC cells x 3 anchors.
+// F64: yolov4 / scaled-yolov4's double Logist everywhere a sigmoid is taken; only TRTX_YOLO_V4 / V4_CSP launch it.
 // Objectness rows are read first; the class rows of anchor k are only streamed when some cell of
 // the tile passes the objectness gate for k (the reference skips its class loop per thread,
 // yololayer.cu:176-177; here the skip is per tile so that the loads stay coalesced).
 // --------------------------------------------------------------------------------------------
-template <typename T, int VEC, int U>
+// scaled-yolov4's box, `(col + (2 * Logist(x0))) - 0.5) * INPUT_W / yoloWidth` with its double literal: the float sum is
+// widened, the subtraction, multiply and divide run in double and the result is stored to float; w, h =
+// powf(2 * Logist(x2), 2) * anchor, the same powf call
+template <typename T>
+__device__ __forceinline__ void v4_csp_box(const T* ck, size_t g, int col, int row, int net_w, int net_h, int gw, int gh,
+                                           float aw, float ah, float& bx, float& by, float& bw, float& bh) {
+    const float sx = logist_f64(Elem<T>::ld1_cached(ck)), sy = logist_f64(Elem<T>::ld1_cached(ck + g));
+    const float sw = logist_f64(Elem<T>::ld1_cached(ck + 2 * g)), sh = logist_f64(Elem<T>::ld1_cached(ck + 3 * g));
+    bx = __double2float_rn(__ddiv_rn(__dmul_rn(__dsub_rn((double)((float)col + 2.0f * sx), 0.5), (double)net_w), (double)gw));
+    by = __double2float_rn(__ddiv_rn(__dmul_rn(__dsub_rn((double)((float)row + 2.0f * sy), 0.5), (double)net_h), (double)gh));
+    bw = powf(2.0f * sw, 2.0f) * aw;
+    bh = powf(2.0f * sh, 2.0f) * ah;
+}
+
+template <typename T, int VEC, int U, bool F64 = false>
 __global__ void __launch_bounds__(128) yolo_v5_scan_kernel(const __grid_constant__ YoloArgs a) {
     constexpr int TILE = 32 * VEC;
     constexpr int SLICES = 4;
@@ -359,7 +374,7 @@ __global__ void __launch_bounds__(128) yolo_v5_scan_kernel(const __grid_constant
             bool pass = false;
             // a NaN logit is evaluated too: its box_prob is NaN, which `box_prob < kIgnoreThresh` does not skip
             if (active && (a0 + j < L.g) && !(x[j] <= a.x_lo)) {
-                pr = logist(x[j]);
+                pr = logist_sel<F64>(x[j]);
                 pass = !(pr < a.gate);  // yololayer.cu:177 `if (box_prob < kIgnoreThresh) continue;`
             }
             s_obj[warp][lane * VEC + j] = pass ? pr : -1.0f;
@@ -413,7 +428,8 @@ __global__ void __launch_bounds__(128) yolo_v5_scan_kernel(const __grid_constant
                 float P = 0.0f;
                 if (!(s_obj[k][lane * VEC + j] < 0.0f) && s.bx[j] > -INFINITY) {
                     const T* cls_row0 = base + ((size_t)k * ilen + 5) * g + a0 + j;
-                    P = finish_best(s.bx[j], s.b2[j], s.bc[j], 0.0f, [&](int i) { return Elem<T>::ld1(cls_row0 + (size_t)i * g); });
+                    P = finish_best<F64>(s.bx[j], s.b2[j], s.bc[j], 0.0f,
+                                         [&](int i) { return Elem<T>::ld1(cls_row0 + (size_t)i * g); });
                 }
                 s_fp[k][lane * VEC + j] = P;
                 s_fc[k][lane * VEC + j] = s.bc[j];
@@ -423,7 +439,7 @@ __global__ void __launch_bounds__(128) yolo_v5_scan_kernel(const __grid_constant
     }
     if (warp > 0) return;
     // ---- compaction in ascending (cell, k) order + box decode (yololayer.cu:188-208) ----
-    const bool v3 = a.variant == TRTX_YOLO_V3;
+    const bool v3 = yolo_is_v3_family(a.variant);
     unsigned flags = 0;
 #pragma unroll
     for (int j = 0; j < VEC; ++j)
@@ -443,12 +459,23 @@ __global__ void __launch_bounds__(128) yolo_v5_scan_kernel(const __grid_constant
                     const int e = a0 + j;
                     const int row = e / L.gw, col = e - row * L.gw;
                     const T* ck = base + (size_t)k * ilen * g + e;
-                    if (v3) {  // yolov3-spp/yololayer.cu:183-189
-                        const float fs = (float)L.stride;
-                        const float bx = ((float)col + logist(Elem<T>::ld1_cached(ck))) * fs;
-                        const float by = ((float)row + logist(Elem<T>::ld1_cached(ck + g))) * fs;
-                        const float bw = expf(Elem<T>::ld1_cached(ck + 2 * g)) * L.anc[2 * k];
-                        const float bh = expf(Elem<T>::ld1_cached(ck + 3 * g)) * L.anc[2 * k + 1];
+                    if (v3) {
+                        float bx, by, bw, bh;
+                        if (a.variant == TRTX_YOLO_V3) {  // yolov3-spp/yololayer.cu:183-189
+                            const float fs = (float)L.stride;
+                            bx = ((float)col + logist(Elem<T>::ld1_cached(ck))) * fs;
+                            by = ((float)row + logist(Elem<T>::ld1_cached(ck + g))) * fs;
+                            bw = expf(Elem<T>::ld1_cached(ck + 2 * g)) * L.anc[2 * k];
+                            bh = expf(Elem<T>::ld1_cached(ck + 3 * g)) * L.anc[2 * k + 1];
+                        } else if (F64 && a.variant == TRTX_YOLO_V4_CSP) {  // scaled-yolov4/yololayer.cu:191-194
+                            v4_csp_box(ck, g, col, row, a.net_w, a.net_h, L.gw, L.gh, L.anc[2 * k], L.anc[2 * k + 1],
+                                       bx, by, bw, bh);
+                        } else {  // yolov3/yololayer.cu:173-176, yolov4 :191-194, yolov3-tiny :172-175: float, left to right
+                            bx = ((float)col + logist_sel<F64>(Elem<T>::ld1_cached(ck))) * (float)a.net_w / (float)L.gw;
+                            by = ((float)row + logist_sel<F64>(Elem<T>::ld1_cached(ck + g))) * (float)a.net_h / (float)L.gh;
+                            bw = expf(Elem<T>::ld1_cached(ck + 2 * g)) * L.anc[2 * k];
+                            bh = expf(Elem<T>::ld1_cached(ck + 3 * g)) * L.anc[2 * k + 1];
+                        }
                         store_record(a.cand, slot0 + off, bx, by, bw, bh, s_obj[k][lane * VEC + j], s_fc[k][lane * VEC + j],
                                      L.slot_begin + e * 3 + k, s_fp[k][lane * VEC + j]);
                         ++off;
@@ -665,7 +692,7 @@ __global__ void __launch_bounds__(256) yolo_pack_rows_kernel(const __grid_consta
                 if (a.is_seg | a.is_pose | a.is_obb) write_extras_v8<T>(a, b, anchor_id, det);
             } else if (a.variant == TRTX_YOLO_V5) {
                 write_extras_v5<T>(a, b, anchor_id, det);
-            } else if (a.variant == TRTX_YOLO_V3) {
+            } else if (yolo_is_v3_family(a.variant)) {
                 det[6] = r1.w;  // class_confidence
             } else {            // V26: the reference memsets the buffer, so the fields gatherKernel skips are zero
                 for (int f = 6; f < a.det_floats; ++f) det[f] = 0.0f;
@@ -697,7 +724,7 @@ int yolo_pick_vec(const trtx_yolo_params* p, const void* const* inputs_dev) {
 
 static int validate(const trtx_yolo_params* p, int batch) {
     if (!p || batch <= 0) return TRTX_ERR_INVALID;
-    if (p->variant < TRTX_YOLO_V8 || p->variant > TRTX_YOLO_V26) return TRTX_ERR_INVALID;
+    if (p->variant < TRTX_YOLO_V8 || p->variant > TRTX_YOLO_V4_CSP) return TRTX_ERR_INVALID;
     if (p->num_levels <= 0 || p->num_levels > TRTX_MAX_LEVELS) return TRTX_ERR_INVALID;
     if (p->num_classes <= 0 || p->max_out <= 0 || p->det_floats < 6) return TRTX_ERR_INVALID;
     if (p->in_dtype != TRTX_F32 && p->in_dtype != TRTX_F16) return TRTX_ERR_INVALID;
@@ -712,11 +739,15 @@ static int validate(const trtx_yolo_params* p, int batch) {
     } else if (p->variant == TRTX_YOLO_V5) {
         if (p->is_seg && p->det_floats < 38) return TRTX_ERR_INVALID;
         if (p->is_pose || p->is_obb) return TRTX_ERR_UNSUPPORTED;
-    } else if (p->variant == TRTX_YOLO_V3) {
+    } else if (yolo_is_v3_family(p->variant)) {
         if (p->det_floats < 7) return TRTX_ERR_INVALID;
         if (p->is_seg || p->is_pose || p->is_obb) return TRTX_ERR_UNSUPPORTED;
-        for (int l = 0; l < p->num_levels; ++l)
-            if (p->strides[l] <= 0) return TRTX_ERR_INVALID;
+        if (p->variant == TRTX_YOLO_V3) {  // the only member whose box takes the stride
+            for (int l = 0; l < p->num_levels; ++l)
+                if (p->strides[l] <= 0) return TRTX_ERR_INVALID;
+        } else if (p->net_w <= 0 || p->net_h <= 0) {
+            return TRTX_ERR_INVALID;
+        }
     } else {  // V26: one AoS input; seg / pose tails are "TODO" in the reference too (yololayer.cu:244)
         if (p->num_levels != 1 || p->in_dtype != TRTX_F32) return TRTX_ERR_UNSUPPORTED;
         if (p->is_seg || p->is_pose) return TRTX_ERR_UNSUPPORTED;
@@ -768,7 +799,7 @@ int yolo_fill_args(const trtx_yolo_params* p, int batch, const void* const* inpu
     } else if (p->variant == TRTX_YOLO_V26) {
         a->info_len = 4 + p->num_classes + (p->is_obb ? 1 : 0);  // yolo26 yololayer.cu:189-194
         a->C = a->info_len;
-    } else if (p->variant == TRTX_YOLO_V3) {
+    } else if (yolo_is_v3_family(p->variant)) {
         a->info_len = 5 + p->num_classes;  // yolov3-spp yololayer.cu:159
         a->C = 3 * a->info_len;
     } else {
@@ -823,6 +854,21 @@ static int launch_v8(const YoloArgs& a, const YoloLayout& L, int grid, cudaStrea
     return TRTX_ERR_UNSUPPORTED;  // (slices, rows in flight) pair that is not built
 }
 
+template <bool F64>
+static void launch_v5(const YoloArgs& a, const YoloLayout& L, int in_dtype, int grid, cudaStream_t st) {
+    if (in_dtype == TRTX_F32) {
+        if (L.vec == 4)
+            yolo_v5_scan_kernel<float, 4, 10, F64><<<grid, 128, 0, st>>>(a);
+        else
+            yolo_v5_scan_kernel<float, 1, 10, F64><<<grid, 128, 0, st>>>(a);
+    } else {
+        if (L.vec == 4)
+            yolo_v5_scan_kernel<__half, 4, 10, F64><<<grid, 128, 0, st>>>(a);
+        else
+            yolo_v5_scan_kernel<__half, 1, 10, F64><<<grid, 128, 0, st>>>(a);
+    }
+}
+
 int yolo_scan_launch(const YoloArgs& a, const YoloLayout& L, int in_dtype, int batch, cudaStream_t st) {
     const int grid = batch * L.tiles_per_image;
     if (a.variant == TRTX_YOLO_V26) {
@@ -843,18 +889,10 @@ int yolo_scan_launch(const YoloArgs& a, const YoloLayout& L, int in_dtype, int b
             rc = L.vec == 8 ? launch_v8<__half, 8>(a, L, grid, st)
                             : (L.vec == 4 ? launch_v8<__half, 4>(a, L, grid, st) : launch_v8<__half, 1>(a, L, grid, st));
         if (rc) return rc;
+    } else if (yolo_logist_f64(a.variant)) {
+        launch_v5<true>(a, L, in_dtype, grid, st);
     } else {
-        if (in_dtype == TRTX_F32) {
-            if (L.vec == 4)
-                yolo_v5_scan_kernel<float, 4, 10><<<grid, 128, 0, st>>>(a);
-            else
-                yolo_v5_scan_kernel<float, 1, 10><<<grid, 128, 0, st>>>(a);
-        } else {
-            if (L.vec == 4)
-                yolo_v5_scan_kernel<__half, 4, 10><<<grid, 128, 0, st>>>(a);
-            else
-                yolo_v5_scan_kernel<__half, 1, 10><<<grid, 128, 0, st>>>(a);
-        }
+        launch_v5<false>(a, L, in_dtype, grid, st);
     }
     return check_launch();
 }

@@ -64,12 +64,21 @@ struct YoloLayout {
     size_t total_bytes;
 };
 
+// The yolov3 family: TRTX_YOLO_V3's gates and 7-float rows, one box formula per driver (trtx_hot.h section 1)
+__host__ __device__ __forceinline__ bool yolo_is_v3_family(int variant) {
+    return variant == TRTX_YOLO_V3 || variant == TRTX_YOLO_V3_NET || variant == TRTX_YOLO_V4 || variant == TRTX_YOLO_V4_CSP;
+}
+// yolov4 and scaled-yolov4 evaluate Logist in double: 1. / (1. + exp(-x)), rounded to float
+__host__ __device__ __forceinline__ bool yolo_logist_f64(int variant) {
+    return variant == TRTX_YOLO_V4 || variant == TRTX_YOLO_V4_CSP;
+}
+
 // vec = 4 (128-bit rows) or 1 (scalar fallback for grids not divisible by 4 / unaligned pointers).
 inline YoloLayout yolo_layout(const trtx_yolo_params* p, int batch, int vec) {
     YoloLayout L{};
     L.vec = vec;
     L.tile_cells = 32 * vec;
-    L.apc = (p->variant == TRTX_YOLO_V5 || p->variant == TRTX_YOLO_V3) ? 3 : 1;
+    L.apc = (p->variant == TRTX_YOLO_V5 || yolo_is_v3_family(p->variant)) ? 3 : 1;
     int tiles = 0, slots = 0;
     for (int l = 0; l < p->num_levels; ++l) {
         int g = p->grid_h[l] * p->grid_w[l];
@@ -88,6 +97,16 @@ inline YoloLayout yolo_layout(const trtx_yolo_params* p, int batch, int vec) {
 }
 
 // ---- device helpers shared by the scan kernels ----
+// Logist of yolov4/yololayer.cu:154 and scaled-yolov4/yololayer.cu:154, `1./(1. + exp(-data))` on a float: exp of a float is
+// the float overload (expf), the add and the divide run in double, the result is rounded to float
+__device__ __forceinline__ float logist_f64(float x) { return __double2float_rn(__ddiv_rn(1.0, __dadd_rn(1.0, (double)expf(-x)))); }
+template <bool F64>
+__device__ __forceinline__ float logist_sel(float x) {
+    if constexpr (F64)
+        return logist_f64(x);
+    else
+        return logist(x);
+}
 // Running state of the reference's class loop
 //     max = 0; cls = 0; for i: p = Logist(x_i); if (p > max) { max = p; cls = i; }        (yololayer.cu:195-201)
 // kept in the LOGIT domain: bx = largest logit so far, bc = the first class holding it, b2 = largest logit seen
@@ -127,9 +146,10 @@ __device__ __forceinline__ void merge_one(Best<VEC>& s, int j, float m, float m2
 //     a few ulps apart, or both saturated at 1.0f).  The largest earlier logit is b2, so Logist(b2) != P rules that
 //     out; when it does collide the class rows before bc are re-read (`ld(i)`) and the reference loop is replayed.
 // Anchors below the gate return early (the caller drops them, yololayer.cu:203).
-template <typename LoadRow>
+// F64: the double Logist of yolov4 / scaled-yolov4, monotone non-decreasing too, so the same argument holds.
+template <bool F64 = false, typename LoadRow>
 __device__ __forceinline__ float finish_best(float bx, float b2, int& cls, float gate, LoadRow ld) {
-    const float P = logist(bx), P2 = logist(b2);  // independent: the two evaluations overlap
+    const float P = logist_sel<F64>(bx), P2 = logist_sel<F64>(b2);  // independent: the two evaluations overlap
     if (P < gate) return P;
     if (P == 0.0f) {
         cls = 0;
@@ -137,7 +157,7 @@ __device__ __forceinline__ float finish_best(float bx, float b2, int& cls, float
     }
     if (P2 == P) {
         for (int i = 0; i < cls; ++i) {
-            if (logist(ld(i)) == P) {
+            if (logist_sel<F64>(ld(i)) == P) {
                 cls = i;
                 break;
             }

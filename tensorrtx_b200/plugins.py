@@ -415,7 +415,8 @@ YOLOV3_KERNELS = (YoloKernelV3(-1, -1, 32, (116, 90, 156, 198, 373, 326)),
 
 
 class YoloLayerPluginV3(_TunableYoloLayer):
-    """yolov3-spp/yololayer.h:58-121 (IPluginV2DynamicExt "YoloLayer_TRT" v1; yolov3 / yolov4 carry the same plugin).
+    """yolov3-spp/yololayer.h:58-121 (IPluginV2DynamicExt "YoloLayer_TRT" v1).  yolov3, yolov4, scaled-yolov4 and yolov3-tiny
+    carry another plugin with other box arithmetic: YoloLayerPluginV3Net.
     The reference compiles CLASS_NUM, the kernels and MAX_OUTPUT_BBOX_COUNT in; here they are constructor arguments with
     the reference's values as defaults.  enqueue() takes the grids from the input tensors like the reference
     (yololayer.cu:207-216)."""
@@ -478,6 +479,102 @@ class YoloLayerPluginV3(_TunableYoloLayer):
         p = cls(cc, ks)
         p.mThreadCount = tc
         return p
+
+
+class YoloLayerPluginV3Net(_TunableYoloLayer):
+    """The YoloLayer_TRT of yolov3, yolov4, scaled-yolov4 and yolov3-tiny (yolov4/yololayer.h:52-121, IPluginV2IOExt): grids,
+    anchors, the net size and MAX_OUTPUT_BBOX_COUNT are compile-time constants of each driver's yololayer.h, and its blob,
+    classCount, threadCount, kernelCount, YoloKernel{int width, height; float anchors[6]}[n] (yolov4/yololayer.cu:58-70), does
+    not say which box formula applies.  So the net size and `variant` (YOLO_V3_NET: yolov3, yolov3-tiny; YOLO_V4: yolov4;
+    YOLO_V4_CSP: scaled-yolov4) are constructor arguments; V3_FAMILY_DRIVERS holds each driver's values."""
+    DET_FLOATS = 7  # x,y,w,h, det_confidence, class_id, class_confidence (yolov4/yololayer.h:41-48)
+
+    def __init__(self, classCount: int, kernels: Sequence[YoloKernel], netWidth: int, netHeight: int, variant: int,
+                 maxOut: int = 1000, in_dtype: int = L.F32):
+        if variant not in (L.YOLO_V3_NET, L.YOLO_V4, L.YOLO_V4_CSP):
+            raise ValueError("variant must be YOLO_V3_NET, YOLO_V4 or YOLO_V4_CSP")
+        self.mClassCount, self.mYoloKernel, self.mMaxOutObject = int(classCount), list(kernels), int(maxOut)
+        self.mKernelCount = len(self.mYoloKernel)
+        self.net_w, self.net_h, self.variant = int(netWidth), int(netHeight), int(variant)
+        self._lib = L.load()
+        p = L.YoloParams()
+        p.variant = self.variant
+        p.num_classes, p.max_out, p.det_floats, p.num_levels = self.mClassCount, self.mMaxOutObject, self.DET_FLOATS, self.mKernelCount
+        p.net_w, p.net_h = self.net_w, self.net_h
+        for i, k in enumerate(self.mYoloKernel):
+            p.grid_w[i], p.grid_h[i] = k.width, k.height
+            for j in range(6):
+                p.anchors[i][j] = k.anchors[j]
+        p.gate = 0.1  # IGNORE_THRESH, yolov4/yololayer.h:11
+        p.in_dtype = in_dtype
+        self.params = p
+
+    @classmethod
+    def for_driver(cls, driver: str, in_dtype: int = L.F32) -> "YoloLayerPluginV3Net":
+        """The plugin a driver's YoloPluginCreator::createPlugin builds: its yololayer.h constants (V3_FAMILY_DRIVERS)."""
+        d = V3_FAMILY_DRIVERS[driver]
+        return cls(d["classes"], [YoloKernel(w, h, a) for w, h, a in d["kernels"]], d["net"][0], d["net"][1], d["variant"],
+                   d["max_out"], in_dtype)
+
+    def getOutputDimensions(self, index=0, inputs=None, nbInputDims=0):
+        return (self.mMaxOutObject * self.DET_FLOATS + 1, 1, 1)  # yolov4/yololayer.cu:82-86
+
+    def enqueue(self, batchSize: int, inputs, outputs, workspace, stream=None) -> int:
+        return self._decode(batchSize, inputs, outputs[0], workspace, stream)
+
+    def clone(self) -> "YoloLayerPluginV3Net":
+        p = YoloLayerPluginV3Net(self.mClassCount, self.mYoloKernel, self.net_w, self.net_h, self.variant, self.mMaxOutObject,
+                                 self.params.in_dtype)
+        p.mPluginNamespace = self.mPluginNamespace
+        return p
+
+    def serialize(self) -> bytes:
+        d = struct.pack("<iii", self.mClassCount, self.mThreadCount, self.mKernelCount)
+        for k in self.mYoloKernel:
+            d += struct.pack("<ii6f", k.width, k.height, *k.anchors)
+        return d
+
+    def getSerializationSize(self) -> int:
+        return 12 + 32 * self.mKernelCount
+
+    @classmethod
+    def deserialize(cls, data: bytes, netWidth: int, netHeight: int, variant: int, maxOut: int = 1000) -> "YoloLayerPluginV3Net":
+        """The blob does not hold the net size, the box formula or maxOut: the caller supplies them, as the driver's
+        compiled-in constants do."""
+        if len(data) < 12:
+            raise L.TrtxError("YoloLayerPluginV3Net.deserialize: length mismatch")
+        cc, tc, kc = struct.unpack_from("<iii", data, 0)
+        if kc <= 0 or 12 + 32 * kc != len(data):
+            raise L.TrtxError("YoloLayerPluginV3Net.deserialize: length mismatch")
+        ks = []
+        for i in range(kc):
+            v = struct.unpack_from("<ii6f", data, 12 + 32 * i)
+            ks.append(YoloKernel(v[0], v[1], v[2:]))
+        p = cls(cc, ks, netWidth, netHeight, variant, maxOut)
+        p.mThreadCount = tc
+        return p
+
+
+# Each driver's compiled-in constants (its yololayer.h: CLASS_NUM, INPUT_W x INPUT_H, the YoloKernel table in the plugin's
+# level order, MAX_OUTPUT_BBOX_COUNT), its decode variant, and its NMS as library parameters: nms() drops
+# `det_confidence <= BBOX_CONF_THRESH` (a double literal; conf_thresh is the float with the same verdict) and erases on
+# `iou > NMS_THRESH`.
+_V4_ANCHORS = ((12, 16, 19, 36, 40, 28), (36, 75, 76, 55, 72, 146), (142, 110, 192, 243, 459, 401))
+V3_FAMILY_DRIVERS = {
+    "yolov3": dict(variant=L.YOLO_V3_NET, net=(608, 608), classes=80, max_out=1000,
+                   kernels=((19, 19, (116, 90, 156, 198, 373, 326)), (38, 38, (30, 61, 62, 45, 59, 119)),
+                            (76, 76, (10, 13, 16, 30, 33, 23))), conf_thresh=0.5, nms_thresh=0.4),
+    "yolov4": dict(variant=L.YOLO_V4, net=(608, 608), classes=80, max_out=1000,
+                   kernels=tuple((608 // s, 608 // s, a) for s, a in zip((8, 16, 32), _V4_ANCHORS)), conf_thresh=0.5,
+                   nms_thresh=0.4),
+    "scaled-yolov4": dict(variant=L.YOLO_V4_CSP, net=(512, 512), classes=80, max_out=1000,
+                          kernels=tuple((512 // s, 512 // s, a) for s, a in zip((8, 16, 32), _V4_ANCHORS)), conf_thresh=0.5,
+                          nms_thresh=0.4),
+    # yolov3-tiny.cpp:27-28: BBOX_CONF_THRESH 0.4 compared as a double with `<=`, so the float just below 0.4f
+    "yolov3-tiny": dict(variant=L.YOLO_V3_NET, net=(608, 608), classes=80, max_out=1000,
+                        kernels=((19, 19, (81, 82, 135, 169, 344, 319)), (38, 38, (23, 27, 37, 58, 81, 82))),
+                        conf_thresh=float_le_threshold(0.4), nms_thresh=0.5),
+}
 
 
 class YoloLayerPlugin26(_YoloLayerBase):
@@ -743,7 +840,7 @@ class FusedYoloDecodeNms:
                  device="cuda", return_index=True):
         self.plugin = plugin
         self.max_batch = max_batch
-        v5 = plugin.params.variant in (L.YOLO_V5, L.YOLO_V3)  # anchor-based rows are cx, cy, w, h
+        v5 = plugin.params.variant in (L.YOLO_V5, L.YOLO_V3, L.YOLO_V3_NET, L.YOLO_V4, L.YOLO_V4_CSP)  # rows are cx, cy, w, h
         self.max_det = max_det or plugin.mMaxOutObject
         self.q = nms_params(L.BOX_CXCYWH if v5 else L.BOX_LTRB, mode, conf_thresh, nms_thresh, self.max_det, True)
         self._lib = L.load()
