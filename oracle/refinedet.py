@@ -209,11 +209,13 @@ def as_dets(result: np.ndarray, max_det: int) -> np.ndarray:
 
 
 # ------------------------------------------------------------------ test inputs ----------------------------------------
-def heads(B: int = 1, net: int = NET, C_: int = NUM_CLASSES, seed: int = 0, objects: int = 50, dense: int = 0):
+def heads(B: int = 1, net: int = NET, C_: int = NUM_CLASSES, seed: int = 0, objects: int = 50, dense: int = 0,
+          always=()):
     """Seeded engine heads [B, P, 4], [B, P, 2], [B, P, 4], [B, P, C] float32 with no tied candidate scores in a class:
     per class `objects` planted objects, each a prior with a high score and its anchors and neighbours with lower ones
     (overlapping boxes for the NMS), about one prior in 20 failing the ARM filter, and with `dense` > 0 that many extra
-    candidates in classes 1 and 2 (above top_k: the cut).  Scores are distinct floats drawn from a permutation."""
+    candidates in classes 1 and 2 (above top_k: the cut).  The priors in `always` are candidates of every class.  Scores
+    are distinct floats drawn from a permutation."""
     rng = np.random.default_rng(seed)
     P = num_priors(net)
     arm_loc = rng.normal(0, 0.5, (B, P, 4)).astype(np.float32)
@@ -231,6 +233,7 @@ def heads(B: int = 1, net: int = NET, C_: int = NUM_CLASSES, seed: int = 0, obje
                 picks.update(q for q in (base, base + 1, base + 2, base + 3, base + 4, base + 5, base - 3) if 0 <= q < P)
             if dense and c <= 2:
                 picks.update(rng.choice(P, dense, replace=False).tolist())
+            picks.update(int(q) for q in always)
             picks = np.array(sorted(picks))
             vals = np.linspace(0.0101, 0.99, len(picks), dtype=np.float32)
             odm_conf[b, picks, c] = rng.permutation(vals)
