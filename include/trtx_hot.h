@@ -51,14 +51,15 @@ TRTX_API int trtx_last_cuda_error(void);
  * mirror of the layout: which = 0 trtx_yolo_params, 1 trtx_nms_params, 2 trtx_retina_params, 3 trtx_image_desc,
  * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_frame, 7 trtx_pose_obb_params, 8 trtx_frame,
  * 9 trtx_face_post_params, 10 trtx_yolop_post_params, 11 trtx_detr_post_params, 12 trtx_centernet_params,
- * 13 trtx_ufld_post_params, 14 trtx_refinedet_params;
+ * 13 trtx_ufld_post_params, 14 trtx_refinedet_params, 15 trtx_yolo_topk_params;
  * anything else 0. */
 TRTX_API size_t trtx_abi_sizeof(int which);
 
 /* =====================================================================================
  * 1. YoloLayer_TRT  -- fused per-anchor sigmoid / argmax / gate / box decode / compaction
  *    replaces CalDetection + forwardGpu of
- *      yolov8/plugin/yololayer.cu:178-316 (anchor-free: yolov8, yolo11, yolov12, yolov13, yolov9/10 subsets)
+ *      yolov8/plugin/yololayer.cu:178-316 (anchor-free: yolov8, yolo11, yolov12; yolov9 with det_floats 38,
+ *        yolov10 and yolov13 with det_floats 6 -- each of their CalDetection is yolov8's arithmetic)
  *      yolov5/plugin/yololayer.cu:161-227 (anchor-based: yolov5, yolov7, yolov5-lite, yolop)
  * ===================================================================================== */
 enum {
@@ -154,6 +155,12 @@ enum {
                             extra_offset = 89 for plugin rows); greedy = nms_obb / probiou `>=`
                             (postprocess.cpp:303-385), one-shot = nms_kernel_obb / box_probiou `>`
                             (postprocess.cu:113-166).  Plugin-row source only (not the fused tile source). */
+    TRTX_BOX_V9 = 4,     /* yolov9 (yolov9/src/postprocess.cpp:48-83): rows arrive x1,y1,x2,y2 and each becomes, in float,
+                            cx = (x1 + x2) / 2, cy = (y1 + y2) / 2, w = x2 - x1, h = y2 - y1 before it is sorted or tested;
+                            then TRTX_BOX_CXCYWH's IoU on the converted boxes, and the output rows hold the converted box
+                            (what yolov9's get_rect receives).  Rounding in the conversion can decide a pair near nms_thresh
+                            differently from TRTX_BOX_LTRB.  Greedy only: TRTX_NMS_ONESHOT is TRTX_ERR_UNSUPPORTED.  Both the
+                            plugin-row and the fused / split tile sources */
 };
 enum {
     TRTX_NMS_GREEDY = 0,  /* CPU nms() semantics (the contract, SURVEY.md section 7 "Hard parts") */
@@ -1119,6 +1126,33 @@ TRTX_API int trtx_yolov3spp_letterbox(int img_w, int img_h, int max_size, int ou
  * than 4 757 pixels (the band's staged source rows in shared memory).  No workspace; can be captured in a CUDA graph. */
 TRTX_API int trtx_linear_preprocess_enqueue(int variant, const trtx_image_desc* images_host, int batch, int net_w, int net_h,
                                             int max_size, float* dst_dev, trtx_stream_t stream);
+
+/* =====================================================================================
+ * 16. Rows of the NMS-free YOLO heads (yolov10)
+ *    replaces the HOST batch_topk / get_topk of yolov10/src/postprocess.cpp:35-52, which run on one core after a D2H copy
+ *    of the whole plugin buffer, and the rectangles draw_bbox takes from get_rect (:3-33).
+ * ===================================================================================== */
+typedef struct trtx_yolo_topk_params {
+    int32_t variant;      /* the rectangle, as trtx_get_rect: TRTX_YOLO_V8 (yolov10: l, t, r, b rows, clamped to the frame)
+                             or TRTX_YOLO_V5 (cx, cy, w, h rows, not clamped) */
+    int32_t net_w, net_h; /* kInputW / kInputH (640) */
+    int32_t row_floats;   /* floats per input row, >= 6 (box4, conf, class): 6 for yolov10's Detection */
+    float conf_thresh;    /* a row is skipped when conf <= conf_thresh (kConfThresh 0.5f): a NaN confidence is kept */
+} trtx_yolo_topk_params;
+
+/* dets_dev [B, 1 + max_rows*row_floats]: the plugin output of trtx_yolo_decode_enqueue (TRTX_YOLO_V8, det_floats 6) or any
+ *   buffer of that layout.  Of the first min(count, max_rows) rows, those with !(conf <= conf_thresh) are used, in input
+ *   order, with no NMS and no sort (get_topk reads up to the count, which the reference's plugin lets run past maxOut; the
+ *   library's decode clamps it).
+ * frame_wh_host: `batch` (img_w, img_h) pairs in HOST memory (copied into launch parameters; sizes may differ in a call).
+ * rows_dev [B, 1 + max_rows*6]: the used count, then per used row (x, y, w, h, conf, class) with x, y, w, h = trtx_get_rect
+ *   of the row's box for the variant ({0, 0, 0, 0} where that is undefined), bit-identical to it; rows past the count are
+ *   zeroed.
+ * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
+ * batch / max_rows / sizes <= 0, a variant other than the two above, row_floats < 6.  One launch per 64 frames, one CTA per
+ * frame, no atomics, no workspace; can be captured in a CUDA graph. */
+TRTX_API int trtx_yolo_topk_postprocess_enqueue(const trtx_yolo_topk_params* p, const int32_t* frame_wh_host, int batch,
+                                                const float* dets_dev, int max_rows, float* rows_dev, trtx_stream_t stream);
 
 #ifdef __cplusplus
 }

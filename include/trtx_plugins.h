@@ -138,18 +138,110 @@ struct YoloCore {
         return true;
     }
     int out_elems() const { return 1 + p.max_out * p.det_floats; }  // yololayer.cu:107-111
+
+    // yolov9, yolov10 and yolov13: yolov8's decode (TRTX_YOLO_V8) in another plugin class with another blob, so `blob` says
+    // which layout serialize() writes: 0 the one the variant implies, 9 or 10 below.
+    //   yolov9 (yolov9/plugin/yololayer.cu:25-63): YoloLayerPlugin(classCount, netW, netH, maxOut, is_seg); strides 8, 16, 32
+    //   and grids net / stride are compiled in (:185-187); 38-float rows, the 32 mask coefficients at float 6; blob classCount,
+    //   threadCount, netW, netH, maxOut, is_seg = 21 bytes.
+    //   yolov10 / yolov13 (yolov10/plugin/yololayer.cu:28-84, yolov13's is the same): (classCount, netW, netH, maxOut, strides,
+    //   n); 6-float rows; blob classCount, threadCount, netW, netH, maxOut, n, strides = 24 + 4n bytes.
+    static constexpr int kV9Floats = 38, kV10Floats = 6;
+    int blob = 0;
+    void init_v9(int nc, int w, int h, int max_out, bool seg) {
+        static const int st[3] = {8, 16, 32};
+        init_v8(nc, 0, 0.0f, w, h, max_out, seg, false, false, st, 3);
+        p.det_floats = kV9Floats;
+        blob = 9;
+    }
+    // false for a level count outside 1..TRTX_MAX_LEVELS or a stride <= 0
+    bool init_v10(int nc, int w, int h, int max_out, const int* strides, int n) {
+        if (n < 1 || n > TRTX_MAX_LEVELS) return false;
+        for (int i = 0; i < n; ++i)
+            if (strides[i] <= 0) return false;
+        init_v8(nc, 0, 0.0f, w, h, max_out, false, false, false, strides, n);
+        p.det_floats = kV10Floats;
+        blob = 10;
+        return true;
+    }
+    // createPlugin: yolov9's one field "netinfo" = {nc, w, h, maxOut, is_seg}, read as ints whatever type it is declared with
+    // (the builder declares kFLOAT32 for int data, block.cpp:405-410, and the plugin casts to int*, yololayer.cu:223)
+    bool v9_fields(const nvinfer1::PluginFieldCollection* fc) {
+        if (!fc || fc->nbFields != 1 || !fc->fields) return false;
+        const nvinfer1::PluginField& f = fc->fields[0];
+        if (!f.name || !f.data || std::strcmp(f.name, "netinfo") != 0 || f.length < 5) return false;
+        const int* ni = static_cast<const int*>(f.data);
+        init_v9(ni[0], ni[1], ni[2], ni[3], ni[4] != 0);
+        return true;
+    }
+    // yolov10's / yolov13's one field "combinedInfo" = {nc, w, h, maxOut, strides...} (yolov10/src/block.cpp:235-262)
+    bool v10_fields(const nvinfer1::PluginFieldCollection* fc) {
+        if (!fc || fc->nbFields != 1 || !fc->fields) return false;
+        const nvinfer1::PluginField& f = fc->fields[0];
+        if (!f.name || !f.data || std::strcmp(f.name, "combinedInfo") != 0 || f.length < 5) return false;
+        const int* ci = static_cast<const int*>(f.data);
+        return init_v10(ci[0], ci[1], ci[2], ci[3], ci + 4, f.length - 4);
+    }
+    // the two blobs: exactly 21 bytes with an is_seg byte of 0 or 1; exactly 24 + 4n bytes with n and the strides valid
+    bool deserialize_v9(const void* data, size_t length) {
+        if (!data || length != 21) return false;
+        const char* d = static_cast<const char*>(data);
+        int nc, tc, w, h, mo;
+        unsigned char seg;
+        detail::read(d, nc);
+        detail::read(d, tc);
+        detail::read(d, w);
+        detail::read(d, h);
+        detail::read(d, mo);
+        detail::read(d, seg);
+        if (seg > 1) return false;
+        init_v9(nc, w, h, mo, seg != 0);
+        thread_count = tc;
+        return true;
+    }
+    bool deserialize_v10(const void* data, size_t length) {
+        if (!data || length < 24) return false;
+        const char* d = static_cast<const char*>(data);
+        int nc, tc, w, h, mo, n;
+        detail::read(d, nc);
+        detail::read(d, tc);
+        detail::read(d, w);
+        detail::read(d, h);
+        detail::read(d, mo);
+        detail::read(d, n);
+        if (n < 1 || n > TRTX_MAX_LEVELS || length != 24 + 4 * (size_t)n) return false;
+        int st[TRTX_MAX_LEVELS];
+        for (int i = 0; i < n; ++i) detail::read(d, st[i]);
+        if (!init_v10(nc, w, h, mo, st, n)) return false;
+        thread_count = tc;
+        return true;
+    }
     // the yolov7 / YOLOP blob: the yolov5 one without the is_seg byte (yolov7/plugin/yololayer.cu:62-77,
     // yolop/yololayer.cu:81-101)
     bool v7_layout() const { return p.variant == TRTX_YOLO_V5 && p.det_floats == kV7Floats; }
 
     size_t serial_size() const {
+        if (blob == 9) return 21;
+        if (blob == 10) return 24 + 4 * (size_t)p.num_levels;
         if (p.variant == TRTX_YOLO_V8) return 4 * 8 + 4 * (size_t)p.num_levels + 3;  // yololayer.cu:97-101
         if (v3_kernel_bytes()) return 12 + (size_t)v3_kernel_bytes() * p.num_levels;
         return (v7_layout() ? 24 : 25) + 32 * (size_t)p.num_levels;                 // yolov5 yololayer.cu:72-83
     }
     void serialize(void* buffer) const {
         char* d = static_cast<char*>(buffer);
-        if (p.variant == TRTX_YOLO_V8) {
+        if (blob == 9 || blob == 10) {
+            detail::write(d, p.num_classes);
+            detail::write(d, thread_count);
+            detail::write(d, p.net_w);
+            detail::write(d, p.net_h);
+            detail::write(d, p.max_out);
+            if (blob == 9) {
+                detail::write(d, (bool)p.is_seg);
+            } else {
+                detail::write(d, p.num_levels);
+                for (int i = 0; i < p.num_levels; ++i) detail::write(d, p.strides[i]);
+            }
+        } else if (p.variant == TRTX_YOLO_V8) {
             detail::write(d, p.num_classes);
             detail::write(d, p.num_kpts);
             detail::write(d, p.kpt_thresh);
@@ -541,6 +633,46 @@ class YoloV3FamilyCreatorT : public nvinfer1::IPluginCreator {
     std::string ns_;
     nvinfer1::PluginFieldCollection fc_;
 };
+
+// ------------------------------------------------------------------------------------------------
+// "YoloLayer_TRT"/"1" of yolov9 (Driver = 9) and of yolov10 / yolov13 (Driver = 10).  yolov10's "combinedInfo" has 4 + n ints and
+// yolov8's 9 + n: with up to TRTX_MAX_LEVELS strides the two length ranges overlap, so YoloPluginCreator cannot tell them
+// apart, and it has no yolov9 layout at all.  These creators read their driver's field and blob only (YoloCore::v9_fields /
+// v10_fields, deserialize_v9 / deserialize_v10) and refuse anything else with nullptr, where the reference asserts.
+// ------------------------------------------------------------------------------------------------
+template <int Driver, bool Dynamic = true>
+class YoloAnchorFreeCreatorT : public nvinfer1::IPluginCreator {
+    static_assert(Driver == 9 || Driver == 10, "Driver: 9 (yolov9) or 10 (yolov10, yolov13)");
+
+   public:
+    YoloAnchorFreeCreatorT() { fc_.nbFields = 0; fc_.fields = nullptr; }
+    const char* getPluginName() const TRTX_NOEXCEPT override { return "YoloLayer_TRT"; }
+    const char* getPluginVersion() const TRTX_NOEXCEPT override { return "1"; }
+    const nvinfer1::PluginFieldCollection* getFieldNames() TRTX_NOEXCEPT override { return &fc_; }
+    nvinfer1::IPluginV2* createPlugin(const char*, const nvinfer1::PluginFieldCollection* fc) TRTX_NOEXCEPT override {
+        YoloCore c;
+        if (!(Driver == 9 ? c.v9_fields(fc) : c.v10_fields(fc))) return nullptr;
+        return make(c);
+    }
+    nvinfer1::IPluginV2* deserializePlugin(const char*, const void* data, size_t len) TRTX_NOEXCEPT override {
+        YoloCore c;
+        if (!(Driver == 9 ? c.deserialize_v9(data, len) : c.deserialize_v10(data, len))) return nullptr;
+        return make(c);
+    }
+    void setPluginNamespace(const char* n) TRTX_NOEXCEPT override { ns_ = n ? n : ""; }
+    const char* getPluginNamespace() const TRTX_NOEXCEPT override { return ns_.c_str(); }
+
+   private:
+    nvinfer1::IPluginV2* make(YoloCore& c) const {
+        c.ns = ns_;
+        if (Dynamic) return new YoloLayerPluginDynamic(c);
+        return new YoloLayerPluginIOExt(c);
+    }
+    std::string ns_;
+    nvinfer1::PluginFieldCollection fc_;
+};
+using YoloV9PluginCreator = YoloAnchorFreeCreatorT<9>;
+using YoloV10PluginCreator = YoloAnchorFreeCreatorT<10>;
 
 // ================================================================================================
 // Decode_TRT (RetinaFace), retinaface/decode.h:22-107.  The reference serializes nothing and bakes 480x640 in
@@ -1157,6 +1289,13 @@ REGISTER_TENSORRT_PLUGIN(YoloV3FamilyRegisteredCreator);
 #elif defined(TRTX_YOLO_V3_FAMILY)
 using YoloV3FamilyRegisteredCreator = YoloV3FamilyCreatorT<TRTX_YOLO_V3_FAMILY, true>;
 REGISTER_TENSORRT_PLUGIN(YoloV3FamilyRegisteredCreator);
+// TRTX_YOLO_ANCHOR_FREE=9 (yolov9) or 10 (yolov10, yolov13): that driver's creator instead of YoloPluginCreator
+#elif defined(TRTX_YOLO_ANCHOR_FREE) && defined(TRTX_IMPLICIT_BATCH_PLUGINS)
+using YoloAnchorFreeRegisteredCreator = YoloAnchorFreeCreatorT<TRTX_YOLO_ANCHOR_FREE, false>;
+REGISTER_TENSORRT_PLUGIN(YoloAnchorFreeRegisteredCreator);
+#elif defined(TRTX_YOLO_ANCHOR_FREE)
+using YoloAnchorFreeRegisteredCreator = YoloAnchorFreeCreatorT<TRTX_YOLO_ANCHOR_FREE, true>;
+REGISTER_TENSORRT_PLUGIN(YoloAnchorFreeRegisteredCreator);
 #elif defined(TRTX_IMPLICIT_BATCH_PLUGINS)
 REGISTER_TENSORRT_PLUGIN(YoloPluginCreatorImplicitBatch);
 #else

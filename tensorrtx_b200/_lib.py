@@ -16,6 +16,7 @@ YOLO_V8, YOLO_V5, YOLO_V3, YOLO_V26 = 0, 1, 2, 3
 YOLO_V3_NET, YOLO_V4, YOLO_V4_CSP = 4, 5, 6  # the rest of the yolov3 family (trtx_hot.h section 1)
 F32, F16 = 0, 1
 BOX_LTRB, BOX_CXCYWH, BOX_RETINA, BOX_OBB = 0, 1, 2, 3
+BOX_V9 = 4  # yolov9's nms(): l, t, r, b rows converted to cx, cy, w, h at load (trtx_hot.h section 2)
 NMS_GREEDY, NMS_ONESHOT = 0, 1
 RETINA_FACE, RETINA_ANTICOV = 0, 1
 TASK_POSE, TASK_OBB, TASK_OBB_NMS_FREE = 1, 2, 3
@@ -139,6 +140,10 @@ class RefinedetParams(C.Structure):
                 ("top_k", C.c_int32), ("max_det", C.c_int32), ("score_thresh", C.c_float)]
 
 
+class YoloTopkParams(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("variant", "net_w", "net_h", "row_floats")] + [("conf_thresh", C.c_float)]
+
+
 # TRTX_LIB: another build of the same ABI (the probe build of tools/nms_probe.py); default = the in-tree release library
 LIB_PATH = Path(os.environ.get("TRTX_LIB") or Path(__file__).resolve().parent / "lib" / "libtrtx_hot.so")
 
@@ -218,6 +223,7 @@ SYMBOLS = {
     "trtx_refinedet_workspace_size": (_sz, [C.POINTER(RefinedetParams), _i]),
     "trtx_refinedet_postprocess_enqueue": (_i, [C.POINTER(RefinedetParams), _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp,
                                                 C.POINTER(C.c_int32), _vp, _vp]),
+    "trtx_yolo_topk_postprocess_enqueue": (_i, [C.POINTER(YoloTopkParams), C.POINTER(C.c_int32), _i, _vp, _i, _vp, _vp]),
     "trtx_yolo_decode_nms_gather_enqueue": (_i, [C.POINTER(YoloParams), C.POINTER(NmsParams), _i, _pp, _vp, _vp, _vp, _sz,
                                                  C.POINTER(Gather), _vp]),
     "trtx_gather_wait_enqueue": (_i, [C.POINTER(Gather), _vp]),
@@ -250,7 +256,7 @@ def load() -> C.CDLL:
         fn.argtypes = args
     for which, st in enumerate((YoloParams, NmsParams, RetinaParams, ImageDesc, MaskParams, RcnnPostParams,
                                    Frame, PoseObbParams, Frame, FacePostParams, YolopPostParams,
-                                   DetrPostParams, CenternetParams, UfldPostParams, RefinedetParams)):
+                                   DetrPostParams, CenternetParams, UfldPostParams, RefinedetParams, YoloTopkParams)):
         if lib.trtx_abi_sizeof(which) != C.sizeof(st):
             raise TrtxError(f"{LIB_PATH} was built from a different trtx_hot.h: sizeof({st.__name__}) = "
                             f"{lib.trtx_abi_sizeof(which)} in the library, {C.sizeof(st)} in the binding (rebuild)")

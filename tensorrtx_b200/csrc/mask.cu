@@ -1210,6 +1210,35 @@ __global__ void __launch_bounds__(kRowsThreads) yolop_rows_kernel(const __grid_c
     frame_rows<YolopRow>(a);
 }
 
+// yolov10: get_topk (yolov10/src/postprocess.cpp:35-44) keeps the plugin rows above the threshold, in plugin order, with no
+// NMS; draw_bbox maps them by get_rect (:3-33, yolov8's) into (x, y, w, h, conf, class) rows.
+struct TopkArgs {
+    RowFrames f;
+    int variant, net_w, net_h;
+    float conf_thresh;
+};
+
+struct TopkRow {
+    static constexpr int kGeo = 4;  // the rectangle
+    const TopkArgs& a;
+    int img_w, img_h;
+    __device__ TopkRow(const TopkArgs& args, int j) : a(args), img_w(args.f.img_w[j]), img_h(args.f.img_h[j]) {}
+    // `if (output[1 + det_size * i + 4] <= conf_thresh) continue;`: a NaN confidence is kept
+    __device__ bool pass(const float* d) const { return !(d[4] <= a.conf_thresh); }
+    // the variant as a literal in each call, so that only its own branch of yolo_get_rect is compiled
+    __device__ void geometry(const float* d, int g[4]) const {
+        if (a.variant == TRTX_YOLO_V8)
+            yolo_get_rect(TRTX_YOLO_V8, a.net_w, a.net_h, img_w, img_h, d, g);
+        else
+            yolo_get_rect(TRTX_YOLO_V5, a.net_w, a.net_h, img_w, img_h, d, g);
+    }
+    __device__ float value(const float* d, const int* g, int e) const { return e < 4 ? (float)g[e] : d[e]; }  // conf, class
+};
+
+__global__ void __launch_bounds__(kRowsThreads) topk_rows_kernel(const __grid_constant__ TopkArgs a) {
+    frame_rows<TopkRow>(a);
+}
+
 // YOLOP's labels (yolop/yolop.cpp:148-169): the drivable-area and lane maps resized to the frame with cv::resize(INTER_NEAREST)
 // and combined per pixel, 2 = lane, else 1 = drivable area, else 0, into the frame's u8 canvas.  Bound by the canvas writes.
 // A CTA owns a band of kLabelBand canvas rows of one frame (grid: bands x frames):
@@ -1712,6 +1741,25 @@ TRTX_API int trtx_retina_postprocess_enqueue(const trtx_face_post_params* p, con
     a.lmk_offset = p->lmk_offset;
     a.conf_thresh = p->conf_thresh;
     return launch_frame_rows(face_rows_kernel, a, frame_wh_host, batch, static_cast<cudaStream_t>(stream));
+}
+
+TRTX_API int trtx_yolo_topk_postprocess_enqueue(const trtx_yolo_topk_params* p, const int32_t* frame_wh_host, int batch,
+                                                const float* dets_dev, int max_rows, float* rows_dev, trtx_stream_t stream) {
+    if (!p || !frame_wh_host || batch <= 0 || !dets_dev || !rows_dev || max_rows <= 0) return TRTX_ERR_INVALID;
+    if (p->variant != TRTX_YOLO_V8 && p->variant != TRTX_YOLO_V5) return TRTX_ERR_INVALID;
+    if (p->net_w <= 0 || p->net_h <= 0 || p->row_floats < 6) return TRTX_ERR_INVALID;
+    if (!frames_valid(frame_wh_host, batch)) return TRTX_ERR_INVALID;
+    TopkArgs a;
+    a.f.dets = dets_dev;
+    a.f.rows = rows_dev;
+    a.f.row_floats = p->row_floats;
+    a.f.out_floats = 6;
+    a.f.max_rows = max_rows;
+    a.variant = p->variant;
+    a.net_w = p->net_w;
+    a.net_h = p->net_h;
+    a.conf_thresh = p->conf_thresh;
+    return launch_frame_rows(topk_rows_kernel, a, frame_wh_host, batch, static_cast<cudaStream_t>(stream));
 }
 
 TRTX_API int trtx_yolop_postprocess_enqueue(const trtx_yolop_post_params* p, const trtx_frame* frames_host, int batch,

@@ -1,7 +1,8 @@
 // nms.cu -- sort + class-aware greedy NMS, one 1024-thread CTA per image, every image of the batch
 // in one launch.  Replaces
 //   host  nms()/batch_nms()      yolov8/src/postprocess.cpp:94-129, yolov5/src/postprocess.cpp:49-80,
-//                                retinaface/common.hpp:110-130           (std::map + std::sort + erase)
+//                                retinaface/common.hpp:110-130, yolov9/src/postprocess.cpp:48-83
+//                                                                         (std::map + std::sort + erase)
 //   device cuda_decode()+cuda_nms()  yolov8/src/postprocess.cu:42-111,168-179   (batch 1 only, one-shot)
 //
 // Phases (all on-chip after the first read of the candidates; latency/occupancy-bound, no roofline):
@@ -166,14 +167,22 @@ __device__ __forceinline__ float obb_probiou_dev(const float4 p1, float c1, cons
 // ---- greedy NMS inner loop: boxes pre-converted to corners, areas precomputed ---------------------------------
 // The three host IoUs above differ only in how corners and areas are formed and in retinaface's +1e-6; with those
 // hoisted out (phase D) one test serves all.  Every operation is the reference's, in the reference's order.
+// rows held as cx, cy, w, h while they are tested: yolov5's and the converted ones of yolov9
+__device__ __forceinline__ bool center_size(int fmt) { return fmt == TRTX_BOX_CXCYWH || fmt == TRTX_BOX_V9; }
+// yolov9's nms() (yolov9/src/postprocess.cpp:58-66) turns every l, t, r, b row into c_x = (b0 + b2) / 2, c_y = (b1 + b3) / 2,
+// w = b2 - b0, h = b3 - b1 in float before it sorts or tests it, and pushes the converted box
+__device__ __forceinline__ float4 v9_center_size(const float4 b) {
+    return make_float4(__fmul_rn(__fadd_rn(b.x, b.z), 0.5f), __fmul_rn(__fadd_rn(b.y, b.w), 0.5f), __fsub_rn(b.z, b.x),
+                       __fsub_rn(b.w, b.y));
+}
 __device__ __forceinline__ float4 to_corners(int fmt, const float4 b) {
-    if (fmt != TRTX_BOX_CXCYWH) return b;
+    if (!center_size(fmt)) return b;
     // x/2 == x*0.5 exactly in binary floating point
     const float hw = __fmul_rn(b.z, 0.5f), hh = __fmul_rn(b.w, 0.5f);
     return make_float4(__fsub_rn(b.x, hw), __fsub_rn(b.y, hh), __fadd_rn(b.x, hw), __fadd_rn(b.y, hh));
 }
 __device__ __forceinline__ float box_area(int fmt, const float4 b) {  // b = the row as stored (before to_corners)
-    if (fmt == TRTX_BOX_CXCYWH) return __fmul_rn(b.z, b.w);
+    if (center_size(fmt)) return __fmul_rn(b.z, b.w);
     return __fmul_rn(__fsub_rn(b.z, b.x), __fsub_rn(b.w, b.y));
 }
 struct IouTest {
@@ -422,7 +431,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
     }
     auto put = [&](int pos, const Row& r, uint32_t id) {  // row r into stash slot pos
         const float c = a.class_aware ? r.cls : 0.0f;
-        u_box[pos] = r.box;
+        u_box[pos] = a.box_format == TRTX_BOX_V9 ? v9_center_size(r.box) : r.box;
         u_conf[pos] = r.conf;
         u_cls[pos] = c;
         u_id[pos] = id;
@@ -849,10 +858,11 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
         __syncthreads();
         const int k = carry + block_scan_warp_offset(s_wsum, &s_nkept) + __popc(bal & ((1u << lane) - 1u));
         if (emit && k < a.max_det) {
-            // rows that were turned into corners / covariances for the overlap tests are emitted as they came in
-            const float4 bx = a.box_format == TRTX_BOX_OBB || (greedy && a.box_format == TRTX_BOX_CXCYWH)
-                                  ? fetch_row(a, b, s_id[i]).box
-                                  : s_box[i];
+            // rows that were turned into corners / covariances for the overlap tests are emitted as they came in (yolov9's
+            // converted)
+            float4 bx = a.box_format == TRTX_BOX_OBB || (greedy && center_size(a.box_format)) ? fetch_row(a, b, s_id[i]).box
+                                                                                               : s_box[i];
+            if (a.box_format == TRTX_BOX_V9) bx = v9_center_size(bx);
             float* row = o + 1 + (size_t)k * R;
             row[0] = bx.x;
             row[1] = bx.y;
@@ -979,10 +989,12 @@ __global__ void __launch_bounds__(64) gather_publish_kernel(NmsArgs::Gather g, i
 
 static int nms_validate(const trtx_nms_params* q) {
     if (!q) return TRTX_ERR_INVALID;
-    if (q->box_format < 0 || q->box_format > TRTX_BOX_OBB) return TRTX_ERR_INVALID;
+    if (q->box_format < 0 || q->box_format > TRTX_BOX_V9) return TRTX_ERR_INVALID;
     if (q->box_format == TRTX_BOX_OBB && q->extra_floats < 1) return TRTX_ERR_INVALID;  // the angle travels as the first extra
     if (q->mode != TRTX_NMS_GREEDY && q->mode != TRTX_NMS_ONESHOT) return TRTX_ERR_INVALID;
     if (q->max_det <= 0 || q->extra_floats < 0 || q->extra_offset < 0) return TRTX_ERR_INVALID;
+    // yolov9 has no device post-process to take one-shot semantics from
+    if (q->box_format == TRTX_BOX_V9 && q->mode == TRTX_NMS_ONESHOT) return TRTX_ERR_UNSUPPORTED;
     return TRTX_OK;
 }
 

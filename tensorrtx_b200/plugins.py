@@ -577,6 +577,124 @@ V3_FAMILY_DRIVERS = {
 }
 
 
+class YoloLayerPluginV9(_TunableYoloLayer):
+    """yolov9/plugin/yololayer.h ("YoloLayer_TRT" v1 of yolov9, IPluginV2IOExt): ctor (classCount, netWidth, netHeight,
+    maxOut, is_segmentation).  The strides 8, 16, 32 and grids net / stride are compiled in (yololayer.cu:185-187); yolov8's
+    decode into 38-float rows (box l, t, r, b, conf, class, 32 mask coefficients when is_segmentation).  Blob: classCount,
+    threadCount, netWidth, netHeight, maxOut, is_segmentation = 21 bytes (yololayer.cu:48-60).  TensorRT creator:
+    trtx::YoloV9PluginCreator (include/trtx_plugins.h)."""
+    DET_FLOATS = 38  # yolov9/include/types.h
+    STRIDES = (8, 16, 32)
+
+    def __init__(self, classCount: int, netWidth: int, netHeight: int, maxOut: int, is_segmentation: bool,
+                 in_dtype: int = L.F32):
+        self.mClassCount, self.mYoloV8NetWidth, self.mYoloV8netHeight = int(classCount), int(netWidth), int(netHeight)
+        self.mMaxOutObject, self.is_segmentation_ = int(maxOut), bool(is_segmentation)
+        self._lib = L.load()
+        self.params = _anchor_free_params(self._lib, self.mClassCount, self.mYoloV8NetWidth, self.mYoloV8netHeight,
+                                          self.mMaxOutObject, self.STRIDES, self.DET_FLOATS, self.is_segmentation_, in_dtype)
+
+    def getOutputDimensions(self, index=0, inputs=None, nbInputDims=0):
+        return (self.mMaxOutObject * self.DET_FLOATS + 1, 1, 1)  # yololayer.cu:70-73
+
+    def enqueue(self, batchSize: int, inputs, outputs, workspace, stream=None) -> int:
+        return self._decode(batchSize, inputs, outputs[0], workspace, stream)
+
+    def clone(self) -> "YoloLayerPluginV9":
+        p = YoloLayerPluginV9(self.mClassCount, self.mYoloV8NetWidth, self.mYoloV8netHeight, self.mMaxOutObject,
+                              self.is_segmentation_, self.params.in_dtype)
+        p.mPluginNamespace, p.mThreadCount = self.mPluginNamespace, self.mThreadCount
+        return p
+
+    def serialize(self) -> bytes:
+        return struct.pack("<iiiii?", self.mClassCount, self.mThreadCount, self.mYoloV8NetWidth, self.mYoloV8netHeight,
+                           self.mMaxOutObject, self.is_segmentation_)
+
+    def getSerializationSize(self) -> int:
+        return 21
+
+    @classmethod
+    def deserialize(cls, data: bytes) -> "YoloLayerPluginV9":
+        if len(data) != 21 or data[20] > 1:
+            raise L.TrtxError("YoloLayerPluginV9.deserialize: not a 21-byte yolov9 blob")
+        cc, tc, w, h, mo, seg = struct.unpack("<iiiii?", data)
+        p = cls(cc, w, h, mo, seg)
+        p.mThreadCount = tc
+        return p
+
+
+class YoloLayerPluginV10(_TunableYoloLayer):
+    """yolov10/plugin/yololayer.h and yolov13's, the same class ("YoloLayer_TRT" v1, IPluginV2IOExt): ctor (classCount,
+    netWidth, netHeight, maxOut, strides).  yolov8's decode into 6-float rows (box l, t, r, b, conf, class).  Blob: classCount,
+    threadCount, netWidth, netHeight, maxOut, len(strides), strides = 24 + 4n bytes (yololayer.cu:64-84).  TensorRT creator:
+    trtx::YoloV10PluginCreator (include/trtx_plugins.h)."""
+    DET_FLOATS = 6  # yolov10/include/types.h, yolov13/include/types.h
+
+    def __init__(self, classCount: int, netWidth: int, netHeight: int, maxOut: int, strides: Sequence[int],
+                 in_dtype: int = L.F32):
+        self.mClassCount, self.mYoloV10NetWidth, self.mYoloV10netHeight = int(classCount), int(netWidth), int(netHeight)
+        self.mMaxOutObject, self.mStrides = int(maxOut), [int(s) for s in strides]
+        self._lib = L.load()
+        self.params = _anchor_free_params(self._lib, self.mClassCount, self.mYoloV10NetWidth, self.mYoloV10netHeight,
+                                          self.mMaxOutObject, self.mStrides, self.DET_FLOATS, False, in_dtype)
+
+    def getOutputDimensions(self, index=0, inputs=None, nbInputDims=0):
+        return (self.mMaxOutObject * self.DET_FLOATS + 1, 1, 1)  # yololayer.cu:90-94
+
+    def enqueue(self, batchSize: int, inputs, outputs, workspace, stream=None) -> int:
+        return self._decode(batchSize, inputs, outputs[0], workspace, stream)
+
+    def clone(self) -> "YoloLayerPluginV10":
+        p = YoloLayerPluginV10(self.mClassCount, self.mYoloV10NetWidth, self.mYoloV10netHeight, self.mMaxOutObject,
+                               self.mStrides, self.params.in_dtype)
+        p.mPluginNamespace, p.mThreadCount = self.mPluginNamespace, self.mThreadCount
+        return p
+
+    def serialize(self) -> bytes:
+        n = len(self.mStrides)
+        return struct.pack(f"<6i{n}i", self.mClassCount, self.mThreadCount, self.mYoloV10NetWidth, self.mYoloV10netHeight,
+                           self.mMaxOutObject, n, *self.mStrides)
+
+    def getSerializationSize(self) -> int:
+        return 24 + 4 * len(self.mStrides)
+
+    @classmethod
+    def deserialize(cls, data: bytes) -> "YoloLayerPluginV10":
+        if len(data) < 24:
+            raise L.TrtxError("YoloLayerPluginV10.deserialize: length mismatch")
+        cc, tc, w, h, mo, n = struct.unpack_from("<6i", data, 0)
+        if not 1 <= n <= L.MAX_LEVELS or len(data) != 24 + 4 * n:
+            raise L.TrtxError("YoloLayerPluginV10.deserialize: length mismatch")
+        p = cls(cc, w, h, mo, struct.unpack_from(f"<{n}i", data, 24))
+        p.mThreadCount = tc
+        return p
+
+
+def _anchor_free_params(lib, nc, w, h, max_out, strides, det_floats, seg, in_dtype) -> L.YoloParams:
+    """TRTX_YOLO_V8 parameters for yolov9 / yolov10 / yolov13: each one's CalDetection is yolov8's arithmetic."""
+    p = L.YoloParams()
+    arr = (C.c_int * len(strides))(*strides)
+    L.check(lib.trtx_yolo_params_init_v8(C.byref(p), nc, w, h, max_out, arr, len(strides)), "trtx_yolo_params_init_v8")
+    p.det_floats, p.is_seg, p.in_dtype = det_floats, int(seg), in_dtype
+    return p
+
+
+# Each driver's compiled-in constants (config.h) and its host post-process as library parameters:
+#   yolov9: nms() (src/postprocess.cpp:48-83) on rows i < kMaxNumOutputBbox, `conf <= kConfThresh` dropped, boxes converted to
+#     cx, cy, w, h (BOX_V9), `iou > kNmsThresh` erased, conf-only sort (no box[0] tie-break); get_rect is yolov5's, unclamped;
+#   yolov10: get_topk (:35-44), no NMS: yolo_topk_postprocess with yolov8's clamped get_rect (YOLO_V8);
+#   yolov13: yolov8's nms() (isnan guard, box[0] tie-break) on l, t, r, b rows, and yolov8's get_rect.  Its device post-process
+#     (postprocess.cu) strides 7-float rows by bbox_element = 4 and is not followed (DESIGN.md section 2).
+ANCHOR_FREE_DRIVERS = {
+    "yolov9": dict(plugin=YoloLayerPluginV9, net=(640, 640), classes=80, max_out=2000, det_floats=38, conf_thresh=0.1,
+                   nms_thresh=0.45, box_format=L.BOX_V9, mode=L.NMS_GREEDY, tie_break_x0=False, rect=L.YOLO_V5),
+    "yolov10": dict(plugin=YoloLayerPluginV10, net=(640, 640), classes=80, max_out=1000, det_floats=6, conf_thresh=0.5,
+                    nms_thresh=None, box_format=None, mode=None, tie_break_x0=None, rect=L.YOLO_V8),
+    "yolov13": dict(plugin=YoloLayerPluginV10, net=(640, 640), classes=80, max_out=1000, det_floats=6, conf_thresh=0.5,
+                    nms_thresh=0.45, box_format=L.BOX_LTRB, mode=L.NMS_GREEDY, tie_break_x0=True, rect=L.YOLO_V8),
+}
+
+
 class YoloLayerPlugin26(_YoloLayerBase):
     """yolo26/plugin/yololayer.h:10-77 ("YoloLayer_TRT" v1 of the NMS-free yolo26 heads): ctor (classCount, numberOfPoints,
     maxDetections, isDetection, isSegmentation, isPose, isObb, anchor_count); setPluginDeviceParams(confThreshold) of the
@@ -801,6 +919,27 @@ def yolo_pose_obb_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[in
     return rows_out
 
 
+def yolo_topk_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]], *, max_rows: int,
+                          conf_thresh: float = 0.5, row_floats: int = 6, variant: int = L.YOLO_V8, net_w: int = 640,
+                          net_h: int = 640, rows_out: torch.Tensor | None = None, stream=None) -> torch.Tensor:
+    """GPU drop-in for yolov10's host post-process: batch_topk / get_topk (yolov10/src/postprocess.cpp:35-52: every plugin row
+    with !(conf <= conf_thresh), a NaN conf included, in plugin order, no NMS) and draw_bbox's get_rect (yolov8's, clamped:
+    variant YOLO_V8) for a batch of frames of any sizes.  dets [B, 1 + max_rows*row_floats]: the YoloLayerPluginV10 output
+    (row_floats 6).  image_sizes[b] = (img_w, img_h) -> rows [B, 1 + max_rows*6] fp32: the used count, then (x, y, w, h,
+    conf, class) per used row; rows past the count are zero.  One launch per 64 frames, no workspace."""
+    lib = L.load()
+    B = len(image_sizes)
+    if dets.dim() != 2 or dets.shape[0] != B or dets.shape[1] < 1 + max_rows * row_floats:
+        raise ValueError(f"dets must be [{B}, >= {1 + max_rows * row_floats}]")
+    _f32_rows(dets)
+    q = L.YoloTopkParams(variant, net_w, net_h, row_floats, conf_thresh)
+    rows_out = _out_tensor(rows_out, (B, 1 + max_rows * 6), torch.float32, dets.device,
+                           f"rows_out must be contiguous float32 [{B}, {1 + max_rows * 6}]")
+    L.check(lib.trtx_yolo_topk_postprocess_enqueue(C.byref(q), _frame_wh(image_sizes), B, _ptr(dets), max_rows, _ptr(rows_out),
+                                                   _stream(stream)), "trtx_yolo_topk_postprocess_enqueue")
+    return rows_out
+
+
 def retina_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]], *, variant: int, max_rows: int,
                        conf_thresh: float, in_w: int, in_h: int, row_floats: int | None = None, lmk_offset: int = 7,
                        rows_out: torch.Tensor | None = None, stream=None) -> torch.Tensor:
@@ -837,12 +976,15 @@ class FusedYoloDecodeNms:
     Owns its workspace/output buffers (allocated once; enqueue itself allocates nothing)."""
 
     def __init__(self, plugin, max_batch: int, conf_thresh=0.5, nms_thresh=0.45, max_det=None, mode=L.NMS_GREEDY,
-                 device="cuda", return_index=True):
+                 device="cuda", return_index=True, box_format=None):
+        """box_format: the NMS box format (e.g. BOX_V9 for yolov9); by default the one the decode variant's rows have."""
         self.plugin = plugin
         self.max_batch = max_batch
         v5 = plugin.params.variant in (L.YOLO_V5, L.YOLO_V3, L.YOLO_V3_NET, L.YOLO_V4, L.YOLO_V4_CSP)  # rows are cx, cy, w, h
+        if box_format is None:
+            box_format = L.BOX_CXCYWH if v5 else L.BOX_LTRB
         self.max_det = max_det or plugin.mMaxOutObject
-        self.q = nms_params(L.BOX_CXCYWH if v5 else L.BOX_LTRB, mode, conf_thresh, nms_thresh, self.max_det, True)
+        self.q = nms_params(box_format, mode, conf_thresh, nms_thresh, self.max_det, True)
         self._lib = L.load()
         self.ws_bytes = plugin.getWorkspaceSize(max_batch)
         self.ws = torch.empty(self.ws_bytes, dtype=torch.uint8, device=device)
