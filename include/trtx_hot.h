@@ -51,7 +51,7 @@ TRTX_API int trtx_last_cuda_error(void);
  * mirror of the layout: which = 0 trtx_yolo_params, 1 trtx_nms_params, 2 trtx_retina_params, 3 trtx_image_desc,
  * 4 trtx_mask_params, 5 trtx_rcnn_post_params, 6 trtx_frame, 7 trtx_pose_obb_params, 8 trtx_frame,
  * 9 trtx_face_post_params, 10 trtx_yolop_post_params, 11 trtx_detr_post_params, 12 trtx_centernet_params,
- * 13 trtx_ufld_post_params, 14 trtx_refinedet_params, 15 trtx_yolo_topk_params;
+ * 13 trtx_ufld_post_params, 14 trtx_refinedet_params, 15 trtx_yolo_topk_params, 16 trtx_pyrunner_params;
  * anything else 0. */
 TRTX_API size_t trtx_abi_sizeof(int which);
 
@@ -1099,6 +1099,9 @@ enum {
                                    (exact) */
     TRTX_LINEAR_YOLOV3_SPP = 2, /* yolov3-spp's letterbox; planes R, G, B; data = (float)u * (float)(1 / 255.0), as
                                    blobFromImage(pr, 1 / 255.0, size, Scalar(0, 0, 0), swapRB = true, crop = false) stores it */
+    TRTX_LINEAR_PY = 4,         /* the Python runners' preprocess_image (section 17): trtx_pyrunner_letterbox_rect's rectangle
+                                   on a 128 canvas; planes R, G, B; data as TRTX_LINEAR_YOLOV3 (float32 u / 255.0f is the same
+                                   float for every byte) */
 };
 
 /* yolov3-spp's letterbox of an img_w x img_h frame for MAX_INPUT_SIZE = max_size (608 in the reference): r = std::min(max_size /
@@ -1118,8 +1121,9 @@ TRTX_API int trtx_yolov3spp_letterbox(int img_w, int img_h, int max_size, int ou
  * and off); a frame
  * resized to its own size is copied.  The rectangle is trtx_calib_letterbox_rect's for TRTX_LINEAR_YOLOV3 / RETINA
  * (INPUT_W x INPUT_H: 608 x 608 for yolov3 / yolov4, 512 x 512 for scaled-yolov4, 640 x 480 for RetinaFace) and
- * trtx_yolov3spp_letterbox's for TRTX_LINEAR_YOLOV3_SPP.  max_size is read by TRTX_LINEAR_YOLOV3_SPP only; its engine binds
- * one input shape per enqueue, so every frame's canvas must be net_w x net_h.
+ * trtx_yolov3spp_letterbox's for TRTX_LINEAR_YOLOV3_SPP, trtx_pyrunner_letterbox_rect's for TRTX_LINEAR_PY (any net_w x
+ * net_h).  max_size is read by TRTX_LINEAR_YOLOV3_SPP only; its engine binds one input shape per enqueue, so every frame's
+ * canvas must be net_w x net_h.
  * Every descriptor is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
  * batch / net sizes <= 0, pitch < 3 * width, an unknown variant, a dst_dev that is not 4-byte aligned, or (SPP) max_size <= 0
  * or a frame whose canvas is not net_w x net_h; TRTX_ERR_UNSUPPORTED for an empty rectangle (cv::resize throws) or one wider
@@ -1153,6 +1157,57 @@ typedef struct trtx_yolo_topk_params {
  * frame, no atomics, no workspace; can be captured in a CUDA graph. */
 TRTX_API int trtx_yolo_topk_postprocess_enqueue(const trtx_yolo_topk_params* p, const int32_t* frame_wh_host, int batch,
                                                 const float* dets_dev, int max_rows, float* rows_dev, trtx_stream_t stream);
+
+/* =====================================================================================
+ * 17. The Python runners' pre- and post-process (the *_trt.py scripts)
+ *    replaces preprocess_image (yolov8/yolov8_det_trt.py:207-253, the same body in every yolov5, yolov7, yolov8, yolo11,
+ *    yolov9, yolov10, yolov12-tubro and yolov13 runner) and the detection runners' post_process + non_max_suppression +
+ *    bbox_iou + xywh2xyxy (yolov8_det_trt.py:255-381, yolov5/yolov5_det_trt.py:250-276), which run in numpy on one core per
+ *    frame after a D2H copy of the whole plugin buffer.  The pre-process is trtx_linear_preprocess_enqueue(TRTX_LINEAR_PY).
+ * ===================================================================================== */
+
+/* preprocess_image's rectangle {x, y, w, h} of a src_w x src_h frame in a net_w x net_h input: r_w = net_w / src_w and
+ * r_h = net_h / src_h in double; if r_h > r_w, w = net_w, h = (int)(r_w * src_h), x = 0, y = (net_h - h) / 2, else the
+ * mirror case.  It differs from trtx_calib_letterbox_rect's float ratios for real frames (592 x 333 into 640 x 640: h = 360
+ * here, 359 there).  TRTX_ERR_INVALID for a null rect or a size <= 0.  Host function. */
+TRTX_API int trtx_pyrunner_letterbox_rect(int src_w, int src_h, int net_w, int net_h, int rect[4]);
+
+typedef struct trtx_pyrunner_params {
+    int32_t box_format;   /* how xywh2xyxy reads the plugin box: TRTX_BOX_LTRB (yolov8, yolo11, yolov9, yolov10,
+                             yolov12-tubro, yolov13: l, t, r, b) or TRTX_BOX_CXCYWH (yolov3, yolov5, yolov7: cx, cy, w, h) */
+    int32_t net_w, net_h; /* the runner's input_w / input_h */
+    int32_t row_floats;   /* floats per plugin row: 90 (yolov8 det / 5u, yolo11, yolov12-tubro), 38 (yolov9, yolov5), 7 (yolov3),
+                             6 (yolov7, yolov10, yolov13, yolov5 cuda-python) */
+    int32_t label_col;    /* the float non_max_suppression compares as the label, boxes[:, -1]: row_floats - 1, or 5 where
+                             the runner slices the row (yolov5 `pred[:, :6]`, yolov3); 5 <= label_col < row_floats */
+    int32_t conf_col;     /* -1, or the column yolov3's post_process multiplies into the confidence (`pred[:, 4] *=
+                             pred[:, 6]`): 6; 5 <= conf_col < row_floats, != label_col */
+    float conf_thresh;    /* CONF_THRESH (0.5): a row is used when conf >= conf_thresh (a NaN conf never is) */
+    float nms_thresh;     /* IOU_THRESHOLD (0.4): row j is removed by a kept row when IoU > nms_thresh and the labels are == */
+} trtx_pyrunner_params;
+
+/* The runner's post_process for a batch of frames of any sizes, one CTA per frame.
+ * dets_dev [B, 1 + max_rows*row_floats]: the plugin output of trtx_yolo_decode_enqueue or any buffer of that layout;
+ *   max_rows <= TRTX_NMS_MAX_ROWS.  The first n rows are read, n = the count float truncated and clamped to [0, max_rows]
+ *   (a count below 1 or NaN reads none: the runner slices from the end for a negative count and raises on a NaN; the
+ *   plugin writes neither).
+ * frame_wh_host: `batch` (img_w, img_h) pairs in HOST memory, copied into launch parameters.
+ * Per frame, all in float32 as numpy computes it: conf = row[4] (times row[conf_col]); rows with conf >= conf_thresh; the
+ *   box mapped by xywh2xyxy (the pad (net - r * origin) / 2 and the ratio r are computed in double and rounded to float,
+ *   then y -= pad, y /= r) and clipped to [0, img_w - 1] x [0, img_h - 1] as np.clip does (a NaN stays NaN); sorted by
+ *   descending conf, equal confs by ascending row (the runner's argsort leaves ties open); then greedy NMS: the front row
+ *   is kept and always consumed, and removes every later row j with bbox_iou > nms_thresh (+1 on widths and heights,
+ *   + 1e-16f in the denominator, no contraction) and row[label_col] == the front row's (a NaN label or box never
+ *   matches).  The runner loops forever where a front row does not remove itself (a NaN label or box, an inverted box);
+ *   the device defines that case by the consume rule and agrees with the runner wherever the runner returns.
+ * rows_dev [B, 1 + max_rows*6]: the kept count, then the kept rows in order as (x1, y1, x2, y2, conf, row[5]) floats at
+ *   the frame's size; floats past the count are zeroed.
+ * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
+ * batch / max_rows / net or frame sizes <= 0, another box format, columns outside the ranges above, or a NaN threshold;
+ * TRTX_ERR_UNSUPPORTED for max_rows > TRTX_NMS_MAX_ROWS.  One launch per 64 frames, no atomics, no workspace,
+ * deterministic; can be captured in a CUDA graph. */
+TRTX_API int trtx_pyrunner_postprocess_enqueue(const trtx_pyrunner_params* p, const int32_t* frame_wh_host, int batch,
+                                               const float* dets_dev, int max_rows, float* rows_dev, trtx_stream_t stream);
 
 #ifdef __cplusplus
 }

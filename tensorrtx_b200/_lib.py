@@ -21,7 +21,7 @@ NMS_GREEDY, NMS_ONESHOT = 0, 1
 RETINA_FACE, RETINA_ANTICOV = 0, 1
 TASK_POSE, TASK_OBB, TASK_OBB_NMS_FREE = 1, 2, 3
 CUBIC_YOLOV3_TINY, CUBIC_ANTICOV = 0, 1
-LINEAR_YOLOV3, LINEAR_RETINA, LINEAR_YOLOV3_SPP = 0, 1, 2
+LINEAR_YOLOV3, LINEAR_RETINA, LINEAR_YOLOV3_SPP, LINEAR_PY = 0, 1, 2, 4
 RECT_YOLOV3_SPP = 16  # trtx_get_rect / the seg rows: yolov3-spp's get_rect
 
 _ERR = {1: "TRTX_ERR_INVALID", 2: "TRTX_ERR_WORKSPACE", 3: "TRTX_ERR_CUDA", 4: "TRTX_ERR_UNSUPPORTED"}
@@ -144,6 +144,11 @@ class YoloTopkParams(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("variant", "net_w", "net_h", "row_floats")] + [("conf_thresh", C.c_float)]
 
 
+class PyrunnerParams(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("box_format", "net_w", "net_h", "row_floats", "label_col", "conf_col")] + \
+               [(n, C.c_float) for n in ("conf_thresh", "nms_thresh")]
+
+
 # TRTX_LIB: another build of the same ABI (the probe build of tools/nms_probe.py); default = the in-tree release library
 LIB_PATH = Path(os.environ.get("TRTX_LIB") or Path(__file__).resolve().parent / "lib" / "libtrtx_hot.so")
 
@@ -224,6 +229,8 @@ SYMBOLS = {
     "trtx_refinedet_postprocess_enqueue": (_i, [C.POINTER(RefinedetParams), _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp,
                                                 C.POINTER(C.c_int32), _vp, _vp]),
     "trtx_yolo_topk_postprocess_enqueue": (_i, [C.POINTER(YoloTopkParams), C.POINTER(C.c_int32), _i, _vp, _i, _vp, _vp]),
+    "trtx_pyrunner_letterbox_rect": (_i, [_i, _i, _i, _i, C.POINTER(C.c_int)]),
+    "trtx_pyrunner_postprocess_enqueue": (_i, [C.POINTER(PyrunnerParams), C.POINTER(C.c_int32), _i, _vp, _i, _vp, _vp]),
     "trtx_yolo_decode_nms_gather_enqueue": (_i, [C.POINTER(YoloParams), C.POINTER(NmsParams), _i, _pp, _vp, _vp, _vp, _sz,
                                                  C.POINTER(Gather), _vp]),
     "trtx_gather_wait_enqueue": (_i, [C.POINTER(Gather), _vp]),
@@ -256,7 +263,8 @@ def load() -> C.CDLL:
         fn.argtypes = args
     for which, st in enumerate((YoloParams, NmsParams, RetinaParams, ImageDesc, MaskParams, RcnnPostParams,
                                    Frame, PoseObbParams, Frame, FacePostParams, YolopPostParams,
-                                   DetrPostParams, CenternetParams, UfldPostParams, RefinedetParams, YoloTopkParams)):
+                                   DetrPostParams, CenternetParams, UfldPostParams, RefinedetParams, YoloTopkParams,
+                                   PyrunnerParams)):
         if lib.trtx_abi_sizeof(which) != C.sizeof(st):
             raise TrtxError(f"{LIB_PATH} was built from a different trtx_hot.h: sizeof({st.__name__}) = "
                             f"{lib.trtx_abi_sizeof(which)} in the library, {C.sizeof(st)} in the binding (rebuild)")

@@ -20,7 +20,7 @@ LIBDIR = PKG / "lib"
 LIB = LIBDIR / "libtrtx_hot.so"
 
 SOURCES = ["yolo_decode.cu", "nms.cu", "retina_decode.cu", "rcnn.cu", "preprocess.cu", "mask.cu", "roi_align.cu", "calib_host.cu", "cls.cu",
-           "detr.cu", "centernet.cu", "ufld.cu", "refinedet.cu"]
+           "detr.cu", "centernet.cu", "ufld.cu", "refinedet.cu", "pyrunner.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

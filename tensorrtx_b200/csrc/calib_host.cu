@@ -59,6 +59,27 @@ TRTX_API int trtx_calib_letterbox_rect(int src_w, int src_h, int net_w, int net_
     return TRTX_OK;
 }
 
+// The Python runners' preprocess_image (yolov8_det_trt.py:223-236): the ratios and products stay double, int() truncates;
+// (net - h) is never negative, so int((net - h) / 2) is the integer division.
+TRTX_API int trtx_pyrunner_letterbox_rect(int src_w, int src_h, int net_w, int net_h, int rect[4]) {
+    if (src_w <= 0 || src_h <= 0 || net_w <= 0 || net_h <= 0 || !rect) return TRTX_ERR_INVALID;
+    const double r_w = (double)net_w / src_w, r_h = (double)net_h / src_h;
+    int w, h, x, y;
+    if (r_h > r_w) {
+        w = net_w;
+        h = (int)(r_w * src_h);
+        x = 0;
+        y = (net_h - h) / 2;
+    } else {
+        w = (int)(r_h * src_w);
+        h = net_h;
+        x = (net_w - w) / 2;
+        y = 0;
+    }
+    rect[0] = x, rect[1] = y, rect[2] = w, rect[3] = h;
+    return TRTX_OK;
+}
+
 TRTX_API int trtx_calib_letterbox_host(const uint8_t* bgr, int src_w, int src_h, size_t src_pitch, int net_w, int net_h, float* out_chw) {
     if (!bgr || !out_chw || src_pitch < (size_t)src_w * 3) return TRTX_ERR_INVALID;
     int rc[4];

@@ -912,6 +912,7 @@ __global__ void __launch_bounds__(kRcnnPreThreads) cubic_preprocess_kernel(const
 // Bilinear letterbox pre-process of yolov3, yolov4, scaled-yolov4, yolov3-spp and RetinaFace: resize_band with a planar store;
 // only the value conventions and the host-side rectangles are their own.
 //   TRTX_LINEAR_YOLOV3      the yolov3-tiny chain, u / 255.0 in double (CubicInput<TRTX_CUBIC_YOLOV3_TINY>), planes R, G, B;
+//   TRTX_LINEAR_PY          the same store over the Python runners' rectangle: their float32 u / 255.0f is that float;
 //   TRTX_LINEAR_RETINA      RetinaInput below;
 //   TRTX_LINEAR_YOLOV3_SPP  blobFromImage's (float)u * (float)(1 / 255.0), planes R, G, B: cls_preprocess_kernel<TRTX_YOLO_V8>,
 //                           whose value chain it is, over yolov3-spp's rectangle.
@@ -943,6 +944,22 @@ static int spp_band_image(const trtx_image_desc& d, int max_size, int net_w, int
     im.sh = d.height;
     im.pitch = d.pitch;
     im.x0 = g[2], im.y0 = g[3], im.rw = g[4], im.rh = g[5];
+    im.scale_x = 1. / ((double)im.rw / im.sw);
+    im.scale_y = 1. / ((double)im.rh / im.sh);
+    return TRTX_OK;
+}
+
+// The band descriptor of frame d in the Python runners' preprocess_image: trtx_pyrunner_letterbox_rect's rectangle, which
+// cv2.resize fills with the frame; TRTX_ERR_UNSUPPORTED where it is empty (cv2.resize raises).
+static int py_band_image(const trtx_image_desc& d, int net_w, int net_h, RcnnPreImage& im) {
+    int r[4];
+    trtx_pyrunner_letterbox_rect(d.width, d.height, net_w, net_h, r);
+    if (r[2] <= 0 || r[3] <= 0) return TRTX_ERR_UNSUPPORTED;
+    im.src = d.data_dev;
+    im.sw = d.width;
+    im.sh = d.height;
+    im.pitch = d.pitch;
+    im.x0 = r[0], im.y0 = r[1], im.rw = r[2], im.rh = r[3];
     im.scale_x = 1. / ((double)im.rw / im.sw);
     im.scale_y = 1. / ((double)im.rh / im.sh);
     return TRTX_OK;
@@ -1306,17 +1323,20 @@ TRTX_API int trtx_yolov3spp_letterbox(int img_w, int img_h, int max_size, int ou
     return lb.unpad_w > 0 && lb.unpad_h > 0 ? TRTX_OK : TRTX_ERR_UNSUPPORTED;
 }
 
-// preprocess_img with INTER_LINEAR (yolov3, yolov4, scaled-yolov4, RetinaFace: cls_band_image's V5 rectangle) or yolov3-spp's
-// letterbox (spp_band_image), the bilinear band kernel with the variant's planar store.
+// preprocess_img with INTER_LINEAR (yolov3, yolov4, scaled-yolov4, RetinaFace: cls_band_image's V5 rectangle), yolov3-spp's
+// letterbox (spp_band_image) or the Python runners' preprocess_image (py_band_image), the bilinear band kernel with the
+// variant's planar store.
 TRTX_API int trtx_linear_preprocess_enqueue(int variant, const trtx_image_desc* images_host, int batch, int net_w, int net_h,
                                             int max_size, float* dst_dev, trtx_stream_t stream) {
     if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
-    if (variant != TRTX_LINEAR_YOLOV3 && variant != TRTX_LINEAR_RETINA && variant != TRTX_LINEAR_YOLOV3_SPP)
+    if (variant != TRTX_LINEAR_YOLOV3 && variant != TRTX_LINEAR_RETINA && variant != TRTX_LINEAR_YOLOV3_SPP &&
+        variant != TRTX_LINEAR_PY)
         return TRTX_ERR_INVALID;
     if (variant == TRTX_LINEAR_YOLOV3_SPP && max_size <= 0) return TRTX_ERR_INVALID;
     if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
     auto make = [&](int i, RcnnPreImage& im) -> int {
         if (variant == TRTX_LINEAR_YOLOV3_SPP) return spp_band_image(images_host[i], max_size, net_w, net_h, im);
+        if (variant == TRTX_LINEAR_PY) return py_band_image(images_host[i], net_w, net_h, im);
         return cls_band_image(TRTX_YOLO_V5, images_host[i], net_w, net_h, im) ? TRTX_OK : TRTX_ERR_UNSUPPORTED;
     };
     // every descriptor is checked before the first launch, so that a rejected call writes nothing
@@ -1333,7 +1353,8 @@ TRTX_API int trtx_linear_preprocess_enqueue(int variant, const trtx_image_desc* 
         if (smem > kClsMaxDynamicSmem) return TRTX_ERR_UNSUPPORTED;
         smem_max = smem > smem_max ? smem : smem_max;
     }
-    auto* kernel = variant == TRTX_LINEAR_YOLOV3  ? linear_preprocess_kernel<CubicInput<TRTX_CUBIC_YOLOV3_TINY>>
+    auto* kernel = variant == TRTX_LINEAR_YOLOV3 || variant == TRTX_LINEAR_PY
+                       ? linear_preprocess_kernel<CubicInput<TRTX_CUBIC_YOLOV3_TINY>>
                    : variant == TRTX_LINEAR_RETINA ? linear_preprocess_kernel<RetinaInput>
                                                    : cls_preprocess_kernel<TRTX_YOLO_V8>;
     return launch_bands(kernel, batch, net_w, net_h, dst_dev, smem_max, static_cast<cudaStream_t>(stream),

@@ -189,24 +189,6 @@ __global__ void __launch_bounds__(kRdThreads) refinedet_nms_kernel(const __grid_
     if (lane == 0) a.count[(size_t)b * ncls + (c - 1)] = nk;
 }
 
-// Exclusive rank of each thread's flag among the CTA's set flags in thread order, and their total.
-template <int kThreads>
-__device__ __forceinline__ int rd_block_rank(bool flag, int* s_warp, int* total) {
-    const int lane = threadIdx.x & (kWarp - 1), warp = threadIdx.x / kWarp;
-    const unsigned mk = __ballot_sync(0xffffffffu, flag);
-    if (lane == 0) s_warp[warp] = __popc(mk);
-    __syncthreads();
-    int before = 0, t = 0;
-#pragma unroll
-    for (int w = 0; w < kThreads / kWarp; ++w) {
-        before += w < warp ? s_warp[w] : 0;
-        t += s_warp[w];
-    }
-    __syncthreads();
-    *total = t;
-    return before + __popc(mk & ((1u << lane) - 1u));
-}
-
 // The driver's rectangle (:974-980): r.x = x1 * cols (float times int, then the int conversion), r.width = x2 * cols - r.x
 // in float, likewise y and height, then RoiCorrect (:22-35) statement by statement.  Conversions as x86-64 performs them
 // (trunc_to_int_x86), and `r.x + r.width` wraps as there.
@@ -271,7 +253,7 @@ __global__ void __launch_bounds__(kRdRowsThreads) refinedet_rows_kernel(const __
         if (!rows) continue;  // uniform
         const bool keep = r < n && !(score < a.score_thresh);  // the driver's `if (score < TH) continue`
         int t;
-        const int rank = rd_block_rank<kRdRowsThreads>(keep, s_warp, &t);
+        const int rank = block_rank<kRdRowsThreads>(keep, s_warp, &t);
         if (keep) {
             int rc[4];
             rd_rect(box, cols, frows, rc);

@@ -110,6 +110,24 @@ __device__ __forceinline__ void block_bitonic_sort_u64(unsigned long long* keys,
     }
 }
 
+// Exclusive rank of each thread's flag among the CTA's set flags in thread order, and their total.
+template <int kThreads>
+__device__ __forceinline__ int block_rank(bool flag, int* s_warp, int* total) {
+    const int lane = threadIdx.x & (kWarp - 1), warp = threadIdx.x / kWarp;
+    const unsigned mk = __ballot_sync(0xffffffffu, flag);
+    if (lane == 0) s_warp[warp] = __popc(mk);
+    __syncthreads();
+    int before = 0, t = 0;
+#pragma unroll
+    for (int w = 0; w < kThreads / kWarp; ++w) {
+        before += w < warp ? s_warp[w] : 0;
+        t += s_warp[w];
+    }
+    __syncthreads();
+    *total = t;
+    return before + __popc(mk & ((1u << lane) - 1u));
+}
+
 // key for "descending score, ascending index" under an ASCENDING 64-bit sort
 __device__ __forceinline__ unsigned long long desc_key(float score, uint32_t idx) {
     return ((unsigned long long)(~float_key(score)) << 32) | idx;

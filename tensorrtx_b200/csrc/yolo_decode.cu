@@ -923,6 +923,7 @@ TRTX_API size_t trtx_abi_sizeof(int which) {
         case 13: return sizeof(trtx_ufld_post_params);
         case 14: return sizeof(trtx_refinedet_params);
         case 15: return sizeof(trtx_yolo_topk_params);
+        case 16: return sizeof(trtx_pyrunner_params);
         default: return 0;
     }
 }

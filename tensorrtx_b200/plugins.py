@@ -1902,3 +1902,87 @@ def letterbox_matrix(src_w: int, src_h: int, dst_w: int, dst_h: int):
     m = (C.c_float * 6)()
     L.load().trtx_letterbox_matrix(src_w, src_h, dst_w, dst_h, m)
     return list(m)
+
+
+# The Python runners (the *_trt.py scripts).  Row format of each detection runner's post_process: (box format its xywh2xyxy
+# reads, floats per plugin row, the float non_max_suppression compares as the label -- boxes[:, -1] after the runner's
+# reshape or slice --, the column yolov3 multiplies into the confidence or -1).  The label is the row's last float, not its
+# class: float 89 of a 90-float row is the OBB angle a detection plugin never writes, so those runners' NMS is class-blind
+# wherever that float is equal; yolov9 compares float 37, a mask coefficient.
+PYRUNNER_PRESETS = {
+    "yolov8_det_trt": (L.BOX_LTRB, 90, 89, -1),
+    "yolov8_5u_det_trt": (L.BOX_LTRB, 90, 89, -1),
+    "yolo11_det_trt": (L.BOX_LTRB, 90, 89, -1),
+    "yolov12_det_trt": (L.BOX_LTRB, 90, 89, -1),  # yolov12-tubro
+    "yolov9_trt": (L.BOX_LTRB, 38, 37, -1),
+    "yolov10_det_trt": (L.BOX_LTRB, 6, 5, -1),
+    "yolov13_det_trt": (L.BOX_LTRB, 6, 5, -1),
+    "yolov7_trt": (L.BOX_CXCYWH, 6, 5, -1),
+    "yolov5_det_trt": (L.BOX_CXCYWH, 38, 5, -1),  # `pred[:, :6]`
+    "yolov5_det_cuda_python": (L.BOX_CXCYWH, 6, 5, -1),
+    "yolov3_trt": (L.BOX_CXCYWH, 7, 5, 6),  # `pred[:, 4] *= pred[:, 6]`, then `pred[:, :-1]`
+}
+
+
+def pyrunner_letterbox_rect(w: int, h: int, net_w: int = 640, net_h: int = 640) -> tuple[int, int, int, int]:
+    """preprocess_image's rectangle (x, y, w, h) of a w x h frame in a net_w x net_h input (ratios in double)."""
+    r = (C.c_int * 4)()
+    L.check(L.load().trtx_pyrunner_letterbox_rect(int(w), int(h), int(net_w), int(net_h), r), "trtx_pyrunner_letterbox_rect")
+    return tuple(r)
+
+
+class PyRunnerPreprocessPlan:
+    """GPU drop-in for the Python runners' preprocess_image (yolov8/yolov8_det_trt.py:207-253; the same body in every
+    yolov5, yolov7, yolov8, yolo11, yolov9, yolov10, yolov12-tubro and yolov13 runner, seg / pose / obb included) for a batch
+    of persistent device frames: images[i] is a u8 HWC BGR cuda tensor [h, w, 3] with packed pixels (rows may be pitched,
+    sizes may differ) -> out [B, 3, net_h, net_w] float32 planes R, G, B, the frame resized by cv2.resize(INTER_LINEAR) into
+    pyrunner_letterbox_rect's rectangle on a 128 canvas, / 255.0, bit for bit.  The descriptors are built once; enqueue() is
+    one C call, one launch per 64 frames, no synchronisation."""
+
+    def __init__(self, images: Sequence[torch.Tensor], out: torch.Tensor | None = None, net_w: int = 640, net_h: int = 640):
+        self._lib = L.load()
+        self.n = len(images)
+        self.descs = _image_descs(images)
+        self._keep = list(images)
+        self.net_w, self.net_h = int(net_w), int(net_h)
+        self.out = _out_tensor(out, (self.n, 3, self.net_h, self.net_w), torch.float32,
+                               images[0].device if self.n else "cuda",
+                               f"out must be float32 [{self.n}, 3, {self.net_h}, {self.net_w}]", contiguous=False)
+
+    def enqueue(self, stream=None) -> torch.Tensor:
+        L.check(self._lib.trtx_linear_preprocess_enqueue(L.LINEAR_PY, self.descs, self.n, self.net_w, self.net_h, 0,
+                                                         _ptr(self.out), _stream(stream)), "trtx_linear_preprocess_enqueue")
+        return self.out
+
+
+class PyRunnerPostprocess:
+    """GPU drop-in for a detection runner's post_process (non_max_suppression, bbox_iou, xywh2xyxy; yolov8_det_trt.py:255-381)
+    for a batch of frames of any sizes.  runner: a key of PYRUNNER_PRESETS; max_rows: the plugin's max output rows (1000).
+    __call__(dets, image_sizes): dets [B, 1 + max_rows*row_floats] float32, the plugin output; image_sizes[b] = (img_w,
+    img_h) -> rows [B, 1 + max_rows*6] float32: the kept count, then (x1, y1, x2, y2, conf, class) per kept row at the frame's
+    size, in the runner's order, zero past the count.  Bit for bit with the runner's numpy where its argsort has no ties;
+    equal confidences keep ascending row order, and a front row that does not suppress itself (a NaN label or box, an
+    inverted box: the runner never returns there) is kept once.  One launch per 64 frames, no workspace."""
+
+    def __init__(self, runner: str, *, max_rows: int = 1000, net_w: int = 640, net_h: int = 640, conf_thresh: float = 0.5,
+                 nms_thresh: float = 0.4):
+        if runner not in PYRUNNER_PRESETS:
+            raise ValueError(f"runner must be one of {sorted(PYRUNNER_PRESETS)}")
+        box, self.row_floats, label_col, conf_col = PYRUNNER_PRESETS[runner]
+        self.max_rows = int(max_rows)
+        self.params = L.PyrunnerParams(box, int(net_w), int(net_h), self.row_floats, label_col, conf_col, conf_thresh,
+                                       nms_thresh)
+
+    def __call__(self, dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]], rows_out: torch.Tensor | None = None,
+                 stream=None) -> torch.Tensor:
+        lib = L.load()
+        B = len(image_sizes)
+        if dets.dim() != 2 or dets.shape[0] != B or dets.shape[1] < 1 + self.max_rows * self.row_floats:
+            raise ValueError(f"dets must be [{B}, >= {1 + self.max_rows * self.row_floats}]")
+        _f32_rows(dets)
+        rows_out = _out_tensor(rows_out, (B, 1 + self.max_rows * 6), torch.float32, dets.device,
+                               f"rows_out must be contiguous float32 [{B}, {1 + self.max_rows * 6}]")
+        L.check(lib.trtx_pyrunner_postprocess_enqueue(C.byref(self.params), _frame_wh(image_sizes), B, _ptr(dets),
+                                                      self.max_rows, _ptr(rows_out), _stream(stream)),
+                "trtx_pyrunner_postprocess_enqueue")
+        return rows_out
