@@ -383,6 +383,22 @@ typedef struct trtx_image_desc {
  * dst_dev that is not aligned to its element size (4 bytes for TRTX_F32, 2 for TRTX_F16). */
 TRTX_API int trtx_preprocess_batch_enqueue(const trtx_image_desc* images_host, int batch, void* dst_dev, int dst_w,
                                            int dst_h, int out_dtype, trtx_stream_t stream);
+/* The band pre-processes: trtx_rcnn_, trtx_cls_, trtx_yolop_, trtx_detr_, trtx_ufld_, trtx_refinedet_, trtx_cubic_ and
+ * trtx_linear_preprocess_enqueue.  Each resizes a batch of frames into the rectangle its model's driver gives each frame on
+ * the engine input, by OpenCV 4.x's own 8-bit INTER_LINEAR (INTER_CUBIC for trtx_cubic_preprocess_enqueue), bit for bit,
+ * and stores every byte as its model's value.  They share one contract:
+ *   images_host: `batch` u8 HWC BGR descriptors in HOST memory (copied into launch parameters; any pitch and base alignment,
+ *     mixed sizes allowed); dst_dev: the engine input, fp32.
+ *   Everything is checked before the first launch, so a rejected call writes nothing, in two passes:
+ *     1. TRTX_ERR_INVALID for a null pointer, batch / net sizes <= 0, pitch < 3 * width, an unknown variant or a dst_dev that
+ *        is not 4-byte aligned;
+ *     2. per frame, what the entry's rectangle rejects (TRTX_ERR_UNSUPPORTED where the reference's cv::resize throws, e.g. an
+ *        empty rectangle for a 1 x 5000 frame); then TRTX_ERR_UNSUPPORTED where the staged source rows of a launch's widest
+ *        rectangle exceed the kernel's shared memory: rectangles up to 4 840 pixels wide for trtx_rcnn_preprocess_enqueue,
+ *        4 757 for the other bilinear entries and, for trtx_cubic_preprocess_enqueue, 1 189 at any scale, 2 378 when enlarging.
+ *     So a call that both passes reject is TRTX_ERR_INVALID, whichever frame comes first.
+ *   One launch per <= 64 frames, no workspace; can be captured in a CUDA graph. */
+
 /* The reference's d2s matrix (preprocess.cu:98-110): scale, centre, cv::invertAffineTransform. */
 TRTX_API void trtx_letterbox_matrix(int src_w, int src_h, int dst_w, int dst_h, float d2s[6]);
 /* get_rect (yolov8/src/postprocess.cpp:6-36, yolov5/src/postprocess.cpp:4-29): maps a detection box from network-input
@@ -639,14 +655,10 @@ TRTX_API int trtx_retina_postprocess_enqueue(const trtx_face_post_params* p, con
  * model input (INPUT_W / INPUT_H of calculateSize, rcnn/rcnn.cpp:349-366).  Host function. */
 TRTX_API int trtx_rcnn_letterbox_pads(int img_w, int img_h, int net_w, int net_h, int pads[4]);
 
-/* preprocessImg (rcnn/common.hpp:79-110) + the float widening of rcnn.cpp:504-505 for a whole batch, one launch per
- * <= 64 images: images_host = `batch` u8 HWC BGR descriptors (trtx_image_desc, any pitch, mixed sizes allowed);
+/* preprocessImg (rcnn/common.hpp:79-110) + the float widening of rcnn.cpp:504-505, a band pre-process (section 5):
  * dst_dev = [batch, net_h, net_w, 3] fp32 BGR, 0..255, 128 outside the resized rectangle: the engine input of
- * rcnn.cpp:259, ready for enqueue.  Image b is resized (OpenCV 4.x's 8-bit INTER_LINEAR, bit for bit) into the rectangle
- * between the pads of trtx_rcnn_letterbox_pads, of size (net_w - left - right) x (net_h - top - bottom).  Every descriptor is
- * checked before the first launch: TRTX_ERR_INVALID for a null pointer, batch / net sizes <= 0, pitch < 3 * width or a
- * dst_dev that is not 4-byte aligned; TRTX_ERR_UNSUPPORTED for an image whose rectangle is empty (cv::resize throws there)
- * or wider than 4 842 pixels (the kernel's shared-memory rows).  No workspace. */
+ * rcnn.cpp:259, ready for enqueue.  Image b is resized into the rectangle between the pads of trtx_rcnn_letterbox_pads, of
+ * size (net_w - left - right) x (net_h - top - bottom). */
 TRTX_API int trtx_rcnn_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h,
                                           float* dst_dev, trtx_stream_t stream);
 
@@ -731,18 +743,13 @@ TRTX_API int trtx_rcnn_contours_enqueue(const trtx_rcnn_post_params* p, const tr
  *    yolo26/yolo26_cls.cpp; yolov5/yolov5_cls.cpp:19-36) and the H2D copy of its fp32 batch, and the HOST softmax + topk
  *    (yolov8_cls.cpp:48-78, yolov5_cls.cpp:38-68, yolo26_cls.cpp:120-135) that run after a D2H copy of every logit.
  * ===================================================================================== */
-/* batch_preprocess for a whole batch, one launch per <= 64 images: images_host = `batch` u8 HWC BGR descriptors in HOST memory
- * (trtx_image_desc, any pitch and base alignment, mixed sizes allowed); dst_dev = [batch, 3, net_h, net_w] fp32 planar RGB,
- * the engine input.  The resize is OpenCV 4.x's 8-bit INTER_LINEAR, bit for bit.
+/* batch_preprocess, a band pre-process (section 5): dst_dev = [batch, 3, net_h, net_w] fp32 planar RGB, the engine input.
  *   variant TRTX_YOLO_V8 (yolov8, yolo11, yolo26): the centre square crop Rect((w - m) / 2, (h - m) / 2, m, m), m = min(w, h),
  *     resized to net_w x net_h, then (float)u * (float)(1 / 255.0) per byte (convertTo(CV_32F, 1 / 255.0));
  *   variant TRTX_YOLO_V5: preprocess_img's letterbox (the rectangle of trtx_calib_letterbox_rect on a 128-grey canvas), then
  *     (float)(((float)u / 255.0 - mean) / std) in double with mean = 0.485, 0.456, 0.406 and std = 0.229, 0.224, 0.225 for
  *     R, G, B.
- * Every descriptor is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
- * batch / net sizes <= 0, pitch < 3 * width, an unknown variant or a dst_dev that is not 4-byte aligned; TRTX_ERR_UNSUPPORTED
- * for a V5 rectangle that is empty (cv::resize throws there, e.g. 1 x 5000) or wider than 4 757 pixels (the kernel's
- * shared-memory rows; V8 rectangles are net_w wide).  No workspace; can be captured in a CUDA graph. */
+ * A V8 rectangle is the whole net_w x net_h; a V5 one can be empty. */
 TRTX_API int trtx_cls_preprocess_enqueue(int variant, const trtx_image_desc* images_host, int batch, int net_w, int net_h,
                                          float* dst_dev, trtx_stream_t stream);
 
@@ -768,16 +775,12 @@ TRTX_API int trtx_cls_postprocess_enqueue(int softmax, int batch, int num_classe
  *    The detection head itself is YoloLayer_TRT with 6-float rows (TRTX_YOLO_V5, det_floats 6); its NMS is
  *    trtx_nms_enqueue with TRTX_BOX_CXCYWH, greedy.
  * ===================================================================================== */
-/* preprocess_img + the plane loop for a whole batch, one launch per <= 64 images: images_host = `batch` u8 HWC BGR descriptors
- * in HOST memory (trtx_image_desc, any pitch and base alignment, mixed sizes allowed); dst_dev = [batch, 3, net_h, net_w] fp32
- * planes in the driver's B, G, R order (Yolo::INPUT_W x INPUT_H = 640 x 384), the engine input.  The resize is OpenCV 4.x's
- * 8-bit INTER_LINEAR into the rectangle of trtx_calib_letterbox_rect on a 114-grey canvas, bit for bit; byte u of plane c
- * (mean = 0.485, 0.456, 0.406 and std = 0.229, 0.224, 0.225 for planes 0, 1, 2) becomes
+/* preprocess_img + the plane loop, a band pre-process (section 5): dst_dev = [batch, 3, net_h, net_w] fp32 planes in the
+ * driver's B, G, R order (Yolo::INPUT_W x INPUT_H = 640 x 384), the engine input.  The frame is resized into the rectangle of
+ * trtx_calib_letterbox_rect on a 114-grey canvas; byte u of plane c (mean = 0.485, 0.456, 0.406 and std = 0.229, 0.224, 0.225
+ * for planes 0, 1, 2) becomes
  *     s = (float)u * (1.f / 255.f) - (float)mean_c  (float),   (float)((double)s / std_c),
- * cv2 4.13's convertTo / subtract / divide chain.  Every descriptor is checked before the first launch (a rejected call writes
- * nothing): TRTX_ERR_INVALID for a null pointer, batch / net sizes <= 0, pitch < 3 * width or a dst_dev that is not 4-byte
- * aligned; TRTX_ERR_UNSUPPORTED for a rectangle that is empty (cv::resize throws there) or wider than 4 757 pixels.  No
- * workspace; can be captured in a CUDA graph. */
+ * cv2 4.13's convertTo / subtract / divide chain. */
 TRTX_API int trtx_yolop_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
                                            trtx_stream_t stream);
 
@@ -822,17 +825,12 @@ TRTX_API int trtx_yolop_postprocess_enqueue(const trtx_yolop_post_params* p, con
  *    preprocessImg), and the HOST stage after inference: the D2H copy of the engine's scores and boxes (:643-648) and the
  *    per-query loop of detr/detr.cpp:777-806 (argmax, score threshold, no-object class, cv::Rect in the frame).
  * ===================================================================================== */
-/* preprocessImg + the plane loop for a whole batch, one launch per <= 64 images: images_host = `batch` u8 HWC BGR descriptors
- * in HOST memory (trtx_image_desc, any pitch and base alignment, mixed sizes allowed); dst_dev = [batch, 3, net_h, net_w] fp32
- * planes in R, G, B order (cvtColor BGR2RGB, then the driver's planes 0, 1, 2; INPUT_W x INPUT_H = 1066 x 800), the engine
- * input.  The whole frame is stretched over the whole net (no letterbox) by OpenCV 4.x's 8-bit INTER_LINEAR, bit for bit
- * (an exact 2x downscale, where OpenCV takes INTER_AREA, gives the same bytes); byte u of plane c (mean = 0.485, 0.456,
- * 0.406 and std = 0.229, 0.224, 0.225 for planes 0, 1, 2) becomes
+/* preprocessImg + the plane loop, a band pre-process (section 5): dst_dev = [batch, 3, net_h, net_w] fp32 planes in R, G, B
+ * order (cvtColor BGR2RGB, then the driver's planes 0, 1, 2; INPUT_W x INPUT_H = 1066 x 800), the engine input.  The whole
+ * frame is stretched over the whole net (no letterbox; an exact 2x downscale, where OpenCV takes INTER_AREA, gives the same
+ * bytes); byte u of plane c (mean = 0.485, 0.456, 0.406 and std = 0.229, 0.224, 0.225 for planes 0, 1, 2) becomes
  *     s = (float)u * (1.f / 255.f) - (float)mean_c  (float),   (float)((double)s / std_c),
- * the driver's convertTo / `/= 255` / `-= Scalar` / `/= Scalar` chain.  Every descriptor is checked before the first launch
- * (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer, batch / net sizes <= 0, pitch < 3 * width or a
- * dst_dev that is not 4-byte aligned; TRTX_ERR_UNSUPPORTED for a net wider than 4 757 pixels (the band's staged source rows
- * in shared memory).  No workspace; can be captured in a CUDA graph. */
+ * the driver's convertTo / `/= 255` / `-= Scalar` / `/= Scalar` chain.  Every rectangle is net_w wide. */
 TRTX_API int trtx_detr_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
                                           trtx_stream_t stream);
 
@@ -931,18 +929,13 @@ TRTX_API int trtx_centernet_decode_enqueue(const trtx_centernet_params* p, int b
  *    and the H2D copy of its input, and after inference the D2H copy of `prob` and the driver's loops (:358-410: the row flip,
  *    argmax and softmax_mul of :223-270, the "no lane" zeroing, the lane choice and the points).  Drawing stays with the caller.
  * ===================================================================================== */
-/* prepareImage for a whole batch, one launch per <= 64 images: images_host = `batch` u8 HWC BGR descriptors in HOST memory
- * (trtx_image_desc, any pitch and base alignment, mixed sizes allowed); dst_dev = [batch, 3, net_h, net_w] fp32 planes in R, G,
- * B order (cvtColor BGR2RGB, then cv::split; INPUT_W x INPUT_H = 800 x 288), the engine input.  The whole frame is stretched
- * over the whole net by OpenCV 4.x's 8-bit INTER_LINEAR, bit for bit (an exact 2x downscale, where OpenCV takes INTER_AREA,
- * gives the same bytes); byte u of plane c (the driver's `static float` mean = 0.485f, 0.456f, 0.406f and std = 0.229f,
- * 0.224f, 0.225f for planes 0, 1, 2) becomes
+/* prepareImage, a band pre-process (section 5): dst_dev = [batch, 3, net_h, net_w] fp32 planes in R, G, B order (cvtColor
+ * BGR2RGB, then cv::split; INPUT_W x INPUT_H = 800 x 288), the engine input.  The whole frame is stretched over the whole net
+ * (an exact 2x downscale, where OpenCV takes INTER_AREA, gives the same bytes); byte u of plane c (the driver's
+ * `static float` mean = 0.485f, 0.456f, 0.406f and std = 0.229f, 0.224f, 0.225f for planes 0, 1, 2) becomes
  *     s = (float)u * (float)(1. / 255.),   fmaf(s, (float)(1. / std_c), (float)(-mean_c / std_c))  (quotients in double),
  * the one convertTo that OpenCV 4.x makes of `(channel - mean[c]) / std[c]`, with the fused multiply-add of its AVX2 kernel.
- * The caller's frame is not converted in place, as the driver's cvtColor(img, img) does.  Every descriptor is checked before
- * the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer, batch / net sizes <= 0, pitch <
- * 3 * width or a dst_dev that is not 4-byte aligned; TRTX_ERR_UNSUPPORTED for a net wider than 4 757 pixels (the band's staged
- * source rows in shared memory).  No workspace; can be captured in a CUDA graph. */
+ * The caller's frame is not converted in place, as the driver's cvtColor(img, img) does.  Every rectangle is net_w wide. */
 TRTX_API int trtx_ufld_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
                                           trtx_stream_t stream);
 
@@ -991,23 +984,18 @@ enum {
     TRTX_CUBIC_ANTICOV = 1,     /* data = ((float)u - 127.5) * 0.0078125 (double), stored to float: exact */
 };
 
-/* preprocess_img + the plane loop for a whole batch, one launch per <= 64 images: images_host = `batch` u8 HWC BGR descriptors
- * in HOST memory (trtx_image_desc, any pitch and base alignment, mixed sizes allowed); dst_dev = [batch, 3, net_h, net_w] fp32
- * planes in R, G, B order (INPUT_W x INPUT_H = 608 x 608 for yolov3-tiny, 640 x 640 for retinafaceAntiCov), the engine input.
- * The frame is resized into the rectangle of trtx_calib_letterbox_rect on a 128-grey canvas by OpenCV 4.x's own 8-bit
- * INTER_CUBIC (the build without IPP, which every non-x86 build runs), bit for bit:
+/* preprocess_img + the plane loop, a band pre-process (section 5): dst_dev = [batch, 3, net_h, net_w] fp32 planes in R, G, B
+ * order (INPUT_W x INPUT_H = 608 x 608 for yolov3-tiny, 640 x 640 for retinafaceAntiCov), the engine input.  The frame is
+ * resized into the rectangle of trtx_calib_letterbox_rect on a 128-grey canvas by OpenCV 4.x's own 8-bit INTER_CUBIC (the
+ * build without IPP, which every non-x86 build runs):
  *   taps      fx = (float)((d + 0.5) * scale - 0.5), scale = 1. / ((double)dsize / ssize), s = floor(fx), fx -= s; taps
  *             s - 1 .. s + 2 clamped into the frame; weights saturate_cast<short>(interpolateCubic(fx) * 2048), A = -0.75;
  *   passes    horizontal: h = sum of the 4 products in int; vertical, for byte i of the 3 * w bytes of a resized row:
  *             i < (3 * w) & ~7: h0 * b0' + (h1 * b1' + (h2 * b2' + h3 * b3')) in float, b' = b / 2048^2, rounded half to even;
  *             otherwise (sum h_k * b_k + 2^21) >> 22; saturated to 0..255.
  * OpenCV with IPP (the default of x86 wheels) differs from this by 1 in a few % of the bytes of a non-integer-ratio resize.
- * Byte u then becomes the variant's value.  Every descriptor is checked before the first launch (a rejected call writes
- * nothing): TRTX_ERR_INVALID for a null pointer, batch / net sizes <= 0, pitch < 3 * width, an unknown variant or a dst_dev
- * that is not 4-byte aligned; TRTX_ERR_UNSUPPORTED for a rectangle that is empty (cv::resize throws there, e.g. 1 x 5000) or
- * whose staged source rows exceed the kernel's shared memory (4 bytes per byte of the rectangle's row times at most 16 rows:
- * rectangles up to 1 189 pixels wide at any scale, 2 378 when enlarging).  No workspace; can be captured in a CUDA
- * graph. */
+ * Byte u then becomes the variant's value.  A launch stages 4 bytes per byte of its widest rectangle's row times at most 16
+ * source rows (8 when enlarging). */
 TRTX_API int trtx_cubic_preprocess_enqueue(int variant, const trtx_image_desc* images_host, int batch, int net_w, int net_h,
                                            float* dst_dev, trtx_stream_t stream);
 
@@ -1017,14 +1005,10 @@ TRTX_API int trtx_cubic_preprocess_enqueue(int variant, const trtx_image_desc* i
  *    post-process of doInference (:730-815: PriorBox, the two decode steps, the ARM filter, the per-class nms() and the rows)
  *    with the driver's rectangles (:957-993 with RoiCorrect, :22-35).  Drawing and the text files stay with the caller.
  * ===================================================================================== */
-/* base_transform for a whole batch, one launch per <= 64 images: images_host = `batch` u8 HWC BGR descriptors in HOST memory
- * (trtx_image_desc, any pitch and base alignment, mixed sizes allowed); dst_dev = [batch, 3, net, net] fp32 planes, the
- * engine input (INPUT_W = INPUT_H = 320; the reference indexes its planes with `i * INPUT_H + j`, right for square nets only,
- * so the call takes one side).  The whole frame is stretched over the net by OpenCV 4.x's 8-bit INTER_LINEAR, bit for bit;
- * plane 0 = R - 123, plane 1 = G - 117, plane 2 = B - 104 (exact in float).  Gray frames are not accepted.  Every descriptor
- * is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer, batch / net <= 0,
- * pitch < 3 * width or a dst_dev that is not 4-byte aligned; TRTX_ERR_UNSUPPORTED for a net above 4 757 (the band's staged
- * source rows in shared memory).  No workspace; can be captured in a CUDA graph. */
+/* base_transform, a band pre-process (section 5): dst_dev = [batch, 3, net, net] fp32 planes, the engine input (INPUT_W =
+ * INPUT_H = 320; the reference indexes its planes with `i * INPUT_H + j`, right for square nets only, so the call takes one
+ * side).  The whole frame is stretched over the net; plane 0 = R - 123, plane 1 = G - 117, plane 2 = B - 104 (exact in
+ * float).  Gray frames are not accepted.  Every rectangle is net wide. */
 TRTX_API int trtx_refinedet_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net, float* dst_dev,
                                                trtx_stream_t stream);
 
@@ -1113,21 +1097,16 @@ enum {
  * empty rectangle (cv::resize throws there, e.g. 1 x 5000).  Host function. */
 TRTX_API int trtx_yolov3spp_letterbox(int img_w, int img_h, int max_size, int out[6]);
 
-/* The pre-process for a whole batch, one launch per <= 64 images: images_host = `batch` u8 HWC BGR descriptors in HOST memory
- * (trtx_image_desc, any pitch and base alignment, mixed sizes allowed); dst_dev = [batch, 3, net_h, net_w] fp32 planes, the
- * engine input.  The frame is resized into its rectangle on a 128-grey canvas by OpenCV 4.x's 8-bit INTER_LINEAR, bit for bit
- * (fx = (float)((d + 0.5) * scale - 0.5), weights saturate_cast<short>((1 - fx) * 2048) and (fx * 2048), horizontal pass in
- * int, vertical pass ((b0 * (S0 >> 4)) >> 16) + ((b1 * (S1 >> 4)) >> 16) + 2) >> 2; cv2 4.13 gives these bytes with IPP on
- * and off); a frame
- * resized to its own size is copied.  The rectangle is trtx_calib_letterbox_rect's for TRTX_LINEAR_YOLOV3 / RETINA
+/* The pre-process, a band pre-process (section 5): dst_dev = [batch, 3, net_h, net_w] fp32 planes, the engine input.  The
+ * frame is resized into its rectangle on a 128-grey canvas (fx = (float)((d + 0.5) * scale - 0.5), weights
+ * saturate_cast<short>((1 - fx) * 2048) and (fx * 2048), horizontal pass in int, vertical pass ((b0 * (S0 >> 4)) >> 16) +
+ * ((b1 * (S1 >> 4)) >> 16) + 2) >> 2; cv2 4.13 gives these bytes with IPP on and off); a frame resized to its own size is
+ * copied.  The rectangle is trtx_calib_letterbox_rect's for TRTX_LINEAR_YOLOV3 / RETINA
  * (INPUT_W x INPUT_H: 608 x 608 for yolov3 / yolov4, 512 x 512 for scaled-yolov4, 640 x 480 for RetinaFace) and
  * trtx_yolov3spp_letterbox's for TRTX_LINEAR_YOLOV3_SPP, trtx_pyrunner_letterbox_rect's for TRTX_LINEAR_PY (any net_w x
  * net_h).  max_size is read by TRTX_LINEAR_YOLOV3_SPP only; its engine binds one input shape per enqueue, so every frame's
- * canvas must be net_w x net_h.
- * Every descriptor is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
- * batch / net sizes <= 0, pitch < 3 * width, an unknown variant, a dst_dev that is not 4-byte aligned, or (SPP) max_size <= 0
- * or a frame whose canvas is not net_w x net_h; TRTX_ERR_UNSUPPORTED for an empty rectangle (cv::resize throws) or one wider
- * than 4 757 pixels (the band's staged source rows in shared memory).  No workspace; can be captured in a CUDA graph. */
+ * canvas must be net_w x net_h: TRTX_ERR_INVALID in the first pass for max_size <= 0 and in the second for a frame whose
+ * canvas is another. */
 TRTX_API int trtx_linear_preprocess_enqueue(int variant, const trtx_image_desc* images_host, int batch, int net_w, int net_h,
                                             int max_size, float* dst_dev, trtx_stream_t stream);
 

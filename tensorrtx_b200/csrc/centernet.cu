@@ -443,10 +443,7 @@ TRTX_API int trtx_centernet_preprocess_enqueue(const trtx_image_desc* images_hos
     if (!images_host || batch <= 0 || !dst_dev || net <= 0) return TRTX_ERR_INVALID;
     if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
     // every descriptor is checked before the first launch, so that a rejected call writes nothing
-    for (int i = 0; i < batch; ++i) {
-        const trtx_image_desc& d = images_host[i];
-        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
-    }
+    if (!valid_images(images_host, batch)) return TRTX_ERR_INVALID;
     if (net > kCnMaxNet) return TRTX_ERR_UNSUPPORTED;
     CnPreArgs a;
     a.net = net;

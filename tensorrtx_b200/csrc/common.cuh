@@ -25,6 +25,15 @@ inline int check_launch() {
     return TRTX_OK;
 }
 
+// The frame descriptors every pre-process accepts: non-null u8 HWC BGR frames of positive size whose rows hold 3 * width bytes.
+inline bool valid_images(const trtx_image_desc* images, int n) {
+    for (int i = 0; i < n; ++i) {
+        const trtx_image_desc& d = images[i];
+        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return false;
+    }
+    return true;
+}
+
 // ---- streaming loads: read-once data bypasses L1 allocation (guide: Guideline 13/14) ----
 __device__ __forceinline__ float4 ldg_stream_f4(const float* p) {
     float4 r;

@@ -411,7 +411,7 @@ static int launch_unit(const trtx_image_desc* const* d, UnitImage* u, int n, voi
 // pass ((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2 saturated to 0..255 (VResizeLinearVec_32s8u).
 //
 // Bound by HBM writes: 4 output bytes per canvas byte (b8 at 1067 x 800: 81.9 MB written, 7.4 MB of u8 read).  A CTA owns a band
-// of kRcnnPreBand full-width destination rows of one image (flat grid over images x bands), which in HWC is ONE contiguous run of
+// of kBandRows full-width destination rows of one image (flat grid over images x bands), which in HWC is ONE contiguous run of
 // band * net_w * 3 floats:
 //   1. y taps: one per destination row of the band inside the rectangle; the distinct clipped source rows they read (at most
 //      2 * band) become the band's slots;
@@ -421,37 +421,45 @@ static int launch_unit(const trtx_image_desc* const* d, UnitImage* u, int n, voi
 //   3. stores: the run is written with 16-byte stores (a head of 0..3 floats up to the first 16-byte boundary and a tail
 //      of 0..3 floats are scalar: rows are 12 * net_w bytes and dst may be only 4-byte aligned); an element outside the
 //      rectangle is 128.0f.  A band wholly in the top / bottom padding skips 1 and 2 and reads nothing.
-constexpr int kRcnnPreBand = 4;            // destination rows per CTA
-constexpr int kRcnnPreSlots = 2 * kRcnnPreBand;  // staged source rows: two taps per destination row at most
-constexpr int kRcnnPreThreads = 256;
-constexpr int kMaxRcnnPreImages = 64;      // descriptors per launch (kernel parameter block)
+constexpr int kBandRows = 4;              // destination rows per CTA
+constexpr int kBandSlots = 2 * kBandRows;  // staged source rows: two taps per destination row at most
+constexpr int kBandThreads = 256;
+constexpr int kMaxBandImages = 64;         // descriptors per launch (kernel parameter block)
 
-struct RcnnPreImage {
+struct BandImage {
     const uint8_t* src;
     double scale_x, scale_y;  // cv::resize: 1. / ((double)dsize / ssize)
     int sw, sh, pitch;
     int x0, y0, rw, rh;       // the resized rectangle on the canvas: (pad_left, pad_top, net - pads)
     int dst_idx;
 };
-struct RcnnPreArgs {
-    RcnnPreImage img[kMaxRcnnPreImages];
+struct BandArgs {
+    BandImage img[kMaxBandImages];
     int net_w, net_h, bands;
-    int stride;               // int16 per staged row: 3 * the widest rectangle of the launch
+    int stride;               // staged elements per row: 3 * the widest rectangle of the launch
 };
 
-// Stages 1 and 2 of a band, shared by the R-CNN and the classification pre-process kernels; Store is stage 3:
-// Store::run(a, im, y0, rows, k_lo, k_hi, pix, dst) writes band rows [0, rows), and pix(k, i), k_lo <= k < k_hi, is the
-// resized byte i (B, G, R interleaved) of the rectangle's row under band row k.
+// The resize of a band pre-process: Resize::run<Store>(a, dst) is stages 1 and 2 of a band, Store::run(a, im, y0, rows, k_lo, k_hi,
+// pix, dst) stage 3, which writes band rows [0, rows), and pix(k, i), k_lo <= k < k_hi, is the resized byte i (B, G, R interleaved)
+// of the rectangle's row under band row k.  On the host, Resize::slots(scale_y) bounds the source rows a band stages and
+// Resize::Staged is the type of a staged element.
+struct LinearBand {
+    using Staged = int16_t;
+    static int slots(double) { return kBandSlots; }
+    template <class Store>
+    static __device__ __forceinline__ void run(const BandArgs& a, float* __restrict__ dst);
+};
+
 template <class Store>
-__device__ __forceinline__ void resize_band(const RcnnPreArgs& a, float* __restrict__ dst) {
-    constexpr int R = kRcnnPreBand;
+__device__ __forceinline__ void LinearBand::run(const BandArgs& a, float* __restrict__ dst) {
+    constexpr int R = kBandRows;
     extern __shared__ __align__(16) int16_t hrows[];  // [slots][a.stride]
-    __shared__ int s_row[kRcnnPreSlots];              // source row of each slot
+    __shared__ int s_row[kBandSlots];                 // source row of each slot
     __shared__ int s_slot[R][2];                      // slots of the two taps of destination row k
     __shared__ int s_coef[R][2];                      // their weights b0, b1
     __shared__ int s_nslots;
     const int item = blockIdx.x / a.bands, band = blockIdx.x - item * a.bands;
-    const RcnnPreImage& im = a.img[item];
+    const BandImage& im = a.img[item];
     const int y0 = band * R, rows = min(R, a.net_h - y0);
     const int k_lo = max(im.y0 - y0, 0), k_hi = min(im.y0 + im.rh - y0, rows);  // band rows inside the rectangle
     const int stride = a.stride;
@@ -539,8 +547,10 @@ __device__ __forceinline__ void store_band_run(float* __restrict__ base, int tot
 
 // R-CNN: HWC, so the band is ONE contiguous run of band * net_w * 3 floats; 128.0f outside the rectangle.
 struct RcnnHwcStore {
+    // the 227 KB opt-in less LinearBand's 128 B of static arrays, which the opt-in also covers: rectangles up to 4 840 pixels wide
+    static constexpr size_t kMaxDynamicSmem = 227 * 1024 - 128;
     template <class Pix>
-    static __device__ __forceinline__ void run(const RcnnPreArgs& a, const RcnnPreImage& im, int y0, int rows, int k_lo, int k_hi,
+    static __device__ __forceinline__ void run(const BandArgs& a, const BandImage& im, int y0, int rows, int k_lo, int k_hi,
                                                Pix pix, float* __restrict__ dst) {
         const int L = 3 * a.net_w;  // floats per canvas row
         float* base = dst + ((size_t)im.dst_idx * a.net_h + y0) * (size_t)L;
@@ -553,22 +563,15 @@ struct RcnnHwcStore {
     }
 };
 
-__global__ void __launch_bounds__(kRcnnPreThreads) rcnn_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
-                                                                          float* __restrict__ dst) {
-    resize_band<RcnnHwcStore>(a, dst);
-}
-
 // ---------------------------------------------------------------------------------------------------------------------
 // YOLO classification pre-process: batch_preprocess of the cls drivers (yolov8/yolov8_cls.cpp:19-46, the same code in yolo11 and
 // yolo26; yolov5/yolov5_cls.cpp:19-36) into the engine's [B, 3, net_h, net_w] fp32 planar RGB input.  The resize is the band
-// kernel's above, over RcnnPreImage descriptors that the host fills per variant:
+// kernel's above, over BandImage descriptors that the host fills per variant:
 //   TRTX_YOLO_V8: the centre square crop Rect((w - m) / 2, (h - m) / 2, m, m), m = min(w, h), as a descriptor offset (cv::resize
 //                 of a ROI reads only the ROI), resized over the whole net_w x net_h;
 //   TRTX_YOLO_V5: preprocess_img's letterbox (trtx_calib_letterbox_rect) on a 128-grey canvas.
 // Only the store stage is new: the band is three contiguous planar runs of band * net_w floats, R, G, B, each written by
 // store_band_run.  The value of byte u in plane c comes from a per-CTA table of 3 x 256 floats (cls_input_value).
-// dynamic shared memory left beside the table and the band's other static arrays: rectangles up to 4 757 pixels wide
-constexpr size_t kClsMaxDynamicSmem = 227 * 1024 - 3 * 256 * sizeof(float) - 1024;
 
 // The engine input value of byte u in plane c (0 = R, 1 = G, 2 = B).
 //   V8: convertTo(CV_32F, 1 / 255.0), i.e. (float)u * (float)(1 / 255.0), one rounded float product;
@@ -632,8 +635,11 @@ struct RefinedetInput {
 // value of a byte comes from a per-CTA table of 3 x 256 floats.
 template <class In>
 struct PlanarStore {
+    // dynamic shared memory left beside the table and the band's other static arrays: bilinear rectangles up to 4 757 pixels
+    // wide, bicubic ones up to 1 189 (2 378 when enlarging)
+    static constexpr size_t kMaxDynamicSmem = 227 * 1024 - 3 * 256 * sizeof(float) - 1024;
     template <class Pix>
-    static __device__ __forceinline__ void run(const RcnnPreArgs& a, const RcnnPreImage& im, int y0, int rows, int k_lo, int k_hi,
+    static __device__ __forceinline__ void run(const BandArgs& a, const BandImage& im, int y0, int rows, int k_lo, int k_hi,
                                                Pix pix, float* __restrict__ dst) {
         __shared__ float lut[3][256];
         for (int j = threadIdx.x; j < 3 * 256; j += blockDim.x) lut[j >> 8][j & 255] = In::value(j >> 8, j & 255);
@@ -652,66 +658,28 @@ struct PlanarStore {
     }
 };
 
-template <int kVariant>
-__global__ void __launch_bounds__(kRcnnPreThreads) cls_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
-                                                                         float* __restrict__ dst) {
-    resize_band<PlanarStore<ClsInput<kVariant>>>(a, dst);
-}
-
-__global__ void __launch_bounds__(kRcnnPreThreads) yolop_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
-                                                                           float* __restrict__ dst) {
-    resize_band<PlanarStore<YolopInput>>(a, dst);
-}
-
-__global__ void __launch_bounds__(kRcnnPreThreads) detr_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
-                                                                          float* __restrict__ dst) {
-    resize_band<PlanarStore<DetrInput>>(a, dst);
-}
-
-__global__ void __launch_bounds__(kRcnnPreThreads) ufld_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
-                                                                          float* __restrict__ dst) {
-    resize_band<PlanarStore<UfldInput>>(a, dst);
-}
-
-__global__ void __launch_bounds__(kRcnnPreThreads) refinedet_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
-                                                                               float* __restrict__ dst) {
-    resize_band<PlanarStore<RefinedetInput>>(a, dst);
-}
-
-// One launch of `kernel` per kMaxRcnnPreImages frames: make(i, im) fills the band descriptor of frame i (validated before).
-template <class Make>
-static int launch_bands(void (*kernel)(RcnnPreArgs, float*), int batch, int net_w, int net_h, float* dst_dev, size_t smem_max,
-                        cudaStream_t st, Make make) {
-    if (smem_max > 48 * 1024 &&
-        cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) != cudaSuccess) {
-        g_last_cuda_error = (int)cudaGetLastError();
-        return TRTX_ERR_CUDA;
-    }
-    RcnnPreArgs a;
-    a.net_w = net_w;
-    a.net_h = net_h;
-    a.bands = (net_h + kRcnnPreBand - 1) / kRcnnPreBand;
-    for (int i0 = 0; i0 < batch; i0 += kMaxRcnnPreImages) {
-        const int n = batch - i0 < kMaxRcnnPreImages ? batch - i0 : kMaxRcnnPreImages;
-        int wmax = 0;
-        for (int j = 0; j < n; ++j) {
-            RcnnPreImage& im = a.img[j];
-            make(i0 + j, im);
-            im.dst_idx = i0 + j;
-            wmax = im.rw > wmax ? im.rw : wmax;
-        }
-        a.stride = 3 * wmax;
-        const size_t smem = (size_t)kRcnnPreSlots * a.stride * sizeof(int16_t);
-        kernel<<<(unsigned)(n * a.bands), kRcnnPreThreads, smem, st>>>(a, dst_dev);
-        const int rc = check_launch();
-        if (rc) return rc;
-    }
+// The band descriptor of frame d for the R-CNN pre-process: the rectangle between trtx_rcnn_letterbox_pads' pads;
+// TRTX_ERR_UNSUPPORTED where the reference's cv::resize or copyTo throws (an empty rectangle, or one that leaves the canvas).
+static int rcnn_band_image(const trtx_image_desc& d, int net_w, int net_h, BandImage& im) {
+    int pads[4];
+    trtx_rcnn_letterbox_pads(d.width, d.height, net_w, net_h, pads);
+    im.src = d.data_dev;
+    im.sw = d.width;
+    im.sh = d.height;
+    im.pitch = d.pitch;
+    im.x0 = pads[0];
+    im.y0 = pads[2];
+    im.rw = net_w - (pads[0] + pads[1]);
+    im.rh = net_h - (pads[2] + pads[3]);
+    if (im.rw <= 0 || im.rh <= 0 || pads[0] < 0 || pads[2] < 0) return TRTX_ERR_UNSUPPORTED;
+    im.scale_x = 1. / ((double)im.rw / d.width);
+    im.scale_y = 1. / ((double)im.rh / d.height);
     return TRTX_OK;
 }
 
-// The band descriptor of frame d for the classification pre-process; false where the reference's cv::resize or copyTo throws
-// (an empty letterbox rectangle, or one that leaves the canvas).
-static bool cls_band_image(int variant, const trtx_image_desc& d, int net_w, int net_h, RcnnPreImage& im) {
+// The band descriptor of frame d for the classification pre-process; TRTX_ERR_UNSUPPORTED where the reference's cv::resize or
+// copyTo throws (an empty letterbox rectangle, or one that leaves the canvas).
+static int cls_band_image(int variant, const trtx_image_desc& d, int net_w, int net_h, BandImage& im) {
     im.src = d.data_dev;
     im.sw = d.width;
     im.sh = d.height;
@@ -727,16 +695,17 @@ static bool cls_band_image(int variant, const trtx_image_desc& d, int net_w, int
         int r[4];
         trtx_calib_letterbox_rect(d.width, d.height, net_w, net_h, r);
         im.x0 = r[0], im.y0 = r[1], im.rw = r[2], im.rh = r[3];
-        if (im.rw <= 0 || im.rh <= 0 || im.x0 < 0 || im.y0 < 0 || im.x0 + im.rw > net_w || im.y0 + im.rh > net_h) return false;
+        if (im.rw <= 0 || im.rh <= 0 || im.x0 < 0 || im.y0 < 0 || im.x0 + im.rw > net_w || im.y0 + im.rh > net_h)
+            return TRTX_ERR_UNSUPPORTED;
     }
     im.scale_x = 1. / ((double)im.rw / im.sw);
     im.scale_y = 1. / ((double)im.rh / im.sh);
-    return true;
+    return TRTX_OK;
 }
 
 // The band descriptor of frame d for a whole frame stretched over the whole net, cv::resize(img, dst, Size(net_w, net_h))
-// (DETR's preprocessImg, UFLD's prepareImage), i.e. cls_band_image's V8 descriptor without the crop.
-static void stretch_band_image(const trtx_image_desc& d, int net_w, int net_h, RcnnPreImage& im) {
+// (DETR's preprocessImg, UFLD's prepareImage, RefineDet's base_transform), i.e. cls_band_image's V8 descriptor without the crop.
+static int stretch_band_image(const trtx_image_desc& d, int net_w, int net_h, BandImage& im) {
     im.src = d.data_dev;
     im.sw = d.width;
     im.sh = d.height;
@@ -746,22 +715,7 @@ static void stretch_band_image(const trtx_image_desc& d, int net_w, int net_h, R
     im.rh = net_h;
     im.scale_x = 1. / ((double)net_w / d.width);
     im.scale_y = 1. / ((double)net_h / d.height);
-}
-
-// The whole-frame pre-processes (DETR, UFLD): one band descriptor per frame (stretch_band_image) into `kernel`'s planar store.
-static int stretch_preprocess(void (*kernel)(RcnnPreArgs, float*), const trtx_image_desc* images_host, int batch, int net_w,
-                              int net_h, float* dst_dev, cudaStream_t st) {
-    if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
-    if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
-    // every descriptor is checked before the first launch, so that a rejected call writes nothing
-    for (int i = 0; i < batch; ++i) {
-        const trtx_image_desc& d = images_host[i];
-        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
-    }
-    const size_t smem = (size_t)kRcnnPreSlots * 3 * (size_t)net_w * sizeof(int16_t);  // every rectangle is net_w wide
-    if (smem > kClsMaxDynamicSmem) return TRTX_ERR_UNSUPPORTED;
-    return launch_bands(kernel, batch, net_w, net_h, dst_dev, smem, st,
-                        [&](int i, RcnnPreImage& im) { stretch_band_image(images_host[i], net_w, net_h, im); });
+    return TRTX_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -776,9 +730,9 @@ static int stretch_preprocess(void (*kernel)(RcnnPreArgs, float*), const trtx_im
 //   vertical:   of the 3 * rw bytes of a destination row, the first (3 * rw) & ~7 are VResizeCubicVec_32s8u's 8-lane float loop:
 //               h0 * b0' + (h1 * b1' + (h2 * b2' + h3 * b3')), b' = b / 2048^2 (exact), every product and sum rounded (no FMA),
 //               then rounded half to even; the rest are the scalar tail's (sum h_k * b_k + 2^21) >> 22; both saturated to 0..255.
-// The band structure is resize_band's with 4 y taps per destination row, the staged rows in int32 and up to 4 slots per row.
+// The band structure is LinearBand's with 4 y taps per destination row, the staged rows in int32 and up to 4 slots per row.
 // The horizontal pass is shared by the band rows that read the same source row; stage 3 is PlanarStore.
-constexpr int kCubicMaxSlots = 4 * kRcnnPreBand;
+constexpr int kCubicMaxSlots = 4 * kBandRows;
 
 // interpolateCubic (imgproc/src/resize.cpp) statement by statement in float, then saturate_cast<short>(c * 2048)
 __device__ __forceinline__ void cv_cubic_coeffs(float x, int (&c)[4]) {
@@ -794,23 +748,26 @@ __device__ __forceinline__ void cv_cubic_coeffs(float x, int (&c)[4]) {
     c[3] = __float2int_rn(__fmul_rn(c3, 2048.f));
 }
 
-// Source rows a band of kRcnnPreBand destination rows can read at y scale `scale`: the low taps of its first and last rows are
-// at most ceil(3 * scale) + 1 apart (the float rounding of fy moves a difference by far less than 1), and each row reads 4 rows
-// from its low tap on.
-static int cubic_band_slots(double scale) {
-    return (int)fmin((double)kCubicMaxSlots, ceil((kRcnnPreBand - 1) * scale) + 5);
-}
+struct CubicBand {
+    using Staged = int;
+    // Source rows a band of kBandRows destination rows can read at y scale `scale`: the low taps of its first and last rows are
+    // at most ceil(3 * scale) + 1 apart (the float rounding of fy moves a difference by far less than 1), and each row reads 4
+    // rows from its low tap on.
+    static int slots(double scale) { return (int)fmin((double)kCubicMaxSlots, ceil((kBandRows - 1) * scale) + 5); }
+    template <class Store>
+    static __device__ __forceinline__ void run(const BandArgs& a, float* __restrict__ dst);
+};
 
 template <class Store>
-__device__ __forceinline__ void cubic_band(const RcnnPreArgs& a, float* __restrict__ dst) {
-    constexpr int R = kRcnnPreBand;
+__device__ __forceinline__ void CubicBand::run(const BandArgs& a, float* __restrict__ dst) {
+    constexpr int R = kBandRows;
     extern __shared__ __align__(16) int hcub[];  // [slots][a.stride]
     __shared__ int s_row[kCubicMaxSlots];
     __shared__ int s_slot[R][4];
     __shared__ int s_coef[R][4];
     __shared__ int s_nslots;
     const int item = blockIdx.x / a.bands, band = blockIdx.x - item * a.bands;
-    const RcnnPreImage& im = a.img[item];
+    const BandImage& im = a.img[item];
     const int y0 = band * R, rows = min(R, a.net_h - y0);
     const int k_lo = max(im.y0 - y0, 0), k_hi = min(im.y0 + im.rh - y0, rows);
     const int stride = a.stride;
@@ -902,20 +859,14 @@ struct CubicInput {
     }
 };
 
-template <int kVariant>
-__global__ void __launch_bounds__(kRcnnPreThreads) cubic_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
-                                                                           float* __restrict__ dst) {
-    cubic_band<PlanarStore<CubicInput<kVariant>>>(a, dst);
-}
-
 // ---------------------------------------------------------------------------------------------------------------------
-// Bilinear letterbox pre-process of yolov3, yolov4, scaled-yolov4, yolov3-spp and RetinaFace: resize_band with a planar store;
+// Bilinear letterbox pre-process of yolov3, yolov4, scaled-yolov4, yolov3-spp and RetinaFace: LinearBand with a planar store;
 // only the value conventions and the host-side rectangles are their own.
 //   TRTX_LINEAR_YOLOV3      the yolov3-tiny chain, u / 255.0 in double (CubicInput<TRTX_CUBIC_YOLOV3_TINY>), planes R, G, B;
 //   TRTX_LINEAR_PY          the same store over the Python runners' rectangle: their float32 u / 255.0f is that float;
 //   TRTX_LINEAR_RETINA      RetinaInput below;
-//   TRTX_LINEAR_YOLOV3_SPP  blobFromImage's (float)u * (float)(1 / 255.0), planes R, G, B: cls_preprocess_kernel<TRTX_YOLO_V8>,
-//                           whose value chain it is, over yolov3-spp's rectangle.
+//   TRTX_LINEAR_YOLOV3_SPP  blobFromImage's (float)u * (float)(1 / 255.0), planes R, G, B: the cls V8 store,
+//                           PlanarStore<ClsInput<TRTX_YOLO_V8>>, whose value chain it is, over yolov3-spp's rectangle.
 // retina_r50.cpp:342-352: plane c (0 = B) takes BGR byte c, `pr_img.at<cv::Vec3b>(i)[c] - mean` in double with means 104, 117,
 // 123, stored to float (exact).
 struct RetinaInput {
@@ -926,15 +877,9 @@ struct RetinaInput {
     }
 };
 
-template <class In>
-__global__ void __launch_bounds__(kRcnnPreThreads) linear_preprocess_kernel(const __grid_constant__ RcnnPreArgs a,
-                                                                            float* __restrict__ dst) {
-    resize_band<PlanarStore<In>>(a, dst);
-}
-
 // The band descriptor of frame d in yolov3-spp's letterbox: TRTX_ERR_UNSUPPORTED where the rectangle is empty (cv::resize
 // throws), TRTX_ERR_INVALID where the canvas is not net_w x net_h (the call binds one input shape).
-static int spp_band_image(const trtx_image_desc& d, int max_size, int net_w, int net_h, RcnnPreImage& im) {
+static int spp_band_image(const trtx_image_desc& d, int max_size, int net_w, int net_h, BandImage& im) {
     int g[6];
     const int rc = trtx_yolov3spp_letterbox(d.width, d.height, max_size, g);
     if (rc) return rc;
@@ -951,7 +896,7 @@ static int spp_band_image(const trtx_image_desc& d, int max_size, int net_w, int
 
 // The band descriptor of frame d in the Python runners' preprocess_image: trtx_pyrunner_letterbox_rect's rectangle, which
 // cv2.resize fills with the frame; TRTX_ERR_UNSUPPORTED where it is empty (cv2.resize raises).
-static int py_band_image(const trtx_image_desc& d, int net_w, int net_h, RcnnPreImage& im) {
+static int py_band_image(const trtx_image_desc& d, int net_w, int net_h, BandImage& im) {
     int r[4];
     trtx_pyrunner_letterbox_rect(d.width, d.height, net_w, net_h, r);
     if (r[2] <= 0 || r[3] <= 0) return TRTX_ERR_UNSUPPORTED;
@@ -962,6 +907,60 @@ static int py_band_image(const trtx_image_desc& d, int net_w, int net_h, RcnnPre
     im.x0 = r[0], im.y0 = r[1], im.rw = r[2], im.rh = r[3];
     im.scale_x = 1. / ((double)im.rw / im.sw);
     im.scale_y = 1. / ((double)im.rh / im.sh);
+    return TRTX_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// The band pre-processes' one kernel and one launch path.  An instantiation's dynamic shared memory holds the staged source
+// rows: Resize::slots rows of 3 * the launch's widest rectangle in Resize::Staged, at most Store::kMaxDynamicSmem bytes.
+template <class Resize, class Store>
+__global__ void __launch_bounds__(kBandThreads) band_preprocess_kernel(const __grid_constant__ BandArgs a, float* __restrict__ dst) {
+    Resize::template run<Store>(a, dst);
+}
+
+// Checks the call in two passes before the first launch, so that a rejected call writes nothing and TRTX_ERR_INVALID wins over
+// TRTX_ERR_UNSUPPORTED: first the arguments and every descriptor (TRTX_ERR_INVALID), then every frame's descriptor from
+// make(i, im) (what make returns) and every launch's shared memory (TRTX_ERR_UNSUPPORTED).  Then one launch per kMaxBandImages
+// frames, a CTA per band of each.
+template <class Resize, class Store, class Make>
+static int band_preprocess(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
+                           trtx_stream_t stream, Make make) {
+    if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
+    if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0 || !valid_images(images_host, batch)) return TRTX_ERR_INVALID;
+    BandArgs a;
+    for (int i = 0; i < batch; ++i)
+        if (const int rc = make(i, a.img[0])) return rc;
+    a.net_w = net_w;
+    a.net_h = net_h;
+    a.bands = (net_h + kBandRows - 1) / kBandRows;
+    // the descriptors of frames [i0, i0 + n), which make accepted above, into a; returns the launch's dynamic shared memory
+    auto fill = [&](int i0, int n) {
+        int wmax = 0, slots = 0;
+        for (int j = 0; j < n; ++j) {
+            BandImage& im = a.img[j];
+            make(i0 + j, im);
+            im.dst_idx = i0 + j;
+            wmax = max(wmax, im.rw);
+            slots = max(slots, Resize::slots(im.scale_y));
+        }
+        a.stride = 3 * wmax;
+        return (size_t)slots * a.stride * sizeof(typename Resize::Staged);
+    };
+    size_t smem_max = 0;
+    for (int i0 = 0; i0 < batch; i0 += kMaxBandImages) smem_max = max(smem_max, fill(i0, min(batch - i0, kMaxBandImages)));
+    if (smem_max > Store::kMaxDynamicSmem) return TRTX_ERR_UNSUPPORTED;
+    auto* kernel = band_preprocess_kernel<Resize, Store>;
+    if (smem_max > 48 * 1024 &&
+        cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) != cudaSuccess) {
+        g_last_cuda_error = (int)cudaGetLastError();
+        return TRTX_ERR_CUDA;
+    }
+    for (int i0 = 0; i0 < batch; i0 += kMaxBandImages) {
+        const int n = min(batch - i0, kMaxBandImages);
+        const size_t smem = fill(i0, n);
+        kernel<<<(unsigned)(n * a.bands), kBandThreads, smem, static_cast<cudaStream_t>(stream)>>>(a, dst_dev);
+        if (const int rc = check_launch()) return rc;
+    }
     return TRTX_OK;
 }
 
@@ -1089,10 +1088,7 @@ TRTX_API int trtx_preprocess_batch_enqueue(const trtx_image_desc* images_host, i
     if (out_dtype != TRTX_F32 && out_dtype != TRTX_F16) return TRTX_ERR_INVALID;
     if (reinterpret_cast<uintptr_t>(dst_dev) % (out_dtype == TRTX_F32 ? sizeof(float) : sizeof(__half)) != 0) return TRTX_ERR_INVALID;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    for (int i = 0; i < batch; ++i) {
-        const trtx_image_desc& d = images_host[i];
-        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
-    }
+    if (!valid_images(images_host, batch)) return TRTX_ERR_INVALID;
     // vector stores of the unit-scale kernel: 4 pixels per thread and plane
     const bool unit_ok = dst_w % 4 == 0 && reinterpret_cast<uintptr_t>(dst_dev) % 16 == 0;
     PreArgs g;  // general-path group
@@ -1154,161 +1150,60 @@ TRTX_API int trtx_preprocess_batch_enqueue(const trtx_image_desc* images_host, i
     return flush_general();
 }
 
+// The band pre-processes: each entry is its rectangle (make) and its kernel instantiation over band_preprocess.
 TRTX_API int trtx_rcnn_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
                                           trtx_stream_t stream) {
-    if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
-    if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
-    // every descriptor is checked before the first launch, so that a rejected call writes nothing
-    size_t smem_max = 0;
-    for (int i = 0; i < batch; ++i) {
-        const trtx_image_desc& d = images_host[i];
-        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
-        int pads[4];
-        trtx_rcnn_letterbox_pads(d.width, d.height, net_w, net_h, pads);
-        const int rw = net_w - (pads[0] + pads[1]), rh = net_h - (pads[2] + pads[3]);
-        if (rw <= 0 || rh <= 0 || pads[0] < 0 || pads[2] < 0) return TRTX_ERR_UNSUPPORTED;  // cv::resize / copyTo would throw
-        const size_t smem = (size_t)kRcnnPreSlots * 3 * (size_t)rw * sizeof(int16_t);
-        if (smem > 227 * 1024) return TRTX_ERR_UNSUPPORTED;
-        smem_max = smem > smem_max ? smem : smem_max;
-    }
-    return launch_bands(rcnn_preprocess_kernel, batch, net_w, net_h, dst_dev, smem_max, static_cast<cudaStream_t>(stream),
-                        [&](int i, RcnnPreImage& im) {
-                            const trtx_image_desc& d = images_host[i];
-                            int pads[4];
-                            trtx_rcnn_letterbox_pads(d.width, d.height, net_w, net_h, pads);
-                            im.src = d.data_dev;
-                            im.sw = d.width;
-                            im.sh = d.height;
-                            im.pitch = d.pitch;
-                            im.x0 = pads[0];
-                            im.y0 = pads[2];
-                            im.rw = net_w - (pads[0] + pads[1]);
-                            im.rh = net_h - (pads[2] + pads[3]);
-                            im.scale_x = 1. / ((double)im.rw / d.width);
-                            im.scale_y = 1. / ((double)im.rh / d.height);
-                        });
+    auto make = [&](int i, BandImage& im) { return rcnn_band_image(images_host[i], net_w, net_h, im); };
+    return band_preprocess<LinearBand, RcnnHwcStore>(images_host, batch, net_w, net_h, dst_dev, stream, make);
 }
 
 TRTX_API int trtx_cls_preprocess_enqueue(int variant, const trtx_image_desc* images_host, int batch, int net_w, int net_h,
                                          float* dst_dev, trtx_stream_t stream) {
-    if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
     if (variant != TRTX_YOLO_V8 && variant != TRTX_YOLO_V5) return TRTX_ERR_INVALID;
-    if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
-    // every descriptor is checked before the first launch, so that a rejected call writes nothing
-    size_t smem_max = 0;
-    for (int i = 0; i < batch; ++i) {
-        const trtx_image_desc& d = images_host[i];
-        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
-        RcnnPreImage im;
-        if (!cls_band_image(variant, d, net_w, net_h, im)) return TRTX_ERR_UNSUPPORTED;
-        const size_t smem = (size_t)kRcnnPreSlots * 3 * (size_t)im.rw * sizeof(int16_t);
-        if (smem > kClsMaxDynamicSmem) return TRTX_ERR_UNSUPPORTED;
-        smem_max = smem > smem_max ? smem : smem_max;
-    }
-    auto* kernel = variant == TRTX_YOLO_V8 ? cls_preprocess_kernel<TRTX_YOLO_V8> : cls_preprocess_kernel<TRTX_YOLO_V5>;
-    return launch_bands(kernel, batch, net_w, net_h, dst_dev, smem_max, static_cast<cudaStream_t>(stream),
-                        [&](int i, RcnnPreImage& im) { cls_band_image(variant, images_host[i], net_w, net_h, im); });
+    auto make = [&](int i, BandImage& im) { return cls_band_image(variant, images_host[i], net_w, net_h, im); };
+    if (variant == TRTX_YOLO_V8)
+        return band_preprocess<LinearBand, PlanarStore<ClsInput<TRTX_YOLO_V8>>>(images_host, batch, net_w, net_h, dst_dev, stream, make);
+    return band_preprocess<LinearBand, PlanarStore<ClsInput<TRTX_YOLO_V5>>>(images_host, batch, net_w, net_h, dst_dev, stream, make);
 }
 
 // YOLOP's preprocess_img letterbox is yolov5-cls's (the same statements, yolop/utils.h:13-25), so its band descriptor is
 // cls_band_image's V5 one; only the store differs (canvas 114, BGR planes, its own value chain).
 TRTX_API int trtx_yolop_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
                                            trtx_stream_t stream) {
-    if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
-    if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
-    // every descriptor is checked before the first launch, so that a rejected call writes nothing
-    size_t smem_max = 0;
-    for (int i = 0; i < batch; ++i) {
-        const trtx_image_desc& d = images_host[i];
-        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
-        RcnnPreImage im;
-        if (!cls_band_image(TRTX_YOLO_V5, d, net_w, net_h, im)) return TRTX_ERR_UNSUPPORTED;
-        const size_t smem = (size_t)kRcnnPreSlots * 3 * (size_t)im.rw * sizeof(int16_t);
-        if (smem > kClsMaxDynamicSmem) return TRTX_ERR_UNSUPPORTED;
-        smem_max = smem > smem_max ? smem : smem_max;
-    }
-    return launch_bands(yolop_preprocess_kernel, batch, net_w, net_h, dst_dev, smem_max, static_cast<cudaStream_t>(stream),
-                        [&](int i, RcnnPreImage& im) { cls_band_image(TRTX_YOLO_V5, images_host[i], net_w, net_h, im); });
+    auto make = [&](int i, BandImage& im) { return cls_band_image(TRTX_YOLO_V5, images_host[i], net_w, net_h, im); };
+    return band_preprocess<LinearBand, PlanarStore<YolopInput>>(images_host, batch, net_w, net_h, dst_dev, stream, make);
 }
 
-// DETR's preprocessImg stretches the whole frame over the whole net: the planar store with DETR's R, G, B planes and value
-// chain.
+// DETR's preprocessImg, UFLD's prepareImage and RefineDet's base_transform stretch the whole frame over the whole net
+// (stretch_band_image); each has its own planes and value chain.
 TRTX_API int trtx_detr_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
                                           trtx_stream_t stream) {
-    return stretch_preprocess(detr_preprocess_kernel, images_host, batch, net_w, net_h, dst_dev,
-                              static_cast<cudaStream_t>(stream));
+    auto make = [&](int i, BandImage& im) { return stretch_band_image(images_host[i], net_w, net_h, im); };
+    return band_preprocess<LinearBand, PlanarStore<DetrInput>>(images_host, batch, net_w, net_h, dst_dev, stream, make);
 }
 
-// UFLD's prepareImage, likewise, with UFLD's fused value chain.
 TRTX_API int trtx_ufld_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
                                           trtx_stream_t stream) {
-    return stretch_preprocess(ufld_preprocess_kernel, images_host, batch, net_w, net_h, dst_dev,
-                              static_cast<cudaStream_t>(stream));
+    auto make = [&](int i, BandImage& im) { return stretch_band_image(images_host[i], net_w, net_h, im); };
+    return band_preprocess<LinearBand, PlanarStore<UfldInput>>(images_host, batch, net_w, net_h, dst_dev, stream, make);
 }
 
-// RefineDet's base_transform, likewise, on a square net with its mean-subtracted planes.
 TRTX_API int trtx_refinedet_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net, float* dst_dev,
                                                trtx_stream_t stream) {
-    return stretch_preprocess(refinedet_preprocess_kernel, images_host, batch, net, net, dst_dev,
-                              static_cast<cudaStream_t>(stream));
+    auto make = [&](int i, BandImage& im) { return stretch_band_image(images_host[i], net, net, im); };
+    return band_preprocess<LinearBand, PlanarStore<RefinedetInput>>(images_host, batch, net, net, dst_dev, stream, make);
 }
 
 // preprocess_img with INTER_CUBIC (yolov3-tiny, retinafaceAntiCov): cls_band_image's V5 rectangle, the bicubic band kernel.
-// A launch's dynamic shared memory is its widest rectangle times its most slots, so every launch is sized (and checked against
-// the budget) before the first one.
 TRTX_API int trtx_cubic_preprocess_enqueue(int variant, const trtx_image_desc* images_host, int batch, int net_w, int net_h,
                                            float* dst_dev, trtx_stream_t stream) {
-    if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
     if (variant != TRTX_CUBIC_YOLOV3_TINY && variant != TRTX_CUBIC_ANTICOV) return TRTX_ERR_INVALID;
-    if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
-    // every descriptor is checked before the first launch, so that a rejected call writes nothing
-    for (int i = 0; i < batch; ++i) {
-        const trtx_image_desc& d = images_host[i];
-        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
-    }
-    size_t smem_max = 0;
-    for (int i0 = 0; i0 < batch; i0 += kMaxRcnnPreImages) {
-        int wmax = 0, slots = 0;
-        for (int i = i0; i < batch && i < i0 + kMaxRcnnPreImages; ++i) {
-            RcnnPreImage im;
-            if (!cls_band_image(TRTX_YOLO_V5, images_host[i], net_w, net_h, im)) return TRTX_ERR_UNSUPPORTED;
-            wmax = im.rw > wmax ? im.rw : wmax;
-            const int s = cubic_band_slots(im.scale_y);
-            slots = s > slots ? s : slots;
-        }
-        const size_t smem = (size_t)slots * 3 * (size_t)wmax * sizeof(int);
-        if (smem > kClsMaxDynamicSmem) return TRTX_ERR_UNSUPPORTED;
-        smem_max = smem > smem_max ? smem : smem_max;
-    }
-    auto* kernel = variant == TRTX_CUBIC_YOLOV3_TINY ? cubic_preprocess_kernel<TRTX_CUBIC_YOLOV3_TINY>
-                                                     : cubic_preprocess_kernel<TRTX_CUBIC_ANTICOV>;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (smem_max > 48 * 1024 &&
-        cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) != cudaSuccess) {
-        g_last_cuda_error = (int)cudaGetLastError();
-        return TRTX_ERR_CUDA;
-    }
-    RcnnPreArgs a;
-    a.net_w = net_w;
-    a.net_h = net_h;
-    a.bands = (net_h + kRcnnPreBand - 1) / kRcnnPreBand;
-    for (int i0 = 0; i0 < batch; i0 += kMaxRcnnPreImages) {
-        const int n = batch - i0 < kMaxRcnnPreImages ? batch - i0 : kMaxRcnnPreImages;
-        int wmax = 0, slots = 0;
-        for (int j = 0; j < n; ++j) {
-            RcnnPreImage& im = a.img[j];
-            cls_band_image(TRTX_YOLO_V5, images_host[i0 + j], net_w, net_h, im);
-            im.dst_idx = i0 + j;
-            wmax = im.rw > wmax ? im.rw : wmax;
-            const int s = cubic_band_slots(im.scale_y);
-            slots = s > slots ? s : slots;
-        }
-        a.stride = 3 * wmax;
-        kernel<<<(unsigned)(n * a.bands), kRcnnPreThreads, (size_t)slots * a.stride * sizeof(int), st>>>(a, dst_dev);
-        const int rc = check_launch();
-        if (rc) return rc;
-    }
-    return TRTX_OK;
+    auto make = [&](int i, BandImage& im) { return cls_band_image(TRTX_YOLO_V5, images_host[i], net_w, net_h, im); };
+    if (variant == TRTX_CUBIC_YOLOV3_TINY)
+        return band_preprocess<CubicBand, PlanarStore<CubicInput<TRTX_CUBIC_YOLOV3_TINY>>>(images_host, batch, net_w, net_h,
+                                                                                           dst_dev, stream, make);
+    return band_preprocess<CubicBand, PlanarStore<CubicInput<TRTX_CUBIC_ANTICOV>>>(images_host, batch, net_w, net_h, dst_dev,
+                                                                                   stream, make);
 }
 
 TRTX_API int trtx_yolov3spp_letterbox(int img_w, int img_h, int max_size, int out[6]) {
@@ -1328,37 +1223,22 @@ TRTX_API int trtx_yolov3spp_letterbox(int img_w, int img_h, int max_size, int ou
 // variant's planar store.
 TRTX_API int trtx_linear_preprocess_enqueue(int variant, const trtx_image_desc* images_host, int batch, int net_w, int net_h,
                                             int max_size, float* dst_dev, trtx_stream_t stream) {
-    if (!images_host || batch <= 0 || !dst_dev || net_w <= 0 || net_h <= 0) return TRTX_ERR_INVALID;
     if (variant != TRTX_LINEAR_YOLOV3 && variant != TRTX_LINEAR_RETINA && variant != TRTX_LINEAR_YOLOV3_SPP &&
         variant != TRTX_LINEAR_PY)
         return TRTX_ERR_INVALID;
     if (variant == TRTX_LINEAR_YOLOV3_SPP && max_size <= 0) return TRTX_ERR_INVALID;
-    if (reinterpret_cast<uintptr_t>(dst_dev) % sizeof(float) != 0) return TRTX_ERR_INVALID;
-    auto make = [&](int i, RcnnPreImage& im) -> int {
+    auto make = [&](int i, BandImage& im) {
         if (variant == TRTX_LINEAR_YOLOV3_SPP) return spp_band_image(images_host[i], max_size, net_w, net_h, im);
         if (variant == TRTX_LINEAR_PY) return py_band_image(images_host[i], net_w, net_h, im);
-        return cls_band_image(TRTX_YOLO_V5, images_host[i], net_w, net_h, im) ? TRTX_OK : TRTX_ERR_UNSUPPORTED;
+        return cls_band_image(TRTX_YOLO_V5, images_host[i], net_w, net_h, im);
     };
-    // every descriptor is checked before the first launch, so that a rejected call writes nothing
-    for (int i = 0; i < batch; ++i) {
-        const trtx_image_desc& d = images_host[i];
-        if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return TRTX_ERR_INVALID;
-    }
-    size_t smem_max = 0;
-    for (int i = 0; i < batch; ++i) {
-        RcnnPreImage im;
-        const int rc = make(i, im);
-        if (rc) return rc;
-        const size_t smem = (size_t)kRcnnPreSlots * 3 * (size_t)im.rw * sizeof(int16_t);
-        if (smem > kClsMaxDynamicSmem) return TRTX_ERR_UNSUPPORTED;
-        smem_max = smem > smem_max ? smem : smem_max;
-    }
-    auto* kernel = variant == TRTX_LINEAR_YOLOV3 || variant == TRTX_LINEAR_PY
-                       ? linear_preprocess_kernel<CubicInput<TRTX_CUBIC_YOLOV3_TINY>>
-                   : variant == TRTX_LINEAR_RETINA ? linear_preprocess_kernel<RetinaInput>
-                                                   : cls_preprocess_kernel<TRTX_YOLO_V8>;
-    return launch_bands(kernel, batch, net_w, net_h, dst_dev, smem_max, static_cast<cudaStream_t>(stream),
-                        [&](int i, RcnnPreImage& im) { make(i, im); });
+    if (variant == TRTX_LINEAR_RETINA)
+        return band_preprocess<LinearBand, PlanarStore<RetinaInput>>(images_host, batch, net_w, net_h, dst_dev, stream, make);
+    if (variant == TRTX_LINEAR_YOLOV3_SPP)
+        return band_preprocess<LinearBand, PlanarStore<ClsInput<TRTX_YOLO_V8>>>(images_host, batch, net_w, net_h, dst_dev, stream,
+                                                                                make);
+    return band_preprocess<LinearBand, PlanarStore<CubicInput<TRTX_CUBIC_YOLOV3_TINY>>>(images_host, batch, net_w, net_h, dst_dev,
+                                                                                        stream, make);
 }
 
 }  // extern "C"

@@ -1325,6 +1325,20 @@ def _image_descs(images: Sequence[torch.Tensor]):
     return descs
 
 
+def _frames_preprocess(entry: str, images: Sequence[torch.Tensor], out: torch.Tensor | None, shape: tuple, stream,
+                       lead: tuple = (), trail: tuple = ()) -> torch.Tensor:
+    """The frame pre-processes' one call: `entry`(*lead, descriptors, n, *trail, out, stream) over the device frames `images`
+    into `out`, a float32 tensor [n, *shape] (new when None), which it returns."""
+    lib = L.load()
+    n = len(images)
+    descs = _image_descs(images)
+    shape = (n, *shape)
+    out = _out_tensor(out, shape, torch.float32, images[0].device if n else "cuda",
+                      f"out must be float32 [{', '.join(map(str, shape))}]", contiguous=False)
+    L.check(getattr(lib, entry)(*lead, descs, n, *trail, _ptr(out), _stream(stream)), entry)
+    return out
+
+
 def _letterbox_dst(dst: torch.Tensor, n: int, dst_width: int, dst_height: int) -> int:
     """TRTX_F32 / TRTX_F16 of the letterbox output dst, which must be a float32 or float16 tensor [n, 3, dst_h, dst_w]:
     TrtxError for another dtype, ValueError for another shape, both before the library is called."""
@@ -1420,13 +1434,7 @@ def rcnn_preprocess(images: Sequence[torch.Tensor], net_w: int, net_h: int, out:
     of every byte to float) for a batch of device frames: images[i] is a u8 HWC BGR cuda tensor [h, w, 3] with packed
     pixels (rows may be pitched, sizes may differ) -> [B, net_h, net_w, 3] float32 BGR, 0..255, 128 around the resized
     image: the engine input.  One launch per 64 images, no synchronisation."""
-    lib = L.load()
-    n = len(images)
-    descs = _image_descs(images)
-    out = _out_tensor(out, (n, net_h, net_w, 3), torch.float32, images[0].device if n else "cuda",
-                      f"out must be float32 [{n}, {net_h}, {net_w}, 3]", contiguous=False)
-    L.check(lib.trtx_rcnn_preprocess_enqueue(descs, n, net_w, net_h, _ptr(out), _stream(stream)), "trtx_rcnn_preprocess_enqueue")
-    return out
+    return _frames_preprocess("trtx_rcnn_preprocess_enqueue", images, out, (net_h, net_w, 3), stream, trail=(net_w, net_h))
 
 
 def cls_preprocess(images: Sequence[torch.Tensor], variant: int, net_w: int, net_h: int, out: torch.Tensor | None = None,
@@ -1435,14 +1443,8 @@ def cls_preprocess(images: Sequence[torch.Tensor], variant: int, net_w: int, net
     tensor [h, w, 3] with packed pixels (rows may be pitched, sizes may differ) -> [B, 3, net_h, net_w] float32 planar RGB, the
     engine input.  variant _lib.YOLO_V8 (yolov8, yolo11, yolo26): centre square crop, resize, / 255; _lib.YOLO_V5 (yolov5): the
     letterbox on a 128-grey canvas, ImageNet mean / std.  One launch per 64 images, no synchronisation."""
-    lib = L.load()
-    n = len(images)
-    descs = _image_descs(images)
-    out = _out_tensor(out, (n, 3, net_h, net_w), torch.float32, images[0].device if n else "cuda",
-                      f"out must be float32 [{n}, 3, {net_h}, {net_w}]", contiguous=False)
-    L.check(lib.trtx_cls_preprocess_enqueue(variant, descs, n, net_w, net_h, _ptr(out), _stream(stream)),
-            "trtx_cls_preprocess_enqueue")
-    return out
+    return _frames_preprocess("trtx_cls_preprocess_enqueue", images, out, (3, net_h, net_w), stream, lead=(variant,),
+                              trail=(net_w, net_h))
 
 
 YOLOP_NET = (640, 384)  # Yolo::INPUT_W, INPUT_H (yolop/yololayer.h)
@@ -1455,13 +1457,7 @@ def yolop_preprocess(images: Sequence[torch.Tensor], out: torch.Tensor | None = 
     for a batch of device frames: images[i] is a u8 HWC BGR cuda tensor [h, w, 3] with packed pixels (rows may be pitched,
     sizes may differ) -> [B, 3, net_h, net_w] float32 planes in B, G, R order, the engine input: the letterbox on a 114-grey
     canvas, / 255, minus the ImageNet mean, over its std.  One launch per 64 images, no synchronisation."""
-    lib = L.load()
-    n = len(images)
-    descs = _image_descs(images)
-    out = _out_tensor(out, (n, 3, net_h, net_w), torch.float32, images[0].device if n else "cuda",
-                      f"out must be float32 [{n}, 3, {net_h}, {net_w}]", contiguous=False)
-    L.check(lib.trtx_yolop_preprocess_enqueue(descs, n, net_w, net_h, _ptr(out), _stream(stream)), "trtx_yolop_preprocess_enqueue")
-    return out
+    return _frames_preprocess("trtx_yolop_preprocess_enqueue", images, out, (3, net_h, net_w), stream, trail=(net_w, net_h))
 
 
 def yolop_get_rect(img_w: int, img_h: int, bbox, net_w: int = YOLOP_NET[0], net_h: int = YOLOP_NET[1]):
@@ -1521,13 +1517,7 @@ def detr_preprocess(images: Sequence[torch.Tensor], out: torch.Tensor | None = N
     batch of device frames: images[i] is a u8 HWC BGR cuda tensor [h, w, 3] with packed pixels (rows may be pitched, sizes
     may differ) -> [B, 3, net_h, net_w] float32 planes in R, G, B order, the engine input: the whole frame resized to the
     whole net, / 255, minus the ImageNet mean, over its std.  One launch per 64 images, no synchronisation."""
-    lib = L.load()
-    n = len(images)
-    descs = _image_descs(images)
-    out = _out_tensor(out, (n, 3, net_h, net_w), torch.float32, images[0].device if n else "cuda",
-                      f"out must be float32 [{n}, 3, {net_h}, {net_w}]", contiguous=False)
-    L.check(lib.trtx_detr_preprocess_enqueue(descs, n, net_w, net_h, _ptr(out), _stream(stream)), "trtx_detr_preprocess_enqueue")
-    return out
+    return _frames_preprocess("trtx_detr_preprocess_enqueue", images, out, (3, net_h, net_w), stream, trail=(net_w, net_h))
 
 
 def detr_get_rect(img_w: int, img_h: int, box):
@@ -1570,14 +1560,7 @@ def centernet_preprocess(images: Sequence[torch.Tensor], out: torch.Tensor | Non
     u8 HWC BGR cuda tensor [h, w, 3] with packed pixels (rows may be pitched, sizes may differ) -> [B, 3, net, net] float32
     planes in B, G, R order, the engine input: the frame at the top-left of an L x L zero canvas (L = max(h, w, 3)), resized
     on float64 as cv.resize does, then ((v / 255.) - 0.5) / 0.5.  One launch per 64 images, no synchronisation."""
-    lib = L.load()
-    n = len(images)
-    descs = _image_descs(images)
-    out = _out_tensor(out, (n, 3, net, net), torch.float32, images[0].device if n else "cuda",
-                      f"out must be float32 [{n}, 3, {net}, {net}]", contiguous=False)
-    L.check(lib.trtx_centernet_preprocess_enqueue(descs, n, net, _ptr(out), _stream(stream)),
-            "trtx_centernet_preprocess_enqueue")
-    return out
+    return _frames_preprocess("trtx_centernet_preprocess_enqueue", images, out, (3, net, net), stream, trail=(net,))
 
 
 def centernet_decode(heat: torch.Tensor, wh: torch.Tensor, reg: torch.Tensor, k: int = 100, *,
@@ -1635,13 +1618,7 @@ def ufld_preprocess(images: Sequence[torch.Tensor], out: torch.Tensor | None = N
     R, G, B order, the engine input: the whole frame resized to the whole net, then fmaf(u * (1 / 255.), 1 / std, -mean / std)
     as OpenCV folds the driver's `(c - mean) / std`.  The frames are not written.  One launch per 64 images, no
     synchronisation."""
-    lib = L.load()
-    n = len(images)
-    descs = _image_descs(images)
-    out = _out_tensor(out, (n, 3, net_h, net_w), torch.float32, images[0].device if n else "cuda",
-                      f"out must be float32 [{n}, 3, {net_h}, {net_w}]", contiguous=False)
-    L.check(lib.trtx_ufld_preprocess_enqueue(descs, n, net_w, net_h, _ptr(out), _stream(stream)), "trtx_ufld_preprocess_enqueue")
-    return out
+    return _frames_preprocess("trtx_ufld_preprocess_enqueue", images, out, (3, net_h, net_w), stream, trail=(net_w, net_h))
 
 
 def ufld_postprocess(prob: torch.Tensor, image_sizes: Sequence[tuple[int, int]] | None = None, *,
@@ -1686,14 +1663,7 @@ def refinedet_preprocess(images: Sequence[torch.Tensor], out: torch.Tensor | Non
     is a u8 HWC BGR cuda tensor [h, w, 3] with packed pixels (rows may be pitched, sizes may differ) -> [B, 3, net, net]
     float32 planes R - 123, G - 117, B - 104 of the whole frame resized to net x net, the engine input.  One launch per 64
     images, no synchronisation."""
-    lib = L.load()
-    n = len(images)
-    descs = _image_descs(images)
-    out = _out_tensor(out, (n, 3, net, net), torch.float32, images[0].device if n else "cuda",
-                      f"out must be float32 [{n}, 3, {net}, {net}]", contiguous=False)
-    L.check(lib.trtx_refinedet_preprocess_enqueue(descs, n, net, _ptr(out), _stream(stream)),
-            "trtx_refinedet_preprocess_enqueue")
-    return out
+    return _frames_preprocess("trtx_refinedet_preprocess_enqueue", images, out, (3, net, net), stream, trail=(net,))
 
 
 def refinedet_postprocess(arm_loc: torch.Tensor, arm_conf: torch.Tensor, odm_loc: torch.Tensor, odm_conf: torch.Tensor,
@@ -1755,14 +1725,8 @@ def cubic_preprocess(images: Sequence[torch.Tensor], variant: int, out: torch.Te
     pitched, sizes may differ) -> [B, 3, net_h, net_w] float32 planes in R, G, B order, the engine input: the letterbox on a
     128-grey canvas, resized as OpenCV's own 8-bit INTER_CUBIC (without IPP) does, bit for bit.  One launch per 64 images,
     no synchronisation."""
-    lib = L.load()
-    n = len(images)
-    descs = _image_descs(images)
-    out = _out_tensor(out, (n, 3, net_h, net_w), torch.float32, images[0].device if n else "cuda",
-                      f"out must be float32 [{n}, 3, {net_h}, {net_w}]", contiguous=False)
-    L.check(lib.trtx_cubic_preprocess_enqueue(variant, descs, n, net_w, net_h, _ptr(out), _stream(stream)),
-            "trtx_cubic_preprocess_enqueue")
-    return out
+    return _frames_preprocess("trtx_cubic_preprocess_enqueue", images, out, (3, net_h, net_w), stream, lead=(variant,),
+                              trail=(net_w, net_h))
 
 
 def yolov3spp_letterbox(w: int, h: int, max_size: int = 608) -> tuple[tuple[int, int], tuple[int, int, int, int]]:
@@ -1784,14 +1748,8 @@ def linear_preprocess(images: Sequence[torch.Tensor], variant: int, out: torch.T
     images[i] is a u8 HWC BGR cuda tensor [h, w, 3] with packed pixels (rows may be pitched, sizes may differ) ->
     [B, 3, net_h, net_w] float32 planes, the engine input: the frame resized as OpenCV's 8-bit INTER_LINEAR does, bit for
     bit, on a 128-grey canvas.  One launch per 64 images, no synchronisation."""
-    lib = L.load()
-    n = len(images)
-    descs = _image_descs(images)
-    out = _out_tensor(out, (n, 3, net_h, net_w), torch.float32, images[0].device if n else "cuda",
-                      f"out must be float32 [{n}, 3, {net_h}, {net_w}]", contiguous=False)
-    L.check(lib.trtx_linear_preprocess_enqueue(variant, descs, n, net_w, net_h, max_size, _ptr(out), _stream(stream)),
-            "trtx_linear_preprocess_enqueue")
-    return out
+    return _frames_preprocess("trtx_linear_preprocess_enqueue", images, out, (3, net_h, net_w), stream, lead=(variant,),
+                              trail=(net_w, net_h, max_size))
 
 
 def cls_postprocess(logits: torch.Tensor, k: int, softmax: bool, probs: bool = False, stream=None):

@@ -79,6 +79,13 @@ def test_rcnn_preprocess_dst_offset_by_4_bytes(dev):
     assert buf[0].item() == SENTINEL
 
 
+def test_rcnn_preprocess_widest_rectangle(dev):
+    """4 840 pixels, the widest rectangle the call accepts: its staged rows and the band's static arrays fill the 227 KB of
+    shared memory a CTA may opt in to."""
+    host, devs = _frames(np.random.default_rng(11), [(4840, 8)], dev)
+    _check(host, devs, 4840, 8, dev)
+
+
 def test_rcnn_preprocess_rejected_call_writes_nothing(dev):
     rng = np.random.default_rng(10)
     _, devs = _frames(rng, [(640, 480), (1, 5000)], dev)
