@@ -4,6 +4,9 @@
 # and the REFERENCE's own YoloLayer plugin of each yolov3-family driver, compiled where it lies, each with
 # oracle/ref_wrap_v3_family.cu:
 #   _ref/libref_v3f_yolov3.so  _ref/libref_v3f_yolov4.so  _ref/libref_v3f_csp.so  _ref/libref_v3f_tiny.so
+# and the same with oracle/ref_wrap_v3_family_blob.cu too (the plugin built from a blob, on any grids and class count), in
+# libraries of their own so that a test never meets a build of the first set that predates the blob entry:
+#   _ref/libref_v3f_blob_<driver>.so
 # and, on the host with oracle/ref_wrap_v3_family_host.cpp, the blob each one's yololayer.h constants make:
 #   _ref/libref_v3f_<driver>_host.so
 # and each driver's own nms() (its .cpp compiled where it lies with its main renamed, oracle/ref_wrap_v3_nms_host.cpp; the
@@ -22,7 +25,7 @@ $(HERE)libv3family_oracle.so: $(HERE)v3family_oracle.c
 V3F_REF := yolov3 yolov4 csp tiny
 ifneq ($(wildcard $(REF)),)
 v3family: $(foreach v,$(V3F_REF),$(HERE)_ref/libref_v3f_$(v).so $(HERE)_ref/libref_v3f_$(v)_host.so \
-                                 $(HERE)_ref/libref_v3f_nms_$(v).so)
+                                 $(HERE)_ref/libref_v3f_nms_$(v).so $(HERE)_ref/libref_v3f_blob_$(v).so)
 endif
 .PHONY: v3family
 
@@ -35,6 +38,15 @@ $(HERE)_ref/libref_v3f_yolov4.so: $(HERE)ref_wrap_v3_family.cu $(REF)/yolov4/yol
 $(HERE)_ref/libref_v3f_csp.so: $(HERE)ref_wrap_v3_family.cu $(REF)/scaled-yolov4/yololayer.cu
 	$(V3F_BUILD) -I$(REF)/scaled-yolov4 -o $@ $^
 $(HERE)_ref/libref_v3f_tiny.so: $(HERE)ref_wrap_v3_family.cu $(REF)/yolov3-tiny/yololayer.cu
+	$(V3F_BUILD) -I$(REF)/yolov3-tiny -o $@ $^
+V3F_BLOB := $(HERE)ref_wrap_v3_family.cu $(HERE)ref_wrap_v3_family_blob.cu
+$(HERE)_ref/libref_v3f_blob_yolov3.so: $(V3F_BLOB) $(REF)/yolov3/yololayer.cu
+	$(V3F_BUILD) -I$(REF)/yolov3 -o $@ $^
+$(HERE)_ref/libref_v3f_blob_yolov4.so: $(V3F_BLOB) $(REF)/yolov4/yololayer.cu
+	$(V3F_BUILD) -I$(REF)/yolov4 -o $@ $^
+$(HERE)_ref/libref_v3f_blob_csp.so: $(V3F_BLOB) $(REF)/scaled-yolov4/yololayer.cu
+	$(V3F_BUILD) -I$(REF)/scaled-yolov4 -o $@ $^
+$(HERE)_ref/libref_v3f_blob_tiny.so: $(V3F_BLOB) $(REF)/yolov3-tiny/yololayer.cu
 	$(V3F_BUILD) -I$(REF)/yolov3-tiny -o $@ $^
 
 $(HERE)_ref/libref_v3f_%_host.so: SHIM := $(HERE)shim_v3

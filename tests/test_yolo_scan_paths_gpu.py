@@ -14,6 +14,15 @@ candidate count, so a test fails if the library took another route than the one 
 | v8 seg / pose / obb (pack kernel's extras) | 13 of 13 pairs | 13 of 13 pairs | 13 of 13 pairs | 13 of 13 pairs | 13 of 13 pairs |
 | v5 / v5-seg / v7 (`yolo_v5_scan_kernel`) | yes | yes (+4 B; 648 net) | n/a | yes | yes |
 | v3 (same kernel, `TRTX_YOLO_V3`) | yes (640 net) | yes (+4 B; 608 net) | n/a | yes (640 net) | yes |
+| v3net: yolov3, yolov3-tiny (same kernel, `TRTX_YOLO_V3_NET`) | yes (20/40/80, 28x16, 20x12 two levels) | yes (+4 B; 19/38/76, 19x11) | n/a | yes | yes |
+| v4: yolov4 (same kernel, `TRTX_YOLO_V4`, double Logist) | yes (20/40/80, 28x16, two levels) | yes (+4 B; 19/38/76, 19x11) | n/a | yes | yes |
+| csp: scaled-yolov4 (same kernel, `TRTX_YOLO_V4_CSP`, double Logist) | yes (20/40/80, 28x16, two levels) | yes (+4 B; 19/38/76, 19x11) | n/a | yes | yes |
+
+The yolov3 family runs on grid sets of its own (V3F_GRIDS: square and non-square, an odd cell count, two levels) at each
+driver's compiled-in net (608 x 608; 512 x 512 for scaled-yolov4), and once at a 608 x 352 net against the oracle alone.
+Its driver's own CalDetection kernel takes the same grids, anchors and class count from the plugin's serialized blob
+(ref_v3f_plugin_enqueue_blob of oracle/_ref/libref_v3f_blob_<driver>.so), so every family case is also held to that
+kernel bit for bit: count, box, both confidences and class, NaNs at the same places.
 
 On these routes:
   * route matrix: all routes give byte-identical plugin buffers, fp16 heads exactly the fp32 call on the widened heads,
@@ -27,7 +36,8 @@ On these routes:
     every variant, against the oracle (NaNs at the same places) and the reference's kernels (bit for bit where the
     reference build contracts no differently);
   * the gate window (+-64 ulps around logf(0.1f / 0.9f), x_lo and one ulp either side) and near-ulp sigmoid collisions,
-    where only the reference's kernels (same CUDA expf) can arbitrate;
+    where only the reference's kernels (same CUDA expf) can arbitrate; for the family also pairs on which its float and
+    double Logist disagree about a collision, the case where finish_best replays the class loop with the double form;
   * class-slice edges: nc smaller than the slice count, ties and saturated collisions on both sides of every slice
     boundary, for every pair.
 Reference outputs come through RefOutputs("ref_gpu"): tests/golden/ref_gpu.npz where oracle/_ref was not built."""
@@ -37,10 +47,13 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import v3family
 from oracle.golden import RefOutputs
 from tensorrtx_b200 import _lib as L
 from tensorrtx_b200 import plugins as P
 from tensorrtx_b200 import synth
+
+from test_yolov3_family_cpu import LIBNAME, _sig
 
 pytestmark = pytest.mark.gpu
 G = RefOutputs("ref_gpu")
@@ -49,8 +62,21 @@ RTOL_EXP = 2e-6   # anchor-based boxes pass through expf / a sigmoid scaled to p
 KT = 0.3          # keypoint threshold of the pose runs
 PAIRS = ((1, 8), (1, 16), (2, 4), (2, 5), (2, 8), (2, 10), (2, 20), (4, 4), (4, 5), (4, 10), (4, 20), (8, 5), (8, 10))
 V8 = {"v8": (80, 0), "seg": (80, 32), "pose": (1, 51), "obb": (15, 1)}   # mode -> (classes, extra channels)
-DET = {"v8": 90, "seg": 90, "pose": 90, "obb": 90, "v5": 38, "v5seg": 38, "v7": 6, "v3": 7}
+# the yolov3 family: mode -> its driver in plugins.V3_FAMILY_DRIVERS (v3net's two-level grid sets: yolov3-tiny)
+V3F = {"v3net": "yolov3", "v4": "yolov4", "csp": "scaled-yolov4"}
+DET = {"v8": 90, "seg": 90, "pose": 90, "obb": 90, "v5": 38, "v5seg": 38, "v7": 6, "v3": 7, **{v: 7 for v in V3F}}
 V3_ANCHORS = [k.anchors for k in P.YOLOV3_KERNELS]
+# the family's grid sets: (gw, gh) per level in the plugin's level order (stride 32 first, as synth.yolov3_heads lays them
+# out), and a net other than the driver's compiled-in INPUT_W x INPUT_H (None: the driver's)
+V3F_GRIDS = {
+    "square": (((20, 20), (40, 40), (80, 80)), None),       # every cell count % 4 == 0: VEC 4 where the view allows it
+    "odd": (((19, 19), (38, 38), (76, 76)), None),          # 361 cells: VEC 1 on every route
+    "rect": (((28, 16), (56, 32), (112, 64)), None),        # non-square: gw != gh and net_w / gw != net_h / gh
+    "rect_odd": (((19, 11), (38, 22), (76, 44)), None),     # non-square, 209 cells: VEC 1
+    "two": (((20, 12), (40, 24)), None),                    # two levels, non-square (v3net: yolov3-tiny's plugin)
+    "net608x352": (((20, 20), (40, 40), (80, 80)), (608, 352)),   # a net no driver compiles in: the oracle alone
+}
+FOUR = {(torch.float32, 4), (torch.float32, 1), (torch.float16, 4), (torch.float16, 1)}
 # route -> (dtype, byte offset of every level's view into its allocation)
 ROUTES = {"f32": (torch.float32, 0), "f32+4": (torch.float32, 4), "f16": (torch.float16, 0), "f16+8": (torch.float16, 8),
           "f16+2": (torch.float16, 2)}
@@ -101,8 +127,28 @@ def _assert_route(ws, B, grids, vec, count, max_out):
     assert np.array_equal(np.minimum(total, max_out), np.asarray(count)), (f"tile counts of a VEC {vec} tiling", total, count)
 
 
-def _plugin(var, dtype, net=640, nc=None, max_out=1000):
+def _v3f_driver(var, gset):
+    return "yolov3-tiny" if var == "v3net" and len(V3F_GRIDS[gset][0]) == 2 else V3F[var]
+
+
+def _v3f_net(var, gset):
+    return V3F_GRIDS[gset][1] or P.V3_FAMILY_DRIVERS[_v3f_driver(var, gset)]["net"]
+
+
+def _v3f_kernels(var, gset):
+    """The grid set's levels with the driver's anchors, stride 32 first."""
+    d = P.V3_FAMILY_DRIVERS[_v3f_driver(var, gset)]
+    anchors = [a for _, _, a in sorted(d["kernels"], key=lambda k: k[0])]
+    return [P.YoloKernel(gw, gh, a) for (gw, gh), a in zip(V3F_GRIDS[gset][0], anchors)]
+
+
+def _plugin(var, dtype, net=640, nc=None, max_out=1000, gset="rect"):
+    """The variant's plugin; the yolov3 family's takes its grids from `gset` (V3F_GRIDS) instead of `net`."""
     f16 = L.F16 if dtype == torch.float16 else L.F32
+    if var in V3F:
+        (w, h), variant = _v3f_net(var, gset), P.V3_FAMILY_DRIVERS[V3F[var]]["variant"]
+        return P.YoloLayerPluginV3Net(80 if nc is None else nc, _v3f_kernels(var, gset), w, h, variant, maxOut=max_out,
+                                      in_dtype=f16)
     if var in V8:
         nc = V8[var][0] if nc is None else nc
         return P.YoloLayerPlugin(nc, 17, KT, net, net, max_out, var == "seg", var == "pose", var == "obb", (8, 16, 32),
@@ -129,9 +175,14 @@ def _decode(plug, hd, B, dev, vec, grids):
     return got
 
 
-def _heads16(var, B, seed, net=640, nc=None, n_obj=64):
+def _heads16(var, B, seed, net=640, nc=None, n_obj=64, gset="rect"):
     """Synthetic heads of `var`, rounded to fp16 (every route reads the same values)."""
-    if var in V8:
+    if var in V3F:
+        grids = V3F_GRIDS[gset][0]
+        hs = synth.yolov3_heads(B, seed=seed, nc=80 if nc is None else nc, net_w=32 * grids[0][0], net_h=32 * grids[0][1],
+                                strides=(32, 16, 8)[:len(grids)], n_obj=n_obj)
+        assert [h.shape[2:] for h in hs] == [(gh, gw) for gw, gh in grids]
+    elif var in V8:
         c, extra = V8[var]
         hs = synth.yolov8_heads(B, seed=seed, nc=c if nc is None else nc, extra=extra, net_w=net, net_h=net, n_obj=n_obj)
     elif var == "v3":
@@ -141,7 +192,10 @@ def _heads16(var, B, seed, net=640, nc=None, n_obj=64):
     return [h.astype(np.float16) for h in hs]
 
 
-def _oracle(oracle, var, wide, net=640, nc=None, max_out=1000):
+def _oracle(oracle, var, wide, net=640, nc=None, max_out=1000, gset="rect"):
+    if var in V3F:
+        return v3family.decode(wide, [k.anchors for k in _v3f_kernels(var, gset)], P.V3_FAMILY_DRIVERS[V3F[var]]["variant"],
+                               net=_v3f_net(var, gset), nc=80 if nc is None else nc, max_out=max_out)
     if var in V8:
         return oracle.yolov8_decode(wide, net_w=net, net_h=net, nc=V8[var][0] if nc is None else nc, max_out=max_out,
                                     kpt_thresh=KT, is_seg=var == "seg", is_pose=var == "pose", is_obb=var == "obb")
@@ -154,7 +208,7 @@ def _oracle(oracle, var, wide, net=640, nc=None, max_out=1000):
 
 def _cols(var):
     return {"seg": list(range(38)), "pose": list(range(6)) + list(range(38, 89)), "obb": list(range(6)) + [89],
-            "v5seg": list(range(38)), "v3": list(range(7))}.get(var, list(range(6)))
+            "v5seg": list(range(38)), "v3": list(range(7)), **{v: list(range(7)) for v in V3F}}.get(var, list(range(6)))
 
 
 def _check_oracle(var, got, ref, max_out=1000):
@@ -187,17 +241,23 @@ def _ptrs(ts):
     return a
 
 
-def _ref_decode(var, wide, dev):
-    """The reference's own plugin kernel on fp32 heads (640x640, the variant's classes, 1000 rows), or None where it was
-    not built."""
-    lib = G.lib(REF_LIB[var])
+def _ref_decode(var, wide, dev, nc=80, gset="rect"):
+    """The reference's own plugin kernel on fp32 heads (640x640, the variant's classes, 1000 rows; the yolov3 family: its
+    driver's kernel built from our plugin's blob, so on gset's grids with nc classes), or None where it was not built."""
+    lib = G.lib(f"libref_v3f_blob_{LIBNAME[_v3f_driver(var, gset)]}.so" if var in V3F else REF_LIB[var])
     if lib is None:
         return None
     B = wide[0].shape[0]
     hd = [torch.from_numpy(np.ascontiguousarray(h)).to(dev) for h in wide]
     out = torch.zeros((B, 1 + 1000 * DET[var]), dtype=torch.float32, device=dev)
     po = C.c_void_p(out.data_ptr())
-    if var in V8:
+    if var in V3F:
+        wh = (C.c_int * 2)()
+        lib.ref_v3f_net(wh)
+        assert V3F_GRIDS[gset][1] is None and tuple(wh) == _v3f_net(var, gset) and lib.ref_v3f_max_out() == 1000
+        blob = _plugin(var, torch.float32, nc=nc, gset=gset).serialize()
+        rc = lib.ref_v3f_plugin_enqueue_blob(blob, C.c_size_t(len(blob)), B, _ptrs(hd), po)
+    elif var in V8:
         rc = lib.ref_v8_plugin_enqueue(_nc(var), 17, C.c_float(KT), 640, 640, 1000, int(var == "seg"), int(var == "pose"),
                                        int(var == "obb"), (C.c_int * 3)(8, 16, 32), 3, B, _ptrs(hd), po, None)
     elif var == "v3":
@@ -220,7 +280,7 @@ def _ref_decode(var, wide, dev):
 
 def _lead(var):
     """Positions, within _cols(var), of the confidence, the class (and v3's class confidence)."""
-    return [4, 5, 6] if var == "v3" else [4, 5]
+    return [4, 5, 6] if var == "v3" or var in V3F else [4, 5]
 
 
 def _canon(buf, b, var):
@@ -237,14 +297,15 @@ def _canon(buf, b, var):
 
 
 def _vs_ref(key, var, got, ref):
-    """Our plugin buffer against the reference kernel's: count exact; v8 rows bit for bit; elsewhere conf / class bit for
-    bit, anchor-based boxes within 3e-7 (the reference build contracts its box arithmetic into FMAs differently), and the
-    rest of a seg / pose / obb row within 1e-6 (fp64 trigonometry and keypoint arithmetic, as
-    tests/test_vs_reference_gpu.py compares them); NaNs at the same places."""
+    """Our plugin buffer against the reference kernel's: count exact; v8 and yolov3-family rows bit for bit (the family's
+    box as tests/test_yolov3_family_gpu.py holds it); elsewhere conf / class bit for bit, anchor-based boxes within 3e-7
+    (the reference build contracts its box arithmetic into FMAs differently), and the rest of a seg / pose / obb row within
+    1e-6 (fp64 trigonometry and keypoint arithmetic, as tests/test_vs_reference_gpu.py compares them); NaNs at the same
+    places."""
     G.equal(key + ".count", got[:, 0], None if ref is None else ref[:, 0])
     for b in range(got.shape[0]):
         g, r = _canon(got, b, var), _canon(ref, b, var)
-        if var == "v8":
+        if var == "v8" or var in V3F:
             G.equal(f"{key}.{b}", g.view(np.uint32), None if r is None else r.view(np.uint32))
             continue
         lead = _lead(var)
@@ -258,13 +319,11 @@ def _vs_ref(key, var, got, ref):
 
 
 # ------------------------------------------------------------------ route matrix -----------------------------------
-@pytest.mark.parametrize("var,net", [("v8", 640), ("v8", 704), ("seg", 640), ("pose", 640), ("obb", 640), ("v5", 640),
-                                     ("v5", 648), ("v5seg", 640), ("v7", 640), ("v3", 640), ("v3", 608)])
-def test_route_matrix(oracle, dev, var, net):
-    """The same heads through every route (and every built (slices, rows) pair of the v8 scan): byte-identical plugin
-    buffers; fp16 heads give exactly the fp32 call on the widened heads; one run matches the oracle."""
+def _route_matrix_case(oracle, dev, var, seed, net=640, gset="rect"):
+    """One heads set through every route (and every built (slices, rows) pair of the v8 scan); returns the (dtype, VEC)
+    pairs it ran."""
     B = 2
-    h16 = _heads16(var, B, seed=700 + net + len(var), net=net, n_obj=24 if var in ("seg", "pose", "obb", "v5seg") else 64)
+    h16 = _heads16(var, B, seed=seed, net=net, gset=gset, n_obj=24 if var in ("seg", "pose", "obb", "v5seg") else 64)
     grids = _grids(h16)
     first, seen = None, set()
     for route, (dtype, off) in ROUTES.items():
@@ -272,7 +331,7 @@ def test_route_matrix(oracle, dev, var, net):
         seen.add((dtype, vec))
         hd = _place(_route_heads(h16, dtype), dtype, off, dev)
         for pair in (PAIRS if var in V8 else (None,)):
-            plug = _plugin(var, dtype, net)
+            plug = _plugin(var, dtype, net, gset=gset)
             if pair:
                 plug.tune(slices=pair[0], rows=pair[1])
             got = _decode(plug, hd, B, dev, vec, grids)
@@ -280,18 +339,45 @@ def test_route_matrix(oracle, dev, var, net):
                 first = got
                 assert got[:, 0].min() > 10
             assert _bits_equal(got, first), (route, pair)
-    expected = {(torch.float32, 4), (torch.float32, 1), (torch.float16, 4), (torch.float16, 1)}
+    wide = [h.astype(np.float32) for h in h16]
+    ref, _ = _oracle(oracle, var, wide, net=net, gset=gset)
+    _check_oracle(var, first, ref)
+    if var in V3F and V3F_GRIDS[gset][1] is None:   # the driver's own kernel, at the net it compiles in
+        _vs_ref(f"scan_route.{var}.{gset}", var, first, _ref_decode(var, wide, dev, gset=gset))
+    return seen
+
+
+@pytest.mark.parametrize("var,net", [("v8", 640), ("v8", 704), ("seg", 640), ("pose", 640), ("obb", 640), ("v5", 640),
+                                     ("v5", 648), ("v5seg", 640), ("v7", 640), ("v3", 640), ("v3", 608)] +
+                         [(v, None) for v in V3F])
+def test_route_matrix(oracle, dev, var, net):
+    """The same heads through every route (and every built (slices, rows) pair of the v8 scan): byte-identical plugin
+    buffers; fp16 heads give exactly the fp32 call on the widened heads; one run matches the oracle.  The yolov3 family
+    (net None) runs every grid set of V3F_GRIDS, each also against its driver's own kernel, and covers all four routes
+    across them."""
+    if var in V3F:
+        seen = set()
+        for i, gset in enumerate(V3F_GRIDS):
+            s = _route_matrix_case(oracle, dev, var, seed=720 + 10 * i + len(var), gset=gset)
+            odd = any(gw * gh % 4 for gw, gh in V3F_GRIDS[gset][0])
+            assert s == ({(torch.float32, 1), (torch.float16, 1)} if odd else FOUR), gset
+            seen |= s
+        assert seen == FOUR
+        return
+    seen = _route_matrix_case(oracle, dev, var, seed=700 + net + len(var), net=net)
+    expected = set(FOUR)
     if var in V8 and net == 640:
         expected.add((torch.float16, 8))
     if net in (648, 608):      # an odd level: VEC 1 whatever the alignment
         expected = {(torch.float32, 1), (torch.float16, 1)}
     assert seen == expected
-    ref, _ = _oracle(oracle, var, [h.astype(np.float32) for h in h16], net=net)
-    _check_oracle(var, first, ref)
 
 
 # ------------------------------------------------------------------ fused and split -------------------------------
-FUSED = {"v8": (0, L.BOX_LTRB, 0.45), "v5": (1, L.BOX_CXCYWH, 0.45), "v3": (1, L.BOX_CXCYWH, 0.4)}
+# mode -> (oracle.nms variant, box format, conf threshold, IoU threshold); the yolov3 family: its driver's nms() parameters
+FUSED = {"v8": (0, L.BOX_LTRB, 0.5, 0.45), "v5": (1, L.BOX_CXCYWH, 0.5, 0.45), "v3": (1, L.BOX_CXCYWH, 0.5, 0.4),
+         **{v: (1, L.BOX_CXCYWH, P.V3_FAMILY_DRIVERS[d]["conf_thresh"], P.V3_FAMILY_DRIVERS[d]["nms_thresh"])
+            for v, d in V3F.items()}}
 
 
 def _fused_three_ways(oracle, dev, var, route, B, seed, net=640):
@@ -300,13 +386,15 @@ def _fused_three_ways(oracle, dev, var, route, B, seed, net=640):
     grids = _grids(h16)
     vec = _expect_vec(var, grids, dtype, off)
     hd = _place(_route_heads(h16, dtype), dtype, off, dev)
-    nms_var, box, iou = FUSED[var]
+    nms_var, box, conf, iou = FUSED[var]
     F = DET[var]
     plug = _plugin(var, dtype, net)
     if var == "v3":
         plug.configure(hd)   # its grids come from the input tensors, and the workspace size from the grids
     buf = _decode(plug, hd, B, dev, vec, grids)
-    fused = P.FusedYoloDecodeNms(plug, B, 0.5, iou, device=dev)
+    if var in V3F:
+        _vs_ref(f"scan_fused.{var}.{route}", var, buf, _ref_decode(var, [h.astype(np.float32) for h in h16], dev))
+    fused = P.FusedYoloDecodeNms(plug, B, conf, iou, device=dev)
     comp1, idx1 = (t.clone() for t in fused.enqueue(B, hd))
     # split form, into the object's own buffers and (as bench.py's double buffer does) into another `out`: every buffer
     # the second half writes starts poisoned, so a row, count or anchor id it leaves out cannot pass
@@ -322,7 +410,7 @@ def _fused_three_ways(oracle, dev, var, route, B, seed, net=640):
         torch.cuda.synchronize()
         if out is not None:
             assert torch.isnan(fused.out).all()   # the object's own output is left alone
-    comp3, row3 = P.batch_nms(torch.from_numpy(buf).to(dev), B, buf.shape[1], 0.5, iou, box_format=box, det_floats=F,
+    comp3, row3 = P.batch_nms(torch.from_numpy(buf).to(dev), B, buf.shape[1], conf, iou, box_format=box, det_floats=F,
                               return_index=True)
     comp1, idx1, comp3, row3 = (t.cpu().numpy() for t in (comp1, idx1, comp3, row3))
     assert _bits_equal(comp1, comp3)
@@ -334,7 +422,7 @@ def _fused_three_ways(oracle, dev, var, route, B, seed, net=640):
     ref, ref_idx = _oracle(oracle, var, [h.astype(np.float32) for h in h16], net=net)
     _check_oracle(var, buf, ref)
     for b in range(B):
-        res, src = oracle.nms(nms_var, ref[b], 1000, F, 0.5, iou)
+        res, src = oracle.nms(nms_var, ref[b], 1000, F, conf, iou)
         n = int(comp1[b, 0])
         assert n == len(res) and n > 5
         ids = ref_idx[b][src]
@@ -347,7 +435,8 @@ def _fused_three_ways(oracle, dev, var, route, B, seed, net=640):
 @pytest.mark.parametrize("var", list(FUSED))
 def test_fused_split_and_two_stage_agree_on_every_route(oracle, dev, var, route):
     """FusedYoloDecodeNms.enqueue, enqueue_scan + enqueue_nms (the split form bench.py times), and the plugin buffer +
-    batch_nms: identical bytes and kept anchor ids on every route, equal to oracle.nms of the oracle's decode."""
+    batch_nms: identical bytes and kept anchor ids on every route, equal to oracle.nms of the oracle's decode (the yolov3
+    family: with its driver's thresholds, and its plugin buffer equal to the driver's own kernel)."""
     _fused_three_ways(oracle, dev, var, route, 3, seed=760 + list(ROUTES).index(route), net=640)
 
 
@@ -483,7 +572,7 @@ def _same_bits(a, b, nan_payloads):
 
 
 @pytest.mark.parametrize("var,group", [("v8", "class"), ("v8", "box")] +
-                         [(v, g) for v in ("v5", "v7", "v3") for g in ("class", "objectness", "box")] +
+                         [(v, g) for v in ("v5", "v7", "v3", *V3F) for g in ("class", "objectness", "box")] +
                          [(v, g) for v in ("seg", "pose", "obb") for g in ("class", "box", "extras")] +
                          [("v5seg", "objectness"), ("v5seg", "extras")])
 def test_non_finite_and_edge_logits(oracle, dev, var, group):
@@ -499,7 +588,7 @@ def test_non_finite_and_edge_logits(oracle, dev, var, group):
     _plant(h16, var, _edge_cases(group, var))
     grids = _grids(h16)
     wide = [h.astype(np.float32) for h in h16]
-    extras = var not in REF_LIB_SCAN
+    extras = var in ("seg", "pose", "obb", "v5seg")
     first = None
     for route, (dtype, off) in ROUTES.items():
         vec = _expect_vec(var, grids, dtype, off)
@@ -549,6 +638,25 @@ def _collision_classes():
     return out
 
 
+def _logist_split_pairs(n=24):
+    """Logit pairs (y, x), y 1 to 8 ulps below x, on which the family's two Logist forms (float: yolov3, yolov3-tiny;
+    double: yolov4, scaled-yolov4), as the oracle evaluates them with glibc expf, disagree about a collision: n whose
+    probabilities round together under the double form only, then n under the float form only, at most one of each per x
+    so that they spread over x from 0.3 up (to about 4.6).  CUDA expf may round otherwise, so the drivers' kernels decide
+    these on the device."""
+    kinds = {True: [], False: []}   # True: the double form collides
+    for i in range(200):
+        x = np.float32(0.3 + 0.0587 * i)
+        found = set()
+        for k in range(1, 9):
+            y = _ulps(x, -k)
+            c64, c32 = _sig(y, True) == _sig(x, True), _sig(y, False) == _sig(x, False)
+            if c64 != c32 and c64 not in found and len(kinds[c64]) < n:
+                kinds[c64].append((y, x))
+                found.add(c64)
+    return kinds[True], kinds[False]
+
+
 def _plant32(heads, var, cases):
     """fp32 cases, one anchor each on image 0's largest level; every other objectness and class logit is -9 (no other
     anchor passes)."""
@@ -571,11 +679,13 @@ def _plant32(heads, var, cases):
             vec[c0 + c] = v
 
 
-@pytest.mark.parametrize("var", ["v8", "v5", "v7", "v3"])
+@pytest.mark.parametrize("var", ["v8", "v5", "v7", "v3", *V3F])
 def test_gate_window_and_near_ulp_collisions_vs_reference_kernel(oracle, dev, var):
     """Whether Logist(x) reaches 0.1f, and whether two logits a few ulps apart round to one probability, depends on CUDA
     expf: only the reference's kernels arbitrate.  The gate window is on the class maximum (v8), the objectness (v5, v7)
-    and both (v3); the collision pairs sit in the class rows.  fp32 heads, VEC 4 and VEC 1; every pair for v8."""
+    and both (v3 and its family); the collision pairs sit in the class rows, and for the family also the pairs on which
+    its float and double Logist disagree (the earlier class wins only where this driver's form collides).  fp32 heads,
+    VEC 4 and VEC 1; every pair for v8."""
     B = 1
     heads = [h.astype(np.float32) for h in _heads16(var, B, seed=850 + len(var), n_obj=0)]
     win = _gate_values()
@@ -584,9 +694,14 @@ def test_gate_window_and_near_ulp_collisions_vs_reference_kernel(oracle, dev, va
         cases += [(None, {i % 30: x}) for i, x in enumerate(win)]
     else:
         cases += [(x, {i % 30: np.float32(2.0)}) for i, x in enumerate(win)]
-        if var == "v3":
+        if var == "v3" or var in V3F:
             cases += [(np.float32(3.0), {i % 30: x}) for i, x in enumerate(win)]
     cases += [(np.float32(3.0), c) for c in _collision_classes()]
+    if var in V3F:
+        dbl, flt = _logist_split_pairs()
+        assert len(dbl) == len(flt) == 24   # both kinds, as the oracle's two forms judge them
+        # the earlier class in slices 0 and 1 (below the collision pairs' 36..60), the later one in slice 3
+        cases += [(np.float32(3.0), {(7 * j) % 36: y, 75: x}) for j, (y, x) in enumerate(dbl + flt)]
     _plant32(heads, var, cases)
     grids = _grids(heads)
     ref = _ref_decode(var, heads, dev)
@@ -623,10 +738,11 @@ def _slice_cases(bounds, base=2.5):
     return [dict(classes=x) for x in cases]
 
 
-@pytest.mark.parametrize("var", ["v8", "v5"])
+@pytest.mark.parametrize("var", ["v8", "v5", *V3F])
 def test_class_slice_boundaries_on_every_pair(oracle, dev, var):
     """Ties and collisions on both sides of every class-slice boundary of every built pair (v8: 80 classes in 1, 2, 4 or
-    8 slices; v5: 4 slices of 20), every route, against the oracle and byte-identical across pairs and routes."""
+    8 slices; v5 and the yolov3 family: 4 slices of 20), every route, against the oracle and byte-identical across pairs
+    and routes; the family also against its driver's own kernel."""
     B = 2
     h16 = _heads16(var, B, seed=870 + len(var), n_obj=8)
     bounds = range(10, 80, 10) if var == "v8" else (20, 40, 60)
@@ -642,15 +758,19 @@ def test_class_slice_boundaries_on_every_pair(oracle, dev, var):
             got = _decode(plug, hd, B, dev, _expect_vec(var, grids, dtype, off), grids)
             first = got if first is None else first
             assert _bits_equal(got, first), (route, pair)
-    ref, _ = _oracle(oracle, var, [h.astype(np.float32) for h in h16])
+    wide = [h.astype(np.float32) for h in h16]
+    ref, _ = _oracle(oracle, var, wide)
     _check_oracle(var, first, ref)
+    if var in V3F:
+        _vs_ref(f"scan_slices.{var}", var, first, _ref_decode(var, wide, dev))
 
 
 @pytest.mark.parametrize("nc", [1, 3, 5])
-@pytest.mark.parametrize("var", ["v8", "v5"])
+@pytest.mark.parametrize("var", ["v8", "v5", *V3F])
 def test_fewer_classes_than_slices(oracle, dev, var, nc):
-    """nc below the slice count (v8 at 8 slices, v5's 4): warps with no class rows must not disturb the others; every pair,
-    every route, against the oracle."""
+    """nc below the slice count (v8 at 8 slices, v5's and the yolov3 family's 4): warps with no class rows must not disturb
+    the others; every pair, every route, against the oracle; the family also against its driver's own kernel, whose blob
+    carries the class count."""
     B = 2
     h16 = _heads16(var, B, seed=890 + nc, nc=nc, n_obj=40)
     grids = _grids(h16)
@@ -664,6 +784,9 @@ def test_fewer_classes_than_slices(oracle, dev, var, nc):
             got = _decode(plug, hd, B, dev, _expect_vec(var, grids, dtype, off), grids)
             first = got if first is None else first
             assert _bits_equal(got, first), (route, pair)
-    ref, _ = _oracle(oracle, var, [h.astype(np.float32) for h in h16], nc=nc)
+    wide = [h.astype(np.float32) for h in h16]
+    ref, _ = _oracle(oracle, var, wide, nc=nc)
     assert ref[:, 0].min() > 10
     _check_oracle(var, first, ref)
+    if var in V3F:
+        _vs_ref(f"scan_fewer.{var}.nc{nc}", var, first, _ref_decode(var, wide, dev, nc=nc))

@@ -5,7 +5,9 @@ scaled-yolov4), each against
     after a canonical sort (the reference's row order is atomicAdd arrival);
 (2) the CPU oracle's decode + that driver's NMS parameters, through every entry point: the plugin decode, the fused
     decode + NMS and the split scan + NMS, fp32 and fp16 heads;
-and the TensorRT creators enqueued through tests/trt_adapter_v3_family_check.cpp --gpu."""
+and the TensorRT creators enqueued through tests/trt_adapter_v3_family_check.cpp --gpu.
+Other grids (non-square, odd cell counts, two levels), class counts, scan routes and edge logits: the family's rows of
+tests/test_yolo_scan_paths_gpu.py, against the same drivers' kernels built from a blob."""
 import ctypes as C
 import subprocess
 
