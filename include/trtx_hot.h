@@ -542,6 +542,21 @@ typedef struct trtx_frame {
 typedef trtx_frame trtx_seg_image;  /* earlier names of trtx_frame, same type */
 typedef trtx_frame trtx_rcnn_image;
 
+/* The per-frame post-processes: trtx_yolo_seg_, trtx_yolo_pose_obb_, trtx_retina_, trtx_rcnn_ (frames), trtx_yolop_,
+ * trtx_detr_, trtx_ufld_, trtx_refinedet_, trtx_yolo_topk_ and trtx_pyrunner_postprocess_enqueue, trtx_rcnn_contours_enqueue
+ * and trtx_centernet_decode_enqueue.  Each maps its model's rows, masks or maps back to every original frame of a batch, and
+ * they share one contract:
+ *   the frames: frame_wh_host, `batch` (img_w, img_h) pairs, or images_host / frames_host, `batch` trtx_frame, in HOST
+ *     memory, copied into launch parameters; sizes may differ in a call.
+ *   Everything is checked before the first launch, so a rejected call writes nothing, in this order:
+ *     1. TRTX_ERR_INVALID for a null pointer, a parameter outside its range, a frame size <= 0 or a bad descriptor, and a
+ *        misaligned workspace;
+ *     2. TRTX_ERR_UNSUPPORTED for a parameter or a frame past the entry's limits;
+ *     3. TRTX_ERR_WORKSPACE for a workspace smaller than the entry's size function returns.
+ *     So a call that fails two ways returns the first of these, whichever frame fails first.
+ *   One launch of each kernel per <= 64 frames; can be captured in a CUDA graph.
+ * Each entry's doc below lists its own cases. */
+
 /* The segmentation models' last host stage on the device: process_mask + scale_mask + draw_mask_bbox's mask selection
  * (yolov8/src/postprocess.cpp:228-248, yolov5/src/postprocess.cpp:148-167), for a batch of original frames of any sizes. */
 
@@ -550,7 +565,6 @@ typedef trtx_frame trtx_rcnn_image;
  *   yolov3-tiny and yolov3-spp, whose models have no masks; with canvases those two are TRTX_ERR_INVALID).
  * dets_dev [B, 1 + max_rows*row_floats]: count, rows with the box at floats 0..3 in the variant's format, conf at 4, class
  *   at 5 (the compact NMS output with extra_floats = 32: row_floats 39, coeff_offset 7; plugin rows: 90 / 6).
- * images_host: `batch` descriptors in HOST memory (copied into launch parameters; sizes may differ within a call).
  * rows_dev [B, 1 + max_rows*6]: n = min(count, max_rows), then per row i < n (x, y, w, h, conf, class) with x, y, w, h =
  *   get_rect(img, bbox) (trtx_get_rect: V8 clamped to the image, V5 not), rows past n zeroed.  A box whose get_rect is
  *   undefined in the reference (non-finite, or corners outside the int range) gets {0, 0, 0, 0}.
@@ -560,12 +574,10 @@ typedef trtx_frame trtx_rcnn_image;
  *   Bit-identical to thresholding trtx_process_mask_enqueue -> trtx_scale_mask_enqueue.  Canvases at or past that count are
  *   left untouched.
  * proto_dev [B, num_coeffs, mask_h, mask_w] may be NULL only when every masks_dev is NULL; NULL and non-NULL masks_dev in one
- * call is TRTX_ERR_INVALID.  Everything is checked before the first launch (a rejected call writes nothing):
- * TRTX_ERR_INVALID for null pointers, batch / max_rows / sizes <= 0, pitch < img_w; TRTX_ERR_UNSUPPORTED for an image whose
- * scale_mask crop is empty (e.g. 1 x 5000: the reference's cv::resize throws), and for nets whose canvas launch would need
- * more than 226 KB of shared memory (227 KB less a 1 KB margin for the kernel's static arrays; square nets above 2408^2
- * with a frame of a few pixels).  Two launches per 64 images, no
- * workspace. */
+ * call is TRTX_ERR_INVALID.  A per-frame post-process: TRTX_ERR_INVALID for batch / max_rows <= 0, pitch < img_w;
+ * TRTX_ERR_UNSUPPORTED for an image whose scale_mask crop is empty (e.g. 1 x 5000: the reference's cv::resize throws), and
+ * for nets whose canvas launch would need more than 226 KB of shared memory (227 KB less a 1 KB margin for the kernel's
+ * static arrays; square nets above 2408^2 with a frame of a few pixels).  Two kernels, no workspace. */
 TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const trtx_frame* images_host, int batch,
                                                const float* proto_dev, const float* dets_dev, int max_rows,
                                                float* rows_dev, trtx_stream_t stream);
@@ -603,15 +615,13 @@ typedef struct trtx_pose_obb_params {
  *   OBB_NMS_FREE: the output of YoloLayerPlugin26 with is_obb (TRTX_YOLO_V26, det_floats 90): row_floats 90,
  *   extra_offset 89, box cx, cy, w, h; every one of the first min(count, max_rows) rows is used (yolo26's
  *   batch_decode_obb, yolo26/src/postprocess.cpp:310-326).
- * frame_wh_host: `batch` (img_w, img_h) pairs in HOST memory (copied into launch parameters; sizes may differ in a call).
  * rows_dev [B, 1 + max_rows*F]: n kept rows in input order, then zeros up to max_rows:
  *   pose, F = 6 + 3*num_kpts: (x, y, w, h, conf, class, kx, ky, kc, ...) = trtx_get_rect_adapt_landmark;
  *   OBB and OBB_NMS_FREE, F = 10: (x0, y0, x1, y1, x2, y2, x3, y3, conf, class) = trtx_get_corner.
  * Bit-identical to those host functions (the device's double cos / sin are not correctly rounded, see trtx_get_corner).
- * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
- * batch / max_rows / sizes <= 0, an unknown task, row_floats < 7 or extras outside the row, num_kpts outside 0..64, an
- * OBB_NMS_FREE angle that is not the row's last float.  One launch per 64 frames, one CTA per frame, no atomics
- * (deterministic), no workspace; can be captured in a CUDA graph. */
+ * A per-frame post-process: TRTX_ERR_INVALID for batch / max_rows <= 0, an unknown task, row_floats < 7 or extras outside
+ * the row, num_kpts outside 0..64, an OBB_NMS_FREE angle that is not the row's last float.  One CTA per frame, no atomics
+ * (deterministic), no workspace. */
 TRTX_API int trtx_yolo_pose_obb_postprocess_enqueue(const trtx_pose_obb_params* p, const int32_t* frame_wh_host, int batch,
                                                     const float* dets_dev, int max_rows, float* rows_dev,
                                                     trtx_stream_t stream);
@@ -633,14 +643,12 @@ typedef struct trtx_face_post_params {
  *   output of trtx_nms_enqueue with TRTX_BOX_RETINA, extra_offset 5 (the landmarks, then AntiCov's mask_confidence).  Of the
  *   first min(count, max_rows) rows those with (int)keep == 1 and !(conf < conf_thresh) are used (a NaN conf is kept, as in
  *   the reference).
- * frame_wh_host: `batch` (img_w, img_h) pairs in HOST memory (copied into launch parameters; sizes may differ in a call).
  * rows_dev [B, 1 + max_rows*F], F = 15 (FACE) or 16 (ANTICOV): the used count, then per used row in input order
  *   (x, y, w, h, conf, lx0, ly0, ..., lx4, ly4[, mask_conf]): the rectangle of trtx_retina_get_rect_adapt_landmark as
  *   floats (exact for |v| <= 2^24) and its mapped landmarks, bit-identical to that host function; rows past the count are
  *   zeroed.
- * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
- * batch / max_rows / sizes <= 0, an unknown variant, row_floats < 7, landmarks or mask_confidence outside the row.  One
- * launch per 64 frames, one CTA per frame, no atomics, no workspace; can be captured in a CUDA graph. */
+ * A per-frame post-process: TRTX_ERR_INVALID for batch / max_rows <= 0, an unknown variant, row_floats < 7, landmarks or
+ * mask_confidence outside the row.  One CTA per frame, no atomics, no workspace. */
 TRTX_API int trtx_retina_postprocess_enqueue(const trtx_face_post_params* p, const int32_t* frame_wh_host, int batch,
                                              const float* dets_dev, int max_rows, float* rows_dev, trtx_stream_t stream);
 
@@ -686,18 +694,16 @@ TRTX_API int trtx_rcnn_postprocess_enqueue(const trtx_rcnn_post_params* p, int b
                                            float* rows_dev, uint8_t* masks_out_dev, trtx_stream_t stream);
 
 /* The same post-process for a batch of frames of mixed original sizes, one trtx_frame per frame.
- * p: as for trtx_rcnn_postprocess_enqueue except img_w / img_h, which are not read.  images_host: `batch` descriptors in
- *   HOST memory (copied into launch parameters).  scores_dev, boxes_dev, classes_dev, masks_dev and rows_dev: the layouts of
+ * p: as for trtx_rcnn_postprocess_enqueue except img_w / img_h, which are not read.  scores_dev, boxes_dev, classes_dev, masks_dev and rows_dev: the layouts of
  *   trtx_rcnn_postprocess_enqueue (the engine input net_w x net_h is one size per call).
  * Image b is rescaled with its own pads, trtx_rcnn_letterbox_pads(img_w_b, img_h_b, net_w, net_h), and its own ratios, and
  *   its canvas k starts at masks_dev_b + k * img_h_b * pitch_b: image b of a call equals a batch-1
  *   trtx_rcnn_postprocess_enqueue of image b with its size.  Pixel rule, threshold and untouched canvases as there; the
  *   bytes of a row past img_w are never written.
  * Canvases for every frame or for none: NULL and non-NULL masks_dev in one call, or canvases with a NULL masks_dev input,
- *   is TRTX_ERR_INVALID (with no canvases masks_dev is not read).  Everything is checked before the first launch (a
- *   rejected call writes nothing): TRTX_ERR_INVALID for null pointers, batch / sizes <= 0, pitch < img_w, mask_size > 32;
- *   TRTX_ERR_UNSUPPORTED for more than INT_MAX paste CTAs in one launch.  Two launches per 64 frames, no workspace, no
- *   atomics; can be captured in a CUDA graph. */
+ *   is TRTX_ERR_INVALID (with no canvases masks_dev is not read).  A per-frame post-process: TRTX_ERR_INVALID for
+ *   batch <= 0, pitch < img_w, mask_size > 32; TRTX_ERR_UNSUPPORTED for more than INT_MAX paste CTAs in one launch.  Two
+ *   kernels, no workspace, no atomics. */
 TRTX_API int trtx_rcnn_postprocess_frames_enqueue(const trtx_rcnn_post_params* p, const trtx_frame* images_host,
                                                   int batch, const float* scores_dev, const float* boxes_dev,
                                                   const float* classes_dev, const float* masks_dev, float* rows_dev,
@@ -709,8 +715,8 @@ TRTX_API int trtx_rcnn_postprocess_frames_enqueue(const trtx_rcnn_post_params* p
  * starting at its component's first pixel in raster order and going down its left side first, the contours in descending
  * raster order of their starts).  The drawing (cv::drawContours) stays with the caller.
  * p: the parameters of the post-process call that wrote rows and canvases; only detections_per_im and max_masks are read.
- * images_host: `batch` descriptors in HOST memory, each with its canvases (the single-size entry's dense canvases are frames
- *   of equal size with pitch = img_w).  rows_dev [B, 1 + D*7]: that call's rows.
+ * images_host: each frame with its canvases (the single-size entry's dense canvases are frames of equal size with
+ *   pitch = img_w).  rows_dev [B, 1 + D*7]: that call's rows.
  * The call reads only the paste rectangle r of each row (trtx_rcnn_postprocess_enqueue's), where the post-process writes;
  *   it returns the contours of the canvas restricted to r, which are those of the whole canvas, since the post-process
  *   leaves 0 outside r.  Where the reference throws (empty r, r leaving the image, a non-finite box) the canvas is all zeros
@@ -726,11 +732,9 @@ TRTX_API int trtx_rcnn_postprocess_frames_enqueue(const trtx_rcnn_post_params* p
  *   only: min(min(batch, 64) * max_masks, 128) slots of (W + 2)(H + 2) + 8 ceil(W/2) ceil(H/2) + 256 ceil(W/2) bytes
  *   (each term the largest over the frames, the sum rounded up to 256), about 3 bytes per frame pixel.  0 when the
  *   arguments are rejected.
- * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
- *   batch / sizes / detections_per_im / max_masks / max_contours / max_points <= 0, a frame without canvases, pitch < img_w,
- *   a misaligned workspace; TRTX_ERR_WORKSPACE for a smaller workspace_bytes; TRTX_ERR_UNSUPPORTED for a frame of more
- *   than 2^29 pixels.  One launch per 64 frames of at most 128 CTAs with 200 KB of dynamic shared memory each, no atomics
- *   (deterministic); can be captured in a CUDA graph. */
+ * A per-frame post-process: TRTX_ERR_INVALID for batch / detections_per_im / max_masks / max_contours / max_points <= 0,
+ *   a frame without canvases, pitch < img_w, a workspace not 16-byte aligned; TRTX_ERR_UNSUPPORTED for a frame of more than
+ *   2^29 pixels.  Launches of at most 128 CTAs with 200 KB of dynamic shared memory each, no atomics (deterministic). */
 TRTX_API size_t trtx_rcnn_contours_workspace_size(const trtx_rcnn_post_params* p, const trtx_frame* images_host, int batch);
 TRTX_API int trtx_rcnn_contours_enqueue(const trtx_rcnn_post_params* p, const trtx_frame* images_host, int batch,
                                         const float* rows_dev, int max_contours, int max_points, int32_t* counts_dev,
@@ -800,7 +804,6 @@ typedef struct trtx_yolop_post_params {
 /* dets_dev [B, 1 + max_rows*row_floats]: count, then (cx, cy, w, h, conf, class, keep, ...) rows -- the compact output of
  *   trtx_nms_enqueue (TRTX_BOX_CXCYWH, greedy, det_floats 6) over the plugin rows.  Of the first min(count, max_rows) rows
  *   those with (int)keep == 1 are used: every row of a greedy output.
- * frames_host: `batch` trtx_frame in HOST memory (copied into launch parameters; sizes may differ in a call).
  * rows_dev [B, 1 + max_rows*6]: the used count, then per used row in input order (x, y, w, h, conf, class) with x, y, w, h =
  *   trtx_yolop_get_rect as floats (exact for |v| <= 2^24); rows past the count are zeroed.
  * Labels, where frames_host[b].masks_dev is an [img_h, pitch] u8 canvas: pixel (x, y) of frame b gets 2 where
@@ -809,11 +812,10 @@ typedef struct trtx_yolop_post_params {
  *   INTER_NEAREST of OpenCV 4.x.  Bytes of a row past img_w are not written.  seg_dev and lane_dev are the engine's
  *   [B, map_h, map_w] int32 index maps.  Frame b reads maps b; the reference reads the first image's maps for every frame
  *   (yolop.cpp:90-92), which is the same at its BATCH_SIZE 1.  Colouring the frame stays with the caller.
- * Canvases for every frame or for none (then seg_dev and lane_dev may be NULL and are not read).  Everything is checked before
- * the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer, batch / max_rows / sizes <= 0,
- * row_floats < 7, NULL and non-NULL masks_dev in one call, pitch < img_w; TRTX_ERR_UNSUPPORTED where a CTA's shared-memory
- * tables, 10 bytes per pixel of the widest frame's row + 8 * map_w bytes, exceed 227 KB (with 640-wide maps: frames wider
- * than about 22 000 pixels).  Two launches per 64 frames, no workspace, no atomics; can be captured in a CUDA graph. */
+ * Canvases for every frame or for none (then seg_dev and lane_dev may be NULL and are not read).  A per-frame post-process:
+ * TRTX_ERR_INVALID for batch / max_rows <= 0, row_floats < 7, NULL and non-NULL masks_dev in one call, pitch < img_w;
+ * TRTX_ERR_UNSUPPORTED where a CTA's shared-memory tables, 10 bytes per pixel of the widest frame's row + 8 * map_w bytes,
+ * exceed 227 KB (with 640-wide maps: frames wider than about 22 000 pixels).  Two kernels, no workspace, no atomics. */
 TRTX_API int trtx_yolop_postprocess_enqueue(const trtx_yolop_post_params* p, const trtx_frame* frames_host, int batch,
                                             const float* dets_dev, int max_rows, const int32_t* seg_dev,
                                             const int32_t* lane_dev, float* rows_dev, trtx_stream_t stream);
@@ -848,17 +850,15 @@ typedef struct trtx_detr_post_params {
 } trtx_detr_post_params;
 
 /* scores_dev [B, Q, C] fp32: the engine's softmax scores; boxes_dev [B, Q, 4] fp32: its (cx, cy, w, h), normalised.
- * frame_wh_host: `batch` pairs (img_w, img_h) in HOST memory (copied into launch parameters; sizes may differ in a call).
  * rows_dev [B, 1 + Q*6]: the kept count, then per kept query in query order (x, y, w, h, score, class) with x, y, w, h =
  *   trtx_detr_get_rect as floats (exact for |v| <= 2^24); rows past the count are zeroed.
  * Per query (detr.cpp:779-799): label = -1, score = -1.f; for j = 0 .. C-1 `if (score < s[j])` takes j, so the first
  * maximum wins and a NaN is never taken; the query is kept when score > score_thresh (float) and label != C - 1.  Frame b
  * reads queries b; the reference's loop runs over every query of the batch for every frame (detr.cpp:778), which is the
  * same at its BATCH_SIZE 1.  Drawing and labels stay with the caller.
- * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
- * batch / Q / a frame size <= 0, C < 2, or a score_thresh that is NaN or below -1 (which would keep the reference's
- * label -1 queries); TRTX_ERR_UNSUPPORTED for Q or C above 2^24 (the count and the class are stored as floats).  One CTA per
- * frame, one launch per 64 frames, no workspace, no atomics; can be captured in a CUDA graph. */
+ * A per-frame post-process: TRTX_ERR_INVALID for batch / Q <= 0, C < 2, or a score_thresh that is NaN or below -1 (which
+ * would keep the reference's label -1 queries); TRTX_ERR_UNSUPPORTED for Q or C above 2^24 (the count and the class are
+ * stored as floats).  One CTA per frame, no workspace, no atomics. */
 TRTX_API int trtx_detr_postprocess_enqueue(const trtx_detr_post_params* p, const int32_t* frame_wh_host, int batch,
                                            const float* scores_dev, const float* boxes_dev, float* rows_dev,
                                            trtx_stream_t stream);
@@ -909,15 +909,14 @@ TRTX_API size_t trtx_centernet_workspace_size(const trtx_centernet_params* p, in
  *   4. class = c, xs = x + reg[0, y, x], ys = y + reg[1, y, x], x1 = xs - wh[0] / 2, y1 = ys - wh[1] / 2, x2 = xs + wh[0] / 2,
  *      y2 = ys + wh[1] / 2, all float without contraction.  The accepted sizes keep the reference's float index divisions
  *      (true_divide(width), true_divide(K)) equal to integer divisions.
- * Frame rows (the driver loop), when frame_wh_host (`batch` pairs img_w, img_h in HOST memory) and rows_dev are both given:
+ * Frame rows (the driver loop), when frame_wh_host and rows_dev are both given:
  * rows_dev [B, 1 + K * 6] gets the count n of detections with score > score_thresh (a NaN score is dropped), then those
  * rows in order as (x1 * k, y1 * k, x2 * k, y2 * k, score, class), zeros past n, with k = (float)(down * (L / (double)net)),
  * L = max(img_h, img_w, 3) -- `i[:4] *= 4*s`, each product rounded once; int(), rectangles and text stay with the caller.
- * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer, batch,
- * C, H, W or K <= 0, K > H * W (the reference's topk raises), only one of frame_wh_host / rows_dev, and with rows a net or down <= 0,
- * a NaN score_thresh or a frame size <= 0; TRTX_ERR_WORKSPACE for a short workspace; TRTX_ERR_INVALID for a workspace that is
- * not 256-byte aligned; TRTX_ERR_UNSUPPORTED for C > 1024, H or W > 1024, H * W > 2^20 or K > 1024.  Two launches per call
- * (one more per 64 frames past the first 64), no host sync, no allocation; can be captured in a CUDA graph. */
+ * A per-frame post-process: TRTX_ERR_INVALID for batch, C, H, W or K <= 0, K > H * W (the reference's topk raises), only
+ * one of frame_wh_host / rows_dev, with rows a net or down <= 0 or a NaN score_thresh, and a workspace that is not 256-byte
+ * aligned; TRTX_ERR_UNSUPPORTED for C > 1024, H or W > 1024, H * W > 2^20 or K > 1024; TRTX_ERR_WORKSPACE for a workspace
+ * short of trtx_centernet_workspace_size.  Two kernels, no host sync, no allocation. */
 TRTX_API int trtx_centernet_decode_enqueue(const trtx_centernet_params* p, int batch, const float* heat_dev,
                                            const float* wh_dev, const float* reg_dev, void* workspace_dev,
                                            size_t workspace_bytes, float* dets_dev, const int32_t* frame_wh_host,
@@ -948,8 +947,8 @@ typedef struct trtx_ufld_post_params {
 } trtx_ufld_post_params;
 
 /* prob_dev [B, C, H, W] fp32: the engine output `prob`.  row_anchor_host: H ints in HOST memory (tusimple_row_anchor);
- * frame_wh_host: `batch` pairs (w, h) in HOST memory, the size of the picture the points are for ((1280, 720) is the driver's
- * `vis`; a frame's own size gives the points on that frame); both are copied into launch parameters.
+ * frame_wh_host: (w, h) of the picture the points are for ((1280, 720) is the driver's `vis`; a frame's own size gives the
+ * points on that frame); the anchors are copied into launch parameters too.
  * rows_dev [B, 1 + H*W*3]: the point count n, then n rows (x, y, lane) as floats in the driver's draw order -- engine rows
  * j = H - 1 .. 0 (the driver flips the rows and indexes the anchors with H - 1 - k), the chosen lanes ascending in each --
  * then zeros.  Per cell (row j, lane l), reading prob[b, :, j, l], each statement of the driver rounded as there:
@@ -964,11 +963,10 @@ typedef struct trtx_ufld_post_params {
  * expect > 0 (NaN excluded) gives x = (int)(((expect * (float)col_sample_w) * (float)w) / (float)net_w) - 1 (float, left to
  * right; (int) as x86-64 converts, the - 1 wrapping) and y = h * anchor[j] / net_h - 1 in int; rows hold (float)x, exact for
  * |x| <= 2^24 (C * col_sample_w * w <= 2^24 * net_w suffices).
- * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer, batch,
- * H, W, net_w, net_h, col_sample_w or a frame side <= 0, or C < 2; TRTX_ERR_UNSUPPORTED for H * W > 1024 or
- * (C - 1) * H * W > 53 248 (one CTA per frame: a thread per cell, the exponentials in shared memory), a frame side above 2^24,
- * or a frame and anchor where h * anchor overflows int32 or |y| > 2^24.  One launch per 64 frames, no workspace, no atomics;
- * can be captured in a CUDA graph. */
+ * A per-frame post-process: TRTX_ERR_INVALID for batch, H, W, net_w, net_h or col_sample_w <= 0, or C < 2;
+ * TRTX_ERR_UNSUPPORTED for H * W > 1024 or (C - 1) * H * W > 53 248 (one CTA per frame: a thread per cell, the exponentials
+ * in shared memory), a frame side above 2^24, or a frame and anchor where h * anchor overflows int32 or |y| > 2^24.  No
+ * workspace, no atomics. */
 TRTX_API int trtx_ufld_postprocess_enqueue(const trtx_ufld_post_params* p, const int32_t* row_anchor_host,
                                            const int32_t* frame_wh_host, int batch, const float* prob_dev, float* rows_dev,
                                            trtx_stream_t stream);
@@ -1051,18 +1049,16 @@ TRTX_API size_t trtx_refinedet_workspace_size(const trtx_refinedet_params* p, in
  *            Ties: the reference's CUDA sort leaves the order among equal scores, and the top_k cut at a tie, open; here a lower
  *            prior index ranks higher.
  * The reference's `score_my[0] < conf_thresh` class skip never fires (a kept score is above conf_thresh).
- * Frame rows, when frame_wh_host (`batch` pairs cols, rows in HOST memory, copied into launch parameters) and rows_dev
+ * Frame rows, when frame_wh_host ((cols, rows) pairs) and rows_dev
  * [B, 1 + max_det * 6] are both given: the count, then per det row in order with score >= score_thresh (the driver's
  * `if (score < TH) continue`) (x, y, w, h, score, label) with x = (int)(x1 * cols) (a float product), w = (int)(x2 * cols -
  * x) in float, likewise y and h, then RoiCorrect: x < 0 -> 0, y < 0 -> 0, x >= cols - 1 -> 0, y >= rows - 1 -> 0, w <= 0 -> 1,
  * h <= 0 -> 1, x + w > cols - 1 -> w = cols - 1 - x, likewise h.  Conversions as x86-64 performs them (INT_MIN for NaN,
  * inf and out of range), x + w wrapping as there; zeros past the count.
- * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
- * batch, net, top_k or max_det <= 0, C < 2, a NaN threshold, only one of frame_wh_host / rows_dev or a frame side <= 0;
- * TRTX_ERR_WORKSPACE for a short workspace; TRTX_ERR_INVALID for a workspace that is not 256-byte aligned;
- * TRTX_ERR_UNSUPPORTED for S not a multiple of 64, P > 2^16 (S > 1024), top_k > 1024, C > 1024, max_det > 2^24 or a frame
- * side above 2^24.  Two launches per call (one more per 64 frames past the first 64), no host sync, no allocation; can be
- * captured in a CUDA graph. */
+ * A per-frame post-process: TRTX_ERR_INVALID for batch, net, top_k or max_det <= 0, C < 2, a NaN threshold, only one of
+ * frame_wh_host / rows_dev, and a workspace that is not 256-byte aligned; TRTX_ERR_UNSUPPORTED for S not a multiple of 64,
+ * P > 2^16 (S > 1024), top_k > 1024, C > 1024, max_det > 2^24 or a frame side above 2^24; TRTX_ERR_WORKSPACE for a
+ * workspace short of trtx_refinedet_workspace_size.  Two kernels, no host sync, no allocation. */
 TRTX_API int trtx_refinedet_postprocess_enqueue(const trtx_refinedet_params* p, int batch, const float* arm_loc_dev,
                                                 const float* arm_conf_dev, const float* odm_loc_dev, const float* odm_conf_dev,
                                                 void* workspace_dev, size_t workspace_bytes, float* dets_dev,
@@ -1127,13 +1123,11 @@ typedef struct trtx_yolo_topk_params {
  *   buffer of that layout.  Of the first min(count, max_rows) rows, those with !(conf <= conf_thresh) are used, in input
  *   order, with no NMS and no sort (get_topk reads up to the count, which the reference's plugin lets run past maxOut; the
  *   library's decode clamps it).
- * frame_wh_host: `batch` (img_w, img_h) pairs in HOST memory (copied into launch parameters; sizes may differ in a call).
  * rows_dev [B, 1 + max_rows*6]: the used count, then per used row (x, y, w, h, conf, class) with x, y, w, h = trtx_get_rect
  *   of the row's box for the variant ({0, 0, 0, 0} where that is undefined), bit-identical to it; rows past the count are
  *   zeroed.
- * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
- * batch / max_rows / sizes <= 0, a variant other than the two above, row_floats < 6.  One launch per 64 frames, one CTA per
- * frame, no atomics, no workspace; can be captured in a CUDA graph. */
+ * A per-frame post-process: TRTX_ERR_INVALID for batch / max_rows <= 0, a variant other than the two above, row_floats < 6.
+ * One CTA per frame, no atomics, no workspace. */
 TRTX_API int trtx_yolo_topk_postprocess_enqueue(const trtx_yolo_topk_params* p, const int32_t* frame_wh_host, int batch,
                                                 const float* dets_dev, int max_rows, float* rows_dev, trtx_stream_t stream);
 
@@ -1170,7 +1164,6 @@ typedef struct trtx_pyrunner_params {
  *   max_rows <= TRTX_NMS_MAX_ROWS.  The first n rows are read, n = the count float truncated and clamped to [0, max_rows]
  *   (a count below 1 or NaN reads none: the runner slices from the end for a negative count and raises on a NaN; the
  *   plugin writes neither).
- * frame_wh_host: `batch` (img_w, img_h) pairs in HOST memory, copied into launch parameters.
  * Per frame, all in float32 as numpy computes it: conf = row[4] (times row[conf_col]); rows with conf >= conf_thresh; the
  *   box mapped by xywh2xyxy (the pad (net - r * origin) / 2 and the ratio r are computed in double and rounded to float,
  *   then y -= pad, y /= r) and clipped to [0, img_w - 1] x [0, img_h - 1] as np.clip does (a NaN stays NaN); sorted by
@@ -1181,10 +1174,9 @@ typedef struct trtx_pyrunner_params {
  *   the device defines that case by the consume rule and agrees with the runner wherever the runner returns.
  * rows_dev [B, 1 + max_rows*6]: the kept count, then the kept rows in order as (x1, y1, x2, y2, conf, row[5]) floats at
  *   the frame's size; floats past the count are zeroed.
- * Everything is checked before the first launch (a rejected call writes nothing): TRTX_ERR_INVALID for a null pointer,
- * batch / max_rows / net or frame sizes <= 0, another box format, columns outside the ranges above, or a NaN threshold;
- * TRTX_ERR_UNSUPPORTED for max_rows > TRTX_NMS_MAX_ROWS.  One launch per 64 frames, no atomics, no workspace,
- * deterministic; can be captured in a CUDA graph. */
+ * A per-frame post-process: TRTX_ERR_INVALID for batch / max_rows / net sizes <= 0, another box format, columns outside
+ * the ranges above, a NaN threshold, or dets_dev / rows_dev not 4-byte aligned; TRTX_ERR_UNSUPPORTED for
+ * max_rows > TRTX_NMS_MAX_ROWS.  No atomics, no workspace, deterministic. */
 TRTX_API int trtx_pyrunner_postprocess_enqueue(const trtx_pyrunner_params* p, const int32_t* frame_wh_host, int batch,
                                                const float* dets_dev, int max_rows, float* rows_dev, trtx_stream_t stream);
 

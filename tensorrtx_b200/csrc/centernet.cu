@@ -34,7 +34,6 @@ constexpr int kCnMaxClasses = 1024;
 constexpr int kCnListCap = kCnStripCells + kCnMaxK;       // the shared candidate list: K kept + one strip
 constexpr int kCnSigFloats = kCnStripCells + 2 * kCnMaxSide;  // the strip's sigmoids with a halo row above and below
 constexpr size_t kCnPeakSmem = (size_t)kCnSigFloats * 4 + (size_t)kCnListCap * 8 + (size_t)kCnMaxK * 4;
-constexpr int kCnMaxFrames = 64;     // frames per select launch (launch-parameter arrays)
 constexpr int kCnRow = 6;            // x1, y1, x2, y2, score, class
 
 // The select key: NaN above everything, then float_key (values are sigmoids or +0, never negative).
@@ -152,7 +151,7 @@ struct CnDecodeArgs {
     int C, H, W, K;
     float score_thresh;
     int base;           // select launch: frames [base, base + gridDim.x)
-    float scale[kCnMaxFrames];  // select launch: (float)(down * (L / net)) per frame
+    float scale[kMaxFrames];  // select launch: (float)(down * (L / net)) per frame
 };
 
 __global__ void __launch_bounds__(kCnPeakThreads) centernet_peaks_kernel(const __grid_constant__ CnDecodeArgs a) {
@@ -314,7 +313,6 @@ __global__ void __launch_bounds__(kCnSelectThreads) centernet_select_kernel(cons
 // with its fraction zeroed at both ends on both axes; each pass is a0 * p0 + a1 * p1 in double.  _rn intrinsics so that nvcc
 // cannot contract a product into a DFMA.  One thread per output pixel, three planes B, G, R.
 constexpr int kCnPreThreads = 256;
-constexpr int kCnMaxPreImages = 64;
 constexpr int kCnMaxNet = 8192;
 
 struct CnPreImage {
@@ -323,7 +321,7 @@ struct CnPreImage {
     int w, h, pitch, L;
 };
 struct CnPreArgs {
-    CnPreImage img[kCnMaxPreImages];
+    CnPreImage img[kMaxFrames];
     int net, base;
 };
 
@@ -367,11 +365,15 @@ using namespace trtx;
 
 extern "C" {
 
-// Everything that can reject a decode call, before the first launch; TRTX_OK or the error code.
-static int centernet_check(const trtx_centernet_params* p, int batch) {
+// Everything in the parameters and the frame sizes (frame_wh_host, may be null) that can reject a decode call, before the
+// first launch, in two passes so that TRTX_ERR_INVALID wins; TRTX_OK or the error code.
+static int centernet_check(const trtx_centernet_params* p, int batch, const int32_t* frame_wh_host) {
     if (!p || batch <= 0) return TRTX_ERR_INVALID;
     if (p->num_classes <= 0 || p->height <= 0 || p->width <= 0 || p->k <= 0) return TRTX_ERR_INVALID;
     if ((int64_t)p->k > (int64_t)p->height * p->width) return TRTX_ERR_INVALID;  // the reference's topk raises
+    if (frame_wh_host && (p->net <= 0 || p->down <= 0 || !(p->score_thresh == p->score_thresh) ||
+                          !frames_valid(frame_wh_host, batch)))
+        return TRTX_ERR_INVALID;
     if (p->num_classes > kCnMaxClasses || p->height > kCnMaxSide || p->width > kCnMaxSide ||
         (int64_t)p->height * p->width > kCnMaxCells || p->k > kCnMaxK)
         return TRTX_ERR_UNSUPPORTED;
@@ -379,7 +381,7 @@ static int centernet_check(const trtx_centernet_params* p, int batch) {
 }
 
 TRTX_API size_t trtx_centernet_workspace_size(const trtx_centernet_params* p, int batch) {
-    if (centernet_check(p, batch) != TRTX_OK) return 0;
+    if (centernet_check(p, batch, nullptr) != TRTX_OK) return 0;
     return align_up((size_t)batch * p->num_classes * p->k * sizeof(float)) * 2;
 }
 
@@ -387,23 +389,14 @@ TRTX_API int trtx_centernet_decode_enqueue(const trtx_centernet_params* p, int b
                                            const float* wh_dev, const float* reg_dev, void* workspace_dev,
                                            size_t workspace_bytes, float* dets_dev, const int32_t* frame_wh_host,
                                            float* rows_dev, trtx_stream_t stream) {
-    const int rc0 = centernet_check(p, batch);
-    if (rc0 != TRTX_OK) return rc0;
     if (!heat_dev || !wh_dev || !reg_dev || !workspace_dev || !dets_dev) return TRTX_ERR_INVALID;
     if (!frame_wh_host != !rows_dev) return TRTX_ERR_INVALID;  // the frame rows need both
-    if (frame_wh_host) {
-        if (p->net <= 0 || p->down <= 0 || !(p->score_thresh == p->score_thresh)) return TRTX_ERR_INVALID;
-        for (int i = 0; i < batch; ++i)
-            if (frame_wh_host[2 * i] <= 0 || frame_wh_host[2 * i + 1] <= 0) return TRTX_ERR_INVALID;
-    }
-    if (workspace_bytes < trtx_centernet_workspace_size(p, batch)) return TRTX_ERR_WORKSPACE;
     if (reinterpret_cast<uintptr_t>(workspace_dev) % kAlign) return TRTX_ERR_INVALID;
+    int rc = centernet_check(p, batch, frame_wh_host);
+    if (rc) return rc;
+    if (workspace_bytes < trtx_centernet_workspace_size(p, batch)) return TRTX_ERR_WORKSPACE;
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (cudaFuncSetAttribute(centernet_peaks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCnPeakSmem) !=
-        cudaSuccess) {
-        g_last_cuda_error = (int)cudaGetLastError();
-        return TRTX_ERR_CUDA;
-    }
+    if ((rc = opt_in_smem(centernet_peaks_kernel, kCnPeakSmem))) return rc;
     CnDecodeArgs a;
     a.heat = heat_dev;
     a.wh = wh_dev;
@@ -420,22 +413,12 @@ TRTX_API int trtx_centernet_decode_enqueue(const trtx_centernet_params* p, int b
     a.score_thresh = p->score_thresh;
     a.base = 0;
     centernet_peaks_kernel<<<(unsigned)(batch * p->num_classes), kCnPeakThreads, kCnPeakSmem, st>>>(a);
-    int rc = check_launch();
-    if (rc) return rc;
-    for (int i0 = 0; i0 < batch; i0 += kCnMaxFrames) {
-        const int n = min(batch - i0, kCnMaxFrames);
-        a.base = i0;
-        for (int j = 0; j < n; ++j) {
-            if (!frame_wh_host) break;
-            const int w = frame_wh_host[2 * (i0 + j)], h = frame_wh_host[2 * (i0 + j) + 1];
-            const int L = max(max(h, w), 3);  // max(image.shape): the channel count takes part
-            a.scale[j] = (float)((double)p->down * ((double)L / (double)p->net));
-        }
-        centernet_select_kernel<<<n, kCnSelectThreads, 0, st>>>(a);
-        rc = check_launch();
-        if (rc) return rc;
-    }
-    return TRTX_OK;
+    if ((rc = check_launch())) return rc;
+    return launch_frames(centernet_select_kernel, a, a.base, batch, kCnSelectThreads, 0, st, frame_wh(frame_wh_host),
+                         [&](int j, int w, int h) {
+                             const int L = max(max(h, w), 3);  // max(image.shape): the channel count takes part
+                             a.scale[j] = (float)((double)p->down * ((double)L / (double)p->net));
+                         });
 }
 
 TRTX_API int trtx_centernet_preprocess_enqueue(const trtx_image_desc* images_host, int batch, int net, float* dst_dev,
@@ -447,8 +430,8 @@ TRTX_API int trtx_centernet_preprocess_enqueue(const trtx_image_desc* images_hos
     if (net > kCnMaxNet) return TRTX_ERR_UNSUPPORTED;
     CnPreArgs a;
     a.net = net;
-    for (int i0 = 0; i0 < batch; i0 += kCnMaxPreImages) {
-        const int n = min(batch - i0, kCnMaxPreImages);
+    for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {
+        const int n = min(batch - i0, kMaxFrames);
         a.base = i0;
         for (int j = 0; j < n; ++j) {
             const trtx_image_desc& d = images_host[i0 + j];

@@ -92,11 +92,7 @@ TRTX_API int trtx_cls_postprocess_enqueue(int softmax, int batch, int num_classe
     while (a.sort_n < a.kk) a.sort_n <<= 1;
     a.softmax = softmax;
     const size_t smem = (size_t)a.sort_n * sizeof(unsigned long long) + (size_t)num_classes * sizeof(float);
-    if (smem > 48 * 1024 &&
-        cudaFuncSetAttribute(cls_postprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-        g_last_cuda_error = (int)cudaGetLastError();
-        return TRTX_ERR_CUDA;
-    }
+    if (const int rc = opt_in_smem(cls_postprocess_kernel, smem)) return rc;
     cls_postprocess_kernel<<<(unsigned)batch, kSelThreads, smem, static_cast<cudaStream_t>(stream)>>>(a);
     return check_launch();
 }

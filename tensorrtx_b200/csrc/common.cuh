@@ -25,6 +25,16 @@ inline int check_launch() {
     return TRTX_OK;
 }
 
+// Opts `kernel` in to `smem` bytes of dynamic shared memory, which a launch may use without that only up to 48 KiB;
+// TRTX_ERR_CUDA, the error in g_last_cuda_error, where the attribute is refused.
+template <class Kernel>
+inline int opt_in_smem(Kernel* kernel, size_t smem) {
+    if (smem <= 48 * 1024 || cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess)
+        return TRTX_OK;
+    g_last_cuda_error = (int)cudaGetLastError();
+    return TRTX_ERR_CUDA;
+}
+
 // The frame descriptors every pre-process accepts: non-null u8 HWC BGR frames of positive size whose rows hold 3 * width bytes.
 inline bool valid_images(const trtx_image_desc* images, int n) {
     for (int i = 0; i < n; ++i) {
@@ -32,6 +42,60 @@ inline bool valid_images(const trtx_image_desc* images, int n) {
         if (!d.data_dev || d.width <= 0 || d.height <= 0 || d.pitch < 3 * d.width) return false;
     }
     return true;
+}
+
+// Frames (or image descriptors) per launch of a per-frame entry: their data rides in the kernel's parameter block.
+constexpr int kMaxFrames = 64;
+
+// The sizes of the frames of one launch of a per-frame post-process, one CTA per frame.
+struct FrameSizes {
+    int w[kMaxFrames], h[kMaxFrames];  // of frame base + blockIdx.x
+    int base;                          // frames [base, base + gridDim.x) of the call
+};
+
+// A per-frame post-process's frame_wh_host: `batch` (w, h) pairs in host memory, every side positive.
+inline bool frames_valid(const int32_t* frame_wh_host, int batch) {
+    for (int i = 0; i < batch; ++i)
+        if (frame_wh_host[2 * i] <= 0 || frame_wh_host[2 * i + 1] <= 0) return false;
+    return true;
+}
+
+// The size source of launch_frames for a frame_wh_host: frame i's (w, h), or 0 x 0 where frame_wh_host is null (a call
+// without frame rows).
+inline auto frame_wh(const int32_t* frame_wh_host) {
+    return [frame_wh_host](int i, int& w, int& h) {
+        w = frame_wh_host ? frame_wh_host[2 * i] : 0;
+        h = frame_wh_host ? frame_wh_host[2 * i + 1] : 0;
+    };
+}
+
+// One launch of `kernel` per <= kMaxFrames frames of a call, one CTA of `threads` per frame.  Before each launch, `base`
+// gets the launch's first frame i0, and for frame j of the launch, frame i0 + j of the call, size(i0 + j, w, h) gives its
+// size and frame(j, w, h) fills the caller's launch parameters.
+template <class Args, class Size, class Frame>
+int launch_frames(void (*kernel)(Args), Args& a, int& base, int batch, int threads, size_t smem, cudaStream_t st, Size size,
+                  Frame frame) {
+    for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {
+        const int n = min(batch - i0, kMaxFrames);
+        base = i0;
+        for (int j = 0; j < n; ++j) {
+            int w, h;
+            size(i0 + j, w, h);
+            frame(j, w, h);
+        }
+        kernel<<<n, threads, smem, st>>>(a);
+        const int rc = check_launch();
+        if (rc) return rc;
+    }
+    return TRTX_OK;
+}
+
+// The same where a frame's launch parameters are its size alone, in `sizes`.
+template <class Args, class Size>
+int launch_frames(void (*kernel)(Args), Args& a, FrameSizes& sizes, int batch, int threads, size_t smem, cudaStream_t st,
+                  Size size) {
+    return launch_frames(kernel, a, sizes.base, batch, threads, smem, st, size,
+                         [&](int j, int w, int h) { sizes.w[j] = w, sizes.h[j] = h; });
 }
 
 // ---- streaming loads: read-once data bypasses L1 allocation (guide: Guideline 13/14) ----

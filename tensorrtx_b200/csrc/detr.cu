@@ -20,18 +20,16 @@ namespace trtx {
 
 constexpr int kDetrThreads = 1024;  // queries per pass: 32 warps, so that DETR's 100 queries take 3 to 4 argmaxes per warp
 constexpr int kDetrWarps = kDetrThreads / kWarp;
-constexpr int kDetrMaxFrames = 64;  // frames per launch (launch-parameter arrays)
 constexpr int kDetrRow = 6;         // x, y, w, h, score, class
 constexpr int kDetrMaxDim = 1 << 24;  // Q and C: the count and the class are stored as floats, exact up to 2^24
 
 struct DetrPostArgs {
-    int img_w[kDetrMaxFrames], img_h[kDetrMaxFrames];
+    FrameSizes sizes;
+    int num_queries, num_classes;
+    float score_thresh;
     const float* scores;  // [B, Q, C]
     const float* boxes;   // [B, Q, 4]
     float* rows;          // [B, 1 + Q * 6]
-    int base;             // frames [base, base + gridDim.x) of the call
-    int num_queries, num_classes;
-    float score_thresh;
 };
 
 __global__ void __launch_bounds__(kDetrThreads) detr_postprocess_kernel(const __grid_constant__ DetrPostArgs a) {
@@ -40,8 +38,8 @@ __global__ void __launch_bounds__(kDetrThreads) detr_postprocess_kernel(const __
     __shared__ int s_src[kDetrThreads];       // query of the pass of each kept slot
     __shared__ int s_rect[kDetrThreads][4];   // its rectangle
     __shared__ int s_warp[kDetrWarps];        // kept queries per warp of the pass
-    const int tid = threadIdx.x, lane = tid & (kWarp - 1), warp = tid / kWarp, b = a.base + blockIdx.x;
-    const int Q = a.num_queries, C = a.num_classes, img_w = a.img_w[blockIdx.x], img_h = a.img_h[blockIdx.x];
+    const int tid = threadIdx.x, lane = tid & (kWarp - 1), warp = tid / kWarp, b = a.sizes.base + blockIdx.x;
+    const int Q = a.num_queries, C = a.num_classes, img_w = a.sizes.w[blockIdx.x], img_h = a.sizes.h[blockIdx.x];
     const float* scores = a.scores + (size_t)b * Q * C;
     const float* boxes = a.boxes + (size_t)b * Q * 4;
     float* out = a.rows + (size_t)b * (1 + (size_t)Q * kDetrRow);
@@ -116,9 +114,7 @@ TRTX_API int trtx_detr_postprocess_enqueue(const trtx_detr_post_params* p, const
     if (!p || !frame_wh_host || batch <= 0 || !scores_dev || !boxes_dev || !rows_dev) return TRTX_ERR_INVALID;
     // a threshold below -1 would keep the queries whose argmax the reference leaves at label -1, score -1
     if (p->num_queries <= 0 || p->num_classes < 2 || !(p->score_thresh >= -1.f)) return TRTX_ERR_INVALID;
-    // every frame size is checked before the first launch, so that a rejected call writes nothing
-    for (int i = 0; i < batch; ++i)
-        if (frame_wh_host[2 * i] <= 0 || frame_wh_host[2 * i + 1] <= 0) return TRTX_ERR_INVALID;
+    if (!frames_valid(frame_wh_host, batch)) return TRTX_ERR_INVALID;
     if (p->num_queries > kDetrMaxDim || p->num_classes > kDetrMaxDim) return TRTX_ERR_UNSUPPORTED;
     DetrPostArgs a;
     a.scores = scores_dev;
@@ -127,15 +123,8 @@ TRTX_API int trtx_detr_postprocess_enqueue(const trtx_detr_post_params* p, const
     a.num_queries = p->num_queries;
     a.num_classes = p->num_classes;
     a.score_thresh = p->score_thresh;
-    for (int i0 = 0; i0 < batch; i0 += kDetrMaxFrames) {
-        const int n = min(batch - i0, kDetrMaxFrames);
-        a.base = i0;
-        for (int j = 0; j < n; ++j) a.img_w[j] = frame_wh_host[2 * (i0 + j)], a.img_h[j] = frame_wh_host[2 * (i0 + j) + 1];
-        detr_postprocess_kernel<<<n, kDetrThreads, 0, static_cast<cudaStream_t>(stream)>>>(a);
-        const int rc = check_launch();
-        if (rc) return rc;
-    }
-    return TRTX_OK;
+    return launch_frames(detr_postprocess_kernel, a, a.sizes, batch, kDetrThreads, 0, static_cast<cudaStream_t>(stream),
+                         frame_wh(frame_wh_host));
 }
 
 }  // extern "C"

@@ -26,7 +26,6 @@ namespace trtx {
 constexpr int kMaskTile = 16;                // low-resolution cells per CTA edge
 constexpr int kMaskHalo = kMaskTile + 2;     // + one cell on each side for the bilinear taps
 constexpr int kMaxCoeffs = 64;
-constexpr int kMaxFrames = 64;               // frames per launch of the per-frame entries (launch-parameter arrays)
 
 struct MaskArgs {
     const float* proto;  // [B, nm, mh, mw]
@@ -1059,11 +1058,10 @@ constexpr int kPoseMaxKpts = 64;
 
 // What every launch of a per-row post-process carries besides the policy's own parameters.
 struct RowFrames {
-    int img_w[kMaxFrames], img_h[kMaxFrames];
+    FrameSizes sizes;   // its base next to row_floats: the prologue loads the two as one pair
+    int row_floats, out_floats, max_rows;
     const float* dets;  // [B, 1 + max_rows * row_floats]
     float* rows;        // [B, 1 + max_rows * out_floats]
-    int base;           // frames [base, base + gridDim.x) of the call
-    int row_floats, out_floats, max_rows;
 };
 
 template <class Row, class Args>
@@ -1072,7 +1070,7 @@ __device__ __forceinline__ void frame_rows(const Args& args) {
     __shared__ int s_src[kRowsThreads];               // input row of each used row of the pass, by output slot
     __shared__ int s_geo[kRowsThreads * Row::kGeo];   // its geometry
     __shared__ int s_warp[kRowsWarps];                // used rows per warp of the pass
-    const int tid = threadIdx.x, lane = tid & (kWarp - 1), warp = tid / kWarp, b = a.base + blockIdx.x;
+    const int tid = threadIdx.x, lane = tid & (kWarp - 1), warp = tid / kWarp, b = a.sizes.base + blockIdx.x;
     const size_t R = (size_t)a.row_floats, F = (size_t)a.out_floats;
     const float* src = a.dets + (size_t)b * (1 + (size_t)a.max_rows * R);
     float* out = a.rows + (size_t)b * (1 + (size_t)a.max_rows * F);
@@ -1133,7 +1131,7 @@ struct PoseObbRow {
     YoloLetterbox lb;
     int geo;  // floats of the output row before conf and class
     __device__ PoseObbRow(const PoseObbArgs& args, int j)
-        : a(args), img_w(args.f.img_w[j]), img_h(args.f.img_h[j]),
+        : a(args), img_w(args.f.sizes.w[j]), img_h(args.f.sizes.h[j]),
           lb(yolo_letterbox(args.net_w, args.net_h, img_w, img_h)), geo(args.pose ? 4 : 8) {}
     // process_decode_ptr_host: `int keep_flag = ...; if (keep_flag == 1)`; yolo26's batch_decode_obb takes every row
     __device__ bool pass(const float* d) const { return a.nms_free || (int)d[6] == 1; }
@@ -1173,7 +1171,7 @@ struct FaceRow {
     const FaceArgs& a;
     YoloLetterbox lb;
     __device__ FaceRow(const FaceArgs& args, int j)
-        : a(args), lb(yolo_letterbox(args.in_w, args.in_h, args.f.img_w[j], args.f.img_h[j])) {}
+        : a(args), lb(yolo_letterbox(args.in_w, args.in_h, args.f.sizes.w[j], args.f.sizes.h[j])) {}
     // `if (res[j].class_confidence < CONF_THRESH) continue;`: a NaN confidence is kept
     __device__ bool pass(const float* d) const { return (int)d[6] == 1 && !(d[4] < a.conf_thresh); }
     __device__ void geometry(const float* d, int g[4]) const { retina_get_rect(lb, d, g); }
@@ -1200,7 +1198,7 @@ struct YolopRowsArgs {
 struct YolopRow {
     static constexpr int kGeo = 4;  // the rectangle
     YoloLetterbox lb;
-    __device__ YolopRow(const YolopRowsArgs& args, int j) : lb(yolo_letterbox(args.net_w, args.net_h, args.f.img_w[j], args.f.img_h[j])) {}
+    __device__ YolopRow(const YolopRowsArgs& args, int j) : lb(yolo_letterbox(args.net_w, args.net_h, args.f.sizes.w[j], args.f.sizes.h[j])) {}
     __device__ bool pass(const float* d) const { return (int)d[6] == 1; }  // every row of a greedy NMS output
     __device__ void geometry(const float* d, int g[4]) const { yolop_get_rect(lb, d, g); }
     __device__ float value(const float* d, const int* g, int e) const { return e < 4 ? (float)g[e] : d[e]; }  // conf, class
@@ -1222,7 +1220,7 @@ struct TopkRow {
     static constexpr int kGeo = 4;  // the rectangle
     const TopkArgs& a;
     int img_w, img_h;
-    __device__ TopkRow(const TopkArgs& args, int j) : a(args), img_w(args.f.img_w[j]), img_h(args.f.img_h[j]) {}
+    __device__ TopkRow(const TopkArgs& args, int j) : a(args), img_w(args.f.sizes.w[j]), img_h(args.f.sizes.h[j]) {}
     // `if (output[1 + det_size * i + 4] <= conf_thresh) continue;`: a NaN confidence is kept
     __device__ bool pass(const float* d) const { return !(d[4] <= a.conf_thresh); }
     // the variant as a literal in each call, so that only its own branch of yolo_get_rect is compiled
@@ -1320,33 +1318,6 @@ __global__ void __launch_bounds__(kLabelThreads) yolop_label_kernel(const __grid
             *reinterpret_cast<uint4*>(row + head + 16 * q) = *reinterpret_cast<const uint4*>(stage + head + pad + 16 * q);
         __syncwarp();  // the next row reuses the stage
     }
-}
-
-// Every frame size of a per-row call is checked before the first launch, so that a rejected call writes nothing.
-inline bool frames_valid(const int32_t* frame_wh_host, int batch) {
-    for (int i = 0; i < batch; ++i)
-        if (frame_wh_host[2 * i] <= 0 || frame_wh_host[2 * i + 1] <= 0) return false;
-    return true;
-}
-
-// One launch of `kernel` per <= kMaxFrames frames, each with its frames' sizes in the launch parameters: size(i, w, h) gives
-// frame i's.
-template <class Args, class Size>
-int launch_frame_rows(void (*kernel)(Args), Args& a, Size size, int batch, cudaStream_t st) {
-    for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {
-        const int n = min(batch - i0, kMaxFrames);
-        a.f.base = i0;
-        for (int j = 0; j < n; ++j) size(i0 + j, a.f.img_w[j], a.f.img_h[j]);
-        kernel<<<n, kRowsThreads, 0, st>>>(a);
-        const int rc = check_launch();
-        if (rc) return rc;
-    }
-    return TRTX_OK;
-}
-template <class Args>
-int launch_frame_rows(void (*kernel)(Args), Args& a, const int32_t* frame_wh_host, int batch, cudaStream_t st) {
-    return launch_frame_rows(kernel, a, [&](int i, int& w, int& h) { w = frame_wh_host[2 * i], h = frame_wh_host[2 * i + 1]; },
-                             batch, st);
 }
 
 }  // namespace trtx
@@ -1539,15 +1510,18 @@ TRTX_API int trtx_rcnn_postprocess_frames_enqueue(const trtx_rcnn_post_params* p
 }
 
 // The slots of a trtx_rcnn_contours_enqueue call and the bytes of one (sized for its largest frame); TRTX_ERR_INVALID /
-// TRTX_ERR_UNSUPPORTED as documented there.
+// TRTX_ERR_UNSUPPORTED as documented there, in two passes over the frames so that TRTX_ERR_INVALID wins.
 static int contour_plan(const trtx_rcnn_post_params* p, const trtx_frame* frames, int batch, int& slots,
                         long long& map_bytes, long long& list_bytes, long long& slot_bytes) {
     if (!p || !frames || batch <= 0 || p->detections_per_im <= 0 || p->max_masks <= 0) return TRTX_ERR_INVALID;
+    for (int i = 0; i < batch; ++i) {
+        const trtx_frame& d = frames[i];
+        if (!d.masks_dev || d.img_w <= 0 || d.img_h <= 0 || d.pitch < d.img_w) return TRTX_ERR_INVALID;
+    }
     long long band_bytes = 0;
     map_bytes = list_bytes = 0;
     for (int i = 0; i < batch; ++i) {
         const trtx_frame& d = frames[i];
-        if (!d.masks_dev || d.img_w <= 0 || d.img_h <= 0 || d.pitch < d.img_w) return TRTX_ERR_INVALID;
         if ((long long)(d.img_w + 2) * (d.img_h + 2) > (1LL << 29)) return TRTX_ERR_UNSUPPORTED;
         long long mb, lb, bb;
         contour_regions(d.img_w, d.img_h, mb, lb, bb);
@@ -1576,7 +1550,7 @@ TRTX_API int trtx_rcnn_contours_enqueue(const trtx_rcnn_post_params* p, const tr
     if (reinterpret_cast<uintptr_t>(workspace_dev) & 15) return TRTX_ERR_INVALID;
     int slots;
     long long map_bytes, list_bytes, slot_bytes;
-    const int rc = contour_plan(p, images_host, batch, slots, map_bytes, list_bytes, slot_bytes);
+    int rc = contour_plan(p, images_host, batch, slots, map_bytes, list_bytes, slot_bytes);
     if (rc) return rc;
     if (workspace_bytes < (size_t)slots * (size_t)slot_bytes) return TRTX_ERR_WORKSPACE;
     ContourArgs a;
@@ -1592,11 +1566,7 @@ TRTX_API int trtx_rcnn_contours_enqueue(const trtx_rcnn_post_params* p, const tr
     a.max_masks = p->max_masks;
     a.max_contours = max_contours;
     a.max_points = max_points;
-    if (cudaFuncSetAttribute(rcnn_contours_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kContourSmem) !=
-        cudaSuccess) {
-        g_last_cuda_error = (int)cudaGetLastError();
-        return TRTX_ERR_CUDA;
-    }
+    if ((rc = opt_in_smem(rcnn_contours_kernel, kContourSmem))) return rc;
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {
         const int n = min(batch - i0, kMaxFrames);
@@ -1607,8 +1577,7 @@ TRTX_API int trtx_rcnn_contours_enqueue(const trtx_rcnn_post_params* p, const tr
         a.base = i0;
         a.n_images = n;
         rcnn_contours_kernel<<<(unsigned)min(n * p->max_masks, kContourCtas), kContourThreads, kContourSmem, st>>>(a);
-        const int r = check_launch();
-        if (r) return r;
+        if ((rc = check_launch())) return rc;
     }
     return TRTX_OK;
 }
@@ -1653,11 +1622,7 @@ TRTX_API int trtx_yolo_seg_postprocess_enqueue(const trtx_mask_params* p, const 
         if ((rc = seg_fill_frames(p, images_host, i0, min(batch - i0, kMaxFrames), masks, a, ctas, smem))) return rc;
         smem_max = max(smem_max, smem);
     }
-    if (smem_max > 48 * 1024 &&
-        cudaFuncSetAttribute(seg_canvas_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) != cudaSuccess) {
-        g_last_cuda_error = (int)cudaGetLastError();
-        return TRTX_ERR_CUDA;
-    }
+    if ((rc = opt_in_smem(seg_canvas_kernel, smem_max))) return rc;
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {
         const int n = min(batch - i0, kMaxFrames);
@@ -1719,7 +1684,8 @@ TRTX_API int trtx_yolo_pose_obb_postprocess_enqueue(const trtx_pose_obb_params* 
     a.net_h = p->net_h;
     a.extra_offset = p->extra_offset;
     a.num_kpts = pose ? p->num_kpts : 0;
-    return launch_frame_rows(pose_obb_rows_kernel, a, frame_wh_host, batch, static_cast<cudaStream_t>(stream));
+    return launch_frames(pose_obb_rows_kernel, a, a.f.sizes, batch, kRowsThreads, 0, static_cast<cudaStream_t>(stream),
+                         frame_wh(frame_wh_host));
 }
 
 TRTX_API int trtx_retina_postprocess_enqueue(const trtx_face_post_params* p, const int32_t* frame_wh_host, int batch,
@@ -1740,7 +1706,8 @@ TRTX_API int trtx_retina_postprocess_enqueue(const trtx_face_post_params* p, con
     a.in_h = p->in_h;
     a.lmk_offset = p->lmk_offset;
     a.conf_thresh = p->conf_thresh;
-    return launch_frame_rows(face_rows_kernel, a, frame_wh_host, batch, static_cast<cudaStream_t>(stream));
+    return launch_frames(face_rows_kernel, a, a.f.sizes, batch, kRowsThreads, 0, static_cast<cudaStream_t>(stream),
+                         frame_wh(frame_wh_host));
 }
 
 TRTX_API int trtx_yolo_topk_postprocess_enqueue(const trtx_yolo_topk_params* p, const int32_t* frame_wh_host, int batch,
@@ -1759,7 +1726,8 @@ TRTX_API int trtx_yolo_topk_postprocess_enqueue(const trtx_yolo_topk_params* p, 
     a.net_w = p->net_w;
     a.net_h = p->net_h;
     a.conf_thresh = p->conf_thresh;
-    return launch_frame_rows(topk_rows_kernel, a, frame_wh_host, batch, static_cast<cudaStream_t>(stream));
+    return launch_frames(topk_rows_kernel, a, a.f.sizes, batch, kRowsThreads, 0, static_cast<cudaStream_t>(stream),
+                         frame_wh(frame_wh_host));
 }
 
 TRTX_API int trtx_yolop_postprocess_enqueue(const trtx_yolop_post_params* p, const trtx_frame* frames_host, int batch,
@@ -1780,11 +1748,8 @@ TRTX_API int trtx_yolop_postprocess_enqueue(const trtx_yolop_post_params* p, con
     const int sx_bytes = (int)align_up(2 * (size_t)w_max, 16), stage_bytes = (int)align_up((size_t)w_max + 15, 16);
     const size_t smem = (size_t)sx_bytes + align_up((size_t)kLabelBand * p->map_w, 16) + (size_t)kLabelWarps * stage_bytes;
     if (labels && smem > 227 * 1024) return TRTX_ERR_UNSUPPORTED;
-    if (labels && smem > 48 * 1024 &&
-        cudaFuncSetAttribute(yolop_label_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-        g_last_cuda_error = (int)cudaGetLastError();
-        return TRTX_ERR_CUDA;
-    }
+    int rc = labels ? opt_in_smem(yolop_label_kernel, smem) : TRTX_OK;
+    if (rc) return rc;
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     YolopRowsArgs r;
     r.f.dets = dets_dev;
@@ -1794,8 +1759,8 @@ TRTX_API int trtx_yolop_postprocess_enqueue(const trtx_yolop_post_params* p, con
     r.f.max_rows = max_rows;
     r.net_w = p->net_w;
     r.net_h = p->net_h;
-    int rc = launch_frame_rows(yolop_rows_kernel, r, [&](int i, int& w, int& h) { w = frames_host[i].img_w, h = frames_host[i].img_h; },
-                               batch, st);
+    rc = launch_frames(yolop_rows_kernel, r, r.f.sizes, batch, kRowsThreads, 0, st,
+                       [&](int i, int& w, int& h) { w = frames_host[i].img_w, h = frames_host[i].img_h; });
     if (rc || !labels) return rc;
     YolopLabelArgs a;
     a.seg = seg_dev;

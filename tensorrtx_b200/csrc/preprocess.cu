@@ -211,7 +211,6 @@ __global__ void __launch_bounds__(256, 8) letterbox_kernel(const __grid_constant
 // short-lived (one band each, 10 KB of shared memory at 640 columns), so SMs free up for concurrent work as the grid drains.
 constexpr int kUnitBand = 4;             // destination rows per CTA (8 measured slower)
 constexpr int kUnitBoxBytes = 256;       // TMA inner box extent: the most one box may span
-constexpr int kMaxUnitImages = 64;
 constexpr int kUnitMaxThreads = 160;     // 640 columns = 160 threads x 4 pixels; wider inputs loop
 
 struct UnitImage {
@@ -222,8 +221,8 @@ struct UnitImage {
     float lx, ly;  // bilinear fractions (0 or 0.5), constant over the image
 };
 struct alignas(64) UnitArgs {
-    CUtensorMap map[kMaxUnitImages];
-    UnitImage img[kMaxUnitImages];
+    CUtensorMap map[kMaxFrames];
+    UnitImage img[kMaxFrames];
     int dw, dh;
     int nbox;  // boxes per window row: nbox * kUnitBoxBytes >= 3 * dw + 4 (the last thread's 16 bytes)
 };
@@ -357,10 +356,7 @@ static bool encode_image_map(CUtensorMap* map, const uint8_t* base, int sw, int 
 template <typename OutT>
 static int launch_unit_t(const UnitArgs& a, int n, size_t smem, OutT* dst, cudaStream_t st) {
     auto* k = letterbox_unit_kernel<OutT, kUnitBand>;
-    if (smem > 48 * 1024 && cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-        cudaGetLastError();
-        return TRTX_ERR_UNSUPPORTED;
-    }
+    if (opt_in_smem(k, smem)) return TRTX_ERR_UNSUPPORTED;
     const int threads = min((a.dw / 4 + kWarp - 1) / kWarp * kWarp, kUnitMaxThreads);
     k<<<dim3((a.dh + kUnitBand - 1) / kUnitBand, n), threads, smem, st>>>(a, dst);
     return check_launch();
@@ -424,7 +420,6 @@ static int launch_unit(const trtx_image_desc* const* d, UnitImage* u, int n, voi
 constexpr int kBandRows = 4;              // destination rows per CTA
 constexpr int kBandSlots = 2 * kBandRows;  // staged source rows: two taps per destination row at most
 constexpr int kBandThreads = 256;
-constexpr int kMaxBandImages = 64;         // descriptors per launch (kernel parameter block)
 
 struct BandImage {
     const uint8_t* src;
@@ -434,7 +429,7 @@ struct BandImage {
     int dst_idx;
 };
 struct BandArgs {
-    BandImage img[kMaxBandImages];
+    BandImage img[kMaxFrames];
     int net_w, net_h, bands;
     int stride;               // staged elements per row: 3 * the widest rectangle of the launch
 };
@@ -920,7 +915,7 @@ __global__ void __launch_bounds__(kBandThreads) band_preprocess_kernel(const __g
 
 // Checks the call in two passes before the first launch, so that a rejected call writes nothing and TRTX_ERR_INVALID wins over
 // TRTX_ERR_UNSUPPORTED: first the arguments and every descriptor (TRTX_ERR_INVALID), then every frame's descriptor from
-// make(i, im) (what make returns) and every launch's shared memory (TRTX_ERR_UNSUPPORTED).  Then one launch per kMaxBandImages
+// make(i, im) (what make returns) and every launch's shared memory (TRTX_ERR_UNSUPPORTED).  Then one launch per kMaxFrames
 // frames, a CTA per band of each.
 template <class Resize, class Store, class Make>
 static int band_preprocess(const trtx_image_desc* images_host, int batch, int net_w, int net_h, float* dst_dev,
@@ -947,16 +942,12 @@ static int band_preprocess(const trtx_image_desc* images_host, int batch, int ne
         return (size_t)slots * a.stride * sizeof(typename Resize::Staged);
     };
     size_t smem_max = 0;
-    for (int i0 = 0; i0 < batch; i0 += kMaxBandImages) smem_max = max(smem_max, fill(i0, min(batch - i0, kMaxBandImages)));
+    for (int i0 = 0; i0 < batch; i0 += kMaxFrames) smem_max = max(smem_max, fill(i0, min(batch - i0, kMaxFrames)));
     if (smem_max > Store::kMaxDynamicSmem) return TRTX_ERR_UNSUPPORTED;
     auto* kernel = band_preprocess_kernel<Resize, Store>;
-    if (smem_max > 48 * 1024 &&
-        cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) != cudaSuccess) {
-        g_last_cuda_error = (int)cudaGetLastError();
-        return TRTX_ERR_CUDA;
-    }
-    for (int i0 = 0; i0 < batch; i0 += kMaxBandImages) {
-        const int n = min(batch - i0, kMaxBandImages);
+    if (const int rc = opt_in_smem(kernel, smem_max)) return rc;
+    for (int i0 = 0; i0 < batch; i0 += kMaxFrames) {
+        const int n = min(batch - i0, kMaxFrames);
         const size_t smem = fill(i0, n);
         kernel<<<(unsigned)(n * a.bands), kBandThreads, smem, static_cast<cudaStream_t>(stream)>>>(a, dst_dev);
         if (const int rc = check_launch()) return rc;
@@ -1095,8 +1086,8 @@ TRTX_API int trtx_preprocess_batch_enqueue(const trtx_image_desc* images_host, i
     g.dw = dst_w;
     g.dh = dst_h;
     int ng = 0;
-    const trtx_image_desc* ud[kMaxUnitImages];
-    UnitImage uu[kMaxUnitImages];
+    const trtx_image_desc* ud[kMaxFrames];
+    UnitImage uu[kMaxFrames];
     int nu = 0;
     auto flush_general = [&]() -> int {
         if (!ng) return TRTX_OK;
@@ -1139,7 +1130,7 @@ TRTX_API int trtx_preprocess_batch_enqueue(const trtx_image_desc* images_host, i
         if (unit_ok && unit_scale_image(d, m, &uu[nu])) {
             ud[nu] = &d;
             uu[nu].dst_idx = i;
-            if (++nu == kMaxUnitImages) rc = flush_unit();
+            if (++nu == kMaxFrames) rc = flush_unit();
         } else {
             rc = add_general(i);
         }

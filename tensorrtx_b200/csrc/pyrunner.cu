@@ -24,7 +24,6 @@ constexpr int kPyThreads = kSelThreads;        // 1024
 constexpr int kPyMaxRows = TRTX_NMS_MAX_ROWS;  // 2048
 constexpr int kPyWords = kPyMaxRows / 64;      // 32: the removed set fits one warp, a 64-bit word per lane
 constexpr int kPyChunk = 64;                   // sorted rows per sweep step: one mask word
-constexpr int kPyMaxFrames = 64;               // frames per launch (launch-parameter arrays)
 constexpr int kPyRow = 6;
 
 // xywh2xyxy's geometry of one frame, computed on the host in double as Python does and rounded to float as numpy casts a
@@ -36,7 +35,7 @@ struct PyFrame {
 };
 
 struct PyArgs {
-    PyFrame fr[kPyMaxFrames];
+    PyFrame fr[kMaxFrames];
     const float* dets;  // [B, 1 + max_rows * row_floats]
     float* rows;        // [B, 1 + max_rows * 6]
     int base, max_rows, row_floats, label_col, conf_col, cxcywh;
@@ -204,14 +203,10 @@ TRTX_API int trtx_pyrunner_postprocess_enqueue(const trtx_pyrunner_params* p, co
     if (p->conf_thresh != p->conf_thresh || p->nms_thresh != p->nms_thresh) return TRTX_ERR_INVALID;
     if (reinterpret_cast<uintptr_t>(dets_dev) % sizeof(float) || reinterpret_cast<uintptr_t>(rows_dev) % sizeof(float))
         return TRTX_ERR_INVALID;
+    if (!frames_valid(frame_wh_host, batch)) return TRTX_ERR_INVALID;
     if (max_rows > kPyMaxRows) return TRTX_ERR_UNSUPPORTED;
-    for (int i = 0; i < batch; ++i)
-        if (frame_wh_host[2 * i] <= 0 || frame_wh_host[2 * i + 1] <= 0) return TRTX_ERR_INVALID;
     const size_t smem = py_smem(max_rows);
-    if (cudaFuncSetAttribute(pyrunner_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-        g_last_cuda_error = (int)cudaGetLastError();
-        return TRTX_ERR_CUDA;
-    }
+    if (const int rc = opt_in_smem(pyrunner_kernel, smem)) return rc;
     PyArgs a;
     memset(&a, 0, sizeof(a));
     a.dets = dets_dev;
@@ -223,25 +218,16 @@ TRTX_API int trtx_pyrunner_postprocess_enqueue(const trtx_pyrunner_params* p, co
     a.cxcywh = p->box_format == TRTX_BOX_CXCYWH;
     a.conf_thresh = p->conf_thresh;
     a.nms_thresh = p->nms_thresh;
-    const cudaStream_t st = static_cast<cudaStream_t>(stream);
-    for (int i0 = 0; i0 < batch; i0 += kPyMaxFrames) {
-        const int n = min(batch - i0, kPyMaxFrames);
-        a.base = i0;
-        for (int j = 0; j < n; ++j) {
-            const int w = frame_wh_host[2 * (i0 + j)], h = frame_wh_host[2 * (i0 + j) + 1];
-            const double r_w = (double)p->net_w / w, r_h = (double)p->net_h / h;
-            PyFrame& f = a.fr[j];
-            f.on_y = r_h > r_w;
-            f.pad = f.on_y ? (float)((p->net_h - r_w * h) / 2) : (float)((p->net_w - r_h * w) / 2);
-            f.r = f.on_y ? (float)r_w : (float)r_h;
-            f.xmax = (float)(w - 1);
-            f.ymax = (float)(h - 1);
-        }
-        pyrunner_kernel<<<n, kPyThreads, smem, st>>>(a);
-        const int rc = check_launch();
-        if (rc) return rc;
-    }
-    return TRTX_OK;
+    return launch_frames(pyrunner_kernel, a, a.base, batch, kPyThreads, smem, static_cast<cudaStream_t>(stream),
+                         frame_wh(frame_wh_host), [&](int j, int w, int h) {
+                             const double r_w = (double)p->net_w / w, r_h = (double)p->net_h / h;
+                             PyFrame& f = a.fr[j];
+                             f.on_y = r_h > r_w;
+                             f.pad = f.on_y ? (float)((p->net_h - r_w * h) / 2) : (float)((p->net_w - r_h * w) / 2);
+                             f.r = f.on_y ? (float)r_w : (float)r_h;
+                             f.xmax = (float)(w - 1);
+                             f.ymax = (float)(h - 1);
+                         });
 }
 
 }  // extern "C"

@@ -26,7 +26,6 @@ constexpr int kRdMaxPriors = 1 << 16;    // prior indices are stored as uint16
 constexpr int kRdMaxClasses = 1024;
 constexpr int kRdMaxDet = 1 << 24;       // counts are stored as floats
 constexpr int kRdMaxSide = 1 << 24;      // frame sides: rectangles are stored as floats
-constexpr int kRdMaxFrames = 64;         // frames per rows launch (launch-parameter arrays)
 constexpr int kRdRow = 6;
 
 struct RdArgs {
@@ -38,9 +37,10 @@ struct RdArgs {
     uint16_t* keep;         // workspace [B, C - 1, top_k]
     float* dets;            // [B, 1 + max_det * 6]
     float* rows;            // [B, 1 + max_det * 6] or null
-    int net, P, C, top_k, max_det, base;
+    int net, P, C, top_k;
+    FrameSizes sizes;       // rows launch: (cols, rows) of each frame, 0 without frame rows
+    int max_det;
     float obj_thresh, conf_thresh, nms_thresh, score_thresh;
-    int wh[2 * kRdMaxFrames];
 };
 
 // Priors of a square net S: levels k = 0..3 with step 8 << k, min_size 32 << k and f = S / step cells a side; prior index
@@ -214,7 +214,7 @@ __device__ __forceinline__ void rd_rect(const float box[4], int cols, int rows, 
 __global__ void __launch_bounds__(kRdRowsThreads) refinedet_rows_kernel(const __grid_constant__ RdArgs a) {
     __shared__ int s_off[kRdMaxClasses];  // s_off[k]: rows of classes 1..k
     __shared__ int s_warp[kRdRowsThreads / kWarp];
-    const int tid = threadIdx.x, b = a.base + blockIdx.x, ncls = a.C - 1, K = a.top_k;
+    const int tid = threadIdx.x, b = a.sizes.base + blockIdx.x, ncls = a.C - 1, K = a.top_k;
     const int32_t* cnt = a.count + (size_t)b * ncls;
     if (tid == 0) {
         int o = 0;
@@ -225,7 +225,7 @@ __global__ void __launch_bounds__(kRdRowsThreads) refinedet_rows_kernel(const __
     const int n = min(s_off[ncls], a.max_det), len = 1 + a.max_det * kRdRow;
     float* dets = a.dets + (size_t)b * len;
     float* rows = a.rows ? a.rows + (size_t)b * len : nullptr;
-    const int cols = a.wh[2 * blockIdx.x], frows = a.wh[2 * blockIdx.x + 1];
+    const int cols = a.sizes.w[blockIdx.x], frows = a.sizes.h[blockIdx.x];
     int kept = 0;
     for (int r0 = 0; r0 < n; r0 += kRdRowsThreads) {  // uniform
         const int r = r0 + tid;
@@ -289,21 +289,28 @@ using namespace trtx;
 
 extern "C" {
 
-// Everything in the parameters that can reject a post-process call, before the first launch; TRTX_OK or the error code.
-static int refinedet_check(const trtx_refinedet_params* p, int batch) {
+// Everything in the parameters and the frame sizes (frame_wh_host, may be null) that can reject a post-process call, before
+// the first launch, in two passes so that TRTX_ERR_INVALID wins; TRTX_OK or the error code.
+static int refinedet_check(const trtx_refinedet_params* p, int batch, const int32_t* frame_wh_host) {
     if (!p || batch <= 0) return TRTX_ERR_INVALID;
     if (p->net <= 0 || p->num_classes < 2 || p->top_k <= 0 || p->max_det <= 0) return TRTX_ERR_INVALID;
     if (p->obj_thresh != p->obj_thresh || p->conf_thresh != p->conf_thresh || p->nms_thresh != p->nms_thresh ||
         p->score_thresh != p->score_thresh)
         return TRTX_ERR_INVALID;
+    if (frame_wh_host && !frames_valid(frame_wh_host, batch)) return TRTX_ERR_INVALID;
     if (p->net % 64 != 0 || rd_num_priors(p->net) > kRdMaxPriors || p->top_k > kRdMaxTopK ||
         p->num_classes > kRdMaxClasses || p->max_det > kRdMaxDet)
         return TRTX_ERR_UNSUPPORTED;
+    for (int i = 0; frame_wh_host && i < batch; ++i) {
+        int w, h;
+        frame_wh(frame_wh_host)(i, w, h);
+        if (w > kRdMaxSide || h > kRdMaxSide) return TRTX_ERR_UNSUPPORTED;
+    }
     return TRTX_OK;
 }
 
 TRTX_API size_t trtx_refinedet_workspace_size(const trtx_refinedet_params* p, int batch) {
-    if (refinedet_check(p, batch) != TRTX_OK) return 0;
+    if (refinedet_check(p, batch, nullptr) != TRTX_OK) return 0;
     const size_t lists = (size_t)batch * (p->num_classes - 1);
     return align_up(lists * sizeof(int32_t)) + align_up(lists * p->top_k * sizeof(uint16_t));
 }
@@ -312,26 +319,16 @@ TRTX_API int trtx_refinedet_postprocess_enqueue(const trtx_refinedet_params* p, 
                                                 const float* arm_conf_dev, const float* odm_loc_dev, const float* odm_conf_dev,
                                                 void* workspace_dev, size_t workspace_bytes, float* dets_dev,
                                                 const int32_t* frame_wh_host, float* rows_dev, trtx_stream_t stream) {
-    const int rc0 = refinedet_check(p, batch);
-    if (rc0 != TRTX_OK) return rc0;
     if (!arm_loc_dev || !arm_conf_dev || !odm_loc_dev || !odm_conf_dev || !workspace_dev || !dets_dev) return TRTX_ERR_INVALID;
     if (!frame_wh_host != !rows_dev) return TRTX_ERR_INVALID;  // the frame rows need both
-    if (frame_wh_host) {
-        for (int i = 0; i < batch; ++i) {
-            const int w = frame_wh_host[2 * i], h = frame_wh_host[2 * i + 1];
-            if (w <= 0 || h <= 0) return TRTX_ERR_INVALID;
-            if (w > kRdMaxSide || h > kRdMaxSide) return TRTX_ERR_UNSUPPORTED;
-        }
-    }
-    if (workspace_bytes < trtx_refinedet_workspace_size(p, batch)) return TRTX_ERR_WORKSPACE;
     if (reinterpret_cast<uintptr_t>(workspace_dev) % kAlign) return TRTX_ERR_INVALID;
+    int rc = refinedet_check(p, batch, frame_wh_host);
+    if (rc) return rc;
+    if (workspace_bytes < trtx_refinedet_workspace_size(p, batch)) return TRTX_ERR_WORKSPACE;
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t smem = rd_nms_smem(p->top_k);
-    if (cudaFuncSetAttribute(refinedet_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-        g_last_cuda_error = (int)cudaGetLastError();
-        return TRTX_ERR_CUDA;
-    }
-    RdArgs a;
+    if ((rc = opt_in_smem(refinedet_nms_kernel, smem))) return rc;
+    RdArgs a{};
     a.arm_loc = arm_loc_dev;
     a.arm_conf = arm_conf_dev;
     a.odm_loc = odm_loc_dev;
@@ -350,23 +347,9 @@ TRTX_API int trtx_refinedet_postprocess_enqueue(const trtx_refinedet_params* p, 
     a.conf_thresh = p->conf_thresh;
     a.nms_thresh = p->nms_thresh;
     a.score_thresh = p->score_thresh;
-    a.base = 0;
-    for (int j = 0; j < 2 * kRdMaxFrames; ++j) a.wh[j] = 0;
     refinedet_nms_kernel<<<(unsigned)lists, kRdThreads, smem, st>>>(a);
-    int rc = check_launch();
-    if (rc) return rc;
-    for (int i0 = 0; i0 < batch; i0 += kRdMaxFrames) {
-        const int n = min(batch - i0, kRdMaxFrames);
-        a.base = i0;
-        for (int j = 0; frame_wh_host && j < n; ++j) {
-            a.wh[2 * j] = frame_wh_host[2 * (i0 + j)];
-            a.wh[2 * j + 1] = frame_wh_host[2 * (i0 + j) + 1];
-        }
-        refinedet_rows_kernel<<<n, kRdRowsThreads, 0, st>>>(a);
-        rc = check_launch();
-        if (rc) return rc;
-    }
-    return TRTX_OK;
+    if ((rc = check_launch())) return rc;
+    return launch_frames(refinedet_rows_kernel, a, a.sizes, batch, kRdRowsThreads, 0, st, frame_wh(frame_wh_host));
 }
 
 }  // extern "C"

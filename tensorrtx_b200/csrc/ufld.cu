@@ -22,18 +22,16 @@ namespace trtx {
 
 constexpr int kUfldThreads = 1024;        // H * W <= kUfldThreads: one thread per cell, one per draw position
 constexpr int kUfldWarps = kUfldThreads / kWarp;
-constexpr int kUfldMaxFrames = 64;        // frames per launch (launch-parameter arrays)
 constexpr int kUfldMaxTable = 52 * 1024;  // (C - 1) * H * W exponentials in dynamic shared memory (208 KiB)
 constexpr int kUfldMaxSide = 1 << 24;     // frame sides: the rows are exact floats
 constexpr int kUfldRow = 3;               // x, y, lane
 
 struct UfldPostArgs {
-    int out_w[kUfldMaxFrames], out_h[kUfldMaxFrames];
+    FrameSizes sizes;          // of the picture the points are for
+    int C, H, W, net_w, net_h, col_sample_w;
     int anchor[kUfldThreads];  // H row anchors
     const float* prob;         // [B, C, H, W]
     float* rows;               // [B, 1 + H * W * 3]
-    int base;                  // frames [base, base + gridDim.x) of the call
-    int C, H, W, net_w, net_h, col_sample_w;
 };
 
 // exp of a float as the double exp, rounded once to float: the correctly rounded expf except within about 2^-29 of a
@@ -45,7 +43,7 @@ __global__ void __launch_bounds__(kUfldThreads) ufld_postprocess_kernel(const __
     __shared__ float s_expect[kUfldThreads];     // per cell
     __shared__ unsigned char s_lane[kUfldThreads];  // lane kept
     __shared__ int s_warp[kUfldWarps];           // points per warp
-    const int tid = threadIdx.x, lane = tid & (kWarp - 1), warp = tid / kWarp, b = a.base + blockIdx.x;
+    const int tid = threadIdx.x, lane = tid & (kWarp - 1), warp = tid / kWarp, b = a.sizes.base + blockIdx.x;
     const int C = a.C, H = a.H, W = a.W, HW = H * W;
     const float* prob = a.prob + (size_t)b * C * HW;
     float* out = a.rows + (size_t)b * (1 + (size_t)HW * kUfldRow);
@@ -89,7 +87,7 @@ __global__ void __launch_bounds__(kUfldThreads) ufld_postprocess_kernel(const __
         total += c;
     }
     if (emit) {
-        const int ow = a.out_w[blockIdx.x], oh = a.out_h[blockIdx.x];
+        const int ow = a.sizes.w[blockIdx.x], oh = a.sizes.h[blockIdx.x];
         const float fx = __fdiv_rn(__fmul_rn(__fmul_rn(e, (float)a.col_sample_w), (float)ow), (float)a.net_w);
         const int x = (int)((uint32_t)trunc_to_int_x86(fx) - 1u);  // wraps as on x86-64
         const int y = oh * a.anchor[j] / a.net_h - 1;               // in range: checked on the host
@@ -114,42 +112,31 @@ TRTX_API int trtx_ufld_postprocess_enqueue(const trtx_ufld_post_params* p, const
     if (!p || !row_anchor_host || !frame_wh_host || batch <= 0 || !prob_dev || !rows_dev) return TRTX_ERR_INVALID;
     const int C = p->num_cells, H = p->num_rows, W = p->num_lanes;
     if (C < 2 || H <= 0 || W <= 0 || p->net_w <= 0 || p->net_h <= 0 || p->col_sample_w <= 0) return TRTX_ERR_INVALID;
-    for (int i = 0; i < batch; ++i)
-        if (frame_wh_host[2 * i] <= 0 || frame_wh_host[2 * i + 1] <= 0) return TRTX_ERR_INVALID;
+    if (!frames_valid(frame_wh_host, batch)) return TRTX_ERR_INVALID;
     if ((int64_t)H * W > kUfldThreads || (int64_t)(C - 1) * H * W > kUfldMaxTable) return TRTX_ERR_UNSUPPORTED;
     // every frame and anchor is checked before the first launch, so that a rejected call writes nothing: h * anchor must not
     // overflow int32 (the driver's int product), and the point's y must be an exact float
     for (int i = 0; i < batch; ++i) {
-        const int64_t w = frame_wh_host[2 * i], h = frame_wh_host[2 * i + 1];
+        int w, h;
+        frame_wh(frame_wh_host)(i, w, h);
         if (w > kUfldMaxSide || h > kUfldMaxSide) return TRTX_ERR_UNSUPPORTED;
         for (int j = 0; j < H; ++j) {
-            const int64_t prod = h * row_anchor_host[j];
+            const int64_t prod = (int64_t)h * row_anchor_host[j];
             if (prod < INT32_MIN || prod > INT32_MAX) return TRTX_ERR_UNSUPPORTED;
             const int64_t y = prod / p->net_h - 1;
             if (y < -kUfldMaxSide || y > kUfldMaxSide) return TRTX_ERR_UNSUPPORTED;
         }
     }
     const size_t smem = (size_t)(C - 1) * H * W * sizeof(float);
-    if (smem > 48 * 1024 &&
-        cudaFuncSetAttribute(ufld_postprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-        g_last_cuda_error = (int)cudaGetLastError();
-        return TRTX_ERR_CUDA;
-    }
+    if (const int rc = opt_in_smem(ufld_postprocess_kernel, smem)) return rc;
     UfldPostArgs a;
     a.prob = prob_dev;
     a.rows = rows_dev;
     a.C = C, a.H = H, a.W = W;
     a.net_w = p->net_w, a.net_h = p->net_h, a.col_sample_w = p->col_sample_w;
     for (int j = 0; j < H; ++j) a.anchor[j] = row_anchor_host[j];
-    for (int i0 = 0; i0 < batch; i0 += kUfldMaxFrames) {
-        const int n = min(batch - i0, kUfldMaxFrames);
-        a.base = i0;
-        for (int j = 0; j < n; ++j) a.out_w[j] = frame_wh_host[2 * (i0 + j)], a.out_h[j] = frame_wh_host[2 * (i0 + j) + 1];
-        ufld_postprocess_kernel<<<n, kUfldThreads, smem, static_cast<cudaStream_t>(stream)>>>(a);
-        const int rc = check_launch();
-        if (rc) return rc;
-    }
-    return TRTX_OK;
+    return launch_frames(ufld_postprocess_kernel, a, a.sizes, batch, kUfldThreads, smem, static_cast<cudaStream_t>(stream),
+                         frame_wh(frame_wh_host));
 }
 
 }  // extern "C"

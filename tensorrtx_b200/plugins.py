@@ -839,9 +839,11 @@ def _f32_rows(dets: torch.Tensor) -> None:
         raise ValueError("dets must be contiguous float32")
 
 
-def _frame_wh(image_sizes: Sequence[tuple[int, int]]):
-    """The per-row entries' host int32 array (img_w, img_h) of every frame."""
-    return (C.c_int32 * (2 * len(image_sizes)))(*[int(v) for s in image_sizes for v in s])
+def _frame_wh(image_sizes: Sequence[tuple[int, int]], batch: int):
+    """The per-frame post-processes' host int32 array (img_w, img_h) of each of the batch's frames."""
+    if len(image_sizes) != batch:
+        raise ValueError(f"expected {batch} image sizes")
+    return (C.c_int32 * (2 * batch))(*[int(v) for s in image_sizes for v in s])
 
 
 def yolo_seg_postprocess(proto: torch.Tensor | None, dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]], *,
@@ -914,7 +916,7 @@ def yolo_pose_obb_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[in
     q = L.PoseObbParams(task, net_w, net_h, row_floats, extra_offset, num_kpts)
     rows_out = _out_tensor(rows_out, (B, 1 + max_rows * F), torch.float32, dets.device,
                            f"rows_out must be contiguous float32 [{B}, {1 + max_rows * F}]")
-    L.check(lib.trtx_yolo_pose_obb_postprocess_enqueue(C.byref(q), _frame_wh(image_sizes), B, _ptr(dets), max_rows,
+    L.check(lib.trtx_yolo_pose_obb_postprocess_enqueue(C.byref(q), _frame_wh(image_sizes, B), B, _ptr(dets), max_rows,
                                                        _ptr(rows_out), _stream(stream)), "trtx_yolo_pose_obb_postprocess_enqueue")
     return rows_out
 
@@ -935,7 +937,7 @@ def yolo_topk_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[int, i
     q = L.YoloTopkParams(variant, net_w, net_h, row_floats, conf_thresh)
     rows_out = _out_tensor(rows_out, (B, 1 + max_rows * 6), torch.float32, dets.device,
                            f"rows_out must be contiguous float32 [{B}, {1 + max_rows * 6}]")
-    L.check(lib.trtx_yolo_topk_postprocess_enqueue(C.byref(q), _frame_wh(image_sizes), B, _ptr(dets), max_rows, _ptr(rows_out),
+    L.check(lib.trtx_yolo_topk_postprocess_enqueue(C.byref(q), _frame_wh(image_sizes, B), B, _ptr(dets), max_rows, _ptr(rows_out),
                                                    _stream(stream)), "trtx_yolo_topk_postprocess_enqueue")
     return rows_out
 
@@ -966,7 +968,7 @@ def retina_postprocess(dets: torch.Tensor, image_sizes: Sequence[tuple[int, int]
     q = L.FacePostParams(variant, in_w, in_h, row_floats, lmk_offset, float_ge_threshold(conf_thresh))
     rows_out = _out_tensor(rows_out, (B, 1 + max_rows * F), torch.float32, dets.device,
                            f"rows_out must be contiguous float32 [{B}, {1 + max_rows * F}]")
-    L.check(lib.trtx_retina_postprocess_enqueue(C.byref(q), _frame_wh(image_sizes), B, _ptr(dets), max_rows, _ptr(rows_out),
+    L.check(lib.trtx_retina_postprocess_enqueue(C.byref(q), _frame_wh(image_sizes, B), B, _ptr(dets), max_rows, _ptr(rows_out),
                                                 _stream(stream)), "trtx_retina_postprocess_enqueue")
     return rows_out
 
@@ -1546,7 +1548,7 @@ def detr_postprocess(scores: torch.Tensor, boxes: torch.Tensor, image_sizes: Seq
     Q, Cn = int(scores.shape[1]), int(scores.shape[2])
     out = _out_tensor(out, (B, 1 + Q * 6), torch.float32, scores.device, f"out must be contiguous float32 [{B}, {1 + Q * 6}]")
     q = L.DetrPostParams(Q, Cn, score_thresh)
-    L.check(lib.trtx_detr_postprocess_enqueue(C.byref(q), _frame_wh(image_sizes), B, _ptr(scores), _ptr(boxes), _ptr(out),
+    L.check(lib.trtx_detr_postprocess_enqueue(C.byref(q), _frame_wh(image_sizes, B), B, _ptr(scores), _ptr(boxes), _ptr(out),
                                               _stream(stream)), "trtx_detr_postprocess_enqueue")
     return out
 
@@ -1592,9 +1594,7 @@ def centernet_decode(heat: torch.Tensor, wh: torch.Tensor, reg: torch.Tensor, k:
     out = _out_tensor(out, (B, k, 6), torch.float32, heat.device, f"out must be contiguous float32 [{B}, {k}, 6]")
     wh_arr = None
     if image_sizes is not None:
-        if len(image_sizes) != B:
-            raise ValueError(f"expected {B} image sizes")
-        wh_arr = _frame_wh(image_sizes)
+        wh_arr = _frame_wh(image_sizes, B)
         rows_out = _out_tensor(rows_out, (B, 1 + k * 6), torch.float32, heat.device,
                                f"rows_out must be contiguous float32 [{B}, {1 + k * 6}]")
     L.check(lib.trtx_centernet_decode_enqueue(C.byref(q), B, _ptr(heat), _ptr(wh), _ptr(reg), _ptr(workspace),
@@ -1636,13 +1636,14 @@ def ufld_postprocess(prob: torch.Tensor, image_sizes: Sequence[tuple[int, int]] 
     B, Cn, H, W = (int(v) for v in prob.shape)
     if image_sizes is None:
         image_sizes = [UFLD_VIS] * B
-    if len(image_sizes) != B or len(row_anchor) != H:
-        raise ValueError(f"expected {B} image sizes and {H} row anchors")
+    wh_arr = _frame_wh(image_sizes, B)
+    if len(row_anchor) != H:
+        raise ValueError(f"expected {H} row anchors")
     out = _out_tensor(out, (B, 1 + H * W * 3), torch.float32, prob.device,
                       f"out must be contiguous float32 [{B}, {1 + H * W * 3}]")
     q = L.UfldPostParams(Cn, H, W, net_w, net_h, col_sample_w)
     anchors = (C.c_int32 * H)(*[int(v) for v in row_anchor])
-    L.check(lib.trtx_ufld_postprocess_enqueue(C.byref(q), anchors, _frame_wh(image_sizes), B, _ptr(prob), _ptr(out),
+    L.check(lib.trtx_ufld_postprocess_enqueue(C.byref(q), anchors, wh_arr, B, _ptr(prob), _ptr(out),
                                               _stream(stream)), "trtx_ufld_postprocess_enqueue")
     return out
 
@@ -1704,9 +1705,7 @@ def refinedet_postprocess(arm_loc: torch.Tensor, arm_conf: torch.Tensor, odm_loc
     out = _out_tensor(out, (B, row), torch.float32, odm_conf.device, f"out must be contiguous float32 [{B}, {row}]")
     wh_arr = None
     if image_sizes is not None:
-        if len(image_sizes) != B:
-            raise ValueError(f"expected {B} image sizes")
-        wh_arr = _frame_wh(image_sizes)
+        wh_arr = _frame_wh(image_sizes, B)
         rows_out = _out_tensor(rows_out, (B, row), torch.float32, odm_conf.device,
                                f"rows_out must be contiguous float32 [{B}, {row}]")
     L.check(lib.trtx_refinedet_postprocess_enqueue(C.byref(q), B, _ptr(arm_loc), _ptr(arm_conf), _ptr(odm_loc),
@@ -1940,7 +1939,7 @@ class PyRunnerPostprocess:
         _f32_rows(dets)
         rows_out = _out_tensor(rows_out, (B, 1 + self.max_rows * 6), torch.float32, dets.device,
                                f"rows_out must be contiguous float32 [{B}, {1 + self.max_rows * 6}]")
-        L.check(lib.trtx_pyrunner_postprocess_enqueue(C.byref(self.params), _frame_wh(image_sizes), B, _ptr(dets),
+        L.check(lib.trtx_pyrunner_postprocess_enqueue(C.byref(self.params), _frame_wh(image_sizes, B), B, _ptr(dets),
                                                       self.max_rows, _ptr(rows_out), _stream(stream)),
                 "trtx_pyrunner_postprocess_enqueue")
         return rows_out
