@@ -25,12 +25,16 @@ inline int check_launch() {
     return TRTX_OK;
 }
 
-// Opts `kernel` in to `smem` bytes of dynamic shared memory, which a launch may use without that only up to 48 KiB;
-// TRTX_ERR_CUDA, the error in g_last_cuda_error, where the attribute is refused.
+// Opts `kernel` in to `smem` bytes of dynamic shared memory where its current limit is lower.  Without an opt-in the limit is
+// 48 KiB less the kernel's static shared memory (so a band kernel's 4 KiB of static arrays and tables leave it 44 KiB), not
+// 48 KiB.  TRTX_ERR_CUDA, the error in g_last_cuda_error, where the limit cannot be read or raised.
 template <class Kernel>
 inline int opt_in_smem(Kernel* kernel, size_t smem) {
-    if (smem <= 48 * 1024 || cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess)
-        return TRTX_OK;
+    cudaFuncAttributes fa;
+    cudaError_t e = cudaFuncGetAttributes(&fa, kernel);
+    if (e == cudaSuccess && smem > (size_t)fa.maxDynamicSharedSizeBytes)
+        e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) return TRTX_OK;
     g_last_cuda_error = (int)cudaGetLastError();
     return TRTX_ERR_CUDA;
 }
