@@ -1,15 +1,16 @@
 """ctypes/numpy wrapper around oracle/libanchor_free_oracle.so: the CPU oracle of yolov9's converting nms() and yolov10's
-get_topk + get_rect (oracle/anchor_free_oracle.c; recipe oracle/anchor_free.mk).
+get_topk + get_rect (oracle/anchor_free_oracle.c; recipe oracle/Makefile).
 
 TEST INFRASTRUCTURE ONLY, like oracle/oracle.py: imported by tests/, never by the product package.
 """
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
+
+from . import oracle as _base
 
 HERE = Path(__file__).resolve().parent
 LIB = HERE / "libanchor_free_oracle.so"
@@ -19,10 +20,7 @@ _lib = None
 def load():
     global _lib
     if _lib is None:
-        src = HERE / "anchor_free_oracle.c"
-        if not LIB.exists() or LIB.stat().st_mtime < src.stat().st_mtime:
-            subprocess.run(["make", "-C", str(HERE), "-f", "anchor_free.mk", str(LIB)], check=True, stdout=subprocess.DEVNULL)
-        _lib = C.CDLL(str(LIB))
+        _lib = _base.build_and_open(LIB)
         _lib.oracle_v9_nms.restype = C.c_int
         _lib.oracle_topk.restype = C.c_int
     return _lib

@@ -1,5 +1,5 @@
 /* anchor_free_oracle.c -- TEST INFRASTRUCTURE.  The CPU oracle of the two host post-processes of yolov9 and yolov10 that the
- * library runs on the device (oracle/anchor_free.mk links it to libtrtx_oracle.so, whose oracle_nms and oracle_get_rect it
+ * library runs on the device (oracle/Makefile links it to libtrtx_oracle.so, whose oracle_nms and oracle_get_rect it
  * reuses):
  *   oracle_v9_nms   yolov9's nms() (yolov9/src/postprocess.cpp:48-83): rows i < output[0] and i < max_rows, each l, t, r, b
  *                   box converted to c_x = (b0 + b2) / 2, c_y = (b1 + b3) / 2, w = b2 - b0, h = b3 - b1 in float, then

@@ -6,7 +6,6 @@ TEST INFRASTRUCTURE ONLY, like oracle/oracle.py: imported by tests/ and tools/, 
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 import sys
 import types
 from importlib.machinery import SourcelessFileLoader
@@ -14,6 +13,8 @@ from importlib.util import module_from_spec, spec_from_loader
 from pathlib import Path
 
 import numpy as np
+
+from . import oracle as _base
 
 HERE = Path(__file__).resolve().parent
 LIB = HERE / "libcenternet_oracle.so"
@@ -26,10 +27,7 @@ def load():
     global _lib
     if _lib is not None:
         return _lib
-    src = HERE / "centernet_oracle.c"
-    if not LIB.exists() or LIB.stat().st_mtime < src.stat().st_mtime:  # recipe: oracle/centernet.mk
-        subprocess.run(["make", "-C", str(HERE), "-f", "centernet.mk", str(LIB)], check=True, stdout=subprocess.DEVNULL)
-    _lib = C.CDLL(str(LIB))
+    _lib = _base.build_and_open(LIB)
     _lib.oracle_centernet_rows.restype = C.c_int
     return _lib
 

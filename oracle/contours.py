@@ -21,7 +21,7 @@ _lib = None
 def load():
     global _lib
     if _lib is None:
-        _lib = _base.build_and_open(LIB, "contours_oracle.c")
+        _lib = _base.build_and_open(LIB)
     return _lib
 
 

@@ -6,10 +6,11 @@ TEST INFRASTRUCTURE ONLY, like oracle/oracle.py: imported by tests/ and tools/, 
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
+
+from . import oracle as _base
 
 HERE = Path(__file__).resolve().parent
 LIB = HERE / "libcubic_oracle.so"
@@ -21,9 +22,7 @@ def load():
     global _lib
     if _lib is not None:
         return _lib
-    if not LIB.exists() or LIB.stat().st_mtime < (HERE / "cubic_oracle.c").stat().st_mtime:  # recipe: oracle/cubic.mk
-        subprocess.run(["make", "-C", str(HERE), "-f", "cubic.mk", str(LIB)], check=True, stdout=subprocess.DEVNULL)
-    _lib = C.CDLL(str(LIB))
+    _lib = _base.build_and_open(LIB)
     _lib.oracle_cubic_input_value.restype = C.c_float
     _lib.oracle_cubic_preprocess.restype = C.c_int
     return _lib

@@ -7,10 +7,11 @@ TEST INFRASTRUCTURE ONLY, like oracle/oracle.py: imported by tests/ and tools/, 
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
+
+from . import oracle as _base
 
 HERE = Path(__file__).resolve().parent
 LIB = HERE / "liblinear_oracle.so"
@@ -22,10 +23,7 @@ def load():
     global _lib
     if _lib is not None:
         return _lib
-    src = [HERE / "linear_oracle.c", HERE / "cls_oracle.c"]
-    if not LIB.exists() or LIB.stat().st_mtime < max(f.stat().st_mtime for f in src):  # recipe: oracle/linear.mk
-        subprocess.run(["make", "-C", str(HERE), "-f", "linear.mk", str(LIB)], check=True, stdout=subprocess.DEVNULL)
-    _lib = C.CDLL(str(LIB))
+    _lib = _base.build_and_open(LIB)
     _lib.oracle_linear_input_value.restype = C.c_float
     _lib.oracle_linear_preprocess.restype = C.c_int
     _lib.oracle_linear_get_rect.restype = C.c_int

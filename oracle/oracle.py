@@ -20,18 +20,17 @@ _i32p = np.ctypeslib.ndpointer(np.int32, flags="C_CONTIGUOUS")
 _u8p = np.ctypeslib.ndpointer(np.uint8, flags="C_CONTIGUOUS")
 
 
-def build_and_open(lib: Path, source: str) -> C.CDLL:
-    """Open the oracle library `lib`, first (re)building it with oracle/Makefile when it is missing or older than its C
-    source oracle/<source>."""
-    if not lib.exists() or lib.stat().st_mtime < (HERE / source).stat().st_mtime:
-        subprocess.run(["make", "-C", str(HERE), str(lib)], check=True, stdout=subprocess.DEVNULL)
+def build_and_open(lib: Path) -> C.CDLL:
+    """Open the oracle library `lib`, first letting oracle/Makefile rebuild it when it is missing or older than any
+    prerequisite of its recipe."""
+    subprocess.run(["make", "-s", "-C", str(HERE), str(lib)], check=True)
     return C.CDLL(str(lib))
 
 
 def load():
     global _lib
     if _lib is None:
-        _lib = build_and_open(LIB, "trtx_oracle.c")
+        _lib = build_and_open(LIB)
     return _lib
 
 

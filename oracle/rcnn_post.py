@@ -22,7 +22,7 @@ def load():
     if _lib is not None:
         return _lib
     _base.load()   # libtrtx_oracle.so, whose bilinear resize this library uses
-    _lib = _base.build_and_open(LIB, "rcnn_post_oracle.c")
+    _lib = _base.build_and_open(LIB)
     _lib.oracle_rcnn_postprocess.restype = C.c_int
     return _lib
 

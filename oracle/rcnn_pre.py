@@ -21,7 +21,7 @@ def load():
     global _lib
     if _lib is not None:
         return _lib
-    _lib = _base.build_and_open(LIB, "rcnn_pre_oracle.c")
+    _lib = _base.build_and_open(LIB)
     _lib.oracle_rcnn_preprocess.restype = C.c_int
     return _lib
 

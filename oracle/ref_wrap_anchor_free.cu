@@ -1,5 +1,5 @@
 // ref_wrap_anchor_free.cu -- TEST INFRASTRUCTURE.  extern "C" entry points around the REFERENCE's own YoloLayer plugin of
-// yolov9 (REF_AF_V9), yolov10 or yolov13 (plugin/yololayer.cu compiled where it lies by oracle/anchor_free.mk, IPluginV2IOExt).
+// yolov9 (REF_AF_V9), yolov10 or yolov13 (plugin/yololayer.cu compiled where it lies by oracle/Makefile, IPluginV2IOExt).
 // The plugin launches on the given stream and memsets there: the wrapper synchronises the stream.
 #include <cuda_runtime_api.h>
 

@@ -1,5 +1,5 @@
 // ref_wrap_anchor_free_host.cpp -- TEST INFRASTRUCTURE.  CPU-only wrapper around one driver's own post-process
-// (src/postprocess.cpp compiled where it lies by oracle/anchor_free.mk, against oracle/shim; unused code dropped with
+// (src/postprocess.cpp compiled where it lies by oracle/Makefile, against oracle/shim; unused code dropped with
 // -Wl,--gc-sections): yolov9's and yolov13's nms() (REF_AF_NMS), yolov10's get_topk (REF_AF_TOPK), and each one's get_rect.
 #include <cstring>
 #include <vector>

@@ -1,4 +1,4 @@
-// ref_wrap_ufld_host.cpp -- TEST INFRASTRUCTURE.  CPU-only wrapper around UFLD's driver compiled where it lies (oracle/ufld.mk:
+// ref_wrap_ufld_host.cpp -- TEST INFRASTRUCTURE.  CPU-only wrapper around UFLD's driver compiled where it lies (oracle/Makefile:
 // -Dmain=ref_ufld_driver_main, against oracle/shim_ufld): its own argmax and softmax_mul, called with the test's arguments.
 #include <type_traits>
 

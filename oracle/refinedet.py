@@ -11,11 +11,12 @@ TEST INFRASTRUCTURE ONLY, like oracle/oracle.py: imported by tests/ and tools/, 
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
 import torch
+
+from . import oracle as _base
 
 
 HERE = Path(__file__).resolve().parent
@@ -32,10 +33,7 @@ def load():
     global _lib
     if _lib is not None:
         return _lib
-    src = [HERE / "refinedet_oracle.c", HERE / "cls_oracle.c"]
-    if not LIB.exists() or LIB.stat().st_mtime < max(f.stat().st_mtime for f in src):  # recipe: oracle/refinedet.mk
-        subprocess.run(["make", "-C", str(HERE), "-f", "refinedet.mk", str(LIB)], check=True, stdout=subprocess.DEVNULL)
-    _lib = C.CDLL(str(LIB))
+    _lib = _base.build_and_open(LIB)
     _lib.oracle_refinedet_input_value.restype = C.c_float
     _lib.oracle_refinedet_postprocess.argtypes = [C.c_void_p] * 4 + [C.c_int, C.c_int, C.c_float, C.c_float, C.c_float,
                                                                      C.c_int, C.c_int, C.c_void_p]

@@ -25,7 +25,7 @@ def load():
     if _lib is not None:
         return _lib
     _base.load()   # libtrtx_oracle.so: process_mask, the bilinear resize, get_rect
-    _lib = _base.build_and_open(LIB, "seg_post_oracle.c")
+    _lib = _base.build_and_open(LIB)
     _lib.oracle_seg_postprocess.restype = C.c_int
     return _lib
 

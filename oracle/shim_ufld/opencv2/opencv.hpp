@@ -1,5 +1,5 @@
 // SHIM, not OpenCV -- TEST INFRASTRUCTURE.  The cv:: names that UFLD's driver (ufld/lane_det.cpp) and ufld/common.hpp mention,
-// so that its argmax and softmax_mul compile where they lie (oracle/ufld.mk).  Type stubs only: no function here does pixel
+// so that its argmax and softmax_mul compile where they lie (oracle/Makefile).  Type stubs only: no function here does pixel
 // work, and prepareImage is never called (the tests pin the pre-process to cv2 itself).
 #pragma once
 #include <cassert>

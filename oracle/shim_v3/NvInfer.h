@@ -1,6 +1,6 @@
 // SHIM, not TensorRT -- TEST INFRASTRUCTURE.  tests/mock_trt/NvInfer.h (the plugin interfaces) plus the builder, network, engine
 // and runtime names that the yolov3 / yolov4 / scaled-yolov4 / yolov3-tiny / yolov3-spp drivers mention outside the functions the
-// tests call (get_rect, letterbox), so that those drivers compile where they lie (oracle/linear.mk).  Declarations only: every
+// tests call (get_rect, letterbox), so that those drivers compile where they lie (oracle/Makefile).  Declarations only: every
 // builder and runtime call is a template that returns an empty value, and the linker drops the code that calls them
 // (-Wl,--gc-sections), because nothing exported reaches it.
 #pragma once

@@ -1,5 +1,5 @@
 // SHIM, not OpenCV -- TEST INFRASTRUCTURE.  The cv:: names that the yolov3 / yolov4 / scaled-yolov4 / yolov3-tiny / yolov3-spp
-// drivers and their headers mention, so that their get_rect and yolov3-spp's letterbox compile where they lie (oracle/linear.mk).
+// drivers and their headers mention, so that their get_rect and yolov3-spp's letterbox compile where they lie (oracle/Makefile).
 // An image is a (rows, cols, type) header with no pixels: get_rect reads rows and cols only; for the letterbox the shim records
 // the last rectangle taken from an image and the last size cv::resize was asked for (Mat::shim_geometry), and the canvas
 // letterbox returns carries its size.

@@ -1,15 +1,16 @@
 """ctypes/numpy wrapper around oracle/libv3family_oracle.so: the CPU oracle of the yolov3 family's decode, each driver's box
-arithmetic and sigmoid (oracle/v3family_oracle.c; recipe oracle/v3family.mk).
+arithmetic and sigmoid (oracle/v3family_oracle.c; recipe oracle/Makefile).
 
 TEST INFRASTRUCTURE ONLY, like oracle/oracle.py: imported by tests/, never by the product package.
 """
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
+
+from . import oracle as _base
 
 HERE = Path(__file__).resolve().parent
 LIB = HERE / "libv3family_oracle.so"
@@ -20,10 +21,7 @@ _lib = None
 def load():
     global _lib
     if _lib is None:
-        src = HERE / "v3family_oracle.c"
-        if not LIB.exists() or LIB.stat().st_mtime < src.stat().st_mtime:
-            subprocess.run(["make", "-C", str(HERE), "-f", "v3family.mk", str(LIB)], check=True, stdout=subprocess.DEVNULL)
-        _lib = C.CDLL(str(LIB))
+        _lib = _base.build_and_open(LIB)
     return _lib
 
 

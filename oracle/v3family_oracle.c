@@ -1,5 +1,5 @@
 /* v3family_oracle.c -- TEST INFRASTRUCTURE.  Plain-C restatement of the yolov3 family's CalDetection, one driver's box
- * arithmetic at a time, built by oracle/v3family.mk into oracle/libv3family_oracle.so (-ffp-contract=off).
+ * arithmetic at a time, built by oracle/Makefile into oracle/libv3family_oracle.so (-ffp-contract=off).
  * box_mode takes the library's variant values (include/trtx_hot.h section 1):
  *   2 (spp)  x = (col + Logist(x0)) * stride                                  yolov3-spp/yololayer.cu:183-186
  *   4 (net)  x = (col + Logist(x0)) * INPUT_W / yoloWidth, in float            yolov3/yololayer.cu:173-176, yolov3-tiny :172-175

@@ -6,10 +6,11 @@ TEST INFRASTRUCTURE ONLY, like oracle/oracle.py: imported by tests/ and tools/, 
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
+
+from . import oracle as _base
 
 
 HERE = Path(__file__).resolve().parent
@@ -23,10 +24,7 @@ def load():
     global _lib
     if _lib is not None:
         return _lib
-    src = [HERE / "yolop_oracle.c", HERE / "cls_oracle.c"]
-    if not LIB.exists() or LIB.stat().st_mtime < max(f.stat().st_mtime for f in src):  # recipe: oracle/yolop.mk
-        subprocess.run(["make", "-C", str(HERE), "-f", "yolop.mk", str(LIB)], check=True, stdout=subprocess.DEVNULL)
-    _lib = C.CDLL(str(LIB))
+    _lib = _base.build_and_open(LIB)
     _lib.oracle_yolop_preprocess.restype = C.c_int
     _lib.oracle_yolop_input_value.restype = C.c_float
     return _lib

@@ -87,12 +87,10 @@ def build(force: bool = False, verbose: bool = False, probe: bool = False) -> Pa
 
 def build_oracle() -> Path:
     """Compile the CPU oracles (test infrastructure) and, when /root/reference exists, oracle/_ref."""
-    for makefile in ("Makefile", "yolop.mk", "detr.mk", "centernet.mk", "ufld.mk", "cubic.mk", "refinedet.mk", "linear.mk",
-                     "v3family.mk", "anchor_free.mk"):
-        r = subprocess.run(["make", "-C", str(ROOT / "oracle"), "-f", makefile, f"PYTHON={sys.executable}"],
-                           stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-        if r.returncode != 0:
-            raise RuntimeError(f"oracle build failed ({makefile}):\n{r.stdout}")
+    r = subprocess.run(["make", "-C", str(ROOT / "oracle"), f"PYTHON={sys.executable}"],
+                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    if r.returncode != 0:
+        raise RuntimeError(f"oracle build failed:\n{r.stdout}")
     return ROOT / "oracle" / "libtrtx_oracle.so"
 
 

@@ -11,9 +11,9 @@ json, torch, rois, feat, out = g["json"], g["torch"], g["rois"], g["feat"], g["o
 B, N, H, W, Pp = g["B"], g["N"], g["H"], g["W"], g["Pp"]
 # the reference's own roiAlign (oracle/_ref/libref_rcnn.so, built from /root/reference/rcnn/RoiAlign.cu) on the same inputs
 import ctypes as C, time
-ref = ROOT / "oracle" / "_ref" / "libref_rcnn.so"
-if ref.exists():
-    lib = C.CDLL(str(ref))
+from oracle.golden import RefOutputs  # importable: roi_probe put the repository root on sys.path
+lib = RefOutputs.lib("libref_rcnn.so")
+if lib is not None:
     for sampling in (0, 2):
         args = (B, C.c_void_p(rois.data_ptr()), C.c_void_p(feat.data_ptr()), C.c_void_p(out.data_ptr()), Pp, C.c_float(1 / 16),
                 sampling, N, 1024, H, W)

@@ -3,7 +3,7 @@ yolov3, yolov4, scaled-yolov4, yolov3-tiny and yolov3-spp, on the CPU: the oracl
 8-bit INTER_LINEAR with IPP on and off and the drivers' plane loops restated around it (cv2.dnn.blobFromImage for yolov3-spp),
 bit for bit; the 256 values of each chain; yolov3-spp's letterbox; trtx_get_rect's two new variants against the oracle and a
 numpy restatement of the drivers' statements; trtx_get_rect, trtx_yolov3spp_letterbox and the oracle against the five drivers'
-own compiled get_rect and yolov3-spp's compiled letterbox (oracle/_ref/libref_v3_*.so, or tests/golden/ref_v3_host.npz where
+own compiled get_rect and yolov3-spp's compiled letterbox (oracle/_ref/libref_v3_*_host.so, or tests/golden/ref_v3_host.npz where
 they were not built); and the argument checks that reject before any launch."""
 import contextlib
 import ctypes as C
@@ -19,7 +19,7 @@ from tensorrtx_b200 import plugins as P
 cv2 = pytest.importorskip("cv2")
 F = np.float32
 VARIANTS = (LO.YOLOV3, LO.RETINA, LO.YOLOV3_SPP)
-# the drivers' own get_rect and yolov3-spp's letterbox, compiled where they lie (oracle/linear.mk), or their stored outputs
+# the drivers' own get_rect and yolov3-spp's letterbox, compiled where they lie (oracle/Makefile), or their stored outputs
 G = RefOutputs("ref_v3_host")
 REF_DRIVERS = ("yolov3", "yolov4", "csp", "tiny", "spp")
 REF_NETS = {"yolov3": (608, 608), "yolov4": (608, 608), "csp": (512, 512), "tiny": (608, 608), "spp": (608, 608)}
@@ -332,7 +332,7 @@ def test_get_rect_equals_the_drivers_compiled_get_rect(driver):
     1 024 boxes x 12 frames, negative, past-the-frame and huge boxes included.  Boxes the oracle finds undefined in the
     reference (non-finite, out of the int range) are left out of the comparison: the compiled code's result there is
     whatever x86-64 gives, and the library's is {0, 0, 0, 0}."""
-    ref = G.lib(f"libref_v3_{driver}.so")
+    ref = G.lib(f"libref_v3_{driver}_host.so")
     net_w, net_h = REF_NETS[driver]
     if ref is not None:
         wh = (C.c_int * 2)()
@@ -362,7 +362,7 @@ def test_get_rect_equals_the_drivers_compiled_get_rect(driver):
 def test_spp_letterbox_equals_the_drivers_compiled_letterbox():
     """trtx_yolov3spp_letterbox and the oracle equal yolov3-spp's own compiled letterbox (its canvas and the rectangle it pastes
     the resized frame into) on frame sizes at, below and above MAX_INPUT_SIZE, tall and wide."""
-    ref = G.lib("libref_v3_spp.so")
+    ref = G.lib("libref_v3_spp_host.so")
     sizes = [(w, h) for w in (1, 2, 31, 127, 128, 300, 607, 608, 609, 1000, 1920, 4000) for h in (1, 3, 129, 200, 608, 1080,
                                                                                                    2432, 70000)]
     lib = L.load()

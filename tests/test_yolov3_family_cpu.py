@@ -4,7 +4,7 @@
   numpy re-derivation of the reference expressions, with libm's expf as the oracle's exp: x, y, w, h of modes 4 and 5 and x,
   y of mode 6 bit for bit; mode 6's w, h (powf(2s, 2)) within 1 ulp of numpy's float32 (2s)*(2s), since the host powf
   need not round as a product does.
-* Each driver's own compiled nms() (oracle/_ref/libref_v3f_nms_<driver>.so; where it was not built, the digests in
+* Each driver's own compiled nms() (oracle/_ref/libref_v3_<driver>_host.so; where it was not built, the digests in
   tests/golden/ref_v3f_host.npz) keeps the same rows in the same order as the library's NMS semantics with the parameters of
   plugins.V3_FAMILY_DRIVERS, on rows whose det_confidence sits on each threshold.
 * The creators' blobs equal the Python mirror's and those the drivers' own yololayer.h constants make."""
@@ -142,7 +142,7 @@ def _nms_rows(driver, seed):
 @pytest.mark.parametrize("driver", DRIVERS)
 def test_library_nms_parameters_equal_driver_nms(oracle, driver):
     d = P.V3_FAMILY_DRIVERS[driver]
-    lib = G.lib(f"libref_v3f_nms_{LIBNAME[driver]}.so")
+    lib = G.lib(f"libref_v3_{LIBNAME[driver]}_host.so")
     for seed in (710, 711):
         buf = _nms_rows(driver, seed)
         res, _ = oracle.nms(1, buf, 1000, 7, d["conf_thresh"], d["nms_thresh"])
@@ -192,7 +192,7 @@ def test_family_creators_host_surface_and_blobs(tmp_path):
         d = P.V3_FAMILY_DRIVERS[driver]
         q = P.YoloLayerPluginV3Net.deserialize(blobs[driver], d["net"][0], d["net"][1], d["variant"])
         assert q.serialize() == blobs[driver] and q.params.variant == d["variant"]
-        lib = G.lib(f"libref_v3f_{LIBNAME[driver]}_host.so")
+        lib = G.lib(f"libref_v3_{LIBNAME[driver]}_host.so")
         ref = None
         if lib is not None:
             buf = (C.c_ubyte * 256)()

@@ -1,6 +1,6 @@
 """The yolov3 family's decode on the device (TRTX_YOLO_V3_NET: yolov3, yolov3-tiny; TRTX_YOLO_V4: yolov4; TRTX_YOLO_V4_CSP:
 scaled-yolov4), each against
-(1) that driver's OWN compiled YoloLayer kernel (oracle/_ref/libref_v3f_<driver>.so, same GPU, same inputs; where it was not
+(1) that driver's OWN compiled YoloLayer kernel (oracle/_ref/libref_v3f_blob_<driver>.so, same GPU, same inputs; where it was not
     built, its outputs stored in tests/golden/ref_v3f_gpu.npz): count, class, both confidences and the box, bit for bit,
     after a canonical sort (the reference's row order is atomicAdd arrival);
 (2) the CPU oracle's decode + that driver's NMS parameters, through every entry point: the plugin decode, the fused
@@ -63,7 +63,7 @@ def _oracle(oracle, driver, heads, max_out=1000):
 @pytest.mark.parametrize("B", [1, 3])
 @pytest.mark.parametrize("driver", DRIVERS)
 def test_plugin_rows_equal_driver_kernel(oracle, dev, driver, B):
-    lib = G.lib(f"libref_v3f_{LIBNAME[driver]}.so")
+    lib = G.lib(f"libref_v3f_blob_{LIBNAME[driver]}.so")
     d = P.V3_FAMILY_DRIVERS[driver]
     heads = _heads(d, B, seed=800 + B + 10 * d["variant"])
     hd = [torch.from_numpy(h).to(dev) for h in heads]
